@@ -1,6 +1,6 @@
 """bench.py — graphs/sec through GPSLayer forward+backward on PCQM4M-shaped synthetic batches.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
 A *step* is one GPSLayer forward+backward (training mode, BatchNorm batch statistics, dropout as
@@ -15,6 +15,10 @@ inside the step.  One JSON line is printed by rank 0.
   roofline  dominant kernel of the step, timed live with CUDA events around its C-ABI stage call
   cpu_baseline  the reference's own GPSLayer (oracle/_ref run verbatim under oracle/ref_shim.py; the
             oracle port if the files are absent) on the host cores, bounded sample of the same workload
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed (the layer outputs, the input
+gradients and the parameter gradients) as DIR/<name>.npy.  Inputs, weights and cotangents are seeded, so two builds
+run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -53,11 +57,12 @@ def peaks():
         p = json.load(open(path))
         return dict(hbm=p["hbm_gbs"], tensor=p["bf16_tflops"], tensor_sustained=p["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tensor=1590.0, tensor_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s; not reached figures, upper bounds
+    return dict(hbm=3350.0, tensor=989.0, tensor_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """SM clock / throttle-reason sampling DURING the timed region (B200_PROFILING.md recipe).
+    """SM clock / throttle-reason sampling DURING the timed region.
 
     The timed region of this benchmark is tens of milliseconds, far below nvidia-smi's loop period, so the
     same counters are read through NVML (nvidia_ml_py) from a thread every ~2 ms; nvidia-smi is the fallback."""
@@ -314,7 +319,7 @@ def run_ours(args):
         if "_gps_b200_graph" in b.__dict__:
             bb.__dict__["_gps_b200_graph"] = b.__dict__["_gps_b200_graph"]
         bucket.zero_()
-        x_in = bb.x
+        x_in, e_in = bb.x, bb.edge_attr
         out = layer(bb)
         if gated:
             torch.autograd.backward([out.x, out.edge_attr], [ctx, cte])
@@ -322,7 +327,7 @@ def run_ours(args):
             torch.autograd.backward([out.x], [ctx])
         if reduce:
             allreduce_grads()
-        return out, x_in
+        return out, x_in, e_in
 
     def barrier():
         if world > 1:
@@ -342,6 +347,8 @@ def run_ours(args):
     launches_per_step = None
     collective_in_graph = False
 
+    captured = {}                  # (reduce, batch) -> (out, x_in) of the captured step: its replays rewrite them
+
     def capture_all(reduce):
         out = []
         nonlocal launches_per_step
@@ -349,7 +356,7 @@ def run_ours(args):
             g = torch.cuda.CUDAGraph()
             l0 = lib.gps_launch_count()
             with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                step(i, reduce=reduce)
+                captured[(reduce, i)] = step(i, reduce=reduce)
             launches_per_step = lib.gps_launch_count() - l0
             out.append(g)
         return out
@@ -376,10 +383,13 @@ def run_ours(args):
         if graphs is None:
             graphs = graphs_local
 
+    last = {}
+
     def run_step(i):
         if graphs is None:
-            step(i)
+            last["res"] = step(i)
         else:
+            last["res"] = captured[(collective_in_graph, i % NUM_BATCHES)]
             graphs[i % NUM_BATCHES].replay()
             if world > 1 and not collective_in_graph:
                 allreduce_grads()
@@ -407,6 +417,8 @@ def run_ours(args):
     launches = launches_per_step if graphs is not None else (lib.gps_launch_count() - l0) // max(1, args.steps)
     ms = sum(a.elapsed_time(b) for a, b in evs)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, layer, *last["res"], gated)
     t = torch.tensor([ms], device=dev, dtype=torch.float64)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -636,12 +648,40 @@ def run_ours(args):
         os._exit(0)
 
 
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_outputs(path, layer, out, x_in, e_in, gated):
+    """What a caller of the timed step receives: out.x (+ out.edge_attr), the input gradients and every parameter
+    gradient, as float32 .npy files.  An array above its share of the 64 MiB budget is written as a fixed seeded
+    sample of its rows (the same rows in every run of the same workload)."""
+    import numpy as np
+    arrays = {"out_x": out.x, "grad_x": x_in.grad}
+    if gated:
+        arrays["out_edge_attr"] = out.edge_attr
+    if e_in.grad is not None:
+        arrays["grad_edge_attr"] = e_in.grad
+    for n, p in layer.named_parameters():
+        if p.grad is not None:
+            arrays["grad_" + n] = p.grad
+    share = DUMP_BUDGET_BYTES // len(arrays)
+    os.makedirs(path, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu()
+        if a.numel() * 4 > share and a.dim() >= 1:
+            row_bytes = max(1, a[0].numel()) * 4
+            k = max(1, share // row_bytes)
+            rows = torch.randperm(a.shape[0], generator=torch.Generator().manual_seed(0))[:k].sort().values
+            a = a[rows]
+        np.save(os.path.join(path, name + ".npy"), a.numpy().astype(np.float32))
+
+
 def roofline_probe(lib, layer, b, spec, heads, args):
     """Times the step's two headline kernels live (CUDA events around their C-ABI stage calls, L2 flushed, host
     launch latency hidden behind a spin kernel): the longest single kernel of the step — the data-gradient GEMM
     g_x = gY1[N,7d] . Wcat[7d,d] (tensor bound, 2*N*7d*d flop) — and the GatedGCN gather-reduce (HBM bound,
-    4*(5N+2E)*d algorithmic bytes, SURVEY.md 8d).  `traffic` = DRAM bytes per launch of the same kernels from the
-    committed `ncu --set full` capture (profiles/r1_roofline_traffic.json)."""
+    4*(5N+2E)*d algorithmic bytes, SURVEY.md 8d).  `traffic` = DRAM bytes per launch of the same kernels from a
+    profiler capture stored as profiles/r2_roofline_traffic.json (null when there is none)."""
     import ctypes as C
     from graphgps_b200.graph import graph_of
     pk = peaks()
@@ -650,7 +690,7 @@ def roofline_probe(lib, layer, b, spec, heads, args):
     N, E, d = gs.N, gs.E, spec.dim
     stream = torch.cuda.current_stream().cuda_stream
     flush = torch.empty(L2_FLUSH_BYTES, dtype=torch.uint8, device=dev)
-    # DRAM bytes per launch from the committed `ncu --set full` capture of THIS workload (null when none was taken)
+    # DRAM bytes per launch from a profiler capture of THIS workload (null when none was taken)
     traffic = {}
     tpath = os.path.join(ROOT, "profiles", "r2_roofline_traffic.json")
     if os.path.exists(tpath):
@@ -694,7 +734,7 @@ def roofline_probe(lib, layer, b, spec, heads, args):
     flops = 2.0 * N * Wy * d
     res["gemm"] = {"bound": "tensor", "achieved": flops / t_g / 1e12, "peak": pk["tensor"], "unit": "TFLOP/s",
                    "frac": flops / t_g / 1e12 / pk["tensor"], "traffic": traffic.get("gemm_dgrad_x"), "seconds": t_g,
-                   "kernel": "k_gemm_tma data gradient g_x[N,d] = gY1[N,7d] x Wcat[7d,d] (TMA-fed tcgen05 on bf16 hi/lo planes, "
+                   "kernel": "k_gemm_tma data gradient g_x[N,d] = gY1[N,7d] x Wcat[7d,d] (TMA-fed wgmma on bf16 hi/lo planes, "
                              + ("3 MMAs per product" if prec == 0 else "1 MMA per product") + ", split-K 4)",
                    "algorithmic_flops": flops, "peak_source": pk["source"]}
     Y = torch.randn(N, Wy, device=dev)
@@ -726,6 +766,8 @@ def main():
     ap.add_argument("--workload", default="pcqm4m-small", choices=sorted(WORKLOADS))
     ap.add_argument("--precision", default="fp32", choices=["fp32", "bf16"])
     ap.add_argument("--no-graph", dest="graph", action="store_false", help="time eager launches instead of CUDA-graph replays")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy (float32, at most 64 MiB)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

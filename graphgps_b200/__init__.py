@@ -1,4 +1,4 @@
-"""graphgps_b200 — B200 (sm_100a) implementation of the GraphGPS `GPSLayer` hot path.
+"""graphgps_b200 — H100 (sm_90a) implementation of the GraphGPS `GPSLayer` hot path.
 
 Public surface (mirrors the reference's module boundary, SURVEY.md section 8b):
     GPSLayer      drop-in for graphgps.layer.gps_layer.GPSLayer

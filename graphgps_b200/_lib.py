@@ -123,7 +123,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} not found: build it with `python -m graphgps_b200.build` "
-            "(nvcc, sm_100a). graphgps_b200 has no CPU/eager fallback.")
+            "(nvcc, sm_90a). graphgps_b200 has no CPU/eager fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SYMBOLS.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing

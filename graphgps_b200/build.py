@@ -1,4 +1,4 @@
-"""In-tree build of libgps_b200.so (nvcc, sm_100a only).  `python -m graphgps_b200.build`."""
+"""In-tree build of libgps_b200.so (nvcc, sm_90a only).  `python -m graphgps_b200.build`."""
 from __future__ import annotations
 
 import glob
@@ -13,7 +13,7 @@ LIB = os.path.join(HERE, "libgps_b200.so")
 OBJ = os.path.join(HERE, "csrc", "_obj")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
 ]
 

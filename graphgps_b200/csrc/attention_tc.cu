@@ -1,23 +1,25 @@
-// attention_tc.cu — softmax attention over each graph's own nodes on the 5th-gen tensor cores (tcgen05 + TMEM + TMA).
+// attention_tc.cu — softmax attention over each graph's own nodes on the Hopper tensor cores (wgmma + TMA).
 //
 // Replaces to_dense_batch -> nn.MultiheadAttention core -> [mask] (graphgps/layer/gps_layer.py:199-201, 234-241) like
-// attention.cu, but as two UMMA products per key tile:  S = Q K^T  and  O += P V.
+// attention.cu, but as two warpgroup MMAs per key tile:  S = Q K^T  and  O += P V.
 //
 //   * Packing instead of padding: a CTA owns 128 CONSECUTIVE node rows of the packed batch (several small graphs, or a
 //     slice of a large one) and one head.  Its keys are the contiguous node range [start of the first row's graph, end
 //     of the last row's graph), walked in tiles of 128.  The dense batch of the reference (B x Nmax, 1.7x - 3x padding)
 //     never exists; the per-graph "key padding mask" is the block-diagonal range test  graph_start(i) <= j < graph_end(i)
-//     applied to the S tile on its way from TMEM to registers (one thread per query row, tcgen05.ld 32x32b).
+//     applied to the S accumulator registers.
 //   * Operands: Q, K, V arrive by tensor-map TMA from the bf16 hi/lo planes that the node-projection GEMM's epilogue wrote
-//     in a per-head layout padded to a multiple of 16 columns (zero pad), already in the UMMA SWIZZLE_128B image:
+//     in a per-head layout padded to a multiple of 16 columns (zero pad), already in the wgmma SWIZZLE_128B image:
 //     Q and K K-major ({64 x 128} boxes), V as an MN-major B operand ({64 x 64} boxes).  fp32-grade mode runs every
 //     product as lo*hi + hi*lo + hi*hi (the probabilities are split hi/lo as well); bf16 mode is a single pass.
-//   * Online softmax in fp32 with the running row max / sum in registers; when a row's max moves, the O accumulator in
-//     TMEM is rescaled in place (tcgen05.ld -> scale -> tcgen05.st) before the next P V product is issued.  Dropout on the
+//   * Each of the two consumer warpgroups owns 64 query rows: S (64 x 128) and O (64 x 64 or 64 x 128) stay in its
+//     registers.  Online softmax in fp32 with the running row max / sum per thread (a row is spread over the 4 lanes of
+//     a quad); when a row's max moves, O is rescaled in registers.  P goes straight from the S registers into the
+//     register A operand of the P V product (the accumulator fragment of S is the A fragment of P).  Dropout on the
 //     probabilities uses the same Philox stream as attention.cu (site GPS_SITE_ATTN_P + head, one draw per 4 keys).
-//   * P goes back to the tensor core through shared memory (K-major SWIZZLE_128B tile written by the softmax threads,
-//     fence.proxy.async); for head dims above 64 it reuses the K tile's storage, which S = Q K^T has finished with.
-// Warp roles (192 threads): warps 0-3 softmax / epilogue (TMEM lane quarter = warp), warp 4 MMA issuer, warp 5 TMA.
+// 256 threads = two MMA / softmax warpgroups; thread 0 also issues the TMA loads.  The K and V tiles have their own
+// full / empty barriers, so the next K tile loads while the softmax and P V of the current one run.  (A separate
+// producer warp would make the CTA count as three warpgroups and cap the registers that S, O and P need.)
 // The CUDA-core kernel in attention.cu stays as the validator (GPS_B200_ATTN=simt) and for head dims above 128.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -33,15 +35,14 @@ namespace {
 using namespace tc;
 
 constexpr int kTile = 128;
-constexpr int kSoftWarps = 4;
-constexpr int kThreadsA = 192;
+constexpr int kSoftWarps = 8;
+constexpr int kThreadsA = 256;
 
 struct AttnTcArgs {
   const int* gptr; int B; int N; int H; int hd; int hd_pad; int planes;
   float* O; int64_t ldo; Planes Op; float* lse;
   float scale; float p_drop; uint64_t seed, offset;
   const unsigned long long* offset_dev;
-  int dbg_only;   // bring-up: >= 0: issue only P V k-step (kk2*4+kk) == dbg_only, hi*hi, no accumulate
   float* dbg;   // bring-up: CTA (0,0) dumps S [128x128], P [128x128] and the raw O accumulator [128x128] of its first tile
 };
 
@@ -59,271 +60,266 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
+// one query row as seen by one lane: graph key range, running max / partial sum, cached dropout draw
+struct RowState {
+  int i, gs, ge;
+  float m, l;
+  int rq_quad;
+  Philox4 rq;
+};
+
+// NKB: 64-column blocks of the padded head dim (1: hd_pad <= 64, 2: <= 128) = the P V instruction width / 64
+template <int NKB, bool SPLIT>
 __global__ void __launch_bounds__(kThreadsA, 1)
 k_attn_tc_fwd(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmV, const AttnTcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int planes = a.planes;
-  const int nkb = (a.hd_pad + 63) >> 6;          // 64-column blocks of the head dim (1 or 2)
-  const int q_bytes = nkb * 16384, k_bytes = nkb * 16384, v_bytes = 2 * nkb * 8192, p_bytes = 2 * 16384;   // per plane
-  const bool alias = nkb == 2;                   // P reuses the K tile (same size) when the head dim exceeds 64
+  constexpr int planes = SPLIT ? 2 : 1;
+  constexpr int q_bytes = NKB * 16384, k_bytes = NKB * 16384, v_bytes = 2 * NKB * 8192;   // per plane
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + planes * q_bytes;
   uint8_t* sV = sK + planes * k_bytes;
-  uint8_t* sP = alias ? sK : sV + planes * v_bytes;
-  uint8_t* tail = alias ? sV + planes * v_bytes : sP + planes * p_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(tail);   // 0 q_full, 1 kv_full, 2 s_full, 3 p_full, 4 pv_done
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-  int* range = reinterpret_cast<int*>(tmem_slot + 2);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + planes * v_bytes);   // q_full, k_full, v_full, k_empty, v_empty
+  int* range = reinterpret_cast<int*>(bars + 8);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int q0 = blockIdx.x * kTile, h = blockIdx.y;
-  const uint32_t b_q = smem_u32(&bars[0]), b_kv = smem_u32(&bars[1]), b_s = smem_u32(&bars[2]), b_p = smem_u32(&bars[3]),
-                 b_pv = smem_u32(&bars[4]);
+  const uint32_t b_q = smem_u32(&bars[0]), b_kf = smem_u32(&bars[1]), b_vf = smem_u32(&bars[2]),
+                 b_ke = smem_u32(&bars[3]), b_ve = smem_u32(&bars[4]);
 
   if (tid == 0) {
-    mbar_init(b_q, 1); mbar_init(b_kv, 1); mbar_init(b_s, 1); mbar_init(b_p, kSoftWarps); mbar_init(b_pv, 1);
+    mbar_init(b_q, 1); mbar_init(b_kf, 1); mbar_init(b_vf, 1); mbar_init(b_ke, kSoftWarps); mbar_init(b_ve, kSoftWarps);
     fence_barrier_init();
     const int last = min(q0 + kTile, a.N) - 1;
     const int g0 = find_graph_tc(a.gptr, a.B, q0), g1 = find_graph_tc(a.gptr, a.B, last);
     range[0] = a.gptr[g0];
     range[1] = a.gptr[g1 + 1];
   }
-  if (warp == 5 && lane == 0) {
-    tma_prefetch_desc(&tmQK);
-    tma_prefetch_desc(&tmV);
-  }
-  if (warp == 4) tmem_alloc(smem_u32(tmem_slot), 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmemS = tmem_base, tmemO = tmem_base + 128;
   const int kmin = range[0], kmax = range[1];
   const int ntiles = max(1, (kmax - kmin + kTile - 1) / kTile);
 
-  if (warp == 5) {
-    // =========================================================== TMA producer
-    if (lane == 0) {
-      mbar_arrive_expect_tx(b_q, (uint32_t)(planes * q_bytes));
-      for (int pl = 0; pl < planes; ++pl)
-        for (int kb = 0; kb < nkb; ++kb)
-          tma_tile_3d(smem_u32(sQ + pl * q_bytes + kb * 16384), &tmQK, h * a.hd_pad + 64 * kb, q0, pl, b_q);
-      for (int t = 0; t < ntiles; ++t) {
-        if (t > 0) mbar_wait(b_pv, (uint32_t)(t - 1) & 1u);     // P V of the previous tile has read P (= K) and V
-        const int key0 = kmin + t * kTile;
-        mbar_arrive_expect_tx(b_kv, (uint32_t)(planes * (k_bytes + v_bytes)));
-        for (int pl = 0; pl < planes; ++pl) {
-          for (int kb = 0; kb < nkb; ++kb)
-            tma_tile_3d(smem_u32(sK + pl * k_bytes + kb * 16384), &tmQK, (a.H + h) * a.hd_pad + 64 * kb, key0, pl, b_kv);
-          for (int kk = 0; kk < 2; ++kk)
-            for (int nb = 0; nb < nkb; ++nb)
-              tma_tile_3d(smem_u32(sV + pl * v_bytes + (kk * nkb + nb) * 8192), &tmV, (2 * a.H + h) * a.hd_pad + 64 * nb,
-                          key0 + 64 * kk, pl, b_kv);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 4) {
-    // =========================================================== MMA issuer
-    // The whole warp walks the loops with identical (warp-uniform) operands; one elected lane issues each instruction.
-    {
-      const uint32_t idesc_s = make_idesc(128, kTile, false, false);
-      const uint32_t idesc_o = make_idesc(128, a.hd_pad, false, true);
-      const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aV = smem_u32(sV), aP = smem_u32(sP);
-      if (lane == 0) mbar_wait(b_q, 0u);
-      __syncwarp();
-      for (int t = 0; t < ntiles; ++t) {
-        if (lane == 0) mbar_wait(b_kv, (uint32_t)t & 1u);
-        __syncwarp();
-        tc_fence_after();
-        bool first = true;
-        for (int kb = 0; kb < nkb; ++kb) {
-          const int ksteps = min(4, (a.hd_pad - 64 * kb) >> 4);
-          for (int kk = 0; kk < ksteps; ++kk) {
-            const uint64_t dq_hi = make_desc(aQ + kb * 16384 + kk * 32, 16, 1024);
-            const uint64_t dk_hi = make_desc(aK + kb * 16384 + kk * 32, 16, 1024);
-            if (planes == 2) {
-              const uint64_t dq_lo = make_desc(aQ + q_bytes + kb * 16384 + kk * 32, 16, 1024);
-              const uint64_t dk_lo = make_desc(aK + k_bytes + kb * 16384 + kk * 32, 16, 1024);
-              umma_bf16_elect(tmemS, dq_lo, dk_hi, idesc_s, first ? 0u : 1u);
-              umma_bf16_elect(tmemS, dq_hi, dk_lo, idesc_s, 1u);
-              umma_bf16_elect(tmemS, dq_hi, dk_hi, idesc_s, 1u);
-            } else {
-              umma_bf16_elect(tmemS, dq_hi, dk_hi, idesc_s, first ? 0u : 1u);
-            }
-            first = false;
-          }
-        }
-        umma_commit_elect(b_s);
-        if (lane == 0) mbar_wait(b_p, (uint32_t)t & 1u);        // softmax threads wrote P (and rescaled O)
-        __syncwarp();
-        tc_fence_after();
-        for (int kk2 = 0; kk2 < 2; ++kk2)
-          for (int kk = 0; kk < 4; ++kk) {
-            const uint32_t acc = (t == 0 && kk2 == 0 && kk == 0) ? 0u : 1u;
-            const uint64_t dp_hi = make_desc(aP + kk2 * 16384 + kk * 32, 16, 1024);
-            const uint64_t dv_hi = make_desc(aV + (kk2 * nkb) * 8192 + kk * 2048, 8192, 1024);
-            if (a.dbg_only >= 0) {
-              if (kk2 * 4 + kk == a.dbg_only) umma_bf16_elect(tmemO, dp_hi, dv_hi, idesc_o, 0u);
-              continue;
-            }
-            if (planes == 2) {
-              const uint64_t dp_lo = make_desc(aP + p_bytes + kk2 * 16384 + kk * 32, 16, 1024);
-              const uint64_t dv_lo = make_desc(aV + v_bytes + (kk2 * nkb) * 8192 + kk * 2048, 8192, 1024);
-              umma_bf16_elect(tmemO, dp_lo, dv_hi, idesc_o, acc);
-              umma_bf16_elect(tmemO, dp_hi, dv_lo, idesc_o, 1u);
-              umma_bf16_elect(tmemO, dp_hi, dv_hi, idesc_o, 1u);
-            } else {
-              umma_bf16_elect(tmemO, dp_hi, dv_hi, idesc_o, acc);
-            }
-          }
-        umma_commit_elect(b_pv);
-      }
-    }
-    __syncwarp();
-  } else {
-    // =========================================================== softmax / epilogue warps: one thread per query row
-    const int r = tid, i = q0 + r;
-    const bool row_ok = i < a.N;
-    int gs = 0, ge = 0;
-    if (row_ok) {
-      const int g = find_graph_tc(a.gptr, a.B, i);
-      gs = a.gptr[g];
-      ge = a.gptr[g + 1];
-    }
-    int wlo = row_ok ? gs : 0x7fffffff, whi = row_ok ? ge : 0;   // key range any row of this warp can see
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      wlo = min(wlo, __shfl_xor_sync(0xffffffffu, wlo, o));
-      whi = max(whi, __shfl_xor_sync(0xffffffffu, whi, o));
-    }
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    const uint64_t offs = a.offset + ((a.p_drop > 0.f && a.offset_dev) ? *a.offset_dev : 0ull);
-    const bool use_drop = a.p_drop > 0.f;
-    const uint32_t drop_thr = (uint32_t)fminf(a.p_drop * 4294967296.f, 4294967295.f);
-    const float keep_scale = use_drop ? 1.f / (1.f - a.p_drop) : 1.f;
-    float m = -INFINITY, l = 0.f;
-    uint8_t* prow = sP + (r >> 3) * 1024 + (r & 7) * 128;
-    for (int t = 0; t < ntiles; ++t) {
-      const int key0 = kmin + t * kTile;
-      if (lane == 0) mbar_wait(b_s, (uint32_t)t & 1u);
-      __syncwarp();
-      tc_fence_after();
-      // ---- pass 1: row maximum of the valid (same-graph) logits of this tile
-      float mnew = m;
-      for (int c = 0; c < 8; ++c) {
-        const int ck0 = key0 + c * 16;
-        if (ck0 >= whi || ck0 + 16 <= wlo) continue;           // warp-uniform: no row of this warp sees these keys
-        float v[16];
-        tmem_ld16(tmemS + lane_base + (uint32_t)(c * 16), v);
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int key = ck0 + e;
-          if (key >= gs && key < ge) mnew = fmaxf(mnew, v[e] * a.scale);
-        }
-      }
-      // ---- the accumulated O follows the new maximum (previous P V must have retired first)
-      if (t > 0) {
-        if (lane == 0) mbar_wait(b_pv, (uint32_t)(t - 1) & 1u);
-        __syncwarp();
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, mnew > m)) {
-          const float corr = (m == -INFINITY) ? 1.f : __expf(m - mnew);
-          l *= corr;
-          for (int c = 0; c < (a.hd_pad >> 4); ++c) {
-            uint32_t u[16];
-            tmem_ld16_nowait(tmemO + lane_base + (uint32_t)(c * 16), u);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) u[e] = __float_as_uint(__uint_as_float(u[e]) * corr);
-            tmem_st16(tmemO + lane_base + (uint32_t)(c * 16), u);
-          }
-          tmem_st_wait();
-        }
-      }
-      m = mnew;
-      // ---- pass 2: P = exp(S - m) (dropout applied, denominators from the undropped values), hi/lo split, to smem
-      Philox4 rq;
-      int rq_quad = -1;
-      for (int c = 0; c < 8; ++c) {
-        const int ck0 = key0 + c * 16;
-        const bool skip = ck0 >= whi || ck0 + 16 <= wlo;
-        float v[16];
-        if (!skip) tmem_ld16(tmemS + lane_base + (uint32_t)(c * 16), v);
-        float pv[16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int key = ck0 + e;
-          float p = 0.f;
-          if (!skip && key >= gs && key < ge) {
-            p = __expf(v[e] * a.scale - m);
-            l += p;
-            if (use_drop) {
-              const int jl = key - gs;
-              if ((jl >> 2) != rq_quad) {
-                rq_quad = jl >> 2;
-                rq = philox4x32(a.seed, offs + (uint64_t)(GPS_SITE_ATTN_P + h), ((uint64_t)i << 20) | (uint64_t)rq_quad);
-              }
-              const int k4 = jl & 3;
-              const uint32_t bits = k4 == 0 ? rq.v[0] : k4 == 1 ? rq.v[1] : k4 == 2 ? rq.v[2] : rq.v[3];
-              p = bits >= drop_thr ? p * keep_scale : 0.f;
-            }
-          }
-          pv[e] = p;
-          if (a.dbg && blockIdx.x == 0 && blockIdx.y == 0 && t == 0) {
-            a.dbg[r * 128 + c * 16 + e] = skip ? 0.f : v[e];
-            a.dbg[16384 + r * 128 + c * 16 + e] = p;
-          }
-        }
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          const int c8 = c * 2 + hf;                            // 8-key chunk of the row: 64-key block c8 >> 3, chunk c8 & 7
-          uint8_t* dst = prow + (c8 >> 3) * 16384 + (((c8 & 7) ^ (r & 7)) << 4);
-          uint32_t hw[4], lw[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float x = pv[hf * 8 + 2 * e], y = pv[hf * 8 + 2 * e + 1];
-            __nv_bfloat162 hb = __floats2bfloat162_rn(x, y);
-            hw[e] = *reinterpret_cast<uint32_t*>(&hb);
-            lw[e] = pack_bf16x2(x - __low2float(hb), y - __high2float(hb));
-          }
-          *reinterpret_cast<uint4*>(dst) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-          if (planes == 2) *reinterpret_cast<uint4*>(dst + p_bytes) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-        }
-      }
-      fence_proxy_async();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(b_p);
-    }
-    // ---- epilogue: O / l -> fp32 rows (+ operand planes for the output projection), log-sum-exp for the backward pass
-    if (lane == 0) mbar_wait(b_pv, (uint32_t)(ntiles - 1) & 1u);
-    __syncwarp();
-    tc_fence_after();
-    const float inv = l > 0.f ? 1.f / l : 0.f;
-    for (int c = 0; c < (a.hd_pad >> 4); ++c) {
-      float v[16];
-      tmem_ld16(tmemO + lane_base + (uint32_t)(c * 16), v);
-      if (a.dbg && blockIdx.x == 0 && blockIdx.y == 0)
-        for (int e = 0; e < 16; ++e) a.dbg[32768 + r * 128 + c * 16 + e] = v[e];
-      if (!row_ok) continue;
-#pragma unroll
-      for (int g4 = 0; g4 < 4; ++g4) {
-        const int col = c * 16 + g4 * 4;
-        if (col >= a.hd) continue;
-        const float4 w = make_float4(v[g4 * 4] * inv, v[g4 * 4 + 1] * inv, v[g4 * 4 + 2] * inv, v[g4 * 4 + 3] * inv);
-        st4(a.O + (int64_t)i * a.ldo + (int64_t)h * a.hd + col, w);
-        if (a.Op.hi) planes_store4(a.Op, i, (int64_t)h * a.hd + col, w);
-      }
-    }
-    if (row_ok) a.lse[(int64_t)i * a.H + h] = m + __logf(l);
+  auto load_k = [&](int t) {   // thread 0: K tile t (its slot was released by both warpgroups' S of tile t - 1)
+    if (t > 0) mbar_wait(b_ke, (uint32_t)(t - 1) & 1u);
+    mbar_arrive_expect_tx(b_kf, (uint32_t)(planes * k_bytes));
+    for (int pl = 0; pl < planes; ++pl)
+      for (int kb = 0; kb < NKB; ++kb)
+        tma_tile_3d(smem_u32(sK + pl * k_bytes + kb * 16384), &tmQK, (a.H + h) * a.hd_pad + 64 * kb, kmin + t * kTile, pl,
+                    b_kf);
+  };
+  auto load_v = [&](int t) {   // thread 0: V tile t (after both warpgroups' P V of tile t - 1)
+    if (t > 0) mbar_wait(b_ve, (uint32_t)(t - 1) & 1u);
+    mbar_arrive_expect_tx(b_vf, (uint32_t)(planes * v_bytes));
+    for (int pl = 0; pl < planes; ++pl)
+      for (int kk = 0; kk < 2; ++kk)
+        for (int nb = 0; nb < NKB; ++nb)
+          tma_tile_3d(smem_u32(sV + pl * v_bytes + (kk * NKB + nb) * 8192), &tmV, (2 * a.H + h) * a.hd_pad + 64 * nb,
+                      kmin + t * kTile + 64 * kk, pl, b_vf);
+  };
+  if (tid == 0) {
+    tma_prefetch_desc(&tmQK);
+    tma_prefetch_desc(&tmV);
+    mbar_arrive_expect_tx(b_q, (uint32_t)(planes * q_bytes));
+    for (int pl = 0; pl < planes; ++pl)
+      for (int kb = 0; kb < NKB; ++kb)
+        tma_tile_3d(smem_u32(sQ + pl * q_bytes + kb * 16384), &tmQK, h * a.hd_pad + 64 * kb, q0, pl, b_q);
+    load_k(0);
+    load_v(0);
   }
 
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 4) tmem_dealloc(tmem_base, 256);
+  // =========================================================== MMA / softmax warpgroups
+  // fragment of a 64 x N accumulator: lane of warp w holds rows 16 (w & 3) + lane / 4 (+ 8) of the warpgroup's 64 rows
+  // and columns 8 j + 2 (lane % 4) (+ 1), at acc[4 j + {0, 1}] (row) and acc[4 j + {2, 3}] (row + 8)
+  const int wg = warp >> 2;
+  const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of the first of this lane's two rows
+  const int cq = 2 * (lane & 3);
+  RowState rs[2];
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    RowState& R = rs[u];
+    R.i = q0 + rloc + 8 * u;
+    R.gs = 0; R.ge = 0;
+    if (R.i < a.N) {
+      const int g = find_graph_tc(a.gptr, a.B, R.i);
+      R.gs = a.gptr[g];
+      R.ge = a.gptr[g + 1];
+    }
+    R.m = -INFINITY; R.l = 0.f; R.rq_quad = -1;
+  }
+  const uint64_t offs = a.offset + ((a.p_drop > 0.f && a.offset_dev) ? *a.offset_dev : 0ull);
+  const bool use_drop = a.p_drop > 0.f;
+  const uint32_t drop_thr = (uint32_t)fminf(a.p_drop * 4294967296.f, 4294967295.f);
+  const float keep_scale = use_drop ? 1.f / (1.f - a.p_drop) : 1.f;
+  const bool dump = a.dbg && blockIdx.x == 0 && blockIdx.y == 0;
+
+  float o[NKB * 32];
+#pragma unroll
+  for (int e = 0; e < NKB * 32; ++e) o[e] = 0.f;
+  const uint32_t aQ = smem_u32(sQ) + (uint32_t)wg * 8192u, aK = smem_u32(sK), aV = smem_u32(sV);
+  const int qk_steps = a.hd_pad >> 4;
+  if (lane == 0) mbar_wait(b_q, 0u);
+  __syncwarp();
+  for (int t = 0; t < ntiles; ++t) {
+    const int key0 = kmin + t * kTile;
+    // ---- S = Q K^T
+    float sacc[64];
+#pragma unroll
+    for (int e = 0; e < 64; ++e) sacc[e] = 0.f;
+    if (lane == 0) mbar_wait(b_kf, (uint32_t)t & 1u);
+    __syncwarp();
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < NKB * 4; ++ks) {
+      if (ks < qk_steps) {
+        const uint32_t off = (ks >> 2) * 16384 + (ks & 3) * 32;
+        const uint64_t dq_hi = make_desc(aQ + off, 16, 1024);
+        const uint64_t dk_hi = make_desc(aK + off, 16, 1024);
+        if (SPLIT) {
+          const uint64_t dq_lo = make_desc(aQ + q_bytes + off, 16, 1024);
+          const uint64_t dk_lo = make_desc(aK + k_bytes + off, 16, 1024);
+          wgmma_ss<128, 0, 0>(sacc, dq_lo, dk_hi, 1u);
+          wgmma_ss<128, 0, 0>(sacc, dq_hi, dk_lo, 1u);
+        }
+        wgmma_ss<128, 0, 0>(sacc, dq_hi, dk_hi, 1u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<64>(sacc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(b_ke);
+    if (tid == 0 && t + 1 < ntiles) load_k(t + 1);
+    // ---- online softmax on the registers: row maximum over the valid (same-graph) logits, quad-reduced
+    float corr[2];
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      RowState& R = rs[u];
+      float mnew = R.m;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int key = key0 + 8 * j + cq + e;
+          if (key >= R.gs && key < R.ge) mnew = fmaxf(mnew, sacc[4 * j + 2 * u + e] * a.scale);
+        }
+      mnew = fmaxf(mnew, __shfl_xor_sync(0xffffffffu, mnew, 1));
+      mnew = fmaxf(mnew, __shfl_xor_sync(0xffffffffu, mnew, 2));
+      corr[u] = (R.m == -INFINITY) ? 1.f : __expf(R.m - mnew);
+      R.l *= corr[u];
+      R.m = mnew;
+    }
+#pragma unroll
+    for (int j = 0; j < NKB * 8; ++j) {
+      o[4 * j] *= corr[0]; o[4 * j + 1] *= corr[0];
+      o[4 * j + 2] *= corr[1]; o[4 * j + 3] *= corr[1];
+    }
+    // ---- P = exp(S - m) (dropout applied, denominators from the undropped values), in place of S
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      RowState& R = rs[u];
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int key = key0 + 8 * j + cq + e;
+          float& v = sacc[4 * j + 2 * u + e];
+          const float sraw = v;
+          float pr = 0.f;
+          if (key >= R.gs && key < R.ge) {
+            pr = __expf(v * a.scale - R.m);
+            R.l += pr;
+            if (use_drop) {
+              const int jl = key - R.gs;
+              if ((jl >> 2) != R.rq_quad) {
+                R.rq_quad = jl >> 2;
+                R.rq = philox4x32(a.seed, offs + (uint64_t)(GPS_SITE_ATTN_P + h), ((uint64_t)R.i << 20) | (uint64_t)R.rq_quad);
+              }
+              const int k4 = jl & 3;
+              const uint32_t bits = k4 == 0 ? R.rq.v[0] : k4 == 1 ? R.rq.v[1] : k4 == 2 ? R.rq.v[2] : R.rq.v[3];
+              pr = bits >= drop_thr ? pr * keep_scale : 0.f;
+            }
+          }
+          v = pr;
+          if (dump && t == 0) {
+            const int r = rloc + 8 * u, c = 8 * j + cq + e;
+            a.dbg[r * 128 + c] = sraw;
+            a.dbg[16384 + r * 128 + c] = pr;
+          }
+        }
+    }
+    // ---- O += P V: the S fragment of keys [16 ks, 16 ks + 16) is the register A fragment of k-step ks
+    uint32_t ph[32], pl[SPLIT ? 32 : 1];
+#pragma unroll
+    for (int x = 0; x < 32; ++x) {
+      const float p0 = sacc[2 * x], p1 = sacc[2 * x + 1];
+      __nv_bfloat162 hb = __floats2bfloat162_rn(p0, p1);
+      ph[x] = *reinterpret_cast<uint32_t*>(&hb);
+      if (SPLIT) pl[x] = pack_bf16x2(p0 - __low2float(hb), p1 - __high2float(hb));
+    }
+    if (lane == 0) mbar_wait(b_vf, (uint32_t)t & 1u);
+    __syncwarp();
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      const uint32_t voff = ((ks >> 2) * NKB) * 8192 + (ks & 3) * 2048;
+      const uint64_t dv_hi = make_desc(aV + voff, 8192, 1024);
+      if (SPLIT) {
+        const uint64_t dv_lo = make_desc(aV + v_bytes + voff, 8192, 1024);
+        wgmma_rs<NKB * 64, 1>(o, pl + 4 * ks, dv_hi, 1u);
+        wgmma_rs<NKB * 64, 1>(o, ph + 4 * ks, dv_lo, 1u);
+      }
+      wgmma_rs<NKB * 64, 1>(o, ph + 4 * ks, dv_hi, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<NKB * 32>(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(b_ve);
+    if (tid == 0 && t + 1 < ntiles) load_v(t + 1);
+  }
+  // ---- epilogue: O / l -> fp32 rows (+ operand planes for the output projection), log-sum-exp for the backward pass
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    RowState& R = rs[u];
+    R.l += __shfl_xor_sync(0xffffffffu, R.l, 1);
+    R.l += __shfl_xor_sync(0xffffffffu, R.l, 2);
+    const float inv = R.l > 0.f ? 1.f / R.l : 0.f;
+    const bool row_ok = R.i < a.N;
+#pragma unroll
+    for (int j = 0; j < NKB * 8; ++j) {
+      const int col = 8 * j + cq;
+      const float v0 = o[4 * j + 2 * u], v1 = o[4 * j + 2 * u + 1];
+      if (dump) {
+        a.dbg[32768 + (rloc + 8 * u) * 128 + col] = v0;
+        a.dbg[32768 + (rloc + 8 * u) * 128 + col + 1] = v1;
+      }
+      if (!row_ok || col >= a.hd) continue;
+      const float w0 = v0 * inv, w1 = v1 * inv;
+      float* dst = a.O + (int64_t)R.i * a.ldo + (int64_t)h * a.hd + col;
+      dst[0] = w0;
+      dst[1] = w1;
+      if (a.Op.hi) {
+        const int64_t off = (int64_t)R.i * a.Op.ld + (int64_t)h * a.hd + col;
+        __nv_bfloat162 hb = __floats2bfloat162_rn(w0, w1);
+        *reinterpret_cast<__nv_bfloat162*>(a.Op.hi + off) = hb;
+        if (a.Op.lo) *reinterpret_cast<uint32_t*>(a.Op.lo + off) = pack_bf16x2(w0 - __low2float(hb), w1 - __high2float(hb));
+      }
+    }
+    if (row_ok && (lane & 3) == 0) a.lse[(int64_t)R.i * a.H + h] = R.m + __logf(R.l);
+  }
+}
+
+template <int NKB, bool SPLIT>
+int launch_attn(const CUtensorMap& tQK, const CUtensorMap& tV, const AttnTcArgs& a, dim3 grid, size_t smem,
+                cudaStream_t stream) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    GPS_CUDA(cudaFuncSetAttribute(k_attn_tc_fwd<NKB, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_done = true;
+  }
+  k_attn_tc_fwd<NKB, SPLIT><<<grid, kThreadsA, smem, stream>>>(tQK, tV, a);
+  GPS_LAUNCH_CHECK();
+  return GPS_OK;
 }
 
 float* g_attn_dbg = nullptr;
@@ -347,23 +343,17 @@ int attention_tc_fwd(const GpsGraph& g, int64_t heads, int64_t hd, Planes qkv, f
   a.O = O; a.ldo = ldo; a.Op = Op; a.lse = lse;
   a.scale = 1.f / sqrtf((float)hd); a.p_drop = p_drop; a.seed = seed; a.offset = offset; a.offset_dev = offset_dev;
   a.dbg = g_attn_dbg;
-  a.dbg_only = getenv("GPS_ATTN_DBG_ONLY") ? atoi(getenv("GPS_ATTN_DBG_ONLY")) : -1;
   const int64_t cols = 3 * heads * a.hd_pad;
   CUtensorMap tQK, tV;
   GPS_TRY(make_tensor_map(qkv.hi, qkv.lo, a.planes, g.N, cols, qkv.ld, 128, &tQK));
   GPS_TRY(make_tensor_map(qkv.hi, qkv.lo, a.planes, g.N, cols, qkv.ld, 64, &tV));
   const int nkb = (a.hd_pad + 63) >> 6;
-  const size_t tiles = (size_t)a.planes * ((size_t)nkb * 16384 * 2 + (size_t)2 * nkb * 8192 + (nkb == 2 ? 0 : 2 * 16384));
-  const size_t smem = tiles + 1024 + 256;
-  static bool attr_done = false;
-  if (!attr_done) {
-    GPS_CUDA(cudaFuncSetAttribute(k_attn_tc_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_done = true;
-  }
+  const size_t smem = (size_t)a.planes * nkb * (16384 + 16384 + 16384) + 1024 + 256;
   dim3 grid((unsigned)ceil_div(g.N, kTile), (unsigned)heads);
-  k_attn_tc_fwd<<<grid, kThreadsA, smem, stream>>>(tQK, tV, a);
-  GPS_LAUNCH_CHECK();
-  return GPS_OK;
+  if (nkb == 1) return a.planes == 2 ? launch_attn<1, true>(tQK, tV, a, grid, smem, stream)
+                                     : launch_attn<1, false>(tQK, tV, a, grid, smem, stream);
+  return a.planes == 2 ? launch_attn<2, true>(tQK, tV, a, grid, smem, stream)
+                       : launch_attn<2, false>(tQK, tV, a, grid, smem, stream);
 }
 
 }  // namespace gps

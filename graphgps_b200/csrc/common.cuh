@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for libgps_b200 (sm_100a only).
+// common.cuh — shared device/host helpers for libgps_b200 (sm_90a).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -42,7 +42,7 @@ void count_launch();  // every kernel launch of the library is counted (gps_laun
     if (_rc != GPS_OK) return _rc; \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 constexpr float kBnEps = 1e-5f;
 constexpr float kBnMomentum = 0.1f;
 

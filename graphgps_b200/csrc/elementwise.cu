@@ -4,6 +4,8 @@
 // One skeleton (k_rowwise): a thread owns one float4 column group and strides over rows, so the
 // per-column BatchNorm constants live in registers and the column statistics are reduced
 // per-thread -> per-CTA (shared memory) -> global (double atomics).  All loads/stores are 128-bit.
+#include <cooperative_groups.h>
+
 #include "kernels.cuh"
 
 namespace gps {
@@ -321,26 +323,38 @@ struct OpAdd3 {
   __device__ void finish(int, int) {}
 };
 
-// out[c] += sum_r a[r, c]: thread -> CTA (shared memory over threadIdx.y) -> one float atomic per column per CTA
-__global__ void __launch_bounds__(1024) k_colsum(const float* __restrict__ a, int64_t lda, int64_t rows,
+// out[c] += sum_r a[r, c]: thread -> CTA (shared memory over threadIdx.y) -> the kColsumCtas CTAs of one cluster
+// (grid y), in rank order through distributed shared memory -> one float add per column, so the sum is the same in every
+// run.  grid x walks column chunks of blockDim.x float4 columns.
+constexpr int kColsumCtas = 8;
+__global__ void __launch_bounds__(1024) k_colsum(const float* __restrict__ a, int64_t lda, int64_t rows, int C4,
                                                  float* __restrict__ out) {
   extern __shared__ float4 sm[];
-  const int c4 = threadIdx.x, ry = threadIdx.y, RY = blockDim.y, C4 = blockDim.x;
+  const int ry = threadIdx.y, RY = blockDim.y, CB = blockDim.x;
+  const int c4 = blockIdx.x * CB + threadIdx.x;
+  const bool col_ok = c4 < C4;
   float4 acc = f4zero();
-  for (int64_t r = (int64_t)blockIdx.x * RY + ry; r < rows; r += (int64_t)gridDim.x * RY)
-    acc = f4add(acc, ld4(a + r * lda + c4 * 4));
+  if (col_ok)
+    for (int64_t r = (int64_t)blockIdx.y * RY + ry; r < rows; r += (int64_t)gridDim.y * RY)
+      acc = f4add(acc, ld4(a + r * lda + c4 * 4));
   if (RY > 1) {
-    sm[ry * C4 + c4] = acc;
+    sm[ry * CB + threadIdx.x] = acc;
     __syncthreads();
     if (ry == 0)
-      for (int y = 1; y < RY; ++y) acc = f4add(acc, sm[y * C4 + c4]);
+      for (int y = 1; y < RY; ++y) acc = f4add(acc, sm[y * CB + threadIdx.x]);
   }
-  if (ry == 0) {
-    atomicAdd(out + c4 * 4 + 0, acc.x);
-    atomicAdd(out + c4 * 4 + 1, acc.y);
-    atomicAdd(out + c4 * 4 + 2, acc.z);
-    atomicAdd(out + c4 * 4 + 3, acc.w);
+  if (ry == 0) sm[threadIdx.x] = acc;   // row-0 slots: read above only by the thread that now overwrites them
+  cooperative_groups::cluster_group cluster = cooperative_groups::this_cluster();
+  cluster.sync();
+  if (blockIdx.y == 0 && ry == 0 && col_ok) {
+    float4 tot = f4zero();
+    for (int k = 0; k < (int)gridDim.y; ++k) tot = f4add(tot, cluster.map_shared_rank(sm, k)[threadIdx.x]);
+    atomicAdd(out + c4 * 4 + 0, tot.x);   // the only adder of this element
+    atomicAdd(out + c4 * 4 + 1, tot.y);
+    atomicAdd(out + c4 * 4 + 2, tot.z);
+    atomicAdd(out + c4 * 4 + 3, tot.w);
   }
+  cluster.sync();   // no CTA leaves while rank 0 still reads its shared memory
 }
 
 template <class Op>
@@ -430,9 +444,23 @@ int add3(const float* a, int64_t lda, const float* b, int64_t ldb, const float* 
 
 int colsum(const float* a, int64_t lda, int64_t rows, int64_t d, float* out, cudaStream_t stream) {
   if (rows == 0) return GPS_OK;
-  RowGeom g;
-  GPS_TRY(row_geom(rows, d, 1, &g));
-  k_colsum<<<g.grid, g.block, g.smem, stream>>>(a, lda, rows, out);
+  GPS_REQUIRE(d > 0 && d % 4 == 0, GPS_ERR_UNSUPPORTED, "colsum needs d %% 4 == 0 (got %lld)", (long long)d);
+  const int C4 = (int)(d / 4);
+  const int CB = C4 < 128 ? C4 : 128;                // float4 columns per CTA
+  const int RY = 1024 / CB < 16 ? 1024 / CB : 16;    // row lanes per CTA
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)ceil_div(C4, CB), kColsumCtas);   // one cluster per column chunk
+  cfg.blockDim = dim3(CB, RY);
+  cfg.dynamicSmemBytes = (size_t)RY * CB * sizeof(float4);
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 1;
+  attr[0].val.clusterDim.y = kColsumCtas;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  GPS_CUDA(cudaLaunchKernelEx(&cfg, k_colsum, a, lda, rows, C4, out));
   GPS_LAUNCH_CHECK();
   return GPS_OK;
 }

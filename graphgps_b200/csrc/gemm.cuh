@@ -55,7 +55,7 @@ struct GemmParams {
 struct ToPlanesItem { const float* src; int64_t ld; int rows; int cols; Planes dst; };
 // fp32 [rows, cols] (pitch ld) -> bf16 hi/lo planes, up to 16 matrices per launch
 int to_planes(const ToPlanesItem* items, int n, cudaStream_t stream);
-// TMA-fed tcgen05 product on plane operands; GPS_ERR_UNSUPPORTED when the planes are missing / misaligned
+// TMA-fed wgmma product on plane operands; GPS_ERR_UNSUPPORTED when the planes are missing / misaligned
 int gemm_tma(const GemmParams& p, cudaStream_t stream);
 // rank-3 tensor map {cols, rows, planes} over a plane pair with a {64, box_rows, 1} SWIZZLE_128B box (cached)
 int make_tensor_map(const __nv_bfloat16* hi, const __nv_bfloat16* lo, int planes, int64_t rows, int64_t cols, int64_t ld,
@@ -63,7 +63,7 @@ int make_tensor_map(const __nv_bfloat16* hi, const __nv_bfloat16* lo, int planes
 void gemm_tma_set_force_bn(int bn);
 void gemm_tma_set_trace(unsigned long long* buf);   // bring-up: per-CTA phase timestamps (tools/gemm_trace.py)
 
-// Pre-packs up to 8 weight matrices (fp32 [rows, K] row-major) into the tcgen05 kernel's shared-memory tile image.
+// Pre-packs up to 8 weight matrices (fp32 [rows, K] row-major) into the wgmma kernel's shared-memory tile image.
 // K-major (mn = 0): W is [rows x K], dst sized by prepack_bytes(rows, K).
 // MN-major (mn = 1): W is [K x rows] (rows = GEMM output columns), dst sized by prepack_bytes_mn(rows, K).
 struct PrepackItem { const float* W; int rows; int K; int ld; void* dst; int mn; };
@@ -77,7 +77,7 @@ int prepack_weights(const PrepackItem* items, int n, cudaStream_t stream);
 
 // exact fp32 CUDA-core product (validation path and shapes the tensor-core kernel does not take)
 int gemm_simt(const GemmParams& p, cudaStream_t stream);
-// tcgen05 tensor-core product; returns GPS_ERR_UNSUPPORTED for shapes it does not take
+// register-staged wgmma tensor-core product; returns GPS_ERR_UNSUPPORTED for shapes it does not take
 int gemm_tc(const GemmParams& p, cudaStream_t stream);
 void gemm_tc_set_debug(int v);
 // dispatcher used by the layer

@@ -1,27 +1,26 @@
-// gemm_tc.cu — tcgen05 (5th-gen tensor core) dense product for every Linear of the GPS layer and
+// gemm_tc.cu — wgmma (Hopper warpgroup MMA) dense product for every Linear of the GPS layer and
 // their data/weight gradients, with the layer's fused epilogues.
 //
 //   C[M,N] (+)= epi( Aop[M,K] * Bop[K,N] ),  fp32 in HBM, bf16 operands on the tensor cores,
-//   fp32 accumulation in TMEM.  precision FP32: split-bf16 x3 (hi*hi + hi*lo + lo*hi, ~2^-16
+//   fp32 accumulation in registers.  precision FP32: split-bf16 x3 (hi*hi + hi*lo + lo*hi, ~2^-16
 //   relative), precision BF16: a single bf16 pass.
 //
-// One 128 x BN output tile per CTA (BN a runtime multiple of 16 up to 256; wide tiles matter: the kernel
-// is bound by L2->SM operand traffic, M*N*K*4*(1/BM + 1/BN) bytes):
+// One 128 x BN output tile per CTA (BN = 64 or 128, the wgmma instruction shape):
 //   * warps 0-7 stage operands: coalesced 128-bit global loads of the fp32 tiles -> bf16 hi/lo split in
-//     registers -> 16-byte st.shared into the canonical UMMA SWIZZLE_128B layout (K-major when the
+//     registers -> 16-byte st.shared into the canonical SWIZZLE_128B layout (K-major when the
 //     reduction dim is contiguous in HBM, MN-major when it is the row dim, e.g. weight gradients
 //     dW = G^T X) -> fence.proxy.async -> one mbarrier arrive per warp.  All per-chunk addresses are
 //     (value for chunk 0) + q * constant, computed once per CTA.  No transposes, no separate conversion
 //     pass; the fp32->bf16 split costs no extra HBM bytes.
-//   * warp 8: one elected lane issues tcgen05.mma.cta_group::1.kind::f16 (UMMA 128 x BN x 16) per
-//     16-wide K step; tcgen05.commit releases the smem stage / signals the epilogue.
-//   * epilogue (warps 0-7): tcgen05.ld 32x32b.x16 -> bias / activation / act' mask / dropout /
+//   * warps 8-15: two consumer warpgroups, each issuing wgmma m64 x BN x k16 for its 64 rows of the tile per
+//     16-wide K step, one commit group per k-block; a stage is released once its group has retired.  After the
+//     last k-block the accumulators go to a shared staging tile (the operand stages are free by then).
+//   * epilogue (warps 0-7): staging tile -> bias / activation / act' mask / dropout /
 //     residuals / 128-bit stores; BatchNorm column sums by a warp butterfly reduce-scatter + double
 //     atomics; split-K partials by fp32 atomics; bias-gradient column sums from the staged A tile.
-// Smem stages form an mbarrier ring (full: one arrival per producer warp; empty: tcgen05.commit).
-// Measured lessons kept in the code: per-thread mbarrier arrivals (256 per stage) serialise on the
-// barrier unit (~1 us per k-block) -> per-warp arrivals; per-chunk integer divisions made the producers
-// issue-bound -> precomputed addressing (tools/gemm_triage.py has the switches and the clock64 trace).
+// Smem stages form an mbarrier ring (full: one arrival per producer warp; empty: one arrival per consumer warp).
+// Per-thread mbarrier arrivals (256 per stage) serialise on the barrier unit, hence per-warp arrivals; per-chunk
+// integer divisions make the producers issue-bound, hence the precomputed addressing.
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -33,12 +32,12 @@ namespace gps {
 
 namespace {
 
-constexpr int BM = 128;          // UMMA M
+constexpr int BM = 128;          // two wgmma M = 64 warpgroups
 constexpr int BK = 64;           // k-block: one 128-byte swizzle row of bf16
 constexpr int kProducerWarps = 8;           // operand staging + epilogue
 constexpr int kProducerThreads = kProducerWarps * 32;
-constexpr int kMmaWarp = kProducerWarps;
-constexpr int kThreads = (kMmaWarp + 1) * 32;
+constexpr int kConsumerWarps = 8;           // two MMA warpgroups
+constexpr int kThreads = (kProducerWarps + kConsumerWarps) * 32;
 constexpr int kATileBytes = BM * BK * 2;       // 16 KB
 constexpr int kBBlockBytes = 64 * BK * 2;      // 8 KB per 64 columns of B
 using namespace tc;   // PTX wrappers: tc_ptx.cuh
@@ -60,11 +59,10 @@ __device__ __forceinline__ uint32_t chunk_offset(int c, int tile_rows) {
 
 struct TcArgs {
   GemmParams p;
-  int BN;          // tile width (multiple of 16, <= 256)
-  int nb_blocks;   // ceil(BN / 64)
+  int BN;          // tile width (64 or 128)
+  int nb_blocks;   // BN / 64
   int stages;
   int kb_per_split;
-  int tmem_cols;
   const uint8_t* bpk_hi;   // pre-packed K-major B planes (BPRE variants), else null
   const uint8_t* bpk_lo;
   int bpk_groups;          // 8-row groups per k-block in the packed planes
@@ -74,16 +72,15 @@ struct TcArgs {
   int debug;       // perf-triage switches (gps_debug_set): 1 no global loads, 2 no convert/store, 4 no MMA, 8 no epilogue
 };
 
-// NBC = B chunks per producer thread per k-block (2: tiles up to 64 columns, 8: up to 256).  The narrow variant
-// fits in 112 registers and ~100 KB of shared memory, so two CTAs share an SM and one CTA's load/convert phase
-// overlaps the other's MMA/epilogue phase.
+// BN_T = tile width; a producer thread stages BN_T / 32 B chunks per k-block.
 // BPRE: the B operand (an nn.Linear weight) was pre-packed once per step by k_prepack_weights into bf16 hi/lo
 // planes that already have the shared-memory image of a tile (SWIZZLE_128B; K-major: 8-row groups, MN-major:
 // 64-column blocks; one 64-deep k-block after the other), so a stage's B tile is ONE contiguous range: a single
 // elected thread fetches it with bulk TMA (cp.async.bulk ... mbarrier::complete_tx) and the producer warps only
 // stage A.  K-major planes serve y = x W^T (forward), MN-major planes serve g_x = g_y W (data gradients).
-template <bool A_MN, bool B_MN, bool SPLIT, int NBC, bool BPRE>
-__global__ void __launch_bounds__(kThreads, NBC == 2 ? 2 : 1) k_gemm_tc(const TcArgs a) {
+template <bool A_MN, bool B_MN, bool SPLIT, int BN_T, bool BPRE>
+__global__ void __launch_bounds__(kThreads, 1) k_gemm_tc(const TcArgs a) {
+  constexpr int NBC = BN_T / 32;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const GemmParams& p = a.p;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -92,9 +89,10 @@ __global__ void __launch_bounds__(kThreads, NBC == 2 ? 2 : 1) k_gemm_tc(const Tc
   const int stage_bytes = plane * (kATileBytes + b_tile_bytes);
   const int S = a.stages;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);
-  // bars[0..S) full, bars[S..2S) empty, bars[2S] accumulator complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 1);
-  float* red = reinterpret_cast<float*>(tmem_slot + 2);  // 16 x 16 x 8 floats (bias-gradient partials)
+  // bars[0..S) full, bars[S..2S) empty
+  float* red = reinterpret_cast<float*>(bars + 2 * S + 2);  // 16 x 16 x 8 floats (bias-gradient partials)
+  float* stage = reinterpret_cast<float*>(smem);            // epilogue staging tile [128][BN + 4], over the stages
+  const int sld = a.BN + 4;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * a.BN;
@@ -106,53 +104,64 @@ __global__ void __launch_bounds__(kThreads, NBC == 2 ? 2 : 1) k_gemm_tc(const Tc
   if (tid == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(smem_u32(&bars[s]), kProducerWarps + (BPRE ? 1 : 0));
-      mbar_init(smem_u32(&bars[S + s]), 1);
+      mbar_init(smem_u32(&bars[S + s]), kConsumerWarps);
     }
-    mbar_init(smem_u32(&bars[2 * S]), 1);
     fence_barrier_init();
   }
-  if (warp == kMmaWarp) tmem_alloc(smem_u32(tmem_slot), (uint32_t)a.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == kMmaWarp) {
-    // =========================================================== MMA issuer
-    if (lane == 0 && nkb > 0) {
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((A_MN ? 1u : 0u) << 15) | ((B_MN ? 1u : 0u) << 16) |
-                             ((uint32_t)(a.BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      const uint32_t a_lbo = A_MN ? kBBlockBytes : 16, b_lbo = B_MN ? kBBlockBytes : 16;
-      const uint32_t a_kstep = A_MN ? 2048 : 32, b_kstep = B_MN ? 2048 : 32;
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % S;
-        mbar_wait(smem_u32(&bars[s]), (uint32_t)(i / S) & 1u);
-        tc_fence_after();
-        const uint32_t sa_hi = smem_u32(smem + (size_t)s * stage_bytes);
-        const uint32_t sb_hi = sa_hi + plane * kATileBytes;
-        const uint32_t sa_lo = sa_hi + kATileBytes;
-        const uint32_t sb_lo = sb_hi + b_tile_bytes;
-        if (!(a.debug & 4)) {
+  if (warp >= kProducerWarps) {
+    // =========================================================== MMA warpgroups
+    // warpgroup wg owns accumulator rows [64 wg, 64 wg + 64): its A operand starts 8 KB into every A plane
+    // (eight 1 KB K-major row groups, or the second 64-row MN-major block)
+    const int wg = (warp - kProducerWarps) >> 2;
+    float acc[BN_T / 2];
 #pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint64_t da_hi = make_desc(sa_hi + kk * a_kstep, a_lbo, 1024);
-            const uint64_t db_hi = make_desc(sb_hi + kk * b_kstep, b_lbo, 1024);
-            if (SPLIT) {
-              const uint64_t da_lo = make_desc(sa_lo + kk * a_kstep, a_lbo, 1024);
-              const uint64_t db_lo = make_desc(sb_lo + kk * b_kstep, b_lbo, 1024);
-              umma_bf16(tmem_base, da_lo, db_hi, idesc, (i | kk) != 0);
-              umma_bf16(tmem_base, da_hi, db_lo, idesc, 1u);
-              umma_bf16(tmem_base, da_hi, db_hi, idesc, 1u);
-            } else {
-              umma_bf16(tmem_base, da_hi, db_hi, idesc, (i | kk) != 0);
-            }
+    for (int e = 0; e < BN_T / 2; ++e) acc[e] = 0.f;
+    constexpr uint32_t a_lbo = A_MN ? kBBlockBytes : 16, b_lbo = B_MN ? kBBlockBytes : 16;
+    constexpr uint32_t a_kstep = A_MN ? 2048 : 32, b_kstep = B_MN ? 2048 : 32;
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % S;
+      if (lane == 0) mbar_wait(smem_u32(&bars[s]), (uint32_t)(i / S) & 1u);
+      __syncwarp();
+      const uint32_t sa_hi = smem_u32(smem + (size_t)s * stage_bytes) + (uint32_t)wg * 8192u;
+      const uint32_t sb_hi = smem_u32(smem + (size_t)s * stage_bytes) + plane * kATileBytes;
+      const uint32_t sa_lo = sa_hi + kATileBytes;
+      const uint32_t sb_lo = sb_hi + b_tile_bytes;
+      if (!(a.debug & 4)) {
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / 16; ++kk) {
+          const uint64_t da_hi = make_desc(sa_hi + kk * a_kstep, a_lbo, 1024);
+          const uint64_t db_hi = make_desc(sb_hi + kk * b_kstep, b_lbo, 1024);
+          if (SPLIT) {
+            const uint64_t da_lo = make_desc(sa_lo + kk * a_kstep, a_lbo, 1024);
+            const uint64_t db_lo = make_desc(sb_lo + kk * b_kstep, b_lbo, 1024);
+            wgmma_ss<BN_T, A_MN, B_MN>(acc, da_lo, db_hi, 1u);
+            wgmma_ss<BN_T, A_MN, B_MN>(acc, da_hi, db_lo, 1u);
           }
+          wgmma_ss<BN_T, A_MN, B_MN>(acc, da_hi, db_hi, 1u);
         }
-        umma_commit(smem_u32(&bars[S + s]));  // frees the smem stage once these MMAs retire
+        wgmma_commit();
       }
-      umma_commit(smem_u32(&bars[2 * S]));    // accumulator complete
+      // at most one group in flight: the previous k-block's MMAs have retired, so its stage goes back to the producers
+      wgmma_wait<1>();
+      reg_fence<BN_T / 2>(acc);
+      __syncwarp();
+      if (i > 0 && lane == 0) mbar_arrive(smem_u32(&bars[S + (i - 1) % S]));
     }
-    __syncwarp();
+    wgmma_wait<0>();
+    reg_fence<BN_T / 2>(acc);
+    asm volatile("bar.sync 2, 256;" ::: "memory");   // both warpgroups are done with the operand stages
+    // wgmma fragment: lane of warp w holds rows 16 (w & 3) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) (+ 1)
+    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int c = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN_T / 8; ++j) {
+      *reinterpret_cast<float2*>(stage + r * sld + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(stage + (r + 8) * sld + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+    asm volatile("barrier.sync 3, %0;" ::"n"(kThreads) : "memory");   // staging tile complete -> epilogue
   } else {
     // =========================================================== operand producers
     // chunk c = tid + 256 q: every per-q quantity is (value at q = 0) + q * constant
@@ -268,11 +277,7 @@ __global__ void __launch_bounds__(kThreads, NBC == 2 ? 2 : 1) k_gemm_tc(const Tc
     }
 
     // =========================================================== epilogue
-    if (nkb > 0) {
-      if (lane == 0) mbar_wait(smem_u32(&bars[2 * S]), 0u);
-      __syncwarp();
-      tc_fence_after();
-    }
+    asm volatile("barrier.sync 3, %0;" ::"n"(kThreads) : "memory");
     const int q = warp & 3, half = warp >> 2;
     const int row = m0 + q * 32 + lane;
     const bool row_ok = row < p.M;
@@ -281,10 +286,10 @@ __global__ void __launch_bounds__(kThreads, NBC == 2 ? 2 : 1) k_gemm_tc(const Tc
       const int gn = n0 + c * 16;
       if (gn >= p.N) break;
       float v[16];
-      if (nkb > 0) tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 16), v);
-      else {
 #pragma unroll
-        for (int e = 0; e < 16; ++e) v[e] = 0.f;
+      for (int e = 0; e < 16; e += 4) {
+        const float4 t = *reinterpret_cast<const float4*>(stage + (q * 32 + lane) * sld + c * 16 + e);
+        v[e] = t.x; v[e + 1] = t.y; v[e + 2] = t.z; v[e + 3] = t.w;
       }
         if (p.splitk > 1) {
           if (row_ok) {
@@ -390,10 +395,6 @@ __global__ void __launch_bounds__(kThreads, NBC == 2 ? 2 : 1) k_gemm_tc(const Tc
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == kMmaWarp) tmem_dealloc(tmem_base, (uint32_t)a.tmem_cols);
 }
 
 int g_tc_debug = 0;
@@ -401,15 +402,15 @@ int g_tc_force_bn = 0;
 
 inline bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
-template <bool A_MN, bool B_MN, bool SPLIT, int NBC, bool BPRE>
+template <bool A_MN, bool B_MN, bool SPLIT, int BN_T, bool BPRE>
 int launch1(const TcArgs& a, dim3 grid, size_t smem, cudaStream_t stream) {
   static bool attr_done = false;
   if (!attr_done) {
-    GPS_CUDA(cudaFuncSetAttribute(k_gemm_tc<A_MN, B_MN, SPLIT, NBC, BPRE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    GPS_CUDA(cudaFuncSetAttribute(k_gemm_tc<A_MN, B_MN, SPLIT, BN_T, BPRE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   227 * 1024));
     attr_done = true;
   }
-  k_gemm_tc<A_MN, B_MN, SPLIT, NBC, BPRE><<<grid, kThreads, smem, stream>>>(a);
+  k_gemm_tc<A_MN, B_MN, SPLIT, BN_T, BPRE><<<grid, kThreads, smem, stream>>>(a);
   GPS_LAUNCH_CHECK();
   return GPS_OK;
 }
@@ -417,11 +418,11 @@ template <bool A_MN, bool B_MN, bool SPLIT>
 int launch(const TcArgs& a, dim3 grid, size_t smem, cudaStream_t stream) {
   if constexpr (!A_MN) {
     if (a.bpk_hi)
-      return a.nb_blocks == 1 ? launch1<false, B_MN, SPLIT, 2, true>(a, grid, smem, stream)
-                              : launch1<false, B_MN, SPLIT, 8, true>(a, grid, smem, stream);
+      return a.nb_blocks == 1 ? launch1<false, B_MN, SPLIT, 64, true>(a, grid, smem, stream)
+                              : launch1<false, B_MN, SPLIT, 128, true>(a, grid, smem, stream);
   }
-  return a.nb_blocks == 1 ? launch1<A_MN, B_MN, SPLIT, 2, false>(a, grid, smem, stream)
-                          : launch1<A_MN, B_MN, SPLIT, 8, false>(a, grid, smem, stream);
+  return a.nb_blocks == 1 ? launch1<A_MN, B_MN, SPLIT, 64, false>(a, grid, smem, stream)
+                          : launch1<A_MN, B_MN, SPLIT, 128, false>(a, grid, smem, stream);
 }
 
 }  // namespace
@@ -462,40 +463,37 @@ int gemm_tc(const GemmParams& p, cudaStream_t stream) {
   const int plane = split ? 2 : 1;
   const int mt = (int)ceil_div(p.M, BM);
   const int nkb = (int)ceil_div(p.K, BK);
-  const int splits_hint = p.splitk > 1 ? (p.splitk < nkb ? p.splitk : nkb) : 1;
 
-  // tile width: BN in {64,128,256}-block granularity (1, 2 or 4 staged 64-column blocks); the kernel is bound
-  // by operand traffic ~ tiles x (128 + staged B rows), so minimise waves x staged rows, wider on ties
+  // tile width: BN in {64, 128} (1 or 2 staged 64-column blocks; the two warpgroups hold 128 x BN fp32 accumulators
+  // beside the producers' staging registers); the kernel is bound by operand traffic ~ tiles x (128 + staged B rows),
+  // so minimise waves x staged rows, wider on ties
   const bool pre_k = p.bpk && !p.bpk_mn && !p.ta && !p.tb && p.bpk_row0 % 8 == 0 && (split ? p.bpk_lo_off > 0 : true);
   const bool pre_mn = p.bpk && p.bpk_mn && !p.ta && p.tb && p.bpk_row0 % 64 == 0 && (split ? p.bpk_lo_off > 0 : true);
   int bestBN = 128;
   long bestCost = -1;
-  for (int nt = (int)ceil_div(p.N, 256); nt <= (int)ceil_div(p.N, 48) + 1; ++nt) {
-    int bn = (int)round_up(ceil_div(p.N, nt), pre_mn ? 64 : 16);   // MN-major planes are cut at 64-column blocks
-    if (bn > 256) continue;
-    if (bn < 16) bn = 16;
-    int nb = bn <= 64 ? 1 : bn <= 128 ? 2 : 4;
-    long tiles = (long)mt * ceil_div(p.N, bn) * splits_hint;
-    long waves = ceil_div(tiles, nb == 1 ? 2L * kNumSMs : (long)kNumSMs);   // narrow tiles: two CTAs per SM
-    long cost = waves * (BM + nb * 64L);
+  for (int bn = 128; bn >= 64; bn >>= 1) {
+    const int nb = bn / 64;
+    const long tiles = (long)mt * ceil_div(p.N, bn);
+    const long waves = ceil_div(tiles, (long)kNumSMs);
+    const long cost = waves * (BM + nb * 64L);
     if (bestCost < 0 || cost < bestCost) { bestCost = cost; bestBN = bn; }
   }
-  if (g_tc_force_bn > 0 && !(pre_mn && g_tc_force_bn % 64)) bestBN = g_tc_force_bn;   // tuning hook (tools/gemm_tune.py)
+  if (g_tc_force_bn == 64 || g_tc_force_bn == 128) bestBN = g_tc_force_bn;   // tuning hook (tools/gemm_tune.py)
   TcArgs a;
   a.p = p;
   a.BN = bestBN;
-  a.nb_blocks = a.BN <= 64 ? 1 : a.BN <= 128 ? 2 : 4;
+  a.nb_blocks = a.BN / 64;
   const int stage_bytes = plane * (kATileBytes + a.nb_blocks * kBBlockBytes);
-  int stages = ((a.nb_blocks == 1 ? 100 : 200) * 1024) / stage_bytes;   // narrow tiles leave room for a second CTA
+  int stages = (200 * 1024) / stage_bytes;
   if (stages > 4) stages = 4;
-  if (stages < 2) return GPS_ERR_UNSUPPORTED;
+  if (stages < 2) return GPS_ERR_UNSUPPORTED;   // (two stages also hold the epilogue's fp32 staging tile)
   a.stages = stages;
-  int splitk = p.splitk > 1 ? p.splitk : 1;
-  if (splitk > nkb) splitk = nkb;
-  a.kb_per_split = (int)ceil_div(nkb, splitk);
-  splitk = (int)ceil_div(nkb, a.kb_per_split);
+  // splitk > 1 keeps its meaning "add into the pre-zeroed C", but the reduction is not split across CTAs: every
+  // element then has a single adder and the result does not depend on the order in which CTAs finish (the TMA
+  // kernel, which the layer uses, splits K deterministically within a cluster)
+  const int splitk = 1;
+  a.kb_per_split = nkb;
   a.p.splitk = p.splitk > 1 ? 2 : 1;   // "accumulate atomically" flag
-  a.tmem_cols = a.BN <= 32 ? 32 : a.BN <= 64 ? 64 : a.BN <= 128 ? 128 : 256;
   a.debug = g_tc_debug;
   a.bpk_hi = a.bpk_lo = nullptr; a.bpk_groups = 0; a.bpk_row0 = 0; a.bpk_shift = 3; a.bpk_kb0 = p.bpk_kb0;
   if (pre_k || pre_mn) {

@@ -1,22 +1,27 @@
-// gemm_tma.cu — TMA-fed tcgen05 dense product: the round-2 operand path of every Linear of the GPS layer.
+// gemm_tma.cu — TMA-fed wgmma dense product: the plane operand path of every Linear of the GPS layer.
 //
 //   C[M,N] (+)= epi( Aop[M,K] * Bop[K,N] )
 //
 // Both operands live in HBM as bf16 "planes": plain row-major bf16 matrices holding the hi part of the fp32 value
 // and (fp32-grade mode) its bf16 residual lo, written ONCE by the kernel that produced the tensor (GEMM epilogues,
 // the row-wise BatchNorm kernels, the gather-reduce kernels, attention) or by k_to_planes for layer inputs and
-// weights.  The consumer therefore never converts anything: one elected thread issues tensor-map TMA
-// (cp.async.bulk.tensor, SASS UTMALDG) boxes that land in shared memory already in the canonical UMMA
-// SWIZZLE_128B image -- a {64 x rows} box is a K-major tile, a {64 x 64} box is one MN-major block -- so the same
-// planes serve y = x W^T (K-major), g_x = g_y W (B MN-major) and dW = G^T X (both MN-major, reduction over rows)
-// without transposes or per-layout copies.  Out-of-range rows/columns are zero-filled by the TMA unit.
+// weights.  The consumer therefore never converts anything: one thread issues tensor-map TMA
+// (cp.async.bulk.tensor) boxes that land in shared memory already in the canonical wgmma SWIZZLE_128B image --
+// a {64 x rows} box is a K-major tile, a {64 x 64} box is one MN-major block -- so the same planes serve
+// y = x W^T (K-major), g_x = g_y W (B MN-major) and dW = G^T X (both MN-major, reduction over rows) without
+// transposes or per-layout copies.  Out-of-range rows/columns are zero-filled by the TMA unit.
 //
-// Warp roles (320 threads): warps 0-7 epilogue (tcgen05.ld -> bias / act / act' / dropout / residuals / fp32 store
-// / bf16 hi-lo plane store / BatchNorm column sums / split-K atomics), warp 8 MMA issuer (one lane,
-// tcgen05.mma kind::f16 128 x BN x 16, fp32 accumulation in TMEM; fp32-grade mode issues lo*hi + hi*lo + hi*hi),
-// warp 9 TMA producer (one lane).  Stages form an mbarrier ring: full = expect_tx bytes, empty = tcgen05.commit
-// (+ one arrival per epilogue warp in CTAs that also reduce the bias gradient from the staged A tiles).
-// Narrow tiles (BN <= 64) are launched two CTAs per SM so one CTA's epilogue overlaps the other's main loop.
+// Warp roles (288 threads): warps 0-7 are two consumer warpgroups, each issuing wgmma m64 x BN x k16 for its 64 rows of
+// the 128-row tile (fp32 accumulators in registers; fp32-grade mode issues lo*hi + hi*lo + hi*hi) and then running the
+// epilogue (bias / act / act' / dropout / residuals / fp32 store / bf16 hi-lo plane store / BatchNorm column sums /
+// split-K atomics); warp 8 is the TMA producer (one lane).  Stages form an mbarrier ring: full = expect_tx bytes,
+// empty = one arrival per consumer warp once the wgmma group reading the stage has retired.
+// Narrow tiles (BN = 64) are launched two CTAs per SM so one CTA's epilogue overlaps the other's main loop.
+// Split-K: the K-splits of one output tile form a thread-block cluster (at most 8).  Each split stages its fp32 partial
+// tile in shared memory; rank r then sums rows [r RB, (r + 1) RB) of all ranks' tiles in rank order through
+// distributed shared memory and is the only CTA that adds those rows (and the residuals) into C, so the result does not
+// depend on the order in which the splits finish.  The bias-gradient partials of the splits are combined the same way.
+#include <cooperative_groups.h>
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -31,20 +36,21 @@ namespace gps {
 namespace {
 
 using namespace tc;
+namespace cgrp = cooperative_groups;
 
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int kEpiWarps = 8;
-constexpr int kMmaWarp = 8;
-constexpr int kTmaWarp = 9;
-constexpr int kThreads = 320;
+constexpr int kTmaWarp = 8;
+constexpr int kThreads = 288;
 constexpr int kATile = BM * BK * 2;     // 16 KB per plane
 constexpr int kBlock = 64 * BK * 2;     // 8 KB: one 64-column MN-major block / 64 K-major rows
+constexpr int kMaxSplits = 8;           // split-K splits of a tile = cluster size (portable limit)
 
 struct TmaArgs {
   GemmParams p;
-  int BN, nb_blocks, stages, kb_per_split, tmem_cols, planes;
-  int debug;                   // bring-up: 1 no global stores in the epilogue, 2 no TMEM loads
+  int BN, nb_blocks, stages, kb_per_split, planes;
+  int debug;                   // bring-up: 1 no global stores in the epilogue
   unsigned long long* trace;   // bring-up: 16 globaltimer stamps per CTA (first 256 CTAs), see tools/gemm_trace.py
 };
 
@@ -58,8 +64,8 @@ __device__ __forceinline__ unsigned long long gtimer() {
     if (a.trace && cta_lin < 256) a.trace[cta_lin * 16 + (slot)] = gtimer();                    \
   } while (0)
 
-template <bool A_MN, bool B_MN, bool NARROW>
-__global__ void __launch_bounds__(kThreads, NARROW ? 2 : 1)
+template <bool A_MN, bool B_MN, int BN_T, bool SPLIT>
+__global__ void __launch_bounds__(kThreads, BN_T == 64 ? 2 : 1)
 k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TmaArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const GemmParams& p = a.p;
@@ -68,9 +74,10 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
   const int b_tile = a.nb_blocks * kBlock;
   const int stage_bytes = planes * (kATile + b_tile);
   const int S = a.stages;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);   // full[S], empty[S], accum
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 1);
-  float* red = reinterpret_cast<float*>(tmem_slot + 2);   // 16 x 16 x 8 floats (bias-gradient partials)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);   // full[S], empty[S]
+  float* red = reinterpret_cast<float*>(bars + 2 * S + 2);   // 16 x 16 x 8 floats (bias-gradient partials)
+  float* ctot = red + 16 * 16 * 8;                           // [128] this split's bias-gradient sums (split-K)
+  const int nsplit = (int)gridDim.z;                         // = cluster size when > 1
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * a.BN;
@@ -90,20 +97,15 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     }
     for (int s = 0; s < S; ++s) {
       mbar_init(smem_u32(&bars[s]), 1);
-      mbar_init(smem_u32(&bars[S + s]), 1 + (do_colsum ? kEpiWarps : 0));
+      mbar_init(smem_u32(&bars[S + s]), kEpiWarps);
     }
-    mbar_init(smem_u32(&bars[2 * S]), 1);
     fence_barrier_init();
   }
   if (warp == kTmaWarp && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == kMmaWarp) tmem_alloc(smem_u32(tmem_slot), (uint32_t)a.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   if (tid == 0) GPS_TRACE(1);
 
   if (warp == kTmaWarp) {
@@ -141,63 +143,59 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
       GPS_TRACE(9);
     }
     __syncwarp();
-  } else if (warp == kMmaWarp) {
-    // =========================================================== MMA issuer
-    if (lane == 0 && nkb > 0) {
-      const uint32_t idesc = make_idesc(BM, a.BN, A_MN, B_MN);
-      const uint32_t a_lbo = A_MN ? kBlock : 16, b_lbo = B_MN ? kBlock : 16;
-      const uint32_t a_kstep = A_MN ? 2048 : 32, b_kstep = B_MN ? 2048 : 32;
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % S;
-        mbar_wait(smem_u32(&bars[s]), (uint32_t)(i / S) & 1u);
-        tc_fence_after();
-        if (i == 0) GPS_TRACE(3);
-        if (i == nkb - 1) GPS_TRACE(10);
-        const uint32_t sa_hi = smem_u32(smem + (size_t)s * stage_bytes);
-        const uint32_t sb_hi = sa_hi + planes * kATile;
-        const uint32_t sa_lo = sa_hi + kATile;
-        const uint32_t sb_lo = sb_hi + b_tile;
-#pragma unroll
-        for (int kk = 0; kk < BK / 16; ++kk) {
-          const uint64_t da_hi = make_desc(sa_hi + kk * a_kstep, a_lbo, 1024);
-          const uint64_t db_hi = make_desc(sb_hi + kk * b_kstep, b_lbo, 1024);
-          if (planes == 2) {
-            const uint64_t da_lo = make_desc(sa_lo + kk * a_kstep, a_lbo, 1024);
-            const uint64_t db_lo = make_desc(sb_lo + kk * b_kstep, b_lbo, 1024);
-            umma_bf16(tmem_base, da_lo, db_hi, idesc, (i | kk) != 0);
-            umma_bf16(tmem_base, da_hi, db_lo, idesc, 1u);
-            umma_bf16(tmem_base, da_hi, db_hi, idesc, 1u);
-          } else {
-            umma_bf16(tmem_base, da_hi, db_hi, idesc, (i | kk) != 0);
-          }
-        }
-        umma_commit(smem_u32(&bars[S + s]));   // frees the smem stage once these MMAs retire
-      }
-      umma_commit(smem_u32(&bars[2 * S]));     // accumulator complete
-      GPS_TRACE(4);
+    if (nsplit > 1) {   // the cluster barriers of the split-K reduction count every thread
+      cgrp::this_cluster().sync();
+      cgrp::this_cluster().sync();
     }
-    __syncwarp();
   } else {
-    // =========================================================== epilogue warps
+    // =========================================================== consumer warpgroups: wgmma main loop
+    // warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) of the tile: its A operand starts 8 KB into every A plane
+    // (eight 1 KB K-major row groups, or the second 64-row MN-major block)
+    const int wg = warp >> 2;
+    float acc[BN_T / 2];
+#pragma unroll
+    for (int e = 0; e < BN_T / 2; ++e) acc[e] = 0.f;
     // bias gradient db[m] = sum_k Aop[m,k]: the n-tile-0 CTAs sum the staged (MN-major) A tiles while the tensor
     // core works on them.  Thread t owns the 8-column chunk (t & 15) and k-rows 4 (t >> 4) .. +3 of every k-block.
-    if (do_colsum) {
-      float csum[8];
+    float csum[8];
 #pragma unroll
-      for (int e = 0; e < 8; ++e) csum[e] = 0.f;
-      const int cm = tid & 15, kq = tid >> 4;
-      const uint32_t blk_off = (uint32_t)(cm >> 3) * kBlock;
-      const int cc = cm & 7;
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % S;
-        if (lane == 0) mbar_wait(smem_u32(&bars[s]), (uint32_t)(i / S) & 1u);
-        __syncwarp();
-        const uint8_t* sa = smem + (size_t)s * stage_bytes;
+    for (int e = 0; e < 8; ++e) csum[e] = 0.f;
+    const int cm = tid & 15, kq = tid >> 4;
+    constexpr uint32_t a_lbo = A_MN ? kBlock : 16, b_lbo = B_MN ? kBlock : 16;
+    constexpr uint32_t a_kstep = A_MN ? 2048 : 32, b_kstep = B_MN ? 2048 : 32;
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % S;
+      if (lane == 0) mbar_wait(smem_u32(&bars[s]), (uint32_t)(i / S) & 1u);
+      __syncwarp();
+      if (i == 0 && tid == 0) GPS_TRACE(3);
+      if (i == nkb - 1 && tid == 0) GPS_TRACE(10);
+      const uint8_t* st = smem + (size_t)s * stage_bytes;
+      const uint32_t sa_hi = smem_u32(st) + (uint32_t)wg * 8192u;
+      const uint32_t sb_hi = smem_u32(st) + planes * kATile;
+      const uint32_t sa_lo = sa_hi + kATile;
+      const uint32_t sb_lo = sb_hi + b_tile;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BK / 16; ++kk) {
+        const uint64_t da_hi = make_desc(sa_hi + kk * a_kstep, a_lbo, 1024);
+        const uint64_t db_hi = make_desc(sb_hi + kk * b_kstep, b_lbo, 1024);
+        if (SPLIT) {
+          const uint64_t da_lo = make_desc(sa_lo + kk * a_kstep, a_lbo, 1024);
+          const uint64_t db_lo = make_desc(sb_lo + kk * b_kstep, b_lbo, 1024);
+          wgmma_ss<BN_T, A_MN, B_MN>(acc, da_lo, db_hi, 1u);
+          wgmma_ss<BN_T, A_MN, B_MN>(acc, da_hi, db_lo, 1u);
+        }
+        wgmma_ss<BN_T, A_MN, B_MN>(acc, da_hi, db_hi, 1u);
+      }
+      wgmma_commit();
+      if (do_colsum) {
+        const uint32_t blk_off = (uint32_t)(cm >> 3) * kBlock;
+        const int cc = cm & 7;
         for (int pl = 0; pl < planes; ++pl) {
 #pragma unroll
           for (int rr = 0; rr < 4; ++rr) {
             const int r = kq * 4 + rr;
-            const uint4 q = *reinterpret_cast<const uint4*>(sa + pl * kATile + blk_off + (r >> 3) * 1024 + (r & 7) * 128 +
+            const uint4 q = *reinterpret_cast<const uint4*>(st + pl * kATile + blk_off + (r >> 3) * 1024 + (r & 7) * 128 +
                                                             ((cc ^ (r & 7)) << 4));
             const uint32_t w[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
@@ -207,50 +205,67 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
             }
           }
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bars[S + s]));
       }
+      // at most one group in flight: the previous k-block's MMAs have retired, so its stage goes back to the producer
+      wgmma_wait<1>();
+      reg_fence<BN_T / 2>(acc);
+      __syncwarp();
+      if (i > 0 && lane == 0) mbar_arrive(smem_u32(&bars[S + (i - 1) % S]));
+    }
+    wgmma_wait<0>();
+    reg_fence<BN_T / 2>(acc);
+    if (tid == 0) GPS_TRACE(4);
+    if (do_colsum) {
 #pragma unroll
       for (int e = 0; e < 8; ++e) red[(kq * 16 + cm) * 8 + e] = csum[e];
     }
+    // every wgmma of both warpgroups has retired: the operand stages are free and become the staging tile
     asm volatile("bar.sync 1, 256;" ::: "memory");
     if (do_colsum && tid < 128) {
-      const int cm = tid >> 3, e = tid & 7;
+      const int cmr = tid >> 3, e = tid & 7;
       float tot = 0.f;
 #pragma unroll
-      for (int o = 0; o < 16; ++o) tot += red[(o * 16 + cm) * 8 + e];
-      const int gm = m0 + cm * 8 + e;
-      if (gm < p.M) atomicAdd(&p.colsum_a[gm], tot);
-    }
-
-    if (nkb > 0) {
-      if (lane == 0) mbar_wait(smem_u32(&bars[2 * S]), 0u);
-      __syncwarp();
-      tc_fence_after();
+      for (int o = 0; o < 16; ++o) tot += red[(o * 16 + cmr) * 8 + e];
+      const int gm = m0 + cmr * 8 + e;
+      if (nsplit > 1) ctot[cmr * 8 + e] = tot;   // combined across the cluster below
+      else if (gm < p.M) atomicAdd(&p.colsum_a[gm], tot);
     }
     if (tid == 0) GPS_TRACE(5);
-    // ---- phase 1: accumulator TMEM -> registers -> shared staging tile [128][BN + 4] fp32.  All MMAs have retired, so
-    // the operand stages are free and double as the staging buffer.  The pad keeps both the row-per-lane writes here and
-    // the row-contiguous reads of phase 2 bank-conflict free.
+    // ---- phase 1: accumulator registers -> shared staging tile [128][BN + 4] fp32.  wgmma fragment: thread lane of warp
+    // w holds rows 16 (w & 3) + lane / 4 (+ 8) and columns 8 j + 2 (lane % 4) (+ 1) of its warpgroup's 64 rows.
     float* stage = reinterpret_cast<float*>(smem);
     const int sld = a.BN + 4;
     {
-      const int q = warp & 3, half = warp >> 2;
-      const int r = q * 32 + lane;
-      const int nchunks = a.BN >> 4;
-      for (int c = half; c < nchunks; c += 2) {
-        float v[16];
-        if (nkb > 0 && !(a.debug & 2)) tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 16), v);
-        else {
+      const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int c = 2 * (lane & 3);
 #pragma unroll
-          for (int e = 0; e < 16; ++e) v[e] = 0.f;
-        }
-        float4* dst = reinterpret_cast<float4*>(stage + r * sld + c * 16);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) dst[e] = make_float4(v[4 * e], v[4 * e + 1], v[4 * e + 2], v[4 * e + 3]);
+      for (int j = 0; j < BN_T / 8; ++j) {
+        *reinterpret_cast<float2*>(stage + r * sld + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(stage + (r + 8) * sld + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
     }
     asm volatile("bar.sync 1, 256;" ::: "memory");
+    // ---- split-K: rank r replaces rows [lo, hi) of its staging tile by the rank-ordered sum over the cluster
+    const int RB = (BM + nsplit - 1) / nsplit;
+    const int lo = (int)blockIdx.z * RB, hi = min(BM, lo + RB);
+    if (nsplit > 1) {
+      cgrp::cluster_group cluster = cgrp::this_cluster();
+      cluster.sync();   // every split's staging tile (and bias-gradient sums) is complete
+      const int c4n = a.BN >> 2;
+      for (int idx = tid; idx < (hi - lo) * c4n; idx += kEpiWarps * 32) {
+        const int r = lo + idx / c4n, c = (idx % c4n) * 4;
+        float4 sum = f4zero();
+        for (int k = 0; k < nsplit; ++k)
+          sum = f4add(sum, *reinterpret_cast<const float4*>(cluster.map_shared_rank(stage, k) + r * sld + c));
+        *reinterpret_cast<float4*>(stage + r * sld + c) = sum;
+      }
+      if (do_colsum && blockIdx.z == 0 && tid < 128 && m0 + tid < p.M) {
+        float tot = 0.f;
+        for (int k = 0; k < nsplit; ++k) tot += cluster.map_shared_rank(ctot, k)[tid];
+        atomicAdd(&p.colsum_a[m0 + tid], tot);   // the only adder of this element
+      }
+      cluster.sync();   // no rank leaves while another still reads its shared memory
+    }
     // ---- phase 2: G = BN/4 threads per row, each owning 4 consecutive columns for all of its rows: every global access
     // (bias, residuals, act' mask, fp32 / plane stores, split-K atomics) is a contiguous row segment, the per-column
     // constants live in registers and the BatchNorm column sums are accumulated per thread.
@@ -264,7 +279,7 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
       // rows of this thread: r = rip + k * rpp, k < nrows.  Everything is addressed through per-thread base pointers
       // advanced by a constant stride, and the loop is unrolled by 4 rows so that the shared/global loads of a group are
       // in flight together: with 2 epilogue warps per scheduler the pass is instruction-latency bound otherwise
-      // (measured: 8.5 us for a 128 x 256 tile with neither the TMEM loads nor the global stores on the critical path).
+      // (even with the global stores off the critical path).
       const int rows_here = min(BM, p.M - m0);
       const int nrows = rip < rows_here ? (rows_here - rip + rpp - 1) / rpp : 0;
       const int64_t row0 = m0 + rip;
@@ -277,22 +292,13 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
       const float* r2 = p.R2 ? p.R2 + row0 * p.ldr2 + col : nullptr;
       const int64_t r2_st = (int64_t)rpp * p.ldr2;
       if (p.splitk > 1) {
-        const bool res = blockIdx.z == 0;            // the first split also carries the residual terms
-        for (int k = 0; k < nrows; k += 4) {
-          float4 w[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) w[u] = k + u < nrows ? *reinterpret_cast<const float4*>(sp + (k + u) * s_st) : f4zero();
-          if (res && r1) {
-#pragma unroll
-            for (int u = 0; u < 4; ++u) if (k + u < nrows) w[u] = f4add(w[u], ld4(r1 + (k + u) * r1_st));
-          }
-          if (res && r2) {
-#pragma unroll
-            for (int u = 0; u < 4; ++u) if (k + u < nrows) w[u] = f4add(w[u], ld4(r2 + (k + u) * r2_st));
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (k + u < nrows) atomicAdd(reinterpret_cast<float4*>(cp + (k + u) * c_st), w[u]);   // red.global.add.v4.f32
+        // accumulate into the pre-zeroed C: this CTA is the only adder of rows [lo, hi) (the whole tile without split)
+        for (int r = lo + rip; r < min(hi, rows_here); r += rpp) {
+          const int64_t row = m0 + r;
+          float4 w = *reinterpret_cast<const float4*>(stage + r * sld + cg * 4);
+          if (p.R1) w = f4add(w, ld4(p.R1 + row * p.ldr1 + col));
+          if (p.R2) w = f4add(w, ld4(p.R2 + row * p.ldr2 + col));
+          atomicAdd(reinterpret_cast<float4*>(p.C + row * p.ldc + col), w);   // red.global.add.v4.f32
         }
       } else {
         const bool fast = !p.C_pre && !(p.mask_src && !p.mask_is_post) && p.p_drop == 0.f && p.p_drop2 == 0.f &&
@@ -442,11 +448,10 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
   }
 
   if (tid == 0) GPS_TRACE(6);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (tid == 0) GPS_TRACE(7);
-  if (warp == kMmaWarp) tmem_dealloc(tmem_base, (uint32_t)a.tmem_cols);
+  if (a.trace) {
+    __syncthreads();
+    if (tid == 0) GPS_TRACE(7);
+  }
 }
 
 // ------------------------------------------------------------------------------------ tensor maps
@@ -530,16 +535,38 @@ namespace {
 
 inline bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
-template <bool A_MN, bool B_MN, bool NARROW>
-int launch(const CUtensorMap& tA, const CUtensorMap& tB, const TmaArgs& a, dim3 grid, size_t smem, cudaStream_t stream) {
+template <bool A_MN, bool B_MN, int BN_T, bool SPLIT>
+int launch1(const CUtensorMap& tA, const CUtensorMap& tB, const TmaArgs& a, dim3 grid, size_t smem, cudaStream_t stream) {
   static bool attr_done = false;
   if (!attr_done) {
-    GPS_CUDA(cudaFuncSetAttribute(k_gemm_tma<A_MN, B_MN, NARROW>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    GPS_CUDA(cudaFuncSetAttribute(k_gemm_tma<A_MN, B_MN, BN_T, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  227 * 1024));
     attr_done = true;
   }
-  k_gemm_tma<A_MN, B_MN, NARROW><<<grid, kThreads, smem, stream>>>(tA, tB, a);
+  if (grid.z == 1) {
+    k_gemm_tma<A_MN, B_MN, BN_T, SPLIT><<<grid, kThreads, smem, stream>>>(tA, tB, a);
+  } else {   // the K-splits of a tile are one cluster
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 1;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = grid.z;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    GPS_CUDA(cudaLaunchKernelEx(&cfg, k_gemm_tma<A_MN, B_MN, BN_T, SPLIT>, tA, tB, a));
+  }
   GPS_LAUNCH_CHECK();
   return GPS_OK;
+}
+template <bool A_MN, bool B_MN, int BN_T>
+int launch(const CUtensorMap& tA, const CUtensorMap& tB, const TmaArgs& a, dim3 grid, size_t smem, cudaStream_t stream) {
+  return a.planes == 2 ? launch1<A_MN, B_MN, BN_T, true>(tA, tB, a, grid, smem, stream)
+                       : launch1<A_MN, B_MN, BN_T, false>(tA, tB, a, grid, smem, stream);
 }
 
 int g_tma_force_bn = 0;
@@ -584,39 +611,37 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream) {
   }
   const int mt = (int)ceil_div(p.M, BM);
   const int nkb = (int)ceil_div(p.K, BK);
-  const int splits_hint = p.splitk > 1 ? (p.splitk < nkb ? p.splitk : nkb) : 1;
-  // tile width: minimise waves x staged bytes per CTA, wider on ties (L2 -> SM operand traffic bounds the kernel)
+  const int splits_hint = p.splitk > 1 ? min(kMaxSplits, min(p.splitk, nkb)) : 1;
+  // tile width (the wgmma instruction shape, so one of 64 / 128 / 256): minimise waves x staged bytes per CTA, wider
+  // on ties (L2 -> SM operand traffic bounds the kernel)
   int bestBN = 128;
   long bestCost = -1;
-  for (int nt = (int)ceil_div(p.N, 256); nt <= (int)ceil_div(p.N, 48) + 1; ++nt) {
-    int bn = (int)round_up(ceil_div(p.N, nt), 16);
-    if (bn > 256) continue;
-    if (bn < 16) bn = 16;
-    const int nb = (bn + 63) / 64;
+  for (int bn = 256; bn >= 64; bn >>= 1) {
+    const int nb = bn / 64;
     const long tiles = (long)mt * ceil_div(p.N, bn) * splits_hint;
     const long waves = ceil_div(tiles, nb == 1 ? 2L * kNumSMs : (long)kNumSMs);   // narrow tiles: two CTAs per SM
     const long cost = waves * (BM + nb * 64L);
     if (bestCost < 0 || cost < bestCost) { bestCost = cost; bestBN = bn; }
   }
-  if (g_tma_force_bn > 0) bestBN = g_tma_force_bn;
+  if (g_tma_force_bn == 64 || g_tma_force_bn == 128 || g_tma_force_bn == 256) bestBN = g_tma_force_bn;
   TmaArgs a;
   a.p = p;
   a.BN = bestBN;
-  a.nb_blocks = (a.BN + 63) / 64;
+  a.nb_blocks = a.BN / 64;
   a.planes = planes;
   const bool narrow = a.nb_blocks == 1;
   const int stage_bytes = planes * (kATile + a.nb_blocks * kBlock);
-  const int fixed = 1024 /*align*/ + 1024 /*barriers*/ + 16 * 16 * 8 * 4;
+  const int fixed = 1024 /*align*/ + 1024 /*barriers*/ + 16 * 16 * 8 * 4 + 128 * 4;
   int stages = ((narrow ? 112 : 226) * 1024 - fixed) / stage_bytes;
   if (stages > 8) stages = 8;
-  if (stages < 2) return GPS_ERR_UNSUPPORTED;
+  if (stages < 2) return GPS_ERR_UNSUPPORTED;   // (two stages also hold the epilogue's fp32 staging tile)
   a.stages = stages;
   int splitk = p.splitk > 1 ? p.splitk : 1;
+  if (splitk > kMaxSplits) splitk = kMaxSplits;
   if (splitk > nkb) splitk = nkb;
   a.kb_per_split = (int)ceil_div(nkb, splitk);
   splitk = (int)ceil_div(nkb, a.kb_per_split);
   a.p.splitk = p.splitk > 1 ? 2 : 1;   // "accumulate atomically" flag
-  a.tmem_cols = a.BN <= 32 ? 32 : a.BN <= 64 ? 64 : a.BN <= 128 ? 128 : 256;
   a.trace = g_tma_trace;
   a.debug = g_tma_debug;
   const bool amn = p.ta != 0, bmn = p.tb != 0;
@@ -626,9 +651,11 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream) {
   GPS_TRY(tensor_map(p.Bp.hi, p.Bp.lo, planes, bmn ? p.K : p.N, bmn ? p.N : p.K, p.Bp.ld, bmn ? 64 : a.BN, &tB));
   const size_t smem = (size_t)stages * stage_bytes + fixed;
   dim3 grid((unsigned)ceil_div(p.N, a.BN), (unsigned)mt, (unsigned)splitk);
-#define GPS_TMA_CASE(AM, BMN)                                                                           \
-  if (amn == AM && bmn == BMN)                                                                          \
-    return narrow ? launch<AM, BMN, true>(tA, tB, a, grid, smem, stream) : launch<AM, BMN, false>(tA, tB, a, grid, smem, stream);
+#define GPS_TMA_CASE(AM, BMN)                                                                              \
+  if (amn == AM && bmn == BMN)                                                                             \
+    return a.BN == 64 ? launch<AM, BMN, 64>(tA, tB, a, grid, smem, stream)                                 \
+           : a.BN == 128 ? launch<AM, BMN, 128>(tA, tB, a, grid, smem, stream)                             \
+                         : launch<AM, BMN, 256>(tA, tB, a, grid, smem, stream);
   GPS_TMA_CASE(false, false)
   GPS_TMA_CASE(false, true)
   GPS_TMA_CASE(true, false)

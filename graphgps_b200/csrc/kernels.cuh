@@ -108,7 +108,7 @@ int attention_bwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, 
                   cudaStream_t stream, const unsigned long long* offset_dev = nullptr, Planes dQp = Planes(),
                   Planes dKp = Planes(), Planes dVp = Planes());
 
-// tcgen05 version (attention_tc.cu): Q, K, V from bf16 hi/lo planes in the per-head padded layout
+// wgmma version (attention_tc.cu): Q, K, V from bf16 hi/lo planes in the per-head padded layout
 // column (which * H + h) * hd_pad + k, hd_pad = attention_tc_hd_pad(hd), pad columns zero
 void attention_tc_set_debug(float* buf);   // bring-up: 3 x 128 x 128 floats (S, P, raw O of CTA (0,0))
 bool attention_tc_supported(int64_t hd);

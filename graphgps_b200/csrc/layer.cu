@@ -59,7 +59,7 @@ void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
 static std::atomic<unsigned long long> g_fallbacks{0};
 
-// Dispatcher: TMA-fed tcgen05 kernel when the caller supplies operand planes, else the register-staged tcgen05 kernel
+// Dispatcher: TMA-fed wgmma kernel when the caller supplies operand planes, else the register-staged wgmma kernel
 // on the fp32 operands, else (odd shapes / alignment) the exact CUDA-core kernel - counted, and an error under
 // GPS_B200_STRICT=1 so that a 10x slower path can never be taken silently.
 int gemm(const GemmParams& p, cudaStream_t stream) {
@@ -138,12 +138,10 @@ struct Side {
 static int opt_flags() {
   static const int v = [] {
     const char* e = getenv("GPS_B200_OPT");
-    return e ? atoi(e) : 7;   // Measured slower on B200 and therefore off (same-box A/B, profiles/r2_ab_switches.txt):
-                              // 8 (split dgrad+wgrad tail) 0.478 vs 0.465; 16 (two-part Wcat wgrad) 0.476 vs 0.465;
-                              // 32 + 64 (bn_node_x reduce inside the norm1_local apply pass, norm1_local / norm1_attn
-                              // reduces in the epilogue of the GEMM producing g_s) 0.4946 vs 0.4856: three launches
-                              // fewer, but the fused kernels run as few fat CTAs and delay the branches behind them on B200 (0.478 vs 0.465 ms/step in round 2 as well); 16 (two-part Wcat
-                              // weight gradient) too: 0.476 vs 0.465 on one GPU and no gain at N = 2
+    return e ? atoi(e) : 7;   // Off by default: 8 (split dgrad+wgrad tail), 16 (two-part Wcat wgrad), 32 + 64
+                              // (bn_node_x reduce inside the norm1_local apply pass, norm1_local / norm1_attn reduces
+                              // in the epilogue of the GEMM producing g_s): three launches fewer, but the fused kernels
+                              // run as few fat CTAs and delay the branches behind them
   }();
   return v;
 }
@@ -219,7 +217,7 @@ struct Plan {
   bool use_planes;
   Planes x_p, e_p, O_p, s_p, hid_p, agg_p, h1_p, Wcat_p, C_p, out_p, ff1_p, ff2_p, g0_p, g1_p, pq_p, pk_p, pv_p;
   Planes gt_p, ghid_p, ghA_p, ge_p, gY1_p, gtmp_p, gtmp2_p, gtmp3_p, gl1_p, gh1_p;
-  Planes qkv_p;        // Q | K | V per head, padded to hd_pad columns: operands of the tcgen05 attention
+  Planes qkv_p;        // Q | K | V per head, padded to hd_pad columns: operands of the wgmma attention
   bool attn_tc;        // softmax attention on the tensor cores (attention_tc.cu)
   int64_t saved_bytes;
   int64_t wplanes_bytes;
@@ -244,9 +242,9 @@ static bool planes_enabled() {
 }
 
 // Forward softmax attention on the tensor cores (attention_tc.cu) when the batch's graphs are large enough for 128 x 128
-// tiles to pay: measured on B200 (round 2) the tcgen05 kernel needs 57 us at the PCQM4M shape (mean 14 nodes per graph:
-// a 128-row tile sees ~45 useful keys of 256, one latency-bound wave of 116 CTAs) against 25 us for the CUDA-core kernel,
-// and wins once a graph fills a tile (ogbg-code2 shape, mean 125 / max ~1000 nodes).  GPS_B200_ATTN=simt | tc overrides.
+// tiles to pay: at the PCQM4M shape (mean 14 nodes per graph) a 128-row tile sees ~45 useful keys of 256 in one
+// latency-bound wave and the CUDA-core kernel is faster; the tensor-core kernel wins once a graph fills a tile
+// (ogbg-code2 shape, mean 125 / max ~1000 nodes).  GPS_B200_ATTN=simt | tc overrides.
 static bool attn_tc_enabled(int64_t N, int64_t B) {
   static const int mode = [] {
     const char* e = getenv("GPS_B200_ATTN");
@@ -682,7 +680,7 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
   cudaStream_t s2 = sd ? sd->s : st;
   const bool two_branches = (P.gated || P.gine || P.gcn) && (P.attn || P.perf);
 
-  // weights: concatenate the node projections, then pre-pack every forward weight into the tcgen05 kernel's
+  // weights: concatenate the node projections, then pre-pack every forward weight into the wgmma kernel's
   // shared-memory tile image (bf16 hi/lo planes) so its B operand arrives by bulk TMA
   if (P.Wy) {
     PackDesc pdsc0 = pack_desc(a, P);
@@ -795,7 +793,7 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
       g.bias = P.bcat + wl; g.precision = a->precision;
       set_bpk(g, P.pk_cat, P.Wy, d, wl);
       g.Ap = P.x_p; g.Bp = P.Wcat_p.rows(wl);
-      if (P.attn_tc) {   // Q | K | V additionally as padded per-head operand planes for the tcgen05 attention
+      if (P.attn_tc) {   // Q | K | V additionally as padded per-head operand planes for the wgmma attention
         g.Cp = P.qkv_p; g.cp_hd = (int)P.hd; g.cp_hd_pad = (int)attention_tc_hd_pad(P.hd); g.cp_col0 = 0;
       }
       GPS_TRY(gemm(g, sg));
@@ -1426,7 +1424,7 @@ using namespace gps;
 
 extern "C" const char* gps_last_error(void) { return g_err; }
 extern "C" int gps_abi_version(void) { return GPS_ABI_VERSION; }
-extern "C" const char* gps_build_arch(void) { return "sm_100a"; }
+extern "C" const char* gps_build_arch(void) { return "sm_90a"; }
 extern "C" unsigned long long gps_launch_count(void) { return g_launches.load(); }
 extern "C" unsigned long long gps_fallback_count(void) { return g_fallbacks.load(); }
 
@@ -1503,7 +1501,7 @@ extern "C" int gps_gemm(const float* A, int64_t lda, int32_t ta, const float* B,
   if (impl == 1) return gemm_simt(g, (cudaStream_t)stream);
   if (impl == 2) {
     int rc = gemm_tc(g, (cudaStream_t)stream);
-    if (rc == GPS_ERR_UNSUPPORTED) set_error("gps_gemm: the tcgen05 kernel does not take this shape/alignment");
+    if (rc == GPS_ERR_UNSUPPORTED) set_error("gps_gemm: the tensor-core kernel does not take this shape/alignment");
     return rc;
   }
   return gemm(g, (cudaStream_t)stream);

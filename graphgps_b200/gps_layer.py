@@ -1,11 +1,11 @@
-"""B200-native drop-in for `graphgps.layer.gps_layer.GPSLayer`.
+"""H100-native drop-in for `graphgps.layer.gps_layer.GPSLayer`.
 
 Same constructor signature, `forward(batch) -> batch` contract and `state_dict` layout as the
 reference module (graphgps/layer/gps_layer.py:16-264; parameter names per SURVEY.md section 8b), so
 `graphgps/network/gps_model.py:85-99` can instantiate it unchanged and reference checkpoints load
 with `load_state_dict`.  All arithmetic of the layer — the five GatedGCN projections, the
 CSR/CSC segmented gather-reduce, softmax attention over each graph's node set, residual/BatchNorm/FFN
-and the whole backward pass — runs in hand-written CUDA (libgps_b200.so, sm_100a) reached through
+and the whole backward pass — runs in hand-written CUDA (libgps_b200.so, sm_90a) reached through
 one C-ABI call per direction; PyTorch only owns memory, streams and the autograd graph edge.
 There is NO fallback: CPU tensors or a missing library raise.
 """
@@ -538,4 +538,4 @@ class GPSLayer(nn.Module):
     def extra_repr(self):
         return (f"summary: dim_h={self.dim_h}, local_gnn_type={self.local_gnn_type}, "
                 f"global_model_type={self.global_model_type}, heads={self.num_heads}, "
-                f"backend=libgps_b200(sm_100a), precision={self.precision}")
+                f"backend=libgps_b200(sm_90a), precision={self.precision}")

@@ -14,7 +14,7 @@ from .gps_layer import GPSLayer
 
 
 def install(gps_model_module=None):
-    """Rebind ``GPSLayer`` inside ``graphgps.network.gps_model`` so ``create_model()`` builds the B200 layer.
+    """Rebind ``GPSLayer`` inside ``graphgps.network.gps_model`` so ``create_model()`` builds the H100 layer.
 
     Call after ``import graphgps`` and before ``create_model()`` (main.py:144).  Returns the class it replaced so a
     caller can restore it."""

@@ -1,7 +1,7 @@
 """The GPSLayer stack of a GPSModel as one component (SURVEY.md section 8 f1).
 
 The reference builds `self.layers = torch.nn.Sequential(*[GPSLayer(...)] * L)` and runs it over ONE batch object
-(graphgps/network/gps_model.py:85-100, 105-108).  `GPSStack` is that container for the B200 layers plus what the
+(graphgps/network/gps_model.py:85-100, 105-108).  `GPSStack` is that container for the H100 layers plus what the
 stack can share that a single layer cannot:
   * the CSR/CSC graph structure is built once per batch and cached on the batch object (graph.py), so all L layers and
     their backward passes reuse it;

@@ -1,5 +1,5 @@
 /*
- * gps_b200.h — C ABI of libgps_b200.so: a B200 (sm_100a) implementation of the GraphGPS
+ * gps_b200.h — C ABI of libgps_b200.so: an H100 (sm_90a) implementation of the GraphGPS
  * `GPSLayer` forward+backward hot path.
  *
  * The reference (rampasek/GraphGPS) is pure Python and has NO FFI of its own (SURVEY.md §8b);
@@ -51,13 +51,13 @@ const char* gps_build_arch(void);
 /* number of CUDA kernels this library has launched in the calling process (bench.py reports the
  * delta over its timed region as `gpu_launches`) */
 unsigned long long gps_launch_count(void);
-/* bring-up / tuning hook of the tcgen05 GEMM (tools/gemm_triage.py, tools/gemm_tune.py): low byte = stage
+/* bring-up / tuning hook of the register-staged wgmma GEMM (tools/gemm_triage.py, tools/gemm_tune.py): low byte = stage
  * switches (1 no global loads, 2 no convert/store, 4 no MMA, 8 no epilogue), bits 8.. = forced tile width. 0 = normal. */
 void gps_debug_set(int v);
 /* bring-up hook of the TMA-fed GEMM (tools/gemm_trace.py): force_bn = forced tile width (0 = heuristic); trace = device
  * buffer of 256 x 16 uint64 that the first 256 CTAs of each launch fill with globaltimer phase stamps (NULL = off) */
 void gps_debug_tma(int force_bn, void* trace);
-/* bring-up hook of the tcgen05 attention: device buffer of 3 x 128 x 128 floats that CTA (0,0) fills with its first
+/* bring-up hook of the wgmma attention: device buffer of 3 x 128 x 128 floats that CTA (0,0) fills with its first
  * S tile, P tile and raw O accumulator (NULL = off) */
 void gps_debug_attn(void* buf);
 
@@ -230,8 +230,8 @@ int gps_linear_forward(const float* A, int64_t lda, const float* W, int64_t ldw,
 /* General dense product used for the data / weight gradients of every Linear:
  *   C[M,N] (+)= Aop[M,K] * Bop[K,N];  ta==0: Aop[m,k]=A[m*lda+k], ta==1: Aop[m,k]=A[k*lda+m];
  *   tb==0: Bop[k,n]=B[n*ldb+k] (an nn.Linear weight), tb==1: Bop[k,n]=B[k*ldb+n].
- * splitk > 1 accumulates atomically into a pre-zeroed C.  impl: 0 = dispatcher (tcgen05 when the
- * shape qualifies), 1 = exact CUDA-core kernel, 2 = tcgen05 kernel (GPS_ERR_UNSUPPORTED if it does
+ * splitk > 1 accumulates into a pre-zeroed C (one adder per element: the same result in every run).  impl: 0 = dispatcher (tensor cores when the
+ * shape qualifies), 1 = exact CUDA-core kernel, 2 = tensor-core kernel (GPS_ERR_UNSUPPORTED if it does
  * not take the shape). */
 int gps_gemm(const float* A, int64_t lda, int32_t ta, const float* B, int64_t ldb, int32_t tb, float* C,
              int64_t ldc, int64_t M, int64_t N, int64_t K, int32_t splitk, int32_t precision, int32_t impl,
@@ -255,7 +255,7 @@ int gps_gine_aggregate_forward(const GpsGraph* g, int64_t d, const float* x, con
 int gps_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q,
                           const float* K, const float* V, int64_t ld, float* O, int64_t ldo,
                           float* lse, float p_drop, uint64_t seed, uint64_t offset, void* stream);
-/* ABI 3: the same forward on the tensor cores (csrc/attention_tc.cu: tcgen05 S = QK^T and O += PV, TMA-staged tiles,
+/* ABI 3: the same forward on the tensor cores (csrc/attention_tc.cu: wgmma S = QK^T and O += PV, TMA-staged tiles,
  * block-diagonal graph mask applied in-kernel).  qkv_hi/qkv_lo: bf16 hi/lo planes [N, ld] holding Q | K | V per head in
  * the padded layout column (which * heads + h) * hd_pad + k with hd_pad = round_up(hd, 16) and zero pad columns
  * (qkv_lo NULL for GPS_PREC_BF16).  Same O / lse conventions as gps_attention_forward, so either backward applies. */
@@ -269,12 +269,13 @@ int gps_attention_backward(const GpsGraph* g, int64_t heads, int64_t hd, const f
                            float* dQ, float* dK, float* dV, int64_t ldg, float p_drop,
                            uint64_t seed, uint64_t offset, void* stream);
 
-/* ABI 3: operand "planes" of the TMA-fed tcgen05 GEMM (csrc/gemm_tma.cu).  A plane pair is the bf16 image of an
+/* ABI 3: operand "planes" of the TMA-fed wgmma GEMM (csrc/gemm_tma.cu).  A plane pair is the bf16 image of an
  * fp32 matrix: hi = bf16(v), lo = bf16(v - hi), both plain row-major with pitch ldp (elements, multiple of 8); lo may
  * be NULL for GPS_PREC_BF16.  gps_to_planes converts; gps_gemm_planes multiplies plane operands stored as
  * A: [M,K] (ta = 0) or [K,M] (ta = 1), B: [N,K] (tb = 0, an nn.Linear weight) or [K,N] (tb = 1), writes fp32 C
  * (may be NULL) and/or the planes of C, optionally adds the row sums of Aop into colsum_a[M] (ta = 1: the bias
- * gradient of dW = G^T X).  splitk > 1 accumulates atomically into a pre-zeroed fp32 C. */
+ * gradient of dW = G^T X).  splitk > 1 splits K over a cluster of at most 8 CTAs whose partial tiles are summed in
+ * rank order, then added into a pre-zeroed fp32 C by one CTA per element: the same result in every run. */
 int gps_to_planes(const float* src, int64_t ld, int64_t rows, int64_t cols, void* hi, void* lo, int64_t ldp,
                   void* stream);
 int gps_gemm_planes(const void* A_hi, const void* A_lo, int64_t lda, int32_t ta, const void* B_hi, const void* B_lo,

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 attention forward (csrc/attention_tc.cu) against float64 dense per-graph softmax attention and against
+"""GPU: the wgmma attention forward (csrc/attention_tc.cu) against float64 dense per-graph softmax attention and against
 the CUDA-core kernel (same Philox dropout stream => identical masks), at the head dims of the BASELINE configs
 (hd 76 C3, 16 zinc, 24 C4-Transformer, 64 code2 incl. graphs far longer than one 128-key tile)."""
 import ctypes as C

@@ -1,4 +1,4 @@
-"""GPU: the dense-product kernels (tcgen05 and exact CUDA-core) against a float64 torch product,
+"""GPU: the dense-product kernels (wgmma and exact CUDA-core) against a float64 torch product,
 all four operand orientations (K-major / MN-major), split-K, ragged sizes."""
 import pytest
 import torch
@@ -47,7 +47,7 @@ def test_gemm_tcgen05(M, N, K, ta, tb, precision, tol):
     if lda % 4 or ldb % 4:
         pytest.skip("128-bit operand path needs leading dimensions that are multiples of 4")
     if (not ta and K % 8) or (not tb and K % 8) or (ta and M % 8) or (tb and N % 8):
-        pytest.skip("tcgen05 kernel takes whole 8-element operand chunks; the dispatcher uses the CUDA-core kernel here")
+        pytest.skip("the tensor-core kernel takes whole 8-element operand chunks; the dispatcher uses the CUDA-core kernel here")
     err = _run(M, N, K, ta, tb, 1, precision, 2)
     assert err < tol, err
 

@@ -1,4 +1,4 @@
-"""GPU: the TMA-fed tcgen05 GEMM (csrc/gemm_tma.cu) on bf16 hi/lo plane operands, every operand orientation the layer
+"""GPU: the TMA-fed wgmma GEMM (csrc/gemm_tma.cu) on bf16 hi/lo plane operands, every operand orientation the layer
 uses, against float64 torch: y = x W^T (forward Linears, gatedgcn_layer.py:57-61, gps_layer.py:253-257), g_x = g_y W
 (data gradients) and dW = G^T X with db = colsum(G) (weight/bias gradients).  fp32-grade mode: <= 2e-5 * max(1, sqrt(K)/8)
 scaled max-abs (the tolerance of the register-staged kernel's tests); bf16 mode: 2e-2."""

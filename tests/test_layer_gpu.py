@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the C ABI, against
+"""GPU parity tests (need an H100): the CUDA path, called through the C ABI, against
 (i) the committed golden fixtures (reference-verbatim, fp64), (ii) the oracle on the same seeded
 inputs, (iii) torch restatements of single stages, and (iv) size-independent properties at the
 BASELINE sizes.  Tolerances: 1e-3 for precision="fp32", 1e-2 for "bf16" (BASELINE.json north_star),
@@ -20,10 +20,9 @@ DEV = "cuda:0"
 TOL = {"fp32": 1e-3, "bf16": 1e-2}
 # Gradient fallback criterion (util.compare): relative L2 when ReLU-kink flips defeat the max-abs one.
 # bf16 rounding (2^-9 per product operand, ~12 chained single-pass products between the loss and the first weight
-# gradient) also flips ~0.3% of the ReLU masks.  Round 1 allowed 15% everywhere, which could hide a defect; measured on
-# B200 (round 2): weight gradients 3.5-4.3e-2 relative L2 at the BASELINE sizes and up to 9e-2 on the small golden
-# batches (120-300 rows per BatchNorm column); the near-cancelling column sums (bias / BatchNorm-bias gradients) up to
-# 7.2e-2 (local_model.bn_node_x.bias).  Bounds: 8e-2 at the BASELINE sizes (GRAD_L2_FULL), 1e-1 on the goldens; the bias gradients are
+# gradient) also flips a fraction of a percent of the ReLU masks, which moves weight gradients by a few 1e-2 relative L2
+# (more on the small golden batches of 120-300 rows per BatchNorm column, and on the near-cancelling column sums of the
+# bias / BatchNorm-bias gradients).  Bounds: 8e-2 at the BASELINE sizes (GRAD_L2_FULL), 1e-1 on the goldens; the bias gradients are
 # exact fp32 column sums in both modes.  A wrong operand or a missing term shows up as O(1).  Smooth-activation
 # (GELU) cases are held to the strict max-abs tolerance in test_layer_gelu_strict_gradients_full_size.
 # util.compare reports raw max-abs errors beside the scaled ones.

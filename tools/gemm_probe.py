@@ -1,4 +1,4 @@
-"""Bring-up probe for the tcgen05 GEMM: prints the error of each orientation/precision separately."""
+"""Bring-up probe for the wgmma GEMM: prints the error of each orientation/precision separately."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))

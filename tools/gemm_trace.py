@@ -2,7 +2,7 @@
 
     python tools/gemm_trace.py M N K [ta tb splitk force_bn]
 slots: 0 start, 1 setup done, 2 first TMA issued, 9 last TMA issued, 3 first stage landed, 10 last stage landed,
-       4 last MMA issued, 5 accumulator ready, 6 epilogue done, 7 all warps done"""
+       4 last MMA retired, 5 bias-gradient sums done, 6 epilogue done, 7 all warps done"""
 import os
 import sys
 

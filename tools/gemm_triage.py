@@ -1,4 +1,4 @@
-"""Perf triage of the tcgen05 GEMM: times the kernel with parts switched off (gps_debug_set)."""
+"""Perf triage of the wgmma GEMM: times the kernel with parts switched off (gps_debug_set)."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""Tile-width / split-K sweep of the tcgen05 GEMM at the layer's shapes (forces BN through gps_debug_set)."""
+"""Tile-width / split-K sweep of the wgmma GEMM at the layer's shapes (forces BN through gps_debug_set)."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
