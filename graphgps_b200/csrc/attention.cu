@@ -106,7 +106,6 @@ struct AttnArgs {
   float* dQ; float* dK; float* dV; int64_t ldg;
   float scale; float p_drop; uint64_t seed, offset;
   const unsigned long long* offset_dev;
-  int role;   // backward: -1 both passes in one grid (blockIdx.z), 0 key-major pass, 1 query-major pass
   Planes Op, dQp, dKp, dVp;   // optional bf16 hi/lo plane copies of O (forward) / dQ, dK, dV (backward)
   int smem_rows;              // rows of the two per-block staging tiles (0: no staging)
 };
@@ -389,12 +388,11 @@ __device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_
   }
 }
 
-// both backward passes in one grid (blockIdx.z picks the role) so they share the SMs instead of queueing
+// both backward passes in one grid (blockIdx.z picks the pass) so they share the SMs instead of queueing
 template <int CH, int LPR>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_bwd(AttnArgs a) {
   extern __shared__ float attn_sm[];
-  const int role = a.role >= 0 ? a.role : (int)blockIdx.z;
-  if (role == 0) attn_bwd_kv_body<CH, LPR>(a, attn_sm);
+  if (blockIdx.z == 0) attn_bwd_kv_body<CH, LPR>(a, attn_sm);
   else attn_bwd_q_body<CH, LPR>(a, attn_sm);
 }
 
@@ -409,7 +407,8 @@ static void launch_one(int which, const AttnArgs& a0, cudaStream_t stream) {
   static const bool stage_on = [] {
     const char* e = getenv("GPS_B200_ATTN_STAGE");   // off by default: the staged kernels are faster in isolation but
     return e && e[0] == '1';                          // their 72 KB blocks crowd the GEMMs running next to them
-                                                      // (same-box A/B at C3: 0.4983 vs 0.4856 ms/step)
+                                                      // (pcqm4m-small fp32, H100 80GB HBM3 at 400 W: 0.854 on vs
+                                                      // 0.846 ms/step off)
   }();
   // staging pays when graphs are small (a block's 32 rows then see few distinct key rows); with large graphs every
   // block would exceed the tile anyway
@@ -422,7 +421,7 @@ static void launch_one(int which, const AttnArgs& a0, cudaStream_t stream) {
     else cudaFuncSetAttribute(k_attn_bwd<CH, LPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
     attr_done[which] = true;
   }
-  dim3 grid((unsigned)ceil_div(a.N, (int64_t)RPW * kWarpsPerBlock), (unsigned)a.H, (which == KFWD || a.role >= 0) ? 1 : 2);
+  dim3 grid((unsigned)ceil_div(a.N, (int64_t)RPW * kWarpsPerBlock), (unsigned)a.H, which == KFWD ? 1 : 2);
   dim3 block(kWarpsPerBlock * 32);
   if (which == KFWD) k_attn_fwd<CH, LPR><<<grid, block, smem, stream>>>(a);
   else k_attn_bwd<CH, LPR><<<grid, block, smem, stream>>>(a);
@@ -464,7 +463,6 @@ int attention_fwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, 
   a.gptr = g.graph_ptr; a.B = (int)g.B; a.N = (int)g.N; a.H = (int)heads; a.hd = (int)hd;
   a.Q = Q; a.K = K; a.V = V; a.ld = ld; a.O = O; a.ldo = ldo; a.lse = lse;
   a.scale = 1.f / sqrtf((float)hd); a.p_drop = p_drop; a.seed = seed; a.offset = offset;
-  a.role = -1;
   return dispatch(KFWD, a, stream);
 }
 
@@ -483,17 +481,6 @@ int attention_bwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, 
   const int64_t nt = (int64_t)a.N * a.H * 8;
   k_attn_delta<<<(unsigned)ceil_div(nt, (int64_t)256), 256, 0, stream>>>(a);
   GPS_LAUNCH_CHECK();
-  static const bool merged = [] {
-    const char* e = getenv("GPS_B200_OPT");
-    return !e || (atoi(e) & 2);
-  }();
-  if (merged) {
-    a.role = -1;
-    return dispatch(KBWD, a, stream);
-  }
-  a.role = 1;
-  GPS_TRY(dispatch(KBWD, a, stream));
-  a.role = 0;
   return dispatch(KBWD, a, stream);
 }
 

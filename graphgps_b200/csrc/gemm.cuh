@@ -33,11 +33,6 @@ struct GemmParams {
   int splitk = 1;
   float* colsum_a = nullptr;               // ta==1 only: += sum_k Aop[m,k]  (bias gradient), [M]
   int precision = GPS_PREC_FP32;
-  // optional pre-packed image of B (tb == 0 only; see prepack_weights): bf16 hi plane at bpk, lo plane at
-  // bpk + bpk_lo_off, bpk_groups 8-row groups per 64-wide k-block, this GEMM's B starts at packed row bpk_row0
-  // bpk_mn: the image is MN-major (tb == 1: B is [K x N]; bpk_groups = 64-column blocks per k-block)
-  const void* bpk = nullptr; int64_t bpk_lo_off = 0; int bpk_groups = 0; int bpk_row0 = 0; int bpk_mn = 0;
-  int bpk_kb0 = 0;   // first 64-deep k-block of this GEMM inside the packed planes (reduction sub-range of a packed matrix)
   // bf16 hi/lo planes of the operands as stored (A: [M,K] or, ta == 1, [K,M]; B: [N,K] or, tb == 1, [K,N]): when both
   // are given the TMA-fed kernel (gemm_tma.cu) runs and A/B (fp32) are not read.  Cp: optional plane copy of the
   // result for the next GEMM; C may then be null (planes-only output).
@@ -63,23 +58,11 @@ int make_tensor_map(const __nv_bfloat16* hi, const __nv_bfloat16* lo, int planes
 void gemm_tma_set_force_bn(int bn);
 void gemm_tma_set_trace(unsigned long long* buf);   // bring-up: per-CTA phase timestamps (tools/gemm_trace.py)
 
-// Pre-packs up to 8 weight matrices (fp32 [rows, K] row-major) into the wgmma kernel's shared-memory tile image.
-// K-major (mn = 0): W is [rows x K], dst sized by prepack_bytes(rows, K).
-// MN-major (mn = 1): W is [K x rows] (rows = GEMM output columns), dst sized by prepack_bytes_mn(rows, K).
-struct PrepackItem { const float* W; int rows; int K; int ld; void* dst; int mn; };
-int64_t prepack_bytes(int rows, int K);          // both planes
-int64_t prepack_plane_bytes(int rows, int K);    // offset of the lo plane
-int prepack_groups(int rows);
-int64_t prepack_bytes_mn(int cols, int K);
-int64_t prepack_plane_bytes_mn(int cols, int K);
-int prepack_groups_mn(int cols);
-int prepack_weights(const PrepackItem* items, int n, cudaStream_t stream);
-
 // exact fp32 CUDA-core product (validation path and shapes the tensor-core kernel does not take)
 int gemm_simt(const GemmParams& p, cudaStream_t stream);
 // register-staged wgmma tensor-core product; returns GPS_ERR_UNSUPPORTED for shapes it does not take
 int gemm_tc(const GemmParams& p, cudaStream_t stream);
-void gemm_tc_set_debug(int v);
+void gemm_tc_set_debug(int v);   // bits 8.. : forced tile width (0 = heuristic)
 // dispatcher used by the layer
 int gemm(const GemmParams& p, cudaStream_t stream);
 

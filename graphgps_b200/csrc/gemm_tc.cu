@@ -63,22 +63,10 @@ struct TcArgs {
   int nb_blocks;   // BN / 64
   int stages;
   int kb_per_split;
-  const uint8_t* bpk_hi;   // pre-packed K-major B planes (BPRE variants), else null
-  const uint8_t* bpk_lo;
-  int bpk_groups;          // 8-row groups per k-block in the packed planes
-  int bpk_row0;            // first row of this GEMM's B inside the packed matrix (multiple of 8)
-  int bpk_kb0;             // k-block offset of this GEMM's reduction range inside the planes
-  int bpk_shift;           // 3: K-major planes (1 KB per 8 rows), 6: MN-major planes (8 KB per 64 columns)
-  int debug;       // perf-triage switches (gps_debug_set): 1 no global loads, 2 no convert/store, 4 no MMA, 8 no epilogue
 };
 
 // BN_T = tile width; a producer thread stages BN_T / 32 B chunks per k-block.
-// BPRE: the B operand (an nn.Linear weight) was pre-packed once per step by k_prepack_weights into bf16 hi/lo
-// planes that already have the shared-memory image of a tile (SWIZZLE_128B; K-major: 8-row groups, MN-major:
-// 64-column blocks; one 64-deep k-block after the other), so a stage's B tile is ONE contiguous range: a single
-// elected thread fetches it with bulk TMA (cp.async.bulk ... mbarrier::complete_tx) and the producer warps only
-// stage A.  K-major planes serve y = x W^T (forward), MN-major planes serve g_x = g_y W (data gradients).
-template <bool A_MN, bool B_MN, bool SPLIT, int BN_T, bool BPRE>
+template <bool A_MN, bool B_MN, bool SPLIT, int BN_T>
 __global__ void __launch_bounds__(kThreads, 1) k_gemm_tc(const TcArgs a) {
   constexpr int NBC = BN_T / 32;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -103,7 +91,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_gemm_tc(const TcArgs a) {
 
   if (tid == 0) {
     for (int s = 0; s < S; ++s) {
-      mbar_init(smem_u32(&bars[s]), kProducerWarps + (BPRE ? 1 : 0));
+      mbar_init(smem_u32(&bars[s]), kProducerWarps);
       mbar_init(smem_u32(&bars[S + s]), kConsumerWarps);
     }
     fence_barrier_init();
@@ -128,22 +116,20 @@ __global__ void __launch_bounds__(kThreads, 1) k_gemm_tc(const TcArgs a) {
       const uint32_t sb_hi = smem_u32(smem + (size_t)s * stage_bytes) + plane * kATileBytes;
       const uint32_t sa_lo = sa_hi + kATileBytes;
       const uint32_t sb_lo = sb_hi + b_tile_bytes;
-      if (!(a.debug & 4)) {
-        wgmma_fence();
+      wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < BK / 16; ++kk) {
-          const uint64_t da_hi = make_desc(sa_hi + kk * a_kstep, a_lbo, 1024);
-          const uint64_t db_hi = make_desc(sb_hi + kk * b_kstep, b_lbo, 1024);
-          if (SPLIT) {
-            const uint64_t da_lo = make_desc(sa_lo + kk * a_kstep, a_lbo, 1024);
-            const uint64_t db_lo = make_desc(sb_lo + kk * b_kstep, b_lbo, 1024);
-            wgmma_ss<BN_T, A_MN, B_MN>(acc, da_lo, db_hi, 1u);
-            wgmma_ss<BN_T, A_MN, B_MN>(acc, da_hi, db_lo, 1u);
-          }
-          wgmma_ss<BN_T, A_MN, B_MN>(acc, da_hi, db_hi, 1u);
+      for (int kk = 0; kk < BK / 16; ++kk) {
+        const uint64_t da_hi = make_desc(sa_hi + kk * a_kstep, a_lbo, 1024);
+        const uint64_t db_hi = make_desc(sb_hi + kk * b_kstep, b_lbo, 1024);
+        if (SPLIT) {
+          const uint64_t da_lo = make_desc(sa_lo + kk * a_kstep, a_lbo, 1024);
+          const uint64_t db_lo = make_desc(sb_lo + kk * b_kstep, b_lbo, 1024);
+          wgmma_ss<BN_T, A_MN, B_MN>(acc, da_lo, db_hi, 1u);
+          wgmma_ss<BN_T, A_MN, B_MN>(acc, da_hi, db_lo, 1u);
         }
-        wgmma_commit();
+        wgmma_ss<BN_T, A_MN, B_MN>(acc, da_hi, db_hi, 1u);
       }
+      wgmma_commit();
       // at most one group in flight: the previous k-block's MMAs have retired, so its stage goes back to the producers
       wgmma_wait<1>();
       reg_fence<BN_T / 2>(acc);
@@ -200,17 +186,16 @@ __global__ void __launch_bounds__(kThreads, 1) k_gemm_tc(const TcArgs a) {
       float4 va[4][2], vb[NBC][2];
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const bool ok = !(a.debug & 1) && (A_MN ? (a_row0 < p.M && a_k0 + q * (kProducerThreads >> a_rcs) < krem)
-                                                : (a_row0 + 32 * q < p.M && a_k0 < krem));
+        const bool ok = A_MN ? (a_row0 < p.M && a_k0 + q * (kProducerThreads >> a_rcs) < krem)
+                             : (a_row0 + 32 * q < p.M && a_k0 < krem);
         const float* src = a_g0 + (int64_t)i * a_kstride + q * a_gq;
         va[q][0] = ok ? ld4(src) : f4zero();
         va[q][1] = ok ? ld4(src + 4) : f4zero();
       }
 #pragma unroll
-      for (int q = 0; q < (BPRE ? 0 : NBC); ++q) {
-        const bool ok = !(a.debug & 1) && q < nb_chunks &&
-                        (B_MN ? (b_row0 < p.N && b_k0 + q * (kProducerThreads >> b_rcs) < krem)
-                              : (b_row0 + 32 * q < p.N && b_k0 < krem));
+      for (int q = 0; q < NBC; ++q) {
+        const bool ok = q < nb_chunks && (B_MN ? (b_row0 < p.N && b_k0 + q * (kProducerThreads >> b_rcs) < krem)
+                                               : (b_row0 + 32 * q < p.N && b_k0 < krem));
         const float* src = b_g0 + (int64_t)i * b_kstride + q * b_gq;
         vb[q][0] = ok ? ld4(src) : f4zero();
         vb[q][1] = ok ? ld4(src + 4) : f4zero();
@@ -230,31 +215,21 @@ __global__ void __launch_bounds__(kThreads, 1) k_gemm_tc(const TcArgs a) {
       uint8_t* sa_lo = st + kATileBytes;
       uint8_t* sb_hi = st + plane * kATileBytes;
       uint8_t* sb_lo = sb_hi + b_tile_bytes;
-      if (BPRE && tid == 0) {   // bulk TMA of the pre-packed weight tile(s) of this k-block
-        const int64_t off = ((int64_t)(kb_begin + i + a.bpk_kb0) * a.bpk_groups + ((n0 + a.bpk_row0) >> a.bpk_shift))
-                            << (7 + a.bpk_shift);
-        const uint32_t bar = smem_u32(&bars[s]);
-        mbar_arrive_expect_tx(bar, (uint32_t)(plane * b_tile_bytes));
-        tma_bulk_g2s(smem_u32(sb_hi), a.bpk_hi + off, (uint32_t)b_tile_bytes, bar);
-        if (SPLIT) tma_bulk_g2s(smem_u32(sb_lo), a.bpk_lo + off, (uint32_t)b_tile_bytes, bar);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        uint4 hi, lo;
+        split8(reinterpret_cast<const float*>(va[q]), hi, lo);
+        *reinterpret_cast<uint4*>(sa_hi + a_s0 + q * a_sq) = hi;
+        if (SPLIT) *reinterpret_cast<uint4*>(sa_lo + a_s0 + q * a_sq) = lo;
       }
-      if (!(a.debug & 2)) {
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
+      for (int q = 0; q < NBC; ++q)
+        if (q < nb_chunks) {
           uint4 hi, lo;
-          split8(reinterpret_cast<const float*>(va[q]), hi, lo);
-          *reinterpret_cast<uint4*>(sa_hi + a_s0 + q * a_sq) = hi;
-          if (SPLIT) *reinterpret_cast<uint4*>(sa_lo + a_s0 + q * a_sq) = lo;
+          split8(reinterpret_cast<const float*>(vb[q]), hi, lo);
+          *reinterpret_cast<uint4*>(sb_hi + b_s0 + q * b_sq) = hi;
+          if (SPLIT) *reinterpret_cast<uint4*>(sb_lo + b_s0 + q * b_sq) = lo;
         }
-#pragma unroll
-        for (int q = 0; q < (BPRE ? 0 : NBC); ++q)
-          if (q < nb_chunks) {
-            uint4 hi, lo;
-            split8(reinterpret_cast<const float*>(vb[q]), hi, lo);
-            *reinterpret_cast<uint4*>(sb_hi + b_s0 + q * b_sq) = hi;
-            if (SPLIT) *reinterpret_cast<uint4*>(sb_lo + b_s0 + q * b_sq) = lo;
-          }
-      } else if (va[0][0].x == 123.456f) { sa_hi[0] = (uint8_t)va[1][0].x; }   // keep the loads alive
       fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor core (async proxy)
       __syncwarp();
       if (lane == 0) mbar_arrive(smem_u32(&bars[s]));
@@ -281,7 +256,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_gemm_tc(const TcArgs a) {
     const int q = warp & 3, half = warp >> 2;
     const int row = m0 + q * 32 + lane;
     const bool row_ok = row < p.M;
-    const int nchunks = (a.debug & 8) ? 0 : (a.BN >> 4);
+    const int nchunks = a.BN >> 4;
     for (int c = half; c < nchunks; c += 2) {
       const int gn = n0 + c * 16;
       if (gn >= p.N) break;
@@ -397,51 +372,37 @@ __global__ void __launch_bounds__(kThreads, 1) k_gemm_tc(const TcArgs a) {
 
 }
 
-int g_tc_debug = 0;
 int g_tc_force_bn = 0;
 
 inline bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
-template <bool A_MN, bool B_MN, bool SPLIT, int BN_T, bool BPRE>
+template <bool A_MN, bool B_MN, bool SPLIT, int BN_T>
 int launch1(const TcArgs& a, dim3 grid, size_t smem, cudaStream_t stream) {
   static bool attr_done = false;
   if (!attr_done) {
-    GPS_CUDA(cudaFuncSetAttribute(k_gemm_tc<A_MN, B_MN, SPLIT, BN_T, BPRE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    GPS_CUDA(cudaFuncSetAttribute(k_gemm_tc<A_MN, B_MN, SPLIT, BN_T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   227 * 1024));
     attr_done = true;
   }
-  k_gemm_tc<A_MN, B_MN, SPLIT, BN_T, BPRE><<<grid, kThreads, smem, stream>>>(a);
+  k_gemm_tc<A_MN, B_MN, SPLIT, BN_T><<<grid, kThreads, smem, stream>>>(a);
   GPS_LAUNCH_CHECK();
   return GPS_OK;
 }
 template <bool A_MN, bool B_MN, bool SPLIT>
 int launch(const TcArgs& a, dim3 grid, size_t smem, cudaStream_t stream) {
-  if constexpr (!A_MN) {
-    if (a.bpk_hi)
-      return a.nb_blocks == 1 ? launch1<false, B_MN, SPLIT, 64, true>(a, grid, smem, stream)
-                              : launch1<false, B_MN, SPLIT, 128, true>(a, grid, smem, stream);
-  }
-  return a.nb_blocks == 1 ? launch1<A_MN, B_MN, SPLIT, 64, false>(a, grid, smem, stream)
-                          : launch1<A_MN, B_MN, SPLIT, 128, false>(a, grid, smem, stream);
+  return a.nb_blocks == 1 ? launch1<A_MN, B_MN, SPLIT, 64>(a, grid, smem, stream)
+                          : launch1<A_MN, B_MN, SPLIT, 128>(a, grid, smem, stream);
 }
 
 }  // namespace
 
-void gemm_tc_set_debug(int v) {   // low 4 bits: triage switches; bits 8.. : forced tile width (0 = heuristic)
-  g_tc_debug = v & 0xFF;
+void gemm_tc_set_debug(int v) {   // bits 8.. : forced tile width (0 = heuristic)
   g_tc_force_bn = (v >> 8) & 0x1FF;
 }
 
 int gemm_tc(const GemmParams& p, cudaStream_t stream) {
-  static const int mode = [] {
-    const char* e = getenv("GPS_B200_TC");
-    return e ? atoi(e) : 3;   // bit0: K-major operands, bit1: MN-major operands
-  }();
   if (p.M <= 0 || p.N <= 0) return GPS_OK;
   if (p.K <= 0) return GPS_ERR_UNSUPPORTED;
-  const bool any_mn = p.ta || p.tb;
-  if (!(mode & 1)) return GPS_ERR_UNSUPPORTED;
-  if (any_mn && !(mode & 2)) return GPS_ERR_UNSUPPORTED;
   // 128-bit paths: aligned bases, leading dimensions and N multiples of 4
   if (!aligned16(p.A) || !aligned16(p.B) || !aligned16(p.C) || p.lda % 4 || p.ldb % 4 || p.ldc % 4 || p.N % 4)
     return GPS_ERR_UNSUPPORTED;
@@ -467,8 +428,6 @@ int gemm_tc(const GemmParams& p, cudaStream_t stream) {
   // tile width: BN in {64, 128} (1 or 2 staged 64-column blocks; the two warpgroups hold 128 x BN fp32 accumulators
   // beside the producers' staging registers); the kernel is bound by operand traffic ~ tiles x (128 + staged B rows),
   // so minimise waves x staged rows, wider on ties
-  const bool pre_k = p.bpk && !p.bpk_mn && !p.ta && !p.tb && p.bpk_row0 % 8 == 0 && (split ? p.bpk_lo_off > 0 : true);
-  const bool pre_mn = p.bpk && p.bpk_mn && !p.ta && p.tb && p.bpk_row0 % 64 == 0 && (split ? p.bpk_lo_off > 0 : true);
   int bestBN = 128;
   long bestCost = -1;
   for (int bn = 128; bn >= 64; bn >>= 1) {
@@ -494,15 +453,6 @@ int gemm_tc(const GemmParams& p, cudaStream_t stream) {
   const int splitk = 1;
   a.kb_per_split = nkb;
   a.p.splitk = p.splitk > 1 ? 2 : 1;   // "accumulate atomically" flag
-  a.debug = g_tc_debug;
-  a.bpk_hi = a.bpk_lo = nullptr; a.bpk_groups = 0; a.bpk_row0 = 0; a.bpk_shift = 3; a.bpk_kb0 = p.bpk_kb0;
-  if (pre_k || pre_mn) {
-    a.bpk_hi = (const uint8_t*)p.bpk;
-    a.bpk_lo = a.bpk_hi + p.bpk_lo_off;
-    a.bpk_groups = p.bpk_groups;
-    a.bpk_row0 = p.bpk_row0;
-    a.bpk_shift = pre_mn ? 6 : 3;
-  }
   const size_t smem = (size_t)stages * stage_bytes + 1024 /*align*/ + (2 * stages + 1) * 8 + 16 + 16 * 16 * 8 * 4;
   dim3 grid((unsigned)ceil_div(p.N, a.BN), (unsigned)mt, (unsigned)splitk);
   const bool amn = p.ta != 0, bmn = p.tb != 0;
@@ -517,90 +467,4 @@ int gemm_tc(const GemmParams& p, cudaStream_t stream) {
   return GPS_ERR_UNSUPPORTED;
 }
 
-}  // namespace gps
-
-// ------------------------------------------------------------------------------------ weight pre-packing
-namespace gps {
-namespace {
-struct PrepackDesc {
-  PrepackItem it[16];
-  int start[17];   // CTA index range of each item (1-D grid: no empty CTAs)
-  int n;
-};
-// K-major item: one CTA per (k-block, 8-row group) writes the 1024-byte swizzled group of both planes.
-// MN-major item (W is [K x cols]): one CTA per (k-block, 64-column block x 8-k-row group).
-__global__ void k_prepack_weights(PrepackDesc d) {
-  int item = 0;
-  while (item + 1 < d.n && (int)blockIdx.x >= d.start[item + 1]) ++item;
-  const PrepackItem& it = d.it[item];
-  const int local = (int)blockIdx.x - d.start[item];
-  const int r = threadIdx.x >> 3, ck = threadIdx.x & 7;      // 64 threads: 8 rows x 8 sixteen-byte chunks
-  const int nkb = (it.K + 63) / 64;
-  float v[8];
-  uint4 hi, lo;
-  if (!it.mn) {
-    const int groups = (it.rows + 256 + 7) / 8;
-    const int kb = local / groups, grp = local - kb * groups;
-    const int row = grp * 8 + r, k = kb * 64 + ck * 8;
-    if (row < it.rows && k + 8 <= it.K) {
-      const float4 x = ld4(it.W + (int64_t)row * it.ld + k), y = ld4(it.W + (int64_t)row * it.ld + k + 4);
-      v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w; v[4] = y.x; v[5] = y.y; v[6] = y.z; v[7] = y.w;
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = (row < it.rows && k + i < it.K) ? it.W[(int64_t)row * it.ld + k + i] : 0.f;
-    }
-    tc::split8(v, hi, lo);
-    const int64_t plane = (int64_t)nkb * groups * 1024;
-    uint8_t* base = reinterpret_cast<uint8_t*>(it.dst) + ((int64_t)kb * groups + grp) * 1024 + r * 128 + ((ck ^ r) << 4);
-    *reinterpret_cast<uint4*>(base) = hi;
-    *reinterpret_cast<uint4*>(base + plane) = lo;
-  } else {
-    // it.K = reduction extent (rows of W), it.rows = output columns of the GEMM (columns of W)
-    const int cblocks = (it.rows + 256 + 63) / 64, nx = cblocks * 8;
-    const int kb = local / nx, x = local - kb * nx;
-    const int cb = x >> 3, kg = x & 7;
-    const int k = kb * 64 + kg * 8 + r, col = cb * 64 + ck * 8;
-    if (k < it.K && col + 8 <= it.rows) {
-      const float4 x0 = ld4(it.W + (int64_t)k * it.ld + col), y0 = ld4(it.W + (int64_t)k * it.ld + col + 4);
-      v[0] = x0.x; v[1] = x0.y; v[2] = x0.z; v[3] = x0.w; v[4] = y0.x; v[5] = y0.y; v[6] = y0.z; v[7] = y0.w;
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = (k < it.K && col + i < it.rows) ? it.W[(int64_t)k * it.ld + col + i] : 0.f;
-    }
-    tc::split8(v, hi, lo);
-    const int64_t plane = (int64_t)nkb * cblocks * 8192;
-    uint8_t* base = reinterpret_cast<uint8_t*>(it.dst) + ((int64_t)kb * cblocks + cb) * 8192 + kg * 1024 + r * 128 +
-                    ((ck ^ r) << 4);
-    *reinterpret_cast<uint4*>(base) = hi;
-    *reinterpret_cast<uint4*>(base + plane) = lo;
-  }
-}
-}  // namespace
-
-int prepack_groups(int rows) { return (rows + 256 + 7) / 8; }
-int64_t prepack_plane_bytes(int rows, int K) { return (int64_t)((K + 63) / 64) * prepack_groups(rows) * 1024; }
-int64_t prepack_bytes(int rows, int K) { return 2 * prepack_plane_bytes(rows, K); }
-int prepack_groups_mn(int cols) { return (cols + 256 + 63) / 64; }
-int64_t prepack_plane_bytes_mn(int cols, int K) { return (int64_t)((K + 63) / 64) * prepack_groups_mn(cols) * 8192; }
-int64_t prepack_bytes_mn(int cols, int K) { return 2 * prepack_plane_bytes_mn(cols, K); }
-
-int prepack_weights(const PrepackItem* items, int n, cudaStream_t stream) {
-  if (n <= 0) return GPS_OK;
-  GPS_REQUIRE(n <= 16, GPS_ERR_ARG, "prepack_weights: at most 16 matrices per call");
-  PrepackDesc d;
-  d.n = n;
-  int total = 0;
-  for (int i = 0; i < n; ++i) {
-    d.it[i] = items[i];
-    GPS_REQUIRE(items[i].ld % 4 == 0 && (reinterpret_cast<uintptr_t>(items[i].W) & 15) == 0, GPS_ERR_ARG,
-                "prepack_weights: weights must be 16-byte aligned with ld %% 4 == 0");
-    d.start[i] = total;
-    total += ((items[i].K + 63) / 64) * (items[i].mn ? prepack_groups_mn(items[i].rows) * 8 : prepack_groups(items[i].rows));
-  }
-  d.start[n] = total;
-  if (total == 0) return GPS_OK;
-  k_prepack_weights<<<(unsigned)total, 64, 0, stream>>>(d);
-  GPS_LAUNCH_CHECK();
-  return GPS_OK;
-}
 }  // namespace gps

@@ -63,15 +63,11 @@ static std::atomic<unsigned long long> g_fallbacks{0};
 // on the fp32 operands, else (odd shapes / alignment) the exact CUDA-core kernel - counted, and an error under
 // GPS_B200_STRICT=1 so that a 10x slower path can never be taken silently.
 int gemm(const GemmParams& p, cudaStream_t stream) {
-  static const int mode = [] {   // GPS_B200_GEMM: "simt" = CUDA-core only, "tc" = no TMA kernel, default = all
-    const char* e = getenv("GPS_B200_GEMM");
-    return e && strcmp(e, "simt") == 0 ? 2 : (e && strcmp(e, "tc") == 0 ? 1 : 0);
-  }();
   static const bool strict = [] {
     const char* e = getenv("GPS_B200_STRICT");
     return e && e[0] == '1';
   }();
-  if (mode == 0 && p.Ap.hi && p.Bp.hi) {
+  if (p.Ap.hi && p.Bp.hi) {
     int rc = gemm_tma(p, stream);
     if (rc != GPS_ERR_UNSUPPORTED) return rc;
   }
@@ -82,15 +78,12 @@ int gemm(const GemmParams& p, cudaStream_t stream) {
   if (q.Cp.hi) {   // the fp32 kernels do not write planes: convert afterwards
     q.Cp = Planes();
   }
-  int rc = GPS_ERR_UNSUPPORTED;
-  if (mode != 2) rc = gemm_tc(q, stream);
+  int rc = gemm_tc(q, stream);
   if (rc == GPS_ERR_UNSUPPORTED) {
-    if (mode != 2) {
-      g_fallbacks.fetch_add(1, std::memory_order_relaxed);
-      GPS_REQUIRE(!strict, GPS_ERR_UNSUPPORTED,
-                  "GPS_B200_STRICT: dense product M=%d N=%d K=%d (ta=%d tb=%d) would fall back to the CUDA-core kernel",
-                  p.M, p.N, p.K, p.ta, p.tb);
-    }
+    g_fallbacks.fetch_add(1, std::memory_order_relaxed);
+    GPS_REQUIRE(!strict, GPS_ERR_UNSUPPORTED,
+                "GPS_B200_STRICT: dense product M=%d N=%d K=%d (ta=%d tb=%d) would fall back to the CUDA-core kernel",
+                p.M, p.N, p.K, p.ta, p.tb);
     rc = gemm_simt(q, stream);
   }
   if (rc == GPS_OK && p.Cp.hi) {
@@ -133,15 +126,13 @@ struct Side {
   int join(cudaStream_t main) { return order(s, main); }
 };
 
-// A/B switches (GPS_B200_OPT): 1 MN-major weight planes, 2 merged attention backward, 4 early edge BN backward,
-// 8 projection gradients split into the message-passing and attention column blocks
+// Backward-pass fusions, off by default (GPS_B200_OPT bit mask): 32 reduces local_model.bn_node_x inside the
+// norm1_local apply pass, 64 reduces norm1_local / norm1_attn in the epilogue of the GEMM producing g_s.  Each saves a
+// launch, but the fused kernels run as few fat CTAs and delay the branches behind them.
 static int opt_flags() {
   static const int v = [] {
     const char* e = getenv("GPS_B200_OPT");
-    return e ? atoi(e) : 7;   // Off by default: 8 (split dgrad+wgrad tail), 16 (two-part Wcat wgrad), 32 + 64
-                              // (bn_node_x reduce inside the norm1_local apply pass, norm1_local / norm1_attn reduces
-                              // in the epilogue of the GEMM producing g_s): three launches fewer, but the fused kernels
-                              // run as few fat CTAs and delay the branches behind them
+    return e ? atoi(e) : 0;
   }();
   return v;
 }
@@ -178,9 +169,8 @@ __global__ void k_pack(PackDesc pd, float* __restrict__ Wcat, float* __restrict_
   for (int c = threadIdx.x * 4; c < pd.d; c += blockDim.x * 4) st4(dst + c, ld4(src + c));
   if (threadIdx.x == 0) bcat[r] = pd.seg[s].b ? pd.seg[s].b[r - row0] : 0.f;
 }
-__global__ void k_unpack(PackDesc pd, const float* __restrict__ gWcat, const float* __restrict__ gbcat, int accumulate,
-                         int row_begin) {
-  const int r = blockIdx.x + row_begin;
+__global__ void k_unpack(PackDesc pd, const float* __restrict__ gWcat, const float* __restrict__ gbcat, int accumulate) {
+  const int r = blockIdx.x;
   int row0 = 0, s = 0;
   while (s < pd.nseg - 1 && r >= row0 + pd.seg[s].rows) row0 += pd.seg[s++].rows;
   if (pd.seg[s].gw) {
@@ -207,11 +197,6 @@ struct Plan {
   float *Wcat, *bcat, *Y1, *ehat, *xt, *xloc, *O, *lse, *hA, *s, *hid, *hid_pre, *t, *bnbuf;
   float *agg, *h1, *h1_pre;
   float* dinv;   // GCN: deg^-1/2 per node
-  // pre-packed bf16 hi/lo weight planes for the forward GEMMs (bulk-TMA B operand)
-  uint8_t *pk_cat, *pk_C, *pk_out, *pk_ff1, *pk_ff2, *pk_g0, *pk_g1;
-  // the same weights as MN-major planes for the data-gradient GEMMs of the backward pass (training only)
-  uint8_t *pt_cat, *pt_C, *pt_out, *pt_ff1, *pt_ff2, *pt_g0, *pt_g1;
-  bool prepack;
   // bf16 hi/lo operand planes of the TMA-fed GEMM (gemm_tma.cu).  Saved: layer inputs, weights and the forward
   // activations the weight gradients re-read; workspace: the backward gradients that feed GEMMs.
   bool use_planes;
@@ -231,15 +216,6 @@ struct Plan {
   int64_t bwd_bytes;
   int64_t fwd_launches, bwd_launches;
 };
-
-// GPS_B200_GEMM=tc|simt keeps the round-1 operand path (register-staged conversion per consuming CTA)
-static bool planes_enabled() {
-  static const bool v = [] {
-    const char* e = getenv("GPS_B200_GEMM");
-    return !(e && (strcmp(e, "tc") == 0 || strcmp(e, "simt") == 0));
-  }();
-  return v;
-}
 
 // Forward softmax attention on the tensor cores (attention_tc.cu) when the batch's graphs are large enough for 128 x 128
 // tiles to pay: at the PCQM4M shape (mean 14 nodes per graph) a 128-row tile sees ~45 useful keys of 256 in one
@@ -339,8 +315,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   P->hid = S.alloc<float>(N * 2 * d);
   if (gelu) P->hid_pre = S.alloc<float>(N * 2 * d);
   P->t = S.alloc<float>(N * d);
-  P->prepack = (d % 8 == 0) && (!P->perf || P->inner % 8 == 0);
-  P->use_planes = P->prepack && planes_enabled();
+  P->use_planes = (d % 8 == 0) && (!P->perf || P->inner % 8 == 0);
   const bool lo = a->precision == GPS_PREC_FP32;
   auto mkplanes = [&](Arena& A, int64_t rows, int64_t cols) {
     Planes q;
@@ -399,29 +374,6 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
     P->wplanes_bytes = Wc.used;
     GPS_REQUIRE(!Wa.overflow, GPS_ERR_ARG, "wplanes buffer too small (%lld < %lld)", (long long)a->wplanes_bytes,
                 (long long)Wc.used);
-  }
-  if (P->prepack && !P->use_planes) {
-    const int64_t kout = P->perf ? P->inner : d;
-    if (P->Wy) P->pk_cat = S.alloc<uint8_t>(prepack_bytes((int)P->Wy, (int)d));
-    if (P->gated) P->pk_C = S.alloc<uint8_t>(prepack_bytes((int)d, (int)d));
-    if (P->attn || P->perf) P->pk_out = S.alloc<uint8_t>(prepack_bytes((int)d, (int)kout));
-    P->pk_ff1 = S.alloc<uint8_t>(prepack_bytes((int)(2 * d), (int)d));
-    P->pk_ff2 = S.alloc<uint8_t>(prepack_bytes((int)d, (int)(2 * d)));
-    if (P->gine) {
-      P->pk_g0 = S.alloc<uint8_t>(prepack_bytes((int)d, (int)d));
-      P->pk_g1 = S.alloc<uint8_t>(prepack_bytes((int)d, (int)d));
-    }
-    if (a->training) {   // W as [K = out features] x [N = in features]
-      if (P->Wy) P->pt_cat = S.alloc<uint8_t>(prepack_bytes_mn((int)d, (int)P->Wy));
-      if (P->gated) P->pt_C = S.alloc<uint8_t>(prepack_bytes_mn((int)d, (int)d));
-      if (P->attn || P->perf) P->pt_out = S.alloc<uint8_t>(prepack_bytes_mn((int)kout, (int)d));
-      P->pt_ff1 = S.alloc<uint8_t>(prepack_bytes_mn((int)d, (int)(2 * d)));
-      P->pt_ff2 = S.alloc<uint8_t>(prepack_bytes_mn((int)(2 * d), (int)d));
-      if (P->gine) {
-        P->pt_g0 = S.alloc<uint8_t>(prepack_bytes_mn((int)d, (int)d));
-        P->pt_g1 = S.alloc<uint8_t>(prepack_bytes_mn((int)d, (int)d));
-      }
-    }
   }
   P->saved_bytes = S.used;
   GPS_REQUIRE(!S.overflow, GPS_ERR_ARG, "saved buffer too small (%lld < %lld)", (long long)a->saved_bytes,
@@ -680,23 +632,12 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
   cudaStream_t s2 = sd ? sd->s : st;
   const bool two_branches = (P.gated || P.gine || P.gcn) && (P.attn || P.perf);
 
-  // weights: concatenate the node projections, then pre-pack every forward weight into the wgmma kernel's
-  // shared-memory tile image (bf16 hi/lo planes) so its B operand arrives by bulk TMA
+  // weights: concatenate the node projections
   if (P.Wy) {
     PackDesc pdsc0 = pack_desc(a, P);
     k_pack<<<(unsigned)pdsc0.total_rows, 128, 0, st>>>(pdsc0, P.Wcat, P.bcat);
     GPS_LAUNCH_CHECK();
   }
-  auto set_bpk = [&](GemmParams& g, const uint8_t* pk, int64_t rows, int64_t K, int64_t row0) {
-    if (!P.prepack || !pk) return;
-    g.bpk = pk;
-    g.bpk_lo_off = prepack_plane_bytes((int)rows, (int)K);
-    g.bpk_groups = prepack_groups((int)rows);
-    g.bpk_row0 = (int)row0;
-  };
-  // Weight planes: the ones the first GEMMs need are packed on the caller's stream; the rest (output projection,
-  // FFN, and the MN-major images the backward pass reads) are packed next to those GEMMs on their own stream.
-  cudaStream_t sp = sd ? sd->s4 : st;
   if (P.use_planes) {
     // layer inputs and every weight -> bf16 hi/lo planes, one launch (the producers inside the layer write the
     // planes of their outputs themselves).  Wcat_p rows follow pack_desc(): [A;B;D;E | conv] then in_proj.
@@ -734,35 +675,6 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
   weights_done:
     GPS_TRY(to_planes(it, ni, st));
   }
-  if (P.prepack && !P.use_planes) {
-    PrepackItem items[16];
-    int ni = 0;
-    const int64_t kout = P.perf ? P.inner : d;
-    if (P.Wy) items[ni++] = PrepackItem{P.Wcat, (int)P.Wy, (int)d, (int)d, P.pk_cat};
-    if (P.gated) items[ni++] = PrepackItem{a->gcn_C.weight, (int)d, (int)d, (int)d, P.pk_C};
-    if (P.gine) {
-      items[ni++] = PrepackItem{a->gine_lin0.weight, (int)d, (int)d, (int)d, P.pk_g0};
-      items[ni++] = PrepackItem{a->gine_lin1.weight, (int)d, (int)d, (int)d, P.pk_g1};
-    }
-    GPS_TRY(prepack_weights(items, ni, st));
-    ni = 0;
-    if (sp != st) GPS_TRY(sd->order(st, sp));
-    if (P.attn || P.perf) items[ni++] = PrepackItem{a->attn_out.weight, (int)d, (int)kout, (int)kout, P.pk_out};
-    items[ni++] = PrepackItem{a->ff1.weight, (int)(2 * d), (int)d, (int)d, P.pk_ff1};
-    items[ni++] = PrepackItem{a->ff2.weight, (int)d, (int)(2 * d), (int)(2 * d), P.pk_ff2};
-    if (a->training && (opt_flags() & 1)) {   // MN-major images for the backward data gradients: W is [K x N] there
-      if (P.Wy) items[ni++] = PrepackItem{P.Wcat, (int)d, (int)P.Wy, (int)d, P.pt_cat, 1};
-      if (P.gated) items[ni++] = PrepackItem{a->gcn_C.weight, (int)d, (int)d, (int)d, P.pt_C, 1};
-      if (P.attn || P.perf) items[ni++] = PrepackItem{a->attn_out.weight, (int)kout, (int)d, (int)kout, P.pt_out, 1};
-      items[ni++] = PrepackItem{a->ff1.weight, (int)d, (int)(2 * d), (int)d, P.pt_ff1, 1};
-      items[ni++] = PrepackItem{a->ff2.weight, (int)(2 * d), (int)d, (int)(2 * d), P.pt_ff2, 1};
-      if (P.gine) {
-        items[ni++] = PrepackItem{a->gine_lin0.weight, (int)d, (int)d, (int)d, P.pt_g0, 1};
-        items[ni++] = PrepackItem{a->gine_lin1.weight, (int)d, (int)d, (int)d, P.pt_g1, 1};
-      }
-    }
-    GPS_TRY(prepack_weights(items, ni, sp));
-  }
   if (P.gated) {   // edge projection has no dependency on the node side: run it next to the node projections
     GPS_REQUIRE(a->edge_out, GPS_ERR_ARG, "edge_out is null");
     if (sd) GPS_TRY(sd->fork(st));
@@ -770,7 +682,6 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     g.M = (int)E; g.N = (int)d; g.K = (int)d;
     g.A = a->edge_attr; g.lda = (int)d; g.B = a->gcn_C.weight; g.ldb = (int)d; g.C = P.ehat; g.ldc = (int)d;
     g.bias = a->gcn_C.bias; g.precision = a->precision;
-    set_bpk(g, P.pk_C, d, d, 0);
     g.Ap = P.e_p; g.Bp = P.C_p;
     GPS_TRY(gemm(g, s2));
   }
@@ -791,7 +702,6 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
       g.M = (int)N; g.N = (int)wg; g.K = (int)d;
       g.A = a->x; g.lda = (int)d; g.B = P.Wcat + wl * d; g.ldb = (int)d; g.C = P.Y1 + wl; g.ldc = (int)P.Wy;
       g.bias = P.bcat + wl; g.precision = a->precision;
-      set_bpk(g, P.pk_cat, P.Wy, d, wl);
       g.Ap = P.x_p; g.Bp = P.Wcat_p.rows(wl);
       if (P.attn_tc) {   // Q | K | V additionally as padded per-head operand planes for the wgmma attention
         g.Cp = P.qkv_p; g.cp_hd = (int)P.hd; g.cp_hd_pad = (int)attention_tc_hd_pad(P.hd); g.cp_col0 = 0;
@@ -803,7 +713,6 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
       g.M = (int)N; g.N = (int)wl; g.K = (int)d;
       g.A = a->x; g.lda = (int)d; g.B = P.Wcat; g.ldb = (int)d; g.C = P.Y1; g.ldc = (int)P.Wy;
       g.bias = P.bcat; g.precision = a->precision;
-      set_bpk(g, P.pk_cat, P.Wy, d, 0);
       g.Ap = P.x_p; g.Bp = P.Wcat_p;
       GPS_TRY(gemm(g, st));
     }
@@ -826,7 +735,6 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     g.M = (int)N; g.N = (int)d; g.K = (int)d;
     g.A = P.agg; g.lda = (int)d; g.B = a->gine_lin0.weight; g.ldb = (int)d; g.C = P.h1; g.ldc = (int)d;
     g.bias = a->gine_lin0.bias; g.act = act; g.C_pre = P.h1_pre; g.ldpre = (int)d; g.precision = a->precision;
-    set_bpk(g, P.pk_g0, d, d, 0);
     g.Ap = P.agg_p; g.Bp = P.g0_p; g.Cp = P.h1_p;
     GPS_TRY(gemm(g, st));
     GemmParams g2;  // x_loc = x + drop(h1 W1^T + b1)  (gps_layer.py:188-189)
@@ -836,7 +744,6 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     g2.p_drop = pd; g2.seed = a->seed; g2.offset = a->offset; g2.site = GPS_SITE_LOCAL;
     g2.offset_dev = (const unsigned long long*)a->offset_dev;
     g2.precision = a->precision;
-    set_bpk(g2, P.pk_g1, d, d, 0);
     g2.Ap = P.h1_p; g2.Bp = P.g1_p;
     GPS_TRY(gemm(g2, st));
   } else if (P.gcn) {
@@ -861,9 +768,7 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     g.p_drop = pd; g.seed = a->seed; g.offset = a->offset; g.site = GPS_SITE_ATTN_OUT;
     g.offset_dev = (const unsigned long long*)a->offset_dev;
     g.precision = a->precision;
-    set_bpk(g, P.pk_out, d, d, 0);
     g.Ap = P.O_p; g.Bp = P.out_p;
-    if (P.prepack && !P.use_planes && sp != st) GPS_TRY(sd->order(sp, sg));
     GPS_TRY(gemm(g, sg));
   }
 
@@ -921,14 +826,12 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
 
   // ---- FFN: t = s + drop(W2 drop(act(W1 s + b1)) + b2)   (gps_layer.py:225, 253-257)
   {
-    if (P.prepack && !P.use_planes && sp != st) GPS_TRY(sd->order(sp, st));
     GemmParams g;
     g.M = (int)N; g.N = (int)(2 * d); g.K = (int)d;
     g.A = P.s; g.lda = (int)d; g.B = a->ff1.weight; g.ldb = (int)d; g.C = P.hid; g.ldc = (int)(2 * d);
     g.bias = a->ff1.bias; g.act = act; g.C_pre = P.hid_pre; g.ldpre = (int)(2 * d);
     g.p_drop = pd; g.seed = a->seed; g.offset = a->offset; g.site = GPS_SITE_FF1; g.precision = a->precision;
     g.offset_dev = (const unsigned long long*)a->offset_dev;
-    set_bpk(g, P.pk_ff1, 2 * d, d, 0);
     g.Ap = P.s_p; g.Bp = P.ff1_p; g.Cp = P.hid_p;
     GPS_TRY(gemm(g, st));
     GemmParams g2;
@@ -937,7 +840,6 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     g2.bias = a->ff2.bias; g2.R1 = P.s; g2.ldr1 = (int)d; g2.stats = stats(BN_2);
     g2.p_drop = pd; g2.seed = a->seed; g2.offset = a->offset; g2.site = GPS_SITE_FF2; g2.precision = a->precision;
     g2.offset_dev = (const unsigned long long*)a->offset_dev;
-    set_bpk(g2, P.pk_ff2, d, 2 * d, 0);
     g2.Ap = P.hid_p; g2.Bp = P.ff2_p;
     GPS_TRY(gemm(g2, st));
     GPS_TRY(bn_combine(P.t, bn_view_fwd(P, a, BN_2, a->norm2, N), nullptr, BnView(), a->x_out, N, d, st,
@@ -992,7 +894,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   const bool two_branches = (P.gated || P.gine || P.gcn) && (P.attn || P.perf);
   cudaStream_t sa = (two_branches && sd) ? sd->s3 : st;   // stream of the attention-branch backward
   const int opt = opt_flags();
-  const bool early_edge = (opt & 4) != 0;
   // data-parallel hook: the caller's event is recorded on the weight-gradient stream once the early gradient group
   // (FFN, attention output projection, norm2 / norm1_local / norm1_attn) has been enqueued there
   // (recorded as EXTERNAL events under stream capture, so that collectives enqueued outside the captured graph can wait
@@ -1006,62 +907,18 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     return GPS_OK;
   };
   auto early_done = [&]() -> int { return record_ev(a->ev_grads_early, s2); };
+  auto mid_done = [&]() -> int { return record_ev(a->ev_grads_mid, s2); };   // after the local model's weight gradients
   // accumulators of the last two GEMMs of the pass are zeroed now, while their streams are idle, instead of on the tail
-  const bool gx_splitk = P.Wy >= 1024 && N > 0 && !((opt & 8) && P.gated && P.attn && sd && P.qkv_off > 0 && P.qkv_off < P.Wy);
+  const bool gx_splitk = P.Wy >= 1024 && N > 0;
   if (P.Wy) {
     if (sd) GPS_TRY(sd->order(st, s2));
     GPS_CUDA(cudaMemsetAsync(P.gWcat, 0, (size_t)(P.Wy * d + P.Wy) * sizeof(float), s2));
   }
   if (gx_splitk) GPS_CUDA(cudaMemsetAsync(a->grad_x, 0, (size_t)(N * d) * sizeof(float), st));
-  // [Ax|Bx|Dx|Ex] gradients are final long before [Q|K|V]'s: their share of dWcat and of g_x = gY1 Wcat is
-  // computed under the attention backward, leaving only the [Q|K|V] share for the tail of the pass
-  const bool split_tail = (opt & 8) && P.gated && P.attn && sd && P.qkv_off > 0 && P.qkv_off < P.Wy && N > 0;
-  auto wcat_wgrad = [&](int64_t r0, int64_t rows) -> int {   // d Wcat[r0 : r0 + rows] (+ bias gradient) on s2
-    GemmParams w;
-    w.M = (int)rows; w.N = (int)d; w.K = (int)N;
-    w.A = P.gY1 + r0; w.lda = (int)P.Wy; w.ta = 1; w.B = a->x; w.ldb = (int)d; w.tb = 1;
-    w.C = P.gWcat + r0 * d; w.ldc = (int)d;
-    w.splitk = splitk_for(N, rows, d) < 2 ? 2 : splitk_for(N, rows, d);
-    w.colsum_a = P.gbcat + r0; w.precision = prec;
-    w.Ap = P.gY1_p.cols(r0); w.Bp = P.x_p;
-    if (prec == GPS_PREC_BF16 && w.Ap.hi && N > 0) {
-      w.colsum_a = nullptr;
-      GPS_TRY(colsum(P.gY1 + r0, P.Wy, N, rows, P.gbcat + r0, s2));
-    }
-    return N > 0 ? gemm(w, s2) : GPS_OK;
-  };
-  // The weight gradient of the fused node projection in two parts (GPS_B200_OPT bit 16, default on): rows [0, qkv_off)
-  // (A, B, D, E / GCN lin) as soon as the message-passing backward has produced their gY1 columns - under the attention
-  // backward - and the in_proj rows at the end.  Shortens the tail of the pass and lets a data-parallel caller reduce
-  // the local model's gradients early (ev_grads_mid).
-  const bool wgrad_split = (opt & 16) && sd && !((opt & 8) && P.gated && P.attn) && P.qkv_off > 0 && P.qkv_off < P.Wy && N > 0;
-  auto unpack_rows = [&](int64_t r0, int64_t rows) -> int {
-    PackDesc pdsc = pack_desc(a, P);
-    k_unpack<<<(unsigned)rows, 128, 0, s2>>>(pdsc, P.gWcat, P.gbcat, g_grads_accumulate ? 1 : 0, (int)r0);
-    GPS_LAUNCH_CHECK();
-    return GPS_OK;
-  };
-  auto mid_done = [&]() -> int {   // on s2, after the local model's weight gradients
-    if (wgrad_split) {
-      GPS_TRY(wcat_wgrad(0, P.qkv_off));
-      GPS_TRY(unpack_rows(0, P.qkv_off));
-    }
-    return record_ev(a->ev_grads_mid, s2);
-  };
 
-  cudaStream_t se = (P.gated && sd && early_edge) ? sd->s4 : st;   // stream of the edge BatchNorm backward
-  // data gradients g_in = g_out W read W through the MN-major planes packed by the forward pass
-  auto set_bpt = [&](GemmParams& g, const uint8_t* pt, int64_t cols, int64_t K) {
-    if (!P.prepack || !pt || !(opt & 1)) return;
-    g.bpk = pt;
-    g.bpk_mn = 1;
-    g.bpk_lo_off = prepack_plane_bytes_mn((int)cols, (int)K);
-    g.bpk_groups = prepack_groups_mn((int)cols);
-    g.bpk_row0 = 0;
-  };
-
-  auto edge_bn_bwd = [&]() -> int {
-    // e_out = e + drop(act(BN_e(e^))) (gatedgcn_layer.py:76-83): g_e^ needs grad_edge_out alone -> off the critical path
+  // e_out = e + drop(act(BN_e(e^))) (gatedgcn_layer.py:76-83): g_e^ needs grad_edge_out alone -> off the critical path
+  cudaStream_t se = (P.gated && sd) ? sd->s4 : st;   // stream of the edge BatchNorm backward
+  if (P.gated) {
     if (se != st) GPS_TRY(sd->order(st, se));
     BnView ve = bview(BN_E, a->bn_edge_e);
     if (a->grad_edge_out && E > 0) {
@@ -1075,9 +932,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
       if (a->bn_edge_e.grad_bias && !g_grads_prezeroed)
         GPS_CUDA(cudaMemsetAsync(a->bn_edge_e.grad_bias, 0, d * sizeof(float), se));
     }
-    return GPS_OK;
-  };
-  if (P.gated && early_edge) GPS_TRY(edge_bn_bwd());
+  }
 
   // ---- norm2 (gps_layer.py:229): g_t
   BnView v2 = bview(BN_2, a->norm2);
@@ -1102,7 +957,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     g.ldmask = (int)(2 * d);
     g.p_drop = pd; g.seed = a->seed; g.offset = a->offset; g.site = GPS_SITE_FF1; g.precision = prec;
     g.offset_dev = (const unsigned long long*)a->offset_dev;
-    set_bpt(g, P.pt_ff2, 2 * d, d);
     g.Ap = g_ff2_p; g.Bp = P.ff2_p; g.Cp = P.ghid_p;
     GPS_TRY(gemm(g, st));
     GPS_TRY(wfork(st));
@@ -1112,7 +966,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     g2.M = (int)N; g2.N = (int)d; g2.K = (int)(2 * d);
     g2.A = P.g_hid; g2.lda = (int)(2 * d); g2.B = a->ff1.weight; g2.ldb = (int)d; g2.tb = 1; g2.C = P.g_s; g2.ldc = (int)d;
     g2.R1 = P.g_t; g2.ldr1 = (int)d; g2.precision = prec;
-    set_bpt(g2, P.pt_ff1, d, 2 * d);
     g2.Ap = P.ghid_p; g2.Bp = P.ff1_p;
     // norm1_local and norm1_attn both take g_s as their upstream gradient (gps_layer.py:194,217,222): their backward
     // reductions ride this GEMM's epilogue instead of two more passes over g_s (GPS_B200_OPT bit 64)
@@ -1169,7 +1022,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     g.M = (int)N; g.N = (int)d; g.K = (int)d;
     g.A = g_ao; g.lda = (int)d; g.B = a->attn_out.weight; g.ldb = (int)d; g.tb = 1; g.C = P.g_O; g.ldc = (int)d;
     g.precision = prec;
-    set_bpt(g, P.pt_out, d, d);
     g.Ap = g_ao_p; g.Bp = P.out_p;
     GPS_TRY(gemm(g, sa));
     GPS_TRY(wfork(sa));
@@ -1197,7 +1049,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     g.M = (int)N; g.N = (int)inner; g.K = (int)d;
     g.A = g_ao; g.lda = (int)d; g.B = a->attn_out.weight; g.ldb = (int)inner; g.tb = 1; g.C = P.g_O; g.ldc = (int)inner;
     g.precision = prec;
-    set_bpt(g, P.pt_out, inner, d);
     GPS_TRY(gemm(g, sa));
     GPS_TRY(wfork(sa));
     GPS_TRY(linear_wgrad(g_ao, d, P.O, inner, N, d, inner, a->attn_out.grad_weight, a->attn_out.grad_bias, prec, s2));
@@ -1242,7 +1093,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     if (!chain_x) GPS_TRY(bn_bwd_reduce(P.g_xloc, d, P.xt, d, N, d, vx, act, drop(GPS_SITE_GCN_X), sums(BN_X), st));
     GPS_TRY(bn_bwd_apply(P.g_xloc, d, P.xt, d, N, d, vx, act, drop(GPS_SITE_GCN_X), sums(BN_X), P.gY1, P.Wy,
                          a->bn_node_x.grad_weight, a->bn_node_x.grad_bias, st, g_grads_accumulate, P.gY1_p));
-    if (!early_edge) GPS_TRY(edge_bn_bwd());
     if (se != st) GPS_TRY(sd->order(se, st));
     // message/aggregate backward (SURVEY Appendix C)
     GPS_TRY(gatedgcn_bwd_dst(a->graph, d, P.gY1, P.Wy, P.ehat, P.Y1 + d, P.Wy, P.g_e, P.g_num, P.gY1 + 2 * d, st, P.ge_p,
@@ -1258,19 +1108,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
       g.M = (int)E; g.N = (int)d; g.K = (int)d;
       g.A = P.g_e; g.lda = (int)d; g.B = a->gcn_C.weight; g.ldb = (int)d; g.tb = 1; g.C = a->grad_edge_attr; g.ldc = (int)d;
       g.R1 = a->grad_edge_out; g.ldr1 = (int)d; g.precision = prec;
-      set_bpt(g, P.pt_C, d, d);
       g.Ap = P.ge_p; g.Bp = P.C_p;
-      GPS_TRY(gemm(g, st));
-    }
-    if (split_tail) {
-      const int64_t wl = P.qkv_off;
-      GPS_TRY(wcat_wgrad(0, wl));
-      GemmParams g;   // g_x = g_xloc + gY1[:, :wl] Wcat[:wl]
-      g.M = (int)N; g.N = (int)d; g.K = (int)wl;
-      g.A = P.gY1; g.lda = (int)P.Wy; g.B = P.Wcat; g.ldb = (int)d; g.tb = 1; g.C = a->grad_x; g.ldc = (int)d;
-      g.R1 = P.g_xloc; g.ldr1 = (int)d; g.precision = prec;
-      set_bpt(g, P.pt_cat, d, P.Wy);
-      g.Ap = P.gY1_p; g.Bp = P.Wcat_p;
       GPS_TRY(gemm(g, st));
     }
     g_x_local = P.g_xloc;  // residual x_in + ...
@@ -1288,7 +1126,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     g.A = g_l1; g.lda = (int)d; g.B = a->gine_lin1.weight; g.ldb = (int)d; g.tb = 1; g.C = P.g_h1; g.ldc = (int)d;
     if (relu) { g.mask_src = P.h1; g.mask_is_post = 1; } else { g.mask_src = P.h1_pre; g.mask_act = act; }
     g.ldmask = (int)d; g.precision = prec;
-    set_bpt(g, P.pt_g1, d, d);
     g.Ap = g_l1_p; g.Bp = P.g1_p; g.Cp = P.gh1_p;
     GPS_TRY(gemm(g, st));
     GPS_TRY(wfork(st));
@@ -1299,7 +1136,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     g2.M = (int)N; g2.N = (int)d; g2.K = (int)d;
     g2.A = P.g_h1; g2.lda = (int)d; g2.B = a->gine_lin0.weight; g2.ldb = (int)d; g2.tb = 1; g2.C = P.g_agg; g2.ldc = (int)d;
     g2.precision = prec;
-    set_bpt(g2, P.pt_g0, d, d);
     g2.Ap = P.gh1_p; g2.Bp = P.g0_p;
     GPS_TRY(gemm(g2, st));
     GPS_REQUIRE(a->grad_edge_attr || E == 0, GPS_ERR_ARG, "grad_edge_attr is required for GINE");
@@ -1326,41 +1162,22 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   if (two_branches && sd) GPS_TRY(sd->order(sa, st));
 
   // ---- g_x = [local paths] + [attention residual] + gY1 Wcat ;  d{A,B,D,E,in_proj}
-  if (P.Wy && split_tail) {
-    const int64_t wl = P.qkv_off, wg = P.Wy - P.qkv_off;
+  if (P.Wy) {
     GPS_TRY(wfork(st));
-    GPS_TRY(wcat_wgrad(wl, wg));
-    GPS_TRY(unpack_rows(0, P.Wy));
-    GemmParams g;   // g_x += g_hA + gY1[:, wl:] Wcat[wl:]  (accumulated onto the first share)
-    g.M = (int)N; g.N = (int)d; g.K = (int)wg;
-    g.A = P.gY1 + wl; g.lda = (int)P.Wy; g.B = P.Wcat + wl * d; g.ldb = (int)d; g.tb = 1; g.C = a->grad_x; g.ldc = (int)d;
-    g.R1 = P.g_hA; g.ldr1 = (int)d; g.precision = prec;
-    g.splitk = 2;
-    if (wl % 64 == 0) {
-      set_bpt(g, P.pt_cat, d, P.Wy);
-      g.bpk_kb0 = (int)(wl / 64);
+    GemmParams w;   // d Wcat (+ bias gradient) on s2, unpacked into the caller's A, B, D, E / conv / in_proj gradients
+    w.M = (int)P.Wy; w.N = (int)d; w.K = (int)N;
+    w.A = P.gY1; w.lda = (int)P.Wy; w.ta = 1; w.B = a->x; w.ldb = (int)d; w.tb = 1; w.C = P.gWcat; w.ldc = (int)d;
+    w.splitk = splitk_for(N, P.Wy, d) < 2 ? 2 : splitk_for(N, P.Wy, d);
+    w.colsum_a = P.gbcat; w.precision = prec;
+    w.Ap = P.gY1_p; w.Bp = P.x_p;
+    if (prec == GPS_PREC_BF16 && w.Ap.hi && N > 0) {   // exact bias gradients in bf16 mode (see linear_wgrad)
+      w.colsum_a = nullptr;
+      GPS_TRY(colsum(P.gY1, P.Wy, N, P.Wy, P.gbcat, s2));
     }
-    g.Ap = P.gY1_p.cols(wl); g.Bp = P.Wcat_p.rows(wl);
-    GPS_TRY(gemm(g, st));
-  } else if (P.Wy) {
-    GPS_TRY(wfork(st));
-    if (wgrad_split) {
-      GPS_TRY(wcat_wgrad(P.qkv_off, P.Wy - P.qkv_off));
-      GPS_TRY(unpack_rows(P.qkv_off, P.Wy - P.qkv_off));
-    } else {
-      GemmParams w;
-      w.M = (int)P.Wy; w.N = (int)d; w.K = (int)N;
-      w.A = P.gY1; w.lda = (int)P.Wy; w.ta = 1; w.B = a->x; w.ldb = (int)d; w.tb = 1; w.C = P.gWcat; w.ldc = (int)d;
-      w.splitk = splitk_for(N, P.Wy, d) < 2 ? 2 : splitk_for(N, P.Wy, d);
-      w.colsum_a = P.gbcat; w.precision = prec;
-      w.Ap = P.gY1_p; w.Bp = P.x_p;
-      if (prec == GPS_PREC_BF16 && w.Ap.hi && N > 0) {   // exact bias gradients in bf16 mode (see linear_wgrad)
-        w.colsum_a = nullptr;
-        GPS_TRY(colsum(P.gY1, P.Wy, N, P.Wy, P.gbcat, s2));
-      }
-      if (N > 0) GPS_TRY(gemm(w, s2));
-      GPS_TRY(unpack_rows(0, P.Wy));
-    }
+    if (N > 0) GPS_TRY(gemm(w, s2));
+    PackDesc pdsc = pack_desc(a, P);
+    k_unpack<<<(unsigned)P.Wy, 128, 0, s2>>>(pdsc, P.gWcat, P.gbcat, g_grads_accumulate ? 1 : 0);
+    GPS_LAUNCH_CHECK();
     GemmParams g;
     g.M = (int)N; g.N = (int)d; g.K = (int)P.Wy;
     g.A = P.gY1; g.lda = (int)P.Wy; g.B = P.Wcat; g.ldb = (int)d; g.tb = 1; g.C = a->grad_x; g.ldc = (int)d;
@@ -1368,7 +1185,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     g.R2 = P.attn ? P.g_hA : (P.perf ? P.g_xp : nullptr); g.ldr2 = (int)d;
     g.precision = prec;
     if (gx_splitk) g.splitk = 4;   // long reduction, few output tiles: split-K fills the machine (grad_x zeroed above)
-    set_bpt(g, P.pt_cat, d, P.Wy);
     g.Ap = P.gY1_p; g.Bp = P.Wcat_p;
     GPS_TRY(gemm(g, st));
   } else if (g_x_local) {

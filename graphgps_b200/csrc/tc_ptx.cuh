@@ -37,12 +37,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// 1-D bulk TMA: global -> shared, completion counted in bytes on an mbarrier (SASS: UBLKCP)
-__device__ __forceinline__ void tma_bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
 // tensor-map TMA (SASS: UTMALDG): one box of a rank-3 tensor {c0 innermost, c1, c2} -> shared
 __device__ __forceinline__ void tma_tile_3d(uint32_t dst_smem, const void* tmap, int c0, int c1, int c2, uint32_t bar) {
   asm volatile(

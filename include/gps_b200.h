@@ -51,8 +51,7 @@ const char* gps_build_arch(void);
 /* number of CUDA kernels this library has launched in the calling process (bench.py reports the
  * delta over its timed region as `gpu_launches`) */
 unsigned long long gps_launch_count(void);
-/* bring-up / tuning hook of the register-staged wgmma GEMM (tools/gemm_triage.py, tools/gemm_tune.py): low byte = stage
- * switches (1 no global loads, 2 no convert/store, 4 no MMA, 8 no epilogue), bits 8.. = forced tile width. 0 = normal. */
+/* tuning hook of the register-staged wgmma GEMM (tools/gemm_tune.py): bits 8.. = forced tile width. 0 = normal. */
 void gps_debug_set(int v);
 /* bring-up hook of the TMA-fed GEMM (tools/gemm_trace.py): force_bn = forced tile width (0 = heuristic); trace = device
  * buffer of 256 x 16 uint64 that the first 256 CTAs of each launch fill with globaltimer phase stamps (NULL = off) */
@@ -195,9 +194,9 @@ typedef struct {
   void* wplanes; int64_t wplanes_bytes; int32_t wplanes_valid; int32_t reserved2;
 
   /* ABI 3 (backward, optional): two more cudaEvent_t of the same kind as ev_grads_early.  ev_grads_mid: the local
-   * model's gradients (A, B, C, D, E / GINE nn / GCN lin, bn_node_x, bn_edge_e) are final - the weight gradient of the
-   * fused node projection is computed in two parts for this, the local column block as soon as the message-passing
-   * backward is done, the in_proj block at the end.  ev_grads_done: every gradient of this layer is final. */
+   * model's gradients outside the fused node projection (C / GINE nn / GCN bias, bn_node_x, bn_edge_e) are final; A, B,
+   * D, E / GCN lin share one weight-gradient GEMM with in_proj at the end of the pass.  ev_grads_done: every gradient
+   * of this layer is final. */
   void* ev_grads_mid;
   void* ev_grads_done;
 } GpsLayerArgs;
