@@ -71,7 +71,7 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
   const GemmParams& p = a.p;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int planes = a.planes;
-  const int b_tile = a.nb_blocks * kBlock;
+  const int b_tile = B_MN ? a.nb_blocks * kBlock : BN_T * 128;   // K-major B: BN rows of 128 bytes
   const int stage_bytes = planes * (kATile + b_tile);
   const int S = a.stages;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);   // full[S], empty[S]
@@ -267,23 +267,23 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
       cluster.sync();   // no rank leaves while another still reads its shared memory
     }
     // ---- phase 2: G = BN/4 threads per row, each owning 4 consecutive columns for all of its rows: every global access
-    // (bias, residuals, act' mask, fp32 / plane stores, split-K atomics) is a contiguous row segment, the per-column
-    // constants live in registers and the BatchNorm column sums are accumulated per thread.
+    // (bias, residuals, act' mask, fp32 / plane stores, split-K atomics) is a contiguous row segment and the per-column
+    // constants live in registers.  When BatchNorm column sums are wanted, w goes back into the staging tile for them.
     const int G = a.BN >> 2;
     const int rpp = kEpiWarps * 32 / G;            // rows per pass
     const int rip = tid / G, cg = tid - rip * G;
     const int col = n0 + cg * 4;
     const bool col_ok = rip < rpp && col < p.N;
-    float4 s1 = f4zero(), s2 = f4zero(), q0 = f4zero(), q1 = f4zero();   // sum w, sum w^2, sum w*zhat_0, sum w*zhat_1
+    const int rows_here = min(BM, p.M - m0);
+    const bool colstats = p.stats || p.bnred[0].sums || p.bnred[1].sums;
     if (col_ok) {
       // rows of this thread: r = rip + k * rpp, k < nrows.  Everything is addressed through per-thread base pointers
       // advanced by a constant stride, and the loop is unrolled by 4 rows so that the shared/global loads of a group are
       // in flight together: with 2 epilogue warps per scheduler the pass is instruction-latency bound otherwise
       // (even with the global stores off the critical path).
-      const int rows_here = min(BM, p.M - m0);
       const int nrows = rip < rows_here ? (rows_here - rip + rpp - 1) / rpp : 0;
       const int64_t row0 = m0 + rip;
-      const float* sp = stage + rip * sld + cg * 4;
+      float* sp = stage + rip * sld + cg * 4;
       const int s_st = rpp * sld;
       float* cp = p.C ? p.C + row0 * p.ldc + col : nullptr;
       const int64_t c_st = (int64_t)rpp * p.ldc;
@@ -317,13 +317,6 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
         __nv_bfloat16* pl = p.Cp.lo ? p.Cp.lo + row0 * p.Cp.ld + pcol : nullptr;
         const int64_t p_st = (int64_t)rpp * p.Cp.ld;
         const bool relu = p.act == GPS_ACT_RELU;
-        // fused BatchNorm-backward reductions (bnred): per-column constants -mean and invstd, row pointers into z_k
-        const float* bz0 = p.bnred[0].sums ? p.bnred[0].z + row0 * p.bnred[0].ldz + col : nullptr;
-        const float* bz1 = p.bnred[1].sums ? p.bnred[1].z + row0 * p.bnred[1].ldz + col : nullptr;
-        const int64_t bz0_st = (int64_t)rpp * p.bnred[0].ldz, bz1_st = (int64_t)rpp * p.bnred[1].ldz;
-        float4 bm0 = f4zero(), bi0 = f4zero(), bm1 = f4zero(), bi1 = f4zero();
-        if (bz0) { bm0 = f4scale(ld4(p.bnred[0].mean + col), -1.f); bi0 = ld4(p.bnred[0].invstd + col); }
-        if (bz1) { bm1 = f4scale(ld4(p.bnred[1].mean + col), -1.f); bi1 = ld4(p.bnred[1].invstd + col); }
         if (fast) {
           for (int k = 0; k < nrows; k += 4) {
             float4 w[4];
@@ -371,10 +364,7 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
                   if (pl) *reinterpret_cast<uint2*>(pl + (k + u) * p_st + 4 + z) = make_uint2(0u, 0u);
                 }
               }
-              s1 = f4add(s1, w[u]);
-              s2 = f4fma(w[u], w[u], s2);
-              if (bz0) q0 = f4fma(w[u], f4mul(f4add(ld4(bz0 + (k + u) * bz0_st), bm0), bi0), q0);
-              if (bz1) q1 = f4fma(w[u], f4mul(f4add(ld4(bz1 + (k + u) * bz1_st), bm1), bi1), q1);
+              if (colstats) *reinterpret_cast<float4*>(sp + (k + u) * s_st) = w[u];
             }
           }
         } else {
@@ -403,29 +393,46 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
               planes_store4(p.Cp, row, pcol, w);
               for (int z = 0; z < npad; z += 4) planes_store4(p.Cp, row, pcol + 4 + z, f4zero());
             }
-            s1 = f4add(s1, w);
-            s2 = f4fma(w, w, s2);
+            if (colstats) *reinterpret_cast<float4*>(sp + k * s_st) = w;
           }
         }
       }
     }
-    if (p.stats || p.bnred[0].sums || p.bnred[1].sums) {
-      // column sums: the rpp threads that share a column group meet in shared memory (the staging tile is free again
-      // after the barrier), one double atomic per column per CTA and accumulator
+    if (colstats) {
+      // BatchNorm column sums over this tile's rows, in the same order for every tile width: task (y, g) sums rows
+      // y, y + 16, ... of column group g (sum w, sum w^2, sum w*zhat_0, sum w*zhat_1, zhat_k = (z_k - mean_k) invstd_k)
+      // and leaves the four partials in rows y, y + 16, y + 32, y + 48 of its own row class; then one thread per
+      // column group adds the 16 classes in order: one double atomic per column per CTA and accumulator.
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      float4* rs = reinterpret_cast<float4*>(stage);
-      if (rip < rpp) {
-        rs[(rip * G + cg) * 4] = s1;
-        rs[(rip * G + cg) * 4 + 1] = s2;
-        rs[(rip * G + cg) * 4 + 2] = q0;
-        rs[(rip * G + cg) * 4 + 3] = q1;
+      for (int t = tid; t < 16 * G; t += kEpiWarps * 32) {
+        const int y = t / G, g = t - y * G, c = n0 + g * 4;
+        if (c >= p.N) continue;
+        const GemmParams::BnRed& b0 = p.bnred[0];
+        const GemmParams::BnRed& b1 = p.bnred[1];
+        float4 bm0 = f4zero(), bi0 = f4zero(), bm1 = f4zero(), bi1 = f4zero();
+        if (b0.sums) { bm0 = f4scale(ld4(b0.mean + c), -1.f); bi0 = ld4(b0.invstd + c); }
+        if (b1.sums) { bm1 = f4scale(ld4(b1.mean + c), -1.f); bi1 = ld4(b1.invstd + c); }
+        float4 s1 = f4zero(), s2 = f4zero(), q0 = f4zero(), q1 = f4zero();
+        for (int r = y; r < rows_here; r += 16) {
+          const float4 w = *reinterpret_cast<const float4*>(stage + r * sld + g * 4);
+          const int64_t row = m0 + r;
+          s1 = f4add(s1, w);
+          s2 = f4fma(w, w, s2);
+          if (b0.sums) q0 = f4fma(w, f4mul(f4add(ld4(b0.z + row * b0.ldz + c), bm0), bi0), q0);
+          if (b1.sums) q1 = f4fma(w, f4mul(f4add(ld4(b1.z + row * b1.ldz + c), bm1), bi1), q1);
+        }
+        float* o = stage + y * sld + g * 4;
+        *reinterpret_cast<float4*>(o) = s1;
+        *reinterpret_cast<float4*>(o + 16 * sld) = s2;
+        *reinterpret_cast<float4*>(o + 32 * sld) = q0;
+        *reinterpret_cast<float4*>(o + 48 * sld) = q1;
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
       if (tid < G && n0 + tid * 4 < p.N) {
         float4 t[4] = {f4zero(), f4zero(), f4zero(), f4zero()};
-        for (int y = 0; y < rpp; ++y)
+        for (int y = 0; y < 16; ++y)
 #pragma unroll
-          for (int k = 0; k < 4; ++k) t[k] = f4add(t[k], rs[(y * G + tid) * 4 + k]);
+          for (int k = 0; k < 4; ++k) t[k] = f4add(t[k], *reinterpret_cast<const float4*>(stage + (y + 16 * k) * sld + tid * 4));
         const int c0 = n0 + tid * 4;
         auto add4 = [&](double* dst, float4 v) {
           atomic_add_f64(dst + 0, (double)v.x); atomic_add_f64(dst + 1, (double)v.y);
@@ -612,29 +619,45 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream) {
   const int mt = (int)ceil_div(p.M, BM);
   const int nkb = (int)ceil_div(p.K, BK);
   const int splits_hint = p.splitk > 1 ? min(kMaxSplits, min(p.splitk, nkb)) : 1;
-  // tile width (the wgmma instruction shape, so one of 64 / 128 / 256): minimise waves x staged bytes per CTA, wider
-  // on ties (L2 -> SM operand traffic bounds the kernel)
-  int bestBN = 128;
-  long bestCost = -1;
-  for (int bn = 256; bn >= 64; bn >>= 1) {
-    const int nb = bn / 64;
+  // Tile width.  Measured at the layer's shapes, a launch takes time in proportion to the MMA columns its busiest SM
+  // issues: waves x BN, where zero-padded columns count (they cost MMAs and staging like real ones) and
+  // waves = ceil(tiles / CTA slots).  The epilogue's stores and the operand loads of a tile grow with BN as well, and
+  // the fixed cost of a tile is small, so this one product ranks the widths.  64-wide tiles run two CTAs per SM; each
+  // stages its own copy of the A tile (1.5x the L2 -> SM operand bytes of one 128-wide tile), which costs them a
+  // quarter: a wave of them counts as 2 x 64 x 1.25 columns, unless every CTA has an SM of its own (64 columns).
+  // Ties go to the wider tile (fewer CTAs re-read A).
+  // 152 = 304 / 2 divides every column count of the d = 304 layer; it exists for a K-major B only (an MN-major B is
+  // staged in 64-column SWIZZLE_128B blocks).  256 exists for a K-major A only: with an MN-major A (the weight
+  // gradients dW = G^T X, split-K clusters) it never costs less than 128 and was measured 20-60 % slower on ties.
+  const auto width_ok = [&](int bn) {
+    return bn == 64 || bn == 128 || (bn == 152 && !p.tb) || (bn == 256 && !p.ta);
+  };
+  int bestBN = 0;
+  long bestCost = 0;
+  for (const int bn : {64, 128, 152, 256}) {
+    if (!width_ok(bn)) continue;
     const long tiles = (long)mt * ceil_div(p.N, bn) * splits_hint;
-    const long waves = ceil_div(tiles, nb == 1 ? 2L * kNumSMs : (long)kNumSMs);   // narrow tiles: two CTAs per SM
-    const long cost = waves * (BM + nb * 64L);
-    if (bestCost < 0 || cost < bestCost) { bestCost = cost; bestBN = bn; }
+    const long cost = bn != 64 ? ceil_div(tiles, (long)kNumSMs) * bn : tiles <= kNumSMs ? 64 : ceil_div(tiles, 2L * kNumSMs) * 160;
+    if (!bestBN || cost <= bestCost) { bestCost = cost; bestBN = bn; }
   }
-  if (g_tma_force_bn == 64 || g_tma_force_bn == 128 || g_tma_force_bn == 256) bestBN = g_tma_force_bn;
+  if (g_tma_force_bn) {
+    if (!width_ok(g_tma_force_bn)) return GPS_ERR_UNSUPPORTED;
+    bestBN = g_tma_force_bn;
+  }
   TmaArgs a;
   a.p = p;
   a.BN = bestBN;
   a.nb_blocks = a.BN / 64;
   a.planes = planes;
   const bool narrow = a.nb_blocks == 1;
-  const int stage_bytes = planes * (kATile + a.nb_blocks * kBlock);
+  const int stage_bytes = planes * (kATile + (p.tb ? a.nb_blocks * kBlock : a.BN * 128));
   const int fixed = 1024 /*align*/ + 1024 /*barriers*/ + 16 * 16 * 8 * 4 + 128 * 4;
   int stages = ((narrow ? 112 : 226) * 1024 - fixed) / stage_bytes;
   if (stages > 8) stages = 8;
-  if (stages < 2) return GPS_ERR_UNSUPPORTED;   // (two stages also hold the epilogue's fp32 staging tile)
+  if (stages < 2) return GPS_ERR_UNSUPPORTED;
+  // the operand stages also hold the epilogue's fp32 staging tile [BM][BN + 4]
+  GPS_REQUIRE((size_t)stages * stage_bytes >= (size_t)BM * (a.BN + 4) * 4, GPS_ERR_ARG,
+              "gemm_tma: BN %d: the staging tile does not fit the operand stages", a.BN);
   a.stages = stages;
   int splitk = p.splitk > 1 ? p.splitk : 1;
   if (splitk > kMaxSplits) splitk = kMaxSplits;
@@ -652,15 +675,19 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream) {
   const size_t smem = (size_t)stages * stage_bytes + fixed;
   dim3 grid((unsigned)ceil_div(p.N, a.BN), (unsigned)mt, (unsigned)splitk);
 #define GPS_TMA_CASE(AM, BMN)                                                                              \
-  if (amn == AM && bmn == BMN)                                                                             \
-    return a.BN == 64 ? launch<AM, BMN, 64>(tA, tB, a, grid, smem, stream)                                 \
-           : a.BN == 128 ? launch<AM, BMN, 128>(tA, tB, a, grid, smem, stream)                             \
-                         : launch<AM, BMN, 256>(tA, tB, a, grid, smem, stream);
+  if (amn == AM && bmn == BMN) {                                                                           \
+    if (a.BN == 64) return launch<AM, BMN, 64>(tA, tB, a, grid, smem, stream);                            \
+    if (a.BN == 128) return launch<AM, BMN, 128>(tA, tB, a, grid, smem, stream);                          \
+  }
   GPS_TMA_CASE(false, false)
   GPS_TMA_CASE(false, true)
   GPS_TMA_CASE(true, false)
   GPS_TMA_CASE(true, true)
 #undef GPS_TMA_CASE
+  if (a.BN == 152 && !bmn)
+    return amn ? launch<true, false, 152>(tA, tB, a, grid, smem, stream) : launch<false, false, 152>(tA, tB, a, grid, smem, stream);
+  if (a.BN == 256 && !amn)
+    return bmn ? launch<false, true, 256>(tA, tB, a, grid, smem, stream) : launch<false, false, 256>(tA, tB, a, grid, smem, stream);
   return GPS_ERR_UNSUPPORTED;
 }
 

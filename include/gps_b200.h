@@ -53,7 +53,9 @@ const char* gps_build_arch(void);
 unsigned long long gps_launch_count(void);
 /* tuning hook of the register-staged wgmma GEMM (tools/gemm_tune.py): bits 8.. = forced tile width. 0 = normal. */
 void gps_debug_set(int v);
-/* bring-up hook of the TMA-fed GEMM (tools/gemm_trace.py): force_bn = forced tile width (0 = heuristic); trace = device
+/* bring-up hook of the TMA-fed GEMM (tools/gemm_trace.py): force_bn = forced tile width (0 = the launch policy; 64, 128,
+ * 152 for a K-major B, 256 for a K-major A; a width the operand layout cannot take makes the product fail with
+ * GPS_ERR_UNSUPPORTED); trace = device
  * buffer of 256 x 16 uint64 that the first 256 CTAs of each launch fill with globaltimer phase stamps (NULL = off) */
 void gps_debug_tma(int force_bn, void* trace);
 /* bring-up hook of the wgmma attention: device buffer of 3 x 128 x 128 floats that CTA (0,0) fills with its first

@@ -7,6 +7,7 @@ from graphgps_b200.graph import graph_of
 from torch.profiler import profile, ProfilerActivity
 
 wl = sys.argv[1] if len(sys.argv) > 1 else "pcqm4m-small"
+precision = sys.argv[2] if len(sys.argv) > 2 else "fp32"
 local, glob, heads, drop, adrop = {"pcqm4m-small": ("CustomGatedGCN", "Transformer", 4, 0.0, 0.5),
                                    "pcqm4m-medium-performer": ("CustomGatedGCN", "Performer", 16, 0.1, 0.1),
                                    "zinc-gine": ("GINE", "Transformer", 4, 0.0, 0.5),
@@ -14,7 +15,8 @@ local, glob, heads, drop, adrop = {"pcqm4m-small": ("CustomGatedGCN", "Transform
 spec = graphgps_b200.SHAPES[wl]
 dev = "cuda:0"
 torch.manual_seed(0)
-layer = graphgps_b200.GPSLayer(spec.dim, local, glob, heads, dropout=drop, attn_dropout=adrop).to(dev).train()
+layer = graphgps_b200.GPSLayer(spec.dim, local, glob, heads, dropout=drop, attn_dropout=adrop,
+                              precision=precision).to(dev).train()
 b = graphgps_b200.make_batch(wl, seed=0).to(dev)
 graph_of(b)
 ct_x, ct_e = torch.randn_like(b.x), torch.randn_like(b.edge_attr)
@@ -44,7 +46,7 @@ for e in prof.key_averages():
         rows.append((e.device_time_total / 10.0, e.count / 10.0, e.key))
 rows.sort(reverse=True)
 tot = sum(r[0] for r in rows)
-print(f"{wl}: sum of kernel time per step = {tot:.1f} us")
+print(f"{wl} {precision}: sum of kernel time per step = {tot:.1f} us")
 for t, c, k in rows[:28]:
     k = k.replace("gps::(anonymous namespace)::", "").replace("void ", "")
     print(f"{t:9.1f} us {100*t/tot:5.1f}%  n={c:4.1f}  avg={t/c:7.1f}  {k[:90]}")
