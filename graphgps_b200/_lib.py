@@ -69,6 +69,8 @@ class GpsLayerArgs(C.Structure):
         ("x_planes_in", GpsPlanes), ("e_planes_in", GpsPlanes), ("x_planes_out", GpsPlanes), ("e_planes_out", GpsPlanes),
         ("wplanes", _fp), ("wplanes_bytes", C.c_int64), ("wplanes_valid", C.c_int32), ("reserved2", C.c_int32),
         ("ev_grads_mid", _fp), ("ev_grads_done", _fp),
+        # appended extension: EquivStableLapPE edge gate (equivstable_pe=True)
+        ("pe", _fp), ("pe_dim", C.c_int64), ("grad_pe", _fp), ("pe_mlp0", GpsLinear), ("pe_mlp1", GpsLinear),
     ]
 
 

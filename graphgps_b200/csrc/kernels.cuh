@@ -69,18 +69,31 @@ int colsum(const float* a, int64_t lda, int64_t rows, int64_t d, float* out, cud
 int copy2d(const float* src, int64_t lds, float* dst, int64_t ldd, int64_t rows, int64_t d, cudaStream_t stream);
 
 // ---- sparse (message passing) stages -------------------------------------------------------
+// rho (optional, [E]): EquivStableLapPE edge gate, sigma_ij = sigmoid(e_ij) * rho_e (eslap.cu)
 int gatedgcn_fwd(const GpsGraph& g, int64_t d, const float* Ax, const float* Bx, const float* Dx,
                  const float* Ex, int64_t ldy, float* Ce, float* xt, double* stats_x, double* stats_e,
-                 cudaStream_t stream);
+                 cudaStream_t stream, const float* rho = nullptr);
 // dst-ordered backward pass: reads g_xt (ld ldg), ehat, Bx; g_e holds the BN_e-path gradient on entry
-// and the total gradient w.r.t. e_ij on exit; writes g_num [N,d] and g_Dx (ld ldg).
+// and the total gradient w.r.t. e_ij on exit; writes g_num [N,d] and g_Dx (ld ldg).  With rho: also g_den [N,d].
 int gatedgcn_bwd_dst(const GpsGraph& g, int64_t d, const float* g_xt, int64_t ldg, const float* ehat,
                      const float* Bx, int64_t ldy, float* g_e, float* g_num, float* g_Dx,
-                     cudaStream_t stream, Planes g_e_p = Planes(), Planes g_Dx_p = Planes());
+                     cudaStream_t stream, Planes g_e_p = Planes(), Planes g_Dx_p = Planes(), const float* rho = nullptr,
+                     float* g_den = nullptr);
 // src-ordered backward pass: g_Ex_j = sum g_e_k, g_Bx_j = sum g_num[dst(k)] * sigmoid(ehat_k)
 int gatedgcn_bwd_src(const GpsGraph& g, int64_t d, const float* g_e, const float* ehat, const float* g_num,
                      float* g_Ex, float* g_Bx, int64_t ldg, cudaStream_t stream, Planes g_Ex_p = Planes(),
-                     Planes g_Bx_p = Planes());
+                     Planes g_Bx_p = Planes(), const float* rho = nullptr);
+
+// EquivStableLapPE edge gate (eslap.cu): PE [N,k] row-major; w1 = mlp_r_ij.0.weight [d,1], b1 [d], w2 = mlp_r_ij.2.weight
+// [1,d], b2 [1].  Forward: r [E], rho [E].  Backward (after gatedgcn_bwd_dst with rho): per-edge scratch gz, gr [E] and
+// part [ceil(E / eslap_wgrad_chunk(E)), 3d+1]; writes (or, accumulate, adds) the four mlp_r_ij gradients and writes grad_pe.
+int64_t eslap_wgrad_chunk(int64_t E);
+int eslap_fwd(const GpsGraph& g, const float* pe, int64_t k, int64_t d, int act, const float* w1, const float* b1,
+              const float* w2, const float* b2, float* r, float* rho, cudaStream_t stream);
+int eslap_bwd(const GpsGraph& g, const float* pe, int64_t k, int64_t d, int act, const float* g_num, const float* g_den,
+              const float* Bx, int64_t ldy, const float* ehat, const float* r, const float* rho, const float* w1,
+              const float* b1, const float* w2, float* gz, float* gr, float* part, float* grad_pe, float* gw1,
+              float* gb1, float* gw2, float* gb2, bool accumulate, cudaStream_t stream);
 int gine_fwd(const GpsGraph& g, int64_t d, const float* x, const float* e, float eps, float* out,
              cudaStream_t stream, Planes outp = Planes());
 // g_e[k] = g_o[dst(k)] * [x_src + e_k > 0];  (dst ordered)

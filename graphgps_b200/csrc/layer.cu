@@ -197,6 +197,9 @@ struct Plan {
   float *Wcat, *bcat, *Y1, *ehat, *xt, *xloc, *O, *lse, *hA, *s, *hid, *hid_pre, *t, *bnbuf;
   float *agg, *h1, *h1_pre;
   float* dinv;   // GCN: deg^-1/2 per node
+  // EquivStableLapPE edge gate (eslap.cu): saved r_e, rho_e; backward g_den [N,d], g_z / g_r [E], column-sum parts
+  bool eslap;
+  float *pe_r, *pe_rho, *g_den, *pe_gz, *pe_gr, *pe_part;
   // bf16 hi/lo operand planes of the TMA-fed GEMM (gemm_tma.cu).  Saved: layer inputs, weights and the forward
   // activations the weight gradients re-read; workspace: the backward gradients that feed GEMMs.
   bool use_planes;
@@ -244,6 +247,9 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   P->gcn = a->local_type == GPS_LOCAL_GCN;
   GPS_REQUIRE(a->local_type == GPS_LOCAL_NONE || P->gated || P->gine || P->gcn, GPS_ERR_ARG, "unknown local_type %d",
               a->local_type);
+  P->eslap = a->pe != nullptr;
+  GPS_REQUIRE(!P->eslap || P->gated, GPS_ERR_ARG, "pe (EquivStableLapPE) is read by the GatedGCN local model only");
+  GPS_REQUIRE(!P->eslap || a->pe_dim >= 1, GPS_ERR_ARG, "pe_dim must be >= 1 (got %lld)", (long long)a->pe_dim);
   GPS_REQUIRE(a->global_type == GPS_GLOBAL_NONE || a->global_type == GPS_GLOBAL_TRANSFORMER ||
                   a->global_type == GPS_GLOBAL_PERFORMER,
               GPS_ERR_ARG, "unknown global_type %d", a->global_type);
@@ -281,6 +287,10 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   if (P->gated) {
     P->ehat = S.alloc<float>(E * d);
     P->xt = S.alloc<float>(N * d);
+    if (P->eslap) {
+      P->pe_r = S.alloc<float>(E);
+      P->pe_rho = S.alloc<float>(E);
+    }
   }
   if (P->gine) {
     P->agg = S.alloc<float>(N * d);
@@ -421,6 +431,12 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   if (P->gated) {
     P->g_e = Bk.alloc<float>(E * d);
     P->g_num = Bk.alloc<float>(N * d);
+    if (P->eslap) {
+      P->g_den = Bk.alloc<float>(N * d);
+      P->pe_gz = Bk.alloc<float>(E);
+      P->pe_gr = Bk.alloc<float>(E);
+      P->pe_part = Bk.alloc<float>(ceil_div(E, eslap_wgrad_chunk(E)) * (3 * d + 1));
+    }
   }
   if (P->gine) {
     P->g_h1 = Bk.alloc<float>(N * d);
@@ -519,6 +535,10 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
     GPS_TRY(check_linear(a->gcn_E, "local_model.E", true));
     GPS_TRY(check_bn(a->bn_node_x, "local_model.bn_node_x"));
     GPS_TRY(check_bn(a->bn_edge_e, "local_model.bn_edge_e"));
+    if (P.eslap) {
+      GPS_TRY(check_linear(a->pe_mlp0, "local_model.mlp_r_ij.0", true));
+      GPS_TRY(check_linear(a->pe_mlp1, "local_model.mlp_r_ij.2", true));
+    }
   }
   if (P.gine) {
     GPS_TRY(check_linear(a->gine_lin0, "local_model.nn.0", true));
@@ -684,6 +704,10 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     g.bias = a->gcn_C.bias; g.precision = a->precision;
     g.Ap = P.e_p; g.Bp = P.C_p;
     GPS_TRY(gemm(g, s2));
+    // EquivStableLapPE gate r_e, rho_e: reads PE, the graph and mlp_r_ij only (gatedgcn_layer.py:101-104)
+    if (P.eslap)
+      GPS_TRY(eslap_fwd(a->graph, a->pe, a->pe_dim, d, act, a->pe_mlp0.weight, a->pe_mlp0.bias, a->pe_mlp1.weight,
+                        a->pe_mlp1.bias, P.pe_r, P.pe_rho, s2));
   }
 
   // ---- node projections: [Ax|Bx|Dx|Ex|Q|K|V] = x Wcat^T + bcat  (gatedgcn_layer.py:57-61, MHA in_proj)
@@ -724,7 +748,7 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
   // ---- local model
   if (P.gated) {
     GPS_TRY(gatedgcn_fwd(a->graph, d, P.Y1, P.Y1 + d, P.Y1 + 2 * d, P.Y1 + 3 * d, P.Wy, P.ehat, P.xt,
-                         stats(BN_X), stats(BN_E), st));
+                         stats(BN_X), stats(BN_E), st, P.pe_rho));
     // x_loc = x + drop(act(BN(x~)));  e_out = e + drop(act(BN(e^)))   (gatedgcn_layer.py:72-83)
     GPS_TRY(bn_act_residual2(P.xt, a->x, P.xloc, N, bn_view_fwd(P, a, BN_X, a->bn_node_x, N), drop(GPS_SITE_GCN_X), stats(BN_L),
                              P.ehat, a->edge_attr, a->edge_out, E, bn_view_fwd(P, a, BN_E, a->bn_edge_e, E),
@@ -1096,12 +1120,23 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     if (se != st) GPS_TRY(sd->order(se, st));
     // message/aggregate backward (SURVEY Appendix C)
     GPS_TRY(gatedgcn_bwd_dst(a->graph, d, P.gY1, P.Wy, P.ehat, P.Y1 + d, P.Wy, P.g_e, P.g_num, P.gY1 + 2 * d, st, P.ge_p,
-                             P.gY1_p.cols(2 * d)));
+                             P.gY1_p.cols(2 * d), P.pe_rho, P.g_den));
+    // EquivStableLapPE gate: mlp_r_ij gradients (mid group) and grad_pe need g_num / g_den only, so they run on the
+    // (by now idle) edge-BatchNorm stream next to the src-ordered pass and the weight gradients
+    cudaStream_t sp = (P.eslap && se != st) ? se : st;
+    if (P.eslap) {
+      if (sp != st) GPS_TRY(sd->order(st, sp));
+      GPS_TRY(eslap_bwd(a->graph, a->pe, a->pe_dim, d, act, P.g_num, P.g_den, P.Y1 + d, P.Wy, P.ehat, P.pe_r, P.pe_rho,
+                        a->pe_mlp0.weight, a->pe_mlp0.bias, a->pe_mlp1.weight, P.pe_gz, P.pe_gr, P.pe_part, a->grad_pe,
+                        a->pe_mlp0.grad_weight, a->pe_mlp0.grad_bias, a->pe_mlp1.grad_weight, a->pe_mlp1.grad_bias,
+                        g_grads_accumulate, sp));
+    }
     GPS_TRY(gatedgcn_bwd_src(a->graph, d, P.g_e, P.ehat, P.g_num, P.gY1 + 3 * d, P.gY1 + d, P.Wy, st, P.gY1_p.cols(3 * d),
-                             P.gY1_p.cols(d)));
+                             P.gY1_p.cols(d), P.pe_rho));
     // C: dC = g_e^T e ; g_edge_attr = grad_edge_out + g_e C
     GPS_TRY(wfork(st));
     GPS_TRY(linear_wgrad(P.g_e, d, a->edge_attr, d, E, d, d, a->gcn_C.grad_weight, a->gcn_C.grad_bias, prec, s2, P.ge_p, P.e_p));
+    if (sp != st) GPS_TRY(sd->order(sp, s2));   // the mlp_r_ij gradients are final at ev_grads_mid; grad_pe joins at the end
     GPS_TRY(mid_done());
     if (a->grad_edge_attr && E > 0) {
       GemmParams g;

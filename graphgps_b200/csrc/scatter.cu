@@ -75,11 +75,12 @@ __device__ __forceinline__ void block_stats(float4* acc, double* const* ptrs, fl
   }
 }
 
-template <bool STATS>
+// PE: EquivStableLapPE gate, sigma_ij = sigmoid(e_ij) * rho_e (gatedgcn_layer.py:101-104; rho from eslap.cu)
+template <bool STATS, bool PE>
 __global__ void __launch_bounds__(1024) k_gatedgcn_fwd(GpsGraph g, int d, const float* __restrict__ Ax, const float* __restrict__ Bx,
                                const float* __restrict__ Dx, const float* __restrict__ Ex, int64_t ldy,
                                float* __restrict__ Ce, float* __restrict__ xt, double* stats_x,
-                               double* stats_e) {
+                               double* stats_e, const float* __restrict__ rho) {
   extern __shared__ float4 sm[];
   const int c = threadIdx.x * 4, ry = threadIdx.y, RY = blockDim.y;
   float4 acc[4] = {f4zero(), f4zero(), f4zero(), f4zero()};  // sum x~, sum x~^2, sum e, sum e^2
@@ -98,7 +99,7 @@ __global__ void __launch_bounds__(1024) k_gatedgcn_fwd(GpsGraph g, int d, const 
       float4 c1 = ld4(Ce + e1 * d + c);
       c0 = f4add(c0, f4add(dx, ex0));
       st4(Ce + e0 * d + c, c0);
-      const float4 s0 = sigmoid4(c0);
+      const float4 s0 = PE ? f4scale(sigmoid4(c0), rho[e0]) : sigmoid4(c0);
       num = f4fma(s0, bx0, num);
       den = f4add(den, s0);
       if (STATS) {
@@ -108,7 +109,7 @@ __global__ void __launch_bounds__(1024) k_gatedgcn_fwd(GpsGraph g, int d, const 
       if (two) {
         c1 = f4add(c1, f4add(dx, ex1));
         st4(Ce + e1 * d + c, c1);
-        const float4 s1 = sigmoid4(c1);
+        const float4 s1 = PE ? f4scale(sigmoid4(c1), rho[e1]) : sigmoid4(c1);
         num = f4fma(s1, bx1, num);
         den = f4add(den, s1);
         if (STATS) {
@@ -132,10 +133,13 @@ __global__ void __launch_bounds__(1024) k_gatedgcn_fwd(GpsGraph g, int d, const 
   }
 }
 
+// PE: the gate is sigmoid(e_ij) * rho_e; also stores g_den = d/d den [N,d] for the gradient of rho (eslap.cu)
+template <bool PE>
 __global__ void k_gatedgcn_bwd_dst(GpsGraph g, int d, const float* __restrict__ g_xt, int64_t ldg,
                                    const float* __restrict__ ehat, const float* __restrict__ Bx, int64_t ldy,
                                    float* __restrict__ g_e, float* __restrict__ g_num,
-                                   float* __restrict__ g_Dx, Planes g_e_p, Planes g_Dx_p) {
+                                   float* __restrict__ g_Dx, Planes g_e_p, Planes g_Dx_p,
+                                   const float* __restrict__ rho, float* __restrict__ g_den) {
   const int c = threadIdx.x * 4, ry = threadIdx.y, RY = blockDim.y;
   for (int64_t i = (int64_t)blockIdx.x * RY + ry; i < g.N; i += (int64_t)gridDim.x * RY) {
     const int kb = g.dst_ptr[i], ke = g.dst_ptr[i + 1];
@@ -143,7 +147,7 @@ __global__ void k_gatedgcn_bwd_dst(GpsGraph g, int d, const float* __restrict__ 
     for (int k = kb; k < ke; ++k) {
       const int j = g.dst_src[k];
       const int64_t eid = g.dst_eid[k];
-      const float4 s = sigmoid4(ld4(ehat + eid * d + c));
+      const float4 s = PE ? f4scale(sigmoid4(ld4(ehat + eid * d + c)), rho[eid]) : sigmoid4(ld4(ehat + eid * d + c));
       num = f4fma(s, ld4(Bx + (int64_t)j * ldy + c), num);
       den = f4add(den, s);
     }
@@ -154,13 +158,14 @@ __global__ void k_gatedgcn_bwd_dst(GpsGraph g, int d, const float* __restrict__ 
     const float4 gn = f4mul(gx, inv);                       // d/d num
     const float4 gd = make_float4(-gn.x * agg.x, -gn.y * agg.y, -gn.z * agg.z, -gn.w * agg.w);  // d/d den
     st4(g_num + i * d + c, gn);
+    if (PE) st4(g_den + i * d + c, gd);
     float4 gdx = f4zero();
     for (int k = kb; k < ke; ++k) {
       const int j = g.dst_src[k];
       const int64_t eid = g.dst_eid[k];
       const float4 s = sigmoid4(ld4(ehat + eid * d + c));
       const float4 bx = ld4(Bx + (int64_t)j * ldy + c);
-      const float4 gs = f4fma(gn, bx, gd);                  // d/d sigma
+      const float4 gs = PE ? f4scale(f4fma(gn, bx, gd), rho[eid]) : f4fma(gn, bx, gd);   // d/d sigmoid(e_ij)
       float4 ge = ld4(g_e + eid * d + c);
       ge.x += gs.x * s.x * (1.f - s.x);
       ge.y += gs.y * s.y * (1.f - s.y);
@@ -175,10 +180,11 @@ __global__ void k_gatedgcn_bwd_dst(GpsGraph g, int d, const float* __restrict__ 
   }
 }
 
+template <bool PE>
 __global__ void k_gatedgcn_bwd_src(GpsGraph g, int d, const float* __restrict__ g_e,
                                    const float* __restrict__ ehat, const float* __restrict__ g_num,
                                    float* __restrict__ g_Ex, float* __restrict__ g_Bx, int64_t ldg, Planes g_Ex_p,
-                                   Planes g_Bx_p) {
+                                   Planes g_Bx_p, const float* __restrict__ rho) {
   const int c = threadIdx.x * 4, ry = threadIdx.y, RY = blockDim.y;
   for (int64_t j = (int64_t)blockIdx.x * RY + ry; j < g.N; j += (int64_t)gridDim.x * RY) {
     float4 gex = f4zero(), gbx = f4zero();
@@ -187,7 +193,7 @@ __global__ void k_gatedgcn_bwd_src(GpsGraph g, int d, const float* __restrict__ 
       const int i = g.src_dst[k];
       const int64_t eid = g.src_eid[k];
       gex = f4add(gex, ld4(g_e + eid * d + c));
-      const float4 s = sigmoid4(ld4(ehat + eid * d + c));
+      const float4 s = PE ? f4scale(sigmoid4(ld4(ehat + eid * d + c)), rho[eid]) : sigmoid4(ld4(ehat + eid * d + c));
       gbx = f4fma(ld4(g_num + (int64_t)i * d + c), s, gbx);
     }
     st4(g_Ex + j * ldg + c, gex);
@@ -338,36 +344,56 @@ int gcn_bwd(const GpsGraph& g, int64_t d, const float* g_h, const float* dinv, f
 }
 
 int gatedgcn_fwd(const GpsGraph& g, int64_t d, const float* Ax, const float* Bx, const float* Dx, const float* Ex,
-                 int64_t ldy, float* Ce, float* xt, double* stats_x, double* stats_e, cudaStream_t stream) {
+                 int64_t ldy, float* Ce, float* xt, double* stats_x, double* stats_e, cudaStream_t stream,
+                 const float* rho) {
   if (g.N == 0) return GPS_OK;
   NodeGeom ng;
   const bool stats = stats_x || stats_e;
   GPS_TRY(node_geom(g.N, d, stats ? 4 : 0, &ng));
-  if (stats)
-    k_gatedgcn_fwd<true><<<ng.grid, ng.block, ng.smem, stream>>>(g, (int)d, Ax, Bx, Dx, Ex, ldy, Ce, xt, stats_x,
-                                                                   stats_e);
+  if (stats && rho)
+    k_gatedgcn_fwd<true, true><<<ng.grid, ng.block, ng.smem, stream>>>(g, (int)d, Ax, Bx, Dx, Ex, ldy, Ce, xt, stats_x,
+                                                                         stats_e, rho);
+  else if (rho)
+    k_gatedgcn_fwd<false, true><<<ng.grid, ng.block, 0, stream>>>(g, (int)d, Ax, Bx, Dx, Ex, ldy, Ce, xt, nullptr, nullptr,
+                                                                  rho);
+  else if (stats)
+    k_gatedgcn_fwd<true, false><<<ng.grid, ng.block, ng.smem, stream>>>(g, (int)d, Ax, Bx, Dx, Ex, ldy, Ce, xt, stats_x,
+                                                                          stats_e, nullptr);
   else
-    k_gatedgcn_fwd<false><<<ng.grid, ng.block, 0, stream>>>(g, (int)d, Ax, Bx, Dx, Ex, ldy, Ce, xt, nullptr, nullptr);
+    k_gatedgcn_fwd<false, false><<<ng.grid, ng.block, 0, stream>>>(g, (int)d, Ax, Bx, Dx, Ex, ldy, Ce, xt, nullptr, nullptr,
+                                                                   nullptr);
   GPS_LAUNCH_CHECK();
   return GPS_OK;
 }
 
 int gatedgcn_bwd_dst(const GpsGraph& g, int64_t d, const float* g_xt, int64_t ldg, const float* ehat, const float* Bx,
-                     int64_t ldy, float* g_e, float* g_num, float* g_Dx, cudaStream_t stream, Planes g_e_p, Planes g_Dx_p) {
+                     int64_t ldy, float* g_e, float* g_num, float* g_Dx, cudaStream_t stream, Planes g_e_p, Planes g_Dx_p,
+                     const float* rho, float* g_den) {
   if (g.N == 0) return GPS_OK;
   NodeGeom ng;
   GPS_TRY(node_geom(g.N, d, 0, &ng));
-  k_gatedgcn_bwd_dst<<<ng.grid, ng.block, 0, stream>>>(g, (int)d, g_xt, ldg, ehat, Bx, ldy, g_e, g_num, g_Dx, g_e_p, g_Dx_p);
+  if (rho)
+    k_gatedgcn_bwd_dst<true><<<ng.grid, ng.block, 0, stream>>>(g, (int)d, g_xt, ldg, ehat, Bx, ldy, g_e, g_num, g_Dx, g_e_p,
+                                                               g_Dx_p, rho, g_den);
+  else
+    k_gatedgcn_bwd_dst<false><<<ng.grid, ng.block, 0, stream>>>(g, (int)d, g_xt, ldg, ehat, Bx, ldy, g_e, g_num, g_Dx, g_e_p,
+                                                                g_Dx_p, nullptr, nullptr);
   GPS_LAUNCH_CHECK();
   return GPS_OK;
 }
 
 int gatedgcn_bwd_src(const GpsGraph& g, int64_t d, const float* g_e, const float* ehat, const float* g_num,
-                     float* g_Ex, float* g_Bx, int64_t ldg, cudaStream_t stream, Planes g_Ex_p, Planes g_Bx_p) {
+                     float* g_Ex, float* g_Bx, int64_t ldg, cudaStream_t stream, Planes g_Ex_p, Planes g_Bx_p,
+                     const float* rho) {
   if (g.N == 0) return GPS_OK;
   NodeGeom ng;
   GPS_TRY(node_geom(g.N, d, 0, &ng));
-  k_gatedgcn_bwd_src<<<ng.grid, ng.block, 0, stream>>>(g, (int)d, g_e, ehat, g_num, g_Ex, g_Bx, ldg, g_Ex_p, g_Bx_p);
+  if (rho)
+    k_gatedgcn_bwd_src<true><<<ng.grid, ng.block, 0, stream>>>(g, (int)d, g_e, ehat, g_num, g_Ex, g_Bx, ldg, g_Ex_p, g_Bx_p,
+                                                               rho);
+  else
+    k_gatedgcn_bwd_src<false><<<ng.grid, ng.block, 0, stream>>>(g, (int)d, g_e, ehat, g_num, g_Ex, g_Bx, ldg, g_Ex_p,
+                                                                g_Bx_p, nullptr);
   GPS_LAUNCH_CHECK();
   return GPS_OK;
 }

@@ -85,13 +85,15 @@ def _batch_planes_put(batch, produced, lo):
 class _GatedGCNParams(nn.Module):
     """Parameter container with the names of graphgps/layer/gatedgcn_layer.py:21-38."""
 
-    def __init__(self, dim):
+    def __init__(self, dim, act="relu", equivstable_pe=False):
         super().__init__()
         self.A = nn.Linear(dim, dim, bias=True)
         self.B = nn.Linear(dim, dim, bias=True)
         self.C = nn.Linear(dim, dim, bias=True)
         self.D = nn.Linear(dim, dim, bias=True)
         self.E = nn.Linear(dim, dim, bias=True)
+        if equivstable_pe:   # EquivStableLapPE edge gate, gatedgcn_layer.py:29-35
+            self.mlp_r_ij = nn.Sequential(nn.Linear(1, dim), _ACT_MODULES[act](), nn.Linear(dim, 1), nn.Sigmoid())
         self.bn_node_x = nn.BatchNorm1d(dim)
         self.bn_edge_e = nn.BatchNorm1d(dim)
 
@@ -167,11 +169,14 @@ class _GPSLayerFn(torch.autograd.Function):
     """One autograd node for the whole layer: forward = gps_layer_forward, backward = gps_layer_backward."""
 
     @staticmethod
-    def forward(ctx, layer, gs, x, e, *params):
+    def forward(ctx, layer, gs, x, e, pe, *params):
         lib = _lib.load()
         dev = x.device
         named = dict(zip(layer._param_names, params))
-        args = layer._base_args(gs, named)
+        pe_k = pe.shape[1] if layer._eslap else 0
+        args = layer._base_args(gs, named, pe_k=pe_k)
+        if pe_k:
+            args.pe = pe.data_ptr()
         N, E, d = gs.N, gs.E, layer.dim_h
         x_out = torch.empty_like(x)
         e_out = torch.empty_like(e) if layer.local_gnn_type == "CustomGatedGCN" else None
@@ -192,7 +197,7 @@ class _GPSLayerFn(torch.autograd.Function):
         ctx.layer, ctx.gs, ctx.saved_buf, ctx.snap = layer, gs, saved, snap
         ctx.hand = hand
         ctx.seed, ctx.offset, ctx.training = args.seed, args.offset, bool(args.training)
-        ctx.save_for_backward(x, e, *params)
+        ctx.save_for_backward(x, e, pe, *params)
         if e_out is not None:
             return x_out, e_out
         return x_out
@@ -201,22 +206,29 @@ class _GPSLayerFn(torch.autograd.Function):
     def backward(ctx, g_x_out, g_e_out=None):
         lib = _lib.load()
         layer, gs = ctx.layer, ctx.gs
-        x, e, *params = ctx.saved_tensors
+        x, e, pe, *params = ctx.saved_tensors
         dev = x.device
         named = dict(zip(layer._param_names, params))
+        pe_k = pe.shape[1] if layer._eslap else 0
         bucket = layer._bucket_grads(named)
         if bucket is not None:
             # static gradient bucket (graphgps_b200.dp.GradBucket): the library ADDS this call's gradients to the
             # parameters' .grad views in place (torch's accumulation semantics), so CUDA-graph replays and the
             # gradient all-reduce see the same memory
             grads = bucket
-            args = layer._base_args(gs, named, grads)
+            args = layer._base_args(gs, named, grads, pe_k=pe_k)
             args.reserved0 = 3
         else:
             grads = {n: torch.empty_like(p) for n, p in named.items()}
             torch._foreach_zero_(list(grads.values()))   # one multi-tensor fill; the library then skips its memsets
-            args = layer._base_args(gs, named, grads)
+            args = layer._base_args(gs, named, grads, pe_k=pe_k)
             args.reserved0 = 1
+        g_pe = None
+        if pe_k:
+            args.pe = pe.data_ptr()
+            if ctx.needs_input_grad[4]:
+                g_pe = torch.empty_like(pe)
+                args.grad_pe = g_pe.data_ptr()
         args.seed, args.offset, args.training = ctx.seed, ctx.offset, 1 if ctx.training else 0
         if ctx.snap is not None:
             args.offset_dev = ctx.snap.data_ptr()
@@ -244,7 +256,7 @@ class _GPSLayerFn(torch.autograd.Function):
         _lib.check(lib.gps_layer_backward(C.byref(args), stream), "gps_layer_backward")
         # (ctx.saved_buf stays alive with the autograd node: backward(retain_graph=True) may run again)
         if bucket is not None:
-            return (None, None, g_x, g_e) + (None,) * len(layer._param_names)
+            return (None, None, g_x, g_e, g_pe) + (None,) * len(layer._param_names)
         # parameters the configuration never reads get no gradient (as under autograd in the reference)
         unused = []
         if layer.local_gnn_type == "None":
@@ -252,7 +264,7 @@ class _GPSLayerFn(torch.autograd.Function):
         if layer.global_model_type == "None":
             unused.append("norm1_attn.")
         pg = tuple(None if any(n.startswith(u) for u in unused) else grads[n] for n in layer._param_names)
-        return (None, None, g_x, g_e) + pg
+        return (None, None, g_x, g_e, g_pe) + pg
 
 
 class GPSLayer(nn.Module):
@@ -290,8 +302,13 @@ class GPSLayer(nn.Module):
         if local_gnn_type not in _SUPPORTED_LOCAL:
             raise NotImplementedError(f"local GNN '{local_gnn_type}' is not built in graphgps_b200 "
                                       f"(available: {_SUPPORTED_LOCAL}); there is no fallback path")
-        if equivstable_pe:
-            raise NotImplementedError("equivstable_pe is not built in graphgps_b200")
+        if equivstable_pe and local_gnn_type == "GINE":
+            raise NotImplementedError(
+                "GINE with equivstable_pe=True is not built in graphgps_b200: the reference itself fails to construct "
+                "it (GINEConvESLapPE.__init__ calls reset_parameters(), which reads self.mlp_r_ij before it is defined: "
+                "gine_conv_layer.py:35,44 raise AttributeError)")
+        # EquivStableLapPE gate: read by GatedGCN only; GCN and None ignore the flag (gps_layer.py:176-187)
+        self._eslap = bool(equivstable_pe) and local_gnn_type == "CustomGatedGCN"
         if local_gnn_type == "None":
             self.local_model = None
         elif local_gnn_type == "GINE":
@@ -300,7 +317,7 @@ class GPSLayer(nn.Module):
             self.local_gnn_with_edge_attr = False
             self.local_model = _GCNConvParams(dim_h)
         else:
-            self.local_model = _GatedGCNParams(dim_h)
+            self.local_model = _GatedGCNParams(dim_h, act, self._eslap)
         self.local_gnn_type = local_gnn_type
 
         # ---- global attention model (gps_layer.py:101-122)
@@ -403,8 +420,9 @@ class GPSLayer(nn.Module):
         return out
 
     def _plan(self, args, gs):
-        """(saved_bytes, workspace_bytes); gps_layer_plan is pure in (config, N, E, B, training, precision)."""
-        key = (gs.N, gs.E, gs.B, bool(self.training), self.precision, float(self.dropout), float(self.attn_dropout))
+        """(saved_bytes, workspace_bytes); gps_layer_plan is pure in (config, N, E, B, training, precision, PE width)."""
+        key = (gs.N, gs.E, gs.B, bool(self.training), self.precision, float(self.dropout), float(self.attn_dropout),
+               bool(args.pe), int(args.pe_dim))
         hit = self._plan_cache.get(key)
         if hit is None:
             plan = _lib.GpsLayerPlan()
@@ -417,7 +435,7 @@ class GPSLayer(nn.Module):
         return hit
 
     # ------------------------------------------------------------------------------------
-    def _base_args(self, gs, named, grads=None):
+    def _base_args(self, gs, named, grads=None, pe_k=0):
         """GpsLayerArgs with configuration, graph and parameter (+gradient) pointers filled in.
 
         The forward-direction struct (no gradient pointers) only depends on the parameter addresses and the
@@ -425,15 +443,15 @@ class GPSLayer(nn.Module):
         time than the GPU needs for the whole layer at the ZINC shape."""
         if grads is None:
             key = (tuple(t.data_ptr() for t in named.values()), self.training, self.precision,
-                   float(self.dropout), float(self.attn_dropout))
+                   float(self.dropout), float(self.attn_dropout), pe_k > 0, pe_k)
             cached = self.__dict__.get("_args_cache")
             if cached is None or cached[0] != key:
                 self._check_params(named)
-                cached = (key, self._build_args(named, None))
+                cached = (key, self._build_args(named, None, pe_k))
                 self.__dict__["_args_cache"] = cached
             a = _lib.GpsLayerArgs.from_buffer_copy(cached[1])
         else:
-            a = self._build_args(named, grads)
+            a = self._build_args(named, grads, pe_k)
         a.seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
         _dropout_calls[0] += 1
         a.offset = _dropout_calls[0] * 4096
@@ -448,7 +466,7 @@ class GPSLayer(nn.Module):
                 raise TypeError(f"graphgps_b200.GPSLayer: parameter/buffer '{n}' must be a contiguous float32 CUDA "
                                 f"tensor (got {t.dtype} on {t.device})")
 
-    def _build_args(self, named, grads):
+    def _build_args(self, named, grads, pe_k=0):
         g = grads or {}
         a = _lib.GpsLayerArgs()
         a.d, a.heads = self.dim_h, self.num_heads
@@ -474,6 +492,9 @@ class GPSLayer(nn.Module):
             a.gcn_D, a.gcn_E = lin("local_model.D"), lin("local_model.E")
             a.bn_node_x = bn("local_model.bn_node_x", self.local_model.bn_node_x)
             a.bn_edge_e = bn("local_model.bn_edge_e", self.local_model.bn_edge_e)
+            if self._eslap:   # the PE pointer itself is set per call
+                a.pe_dim = pe_k
+                a.pe_mlp0, a.pe_mlp1 = lin("local_model.mlp_r_ij.0"), lin("local_model.mlp_r_ij.2")
         elif self.local_gnn_type == "GINE":
             a.gine_lin0, a.gine_lin1 = lin("local_model.nn.0"), lin("local_model.nn.2")
             a.gine_eps = float(self._gine_eps_host)
@@ -522,11 +543,13 @@ class GPSLayer(nn.Module):
             e = e.contiguous()
         else:
             e = None
+        pe = self._read_pe(batch, x) if self._eslap else None
         gs = graph_of(batch)
         params = [p for _, p in self.named_parameters()]
         e_arg = e if e is not None else x.new_empty(0)
+        pe_arg = pe if pe is not None else x.new_empty(0)
         self.__dict__["_planes_in"] = _batch_planes_get(batch)
-        out = _GPSLayerFn.apply(self, gs, x, e_arg, *params)
+        out = _GPSLayerFn.apply(self, gs, x, e_arg, pe_arg, *params)
         produced = self.__dict__.pop("_planes_out", None)
         if self.local_gnn_type == "CustomGatedGCN":
             batch.x, batch.edge_attr = out           # gps_layer.py:173-174, :231
@@ -534,6 +557,21 @@ class GPSLayer(nn.Module):
             batch.x = out
         _batch_planes_put(batch, produced, self.precision == "fp32")
         return batch
+
+    @staticmethod
+    def _read_pe(batch, x):
+        """batch.pe_EquivStableLapPE [N, k] (gps_layer.py:165-166): float32, on the device of x, one row per node."""
+        pe = getattr(batch, "pe_EquivStableLapPE", None)
+        if pe is None:
+            raise AttributeError("GPSLayer(equivstable_pe=True) reads batch.pe_EquivStableLapPE [num_nodes, k], which "
+                                 "this batch does not have (posenc_EquivStableLapPE's node encoder writes it)")
+        if not torch.is_tensor(pe) or pe.dtype != torch.float32 or pe.device != x.device:
+            raise TypeError("batch.pe_EquivStableLapPE must be a float32 tensor on the device of batch.x (got "
+                            f"{getattr(pe, 'dtype', type(pe))} on {getattr(pe, 'device', None)})")
+        if pe.dim() != 2 or pe.shape[0] != x.shape[0] or pe.shape[1] < 1:
+            raise ValueError(f"batch.pe_EquivStableLapPE must have shape [num_nodes={x.shape[0]}, k >= 1] "
+                             f"(got {tuple(pe.shape)})")
+        return pe.contiguous()
 
     def extra_repr(self):
         return (f"summary: dim_h={self.dim_h}, local_gnn_type={self.local_gnn_type}, "

@@ -201,6 +201,16 @@ typedef struct {
    * of this layer is final. */
   void* ev_grads_mid;
   void* ev_grads_done;
+
+  /* ABI 3, appended extension (optional): the EquivStableLapPE edge gate of GatedGCN (equivstable_pe=True,
+   * gatedgcn_layer.py:29-35,101-104).  pe = batch.pe_EquivStableLapPE, row-major contiguous [N, pe_dim], pe_dim >= 1.
+   * For edge j->i: r = sum_c (pe_i - pe_j)^2, rho = mlp_r_ij(r) and the gate becomes sigmoid(e_ij) * rho.
+   * pe == NULL: no gate (the fields below are not read).  pe != NULL with a local_type other than GPS_LOCAL_GATEDGCN
+   * is GPS_ERR_ARG.  Backward writes grad_pe [N, pe_dim] (NULL = not needed) and the gradients of pe_mlp0 / pe_mlp1,
+   * which are final when ev_grads_mid fires. */
+  const float* pe; int64_t pe_dim;
+  float* grad_pe;
+  GpsLinear pe_mlp0 /* mlp_r_ij.0 [d,1] */, pe_mlp1 /* mlp_r_ij.2 [1,d] */;
 } GpsLayerArgs;
 
 typedef struct {
