@@ -20,7 +20,7 @@
 // 256 threads = two MMA / softmax warpgroups; thread 0 also issues the TMA loads.  The K and V tiles have their own
 // full / empty barriers, so the next K tile loads while the softmax and P V of the current one run.  (A separate
 // producer warp would make the CTA count as three warpgroups and cap the registers that S, O and P need.)
-// The CUDA-core kernel in attention.cu stays as the validator (GPS_B200_ATTN=simt) and for head dims above 128.
+// The CUDA-core kernel in attention.cu serves batches of small graphs (mean below 64 nodes) and head dims above 128.
 #include <cuda.h>
 #include <cuda_bf16.h>
 

@@ -6,7 +6,8 @@
 //   pack W -> [Ax|Bx|Dx|Ex|Q|K|V] = x Wcat^T -> Ce = e C^T -> segmented gather-reduce (+BN stats)
 //   -> x_loc = x + act(BN(x~)) (+stats), e_out = e + act(BN(e^)) -> attention -> hA = x + O Wo^T (+stats)
 //   -> s = BN(x_loc) + BN(hA) -> FFN (+stats) -> BN.
-// Training-mode BatchNorm is "producer accumulates column sums, tiny finalize, consumer normalises".
+// Training-mode BatchNorm: the producer accumulates column sums, and the consumer kernel finalises the statistics from
+// them and normalises (BnView mode 1), so no launch sits between the two.
 #include <stdarg.h>
 #include <string.h>
 
@@ -137,17 +138,16 @@ static int opt_flags() {
   return v;
 }
 
-static Side* side_stream() {
-  static const bool enabled = [] {
-    const char* e = getenv("GPS_B200_STREAMS");
-    return !(e && e[0] == '0');
-  }();
-  if (!enabled) return nullptr;
+// the side streams of the current device, created on its first use
+static int side_stream(Side** out) {
   static thread_local Side sides[64];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
-  if (sides[dev].init() != GPS_OK) return nullptr;
-  return &sides[dev];
+  GPS_CUDA(cudaGetDevice(&dev));
+  GPS_REQUIRE(dev >= 0 && dev < 64, GPS_ERR_ARG, "device index %d out of range: side streams exist for devices 0..63",
+              dev);
+  GPS_TRY(sides[dev].init());
+  *out = &sides[dev];
+  return GPS_OK;
 }
 
 // ------------------------------------------------------------------------------- weight packing
@@ -182,7 +182,38 @@ __global__ void k_unpack(PackDesc pd, const float* __restrict__ gWcat, const flo
   if (threadIdx.x == 0 && pd.seg[s].gb) pd.seg[s].gb[r - row0] = (accumulate ? pd.seg[s].gb[r - row0] : 0.f) + gbcat[r];
 }
 
+// ---- dropout-only pass: reuse the BN-apply skeleton with an identity BatchNorm is overkill; a
+// dedicated tiny kernel keeps it explicit.
+__global__ void k_dropmul(const float* __restrict__ src, float* __restrict__ dst, int64_t n4, int64_t c4n, float p,
+                          uint64_t seed, uint64_t offset, int site, const unsigned long long* offset_dev, float p2,
+                          int site2, Planes dstp) {
+  if (offset_dev) offset += *offset_dev;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    float4 v = ld4(src + i * 4);
+    if (p > 0.f) v = f4mul(v, dropout_scale4(p, seed, offset, site, (uint64_t)i));
+    if (p2 > 0.f) v = f4mul(v, dropout_scale4(p2, seed, offset, site2, (uint64_t)i));
+    st4(dst + i * 4, v);
+    if (dstp.hi) planes_store4(dstp, i / c4n, (i % c4n) * 4, v);
+  }
+}
+__global__ void k_dropmask(float* __restrict__ dst, int64_t n4, float p, uint64_t seed, uint64_t offset, int site) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    float4 s = dropout_scale4(p, seed, offset, site, (uint64_t)i);
+    st4(dst + i * 4, make_float4(s.x > 0.f ? 1.f : 0.f, s.y > 0.f ? 1.f : 0.f, s.z > 0.f ? 1.f : 0.f,
+                                 s.w > 0.f ? 1.f : 0.f));
+  }
+}
+
 enum { BN_X = 0, BN_E = 1, BN_L = 2, BN_A = 3, BN_2 = 4, BN_COUNT = 5 };
+
+struct Plan;
+// A weight that the dense products read as bf16 operand planes.  The segments of Wcat (planes == &Plan::Wcat_p) are the
+// Linears k_pack concatenates; row0 is a segment's first row in Wcat.
+struct LayerWeight {
+  PackSeg lin;   // weight [rows, cols] with the bias and gradients k_pack / k_unpack use for a Wcat segment
+  int64_t cols, row0;
+  Planes Plan::*planes;
+};
 
 struct Plan {
   int64_t N, E, d, H, hd, Wy, qkv_off;
@@ -207,6 +238,9 @@ struct Plan {
   Planes gt_p, ghid_p, ghA_p, ge_p, gY1_p, gtmp_p, gtmp2_p, gtmp3_p, gl1_p, gh1_p;
   Planes qkv_p;        // Q | K | V per head, padded to hd_pad columns: operands of the wgmma attention
   bool attn_tc;        // softmax attention on the tensor cores (attention_tc.cu)
+  // the weights with operand planes, in the order their planes are allocated and converted (list_weights)
+  LayerWeight weights[12];
+  int nweights;
   int64_t saved_bytes;
   int64_t wplanes_bytes;
   // forward workspace
@@ -217,20 +251,63 @@ struct Plan {
   float *g_t, *g_hid, *g_s, *g_xloc, *g_hA, *g_O, *gY1, *g_e, *g_num, *delta, *g_tmp, *g_tmp2, *g_tmp3, *g_h1, *g_agg, *gWcat,
       *gbcat, *g_xl;
   int64_t bwd_bytes;
-  int64_t fwd_launches, bwd_launches;
+  // per call
+  bool train;
+  int prec;                // GPS_PREC_*
+  DropCfg dropout;         // GPSLayer.dropout: p = 0 in eval mode; the site is set per use (drop())
+  float pa;                // attn_dropout, 0 in eval mode
+  bool grads_prezeroed;    // GpsLayerArgs.reserved0 bit 0: the caller already zeroed every parameter-gradient buffer
+                           // (one multi-tensor fill instead of a memset per weight and bias)
+  bool grads_accumulate;   // bit 1: parameter gradients are ADDED to the caller's buffers (torch's .grad accumulation
+                           // semantics on a static gradient bucket: graphgps_b200/dp.py); implies bit 0
+  DropCfg drop(int site) const {
+    DropCfg c = dropout;
+    c.site = site;
+    return c;
+  }
 };
 
-// Forward softmax attention on the tensor cores (attention_tc.cu) when the batch's graphs are large enough for 128 x 128
-// tiles to pay: at the PCQM4M shape (mean 14 nodes per graph) a 128-row tile sees ~45 useful keys of 256 in one
-// latency-bound wave and the CUDA-core kernel is faster; the tensor-core kernel wins once a graph fills a tile
-// (ogbg-code2 shape, mean 125 / max ~1000 nodes).  GPS_B200_ATTN=simt | tc overrides.
-static bool attn_tc_enabled(int64_t N, int64_t B) {
-  static const int mode = [] {
-    const char* e = getenv("GPS_B200_ATTN");
-    return e && strcmp(e, "simt") == 0 ? 0 : (e && strcmp(e, "tc") == 0 ? 2 : 1);
-  }();
-  if (mode != 1) return mode == 2;
-  return B > 0 && N >= 64 * B;
+// The weights with operand planes.  Wcat = [A;B;D;E | conv | in_proj] holds the node projections, so that one GEMM
+// computes [Ax|Bx|Dx|Ex|Q|K|V]; this list is the one statement of that layout and sets Wy and qkv_off.
+static void list_weights(const GpsLayerArgs* a, Plan* P) {
+  const int64_t d = P->d, kout = P->perf ? P->inner : d;
+  auto add = [&](const GpsLinear& l, int64_t rows, int64_t cols, Planes Plan::*planes, bool bias = true) {
+    const bool wcat = planes == &Plan::Wcat_p;
+    const PackSeg seg{l.weight, bias ? l.bias : nullptr, l.grad_weight, bias ? l.grad_bias : nullptr, (int)rows};
+    P->weights[P->nweights++] = LayerWeight{seg, cols, wcat ? P->Wy : 0, planes};
+    if (wcat) P->Wy += rows;
+  };
+  if (P->gated) {
+    add(a->gcn_A, d, d, &Plan::Wcat_p);
+    add(a->gcn_B, d, d, &Plan::Wcat_p);
+    add(a->gcn_D, d, d, &Plan::Wcat_p);
+    add(a->gcn_E, d, d, &Plan::Wcat_p);
+    add(a->gcn_C, d, d, &Plan::C_p);
+  }
+  // GCNConv.lin has no bias; GCNConv.bias is added after the aggregation (scatter.cu)
+  if (P->gcn) add(a->gcn_conv, d, d, &Plan::Wcat_p, false);
+  P->qkv_off = P->Wy;
+  if (P->attn) add(a->attn_in, 3 * d, d, &Plan::Wcat_p);
+  if (P->attn || P->perf) add(a->attn_out, d, kout, &Plan::out_p);
+  add(a->ff1, 2 * d, d, &Plan::ff1_p);
+  add(a->ff2, d, 2 * d, &Plan::ff2_p);
+  if (P->gine) {
+    add(a->gine_lin0, d, d, &Plan::g0_p);
+    add(a->gine_lin1, d, d, &Plan::g1_p);
+  }
+  if (P->perf) {
+    add(a->perf_q, P->inner, d, &Plan::pq_p);
+    add(a->perf_k, P->inner, d, &Plan::pk_p);
+    add(a->perf_v, P->inner, d, &Plan::pv_p);
+  }
+}
+
+// Planes the caller hands over: a previous layer's output planes, or buffers for this layer's output planes.  Taken
+// when they hold what the precision needs (lo in fp32 mode) with a TMA-aligned pitch, else empty.
+static Planes caller_planes(const GpsPlanes& g, int64_t d, int precision) {
+  const bool lo = precision == GPS_PREC_FP32;
+  if (!g.hi || (lo && !g.lo) || g.ld < d || g.ld % 8 != 0) return Planes();
+  return Planes{(__nv_bfloat16*)g.hi, lo ? (__nv_bfloat16*)g.lo : nullptr, g.ld};
 }
 
 static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
@@ -272,9 +349,17 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   GPS_REQUIRE(a->act == GPS_ACT_RELU || a->act == GPS_ACT_GELU, GPS_ERR_ARG, "unknown activation %d", a->act);
   GPS_REQUIRE(a->dropout >= 0.f && a->dropout < 1.f && a->attn_dropout >= 0.f && a->attn_dropout < 1.f,
               GPS_ERR_ARG, "dropout probabilities must be in [0,1)");
+  P->train = a->training != 0;
+  P->prec = a->precision;
+  P->dropout.p = P->train && a->dropout > 0.f ? a->dropout : 0.f;
+  P->dropout.seed = a->seed;
+  P->dropout.offset = a->offset;
+  P->dropout.offset_dev = (const unsigned long long*)a->offset_dev;
+  P->pa = P->train ? a->attn_dropout : 0.f;
+  P->grads_accumulate = (a->reserved0 & 2) != 0;
+  P->grads_prezeroed = (a->reserved0 & 1) != 0 || P->grads_accumulate;
+  list_weights(a, P);
   const int64_t N = P->N, E = P->E, d = P->d;
-  P->qkv_off = P->gated ? 4 * d : (P->gcn ? d : 0);
-  P->Wy = P->qkv_off + (P->attn ? 3 * d : 0);
   const bool gelu = a->act == GPS_ACT_GELU;
 
   Arena S(bind ? a->saved : nullptr, a->saved_bytes);
@@ -336,17 +421,19 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   };
   if (P->use_planes) {
     const int64_t kout = P->perf ? P->inner : d;
-    auto handed = [&](const GpsPlanes& g) {   // planes written by the previous layer of the stack
-      Planes q;
-      q.hi = (__nv_bfloat16*)g.hi; q.lo = lo ? (__nv_bfloat16*)g.lo : nullptr; q.ld = g.ld;
-      return q;
-    };
-    const bool x_in = a->x_planes_in.hi && (!lo || a->x_planes_in.lo) && a->x_planes_in.ld >= d && a->x_planes_in.ld % 8 == 0;
-    const bool e_in = a->e_planes_in.hi && (!lo || a->e_planes_in.lo) && a->e_planes_in.ld >= d && a->e_planes_in.ld % 8 == 0;
-    P->x_p = x_in ? handed(a->x_planes_in) : mkplanes(S, N, d);
-    if (P->gated || P->gine) P->e_p = e_in ? handed(a->e_planes_in) : mkplanes(S, E, d);
+    // inputs: the planes written by the previous layer of the stack when it hands them over
+    P->x_p = caller_planes(a->x_planes_in, d, a->precision);
+    if (!P->x_p.hi) P->x_p = mkplanes(S, N, d);
+    if (P->gated || P->gine) {
+      P->e_p = caller_planes(a->e_planes_in, d, a->precision);
+      if (!P->e_p.hi) P->e_p = mkplanes(S, E, d);
+    }
     if (P->attn || P->perf) P->O_p = mkplanes(S, N, kout);
-    P->attn_tc = P->attn && attention_tc_supported(P->hd) && attn_tc_enabled(N, a->graph.B);
+    // Forward softmax attention on the tensor cores (attention_tc.cu) when the batch's graphs are large enough for
+    // 128 x 128 tiles to pay: at the PCQM4M shape (mean 14 nodes per graph) a 128-row tile sees ~45 useful keys of 256
+    // in one latency-bound wave and the CUDA-core kernel is faster; the tensor-core kernel wins once a graph fills a
+    // tile (ogbg-code2 shape, mean 125 / max ~1000 nodes).
+    P->attn_tc = P->attn && attention_tc_supported(P->hd) && a->graph.B > 0 && N >= 64 * a->graph.B;
     if (P->attn_tc) P->qkv_p = mkplanes(S, N, 3 * P->H * attention_tc_hd_pad(P->hd));
     P->s_p = mkplanes(S, N, d);
     P->hid_p = mkplanes(S, N, 2 * d);
@@ -356,34 +443,15 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
     }
     // weight planes: in the caller's persistent buffer when one is given (packed once per optimiser step), else in `saved`
     Arena Wa(bind ? a->wplanes : nullptr, a->wplanes_bytes);
-    const bool persistent = bind && a->wplanes != nullptr;
-    Arena& WA = persistent ? Wa : S;
-    Arena Wc(nullptr, 0);            // size of the persistent buffer, counted independently of `saved`
-    for (int pass = 0; pass < 2; ++pass) {
-      Arena& A = pass == 0 ? Wc : WA;
-      Planes wcat, cp, outp, f1, f2, g0, g1, pq, pk, pv;
-      if (P->Wy) wcat = mkplanes(A, P->Wy, d);
-      if (P->gated) cp = mkplanes(A, d, d);
-      if (P->attn || P->perf) outp = mkplanes(A, d, kout);
-      f1 = mkplanes(A, 2 * d, d);
-      f2 = mkplanes(A, d, 2 * d);
-      if (P->gine) {
-        g0 = mkplanes(A, d, d);
-        g1 = mkplanes(A, d, d);
-      }
-      if (P->perf) {
-        pq = mkplanes(A, P->inner, d);
-        pk = mkplanes(A, P->inner, d);
-        pv = mkplanes(A, P->inner, d);
-      }
-      if (pass == 1) {
-        P->Wcat_p = wcat; P->C_p = cp; P->out_p = outp; P->ff1_p = f1; P->ff2_p = f2; P->g0_p = g0; P->g1_p = g1;
-        P->pq_p = pq; P->pk_p = pk; P->pv_p = pv;
-      }
+    Arena& WA = bind && a->wplanes != nullptr ? Wa : S;
+    const int64_t w0 = WA.used;
+    for (int i = 0; i < P->nweights; ++i) {
+      const LayerWeight& w = P->weights[i];
+      if (w.row0 == 0) P->*w.planes = mkplanes(WA, w.planes == &Plan::Wcat_p ? P->Wy : w.lin.rows, w.cols);
     }
-    P->wplanes_bytes = Wc.used;
+    P->wplanes_bytes = WA.used - w0;
     GPS_REQUIRE(!Wa.overflow, GPS_ERR_ARG, "wplanes buffer too small (%lld < %lld)", (long long)a->wplanes_bytes,
-                (long long)Wc.used);
+                (long long)P->wplanes_bytes);
   }
   P->saved_bytes = S.used;
   GPS_REQUIRE(!S.overflow, GPS_ERR_ARG, "saved buffer too small (%lld < %lld)", (long long)a->saved_bytes,
@@ -463,22 +531,26 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   return GPS_OK;
 }
 
-static BnView bn_view(const Plan& P, int which, const GpsBatchNorm& bn) {
+// BatchNorm `which` as its consumer kernels see it.  Eval: the running statistics (mode 2); BatchNorm is then a
+// per-column affine map and its backward has no batch terms.  Training backward: the batch statistics the forward pass
+// saved (mode 0).  Training forward, over fwd_rows rows: the consumer kernel finalises the statistics from the
+// producer's column sums, saves them for the backward and updates the running statistics (mode 1).
+static BnView bn_view(const Plan& P, int which, const GpsBatchNorm& bn, int64_t fwd_rows = -1) {
+  const bool fwd = fwd_rows >= 0;
   BnView v;
   v.mean = P.bnbuf + (int64_t)which * 2 * P.d;
   v.invstd = v.mean + P.d;
   v.gamma = bn.weight;
   v.beta = bn.bias;
-  return v;
-}
-
-// forward view: the consumer kernel finalises the statistics itself (BnView mode 1 / 2)
-static BnView bn_view_fwd(const Plan& P, const GpsLayerArgs* a, int which, const GpsBatchNorm& bn, int64_t n) {
-  BnView v = bn_view(P, which, bn);
-  v.d = P.d;
-  v.running_mean = bn.running_mean;
-  v.running_var = bn.running_var;
-  if (a->training) {
+  if (fwd) v.d = P.d;
+  if (fwd || !P.train) {
+    v.running_mean = bn.running_mean;
+    v.running_var = bn.running_var;
+  }
+  if (!P.train) {
+    v.mode = 2;
+  } else if (fwd) {
+    const int64_t n = fwd_rows;
     v.mode = 1;
     v.sums = P.fstats + (int64_t)which * 2 * P.d;
     v.inv_n = 1.0 / (double)(n > 0 ? n : 1);
@@ -486,31 +558,19 @@ static BnView bn_view_fwd(const Plan& P, const GpsLayerArgs* a, int which, const
     v.save_mean = P.bnbuf + (int64_t)which * 2 * P.d;
     v.save_invstd = v.save_mean + P.d;
     v.nbt = (long long*)bn.num_batches_tracked;
-  } else {
-    v.mode = 2;
   }
   return v;
 }
 
-static PackDesc pack_desc(const GpsLayerArgs* a, const Plan& P) {
+static PackDesc pack_desc(const Plan& P) {
   PackDesc pd;
   memset(&pd, 0, sizeof(pd));
   pd.d = (int)P.d;
-  auto add = [&](const GpsLinear& l, int rows) {
-    pd.seg[pd.nseg++] = PackSeg{l.weight, l.bias, l.grad_weight, l.grad_bias, rows};
-    pd.total_rows += rows;
-  };
-  if (P.gated) {
-    add(a->gcn_A, (int)P.d);
-    add(a->gcn_B, (int)P.d);
-    add(a->gcn_D, (int)P.d);
-    add(a->gcn_E, (int)P.d);
+  for (int i = 0; i < P.nweights; ++i) {
+    if (P.weights[i].planes != &Plan::Wcat_p) continue;
+    pd.seg[pd.nseg++] = P.weights[i].lin;
+    pd.total_rows += P.weights[i].lin.rows;
   }
-  if (P.gcn) {   // GCNConv.lin has no bias; GCNConv.bias is added after the aggregation (scatter.cu)
-    pd.seg[pd.nseg++] = PackSeg{a->gcn_conv.weight, nullptr, a->gcn_conv.grad_weight, nullptr, (int)P.d};
-    pd.total_rows += (int)P.d;
-  }
-  if (P.attn) add(a->attn_in, (int)(3 * P.d));
   return pd;
 }
 
@@ -565,14 +625,50 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
   return GPS_OK;
 }
 
-// set per call from GpsLayerArgs.reserved0 bit 0: the caller already zeroed every parameter-gradient buffer
-// (one multi-tensor fill instead of a memset per weight and bias)
-static thread_local bool g_grads_prezeroed = false;
-// GpsLayerArgs.reserved0 bit 1: parameter gradients are ADDED to the caller's buffers (torch's .grad accumulation
-// semantics on a static gradient bucket: graphgps_b200/dp.py); implies bit 0
-static thread_local bool g_grads_accumulate = false;
+// ------------------------------------------------------------------------------- dense products
+// An operand: fp32 values with leading dimension ld and, where the layer keeps them, their bf16 planes.
+struct Operand {
+  const float* f;
+  int64_t ld;
+  Planes p;
+};
 
-static int splitk_for(int64_t rows, int64_t out = 304, int64_t in = 304) {
+// y[M,N] = x[M,K] W[N,K]^T (+ bias[N]); the caller adds the rest of the epilogue
+static GemmParams linear_fwd(const Plan& P, int64_t M, int64_t N, int64_t K, Operand x, Operand W, float* y, int64_t ldy,
+                             const float* bias = nullptr) {
+  GemmParams g;
+  g.M = (int)M; g.N = (int)N; g.K = (int)K;
+  g.A = x.f; g.lda = (int)x.ld; g.Ap = x.p;
+  g.B = W.f; g.ldb = (int)W.ld; g.Bp = W.p;
+  g.C = y; g.ldc = (int)ldy;
+  g.bias = bias;
+  g.precision = P.prec;
+  return g;
+}
+
+// g_x[M,N] = g[M,K] W[K,N]: the input gradient of linear_fwd
+static GemmParams linear_dgrad(const Plan& P, int64_t M, int64_t N, int64_t K, Operand g, Operand W, float* gx,
+                               int64_t ldgx) {
+  GemmParams p = linear_fwd(P, M, N, K, g, W, gx, ldgx);
+  p.tb = 1;
+  return p;
+}
+
+static void set_dropout(GemmParams& g, const DropCfg& c) {
+  g.p_drop = c.p; g.seed = c.seed; g.offset = c.offset; g.site = c.site; g.offset_dev = c.offset_dev;
+}
+
+// multiply by act'(pre-activation); ReLU reads the mask off the stored post-activation value instead
+static void set_act_mask(GemmParams& g, int act, const float* post, const float* pre, int64_t ld) {
+  if (act == GPS_ACT_RELU) {
+    g.mask_src = post; g.mask_is_post = 1;
+  } else {
+    g.mask_src = pre; g.mask_act = act;
+  }
+  g.ldmask = (int)ld;
+}
+
+static int splitk_for(int64_t rows, int64_t out, int64_t in) {
   // Weight gradients reduce over `rows` (nodes/edges) into a small [out, in] tile grid: split the reduction so
   // that tiles x splits ~ 300 CTAs (two per SM), at least 4 k-blocks of 64 rows per CTA (tools/gemm_tune.py).
   const int64_t tiles = ceil_div(out, 128) * ceil_div(in, in >= 160 ? 160 : 64);
@@ -584,33 +680,52 @@ static int splitk_for(int64_t rows, int64_t out = 304, int64_t in = 304) {
   return (int)s;
 }
 
-// weight gradient of a Linear: dW[out,in] = G[rows,out]^T X[rows,in], db[out] = colsum(G)
-static int linear_wgrad(const float* G, int64_t ldg, const float* X, int64_t ldx, int64_t rows, int64_t out,
-                        int64_t in, float* dW, float* db, int precision, cudaStream_t st, Planes Gp = Planes(),
-                        Planes Xp = Planes()) {
-  if (!dW) return GPS_OK;
-  if (!g_grads_prezeroed) {
-    GPS_CUDA(cudaMemsetAsync(dW, 0, (size_t)(out * in) * sizeof(float), st));
-    if (db) GPS_CUDA(cudaMemsetAsync(db, 0, (size_t)out * sizeof(float), st));
-  }
+// dW[out,in] += G[rows,out]^T X[rows,in], db[out] += colsum(G), into zeroed dW / db
+static int wgrad_add(const Plan& P, Operand G, Operand X, int64_t rows, int64_t out, int64_t in, float* dW, float* db,
+                     cudaStream_t st) {
   if (rows == 0) return GPS_OK;
   GemmParams p;
   p.M = (int)out; p.N = (int)in; p.K = (int)rows;
-  p.A = G; p.lda = (int)ldg; p.ta = 1;
-  p.B = X; p.ldb = (int)ldx; p.tb = 1;
+  p.A = G.f; p.lda = (int)G.ld; p.ta = 1; p.Ap = G.p;
+  p.B = X.f; p.ldb = (int)X.ld; p.tb = 1; p.Bp = X.p;
   p.C = dW; p.ldc = (int)in;
-  p.splitk = splitk_for(rows, out, in);
-  if (p.splitk == 1) p.splitk = 2;  // accumulate path (C pre-zeroed) also for tiny inputs
+  p.splitk = std::max(2, splitk_for(rows, out, in));   // the accumulating split-K path also for tiny inputs
   p.colsum_a = db;
-  p.precision = precision;
-  p.Ap = Gp; p.Bp = Xp;
-  if (precision == GPS_PREC_BF16 && Gp.hi && db) {
+  p.precision = P.prec;
+  if (P.prec == GPS_PREC_BF16 && G.p.hi && db) {
     // bf16 mode stores no lo plane: summing ~N bf16-rounded rows would put ~sqrt(N) 2^-9 of noise on a bias gradient
     // that is often a near-cancelling sum (every Linear here feeds a BatchNorm) -> exact fp32 column sum instead
     p.colsum_a = nullptr;
-    GPS_TRY(colsum(G, ldg, rows, out, db, st));
+    GPS_TRY(colsum(G.f, G.ld, rows, out, db, st));
   }
   return gemm(p, st);
+}
+
+// weight gradient of a Linear into the caller's buffers: dW[out,in] = G[rows,out]^T X[rows,in], db[out] = colsum(G)
+static int linear_wgrad(const Plan& P, Operand G, Operand X, int64_t rows, int64_t out, int64_t in, float* dW, float* db,
+                        cudaStream_t st) {
+  if (!dW) return GPS_OK;
+  if (!P.grads_prezeroed) {
+    GPS_CUDA(cudaMemsetAsync(dW, 0, (size_t)(out * in) * sizeof(float), st));
+    if (db) GPS_CUDA(cudaMemsetAsync(db, 0, (size_t)out * sizeof(float), st));
+  }
+  return wgrad_add(P, G, X, rows, out, in, dW, db, st);
+}
+
+// The [N, d] gradient g in front of the dropout at `site` (and, p2 > 0, of the inner one at site2 before it): g times
+// the dropout scales, written to the temporary tmp (and its planes tmp_p), when a dropout is active, else g itself.
+static int dropmul(const Plan& P, Operand g, float* tmp, Planes tmp_p, int site, cudaStream_t st, Operand* out,
+                   float p2 = 0.f, int site2 = 0) {
+  *out = g;
+  if (!(P.dropout.p > 0.f || p2 > 0.f)) return GPS_OK;
+  *out = Operand{tmp, P.d, tmp_p};
+  const int64_t n4 = P.N * P.d / 4;
+  if (n4 == 0) return GPS_OK;
+  const DropCfg c = P.drop(site);
+  k_dropmul<<<(unsigned)std::min<int64_t>(ceil_div(n4, 256), kNumSMs * 8), 256, 0, st>>>(
+      g.f, tmp, n4, P.d / 4, c.p, c.seed, c.offset, c.site, c.offset_dev, p2, site2, tmp_p);
+  GPS_LAUNCH_CHECK();
+  return GPS_OK;
 }
 
 }  // namespace
@@ -626,84 +741,48 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
   GPS_REQUIRE(a->x_out, GPS_ERR_ARG, "x_out is null");
   const int64_t N = P.N, E = P.E, d = P.d;
   const int act = a->act;
-  const bool train = a->training != 0;
-  const float pd = train ? a->dropout : 0.f;
-  const float pa = train ? a->attn_dropout : 0.f;
-  auto drop = [&](int site) {
-    DropCfg c;
-    c.p = pd; c.seed = a->seed; c.offset = a->offset; c.site = site;
-    c.offset_dev = (const unsigned long long*)a->offset_dev;
-    return c;
-  };
-  auto stats = [&](int which) -> double* { return train ? P.fstats + (int64_t)which * 2 * d : nullptr; };
+  auto stats = [&](int which) -> double* { return P.train ? P.fstats + (int64_t)which * 2 * d : nullptr; };
   auto out_planes = [&](const GpsPlanes& g) {   // planes of this layer's outputs for the next layer of the stack
-    Planes q;
-    if (P.use_planes && g.hi && g.ld >= d && g.ld % 8 == 0) {
-      q.hi = (__nv_bfloat16*)g.hi;
-      q.lo = a->precision == GPS_PREC_FP32 ? (__nv_bfloat16*)g.lo : nullptr;
-      q.ld = g.ld;
-      if (a->precision == GPS_PREC_FP32 && !q.lo) q = Planes();
-    }
-    return q;
+    return P.use_planes ? caller_planes(g, d, P.prec) : Planes();
   };
 
-  if (train) GPS_CUDA(cudaMemsetAsync(P.fstats, 0, (size_t)BN_COUNT * 2 * d * sizeof(double), st));
-  Side* sd = side_stream();
-  cudaStream_t s2 = sd ? sd->s : st;
+  if (P.train) GPS_CUDA(cudaMemsetAsync(P.fstats, 0, (size_t)BN_COUNT * 2 * d * sizeof(double), st));
+  Side* sd;
+  GPS_TRY(side_stream(&sd));
+  cudaStream_t s2 = sd->s;
   const bool two_branches = (P.gated || P.gine || P.gcn) && (P.attn || P.perf);
 
   // weights: concatenate the node projections
   if (P.Wy) {
-    PackDesc pdsc0 = pack_desc(a, P);
+    PackDesc pdsc0 = pack_desc(P);
     k_pack<<<(unsigned)pdsc0.total_rows, 128, 0, st>>>(pdsc0, P.Wcat, P.bcat);
     GPS_LAUNCH_CHECK();
   }
   if (P.use_planes) {
     // layer inputs and every weight -> bf16 hi/lo planes, one launch (the producers inside the layer write the
-    // planes of their outputs themselves).  Wcat_p rows follow pack_desc(): [A;B;D;E | conv] then in_proj.
+    // planes of their outputs themselves)
     ToPlanesItem it[16];
     int ni = 0;
     auto add = [&](const float* src, int64_t ld, int64_t rows, int64_t cols, Planes dst) {
       if (src && dst.hi && rows > 0) it[ni++] = ToPlanesItem{src, ld, (int)rows, (int)cols, dst};
     };
-    const int64_t kout = P.perf ? P.inner : d;
     if (P.x_p.hi != (__nv_bfloat16*)a->x_planes_in.hi) add(a->x, d, N, d, P.x_p);
     if ((P.gated || P.gine) && P.e_p.hi != (__nv_bfloat16*)a->e_planes_in.hi) add(a->edge_attr, d, E, d, P.e_p);
-    const bool wvalid = a->wplanes && a->wplanes_valid;
-    if (wvalid) goto weights_done;
-    if (P.gated) {
-      add(a->gcn_A.weight, d, d, d, P.Wcat_p.rows(0));
-      add(a->gcn_B.weight, d, d, d, P.Wcat_p.rows(d));
-      add(a->gcn_D.weight, d, d, d, P.Wcat_p.rows(2 * d));
-      add(a->gcn_E.weight, d, d, d, P.Wcat_p.rows(3 * d));
-      add(a->gcn_C.weight, d, d, d, P.C_p);
+    if (!(a->wplanes && a->wplanes_valid)) {
+      for (int i = 0; i < P.nweights; ++i) {
+        const LayerWeight& w = P.weights[i];
+        add(w.lin.w, w.cols, w.lin.rows, w.cols, (P.*w.planes).rows(w.row0));
+      }
     }
-    if (P.gcn) add(a->gcn_conv.weight, d, d, d, P.Wcat_p.rows(0));
-    if (P.attn) add(a->attn_in.weight, d, 3 * d, d, P.Wcat_p.rows(P.qkv_off));
-    if (P.gine) {
-      add(a->gine_lin0.weight, d, d, d, P.g0_p);
-      add(a->gine_lin1.weight, d, d, d, P.g1_p);
-    }
-    if (P.attn || P.perf) add(a->attn_out.weight, kout, d, kout, P.out_p);
-    add(a->ff1.weight, d, 2 * d, d, P.ff1_p);
-    add(a->ff2.weight, 2 * d, d, 2 * d, P.ff2_p);
-    if (P.perf) {
-      add(a->perf_q.weight, d, P.inner, d, P.pq_p);
-      add(a->perf_k.weight, d, P.inner, d, P.pk_p);
-      add(a->perf_v.weight, d, P.inner, d, P.pv_p);
-    }
-  weights_done:
     GPS_TRY(to_planes(it, ni, st));
   }
   if (P.gated) {   // edge projection has no dependency on the node side: run it next to the node projections
     GPS_REQUIRE(a->edge_out, GPS_ERR_ARG, "edge_out is null");
-    if (sd) GPS_TRY(sd->fork(st));
-    GemmParams g;  // Ce = e C^T + bC (gatedgcn_layer.py:59)
-    g.M = (int)E; g.N = (int)d; g.K = (int)d;
-    g.A = a->edge_attr; g.lda = (int)d; g.B = a->gcn_C.weight; g.ldb = (int)d; g.C = P.ehat; g.ldc = (int)d;
-    g.bias = a->gcn_C.bias; g.precision = a->precision;
-    g.Ap = P.e_p; g.Bp = P.C_p;
-    GPS_TRY(gemm(g, s2));
+    GPS_TRY(sd->fork(st));
+    // Ce = e C^T + bC (gatedgcn_layer.py:59)
+    GPS_TRY(gemm(linear_fwd(P, E, d, d, {a->edge_attr, d, P.e_p}, {a->gcn_C.weight, d, P.C_p}, P.ehat, d,
+                            a->gcn_C.bias),
+                 s2));
     // EquivStableLapPE gate r_e, rho_e: reads PE, the graph and mlp_r_ij only (gatedgcn_layer.py:101-104)
     if (P.eslap)
       GPS_TRY(eslap_fwd(a->graph, a->pe, a->pe_dim, d, act, a->pe_mlp0.weight, a->pe_mlp0.bias, a->pe_mlp1.weight,
@@ -715,84 +794,67 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
   // message-passing branch, [Q|K|V] on the attention branch's stream, so both branches start ~25 us after the
   // pack instead of after one 50 us GEMM.
   cudaStream_t sg = st;   // stream of the global-attention branch
-  if (two_branches && sd) {
+  if (two_branches) {
     GPS_TRY(sd->order(st, sd->s3));
     sg = sd->s3;
   }
   if (P.Wy) {
     const int64_t wl = P.qkv_off, wg = P.Wy - P.qkv_off;   // local / global column blocks
+    const Operand x{a->x, d, P.x_p};
     if (wg > 0) {
-      GemmParams g;
-      g.M = (int)N; g.N = (int)wg; g.K = (int)d;
-      g.A = a->x; g.lda = (int)d; g.B = P.Wcat + wl * d; g.ldb = (int)d; g.C = P.Y1 + wl; g.ldc = (int)P.Wy;
-      g.bias = P.bcat + wl; g.precision = a->precision;
-      g.Ap = P.x_p; g.Bp = P.Wcat_p.rows(wl);
+      GemmParams g = linear_fwd(P, N, wg, d, x, {P.Wcat + wl * d, d, P.Wcat_p.rows(wl)}, P.Y1 + wl, P.Wy, P.bcat + wl);
       if (P.attn_tc) {   // Q | K | V additionally as padded per-head operand planes for the wgmma attention
         g.Cp = P.qkv_p; g.cp_hd = (int)P.hd; g.cp_hd_pad = (int)attention_tc_hd_pad(P.hd); g.cp_col0 = 0;
       }
       GPS_TRY(gemm(g, sg));
     }
-    if (wl > 0) {
-      GemmParams g;
-      g.M = (int)N; g.N = (int)wl; g.K = (int)d;
-      g.A = a->x; g.lda = (int)d; g.B = P.Wcat; g.ldb = (int)d; g.C = P.Y1; g.ldc = (int)P.Wy;
-      g.bias = P.bcat; g.precision = a->precision;
-      g.Ap = P.x_p; g.Bp = P.Wcat_p;
-      GPS_TRY(gemm(g, st));
-    }
+    if (wl > 0) GPS_TRY(gemm(linear_fwd(P, N, wl, d, x, {P.Wcat, d, P.Wcat_p}, P.Y1, P.Wy, P.bcat), st));
   }
 
   // main waits for the edge projection
-  if (P.gated && sd) GPS_TRY(sd->join(st));
+  if (P.gated) GPS_TRY(sd->join(st));
 
   // ---- local model
   if (P.gated) {
     GPS_TRY(gatedgcn_fwd(a->graph, d, P.Y1, P.Y1 + d, P.Y1 + 2 * d, P.Y1 + 3 * d, P.Wy, P.ehat, P.xt,
                          stats(BN_X), stats(BN_E), st, P.pe_rho));
     // x_loc = x + drop(act(BN(x~)));  e_out = e + drop(act(BN(e^)))   (gatedgcn_layer.py:72-83)
-    GPS_TRY(bn_act_residual2(P.xt, a->x, P.xloc, N, bn_view_fwd(P, a, BN_X, a->bn_node_x, N), drop(GPS_SITE_GCN_X), stats(BN_L),
-                             P.ehat, a->edge_attr, a->edge_out, E, bn_view_fwd(P, a, BN_E, a->bn_edge_e, E),
-                             drop(GPS_SITE_GCN_E), out_planes(a->e_planes_out), d, act, st));
+    GPS_TRY(bn_act_residual2(P.xt, a->x, P.xloc, N, bn_view(P, BN_X, a->bn_node_x, N), P.drop(GPS_SITE_GCN_X),
+                             stats(BN_L), P.ehat, a->edge_attr, a->edge_out, E, bn_view(P, BN_E, a->bn_edge_e, E),
+                             P.drop(GPS_SITE_GCN_E), out_planes(a->e_planes_out), d, act, st));
   } else if (P.gine) {
     GPS_TRY(gine_fwd(a->graph, d, a->x, a->edge_attr, a->gine_eps, P.agg, st, P.agg_p));
-    GemmParams g;  // h1 = act(agg W0^T + b0)
-    g.M = (int)N; g.N = (int)d; g.K = (int)d;
-    g.A = P.agg; g.lda = (int)d; g.B = a->gine_lin0.weight; g.ldb = (int)d; g.C = P.h1; g.ldc = (int)d;
-    g.bias = a->gine_lin0.bias; g.act = act; g.C_pre = P.h1_pre; g.ldpre = (int)d; g.precision = a->precision;
-    g.Ap = P.agg_p; g.Bp = P.g0_p; g.Cp = P.h1_p;
+    // h1 = act(agg W0^T + b0)
+    GemmParams g = linear_fwd(P, N, d, d, {P.agg, d, P.agg_p}, {a->gine_lin0.weight, d, P.g0_p}, P.h1, d,
+                              a->gine_lin0.bias);
+    g.act = act; g.C_pre = P.h1_pre; g.ldpre = (int)d; g.Cp = P.h1_p;
     GPS_TRY(gemm(g, st));
-    GemmParams g2;  // x_loc = x + drop(h1 W1^T + b1)  (gps_layer.py:188-189)
-    g2.M = (int)N; g2.N = (int)d; g2.K = (int)d;
-    g2.A = P.h1; g2.lda = (int)d; g2.B = a->gine_lin1.weight; g2.ldb = (int)d; g2.C = P.xloc; g2.ldc = (int)d;
-    g2.bias = a->gine_lin1.bias; g2.R1 = a->x; g2.ldr1 = (int)d; g2.stats = stats(BN_L);
-    g2.p_drop = pd; g2.seed = a->seed; g2.offset = a->offset; g2.site = GPS_SITE_LOCAL;
-    g2.offset_dev = (const unsigned long long*)a->offset_dev;
-    g2.precision = a->precision;
-    g2.Ap = P.h1_p; g2.Bp = P.g1_p;
+    // x_loc = x + drop(h1 W1^T + b1)  (gps_layer.py:188-189)
+    GemmParams g2 = linear_fwd(P, N, d, d, {P.h1, d, P.h1_p}, {a->gine_lin1.weight, d, P.g1_p}, P.xloc, d,
+                               a->gine_lin1.bias);
+    g2.R1 = a->x; g2.ldr1 = (int)d; g2.stats = stats(BN_L);
+    set_dropout(g2, P.drop(GPS_SITE_LOCAL));
     GPS_TRY(gemm(g2, st));
   } else if (P.gcn) {
     // x_loc = x + drop(GCNConv(x))  (gps_layer.py:49-51,186-189); Y = x W^T is column block 0 of Y1
     GPS_TRY(gcn_dinv(a->graph, P.dinv, st));
-    GPS_TRY(gcn_fwd(a->graph, d, P.Y1, P.Wy, P.dinv, a->gcn_conv.bias, a->x, P.xloc, drop(GPS_SITE_LOCAL), stats(BN_L), st));
+    GPS_TRY(gcn_fwd(a->graph, d, P.Y1, P.Wy, P.dinv, a->gcn_conv.bias, a->x, P.xloc, P.drop(GPS_SITE_LOCAL),
+                    stats(BN_L), st));
   }
 
   // ---- global attention  (gps_layer.py:198-218, 234-241)
   if (P.attn) {
     const float* Q = P.Y1 + P.qkv_off;
     if (P.attn_tc)
-      GPS_TRY(attention_tc_fwd(a->graph, P.H, P.hd, P.qkv_p, P.O, d, P.O_p, P.lse, pa, a->seed, a->offset,
-                               (const unsigned long long*)a->offset_dev, a->precision, sg));
+      GPS_TRY(attention_tc_fwd(a->graph, P.H, P.hd, P.qkv_p, P.O, d, P.O_p, P.lse, P.pa, a->seed, a->offset,
+                               (const unsigned long long*)a->offset_dev, P.prec, sg));
     else
-      GPS_TRY(attention_fwd(a->graph, P.H, P.hd, Q, Q + d, Q + 2 * d, P.Wy, P.O, d, P.lse, pa, a->seed, a->offset, sg,
-                            (const unsigned long long*)a->offset_dev, P.O_p));
-    GemmParams g;  // hA = x + drop(O Wo^T + bo)
-    g.M = (int)N; g.N = (int)d; g.K = (int)d;
-    g.A = P.O; g.lda = (int)d; g.B = a->attn_out.weight; g.ldb = (int)d; g.C = P.hA; g.ldc = (int)d;
-    g.bias = a->attn_out.bias; g.R1 = a->x; g.ldr1 = (int)d; g.stats = stats(BN_A);
-    g.p_drop = pd; g.seed = a->seed; g.offset = a->offset; g.site = GPS_SITE_ATTN_OUT;
-    g.offset_dev = (const unsigned long long*)a->offset_dev;
-    g.precision = a->precision;
-    g.Ap = P.O_p; g.Bp = P.out_p;
+      GPS_TRY(attention_fwd(a->graph, P.H, P.hd, Q, Q + d, Q + 2 * d, P.Wy, P.O, d, P.lse, P.pa, a->seed, a->offset,
+                            sg, (const unsigned long long*)a->offset_dev, P.O_p));
+    // hA = x + drop(O Wo^T + bo)
+    GemmParams g = linear_fwd(P, N, d, d, {P.O, d, P.O_p}, {a->attn_out.weight, d, P.out_p}, P.hA, d, a->attn_out.bias);
+    g.R1 = a->x; g.ldr1 = (int)d; g.stats = stats(BN_A);
+    set_dropout(g, P.drop(GPS_SITE_ATTN_OUT));
     GPS_TRY(gemm(g, sg));
   }
 
@@ -800,83 +862,59 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
   if (P.perf) {
     const int64_t inner = P.inner, NH = N * P.H, dh = a->perf_dim_head;
     const GpsLinear* lin[3] = {&a->perf_q, &a->perf_k, &a->perf_v};
+    const Planes wp[3] = {P.pq_p, P.pk_p, P.pv_p};
     float* dst[3] = {P.pQ, P.pK, P.pV};
-    for (int i = 0; i < 3; ++i) {   // q, k, v = x W^T (no bias)
-      GemmParams g;
-      g.M = (int)N; g.N = (int)inner; g.K = (int)d;
-      g.A = a->x; g.lda = (int)d; g.B = lin[i]->weight; g.ldb = (int)d; g.C = dst[i]; g.ldc = (int)inner;
-      g.precision = a->precision;
-      g.Ap = P.x_p; g.Bp = i == 0 ? P.pq_p : (i == 1 ? P.pk_p : P.pv_p);
-      GPS_TRY(gemm(g, sg));
-    }
+    for (int i = 0; i < 3; ++i)   // q, k, v = x W^T (no bias)
+      GPS_TRY(gemm(linear_fwd(P, N, inner, d, {a->x, d, P.x_p}, {lin[i]->weight, d, wp[i]}, dst[i], inner), sg));
     GPS_TRY(perf_prep(a->perf_proj, P.m, P.pPn, a->graph, P.H, P.pnmax, P.pgmax, P.pargk, sg));
     float* ddst[2] = {P.pfq, P.pfk};
-    for (int i = 0; i < 2; ++i) {   // dd = (x dn) P^T for every (node, head) row
-      GemmParams g;
-      g.M = (int)NH; g.N = (int)P.mp; g.K = (int)dh;
-      g.A = dst[i]; g.lda = (int)dh; g.B = P.pPn; g.ldb = (int)dh; g.C = ddst[i]; g.ldc = (int)P.mp;
-      g.precision = a->precision;
-      GPS_TRY(gemm(g, sg));
-    }
+    for (int i = 0; i < 2; ++i)   // dd = (x dn) P^T for every (node, head) row
+      GPS_TRY(gemm(linear_fwd(P, NH, P.mp, dh, {dst[i], dh}, {P.pPn, dh}, ddst[i], P.mp), sg));
     GPS_TRY(perf_features_fwd(P.pfq, P.pfk, P.pQ, P.pK, a->graph, P.H, P.m, P.pgmax, P.pargq, P.pargk, sg));
     if (P.perf_pairwise)
       GPS_TRY(perf_quad_fwd(a->graph, P.H, P.m, P.pnmax, P.pfq, P.pfk, P.pV, P.pgmax, P.O, P.pden, sg));
     else
       GPS_TRY(perf_linattn_fwd(a->graph, P.H, P.m, P.pnmax, P.pfq, P.pfk, P.pV, P.pgmax, P.O, sg));
-    GemmParams g;  // hA = x + drop(to_out(O))
-    g.M = (int)N; g.N = (int)d; g.K = (int)inner;
-    g.A = P.O; g.lda = (int)inner; g.B = a->attn_out.weight; g.ldb = (int)inner; g.C = P.hA; g.ldc = (int)d;
-    g.bias = a->attn_out.bias; g.R1 = a->x; g.ldr1 = (int)d; g.stats = stats(BN_A);
+    // hA = x + drop(to_out(O))
+    GemmParams g = linear_fwd(P, N, d, inner, {P.O, inner}, {a->attn_out.weight, inner}, P.hA, d, a->attn_out.bias);
+    g.R1 = a->x; g.ldr1 = (int)d; g.stats = stats(BN_A);
     // SelfAttention ends with dropout(p = attn_dropout) on to_out(O) (performer_layer.py:501-503, built with
     // dropout=self.attn_dropout at gps_layer.py:112-114); GPSLayer.dropout_attn (p = dropout) follows (:212)
-    g.p_drop = pd > 0.f ? pd : 0.f; g.seed = a->seed; g.offset = a->offset; g.site = GPS_SITE_ATTN_OUT;
-    g.p_drop2 = pa; g.site2 = GPS_SITE_PERF_OUT;
-    g.offset_dev = (const unsigned long long*)a->offset_dev;
-    g.precision = a->precision;
+    set_dropout(g, P.drop(GPS_SITE_ATTN_OUT));
+    g.p_drop2 = P.pa; g.site2 = GPS_SITE_PERF_OUT;
     GPS_TRY(gemm(g, sg));
   }
 
-  if (two_branches && sd) GPS_TRY(sd->order(sd->s3, st));
+  if (two_branches) GPS_TRY(sd->order(sd->s3, st));
 
   // ---- s = norm1_local(x_loc) + norm1_attn(hA)   (gps_layer.py:194,217,222)
   {
     const bool loc = P.gated || P.gine || P.gcn;
     const float* first = loc ? P.xloc : P.hA;
-    BnView bf = loc ? bn_view_fwd(P, a, BN_L, a->norm1_local, N) : bn_view_fwd(P, a, BN_A, a->norm1_attn, N);
+    BnView bf = loc ? bn_view(P, BN_L, a->norm1_local, N) : bn_view(P, BN_A, a->norm1_attn, N);
     const float* second = (loc && (P.attn || P.perf)) ? P.hA : nullptr;
-    BnView bs = bn_view_fwd(P, a, BN_A, a->norm1_attn, N);
+    BnView bs = bn_view(P, BN_A, a->norm1_attn, N);
     GPS_TRY(bn_combine(first, bf, second, bs, P.s, N, d, st, P.s_p));
   }
 
   // ---- FFN: t = s + drop(W2 drop(act(W1 s + b1)) + b2)   (gps_layer.py:225, 253-257)
   {
-    GemmParams g;
-    g.M = (int)N; g.N = (int)(2 * d); g.K = (int)d;
-    g.A = P.s; g.lda = (int)d; g.B = a->ff1.weight; g.ldb = (int)d; g.C = P.hid; g.ldc = (int)(2 * d);
-    g.bias = a->ff1.bias; g.act = act; g.C_pre = P.hid_pre; g.ldpre = (int)(2 * d);
-    g.p_drop = pd; g.seed = a->seed; g.offset = a->offset; g.site = GPS_SITE_FF1; g.precision = a->precision;
-    g.offset_dev = (const unsigned long long*)a->offset_dev;
-    g.Ap = P.s_p; g.Bp = P.ff1_p; g.Cp = P.hid_p;
+    GemmParams g = linear_fwd(P, N, 2 * d, d, {P.s, d, P.s_p}, {a->ff1.weight, d, P.ff1_p}, P.hid, 2 * d, a->ff1.bias);
+    g.act = act; g.C_pre = P.hid_pre; g.ldpre = (int)(2 * d); g.Cp = P.hid_p;
+    set_dropout(g, P.drop(GPS_SITE_FF1));
     GPS_TRY(gemm(g, st));
-    GemmParams g2;
-    g2.M = (int)N; g2.N = (int)d; g2.K = (int)(2 * d);
-    g2.A = P.hid; g2.lda = (int)(2 * d); g2.B = a->ff2.weight; g2.ldb = (int)(2 * d); g2.C = P.t; g2.ldc = (int)d;
-    g2.bias = a->ff2.bias; g2.R1 = P.s; g2.ldr1 = (int)d; g2.stats = stats(BN_2);
-    g2.p_drop = pd; g2.seed = a->seed; g2.offset = a->offset; g2.site = GPS_SITE_FF2; g2.precision = a->precision;
-    g2.offset_dev = (const unsigned long long*)a->offset_dev;
-    g2.Ap = P.hid_p; g2.Bp = P.ff2_p;
+    GemmParams g2 = linear_fwd(P, N, d, 2 * d, {P.hid, 2 * d, P.hid_p}, {a->ff2.weight, 2 * d, P.ff2_p}, P.t, d,
+                               a->ff2.bias);
+    g2.R1 = P.s; g2.ldr1 = (int)d; g2.stats = stats(BN_2);
+    set_dropout(g2, P.drop(GPS_SITE_FF2));
     GPS_TRY(gemm(g2, st));
-    GPS_TRY(bn_combine(P.t, bn_view_fwd(P, a, BN_2, a->norm2, N), nullptr, BnView(), a->x_out, N, d, st,
+    GPS_TRY(bn_combine(P.t, bn_view(P, BN_2, a->norm2, N), nullptr, BnView(), a->x_out, N, d, st,
                        out_planes(a->x_planes_out)));  // :229
   }
   return GPS_OK;
 }
 
 // =================================================================================== backward
-// out = a * dropout_scale(site)  (only launched when p > 0)
-static int dropmul(const float* src, float* dst, int64_t rows, int64_t d, const Plan& P, const GpsLayerArgs* a,
-                   int site, cudaStream_t st, float p2 = 0.f, int site2 = 0, Planes dstp = Planes());
-
 static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   Plan P;
   GPS_TRY(make_plan(a, &P, true));
@@ -884,39 +922,20 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   GPS_REQUIRE(a->workspace_bytes >= P.bwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.bwd_bytes);
   GPS_TRY(check_params(a, P));
-  // eval mode (running statistics, no dropout): BatchNorm is a per-column affine map, its backward has no batch terms
-  g_grads_accumulate = (a->reserved0 & 2) != 0;
-  g_grads_prezeroed = (a->reserved0 & 1) != 0 || g_grads_accumulate;
   GPS_REQUIRE(a->grad_x_out && a->grad_x, GPS_ERR_ARG, "grad_x_out / grad_x are required");
   const int64_t N = P.N, E = P.E, d = P.d;
-  const int act = a->act, prec = a->precision;
-  const float pd = a->training ? a->dropout : 0.f, pa = a->training ? a->attn_dropout : 0.f;
-  const bool relu = act == GPS_ACT_RELU;
-  auto drop = [&](int site) {
-    DropCfg c;
-    c.p = pd; c.seed = a->seed; c.offset = a->offset; c.site = site;
-    c.offset_dev = (const unsigned long long*)a->offset_dev;
-    return c;
-  };
+  const int act = a->act;
   DropCfg nodrop;
-  // training: the batch statistics saved by the forward pass; eval: the running statistics the forward pass used
-  auto bview = [&](int which, const GpsBatchNorm& bn) {
-    BnView v = bn_view(P, which, bn);
-    if (!a->training) {
-      v.mode = 2;
-      v.running_mean = bn.running_mean;
-      v.running_var = bn.running_var;
-    }
-    return v;
-  };
   auto sums = [&](int which) { return P.bsums + (int64_t)which * 2 * d; };
   GPS_CUDA(cudaMemsetAsync(P.bsums, 0, (size_t)BN_COUNT * 2 * d * sizeof(double), st));
   // weight-gradient GEMMs run on the side stream, each forked where its operands become final
-  Side* sd = side_stream();
-  cudaStream_t s2 = sd ? sd->s : st;
-  auto wfork = [&](cudaStream_t from) -> int { return sd ? sd->order(from, s2) : GPS_OK; };
+  Side* sd;
+  GPS_TRY(side_stream(&sd));
+  cudaStream_t s2 = sd->s;
+  auto wfork = [&](cudaStream_t from) -> int { return sd->order(from, s2); };
   const bool two_branches = (P.gated || P.gine || P.gcn) && (P.attn || P.perf);
-  cudaStream_t sa = (two_branches && sd) ? sd->s3 : st;   // stream of the attention-branch backward
+  cudaStream_t sa = two_branches ? sd->s3 : st;   // stream of the attention-branch backward
+  cudaStream_t se = sd->s4;                       // stream of the edge BatchNorm backward (GatedGCN)
   const int opt = opt_flags();
   // data-parallel hook: the caller's event is recorded on the weight-gradient stream once the early gradient group
   // (FFN, attention output projection, norm2 / norm1_local / norm1_attn) has been enqueued there
@@ -935,73 +954,63 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   // accumulators of the last two GEMMs of the pass are zeroed now, while their streams are idle, instead of on the tail
   const bool gx_splitk = P.Wy >= 1024 && N > 0;
   if (P.Wy) {
-    if (sd) GPS_TRY(sd->order(st, s2));
+    GPS_TRY(wfork(st));
     GPS_CUDA(cudaMemsetAsync(P.gWcat, 0, (size_t)(P.Wy * d + P.Wy) * sizeof(float), s2));
   }
   if (gx_splitk) GPS_CUDA(cudaMemsetAsync(a->grad_x, 0, (size_t)(N * d) * sizeof(float), st));
 
   // e_out = e + drop(act(BN_e(e^))) (gatedgcn_layer.py:76-83): g_e^ needs grad_edge_out alone -> off the critical path
-  cudaStream_t se = (P.gated && sd) ? sd->s4 : st;   // stream of the edge BatchNorm backward
   if (P.gated) {
-    if (se != st) GPS_TRY(sd->order(st, se));
-    BnView ve = bview(BN_E, a->bn_edge_e);
+    GPS_TRY(sd->order(st, se));
+    BnView ve = bn_view(P, BN_E, a->bn_edge_e);
     if (a->grad_edge_out && E > 0) {
-      GPS_TRY(bn_bwd_reduce(a->grad_edge_out, d, P.ehat, d, E, d, ve, act, drop(GPS_SITE_GCN_E), sums(BN_E), se));
-      GPS_TRY(bn_bwd_apply(a->grad_edge_out, d, P.ehat, d, E, d, ve, act, drop(GPS_SITE_GCN_E), sums(BN_E), P.g_e, d,
-                           a->bn_edge_e.grad_weight, a->bn_edge_e.grad_bias, se, g_grads_accumulate));
+      GPS_TRY(bn_bwd_reduce(a->grad_edge_out, d, P.ehat, d, E, d, ve, act, P.drop(GPS_SITE_GCN_E), sums(BN_E), se));
+      GPS_TRY(bn_bwd_apply(a->grad_edge_out, d, P.ehat, d, E, d, ve, act, P.drop(GPS_SITE_GCN_E), sums(BN_E), P.g_e, d,
+                           a->bn_edge_e.grad_weight, a->bn_edge_e.grad_bias, se, P.grads_accumulate));
     } else {
       if (E > 0) GPS_CUDA(cudaMemsetAsync(P.g_e, 0, (size_t)(E * d) * sizeof(float), se));
-      if (a->bn_edge_e.grad_weight && !g_grads_prezeroed)
+      if (a->bn_edge_e.grad_weight && !P.grads_prezeroed)
         GPS_CUDA(cudaMemsetAsync(a->bn_edge_e.grad_weight, 0, d * sizeof(float), se));
-      if (a->bn_edge_e.grad_bias && !g_grads_prezeroed)
+      if (a->bn_edge_e.grad_bias && !P.grads_prezeroed)
         GPS_CUDA(cudaMemsetAsync(a->bn_edge_e.grad_bias, 0, d * sizeof(float), se));
     }
   }
 
   // ---- norm2 (gps_layer.py:229): g_t
-  BnView v2 = bview(BN_2, a->norm2);
+  BnView v2 = bn_view(P, BN_2, a->norm2);
   GPS_TRY(bn_bwd_reduce(a->grad_x_out, d, P.t, d, N, d, v2, -1, nodrop, sums(BN_2), st));
   GPS_TRY(bn_bwd_apply(a->grad_x_out, d, P.t, d, N, d, v2, -1, nodrop, sums(BN_2), P.g_t, d, a->norm2.grad_weight,
-                       a->norm2.grad_bias, st, g_grads_accumulate, P.gt_p));
+                       a->norm2.grad_bias, st, P.grads_accumulate, P.gt_p));
 
   bool fused_la = false;
   // ---- FFN (gps_layer.py:253-257)
-  const float* g_ff2 = P.g_t;  // gradient at the output of ff_linear2 (after ff_dropout2)
-  Planes g_ff2_p = P.gt_p;
-  if (pd > 0.f) {
-    GPS_TRY(dropmul(P.g_t, P.g_tmp, N, d, P, a, GPS_SITE_FF2, st, 0.f, 0, P.gtmp_p));
-    g_ff2 = P.g_tmp;
-    g_ff2_p = P.gtmp_p;
-  }
   {
-    GemmParams g;  // g_hid = (g_ff2 W2) * act'(pre) * drop1
-    g.M = (int)N; g.N = (int)(2 * d); g.K = (int)d;
-    g.A = g_ff2; g.lda = (int)d; g.B = a->ff2.weight; g.ldb = (int)(2 * d); g.tb = 1; g.C = P.g_hid; g.ldc = (int)(2 * d);
-    if (relu) { g.mask_src = P.hid; g.mask_is_post = 1; } else { g.mask_src = P.hid_pre; g.mask_act = act; }
-    g.ldmask = (int)(2 * d);
-    g.p_drop = pd; g.seed = a->seed; g.offset = a->offset; g.site = GPS_SITE_FF1; g.precision = prec;
-    g.offset_dev = (const unsigned long long*)a->offset_dev;
-    g.Ap = g_ff2_p; g.Bp = P.ff2_p; g.Cp = P.ghid_p;
+    Operand g_ff2;   // gradient at the output of ff_linear2 (after ff_dropout2)
+    GPS_TRY(dropmul(P, {P.g_t, d, P.gt_p}, P.g_tmp, P.gtmp_p, GPS_SITE_FF2, st, &g_ff2));
+    // g_hid = (g_ff2 W2) * act'(pre) * drop1
+    GemmParams g = linear_dgrad(P, N, 2 * d, d, g_ff2, {a->ff2.weight, 2 * d, P.ff2_p}, P.g_hid, 2 * d);
+    set_act_mask(g, act, P.hid, P.hid_pre, 2 * d);
+    set_dropout(g, P.drop(GPS_SITE_FF1));
+    g.Cp = P.ghid_p;
     GPS_TRY(gemm(g, st));
+    const Operand g_hid{P.g_hid, 2 * d, P.ghid_p};
     GPS_TRY(wfork(st));
-    GPS_TRY(linear_wgrad(g_ff2, d, P.hid, 2 * d, N, d, 2 * d, a->ff2.grad_weight, a->ff2.grad_bias, prec, s2, g_ff2_p, P.hid_p));
-    GPS_TRY(linear_wgrad(P.g_hid, 2 * d, P.s, d, N, 2 * d, d, a->ff1.grad_weight, a->ff1.grad_bias, prec, s2, P.ghid_p, P.s_p));
-    GemmParams g2;  // g_s = g_t + g_hid W1
-    g2.M = (int)N; g2.N = (int)d; g2.K = (int)(2 * d);
-    g2.A = P.g_hid; g2.lda = (int)(2 * d); g2.B = a->ff1.weight; g2.ldb = (int)d; g2.tb = 1; g2.C = P.g_s; g2.ldc = (int)d;
-    g2.R1 = P.g_t; g2.ldr1 = (int)d; g2.precision = prec;
-    g2.Ap = P.ghid_p; g2.Bp = P.ff1_p;
+    GPS_TRY(linear_wgrad(P, g_ff2, {P.hid, 2 * d, P.hid_p}, N, d, 2 * d, a->ff2.grad_weight, a->ff2.grad_bias, s2));
+    GPS_TRY(linear_wgrad(P, g_hid, {P.s, d, P.s_p}, N, 2 * d, d, a->ff1.grad_weight, a->ff1.grad_bias, s2));
+    // g_s = g_t + g_hid W1
+    GemmParams g2 = linear_dgrad(P, N, d, 2 * d, g_hid, {a->ff1.weight, d, P.ff1_p}, P.g_s, d);
+    g2.R1 = P.g_t; g2.ldr1 = (int)d;
     // norm1_local and norm1_attn both take g_s as their upstream gradient (gps_layer.py:194,217,222): their backward
     // reductions ride this GEMM's epilogue instead of two more passes over g_s (GPS_B200_OPT bit 64)
-    fused_la = (opt & 64) && P.use_planes && g2.Ap.hi && g2.Bp.hi && N > 0 && a->training;
+    fused_la = (opt & 64) && P.use_planes && g2.Ap.hi && g2.Bp.hi && N > 0 && P.train;
     if (fused_la) {
       if (P.gated || P.gine || P.gcn) {
-        BnView v = bview(BN_L, a->norm1_local);
+        BnView v = bn_view(P, BN_L, a->norm1_local);
         g2.bnred[0].z = P.xloc; g2.bnred[0].ldz = (int)d; g2.bnred[0].mean = v.mean; g2.bnred[0].invstd = v.invstd;
         g2.bnred[0].sums = sums(BN_L);
       }
       if (P.attn || P.perf) {
-        BnView v = bview(BN_A, a->norm1_attn);
+        BnView v = bn_view(P, BN_A, a->norm1_attn);
         g2.bnred[1].z = P.hA; g2.bnred[1].ldz = (int)d; g2.bnred[1].mean = v.mean; g2.bnred[1].invstd = v.invstd;
         g2.bnred[1].sums = sums(BN_A);
       }
@@ -1013,69 +1022,54 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   bool chain_x = false;
   // ---- norm1_local / norm1_attn (gps_layer.py:194,217): g_xloc, g_hA
   if (loc) {
-    BnView v = bview(BN_L, a->norm1_local);
+    BnView v = bn_view(P, BN_L, a->norm1_local);
     if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.xloc, d, N, d, v, -1, nodrop, sums(BN_L), st));
-    chain_x = P.gated && N > 0 && (opt & 32) && a->training;
+    chain_x = P.gated && N > 0 && (opt & 32) && P.train;
     if (chain_x)   // ... and the reduction of local_model.bn_node_x's backward in the same pass (one launch less)
       GPS_TRY(bn_bwd_apply_chain(P.g_s, d, P.xloc, d, N, d, v, sums(BN_L), P.g_xloc, d, a->norm1_local.grad_weight,
-                                 a->norm1_local.grad_bias, g_grads_accumulate, P.gl1_p, P.xt, d,
-                                 bview(BN_X, a->bn_node_x), act, drop(GPS_SITE_GCN_X), sums(BN_X), st));
+                                 a->norm1_local.grad_bias, P.grads_accumulate, P.gl1_p, P.xt, d,
+                                 bn_view(P, BN_X, a->bn_node_x), act, P.drop(GPS_SITE_GCN_X), sums(BN_X), st));
     else
       GPS_TRY(bn_bwd_apply(P.g_s, d, P.xloc, d, N, d, v, -1, nodrop, sums(BN_L), P.g_xloc, d,
-                           a->norm1_local.grad_weight, a->norm1_local.grad_bias, st, g_grads_accumulate, P.gl1_p));
+                           a->norm1_local.grad_weight, a->norm1_local.grad_bias, st, P.grads_accumulate, P.gl1_p));
   }
   if (!P.attn && !P.perf) {   // no global model: the early group ends with norm1_local's gradients (stream st)
     GPS_TRY(wfork(st));
     GPS_TRY(early_done());
   }
-  if (two_branches && sd) GPS_TRY(sd->order(st, sa));   // attention-branch backward runs next to the local-model backward
+  if (two_branches) GPS_TRY(sd->order(st, sa));   // attention-branch backward runs next to the local-model backward
   if (P.attn) {
-    BnView v = bview(BN_A, a->norm1_attn);
+    BnView v = bn_view(P, BN_A, a->norm1_attn);
     if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
     GPS_TRY(bn_bwd_apply(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), P.g_hA, d, a->norm1_attn.grad_weight,
-                         a->norm1_attn.grad_bias, sa, g_grads_accumulate, P.ghA_p));
+                         a->norm1_attn.grad_bias, sa, P.grads_accumulate, P.ghA_p));
     // hA = x + drop(O Wo^T + bo)
-    const float* g_ao = P.g_hA;
-    Planes g_ao_p = P.ghA_p;
-    if (pd > 0.f) {
-      GPS_TRY(dropmul(P.g_hA, P.g_tmp2, N, d, P, a, GPS_SITE_ATTN_OUT, sa, 0.f, 0, P.gtmp2_p));
-      g_ao = P.g_tmp2;
-      g_ao_p = P.gtmp2_p;
-    }
-    GemmParams g;  // g_O = g_ao Wo
-    g.M = (int)N; g.N = (int)d; g.K = (int)d;
-    g.A = g_ao; g.lda = (int)d; g.B = a->attn_out.weight; g.ldb = (int)d; g.tb = 1; g.C = P.g_O; g.ldc = (int)d;
-    g.precision = prec;
-    g.Ap = g_ao_p; g.Bp = P.out_p;
-    GPS_TRY(gemm(g, sa));
+    Operand g_ao;
+    GPS_TRY(dropmul(P, {P.g_hA, d, P.ghA_p}, P.g_tmp2, P.gtmp2_p, GPS_SITE_ATTN_OUT, sa, &g_ao));
+    // g_O = g_ao Wo
+    GPS_TRY(gemm(linear_dgrad(P, N, d, d, g_ao, {a->attn_out.weight, d, P.out_p}, P.g_O, d), sa));
     GPS_TRY(wfork(sa));
-    GPS_TRY(linear_wgrad(g_ao, d, P.O, d, N, d, d, a->attn_out.grad_weight, a->attn_out.grad_bias, prec, s2, g_ao_p, P.O_p));
+    GPS_TRY(linear_wgrad(P, g_ao, {P.O, d, P.O_p}, N, d, d, a->attn_out.grad_weight, a->attn_out.grad_bias, s2));
     GPS_TRY(early_done());
     const float* Q = P.Y1 + P.qkv_off;
     float* gQ = P.gY1 + P.qkv_off;
     GPS_TRY(attention_bwd(a->graph, P.H, P.hd, Q, Q + d, Q + 2 * d, P.Wy, P.O, P.g_O, d, P.lse, P.delta, gQ, gQ + d,
-                          gQ + 2 * d, P.Wy, pa, a->seed, a->offset, sa, (const unsigned long long*)a->offset_dev,
+                          gQ + 2 * d, P.Wy, P.pa, a->seed, a->offset, sa, (const unsigned long long*)a->offset_dev,
                           P.gY1_p.cols(P.qkv_off), P.gY1_p.cols(P.qkv_off + d), P.gY1_p.cols(P.qkv_off + 2 * d)));
   }
 
   if (P.perf) {
     const int64_t inner = P.inner, NH = N * P.H, dh = a->perf_dim_head;
-    BnView v = bview(BN_A, a->norm1_attn);
+    BnView v = bn_view(P, BN_A, a->norm1_attn);
     if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
     GPS_TRY(bn_bwd_apply(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), P.g_hA, d, a->norm1_attn.grad_weight,
-                         a->norm1_attn.grad_bias, sa, g_grads_accumulate));
-    const float* g_ao = P.g_hA;   // hA = x + drop_pd(drop_pa(to_out(O)))
-    if (pd > 0.f || pa > 0.f) {
-      GPS_TRY(dropmul(P.g_hA, P.g_tmp2, N, d, P, a, GPS_SITE_ATTN_OUT, sa, pa, GPS_SITE_PERF_OUT));
-      g_ao = P.g_tmp2;
-    }
-    GemmParams g;  // g_O = g_ao Wout   [N, inner]
-    g.M = (int)N; g.N = (int)inner; g.K = (int)d;
-    g.A = g_ao; g.lda = (int)d; g.B = a->attn_out.weight; g.ldb = (int)inner; g.tb = 1; g.C = P.g_O; g.ldc = (int)inner;
-    g.precision = prec;
-    GPS_TRY(gemm(g, sa));
+                         a->norm1_attn.grad_bias, sa, P.grads_accumulate));
+    Operand g_ao;   // hA = x + drop_pd(drop_pa(to_out(O)))
+    GPS_TRY(dropmul(P, {P.g_hA, d}, P.g_tmp2, Planes(), GPS_SITE_ATTN_OUT, sa, &g_ao, P.pa, GPS_SITE_PERF_OUT));
+    // g_O = g_ao Wout   [N, inner]
+    GPS_TRY(gemm(linear_dgrad(P, N, inner, d, g_ao, {a->attn_out.weight, inner}, P.g_O, inner), sa));
     GPS_TRY(wfork(sa));
-    GPS_TRY(linear_wgrad(g_ao, d, P.O, inner, N, d, inner, a->attn_out.grad_weight, a->attn_out.grad_bias, prec, s2));
+    GPS_TRY(linear_wgrad(P, g_ao, {P.O, inner}, N, d, inner, a->attn_out.grad_weight, a->attn_out.grad_bias, s2));
     GPS_TRY(early_done());
     // linear attention and feature maps (performer_layer.py:200-205, 119-144)
     if (P.perf_pairwise)
@@ -1089,10 +1083,8 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     float* gdd[2] = {P.g_pfq, P.g_pfk};
     float* gqk[2] = {P.g_pQ, P.g_pK};
     for (int i = 0; i < 2; ++i) {   // g_q += g_dd Pn   (dd = q Pn^T)
-      GemmParams h;
-      h.M = (int)NH; h.N = (int)dh; h.K = (int)P.mp;
-      h.A = gdd[i]; h.lda = (int)P.mp; h.B = P.pPn; h.ldb = (int)dh; h.tb = 1; h.C = gqk[i]; h.ldc = (int)dh;
-      h.R1 = gqk[i]; h.ldr1 = (int)dh; h.precision = prec;
+      GemmParams h = linear_dgrad(P, NH, dh, P.mp, {gdd[i], P.mp}, {P.pPn, dh}, gqk[i], dh);
+      h.R1 = gqk[i]; h.ldr1 = (int)dh;
       GPS_TRY(gemm(h, sa));
     }
     // projections: dW = g^T x ;  g_xp = g_hA + gQ Wq + gK Wk + gV Wv
@@ -1100,11 +1092,9 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     const float* gsrc[3] = {P.g_pQ, P.g_pK, P.g_pV};
     GPS_TRY(wfork(sa));
     for (int i = 0; i < 3; ++i) {
-      GPS_TRY(linear_wgrad(gsrc[i], inner, a->x, d, N, inner, d, lin[i]->grad_weight, nullptr, prec, s2));
-      GemmParams h;
-      h.M = (int)N; h.N = (int)d; h.K = (int)inner;
-      h.A = gsrc[i]; h.lda = (int)inner; h.B = lin[i]->weight; h.ldb = (int)d; h.tb = 1; h.C = P.g_xp; h.ldc = (int)d;
-      h.R1 = i == 0 ? P.g_hA : P.g_xp; h.ldr1 = (int)d; h.precision = prec;
+      GPS_TRY(linear_wgrad(P, {gsrc[i], inner}, {a->x, d}, N, inner, d, lin[i]->grad_weight, nullptr, s2));
+      GemmParams h = linear_dgrad(P, N, d, inner, {gsrc[i], inner}, {lin[i]->weight, d}, P.g_xp, d);
+      h.R1 = i == 0 ? P.g_hA : P.g_xp; h.ldr1 = (int)d;
       GPS_TRY(gemm(h, sa));
     }
   }
@@ -1113,158 +1103,95 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   const float* g_x_local = nullptr;  // direct gradient paths into x besides the projections
   if (P.gated) {
     // x_loc = x + drop(act(BN_x(x~))): g_x~ -> gY1[:, 0:d]  (gatedgcn_layer.py:72-83)
-    BnView vx = bview(BN_X, a->bn_node_x);
-    if (!chain_x) GPS_TRY(bn_bwd_reduce(P.g_xloc, d, P.xt, d, N, d, vx, act, drop(GPS_SITE_GCN_X), sums(BN_X), st));
-    GPS_TRY(bn_bwd_apply(P.g_xloc, d, P.xt, d, N, d, vx, act, drop(GPS_SITE_GCN_X), sums(BN_X), P.gY1, P.Wy,
-                         a->bn_node_x.grad_weight, a->bn_node_x.grad_bias, st, g_grads_accumulate, P.gY1_p));
-    if (se != st) GPS_TRY(sd->order(se, st));
+    BnView vx = bn_view(P, BN_X, a->bn_node_x);
+    if (!chain_x)
+      GPS_TRY(bn_bwd_reduce(P.g_xloc, d, P.xt, d, N, d, vx, act, P.drop(GPS_SITE_GCN_X), sums(BN_X), st));
+    GPS_TRY(bn_bwd_apply(P.g_xloc, d, P.xt, d, N, d, vx, act, P.drop(GPS_SITE_GCN_X), sums(BN_X), P.gY1, P.Wy,
+                         a->bn_node_x.grad_weight, a->bn_node_x.grad_bias, st, P.grads_accumulate, P.gY1_p));
+    GPS_TRY(sd->order(se, st));
     // message/aggregate backward (SURVEY Appendix C)
     GPS_TRY(gatedgcn_bwd_dst(a->graph, d, P.gY1, P.Wy, P.ehat, P.Y1 + d, P.Wy, P.g_e, P.g_num, P.gY1 + 2 * d, st, P.ge_p,
                              P.gY1_p.cols(2 * d), P.pe_rho, P.g_den));
     // EquivStableLapPE gate: mlp_r_ij gradients (mid group) and grad_pe need g_num / g_den only, so they run on the
     // (by now idle) edge-BatchNorm stream next to the src-ordered pass and the weight gradients
-    cudaStream_t sp = (P.eslap && se != st) ? se : st;
     if (P.eslap) {
-      if (sp != st) GPS_TRY(sd->order(st, sp));
+      GPS_TRY(sd->order(st, se));
       GPS_TRY(eslap_bwd(a->graph, a->pe, a->pe_dim, d, act, P.g_num, P.g_den, P.Y1 + d, P.Wy, P.ehat, P.pe_r, P.pe_rho,
                         a->pe_mlp0.weight, a->pe_mlp0.bias, a->pe_mlp1.weight, P.pe_gz, P.pe_gr, P.pe_part, a->grad_pe,
                         a->pe_mlp0.grad_weight, a->pe_mlp0.grad_bias, a->pe_mlp1.grad_weight, a->pe_mlp1.grad_bias,
-                        g_grads_accumulate, sp));
+                        P.grads_accumulate, se));
     }
     GPS_TRY(gatedgcn_bwd_src(a->graph, d, P.g_e, P.ehat, P.g_num, P.gY1 + 3 * d, P.gY1 + d, P.Wy, st, P.gY1_p.cols(3 * d),
                              P.gY1_p.cols(d), P.pe_rho));
     // C: dC = g_e^T e ; g_edge_attr = grad_edge_out + g_e C
+    const Operand g_e{P.g_e, d, P.ge_p};
     GPS_TRY(wfork(st));
-    GPS_TRY(linear_wgrad(P.g_e, d, a->edge_attr, d, E, d, d, a->gcn_C.grad_weight, a->gcn_C.grad_bias, prec, s2, P.ge_p, P.e_p));
-    if (sp != st) GPS_TRY(sd->order(sp, s2));   // the mlp_r_ij gradients are final at ev_grads_mid; grad_pe joins at the end
+    GPS_TRY(linear_wgrad(P, g_e, {a->edge_attr, d, P.e_p}, E, d, d, a->gcn_C.grad_weight, a->gcn_C.grad_bias, s2));
+    if (P.eslap) GPS_TRY(sd->order(se, s2));   // the mlp_r_ij gradients are final at ev_grads_mid; grad_pe joins at the end
     GPS_TRY(mid_done());
     if (a->grad_edge_attr && E > 0) {
-      GemmParams g;
-      g.M = (int)E; g.N = (int)d; g.K = (int)d;
-      g.A = P.g_e; g.lda = (int)d; g.B = a->gcn_C.weight; g.ldb = (int)d; g.tb = 1; g.C = a->grad_edge_attr; g.ldc = (int)d;
-      g.R1 = a->grad_edge_out; g.ldr1 = (int)d; g.precision = prec;
-      g.Ap = P.ge_p; g.Bp = P.C_p;
+      GemmParams g = linear_dgrad(P, E, d, d, g_e, {a->gcn_C.weight, d, P.C_p}, a->grad_edge_attr, d);
+      g.R1 = a->grad_edge_out; g.ldr1 = (int)d;
       GPS_TRY(gemm(g, st));
     }
     g_x_local = P.g_xloc;  // residual x_in + ...
   } else if (P.gine) {
     // x_loc = x + drop(h1 W1^T + b1)
-    const float* g_l1 = P.g_xloc;
-    Planes g_l1_p = P.gl1_p;
-    if (pd > 0.f) {
-      GPS_TRY(dropmul(P.g_xloc, P.g_tmp3, N, d, P, a, GPS_SITE_LOCAL, st, 0.f, 0, P.gtmp3_p));
-      g_l1 = P.g_tmp3;
-      g_l1_p = P.gtmp3_p;
-    }
-    GemmParams g;  // g_h1 = (g_l1 W1) * act'(pre)
-    g.M = (int)N; g.N = (int)d; g.K = (int)d;
-    g.A = g_l1; g.lda = (int)d; g.B = a->gine_lin1.weight; g.ldb = (int)d; g.tb = 1; g.C = P.g_h1; g.ldc = (int)d;
-    if (relu) { g.mask_src = P.h1; g.mask_is_post = 1; } else { g.mask_src = P.h1_pre; g.mask_act = act; }
-    g.ldmask = (int)d; g.precision = prec;
-    g.Ap = g_l1_p; g.Bp = P.g1_p; g.Cp = P.gh1_p;
+    Operand g_l1;
+    GPS_TRY(dropmul(P, {P.g_xloc, d, P.gl1_p}, P.g_tmp3, P.gtmp3_p, GPS_SITE_LOCAL, st, &g_l1));
+    // g_h1 = (g_l1 W1) * act'(pre)
+    GemmParams g = linear_dgrad(P, N, d, d, g_l1, {a->gine_lin1.weight, d, P.g1_p}, P.g_h1, d);
+    set_act_mask(g, act, P.h1, P.h1_pre, d);
+    g.Cp = P.gh1_p;
     GPS_TRY(gemm(g, st));
+    const Operand g_h1{P.g_h1, d, P.gh1_p};
     GPS_TRY(wfork(st));
-    GPS_TRY(linear_wgrad(g_l1, d, P.h1, d, N, d, d, a->gine_lin1.grad_weight, a->gine_lin1.grad_bias, prec, s2, g_l1_p, P.h1_p));
-    GPS_TRY(linear_wgrad(P.g_h1, d, P.agg, d, N, d, d, a->gine_lin0.grad_weight, a->gine_lin0.grad_bias, prec, s2, P.gh1_p, P.agg_p));
+    GPS_TRY(linear_wgrad(P, g_l1, {P.h1, d, P.h1_p}, N, d, d, a->gine_lin1.grad_weight, a->gine_lin1.grad_bias, s2));
+    GPS_TRY(linear_wgrad(P, g_h1, {P.agg, d, P.agg_p}, N, d, d, a->gine_lin0.grad_weight, a->gine_lin0.grad_bias, s2));
     GPS_TRY(mid_done());
-    GemmParams g2;  // g_agg = g_h1 W0
-    g2.M = (int)N; g2.N = (int)d; g2.K = (int)d;
-    g2.A = P.g_h1; g2.lda = (int)d; g2.B = a->gine_lin0.weight; g2.ldb = (int)d; g2.tb = 1; g2.C = P.g_agg; g2.ldc = (int)d;
-    g2.precision = prec;
-    g2.Ap = P.gh1_p; g2.Bp = P.g0_p;
-    GPS_TRY(gemm(g2, st));
+    // g_agg = g_h1 W0
+    GPS_TRY(gemm(linear_dgrad(P, N, d, d, g_h1, {a->gine_lin0.weight, d, P.g0_p}, P.g_agg, d), st));
     GPS_REQUIRE(a->grad_edge_attr || E == 0, GPS_ERR_ARG, "grad_edge_attr is required for GINE");
     GPS_TRY(gine_bwd_dst(a->graph, d, a->x, a->edge_attr, P.g_agg, a->grad_edge_attr, st));
     GPS_TRY(gine_bwd_src(a->graph, d, a->grad_edge_attr, P.g_agg, a->gine_eps, P.g_xloc, P.g_xl, st));
     g_x_local = P.g_xl;
   } else if (P.gcn) {
     // x_loc = x + drop(b + A_hat Y): g_h = drop * g_xloc; g_b = colsum(g_h); gY = A_hat^T g_h -> gY1[:, 0:d]
-    const float* g_h = P.g_xloc;
-    if (pd > 0.f) {
-      GPS_TRY(dropmul(P.g_xloc, P.g_tmp3, N, d, P, a, GPS_SITE_LOCAL, st));
-      g_h = P.g_tmp3;
-    }
+    Operand g_h;
+    GPS_TRY(dropmul(P, {P.g_xloc, d}, P.g_tmp3, Planes(), GPS_SITE_LOCAL, st, &g_h));
     if (a->gcn_conv.grad_bias) {
-      if (!g_grads_prezeroed) GPS_CUDA(cudaMemsetAsync(a->gcn_conv.grad_bias, 0, (size_t)d * sizeof(float), st));
-      GPS_TRY(colsum(g_h, d, N, d, a->gcn_conv.grad_bias, st));
+      if (!P.grads_prezeroed) GPS_CUDA(cudaMemsetAsync(a->gcn_conv.grad_bias, 0, (size_t)d * sizeof(float), st));
+      GPS_TRY(colsum(g_h.f, d, N, d, a->gcn_conv.grad_bias, st));
     }
-    GPS_TRY(gcn_bwd(a->graph, d, g_h, P.dinv, P.gY1, P.Wy, st, P.gY1_p));
+    GPS_TRY(gcn_bwd(a->graph, d, g_h.f, P.dinv, P.gY1, P.Wy, st, P.gY1_p));
     GPS_TRY(wfork(st));
     GPS_TRY(mid_done());
     g_x_local = P.g_xloc;
   }
 
-  if (two_branches && sd) GPS_TRY(sd->order(sa, st));
+  if (two_branches) GPS_TRY(sd->order(sa, st));
 
   // ---- g_x = [local paths] + [attention residual] + gY1 Wcat ;  d{A,B,D,E,in_proj}
   if (P.Wy) {
+    const Operand gY1{P.gY1, P.Wy, P.gY1_p};
     GPS_TRY(wfork(st));
-    GemmParams w;   // d Wcat (+ bias gradient) on s2, unpacked into the caller's A, B, D, E / conv / in_proj gradients
-    w.M = (int)P.Wy; w.N = (int)d; w.K = (int)N;
-    w.A = P.gY1; w.lda = (int)P.Wy; w.ta = 1; w.B = a->x; w.ldb = (int)d; w.tb = 1; w.C = P.gWcat; w.ldc = (int)d;
-    w.splitk = splitk_for(N, P.Wy, d) < 2 ? 2 : splitk_for(N, P.Wy, d);
-    w.colsum_a = P.gbcat; w.precision = prec;
-    w.Ap = P.gY1_p; w.Bp = P.x_p;
-    if (prec == GPS_PREC_BF16 && w.Ap.hi && N > 0) {   // exact bias gradients in bf16 mode (see linear_wgrad)
-      w.colsum_a = nullptr;
-      GPS_TRY(colsum(P.gY1, P.Wy, N, P.Wy, P.gbcat, s2));
-    }
-    if (N > 0) GPS_TRY(gemm(w, s2));
-    PackDesc pdsc = pack_desc(a, P);
-    k_unpack<<<(unsigned)P.Wy, 128, 0, s2>>>(pdsc, P.gWcat, P.gbcat, g_grads_accumulate ? 1 : 0);
+    // d Wcat (+ bias gradient) on s2, unpacked into the caller's A, B, D, E / conv / in_proj gradients
+    GPS_TRY(wgrad_add(P, gY1, {a->x, d, P.x_p}, N, P.Wy, d, P.gWcat, P.gbcat, s2));
+    PackDesc pdsc = pack_desc(P);
+    k_unpack<<<(unsigned)P.Wy, 128, 0, s2>>>(pdsc, P.gWcat, P.gbcat, P.grads_accumulate ? 1 : 0);
     GPS_LAUNCH_CHECK();
-    GemmParams g;
-    g.M = (int)N; g.N = (int)d; g.K = (int)P.Wy;
-    g.A = P.gY1; g.lda = (int)P.Wy; g.B = P.Wcat; g.ldb = (int)d; g.tb = 1; g.C = a->grad_x; g.ldc = (int)d;
+    GemmParams g = linear_dgrad(P, N, d, P.Wy, gY1, {P.Wcat, d, P.Wcat_p}, a->grad_x, d);
     g.R1 = g_x_local; g.ldr1 = (int)d;
     g.R2 = P.attn ? P.g_hA : (P.perf ? P.g_xp : nullptr); g.ldr2 = (int)d;
-    g.precision = prec;
     if (gx_splitk) g.splitk = 4;   // long reduction, few output tiles: split-K fills the machine (grad_x zeroed above)
-    g.Ap = P.gY1_p; g.Bp = P.Wcat_p;
     GPS_TRY(gemm(g, st));
   } else if (g_x_local) {
     GPS_TRY(add3(g_x_local, d, P.perf ? P.g_xp : nullptr, d, nullptr, 0, a->grad_x, d, N, d, st));
   } else {
     GPS_TRY(add3(P.g_xp, d, nullptr, 0, nullptr, 0, a->grad_x, d, N, d, st));   // Performer only
   }
-  if (sd) GPS_TRY(sd->join(st));
+  GPS_TRY(sd->join(st));
   GPS_TRY(record_ev(a->ev_grads_done, st));
-  return GPS_OK;
-}
-
-// ---- dropout-only pass: reuse the BN-apply skeleton with an identity BatchNorm is overkill; a
-// dedicated tiny kernel keeps it explicit.
-namespace {
-__global__ void k_dropmul(const float* __restrict__ src, float* __restrict__ dst, int64_t n4, int64_t c4n, float p,
-                          uint64_t seed, uint64_t offset, int site, const unsigned long long* offset_dev, float p2,
-                          int site2, Planes dstp) {
-  if (offset_dev) offset += *offset_dev;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 v = ld4(src + i * 4);
-    if (p > 0.f) v = f4mul(v, dropout_scale4(p, seed, offset, site, (uint64_t)i));
-    if (p2 > 0.f) v = f4mul(v, dropout_scale4(p2, seed, offset, site2, (uint64_t)i));
-    st4(dst + i * 4, v);
-    if (dstp.hi) planes_store4(dstp, i / c4n, (i % c4n) * 4, v);
-  }
-}
-__global__ void k_dropmask(float* __restrict__ dst, int64_t n4, float p, uint64_t seed, uint64_t offset, int site) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 s = dropout_scale4(p, seed, offset, site, (uint64_t)i);
-    st4(dst + i * 4, make_float4(s.x > 0.f ? 1.f : 0.f, s.y > 0.f ? 1.f : 0.f, s.z > 0.f ? 1.f : 0.f,
-                                 s.w > 0.f ? 1.f : 0.f));
-  }
-}
-}  // namespace
-
-static int dropmul(const float* src, float* dst, int64_t rows, int64_t d, const Plan&, const GpsLayerArgs* a, int site,
-                   cudaStream_t st, float p2, int site2, Planes dstp) {
-  int64_t n4 = rows * d / 4;
-  if (n4 == 0) return GPS_OK;
-  k_dropmul<<<(unsigned)std::min<int64_t>(ceil_div(n4, 256), kNumSMs * 8), 256, 0, st>>>(src, dst, n4, d / 4, a->dropout,
-                                                                                        a->seed, a->offset, site,
-                                                                                        (const unsigned long long*)a->offset_dev,
-                                                                                        p2, site2, dstp);
-  GPS_LAUNCH_CHECK();
   return GPS_OK;
 }
 

@@ -217,8 +217,8 @@ typedef struct {
   int64_t saved_bytes;          /* activations kept for backward (0 needed if eval-only) */
   int64_t fwd_workspace_bytes;
   int64_t bwd_workspace_bytes;
-  int64_t fwd_launches;         /* kernels the forward enqueues  */
-  int64_t bwd_launches;         /* kernels the backward enqueues */
+  int64_t fwd_launches;         /* reserved, always 0 */
+  int64_t bwd_launches;         /* reserved, always 0 */
   int64_t wplanes_bytes;        /* ABI 3: size of the optional persistent weight-plane buffer (GpsLayerArgs.wplanes) */
 } GpsLayerPlan;
 
