@@ -18,6 +18,7 @@ LOCAL = {"None": 0, "CustomGatedGCN": 1, "GINE": 2, "GCN": 3}
 GLOBAL = {"None": 0, "Transformer": 1, "Performer": 2}
 ACT = {"relu": 0, "gelu": 1}
 PRECISION = {"fp32": 0, "bf16": 1}
+NORM = {"batch": 0, "none": 1}
 
 _fp = C.c_void_p  # device pointers travel as void*
 
@@ -48,7 +49,7 @@ class GpsLayerArgs(C.Structure):
         ("training", C.c_int32), ("precision", C.c_int32), ("reserved0", C.c_int32),
         ("dropout", C.c_float), ("attn_dropout", C.c_float),
         ("seed", C.c_uint64), ("offset", C.c_uint64),
-        ("gine_eps", C.c_float), ("reserved1", C.c_int32),
+        ("gine_eps", C.c_float), ("norm_type", C.c_int32),   # NORM (formerly reserved1)
         ("graph", GpsGraph),
         ("x", _fp), ("edge_attr", _fp), ("x_out", _fp), ("edge_out", _fp),
         ("gcn_A", GpsLinear), ("gcn_B", GpsLinear), ("gcn_C", GpsLinear), ("gcn_D", GpsLinear),

@@ -6,6 +6,8 @@
 //   pack W -> [Ax|Bx|Dx|Ex|Q|K|V] = x Wcat^T -> Ce = e C^T -> segmented gather-reduce (+BN stats)
 //   -> x_loc = x + act(BN(x~)) (+stats), e_out = e + act(BN(e^)) -> attention -> hA = x + O Wo^T (+stats)
 //   -> s = BN(x_loc) + BN(hA) -> FFN (+stats) -> BN.
+// Without normalisation (GPS_NORM_NONE, batch_norm=False): the local branch joins the attention branch before the output
+// projection, whose epilogue writes s = x + hA' + x_loc; the FF2 epilogue writes x_out = s + FFN(s).
 // Training-mode BatchNorm: the producer accumulates column sums, and the consumer kernel finalises the statistics from
 // them and normalises (BnView mode 1), so no launch sits between the two.
 #include <stdarg.h>
@@ -218,6 +220,11 @@ struct LayerWeight {
 struct Plan {
   int64_t N, E, d, H, hd, Wy, qkv_off;
   bool gated, gine, gcn, attn, perf;
+  // GPS_NORM_NONE: no norm1_local / norm1_attn / norm2.  Only the local model's own BatchNorms (BN_X, BN_E) remain, so
+  // nbn = 2 statistics slots instead of BN_COUNT; s = x_loc + hA is written by the GEMM that closes the second branch
+  // and x_out by the FF2 GEMM.
+  bool nonorm;
+  int nbn;
   int64_t inner, mp, m;   // Performer: H*64, padded / real feature count
   float *pQ, *pK, *pV, *pfq, *pfk, *pPn, *pgmax;   // saved (Performer)
   int *pargq, *pargk, *pnmax;
@@ -236,6 +243,7 @@ struct Plan {
   bool use_planes;
   Planes x_p, e_p, O_p, s_p, hid_p, agg_p, h1_p, Wcat_p, C_p, out_p, ff1_p, ff2_p, g0_p, g1_p, pq_p, pk_p, pv_p;
   Planes gt_p, ghid_p, ghA_p, ge_p, gY1_p, gtmp_p, gtmp2_p, gtmp3_p, gl1_p, gh1_p;
+  Planes gs_p;         // GPS_NORM_NONE: planes of g_s, the upstream gradient of both branches
   Planes qkv_p;        // Q | K | V per head, padded to hd_pad columns: operands of the wgmma attention
   bool attn_tc;        // softmax attention on the tensor cores (attention_tc.cu)
   // the weights with operand planes, in the order their planes are allocated and converted (list_weights)
@@ -341,6 +349,10 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   }
   GPS_REQUIRE(a->local_type != GPS_LOCAL_NONE || P->attn || P->perf, GPS_ERR_ARG,
               "GPSLayer needs a local model or a global model");
+  GPS_REQUIRE(a->norm_type == GPS_NORM_BATCH || a->norm_type == GPS_NORM_NONE, GPS_ERR_UNSUPPORTED,
+              "norm_type %d is not built (GPS_NORM_BATCH = 0, GPS_NORM_NONE = 1)", a->norm_type);
+  P->nonorm = a->norm_type == GPS_NORM_NONE;
+  P->nbn = P->nonorm ? BN_L : BN_COUNT;   // BN_X, BN_E come first
   if (P->attn) {
     GPS_REQUIRE(a->heads > 0 && a->d % a->heads == 0, GPS_ERR_ARG, "dim_h %% num_heads != 0");
     P->hd = a->d / a->heads;
@@ -363,7 +375,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   const bool gelu = a->act == GPS_ACT_GELU;
 
   Arena S(bind ? a->saved : nullptr, a->saved_bytes);
-  P->bnbuf = S.alloc<float>(BN_COUNT * 2 * d);
+  P->bnbuf = S.alloc<float>(P->nbn * 2 * d);
   if (P->Wy) {
     P->Wcat = S.alloc<float>(P->Wy * d);
     P->bcat = S.alloc<float>(P->Wy);
@@ -383,11 +395,12 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
     if (gelu) P->h1_pre = S.alloc<float>(N * d);
   }
   if (P->gcn) P->dinv = S.alloc<float>(N);
-  if (P->gated || P->gine || P->gcn) P->xloc = S.alloc<float>(N * d);
+  const bool loc = P->gated || P->gine || P->gcn;
+  if (loc && !P->nonorm) P->xloc = S.alloc<float>(N * d);   // read by norm1_local's backward
   if (P->attn) {
     P->O = S.alloc<float>(N * d);
     P->lse = S.alloc<float>(N * P->H);
-    P->hA = S.alloc<float>(N * d);
+    if (!P->nonorm) P->hA = S.alloc<float>(N * d);
   }
   if (P->perf) {
     const int64_t NH = N * P->H, BH = a->graph.B * P->H;
@@ -404,12 +417,12 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
     P->pden = S.alloc<float>(NH);
     P->perf_pairwise = a->graph.B > 0 && N <= 48 * a->graph.B;
     P->O = S.alloc<float>(N * P->inner);
-    P->hA = S.alloc<float>(N * d);
+    if (!P->nonorm) P->hA = S.alloc<float>(N * d);
   }
   P->s = S.alloc<float>(N * d);
   P->hid = S.alloc<float>(N * 2 * d);
   if (gelu) P->hid_pre = S.alloc<float>(N * 2 * d);
-  P->t = S.alloc<float>(N * d);
+  if (!P->nonorm) P->t = S.alloc<float>(N * d);   // norm2's input
   P->use_planes = (d % 8 == 0) && (!P->perf || P->inner % 8 == 0);
   const bool lo = a->precision == GPS_PREC_FP32;
   auto mkplanes = [&](Arena& A, int64_t rows, int64_t cols) {
@@ -459,12 +472,16 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
 
   // forward and backward share the caller's workspace (never live at the same time)
   Arena F(bind ? a->workspace : nullptr, a->workspace_bytes);
-  P->fstats = F.alloc<double>(BN_COUNT * 2 * d);
+  P->fstats = F.alloc<double>(P->nbn * 2 * d);
+  if (P->nonorm && loc) {
+    // x_loc is an operand of the GEMM that writes s (and of nothing in the backward pass); a lone local model writes s
+    P->xloc = (P->attn || P->perf) ? F.alloc<float>(N * d) : P->s;
+  }
   P->fwd_bytes = F.used;
 
   Arena Bk(bind ? a->workspace : nullptr, a->workspace_bytes);
-  P->bsums = Bk.alloc<double>(BN_COUNT * 2 * d);
-  P->g_t = Bk.alloc<float>(N * d);
+  P->bsums = Bk.alloc<double>(P->nbn * 2 * d);
+  if (!P->nonorm) P->g_t = Bk.alloc<float>(N * d);   // GPS_NORM_NONE: g_t is grad_x_out itself
   P->g_hid = Bk.alloc<float>(N * 2 * d);
   P->g_s = Bk.alloc<float>(N * d);
   P->g_tmp = Bk.alloc<float>(N * d);
@@ -472,15 +489,16 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
     P->g_tmp2 = Bk.alloc<float>(N * d);                            // gradients still read the earlier ones
     P->g_tmp3 = Bk.alloc<float>(N * d);
   }
-  if (P->gated || P->gine || P->gcn) P->g_xloc = Bk.alloc<float>(N * d);
+  // GPS_NORM_NONE: the upstream gradients of x_loc and hA are both g_s
+  if (loc && !P->nonorm) P->g_xloc = Bk.alloc<float>(N * d);
   if (P->attn) {
-    P->g_hA = Bk.alloc<float>(N * d);
+    if (!P->nonorm) P->g_hA = Bk.alloc<float>(N * d);
     P->g_O = Bk.alloc<float>(N * d);
     P->delta = Bk.alloc<float>(N * P->H);
   }
   if (P->perf) {
     const int64_t NH = N * P->H, BH = a->graph.B * P->H;
-    P->g_hA = Bk.alloc<float>(N * d);
+    if (!P->nonorm) P->g_hA = Bk.alloc<float>(N * d);
     P->g_O = Bk.alloc<float>(N * P->inner);
     P->g_pfq = Bk.alloc<float>(NH * P->mp);
     P->g_pfk = Bk.alloc<float>(NH * P->mp);
@@ -514,7 +532,8 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   if (P->use_planes) {
     P->gt_p = mkplanes(Bk, N, d);
     P->ghid_p = mkplanes(Bk, N, 2 * d);
-    if (P->attn || P->perf) P->ghA_p = mkplanes(Bk, N, d);
+    if ((P->attn || P->perf) && !P->nonorm) P->ghA_p = mkplanes(Bk, N, d);
+    if (P->nonorm) P->gs_p = mkplanes(Bk, N, d);
     if (P->gated) P->ge_p = mkplanes(Bk, E, d);
     if (P->Wy) P->gY1_p = mkplanes(Bk, N, P->Wy);
     if (a->dropout > 0.f || (P->perf && a->attn_dropout > 0.f)) {
@@ -523,7 +542,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
       P->gtmp3_p = mkplanes(Bk, N, d);
     }
     if (P->gine) {
-      P->gl1_p = mkplanes(Bk, N, d);
+      if (!P->nonorm) P->gl1_p = mkplanes(Bk, N, d);
       P->gh1_p = mkplanes(Bk, N, d);
     }
   }
@@ -605,11 +624,12 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
     GPS_TRY(check_linear(a->gine_lin1, "local_model.nn.2", true));
   }
   if (P.gcn) GPS_TRY(check_linear(a->gcn_conv, "local_model.lin / local_model.bias", true));
-  if (P.gated || P.gine || P.gcn) GPS_TRY(check_bn(a->norm1_local, "norm1_local"));
+  const bool bn = !P.nonorm;   // norm1_local / norm1_attn / norm2 exist in BatchNorm mode only
+  if ((P.gated || P.gine || P.gcn) && bn) GPS_TRY(check_bn(a->norm1_local, "norm1_local"));
   if (P.attn) {
     GPS_TRY(check_linear(a->attn_in, "self_attn.in_proj", true));
     GPS_TRY(check_linear(a->attn_out, "self_attn.out_proj", true));
-    GPS_TRY(check_bn(a->norm1_attn, "norm1_attn"));
+    if (bn) GPS_TRY(check_bn(a->norm1_attn, "norm1_attn"));
   }
   if (P.perf) {
     GPS_TRY(check_linear(a->perf_q, "self_attn.to_q", false));
@@ -617,11 +637,11 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
     GPS_TRY(check_linear(a->perf_v, "self_attn.to_v", false));
     GPS_TRY(check_linear(a->attn_out, "self_attn.to_out", true));
     GPS_REQUIRE(a->perf_proj, GPS_ERR_ARG, "missing buffer self_attn.fast_attention.projection_matrix");
-    GPS_TRY(check_bn(a->norm1_attn, "norm1_attn"));
+    if (bn) GPS_TRY(check_bn(a->norm1_attn, "norm1_attn"));
   }
   GPS_TRY(check_linear(a->ff1, "ff_linear1", true));
   GPS_TRY(check_linear(a->ff2, "ff_linear2", true));
-  GPS_TRY(check_bn(a->norm2, "norm2"));
+  if (bn) GPS_TRY(check_bn(a->norm2, "norm2"));
   return GPS_OK;
 }
 
@@ -741,16 +761,29 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
   GPS_REQUIRE(a->x_out, GPS_ERR_ARG, "x_out is null");
   const int64_t N = P.N, E = P.E, d = P.d;
   const int act = a->act;
-  auto stats = [&](int which) -> double* { return P.train ? P.fstats + (int64_t)which * 2 * d : nullptr; };
+  auto stats = [&](int which) -> double* { return P.train && which < P.nbn ? P.fstats + (int64_t)which * 2 * d : nullptr; };
   auto out_planes = [&](const GpsPlanes& g) {   // planes of this layer's outputs for the next layer of the stack
     return P.use_planes ? caller_planes(g, d, P.prec) : Planes();
   };
 
-  if (P.train) GPS_CUDA(cudaMemsetAsync(P.fstats, 0, (size_t)BN_COUNT * 2 * d * sizeof(double), st));
+  if (P.train) GPS_CUDA(cudaMemsetAsync(P.fstats, 0, (size_t)P.nbn * 2 * d * sizeof(double), st));
   Side* sd;
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
   const bool two_branches = (P.gated || P.gine || P.gcn) && (P.attn || P.perf);
+  // GPS_NORM_NONE: the producer that closes the last branch writes s = x_loc + hA with its planes (x_loc = s when the
+  // local model is alone)
+  const bool local_writes_s = P.nonorm && !(P.attn || P.perf);
+  // GPS_NORM_NONE, attention output projection on stream sg: writes s = x + drop(.) [+ x_loc] and its planes instead of
+  // hA; with a local branch, sg first waits for it
+  auto close_with_s = [&](GemmParams& g, cudaStream_t sg) -> int {
+    g.C = P.s; g.Cp = P.s_p;
+    if (two_branches) {
+      g.R2 = P.xloc; g.ldr2 = (int)d;
+      GPS_TRY(sd->order(st, sg));
+    }
+    return GPS_OK;
+  };
 
   // weights: concatenate the node projections
   if (P.Wy) {
@@ -833,6 +866,7 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     GemmParams g2 = linear_fwd(P, N, d, d, {P.h1, d, P.h1_p}, {a->gine_lin1.weight, d, P.g1_p}, P.xloc, d,
                                a->gine_lin1.bias);
     g2.R1 = a->x; g2.ldr1 = (int)d; g2.stats = stats(BN_L);
+    if (local_writes_s) g2.Cp = P.s_p;
     set_dropout(g2, P.drop(GPS_SITE_LOCAL));
     GPS_TRY(gemm(g2, st));
   } else if (P.gcn) {
@@ -840,6 +874,10 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     GPS_TRY(gcn_dinv(a->graph, P.dinv, st));
     GPS_TRY(gcn_fwd(a->graph, d, P.Y1, P.Wy, P.dinv, a->gcn_conv.bias, a->x, P.xloc, P.drop(GPS_SITE_LOCAL),
                     stats(BN_L), st));
+  }
+  if (local_writes_s && !P.gine && P.s_p.hi && N > 0) {   // the GatedGCN / GCN aggregation kernels write fp32 only
+    ToPlanesItem it{P.s, d, (int)N, (int)d, P.s_p};
+    GPS_TRY(to_planes(&it, 1, st));
   }
 
   // ---- global attention  (gps_layer.py:198-218, 234-241)
@@ -855,6 +893,7 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     GemmParams g = linear_fwd(P, N, d, d, {P.O, d, P.O_p}, {a->attn_out.weight, d, P.out_p}, P.hA, d, a->attn_out.bias);
     g.R1 = a->x; g.ldr1 = (int)d; g.stats = stats(BN_A);
     set_dropout(g, P.drop(GPS_SITE_ATTN_OUT));
+    if (P.nonorm) GPS_TRY(close_with_s(g, sg));
     GPS_TRY(gemm(g, sg));
   }
 
@@ -882,13 +921,14 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     // dropout=self.attn_dropout at gps_layer.py:112-114); GPSLayer.dropout_attn (p = dropout) follows (:212)
     set_dropout(g, P.drop(GPS_SITE_ATTN_OUT));
     g.p_drop2 = P.pa; g.site2 = GPS_SITE_PERF_OUT;
+    if (P.nonorm) GPS_TRY(close_with_s(g, sg));
     GPS_TRY(gemm(g, sg));
   }
 
   if (two_branches) GPS_TRY(sd->order(sd->s3, st));
 
   // ---- s = norm1_local(x_loc) + norm1_attn(hA)   (gps_layer.py:194,217,222)
-  {
+  if (!P.nonorm) {
     const bool loc = P.gated || P.gine || P.gcn;
     const float* first = loc ? P.xloc : P.hA;
     BnView bf = loc ? bn_view(P, BN_L, a->norm1_local, N) : bn_view(P, BN_A, a->norm1_attn, N);
@@ -907,9 +947,14 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
                                a->ff2.bias);
     g2.R1 = P.s; g2.ldr1 = (int)d; g2.stats = stats(BN_2);
     set_dropout(g2, P.drop(GPS_SITE_FF2));
+    if (P.nonorm) {   // x_out = t (no norm2)
+      g2.C = a->x_out;
+      g2.Cp = out_planes(a->x_planes_out);
+    }
     GPS_TRY(gemm(g2, st));
-    GPS_TRY(bn_combine(P.t, bn_view(P, BN_2, a->norm2, N), nullptr, BnView(), a->x_out, N, d, st,
-                       out_planes(a->x_planes_out)));  // :229
+    if (!P.nonorm)
+      GPS_TRY(bn_combine(P.t, bn_view(P, BN_2, a->norm2, N), nullptr, BnView(), a->x_out, N, d, st,
+                         out_planes(a->x_planes_out)));  // :229
   }
   return GPS_OK;
 }
@@ -927,7 +972,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   const int act = a->act;
   DropCfg nodrop;
   auto sums = [&](int which) { return P.bsums + (int64_t)which * 2 * d; };
-  GPS_CUDA(cudaMemsetAsync(P.bsums, 0, (size_t)BN_COUNT * 2 * d * sizeof(double), st));
+  GPS_CUDA(cudaMemsetAsync(P.bsums, 0, (size_t)P.nbn * 2 * d * sizeof(double), st));
   // weight-gradient GEMMs run on the side stream, each forked where its operands become final
   Side* sd;
   GPS_TRY(side_stream(&sd));
@@ -976,17 +1021,29 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     }
   }
 
-  // ---- norm2 (gps_layer.py:229): g_t
-  BnView v2 = bn_view(P, BN_2, a->norm2);
-  GPS_TRY(bn_bwd_reduce(a->grad_x_out, d, P.t, d, N, d, v2, -1, nodrop, sums(BN_2), st));
-  GPS_TRY(bn_bwd_apply(a->grad_x_out, d, P.t, d, N, d, v2, -1, nodrop, sums(BN_2), P.g_t, d, a->norm2.grad_weight,
-                       a->norm2.grad_bias, st, P.grads_accumulate, P.gt_p));
+  // ---- norm2 (gps_layer.py:229): g_t.  GPS_NORM_NONE: g_t = grad_x_out, whose planes the FF2 products read unless
+  // the dropout in front of them writes its own
+  const float* g_t = P.nonorm ? a->grad_x_out : P.g_t;
+  if (!P.nonorm) {
+    BnView v2 = bn_view(P, BN_2, a->norm2);
+    GPS_TRY(bn_bwd_reduce(a->grad_x_out, d, P.t, d, N, d, v2, -1, nodrop, sums(BN_2), st));
+    GPS_TRY(bn_bwd_apply(a->grad_x_out, d, P.t, d, N, d, v2, -1, nodrop, sums(BN_2), P.g_t, d, a->norm2.grad_weight,
+                         a->norm2.grad_bias, st, P.grads_accumulate, P.gt_p));
+  } else if (!(P.dropout.p > 0.f) && P.gt_p.hi && N > 0) {
+    ToPlanesItem it{g_t, d, (int)N, (int)d, P.gt_p};
+    GPS_TRY(to_planes(&it, 1, st));
+  }
+  // upstream gradients of x_loc and hA: norm1_local's / norm1_attn's input gradients, or g_s itself without them
+  const float* g_xloc = P.nonorm ? P.g_s : P.g_xloc;
+  const Planes g_xloc_p = P.nonorm ? P.gs_p : P.gl1_p;
+  const float* g_hA = P.nonorm ? P.g_s : P.g_hA;
+  const Planes g_hA_p = P.nonorm ? P.gs_p : P.ghA_p;
 
   bool fused_la = false;
   // ---- FFN (gps_layer.py:253-257)
   {
     Operand g_ff2;   // gradient at the output of ff_linear2 (after ff_dropout2)
-    GPS_TRY(dropmul(P, {P.g_t, d, P.gt_p}, P.g_tmp, P.gtmp_p, GPS_SITE_FF2, st, &g_ff2));
+    GPS_TRY(dropmul(P, {g_t, d, P.gt_p}, P.g_tmp, P.gtmp_p, GPS_SITE_FF2, st, &g_ff2));
     // g_hid = (g_ff2 W2) * act'(pre) * drop1
     GemmParams g = linear_dgrad(P, N, 2 * d, d, g_ff2, {a->ff2.weight, 2 * d, P.ff2_p}, P.g_hid, 2 * d);
     set_act_mask(g, act, P.hid, P.hid_pre, 2 * d);
@@ -999,10 +1056,11 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     GPS_TRY(linear_wgrad(P, g_hid, {P.s, d, P.s_p}, N, 2 * d, d, a->ff1.grad_weight, a->ff1.grad_bias, s2));
     // g_s = g_t + g_hid W1
     GemmParams g2 = linear_dgrad(P, N, d, 2 * d, g_hid, {a->ff1.weight, d, P.ff1_p}, P.g_s, d);
-    g2.R1 = P.g_t; g2.ldr1 = (int)d;
+    g2.R1 = g_t; g2.ldr1 = (int)d;
+    g2.Cp = P.gs_p;   // GPS_NORM_NONE only: the branches' products read g_s
     // norm1_local and norm1_attn both take g_s as their upstream gradient (gps_layer.py:194,217,222): their backward
     // reductions ride this GEMM's epilogue instead of two more passes over g_s (GPS_B200_OPT bit 64)
-    fused_la = (opt & 64) && P.use_planes && g2.Ap.hi && g2.Bp.hi && N > 0 && P.train;
+    fused_la = (opt & 64) && !P.nonorm && P.use_planes && g2.Ap.hi && g2.Bp.hi && N > 0 && P.train;
     if (fused_la) {
       if (P.gated || P.gine || P.gcn) {
         BnView v = bn_view(P, BN_L, a->norm1_local);
@@ -1021,7 +1079,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   const bool loc = P.gated || P.gine || P.gcn;
   bool chain_x = false;
   // ---- norm1_local / norm1_attn (gps_layer.py:194,217): g_xloc, g_hA
-  if (loc) {
+  if (loc && !P.nonorm) {
     BnView v = bn_view(P, BN_L, a->norm1_local);
     if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.xloc, d, N, d, v, -1, nodrop, sums(BN_L), st));
     chain_x = P.gated && N > 0 && (opt & 32) && P.train;
@@ -1039,13 +1097,15 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   }
   if (two_branches) GPS_TRY(sd->order(st, sa));   // attention-branch backward runs next to the local-model backward
   if (P.attn) {
-    BnView v = bn_view(P, BN_A, a->norm1_attn);
-    if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
-    GPS_TRY(bn_bwd_apply(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), P.g_hA, d, a->norm1_attn.grad_weight,
-                         a->norm1_attn.grad_bias, sa, P.grads_accumulate, P.ghA_p));
+    if (!P.nonorm) {
+      BnView v = bn_view(P, BN_A, a->norm1_attn);
+      if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
+      GPS_TRY(bn_bwd_apply(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), P.g_hA, d, a->norm1_attn.grad_weight,
+                           a->norm1_attn.grad_bias, sa, P.grads_accumulate, P.ghA_p));
+    }
     // hA = x + drop(O Wo^T + bo)
     Operand g_ao;
-    GPS_TRY(dropmul(P, {P.g_hA, d, P.ghA_p}, P.g_tmp2, P.gtmp2_p, GPS_SITE_ATTN_OUT, sa, &g_ao));
+    GPS_TRY(dropmul(P, {g_hA, d, g_hA_p}, P.g_tmp2, P.gtmp2_p, GPS_SITE_ATTN_OUT, sa, &g_ao));
     // g_O = g_ao Wo
     GPS_TRY(gemm(linear_dgrad(P, N, d, d, g_ao, {a->attn_out.weight, d, P.out_p}, P.g_O, d), sa));
     GPS_TRY(wfork(sa));
@@ -1060,12 +1120,14 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
 
   if (P.perf) {
     const int64_t inner = P.inner, NH = N * P.H, dh = a->perf_dim_head;
-    BnView v = bn_view(P, BN_A, a->norm1_attn);
-    if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
-    GPS_TRY(bn_bwd_apply(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), P.g_hA, d, a->norm1_attn.grad_weight,
-                         a->norm1_attn.grad_bias, sa, P.grads_accumulate));
+    if (!P.nonorm) {
+      BnView v = bn_view(P, BN_A, a->norm1_attn);
+      if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
+      GPS_TRY(bn_bwd_apply(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), P.g_hA, d, a->norm1_attn.grad_weight,
+                           a->norm1_attn.grad_bias, sa, P.grads_accumulate));
+    }
     Operand g_ao;   // hA = x + drop_pd(drop_pa(to_out(O)))
-    GPS_TRY(dropmul(P, {P.g_hA, d}, P.g_tmp2, Planes(), GPS_SITE_ATTN_OUT, sa, &g_ao, P.pa, GPS_SITE_PERF_OUT));
+    GPS_TRY(dropmul(P, {g_hA, d}, P.g_tmp2, Planes(), GPS_SITE_ATTN_OUT, sa, &g_ao, P.pa, GPS_SITE_PERF_OUT));
     // g_O = g_ao Wout   [N, inner]
     GPS_TRY(gemm(linear_dgrad(P, N, inner, d, g_ao, {a->attn_out.weight, inner}, P.g_O, inner), sa));
     GPS_TRY(wfork(sa));
@@ -1094,7 +1156,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     for (int i = 0; i < 3; ++i) {
       GPS_TRY(linear_wgrad(P, {gsrc[i], inner}, {a->x, d}, N, inner, d, lin[i]->grad_weight, nullptr, s2));
       GemmParams h = linear_dgrad(P, N, d, inner, {gsrc[i], inner}, {lin[i]->weight, d}, P.g_xp, d);
-      h.R1 = i == 0 ? P.g_hA : P.g_xp; h.ldr1 = (int)d;
+      h.R1 = i == 0 ? g_hA : P.g_xp; h.ldr1 = (int)d;
       GPS_TRY(gemm(h, sa));
     }
   }
@@ -1105,8 +1167,8 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     // x_loc = x + drop(act(BN_x(x~))): g_x~ -> gY1[:, 0:d]  (gatedgcn_layer.py:72-83)
     BnView vx = bn_view(P, BN_X, a->bn_node_x);
     if (!chain_x)
-      GPS_TRY(bn_bwd_reduce(P.g_xloc, d, P.xt, d, N, d, vx, act, P.drop(GPS_SITE_GCN_X), sums(BN_X), st));
-    GPS_TRY(bn_bwd_apply(P.g_xloc, d, P.xt, d, N, d, vx, act, P.drop(GPS_SITE_GCN_X), sums(BN_X), P.gY1, P.Wy,
+      GPS_TRY(bn_bwd_reduce(g_xloc, d, P.xt, d, N, d, vx, act, P.drop(GPS_SITE_GCN_X), sums(BN_X), st));
+    GPS_TRY(bn_bwd_apply(g_xloc, d, P.xt, d, N, d, vx, act, P.drop(GPS_SITE_GCN_X), sums(BN_X), P.gY1, P.Wy,
                          a->bn_node_x.grad_weight, a->bn_node_x.grad_bias, st, P.grads_accumulate, P.gY1_p));
     GPS_TRY(sd->order(se, st));
     // message/aggregate backward (SURVEY Appendix C)
@@ -1134,11 +1196,11 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
       g.R1 = a->grad_edge_out; g.ldr1 = (int)d;
       GPS_TRY(gemm(g, st));
     }
-    g_x_local = P.g_xloc;  // residual x_in + ...
+    g_x_local = g_xloc;  // residual x_in + ...
   } else if (P.gine) {
     // x_loc = x + drop(h1 W1^T + b1)
     Operand g_l1;
-    GPS_TRY(dropmul(P, {P.g_xloc, d, P.gl1_p}, P.g_tmp3, P.gtmp3_p, GPS_SITE_LOCAL, st, &g_l1));
+    GPS_TRY(dropmul(P, {g_xloc, d, g_xloc_p}, P.g_tmp3, P.gtmp3_p, GPS_SITE_LOCAL, st, &g_l1));
     // g_h1 = (g_l1 W1) * act'(pre)
     GemmParams g = linear_dgrad(P, N, d, d, g_l1, {a->gine_lin1.weight, d, P.g1_p}, P.g_h1, d);
     set_act_mask(g, act, P.h1, P.h1_pre, d);
@@ -1153,12 +1215,12 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     GPS_TRY(gemm(linear_dgrad(P, N, d, d, g_h1, {a->gine_lin0.weight, d, P.g0_p}, P.g_agg, d), st));
     GPS_REQUIRE(a->grad_edge_attr || E == 0, GPS_ERR_ARG, "grad_edge_attr is required for GINE");
     GPS_TRY(gine_bwd_dst(a->graph, d, a->x, a->edge_attr, P.g_agg, a->grad_edge_attr, st));
-    GPS_TRY(gine_bwd_src(a->graph, d, a->grad_edge_attr, P.g_agg, a->gine_eps, P.g_xloc, P.g_xl, st));
+    GPS_TRY(gine_bwd_src(a->graph, d, a->grad_edge_attr, P.g_agg, a->gine_eps, g_xloc, P.g_xl, st));
     g_x_local = P.g_xl;
   } else if (P.gcn) {
     // x_loc = x + drop(b + A_hat Y): g_h = drop * g_xloc; g_b = colsum(g_h); gY = A_hat^T g_h -> gY1[:, 0:d]
     Operand g_h;
-    GPS_TRY(dropmul(P, {P.g_xloc, d}, P.g_tmp3, Planes(), GPS_SITE_LOCAL, st, &g_h));
+    GPS_TRY(dropmul(P, {g_xloc, d}, P.g_tmp3, Planes(), GPS_SITE_LOCAL, st, &g_h));
     if (a->gcn_conv.grad_bias) {
       if (!P.grads_prezeroed) GPS_CUDA(cudaMemsetAsync(a->gcn_conv.grad_bias, 0, (size_t)d * sizeof(float), st));
       GPS_TRY(colsum(g_h.f, d, N, d, a->gcn_conv.grad_bias, st));
@@ -1166,7 +1228,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     GPS_TRY(gcn_bwd(a->graph, d, g_h.f, P.dinv, P.gY1, P.Wy, st, P.gY1_p));
     GPS_TRY(wfork(st));
     GPS_TRY(mid_done());
-    g_x_local = P.g_xloc;
+    g_x_local = g_xloc;
   }
 
   if (two_branches) GPS_TRY(sd->order(sa, st));
@@ -1182,7 +1244,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     GPS_LAUNCH_CHECK();
     GemmParams g = linear_dgrad(P, N, d, P.Wy, gY1, {P.Wcat, d, P.Wcat_p}, a->grad_x, d);
     g.R1 = g_x_local; g.ldr1 = (int)d;
-    g.R2 = P.attn ? P.g_hA : (P.perf ? P.g_xp : nullptr); g.ldr2 = (int)d;
+    g.R2 = P.attn ? g_hA : (P.perf ? P.g_xp : nullptr); g.ldr2 = (int)d;
     if (gx_splitk) g.splitk = 4;   // long reduction, few output tiles: split-K fills the machine (grad_x zeroed above)
     GPS_TRY(gemm(g, st));
   } else if (g_x_local) {

@@ -339,16 +339,19 @@ class GPSLayer(nn.Module):
 
         if self.layer_norm and self.batch_norm:
             raise ValueError("Cannot apply two types of normalization together")   # gps_layer.py:125-126
-        if self.layer_norm or not self.batch_norm:
-            raise NotImplementedError("graphgps_b200 builds the BatchNorm configuration "
-                                      "(layer_norm=False, batch_norm=True) used by every shipped config")
+        if self.layer_norm:
+            raise NotImplementedError("graphgps_b200 does not build PyG graph LayerNorm (layer_norm=True); "
+                                      "batch_norm=True and batch_norm=False are built")
         if self.local_model is None and self.self_attn is None:
             raise ValueError("GPSLayer needs a local model or a global model")
-        self.norm1_local = nn.BatchNorm1d(dim_h)
-        self.norm1_attn = nn.BatchNorm1d(dim_h)
+        # batch_norm=False: norm1_local / norm1_attn / norm2 do not exist, as in the reference (gps_layer.py:128-151)
+        if self.batch_norm:
+            self.norm1_local = nn.BatchNorm1d(dim_h)
+            self.norm1_attn = nn.BatchNorm1d(dim_h)
         self.ff_linear1 = nn.Linear(dim_h, dim_h * 2)
         self.ff_linear2 = nn.Linear(dim_h * 2, dim_h)
-        self.norm2 = nn.BatchNorm1d(dim_h)
+        if self.batch_norm:
+            self.norm2 = nn.BatchNorm1d(dim_h)
         self._param_names = [n for n, _ in self.named_parameters()]
         self._grad_shapes = [tuple(p.shape) for _, p in self.named_parameters()]
         self._grad_sizes = [p.numel() for _, p in self.named_parameters()]
@@ -476,6 +479,7 @@ class GPSLayer(nn.Module):
         a.training = 1 if self.training else 0
         a.precision = _lib.PRECISION[self.precision]
         a.dropout, a.attn_dropout = float(self.dropout), float(self.attn_dropout)
+        a.norm_type = _lib.NORM["batch" if self.batch_norm else "none"]
 
         def lin(prefix, bias=True):
             return _lin(named[prefix + ".weight"], named.get(prefix + ".bias") if bias else None,
@@ -511,9 +515,10 @@ class GPSLayer(nn.Module):
             a.attn_out = lin("self_attn.to_out")
             pm = self.self_attn.fast_attention.projection_matrix
             a.perf_proj, a.perf_features, a.perf_dim_head = pm.data_ptr(), pm.shape[0], pm.shape[1]
-        a.norm1_local = bn("norm1_local", self.norm1_local)
-        a.norm1_attn = bn("norm1_attn", self.norm1_attn)
-        a.norm2 = bn("norm2", self.norm2)
+        if self.batch_norm:   # else the three structs stay zero: the library does not read them
+            a.norm1_local = bn("norm1_local", self.norm1_local)
+            a.norm1_attn = bn("norm1_attn", self.norm1_attn)
+            a.norm2 = bn("norm2", self.norm2)
         a.ff1, a.ff2 = lin("ff_linear1"), lin("ff_linear2")
         return a
 

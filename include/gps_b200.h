@@ -43,6 +43,8 @@ enum { GPS_ACT_RELU = 0, GPS_ACT_GELU = 1 };
 /* arithmetic of the dense products: FP32 = fp32-grade result (split-bf16 x3 on the tensor cores,
  * tolerance 1e-3 vs the reference); BF16 = single bf16 pass, fp32 accumulate (tolerance 1e-2) */
 enum { GPS_PREC_FP32 = 0, GPS_PREC_BF16 = 1 };
+/* GpsLayerArgs.norm_type: cfg.gt.batch_norm = True / False with cfg.gt.layer_norm = False (gps_layer.py:125-151) */
+enum { GPS_NORM_BATCH = 0, GPS_NORM_NONE = 1 };
 
 const char* gps_last_error(void);
 int gps_abi_version(void);
@@ -137,7 +139,12 @@ typedef struct {
   uint64_t seed;             /* Philox key for this call's dropout masks            */
   uint64_t offset;           /* Philox counter base (caller advances per call)      */
   float gine_eps;            /* local_model.eps buffer value (GINE)                 */
-  int32_t reserved1;
+  /* ABI 3 (formerly reserved1, zero in every earlier caller): normalisation of the GPSLayer (gps_layer.py:125-151,
+   * 191-229), GPS_NORM_*.  BATCH: norm1_local, norm1_attn and norm2 are BatchNorm1d.  NONE (batch_norm=False,
+   * layer_norm=False): the three modules do not exist and are not read; x_loc = x + local(x), hA = x + MHA(x),
+   * s = x_loc + hA, x_out = s + FFN(s).  GatedGCN's bn_node_x / bn_edge_e belong to the local model and are required
+   * in both modes.  Any other value makes gps_layer_plan / _forward / _backward return GPS_ERR_UNSUPPORTED. */
+  int32_t norm_type;
 
   GpsGraph graph;
 
