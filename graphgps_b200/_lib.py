@@ -97,6 +97,18 @@ SYMBOLS = {
     "gps_gatedgcn_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _i64, _fp, _fp,
                                                  _fp, _fp, _fp]),
     "gps_gine_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _f32, _fp, _fp]),
+    "gps_gatedgcn_aggregate_forward_gated": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _i64, _fp, _fp,
+                                                       _fp, _fp, _fp, _fp]),
+    "gps_gatedgcn_aggregate_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _i64, _fp, _fp, _i64, _fp, _fp,
+                                                  _fp, C.POINTER(GpsPlanes), C.POINTER(GpsPlanes), _fp]),
+    "gps_eslap_forward": (C.c_int, [C.POINTER(GpsGraph), _fp, _i64, _i64, _i32, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    "gps_eslap_workspace_bytes": (_i64, [_i64, _i64]),
+    "gps_eslap_backward": (C.c_int, [C.POINTER(GpsGraph), _fp, _i64, _i64, _i32, _fp, _fp, _fp, _i64, _fp, _fp, _fp,
+                                     _fp, _fp, _fp, _fp, _i64, _fp, _fp, _fp, _fp, _fp, _i32, _fp]),
+    "gps_gine_aggregate_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _f32, _fp, _fp, _fp, _fp]),
+    "gps_gcn_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _i64, _fp, _fp, _fp, _fp, _f32, _u64, _u64,
+                                            _fp, _fp]),
+    "gps_gcn_aggregate_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _i64, C.POINTER(GpsPlanes), _fp]),
     "gps_attention_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _fp, _fp, _i64, _fp, _i64, _fp,
                                         _f32, _u64, _u64, _fp]),
     "gps_attention_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _fp, _fp, _i64, _fp, _fp, _i64,

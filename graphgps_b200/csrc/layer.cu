@@ -1356,8 +1356,118 @@ extern "C" int gps_gatedgcn_aggregate_forward(const GpsGraph* g, int64_t d, cons
 
 extern "C" int gps_gine_aggregate_forward(const GpsGraph* g, int64_t d, const float* x, const float* e, float eps,
                                           float* out, void* stream) {
-  GPS_REQUIRE(g && x && out, GPS_ERR_ARG, "gine_aggregate: null argument");
+  GPS_REQUIRE(g && x && out && (e || g->E == 0), GPS_ERR_ARG, "gine_aggregate: null argument");
   return gine_fwd(*g, d, x, e, eps, out, (cudaStream_t)stream);
+}
+
+// ---- stage entry points of the message-passing backward passes, the EquivStableLapPE gate and GCN.  Each validates
+// its arguments before it enqueues anything: the sparse kernels take d > 0, d % 4 == 0, d <= 4096 (scatter.cu,
+// node_geom), checked here up front because some of them launch a kernel before the first one that checks it.
+static int stage_width(int64_t d, const char* what) {
+  GPS_REQUIRE(d > 0 && d % 4 == 0 && d <= 4096, GPS_ERR_UNSUPPORTED, "%s needs d %% 4 == 0 and 0 < d <= 4096 (got %lld)",
+              what, (long long)d);
+  return GPS_OK;
+}
+// optional caller planes: hi == NULL means none; else a pitch that is a multiple of 8 and holds `cols` columns
+static int stage_planes(const GpsPlanes* p, int64_t cols, Planes* out, const char* what) {
+  *out = Planes();
+  if (!p || !p->hi) return GPS_OK;
+  GPS_REQUIRE(p->ld >= cols && p->ld % 8 == 0, GPS_ERR_ARG, "%s: plane pitch %lld must be a multiple of 8 and >= %lld",
+              what, (long long)p->ld, (long long)cols);
+  *out = Planes{(__nv_bfloat16*)p->hi, (__nv_bfloat16*)p->lo, p->ld};
+  return GPS_OK;
+}
+
+extern "C" int gps_gatedgcn_aggregate_forward_gated(const GpsGraph* g, int64_t d, const float* Ax, const float* Bx,
+                                                    const float* Dx, const float* Ex, int64_t ldy, float* Ce, float* xt,
+                                                    double* stats_x, double* stats_e, const float* rho, void* stream) {
+  GPS_REQUIRE(g && Ax && Bx && Dx && Ex && (Ce || g->E == 0) && xt, GPS_ERR_ARG, "gatedgcn_aggregate_gated: null argument");
+  GPS_TRY(stage_width(d, "gatedgcn_aggregate_gated"));
+  GPS_REQUIRE(ldy >= d, GPS_ERR_ARG, "gatedgcn_aggregate_gated: ldy < d");
+  return gatedgcn_fwd(*g, d, Ax, Bx, Dx, Ex, ldy, Ce, xt, stats_x, stats_e, (cudaStream_t)stream, rho);
+}
+
+extern "C" int gps_gatedgcn_aggregate_backward(const GpsGraph* g, int64_t d, const float* ehat, const float* Bx,
+                                               int64_t ldy, const float* rho, float* gY, int64_t ldg, float* g_e,
+                                               float* g_num, float* g_den, const GpsPlanes* gY_planes,
+                                               const GpsPlanes* g_e_planes, void* stream) {
+  GPS_REQUIRE(g && gY && g_num && (g->E == 0 || (ehat && Bx && g_e)) && (!rho || g_den), GPS_ERR_ARG,
+              "gatedgcn_aggregate_backward: null argument");
+  GPS_TRY(stage_width(d, "gatedgcn_aggregate_backward"));
+  GPS_REQUIRE(ldy >= d && ldg >= 4 * d, GPS_ERR_ARG, "gatedgcn_aggregate_backward: ldy < d or ldg < 4 d");
+  Planes yp, ep;
+  GPS_TRY(stage_planes(gY_planes, 4 * d, &yp, "gatedgcn_aggregate_backward gY_planes"));
+  GPS_TRY(stage_planes(g_e_planes, d, &ep, "gatedgcn_aggregate_backward g_e_planes"));
+  const cudaStream_t st = (cudaStream_t)stream;
+  // as layer_backward: block 0 of gY is g_xt; the passes write g_Dx (block 2), then g_Ex (block 3) and g_Bx (block 1)
+  GPS_TRY(gatedgcn_bwd_dst(*g, d, gY, ldg, ehat, Bx, ldy, g_e, g_num, gY + 2 * d, st, ep, yp.cols(2 * d), rho, g_den));
+  return gatedgcn_bwd_src(*g, d, g_e, ehat, g_num, gY + 3 * d, gY + d, ldg, st, yp.cols(3 * d), yp.cols(d), rho);
+}
+
+extern "C" int gps_eslap_forward(const GpsGraph* g, const float* pe, int64_t k, int64_t d, int32_t act, const float* w1,
+                                 const float* b1, const float* w2, const float* b2, float* r, float* rho, void* stream) {
+  GPS_REQUIRE(g && (g->E == 0 || (pe && w1 && b1 && w2 && b2 && r && rho)), GPS_ERR_ARG, "eslap_forward: null argument");
+  GPS_TRY(stage_width(d, "eslap_forward"));
+  GPS_REQUIRE(k >= 1 && (act == GPS_ACT_RELU || act == GPS_ACT_GELU), GPS_ERR_ARG, "eslap_forward: k < 1 or unknown act");
+  return eslap_fwd(*g, pe, k, d, act, w1, b1, w2, b2, r, rho, (cudaStream_t)stream);
+}
+
+// workspace of gps_eslap_backward: gz [E], gr [E], then part [ceil(E / chunk), 3d + 1] (floats)
+extern "C" int64_t gps_eslap_workspace_bytes(int64_t E, int64_t d) {
+  if (E <= 0) return 0;
+  return (2 * E + ceil_div(E, eslap_wgrad_chunk(E)) * (3 * d + 1)) * (int64_t)sizeof(float);
+}
+
+extern "C" int gps_eslap_backward(const GpsGraph* g, const float* pe, int64_t k, int64_t d, int32_t act,
+                                  const float* g_num, const float* g_den, const float* Bx, int64_t ldy, const float* ehat,
+                                  const float* r, const float* rho, const float* w1, const float* b1, const float* w2,
+                                  void* workspace, int64_t workspace_bytes, float* grad_pe, float* gw1, float* gb1,
+                                  float* gw2, float* gb2, int32_t accumulate, void* stream) {
+  const int64_t E = g ? g->E : 0;
+  GPS_REQUIRE(g && (E == 0 || (g_num && g_den && Bx && ehat && r && rho && w1 && b1 && w2 && workspace)) &&
+                  (pe || (E == 0 && !grad_pe)),
+              GPS_ERR_ARG, "eslap_backward: null argument");
+  GPS_TRY(stage_width(d, "eslap_backward"));
+  GPS_REQUIRE(k >= 1 && (act == GPS_ACT_RELU || act == GPS_ACT_GELU) && ldy >= d, GPS_ERR_ARG,
+              "eslap_backward: k < 1, unknown act or ldy < d");
+  GPS_REQUIRE(workspace_bytes >= gps_eslap_workspace_bytes(E, d), GPS_ERR_ARG, "eslap_backward: workspace too small");
+  float* ws = (float*)workspace;
+  float* gz = E > 0 ? ws : nullptr;
+  float* gr = E > 0 ? ws + E : nullptr;
+  float* part = E > 0 ? ws + 2 * E : nullptr;
+  return eslap_bwd(*g, pe, k, d, act, g_num, g_den, Bx, ldy, ehat, r, rho, w1, b1, w2, gz, gr, part, grad_pe, gw1, gb1,
+                   gw2, gb2, accumulate != 0, (cudaStream_t)stream);
+}
+
+extern "C" int gps_gine_aggregate_backward(const GpsGraph* g, int64_t d, const float* x, const float* e,
+                                           const float* g_out, float eps, const float* add, float* g_e, float* g_x,
+                                           void* stream) {
+  GPS_REQUIRE(g && g_out && g_x && (g->E == 0 || (x && e && g_e)), GPS_ERR_ARG, "gine_aggregate_backward: null argument");
+  GPS_TRY(stage_width(d, "gine_aggregate_backward"));
+  GPS_TRY(gine_bwd_dst(*g, d, x, e, g_out, g_e, (cudaStream_t)stream));
+  return gine_bwd_src(*g, d, g_e, g_out, eps, add, g_x, (cudaStream_t)stream);
+}
+
+extern "C" int gps_gcn_aggregate_forward(const GpsGraph* g, int64_t d, const float* Y, int64_t ldy, const float* bias,
+                                         const float* x, float* dinv, float* xloc, float p_drop, uint64_t seed,
+                                         uint64_t offset, double* stats, void* stream) {
+  GPS_REQUIRE(g && Y && bias && x && dinv && xloc, GPS_ERR_ARG, "gcn_aggregate_forward: null argument");
+  GPS_TRY(stage_width(d, "gcn_aggregate_forward"));
+  GPS_REQUIRE(ldy >= d && p_drop >= 0.f && p_drop < 1.f, GPS_ERR_ARG, "gcn_aggregate_forward: ldy < d or p_drop not in [0,1)");
+  DropCfg drop;
+  drop.p = p_drop; drop.seed = seed; drop.offset = offset; drop.site = GPS_SITE_LOCAL;
+  GPS_TRY(gcn_dinv(*g, dinv, (cudaStream_t)stream));
+  return gcn_fwd(*g, d, Y, ldy, dinv, bias, x, xloc, drop, stats, (cudaStream_t)stream);
+}
+
+extern "C" int gps_gcn_aggregate_backward(const GpsGraph* g, int64_t d, const float* g_h, const float* dinv, float* gY,
+                                          int64_t ldg, const GpsPlanes* gY_planes, void* stream) {
+  GPS_REQUIRE(g && g_h && dinv && gY, GPS_ERR_ARG, "gcn_aggregate_backward: null argument");
+  GPS_TRY(stage_width(d, "gcn_aggregate_backward"));
+  GPS_REQUIRE(ldg >= d, GPS_ERR_ARG, "gcn_aggregate_backward: ldg < d");
+  Planes yp;
+  GPS_TRY(stage_planes(gY_planes, d, &yp, "gcn_aggregate_backward gY_planes"));
+  return gcn_bwd(*g, d, g_h, dinv, gY, ldg, (cudaStream_t)stream, yp);
 }
 
 extern "C" int gps_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q, const float* K,

@@ -267,6 +267,48 @@ int gps_gatedgcn_aggregate_forward(const GpsGraph* g, int64_t d, const float* Ax
 int gps_gine_aggregate_forward(const GpsGraph* g, int64_t d, const float* x, const float* e,
                                float eps, float* out, void* stream);
 
+/* The stage entry points below take d > 0, d % 4 == 0, d <= 4096 (else GPS_ERR_UNSUPPORTED) and validate every pointer
+ * they read or write before any CUDA call (GPS_ERR_ARG); pointers that only edges use may be NULL when E == 0. */
+/* as gps_gatedgcn_aggregate_forward, plus rho [E] (NULL = no gate): sigma_ij = sigmoid(e_ij) * rho_e
+ * (EquivStableLapPE, gatedgcn_layer.py:101-104) */
+int gps_gatedgcn_aggregate_forward_gated(const GpsGraph* g, int64_t d, const float* Ax, const float* Bx,
+                                         const float* Dx, const float* Ex, int64_t ldy, float* Ce, float* xt,
+                                         double* stats_x, double* stats_e, const float* rho, void* stream);
+/* backward of the above: the dst-ordered pass, then the src-ordered pass.  gY [N, ldg] holds the column blocks
+ * [g_Ax | g_Bx | g_Dx | g_Ex]: block 0 holds g_xt on entry and is only read; blocks 1..3 are written.  g_e [E,d] holds
+ * the BN_e-path gradient on entry and the total gradient of e_ij on exit.  g_num [N,d] is written; g_den [N,d] is written
+ * when rho != NULL.  gY_planes (4d columns) / g_e_planes: optional bf16 hi/lo images of gY blocks 1..3 / g_e (hi NULL
+ * = none). */
+int gps_gatedgcn_aggregate_backward(const GpsGraph* g, int64_t d, const float* ehat, const float* Bx, int64_t ldy,
+                                    const float* rho, float* gY, int64_t ldg, float* g_e, float* g_num, float* g_den,
+                                    const GpsPlanes* gY_planes, const GpsPlanes* g_e_planes, void* stream);
+/* EquivStableLapPE gate (gatedgcn_layer.py:29-35,101-104): r [E] = |pe_i - pe_j|^2, rho [E] = mlp_r_ij(r); pe [N,k],
+ * w1 = mlp_r_ij.0.weight [d,1], b1 [d], w2 = mlp_r_ij.2.weight [1,d], b2 [1]; act GPS_ACT_* */
+int gps_eslap_forward(const GpsGraph* g, const float* pe, int64_t k, int64_t d, int32_t act, const float* w1,
+                      const float* b1, const float* w2, const float* b2, float* r, float* rho, void* stream);
+/* bytes of scratch gps_eslap_backward needs */
+int64_t gps_eslap_workspace_bytes(int64_t E, int64_t d);
+/* its backward, after gps_gatedgcn_aggregate_backward with rho: grad_pe [N,k] (NULL = not needed) and the mlp_r_ij
+ * gradients (each NULL = not needed), written, or added to when accumulate != 0 */
+int gps_eslap_backward(const GpsGraph* g, const float* pe, int64_t k, int64_t d, int32_t act, const float* g_num,
+                       const float* g_den, const float* Bx, int64_t ldy, const float* ehat, const float* r,
+                       const float* rho, const float* w1, const float* b1, const float* w2, void* workspace,
+                       int64_t workspace_bytes, float* grad_pe, float* gw1, float* gb1, float* gw2, float* gb2,
+                       int32_t accumulate, void* stream);
+/* backward of gps_gine_aggregate_forward: g_e [E,d] = g_out[dst] * [x_src + e > 0],
+ * g_x [N,d] = (1+eps) g_out + sum over out-edges of g_e (+ add [N,d], NULL = none) */
+int gps_gine_aggregate_backward(const GpsGraph* g, int64_t d, const float* x, const float* e, const float* g_out,
+                                float eps, const float* add, float* g_e, float* g_x, void* stream);
+/* GCN aggregation (gps_layer.py:49-51): dinv [N] = (1 + #non-self in-edges)^-1/2, then
+ * xloc = x + dropout(bias + A_hat Y) with the layer's local dropout site and (seed, offset) (gps_dropout_mask site 3);
+ * stats: optional double [2][d] column sums of xloc.  Y [N, ldy]. */
+int gps_gcn_aggregate_forward(const GpsGraph* g, int64_t d, const float* Y, int64_t ldy, const float* bias,
+                              const float* x, float* dinv, float* xloc, float p_drop, uint64_t seed, uint64_t offset,
+                              double* stats, void* stream);
+/* its backward: gY [N, ldg] = A_hat^T g_h (+ optional bf16 hi/lo planes of it) */
+int gps_gcn_aggregate_backward(const GpsGraph* g, int64_t d, const float* g_h, const float* dinv, float* gY,
+                               int64_t ldg, const GpsPlanes* gY_planes, void* stream);
+
 /* Dense softmax attention over each graph's own nodes — replaces to_dense_batch +
  * nn.MultiheadAttention core + [mask] (gps_layer.py:199-201,234-241) without padding.
  * Q,K,V: [N, heads*hd] slices with row stride ld; O [N, heads*hd] (row stride ldo); lse [N,heads]. */
