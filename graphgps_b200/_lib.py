@@ -109,6 +109,15 @@ SYMBOLS = {
     "gps_gcn_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _i64, _fp, _fp, _fp, _fp, _f32, _u64, _u64,
                                             _fp, _fp]),
     "gps_gcn_aggregate_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _i64, C.POINTER(GpsPlanes), _fp]),
+    "gps_performer_prep": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp]),
+    "gps_performer_features_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp,
+                                                 _fp, _fp]),
+    "gps_performer_attention_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _i32, _fp, _fp, _fp, _fp, _fp,
+                                                  _fp, _fp, _fp]),
+    "gps_performer_attention_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _i32, _fp, _fp, _fp, _fp,
+                                                   _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    "gps_performer_features_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _i32, _fp, _fp, _fp, _fp, _fp,
+                                                  _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     "gps_attention_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _fp, _fp, _i64, _fp, _i64, _fp,
                                         _f32, _u64, _u64, _fp]),
     "gps_attention_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _fp, _fp, _i64, _fp, _fp, _i64,

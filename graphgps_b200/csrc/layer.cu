@@ -24,6 +24,7 @@ namespace gps {
 // performer.cu
 int perf_supported(int64_t dim_head, int64_t features);
 int64_t perf_mp();
+int perf_index_range(int64_t N, int64_t H);
 int perf_prep(const float* P, int64_t m, float* Pn, const GpsGraph& g, int64_t H, int* nmax, float* gmax, int* argk,
               cudaStream_t st);
 int perf_features_fwd(float* fq, float* fk, const float* Q, const float* K, const GpsGraph& g, int64_t H, int64_t m,
@@ -35,14 +36,14 @@ int perf_linattn_bwd(const GpsGraph& g, int64_t H, int64_t m, const int* nmax, c
                      float* ggmax, cudaStream_t st);
 int perf_features_bwd(float* g_fq, float* g_fk, const float* fq, const float* fk, const float* Q, const float* K,
                       float* gQ, float* gK, const GpsGraph& g, int64_t H, int64_t m, const int* argq, const int* argk,
-                      float* ggmax, cudaStream_t st);
+                      const float* ggmax, float* gmrow, bool pairwise, cudaStream_t st);
 
 // performer_quad.cu (pairwise form for batches of small graphs)
 int perf_quad_fwd(const GpsGraph& g, int64_t H, int64_t m, const int* nmax, const float* qf, const float* kf,
                   const float* V, const float* gmax, float* O, float* den, cudaStream_t st);
 int perf_quad_bwd(const GpsGraph& g, int64_t H, int64_t m, const int* nmax, const float* qf, const float* kf,
                   const float* V, const float* gmax, const float* O, const float* den, const float* gO, float* gden,
-                  float* g_qf, float* g_kf, float* gV, float* ggmax, cudaStream_t st);
+                  float* g_qf, float* g_kf, float* gV, float* gmrow, cudaStream_t st);
 
 // ------------------------------------------------------------------------------- error plumbing
 static thread_local char g_err[512] = "";
@@ -231,6 +232,7 @@ struct Plan {
   float *pden, *g_pden;   // pairwise form: denominators (saved) and their gradients
   bool perf_pairwise;     // mean graph size <= 48: n^2 (m+64) < 2 n m 64
   float *g_pfq, *g_pfk, *g_pQ, *g_pK, *g_pV, *g_pgmax, *g_xp;   // backward workspace (Performer)
+  float* g_pgrow;         // [N*H] per-row stabiliser gradients, summed per (graph, head) in a fixed order
   // saved
   float *Wcat, *bcat, *Y1, *ehat, *xt, *xloc, *O, *lse, *hA, *s, *hid, *hid_pre, *t, *bnbuf;
   float *agg, *h1, *h1_pre;
@@ -343,6 +345,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   if (P->perf) {
     GPS_TRY(perf_supported(a->perf_dim_head, a->perf_features));
     GPS_REQUIRE(a->heads > 0, GPS_ERR_ARG, "num_heads must be positive");
+    GPS_TRY(perf_index_range(a->graph.N, a->heads));
     P->inner = a->heads * a->perf_dim_head;
     P->mp = perf_mp();
     P->m = a->perf_features;
@@ -506,6 +509,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
     P->g_pK = Bk.alloc<float>(N * P->inner);
     P->g_pV = Bk.alloc<float>(N * P->inner);
     P->g_pgmax = Bk.alloc<float>(BH);
+    P->g_pgrow = Bk.alloc<float>(NH);
     P->g_pden = Bk.alloc<float>(NH);
     P->g_xp = Bk.alloc<float>(N * d);
   }
@@ -1136,12 +1140,12 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     // linear attention and feature maps (performer_layer.py:200-205, 119-144)
     if (P.perf_pairwise)
       GPS_TRY(perf_quad_bwd(a->graph, P.H, P.m, P.pnmax, P.pfq, P.pfk, P.pV, P.pgmax, P.O, P.pden, P.g_O, P.g_pden,
-                            P.g_pfq, P.g_pfk, P.g_pV, P.g_pgmax, sa));
+                            P.g_pfq, P.g_pfk, P.g_pV, P.g_pgrow, sa));
     else
       GPS_TRY(perf_linattn_bwd(a->graph, P.H, P.m, P.pnmax, P.pfq, P.pfk, P.pV, P.pgmax, P.g_O, P.g_pfq, P.g_pfk, P.g_pV,
                                P.g_pgmax, sa));
     GPS_TRY(perf_features_bwd(P.g_pfq, P.g_pfk, P.pfq, P.pfk, P.pQ, P.pK, P.g_pQ, P.g_pK, a->graph, P.H, P.m, P.pargq,
-                              P.pargk, P.g_pgmax, sa));
+                              P.pargk, P.g_pgmax, P.g_pgrow, P.perf_pairwise, sa));
     float* gdd[2] = {P.g_pfq, P.g_pfk};
     float* gqk[2] = {P.g_pQ, P.g_pK};
     for (int i = 0; i < 2; ++i) {   // g_q += g_dd Pn   (dd = q Pn^T)
@@ -1468,6 +1472,66 @@ extern "C" int gps_gcn_aggregate_backward(const GpsGraph* g, int64_t d, const fl
   Planes yp;
   GPS_TRY(stage_planes(gY_planes, d, &yp, "gcn_aggregate_backward gY_planes"));
   return gcn_bwd(*g, d, g_h, dinv, gY, ldg, (cudaStream_t)stream, yp);
+}
+
+// ---- stage entry points of the Performer (performer.cu, performer_quad.cu).  Each validates its arguments before it
+// enqueues anything: dim_head 64, 256 < m <= 272 (perf_supported), H > 0 and N * H * 272 < 2^31.
+static int perf_stage(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m) {
+  GPS_TRY(perf_supported(dim_head, m));
+  return perf_index_range(g->N, H);
+}
+
+extern "C" int gps_performer_prep(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m, const float* P, float* Pn,
+                                  int* nmax, float* gmax, int* argk, void* stream) {
+  GPS_REQUIRE(g && P && Pn && nmax && gmax && argk, GPS_ERR_ARG, "performer_prep: null argument");
+  GPS_TRY(perf_stage(g, H, dim_head, m));
+  return perf_prep(P, m, Pn, *g, H, nmax, gmax, argk, (cudaStream_t)stream);
+}
+
+extern "C" int gps_performer_features_forward(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m, float* fq,
+                                              float* fk, const float* Q, const float* K, float* gmax, int* argq,
+                                              int* argk, void* stream) {
+  GPS_REQUIRE(g && fq && fk && Q && K && gmax && argq && argk, GPS_ERR_ARG, "performer_features_forward: null argument");
+  GPS_TRY(perf_stage(g, H, dim_head, m));
+  return perf_features_fwd(fq, fk, Q, K, *g, H, m, gmax, argq, argk, (cudaStream_t)stream);
+}
+
+extern "C" int gps_performer_attention_forward(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m, int32_t form,
+                                               const int* nmax, const float* qf, const float* kf, const float* V,
+                                               const float* gmax, float* O, float* den, void* stream) {
+  GPS_REQUIRE(form == 0 || form == 1, GPS_ERR_ARG, "performer_attention_forward: form must be 0 (context) or 1 (pairwise)");
+  GPS_REQUIRE(g && nmax && qf && kf && V && gmax && O && (form == 0 || den), GPS_ERR_ARG,
+              "performer_attention_forward: null argument");
+  GPS_TRY(perf_stage(g, H, dim_head, m));
+  if (form == 1) return perf_quad_fwd(*g, H, m, nmax, qf, kf, V, gmax, O, den, (cudaStream_t)stream);
+  return perf_linattn_fwd(*g, H, m, nmax, qf, kf, V, gmax, O, (cudaStream_t)stream);
+}
+
+extern "C" int gps_performer_attention_backward(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m, int32_t form,
+                                                const int* nmax, const float* qf, const float* kf, const float* V,
+                                                const float* gmax, const float* O, const float* den, const float* gO,
+                                                float* gden, float* g_qf, float* g_kf, float* gV, float* ggmax,
+                                                float* gmrow, void* stream) {
+  GPS_REQUIRE(form == 0 || form == 1, GPS_ERR_ARG, "performer_attention_backward: form must be 0 (context) or 1 (pairwise)");
+  GPS_REQUIRE(g && nmax && qf && kf && V && gmax && gO && g_qf && g_kf && gV &&
+                  (form == 0 ? ggmax != nullptr : (O && den && gden && gmrow)),
+              GPS_ERR_ARG, "performer_attention_backward: null argument");
+  GPS_TRY(perf_stage(g, H, dim_head, m));
+  if (form == 1)
+    return perf_quad_bwd(*g, H, m, nmax, qf, kf, V, gmax, O, den, gO, gden, g_qf, g_kf, gV, gmrow, (cudaStream_t)stream);
+  return perf_linattn_bwd(*g, H, m, nmax, qf, kf, V, gmax, gO, g_qf, g_kf, gV, ggmax, (cudaStream_t)stream);
+}
+
+extern "C" int gps_performer_features_backward(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m, int32_t form,
+                                               float* g_fq, float* g_fk, const float* fq, const float* fk, const float* Q,
+                                               const float* K, float* gQ, float* gK, const int* argq, const int* argk,
+                                               const float* ggmax, float* gmrow, void* stream) {
+  GPS_REQUIRE(form == 0 || form == 1, GPS_ERR_ARG, "performer_features_backward: form must be 0 (context) or 1 (pairwise)");
+  GPS_REQUIRE(g && g_fq && g_fk && fq && fk && Q && K && gQ && gK && argq && argk && gmrow && (form == 1 || ggmax),
+              GPS_ERR_ARG, "performer_features_backward: null argument");
+  GPS_TRY(perf_stage(g, H, dim_head, m));
+  return perf_features_bwd(g_fq, g_fk, fq, fk, Q, K, gQ, gK, *g, H, m, argq, argk, ggmax, gmrow, form == 1,
+                           (cudaStream_t)stream);
 }
 
 extern "C" int gps_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q, const float* K,

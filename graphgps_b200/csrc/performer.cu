@@ -15,8 +15,15 @@
 // no padding is materialised (SURVEY.md section 7, hard part 6).  The stabiliser is NOT detached in the in-repo
 // copy, so its gradient (to the arg-max element) is propagated as autograd does.
 //
+// Ties: when several elements share the maximum, the kernels give the whole stabiliser gradient to the lowest index
+// (the lowest feature of a query row; the lowest flat (row, feature) index of a (graph, head), real rows before the
+// padded ones), where torch.amax splits it evenly among the tied elements.  The total per max is the same, and g_Q /
+// g_K differ from the reference only when the tied elements come from rows of Pn that differ.
+//
 // Kernels: feature maps are warp-per-row; the per-(graph, head) linear attention keeps the 272x64 context in
-// registers (68 per thread) in forward and additionally in shared memory in backward.
+// registers (68 per thread) in forward and additionally in shared memory in backward.  The backward has no float
+// atomics: the stabiliser gradient of each key row goes to its own slot of a [N*H] buffer, and k_perf_gmax_scatter
+// sums each (graph, head)'s slots in a fixed order, so two runs give the same bits.
 #include <limits.h>
 
 #include "kernels.cuh"
@@ -40,8 +47,8 @@ __device__ __forceinline__ int find_graph_p(const int* __restrict__ gptr, int B,
 }
 
 __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
-  // valid for any mix of signs (IEEE ordering trick)
-  if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
+  // valid for any mix of signs (IEEE ordering trick); -0.0 takes the first branch with its sign bit cleared
+  if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v) & 0x7fffffff);
   else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 
@@ -297,12 +304,12 @@ __global__ void __launch_bounds__(256) k_perf_linattn_bwd(LinArgs a) {
   }
 }
 
-// warp per row: g_f -> g_dd in place, diag gradient into gQ/gK, stabiliser gradients
+// warp per row: g_f -> g_dd in place, diag gradient into gQ/gK, stabiliser gradients.  Key row r's gradient of its
+// (graph, head)'s max, -S, goes to gmrow[r]: added to the pairwise form's padded-row term there (add_rows), else stored.
 __global__ void k_perf_features_bwd(float* __restrict__ gq, float* __restrict__ gk, const float* __restrict__ fq,
                                     const float* __restrict__ fk, const float* __restrict__ Q, const float* __restrict__ K,
                                     float* __restrict__ gQ, float* __restrict__ gK, int N, int H, int m, float dn,
-                                    float ratio, const int* __restrict__ gptr, int B, const int* __restrict__ argq,
-                                    float* __restrict__ ggmax) {
+                                    float ratio, const int* __restrict__ argq, float* __restrict__ gmrow, bool add_rows) {
   const int NH = N * H;
   int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -331,10 +338,7 @@ __global__ void k_perf_features_bwd(float* __restrict__ gq, float* __restrict__ 
     const int j = lane + 32 * i;
     if (j < MP) grow[j] = tv[i] - (j == aj ? S : 0.f);   // row-max stabiliser of the queries
   }
-  if (!is_q && lane == 0) {
-    const int n = r / H, h = r % H;
-    atomicAdd(&ggmax[find_graph_p(gptr, B, n) * H + h], -S);
-  }
+  if (!is_q && lane == 0) gmrow[r] = (add_rows ? gmrow[r] : 0.f) - S;
   // diag = |x|^2 / 2 * dn^2  ->  g_x = -S * dn^2 * x
   const float* xrow = (is_q ? Q : K) + (int64_t)r * DH;
   float* gx = (is_q ? gQ : gK) + (int64_t)r * DH;
@@ -343,12 +347,20 @@ __global__ void k_perf_features_bwd(float* __restrict__ gq, float* __restrict__ 
   gx[lane + 32] = c * xrow[lane + 32];
 }
 
+// warp per (graph, head): the gradient of its key max is the sum of its rows' gmrow slots (lane-strided, then a fixed
+// shuffle tree) plus the context form's ggmax; it goes to the arg-max element, unless the max is a padded row's 0
 __global__ void k_perf_gmax_scatter(float* __restrict__ g_ddk, const int* __restrict__ argk, const float* __restrict__ ggmax,
-                                    int BH) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= BH) return;
-  const int a = argk[i];
-  if (a != INT_MAX) g_ddk[a] += ggmax[i];
+                                    const float* __restrict__ gmrow, const int* __restrict__ gptr, int B, int H) {
+  const int bh = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (bh >= B * H) return;
+  const int a = argk[bh];
+  if (a == INT_MAX) return;
+  const int b = bh / H, h = bh % H, gs = gptr[b], n = gptr[b + 1] - gs;
+  float s = 0.f;
+  for (int nn = lane; nn < n; nn += 32) s += gmrow[(int64_t)(gs + nn) * H + h];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) g_ddk[a] += (ggmax ? ggmax[bh] : 0.f) + s;
 }
 
 }  // namespace
@@ -360,6 +372,13 @@ int perf_supported(int64_t dim_head, int64_t features) {
   return GPS_OK;
 }
 int64_t perf_mp() { return MP; }
+// argk holds the flat int index r * MP + j of the [N*H, MP] key feature map
+int perf_index_range(int64_t N, int64_t H) {
+  GPS_REQUIRE(H > 0 && N >= 0 && N <= INT_MAX / MP / H, GPS_ERR_UNSUPPORTED,
+              "Performer kernels index the [N*H, %d] feature maps with int32: N*H = %lld*%lld exceeds %d", MP,
+              (long long)N, (long long)H, INT_MAX / MP);
+  return GPS_OK;
+}
 
 int perf_prep(const float* P, int64_t m, float* Pn, const GpsGraph& g, int64_t H, int* nmax, float* gmax, int* argk,
               cudaStream_t st) {
@@ -413,15 +432,16 @@ int perf_linattn_bwd(const GpsGraph& g, int64_t H, int64_t m, const int* nmax, c
 
 int perf_features_bwd(float* g_fq, float* g_fk, const float* fq, const float* fk, const float* Q, const float* K,
                       float* gQ, float* gK, const GpsGraph& g, int64_t H, int64_t m, const int* argq, const int* argk,
-                      float* ggmax, cudaStream_t st) {
+                      const float* ggmax, float* gmrow, bool pairwise, cudaStream_t st) {
   const int64_t NH = g.N * H;
   if (NH == 0) return GPS_OK;
   const float dn = powf((float)DH, -0.25f), ratio = 1.f / sqrtf((float)m);
   k_perf_features_bwd<<<(unsigned)ceil_div(2 * NH, 8), 256, 0, st>>>(g_fq, g_fk, fq, fk, Q, K, gQ, gK, (int)g.N, (int)H,
-                                                                      (int)m, dn, ratio, g.graph_ptr, (int)g.B, argq, ggmax);
+                                                                      (int)m, dn, ratio, argq, gmrow, pairwise);
   GPS_LAUNCH_CHECK();
-  const int BH = (int)(g.B * H);
-  k_perf_gmax_scatter<<<(unsigned)ceil_div(BH, 128), 128, 0, st>>>(g_fk, argk, ggmax, BH);
+  const int64_t BH = g.B * H;
+  k_perf_gmax_scatter<<<(unsigned)ceil_div(BH, 8), 256, 0, st>>>(g_fk, argk, pairwise ? nullptr : ggmax, gmrow,
+                                                                  g.graph_ptr, (int)g.B, (int)H);
   GPS_LAUNCH_CHECK();
   return GPS_OK;
 }

@@ -77,7 +77,7 @@ struct QArgs {
   const int* gptr; const int* nmax; int B, N, H, m; float ratio;
   const float* qf; const float* kf; const float* V; const float* gmax;
   float* O; float* den;                                  // forward outputs ([N,H*64], [N*H])
-  const float* gO; float* gden; float* g_qf; float* g_kf; float* gV; float* ggmax;   // backward
+  const float* gO; float* gden; float* g_qf; float* g_kf; float* gV; float* gmrow;   // backward
 };
 
 // row r = (node i, head h) lives at qf/kf + (i*H + h)*MP and V/O + (i*H + h)*64
@@ -124,7 +124,7 @@ __global__ void __launch_bounds__(kWarps * 32) k_perf_quad_fwd(QArgs a) {
   }
 }
 
-// query-major backward: g_q'_i, g_den_i, pad-term stabiliser gradient
+// query-major backward: g_q'_i, g_den_i, and row i's pad-term stabiliser gradient into its own slot gmrow[i*H + h]
 __global__ void __launch_bounds__(kWarps * 32) k_perf_quad_bwd_q(QArgs a) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, sub = lane % LPR, rloc = lane / LPR;
   const int h = blockIdx.y;
@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(kWarps * 32) k_perf_quad_bwd_q(QArgs a) {
     if (sub == 0) {
       a.gden[r] = gden;
       // k'_pad = ratio (exp(-gmax) + eps):  d den / d gmax = -npad * ratio * exp(-gmax) * sum_j q'_j
-      if (npad > 0.f) atomicAdd(&a.ggmax[g * a.H + h], -gden * npad * a.ratio * __expf(-gm) * rq);
+      a.gmrow[r] = npad > 0.f ? -gden * npad * a.ratio * __expf(-gm) * rq : 0.f;
     }
   }
 }
@@ -249,14 +249,13 @@ int perf_quad_fwd(const GpsGraph& g, int64_t H, int64_t m, const int* nmax, cons
 
 int perf_quad_bwd(const GpsGraph& g, int64_t H, int64_t m, const int* nmax, const float* qf, const float* kf,
                   const float* V, const float* gmax, const float* O, const float* den, const float* gO, float* gden,
-                  float* g_qf, float* g_kf, float* gV, float* ggmax, cudaStream_t st) {
-  if (g.B > 0) GPS_CUDA(cudaMemsetAsync(ggmax, 0, (size_t)(g.B * H) * sizeof(float), st));
+                  float* g_qf, float* g_kf, float* gV, float* gmrow, cudaStream_t st) {
   if (g.N == 0) return GPS_OK;
   QArgs a{};
   a.gptr = g.graph_ptr; a.nmax = nmax; a.B = (int)g.B; a.N = (int)g.N; a.H = (int)H; a.m = (int)m;
   a.ratio = 1.f / sqrtf((float)m); a.qf = qf; a.kf = kf; a.V = V; a.gmax = gmax;
   a.O = const_cast<float*>(O); a.den = const_cast<float*>(den); a.gO = gO; a.gden = gden;
-  a.g_qf = g_qf; a.g_kf = g_kf; a.gV = gV; a.ggmax = ggmax;
+  a.g_qf = g_qf; a.g_kf = g_kf; a.gV = gV; a.gmrow = gmrow;
   dim3 grid((unsigned)ceil_div(g.N, (int64_t)RPW * kWarps), (unsigned)H);
   k_perf_quad_bwd_q<<<grid, kWarps * 32, 0, st>>>(a);
   GPS_LAUNCH_CHECK();

@@ -309,6 +309,39 @@ int gps_gcn_aggregate_forward(const GpsGraph* g, int64_t d, const float* Y, int6
 int gps_gcn_aggregate_backward(const GpsGraph* g, int64_t d, const float* g_h, const float* dinv, float* gY,
                                int64_t ldg, const GpsPlanes* gY_planes, void* stream);
 
+/* Performer stage entry points (FAVOR+, performer_layer.py:119-144,200-205), the calls one layer makes, in order.
+ * They take dim_head == 64 and 256 < m <= 272 features (else GPS_ERR_UNSUPPORTED), H > 0 and N * H * 272 < 2^31 (else
+ * GPS_ERR_UNSUPPORTED), and reject NULL pointers with GPS_ERR_ARG, before any CUDA call.  Layout: a (node, head) row
+ * r = n * H + h; Q, K, V, O [N*H, 64]; feature maps [N*H, 272] with columns m..271 zero; gmax, ggmax, argk [B*H];
+ * argq, den, gden, gmrow [N*H].  form: 0 = per-graph context, 1 = pairwise; either runs on any batch. */
+/* P [m, 64] -> Pn [272, 64] = 64^-1/4 P padded with zero rows; nmax [1] = max graph size; gmax = 0 for graphs with
+ * padded rows of the dense batch (n < nmax), else -inf; argk = INT_MAX */
+int gps_performer_prep(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m, const float* P, float* Pn, int* nmax,
+                       float* gmax, int* argk, void* stream);
+/* fq / fk hold dd = x Pn^T on entry (only columns < m are read) and the feature maps q', k' on exit; gmax: key max
+ * per (graph, head) (prep's value on entry); argq: per-row arg-max feature; argk: flat arg-max r * 272 + j, INT_MAX
+ * when the max is a padded row's 0.  Ties go to the lowest index. */
+int gps_performer_features_forward(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m, float* fq, float* fk,
+                                   const float* Q, const float* K, float* gmax, int* argq, int* argk, void* stream);
+/* O = (q' . sum k'^T v) / den, den = q' . (sum k' + (nmax - n) k'_pad); den written by the pairwise form only */
+int gps_performer_attention_forward(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m, int32_t form,
+                                    const int* nmax, const float* qf, const float* kf, const float* V,
+                                    const float* gmax, float* O, float* den, void* stream);
+/* its backward from gO: g_qf, g_kf (all 272 columns), gV, and the gradient of gmax through k'_pad: the context form
+ * writes it per (graph, head) to ggmax; the pairwise form writes each query row's share to gmrow (and gden; O, den from
+ * its forward) */
+int gps_performer_attention_backward(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m, int32_t form,
+                                     const int* nmax, const float* qf, const float* kf, const float* V,
+                                     const float* gmax, const float* O, const float* den, const float* gO, float* gden,
+                                     float* g_qf, float* g_kf, float* gV, float* ggmax, float* gmrow, void* stream);
+/* backward of gps_performer_features_forward: g_fq / g_fk hold the feature-map gradients on entry (columns < m read)
+ * and the gradients of dd on exit; gQ / gK [N*H, 64] = the gradients through diag (written).  The upstream gradient
+ * of gmax is ggmax (form 0) or the per-(graph, head) sum of gmrow (form 1); gmrow is overwritten. */
+int gps_performer_features_backward(const GpsGraph* g, int64_t H, int64_t dim_head, int64_t m, int32_t form,
+                                    float* g_fq, float* g_fk, const float* fq, const float* fk, const float* Q,
+                                    const float* K, float* gQ, float* gK, const int* argq, const int* argk,
+                                    const float* ggmax, float* gmrow, void* stream);
+
 /* Dense softmax attention over each graph's own nodes — replaces to_dense_batch +
  * nn.MultiheadAttention core + [mask] (gps_layer.py:199-201,234-241) without padding.
  * Q,K,V: [N, heads*hd] slices with row stride ld; O [N, heads*hd] (row stride ldo); lse [N,heads]. */
