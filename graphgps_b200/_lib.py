@@ -75,6 +75,11 @@ class GpsLayerArgs(C.Structure):
     ]
 
 
+class GpsAttnBias(C.Structure):
+    """Attention bias of the BiasedTransformer: bias / grad_bias [B*heads, nmax, nmax] float32."""
+    _fields_ = [("bias", _fp), ("nmax", C.c_int64), ("grad_bias", _fp)]
+
+
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
                 ("bwd_workspace_bytes", C.c_int64), ("fwd_launches", C.c_int64),
@@ -92,6 +97,8 @@ SYMBOLS = {
     "gps_layer_plan": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsLayerPlan)]),
     "gps_layer_forward": (C.c_int, [C.POINTER(GpsLayerArgs), _fp]),
     "gps_layer_backward": (C.c_int, [C.POINTER(GpsLayerArgs), _fp]),
+    "gps_layer_forward_biased": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsAttnBias), _fp]),
+    "gps_layer_backward_biased": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsAttnBias), _fp]),
     "gps_linear_forward": (C.c_int, [_fp, _i64, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _fp]),
     "gps_gemm": (C.c_int, [_fp, _i64, _i32, _fp, _i64, _i32, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _fp]),
     "gps_gatedgcn_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _i64, _fp, _fp,
@@ -124,6 +131,13 @@ SYMBOLS = {
                                          _fp, _fp, _fp, _fp, _fp, _i64, _f32, _u64, _u64, _fp]),
     "gps_attention_forward_tc": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _fp, _i64, _fp, _i64, _fp, _f32, _u64, _u64,
                                            _i32, _fp]),
+    "gps_attention_forward_biased": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _fp, _fp, _i64, _fp, _i64, _fp,
+                                               _f32, _u64, _u64, C.POINTER(GpsAttnBias), _fp]),
+    "gps_attention_forward_tc_biased": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _fp, _i64, _fp, _i64, _fp, _f32,
+                                                  _u64, _u64, _i32, C.POINTER(GpsAttnBias), _fp]),
+    "gps_attention_backward_biased": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _fp, _fp, _i64, _fp, _fp, _i64,
+                                                _fp, _fp, _fp, _fp, _fp, _i64, _f32, _u64, _u64, C.POINTER(GpsAttnBias),
+                                                _fp]),
     "gps_dropout_mask": (C.c_int, [_fp, _i64, _i64, _f32, _u64, _u64, _i32, _fp]),
     "gps_to_planes": (C.c_int, [_fp, _i64, _i64, _i64, _fp, _fp, _i64, _fp]),
     "gps_gemm_planes": (C.c_int, [_fp, _fp, _i64, _i32, _fp, _fp, _i64, _i32, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64,

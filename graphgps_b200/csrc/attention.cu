@@ -12,6 +12,9 @@
 // an LPR-lane shuffle reduction.  Online softmax in fp32; dropout on the probabilities uses the
 // Philox stream (site GPS_SITE_ATTN_P + head).
 // Backward = two passes (query-major for dQ and delta, key-major for dK, dV): no atomics.
+// BIAS (BiasedTransformer, gps_layer.py:202-204): S = (q . k) / sqrt(hd) + bias[g, h, i - gs, j - gs] with the caller's
+// dense [B*H, nmax, nmax] bias.  The query-major backward visits every (query, key, head) once and writes the score
+// gradient there, so grad_bias needs no atomics either.
 #include "kernels.cuh"
 
 namespace gps {
@@ -108,6 +111,7 @@ struct AttnArgs {
   const unsigned long long* offset_dev;
   Planes Op, dQp, dKp, dVp;   // optional bf16 hi/lo plane copies of O (forward) / dQ, dK, dV (backward)
   int smem_rows;              // rows of the two per-block staging tiles (0: no staging)
+  const float* bias; int64_t nmax; float* gbias;   // BIAS kernels only: [B*H, nmax, nmax], grad_bias (may be NULL)
 };
 __device__ __forceinline__ uint64_t eff_offset(const AttnArgs& a) {
   return a.offset + ((a.p_drop > 0.f && a.offset_dev) ? *a.offset_dev : 0ull);
@@ -148,7 +152,7 @@ __device__ __forceinline__ StagedRows stage_rows(const AttnArgs& a, const float*
   return r;
 }
 
-template <int CH, int LPR>
+template <int CH, int LPR, bool BIAS>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
   extern __shared__ float attn_sm[];
   constexpr int RPW = 32 / LPR;
@@ -160,10 +164,12 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
   const int nch = a.hd / 4;
   const uint64_t offs = eff_offset(a);
   int gs = 0, n = 0;
+  const float* brow = nullptr;   // BIAS: bias row of (graph, head, query)
   if (row_ok) {
     int g = find_graph(a.gptr, a.B, i);
     gs = a.gptr[g];
     n = a.gptr[g + 1] - gs;
+    if constexpr (BIAS) brow = a.bias + (((int64_t)g * a.H + h) * a.nmax + (i - gs)) * a.nmax;
   }
   const int nloop = warp_max_i(n);
   const int64_t hoff = (int64_t)h * a.hd;
@@ -184,6 +190,8 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
   float4 kc[CH], vc[CH];
   load_slice<CH, LPR>(kc, kv.x + (int64_t)gs * kv.ldx, sub, nch, n > 0);
   load_slice<CH, LPR>(vc, kv.y + (int64_t)gs * kv.ldy, sub, nch, n > 0);
+  float bc = 0.f;
+  if constexpr (BIAS) bc = n > 0 ? brow[0] : 0.f;
   for (int jl = 0; jl < nloop; ++jl) {
     if (use_drop && (jl & 3) == 0) drop_quad_refresh(dq, a.p_drop, a.seed, offs, h, i, jl);
     const bool valid = jl < n;
@@ -192,7 +200,10 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
     float4 kn[CH], vn[CH];
     load_slice<CH, LPR>(kn, kv.x + (int64_t)jn * kv.ldx, sub, nch, nvalid);
     load_slice<CH, LPR>(vn, kv.y + (int64_t)jn * kv.ldy, sub, nch, nvalid);
+    float bn = 0.f;
+    if constexpr (BIAS) bn = nvalid ? brow[jl + 1] : 0.f;
     float s = group_sum<LPR>(dot_slice<CH>(q, kc));
+    if constexpr (BIAS) s += bc;
     s = valid ? s : -INFINITY;
     const float m_new = fmaxf(m, s);
     const float corr = (m_new == -INFINITY) ? 1.f : __expf(m - m_new);
@@ -208,6 +219,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
       kc[c] = kn[c];
       vc[c] = vn[c];
     }
+    if constexpr (BIAS) bc = bn;
     m = m_new;
   }
   if (row_ok) {
@@ -241,8 +253,8 @@ __global__ void k_attn_delta(AttnArgs a) {
   if (ok && sub == 0) a.delta[t] = acc;
 }
 
-// query-major backward: dQ_i (delta precomputed by k_attn_delta)
-template <int CH, int LPR>
+// query-major backward: dQ_i (delta precomputed by k_attn_delta); BIAS: grad_bias[g, h, i - gs, jl] = ds
+template <int CH, int LPR, bool BIAS>
 __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_sm) {
   constexpr int RPW = 32 / LPR;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -253,10 +265,12 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
   const int nch = a.hd / 4;
   const uint64_t offs = eff_offset(a);
   int gs = 0, n = 0;
+  int64_t brow = 0;   // BIAS: offset of the (graph, head, query) row in bias / grad_bias
   if (row_ok) {
     int g = find_graph(a.gptr, a.B, i);
     gs = a.gptr[g];
     n = a.gptr[g + 1] - gs;
+    if constexpr (BIAS) brow = (((int64_t)g * a.H + h) * a.nmax + (i - gs)) * a.nmax;
   }
   const int nloop = warp_max_i(n);
   const int64_t hoff = (int64_t)h * a.hd;
@@ -278,6 +292,8 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
     float4 kk[CH], vv[CH];
     load_slice<CH, LPR>(kk, kv.x + (int64_t)gs * kv.ldx, sub, nch, n > 0);
     load_slice<CH, LPR>(vv, kv.y + (int64_t)gs * kv.ldy, sub, nch, n > 0);
+    float bc = 0.f;
+    if constexpr (BIAS) bc = n > 0 ? a.bias[brow] : 0.f;
     for (int jl = 0; jl < nloop; ++jl) {
       if (use_drop && (jl & 3) == 0) drop_quad_refresh(dq, a.p_drop, a.seed, offs, h, i, jl);
       const bool valid = jl < n;
@@ -286,14 +302,21 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
       float4 kn[CH], vn[CH];
       load_slice<CH, LPR>(kn, kv.x + (int64_t)jn * kv.ldx, sub, nch, nvalid);
       load_slice<CH, LPR>(vn, kv.y + (int64_t)jn * kv.ldy, sub, nch, nvalid);
+      float bn = 0.f;
+      if constexpr (BIAS) bn = nvalid ? a.bias[brow + jl + 1] : 0.f;
       float s = dot_slice<CH>(q, kk), dp = dot_slice<CH>(go, vv);
 #pragma unroll
       for (int ofs = LPR / 2; ofs > 0; ofs >>= 1) {
         s += __shfl_xor_sync(0xffffffffu, s, ofs);
         dp += __shfl_xor_sync(0xffffffffu, dp, ofs);
       }
+      if constexpr (BIAS) s += bc;
       const float p = valid ? __expf(s - lse) : 0.f;
       const float ds = p * (dp * (use_drop ? drop_quad_scale(dq, jl) : 1.f) - dl);
+      if constexpr (BIAS) {
+        if (a.gbias && valid && sub == 0) a.gbias[brow + jl] = ds;
+        bc = bn;
+      }
 #pragma unroll
       for (int c = 0; c < CH; ++c) {
         gq[c].x += ds * kk[c].x;
@@ -313,8 +336,8 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
   }
 }
 
-// key-major backward: dK_j, dV_j
-template <int CH, int LPR>
+// key-major backward: dK_j, dV_j (BIAS: p recomputed with the bias column of key j)
+template <int CH, int LPR, bool BIAS>
 __device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_sm) {
   constexpr int RPW = 32 / LPR;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -325,10 +348,12 @@ __device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_
   const int nch = a.hd / 4;
   const uint64_t offs = eff_offset(a);
   int gs = 0, n = 0;
+  const float* bcol = nullptr;   // BIAS: bias column of (graph, head, key); query il at bcol[il * nmax]
   if (row_ok) {
     int g = find_graph(a.gptr, a.B, j);
     gs = a.gptr[g];
     n = a.gptr[g + 1] - gs;
+    if constexpr (BIAS) bcol = a.bias + ((int64_t)g * a.H + h) * a.nmax * a.nmax + (j - gs);
   }
   const int nloop = warp_max_i(n);
   const int jl = j - gs;
@@ -362,7 +387,9 @@ __device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_
     }
     const float lse = valid ? a.lsec[(int64_t)i * a.H + h] : 0.f;
     const float dl = valid ? a.deltac[(int64_t)i * a.H + h] : 0.f;
-    const float p = valid ? __expf(s * a.scale - lse) : 0.f;
+    float p;
+    if constexpr (BIAS) p = valid ? __expf(s * a.scale + bcol[(int64_t)il * a.nmax] - lse) : 0.f;
+    else p = valid ? __expf(s * a.scale - lse) : 0.f;
     float dsc = 1.f;
     if (a.p_drop > 0.f) {
       DropQuad dq;
@@ -389,18 +416,18 @@ __device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_
 }
 
 // both backward passes in one grid (blockIdx.z picks the pass) so they share the SMs instead of queueing
-template <int CH, int LPR>
+template <int CH, int LPR, bool BIAS>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_bwd(AttnArgs a) {
   extern __shared__ float attn_sm[];
-  if (blockIdx.z == 0) attn_bwd_kv_body<CH, LPR>(a, attn_sm);
-  else attn_bwd_q_body<CH, LPR>(a, attn_sm);
+  if (blockIdx.z == 0) attn_bwd_kv_body<CH, LPR, BIAS>(a, attn_sm);
+  else attn_bwd_q_body<CH, LPR, BIAS>(a, attn_sm);
 }
 
 enum { KFWD = 0, KBWD = 1 };
 
 constexpr int kStageBytes = 72 * 1024;   // two staging tiles per block; 3 blocks per SM still fit
 
-template <int CH, int LPR>
+template <int CH, int LPR, bool BIAS>
 static void launch_one(int which, const AttnArgs& a0, cudaStream_t stream) {
   constexpr int RPW = 32 / LPR;
   AttnArgs a = a0;
@@ -417,14 +444,14 @@ static void launch_one(int which, const AttnArgs& a0, cudaStream_t stream) {
   const size_t smem = a.smem_rows > 0 ? (size_t)2 * a.smem_rows * pitch * 4 : 0;
   static bool attr_done[2] = {false, false};
   if (smem > 0 && !attr_done[which]) {
-    if (which == KFWD) cudaFuncSetAttribute(k_attn_fwd<CH, LPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
-    else cudaFuncSetAttribute(k_attn_bwd<CH, LPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
+    if (which == KFWD) cudaFuncSetAttribute(k_attn_fwd<CH, LPR, BIAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
+    else cudaFuncSetAttribute(k_attn_bwd<CH, LPR, BIAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
     attr_done[which] = true;
   }
   dim3 grid((unsigned)ceil_div(a.N, (int64_t)RPW * kWarpsPerBlock), (unsigned)a.H, which == KFWD ? 1 : 2);
   dim3 block(kWarpsPerBlock * 32);
-  if (which == KFWD) k_attn_fwd<CH, LPR><<<grid, block, smem, stream>>>(a);
-  else k_attn_bwd<CH, LPR><<<grid, block, smem, stream>>>(a);
+  if (which == KFWD) k_attn_fwd<CH, LPR, BIAS><<<grid, block, smem, stream>>>(a);
+  else k_attn_bwd<CH, LPR, BIAS><<<grid, block, smem, stream>>>(a);
 }
 
 static int dispatch(int which, const AttnArgs& a, cudaStream_t stream) {
@@ -440,7 +467,8 @@ static int dispatch(int which, const AttnArgs& a, cudaStream_t stream) {
   const int ch = (nch + lpr - 1) / lpr;
 #define GPS_ATTN_CASE(CHV, LPRV)                                  \
   if (ch == CHV && lpr == LPRV) {                                 \
-    launch_one<CHV, LPRV>(which, a, stream);                      \
+    if (a.bias) launch_one<CHV, LPRV, true>(which, a, stream);    \
+    else launch_one<CHV, LPRV, false>(which, a, stream);          \
     GPS_LAUNCH_CHECK();                                           \
     return GPS_OK;                                                \
   }
@@ -456,10 +484,11 @@ static int dispatch(int which, const AttnArgs& a, cudaStream_t stream) {
 
 int attention_fwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, const float* K, const float* V,
                   int64_t ld, float* O, int64_t ldo, float* lse, float p_drop, uint64_t seed, uint64_t offset,
-                  cudaStream_t stream, const unsigned long long* offset_dev, Planes Op) {
+                  cudaStream_t stream, const unsigned long long* offset_dev, Planes Op, const GpsAttnBias* bias) {
   AttnArgs a{};
   a.offset_dev = offset_dev;
   a.Op = Op;
+  if (bias) { a.bias = bias->bias; a.nmax = bias->nmax; }
   a.gptr = g.graph_ptr; a.B = (int)g.B; a.N = (int)g.N; a.H = (int)heads; a.hd = (int)hd;
   a.Q = Q; a.K = K; a.V = V; a.ld = ld; a.O = O; a.ldo = ldo; a.lse = lse;
   a.scale = 1.f / sqrtf((float)hd); a.p_drop = p_drop; a.seed = seed; a.offset = offset;
@@ -469,14 +498,18 @@ int attention_fwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, 
 int attention_bwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, const float* K, const float* V,
                   int64_t ld, const float* O, const float* dO, int64_t ldo, const float* lse, float* delta,
                   float* dQ, float* dK, float* dV, int64_t ldg, float p_drop, uint64_t seed, uint64_t offset,
-                  cudaStream_t stream, const unsigned long long* offset_dev, Planes dQp, Planes dKp, Planes dVp) {
+                  cudaStream_t stream, const unsigned long long* offset_dev, Planes dQp, Planes dKp, Planes dVp,
+                  const GpsAttnBias* bias) {
   AttnArgs a{};
   a.offset_dev = offset_dev;
+  if (bias) { a.bias = bias->bias; a.nmax = bias->nmax; a.gbias = bias->grad_bias; }
   a.dQp = dQp; a.dKp = dKp; a.dVp = dVp;
   a.gptr = g.graph_ptr; a.B = (int)g.B; a.N = (int)g.N; a.H = (int)heads; a.hd = (int)hd;
   a.Q = Q; a.K = K; a.V = V; a.ld = ld; a.Oc = O; a.dO = dO; a.ldo = ldo; a.lsec = lse;
   a.delta = delta; a.deltac = delta; a.dQ = dQ; a.dK = dK; a.dV = dV; a.ldg = ldg;
   a.scale = 1.f / sqrtf((float)hd); a.p_drop = p_drop; a.seed = seed; a.offset = offset;
+  if (a.gbias)   // entries of padded rows / columns stay 0; the kernel writes every in-graph (query, key) pair
+    GPS_CUDA(cudaMemsetAsync(a.gbias, 0, (size_t)(g.B * heads * a.nmax * a.nmax) * sizeof(float), stream));
   if (a.N == 0) return GPS_OK;
   const int64_t nt = (int64_t)a.N * a.H * 8;
   k_attn_delta<<<(unsigned)ceil_div(nt, (int64_t)256), 256, 0, stream>>>(a);

@@ -21,6 +21,8 @@
 // full / empty barriers, so the next K tile loads while the softmax and P V of the current one run.  (A separate
 // producer warp would make the CTA count as three warpgroups and cap the registers that S, O and P need.)
 // The CUDA-core kernel in attention.cu serves batches of small graphs (mean below 64 nodes) and head dims above 128.
+// BIAS (BiasedTransformer): after the range mask, each valid S element becomes S * scale + bias[g, h, i - gs, j - gs]
+// (the caller's dense [B*H, nmax, nmax] bias) before the row max, and the softmax then runs with scale 1.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -44,6 +46,10 @@ struct AttnTcArgs {
   float scale; float p_drop; uint64_t seed, offset;
   const unsigned long long* offset_dev;
   float* dbg;   // bring-up: CTA (0,0) dumps S [128x128], P [128x128] and the raw O accumulator [128x128] of its first tile
+};
+// the bias travels as a kernel parameter of its own: growing AttnTcArgs changes the unbiased kernels' code
+struct TcBias {
+  const float* bias; int64_t nmax;   // read by the BIAS kernels only
 };
 
 __device__ __forceinline__ int find_graph_tc(const int* __restrict__ gptr, int B, int node) {
@@ -69,9 +75,10 @@ struct RowState {
 };
 
 // NKB: 64-column blocks of the padded head dim (1: hd_pad <= 64, 2: <= 128) = the P V instruction width / 64
-template <int NKB, bool SPLIT>
+template <int NKB, bool SPLIT, bool BIAS>
 __global__ void __launch_bounds__(kThreadsA, 1)
-k_attn_tc_fwd(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmV, const AttnTcArgs a) {
+k_attn_tc_fwd(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmV, const AttnTcArgs a,
+              const TcBias tb) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr int planes = SPLIT ? 2 : 1;
@@ -134,6 +141,7 @@ k_attn_tc_fwd(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ 
   const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of the first of this lane's two rows
   const int cq = 2 * (lane & 3);
   RowState rs[2];
+  const float* brow[2] = {nullptr, nullptr};   // BIAS: bias rows of the lane's two queries
 #pragma unroll
   for (int u = 0; u < 2; ++u) {
     RowState& R = rs[u];
@@ -143,6 +151,7 @@ k_attn_tc_fwd(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ 
       const int g = find_graph_tc(a.gptr, a.B, R.i);
       R.gs = a.gptr[g];
       R.ge = a.gptr[g + 1];
+      if constexpr (BIAS) brow[u] = tb.bias + (((int64_t)g * a.H + h) * tb.nmax + (R.i - R.gs)) * tb.nmax;
     }
     R.m = -INFINITY; R.l = 0.f; R.rq_quad = -1;
   }
@@ -151,6 +160,7 @@ k_attn_tc_fwd(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ 
   const uint32_t drop_thr = (uint32_t)fminf(a.p_drop * 4294967296.f, 4294967295.f);
   const float keep_scale = use_drop ? 1.f / (1.f - a.p_drop) : 1.f;
   const bool dump = a.dbg && blockIdx.x == 0 && blockIdx.y == 0;
+  const float sc = BIAS ? 1.f : a.scale;   // BIAS: S is scaled (and biased) in place before the softmax
 
   float o[NKB * 32];
 #pragma unroll
@@ -189,6 +199,18 @@ k_attn_tc_fwd(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ 
     __syncwarp();
     if (lane == 0) mbar_arrive(b_ke);
     if (tid == 0 && t + 1 < ntiles) load_k(t + 1);
+    if constexpr (BIAS) {
+#pragma unroll
+      for (int u = 0; u < 2; ++u)
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int key = key0 + 8 * j + cq + e;
+            float& v = sacc[4 * j + 2 * u + e];
+            if (key >= rs[u].gs && key < rs[u].ge) v = v * a.scale + brow[u][key - rs[u].gs];
+          }
+    }
     // ---- online softmax on the registers: row maximum over the valid (same-graph) logits, quad-reduced
     float corr[2];
 #pragma unroll
@@ -200,7 +222,7 @@ k_attn_tc_fwd(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ 
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int key = key0 + 8 * j + cq + e;
-          if (key >= R.gs && key < R.ge) mnew = fmaxf(mnew, sacc[4 * j + 2 * u + e] * a.scale);
+          if (key >= R.gs && key < R.ge) mnew = fmaxf(mnew, sacc[4 * j + 2 * u + e] * sc);
         }
       mnew = fmaxf(mnew, __shfl_xor_sync(0xffffffffu, mnew, 1));
       mnew = fmaxf(mnew, __shfl_xor_sync(0xffffffffu, mnew, 2));
@@ -226,7 +248,7 @@ k_attn_tc_fwd(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ 
           const float sraw = v;
           float pr = 0.f;
           if (key >= R.gs && key < R.ge) {
-            pr = __expf(v * a.scale - R.m);
+            pr = __expf(v * sc - R.m);
             R.l += pr;
             if (use_drop) {
               const int jl = key - R.gs;
@@ -309,15 +331,15 @@ k_attn_tc_fwd(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ 
   }
 }
 
-template <int NKB, bool SPLIT>
-int launch_attn(const CUtensorMap& tQK, const CUtensorMap& tV, const AttnTcArgs& a, dim3 grid, size_t smem,
-                cudaStream_t stream) {
+template <int NKB, bool SPLIT, bool BIAS>
+int launch_attn(const CUtensorMap& tQK, const CUtensorMap& tV, const AttnTcArgs& a, const TcBias& tb, dim3 grid,
+                size_t smem, cudaStream_t stream) {
   static bool attr_done = false;
   if (!attr_done) {
-    GPS_CUDA(cudaFuncSetAttribute(k_attn_tc_fwd<NKB, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    GPS_CUDA(cudaFuncSetAttribute(k_attn_tc_fwd<NKB, SPLIT, BIAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_done = true;
   }
-  k_attn_tc_fwd<NKB, SPLIT><<<grid, kThreadsA, smem, stream>>>(tQK, tV, a);
+  k_attn_tc_fwd<NKB, SPLIT, BIAS><<<grid, kThreadsA, smem, stream>>>(tQK, tV, a, tb);
   GPS_LAUNCH_CHECK();
   return GPS_OK;
 }
@@ -332,7 +354,7 @@ int64_t attention_tc_hd_pad(int64_t hd) { return round_up(hd, 16); }
 // qkv: bf16 hi/lo planes [N, 3 * H * hd_pad] in the per-head padded layout (which * H + h) * hd_pad + k, pads zero.
 int attention_tc_fwd(const GpsGraph& g, int64_t heads, int64_t hd, Planes qkv, float* O, int64_t ldo, Planes Op, float* lse,
                      float p_drop, uint64_t seed, uint64_t offset, const unsigned long long* offset_dev, int precision,
-                     cudaStream_t stream) {
+                     cudaStream_t stream, const GpsAttnBias* bias) {
   if (g.N == 0) return GPS_OK;
   GPS_REQUIRE(attention_tc_supported(hd) && qkv.hi && (precision != GPS_PREC_FP32 || qkv.lo) && qkv.ld % 8 == 0, GPS_ERR_UNSUPPORTED,
               "attention_tc: head dim %lld / planes not supported", (long long)hd);
@@ -343,6 +365,8 @@ int attention_tc_fwd(const GpsGraph& g, int64_t heads, int64_t hd, Planes qkv, f
   a.O = O; a.ldo = ldo; a.Op = Op; a.lse = lse;
   a.scale = 1.f / sqrtf((float)hd); a.p_drop = p_drop; a.seed = seed; a.offset = offset; a.offset_dev = offset_dev;
   a.dbg = g_attn_dbg;
+  TcBias tb{};
+  if (bias) tb = TcBias{bias->bias, bias->nmax};
   const int64_t cols = 3 * heads * a.hd_pad;
   CUtensorMap tQK, tV;
   GPS_TRY(make_tensor_map(qkv.hi, qkv.lo, a.planes, g.N, cols, qkv.ld, 128, &tQK));
@@ -350,10 +374,16 @@ int attention_tc_fwd(const GpsGraph& g, int64_t heads, int64_t hd, Planes qkv, f
   const int nkb = (a.hd_pad + 63) >> 6;
   const size_t smem = (size_t)a.planes * nkb * (16384 + 16384 + 16384) + 1024 + 256;
   dim3 grid((unsigned)ceil_div(g.N, kTile), (unsigned)heads);
-  if (nkb == 1) return a.planes == 2 ? launch_attn<1, true>(tQK, tV, a, grid, smem, stream)
-                                     : launch_attn<1, false>(tQK, tV, a, grid, smem, stream);
-  return a.planes == 2 ? launch_attn<2, true>(tQK, tV, a, grid, smem, stream)
-                       : launch_attn<2, false>(tQK, tV, a, grid, smem, stream);
+  if (bias) {
+    if (nkb == 1) return a.planes == 2 ? launch_attn<1, true, true>(tQK, tV, a, tb, grid, smem, stream)
+                                       : launch_attn<1, false, true>(tQK, tV, a, tb, grid, smem, stream);
+    return a.planes == 2 ? launch_attn<2, true, true>(tQK, tV, a, tb, grid, smem, stream)
+                         : launch_attn<2, false, true>(tQK, tV, a, tb, grid, smem, stream);
+  }
+  if (nkb == 1) return a.planes == 2 ? launch_attn<1, true, false>(tQK, tV, a, tb, grid, smem, stream)
+                                     : launch_attn<1, false, false>(tQK, tV, a, tb, grid, smem, stream);
+  return a.planes == 2 ? launch_attn<2, true, false>(tQK, tV, a, tb, grid, smem, stream)
+                       : launch_attn<2, false, false>(tQK, tV, a, tb, grid, smem, stream);
 }
 
 }  // namespace gps

@@ -114,12 +114,14 @@ int gcn_bwd(const GpsGraph& g, int64_t d, const float* g_h, const float* dinv, f
 // ---- attention ------------------------------------------------------------------------------
 int attention_fwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, const float* K, const float* V,
                   int64_t ld, float* O, int64_t ldo, float* lse, float p_drop, uint64_t seed, uint64_t offset,
-                  cudaStream_t stream, const unsigned long long* offset_dev = nullptr, Planes Op = Planes());
+                  cudaStream_t stream, const unsigned long long* offset_dev = nullptr, Planes Op = Planes(),
+                  const GpsAttnBias* bias = nullptr);
+// bias (BiasedTransformer): NULL = none; its grad_bias, when set, is written whole by attention_bwd (padding zeroed)
 int attention_bwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, const float* K, const float* V,
                   int64_t ld, const float* O, const float* dO, int64_t ldo, const float* lse, float* delta,
                   float* dQ, float* dK, float* dV, int64_t ldg, float p_drop, uint64_t seed, uint64_t offset,
                   cudaStream_t stream, const unsigned long long* offset_dev = nullptr, Planes dQp = Planes(),
-                  Planes dKp = Planes(), Planes dVp = Planes());
+                  Planes dKp = Planes(), Planes dVp = Planes(), const GpsAttnBias* bias = nullptr);
 
 // wgmma version (attention_tc.cu): Q, K, V from bf16 hi/lo planes in the per-head padded layout
 // column (which * H + h) * hd_pad + k, hd_pad = attention_tc_hd_pad(hd), pad columns zero
@@ -128,6 +130,6 @@ bool attention_tc_supported(int64_t hd);
 int64_t attention_tc_hd_pad(int64_t hd);
 int attention_tc_fwd(const GpsGraph& g, int64_t heads, int64_t hd, Planes qkv, float* O, int64_t ldo, Planes Op, float* lse,
                      float p_drop, uint64_t seed, uint64_t offset, const unsigned long long* offset_dev, int precision,
-                     cudaStream_t stream);
+                     cudaStream_t stream, const GpsAttnBias* bias = nullptr);
 
 }  // namespace gps

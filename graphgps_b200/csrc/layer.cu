@@ -754,8 +754,18 @@ static int dropmul(const Plan& P, Operand g, float* tmp, Planes tmp_p, int site,
 
 }  // namespace
 
+// attention bias of the BiasedTransformer (gps_b200.h GpsAttnBias): checked before any CUDA call
+static int check_bias(const GpsLayerArgs* a, const GpsAttnBias* bias) {
+  if (!bias) return GPS_OK;
+  GPS_REQUIRE(a->global_type == GPS_GLOBAL_TRANSFORMER, GPS_ERR_ARG,
+              "an attention bias needs global_type GPS_GLOBAL_TRANSFORMER (got %d)", a->global_type);
+  GPS_REQUIRE(bias->nmax >= 1, GPS_ERR_ARG, "attention bias: nmax must be >= 1 (got %lld)", (long long)bias->nmax);
+  GPS_REQUIRE(bias->bias, GPS_ERR_ARG, "attention bias: null bias pointer");
+  return GPS_OK;
+}
+
 // =================================================================================== forward
-static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
+static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaStream_t st) {
   Plan P;
   GPS_TRY(make_plan(a, &P, true));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
@@ -889,10 +899,10 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     const float* Q = P.Y1 + P.qkv_off;
     if (P.attn_tc)
       GPS_TRY(attention_tc_fwd(a->graph, P.H, P.hd, P.qkv_p, P.O, d, P.O_p, P.lse, P.pa, a->seed, a->offset,
-                               (const unsigned long long*)a->offset_dev, P.prec, sg));
+                               (const unsigned long long*)a->offset_dev, P.prec, sg, bias));
     else
       GPS_TRY(attention_fwd(a->graph, P.H, P.hd, Q, Q + d, Q + 2 * d, P.Wy, P.O, d, P.lse, P.pa, a->seed, a->offset,
-                            sg, (const unsigned long long*)a->offset_dev, P.O_p));
+                            sg, (const unsigned long long*)a->offset_dev, P.O_p, bias));
     // hA = x + drop(O Wo^T + bo)
     GemmParams g = linear_fwd(P, N, d, d, {P.O, d, P.O_p}, {a->attn_out.weight, d, P.out_p}, P.hA, d, a->attn_out.bias);
     g.R1 = a->x; g.ldr1 = (int)d; g.stats = stats(BN_A);
@@ -964,7 +974,7 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
 }
 
 // =================================================================================== backward
-static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
+static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaStream_t st) {
   Plan P;
   GPS_TRY(make_plan(a, &P, true));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
@@ -1119,7 +1129,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     float* gQ = P.gY1 + P.qkv_off;
     GPS_TRY(attention_bwd(a->graph, P.H, P.hd, Q, Q + d, Q + 2 * d, P.Wy, P.O, P.g_O, d, P.lse, P.delta, gQ, gQ + d,
                           gQ + 2 * d, P.Wy, P.pa, a->seed, a->offset, sa, (const unsigned long long*)a->offset_dev,
-                          P.gY1_p.cols(P.qkv_off), P.gY1_p.cols(P.qkv_off + d), P.gY1_p.cols(P.qkv_off + 2 * d)));
+                          P.gY1_p.cols(P.qkv_off), P.gY1_p.cols(P.qkv_off + d), P.gY1_p.cols(P.qkv_off + 2 * d), bias));
   }
 
   if (P.perf) {
@@ -1317,12 +1327,24 @@ extern "C" int gps_layer_plan(const GpsLayerArgs* args, GpsLayerPlan* plan) {
 
 extern "C" int gps_layer_forward(const GpsLayerArgs* args, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_forward: null args");
-  return layer_forward(args, (cudaStream_t)stream);
+  return layer_forward(args, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward(const GpsLayerArgs* args, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_backward: null args");
-  return layer_backward(args, (cudaStream_t)stream);
+  return layer_backward(args, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int gps_layer_forward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream) {
+  GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_forward_biased: null args");
+  GPS_TRY(check_bias(args, bias));
+  return layer_forward(args, bias, (cudaStream_t)stream);
+}
+
+extern "C" int gps_layer_backward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream) {
+  GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_backward_biased: null args");
+  GPS_TRY(check_bias(args, bias));
+  return layer_backward(args, bias, (cudaStream_t)stream);
 }
 
 extern "C" int gps_linear_forward(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias,
@@ -1558,6 +1580,46 @@ extern "C" int gps_attention_backward(const GpsGraph* g, int64_t heads, int64_t 
               "attention_backward: null argument");
   return attention_bwd(*g, heads, hd, Q, K, V, ld, O, dO, ldo, lse, delta, dQ, dK, dV, ldg, p_drop, seed, offset,
                        (cudaStream_t)stream);
+}
+
+// the three attention stages with an attention bias
+static int check_stage_bias(const GpsAttnBias* bias, const char* what) {
+  GPS_REQUIRE(bias && bias->bias, GPS_ERR_ARG, "%s: null attention bias", what);
+  GPS_REQUIRE(bias->nmax >= 1, GPS_ERR_ARG, "%s: nmax must be >= 1 (got %lld)", what, (long long)bias->nmax);
+  return GPS_OK;
+}
+
+extern "C" int gps_attention_forward_biased(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q,
+                                            const float* K, const float* V, int64_t ld, float* O, int64_t ldo,
+                                            float* lse, float p_drop, uint64_t seed, uint64_t offset,
+                                            const GpsAttnBias* bias, void* stream) {
+  GPS_REQUIRE(g && Q && K && V && O && lse, GPS_ERR_ARG, "attention_forward_biased: null argument");
+  GPS_TRY(check_stage_bias(bias, "attention_forward_biased"));
+  return attention_fwd(*g, heads, hd, Q, K, V, ld, O, ldo, lse, p_drop, seed, offset, (cudaStream_t)stream, nullptr,
+                       Planes(), bias);
+}
+
+extern "C" int gps_attention_forward_tc_biased(const GpsGraph* g, int64_t heads, int64_t hd, const void* qkv_hi,
+                                               const void* qkv_lo, int64_t ld, float* O, int64_t ldo, float* lse,
+                                               float p_drop, uint64_t seed, uint64_t offset, int32_t precision,
+                                               const GpsAttnBias* bias, void* stream) {
+  GPS_REQUIRE(g && qkv_hi && O && lse, GPS_ERR_ARG, "attention_forward_tc_biased: null argument");
+  GPS_TRY(check_stage_bias(bias, "attention_forward_tc_biased"));
+  Planes q{(__nv_bfloat16*)qkv_hi, (__nv_bfloat16*)qkv_lo, ld};
+  return attention_tc_fwd(*g, heads, hd, q, O, ldo, Planes(), lse, p_drop, seed, offset, nullptr, precision,
+                          (cudaStream_t)stream, bias);
+}
+
+extern "C" int gps_attention_backward_biased(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q,
+                                             const float* K, const float* V, int64_t ld, const float* O,
+                                             const float* dO, int64_t ldo, const float* lse, float* delta, float* dQ,
+                                             float* dK, float* dV, int64_t ldg, float p_drop, uint64_t seed,
+                                             uint64_t offset, const GpsAttnBias* bias, void* stream) {
+  GPS_REQUIRE(g && Q && K && V && O && dO && lse && delta && dQ && dK && dV, GPS_ERR_ARG,
+              "attention_backward_biased: null argument");
+  GPS_TRY(check_stage_bias(bias, "attention_backward_biased"));
+  return attention_bwd(*g, heads, hd, Q, K, V, ld, O, dO, ldo, lse, delta, dQ, dK, dV, ldg, p_drop, seed, offset,
+                       (cudaStream_t)stream, nullptr, Planes(), Planes(), Planes(), bias);
 }
 
 extern "C" int gps_dropout_mask(float* mask, int64_t rows, int64_t cols, float p, uint64_t seed, uint64_t offset,

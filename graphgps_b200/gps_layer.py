@@ -23,8 +23,11 @@ from .graph import graph_of
 _SUPPORTED_LOCAL = ("None", "CustomGatedGCN", "GINE", "GCN")
 _EDGE_LOCAL = ("CustomGatedGCN", "GINE")   # local models that read batch.edge_attr (gps_layer.py:44-53)
 _KNOWN_LOCAL = _SUPPORTED_LOCAL + ("GIN", "GENConv", "GAT", "PNA")
-_SUPPORTED_GLOBAL = ("None", "Transformer", "Performer")
-_KNOWN_GLOBAL = _SUPPORTED_GLOBAL + ("BiasedTransformer", "BigBird")
+_SUPPORTED_GLOBAL = ("None", "Transformer", "BiasedTransformer", "Performer")
+_KNOWN_GLOBAL = _SUPPORTED_GLOBAL + ("BigBird",)
+_MHA_GLOBAL = ("Transformer", "BiasedTransformer")   # torch's MultiheadAttention (gps_layer.py:104-106)
+# the library's global model: BiasedTransformer is the Transformer called with a GpsAttnBias
+_GLOBAL_ABI = dict(_lib.GLOBAL, BiasedTransformer=_lib.GLOBAL["Transformer"])
 _ACT_MODULES = {"relu": nn.ReLU, "gelu": nn.GELU}
 
 _workspaces = {}
@@ -169,7 +172,7 @@ class _GPSLayerFn(torch.autograd.Function):
     """One autograd node for the whole layer: forward = gps_layer_forward, backward = gps_layer_backward."""
 
     @staticmethod
-    def forward(ctx, layer, gs, x, e, pe, *params):
+    def forward(ctx, layer, gs, x, e, pe, bias, *params):
         lib = _lib.load()
         dev = x.device
         named = dict(zip(layer._param_names, params))
@@ -193,11 +196,16 @@ class _GPSLayerFn(torch.autograd.Function):
             snap = _next_dropout_offset(dev)
             args.offset, args.offset_dev = 0, snap.data_ptr()
         stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gps_layer_forward(C.byref(args), stream), "gps_layer_forward")
+        ctx.nmax = gs.nmax if bias.numel() else 0
+        if ctx.nmax:
+            ab = _lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)
+            _lib.check(lib.gps_layer_forward_biased(C.byref(args), C.byref(ab), stream), "gps_layer_forward_biased")
+        else:
+            _lib.check(lib.gps_layer_forward(C.byref(args), stream), "gps_layer_forward")
         ctx.layer, ctx.gs, ctx.saved_buf, ctx.snap = layer, gs, saved, snap
         ctx.hand = hand
         ctx.seed, ctx.offset, ctx.training = args.seed, args.offset, bool(args.training)
-        ctx.save_for_backward(x, e, pe, *params)
+        ctx.save_for_backward(x, e, pe, bias, *params)
         if e_out is not None:
             return x_out, e_out
         return x_out
@@ -206,7 +214,7 @@ class _GPSLayerFn(torch.autograd.Function):
     def backward(ctx, g_x_out, g_e_out=None):
         lib = _lib.load()
         layer, gs = ctx.layer, ctx.gs
-        x, e, pe, *params = ctx.saved_tensors
+        x, e, pe, bias, *params = ctx.saved_tensors
         dev = x.device
         named = dict(zip(layer._param_names, params))
         pe_k = pe.shape[1] if layer._eslap else 0
@@ -253,10 +261,17 @@ class _GPSLayerFn(torch.autograd.Function):
         if evs is not None:
             args.ev_grads_early, args.ev_grads_mid, args.ev_grads_done = (e.cuda_event for e in evs)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gps_layer_backward(C.byref(args), stream), "gps_layer_backward")
+        g_bias = None
+        if ctx.nmax:
+            if ctx.needs_input_grad[5]:
+                g_bias = torch.empty_like(bias)
+            ab = _lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))
+            _lib.check(lib.gps_layer_backward_biased(C.byref(args), C.byref(ab), stream), "gps_layer_backward_biased")
+        else:
+            _lib.check(lib.gps_layer_backward(C.byref(args), stream), "gps_layer_backward")
         # (ctx.saved_buf stays alive with the autograd node: backward(retain_graph=True) may run again)
         if bucket is not None:
-            return (None, None, g_x, g_e, g_pe) + (None,) * len(layer._param_names)
+            return (None, None, g_x, g_e, g_pe, g_bias) + (None,) * len(layer._param_names)
         # parameters the configuration never reads get no gradient (as under autograd in the reference)
         unused = []
         if layer.local_gnn_type == "None":
@@ -264,7 +279,7 @@ class _GPSLayerFn(torch.autograd.Function):
         if layer.global_model_type == "None":
             unused.append("norm1_attn.")
         pg = tuple(None if any(n.startswith(u) for u in unused) else grads[n] for n in layer._param_names)
-        return (None, None, g_x, g_e, g_pe) + pg
+        return (None, None, g_x, g_e, g_pe, g_bias) + pg
 
 
 class GPSLayer(nn.Module):
@@ -327,7 +342,7 @@ class GPSLayer(nn.Module):
             raise NotImplementedError(f"global model '{global_model_type}' is not built in graphgps_b200")
         if global_model_type == "None":
             self.self_attn = None
-        elif global_model_type == "Transformer":
+        elif global_model_type in _MHA_GLOBAL:
             if dim_h % num_heads != 0:
                 raise ValueError("embed_dim must be divisible by num_heads")
             # torch's own module is the parameter container (same init, same state_dict keys);
@@ -474,7 +489,7 @@ class GPSLayer(nn.Module):
         a = _lib.GpsLayerArgs()
         a.d, a.heads = self.dim_h, self.num_heads
         a.local_type = _lib.LOCAL[self.local_gnn_type]
-        a.global_type = _lib.GLOBAL[self.global_model_type]
+        a.global_type = _GLOBAL_ABI[self.global_model_type]
         a.act = _lib.ACT[self.act]
         a.training = 1 if self.training else 0
         a.precision = _lib.PRECISION[self.precision]
@@ -505,7 +520,7 @@ class GPSLayer(nn.Module):
         elif self.local_gnn_type == "GCN":
             a.gcn_conv = _lin(named["local_model.lin.weight"], named["local_model.bias"],
                               g.get("local_model.lin.weight"), g.get("local_model.bias"))
-        if self.global_model_type == "Transformer":
+        if self.global_model_type in _MHA_GLOBAL:
             a.attn_in = _lin(named["self_attn.in_proj_weight"], named["self_attn.in_proj_bias"],
                              g.get("self_attn.in_proj_weight"), g.get("self_attn.in_proj_bias"))
             a.attn_out = lin("self_attn.out_proj")
@@ -550,11 +565,13 @@ class GPSLayer(nn.Module):
             e = None
         pe = self._read_pe(batch, x) if self._eslap else None
         gs = graph_of(batch)
+        bias = self._read_attn_bias(batch, x, gs) if self.global_model_type == "BiasedTransformer" else None
         params = [p for _, p in self.named_parameters()]
         e_arg = e if e is not None else x.new_empty(0)
         pe_arg = pe if pe is not None else x.new_empty(0)
+        bias_arg = bias if bias is not None else x.new_empty(0)
         self.__dict__["_planes_in"] = _batch_planes_get(batch)
-        out = _GPSLayerFn.apply(self, gs, x, e_arg, pe_arg, *params)
+        out = _GPSLayerFn.apply(self, gs, x, e_arg, pe_arg, bias_arg, *params)
         produced = self.__dict__.pop("_planes_out", None)
         if self.local_gnn_type == "CustomGatedGCN":
             batch.x, batch.edge_attr = out           # gps_layer.py:173-174, :231
@@ -577,6 +594,27 @@ class GPSLayer(nn.Module):
             raise ValueError(f"batch.pe_EquivStableLapPE must have shape [num_nodes={x.shape[0]}, k >= 1] "
                              f"(got {tuple(pe.shape)})")
         return pe.contiguous()
+
+    def _read_attn_bias(self, batch, x, gs):
+        """batch.attn_bias [num_graphs * heads, Nmax, Nmax] (gps_layer.py:202-204), row g * heads + h for graph g and
+        head h, Nmax = the largest graph: float32 on the device of x.  Missing: AttributeError, as in the reference;
+        None: no bias, as torch's MultiheadAttention treats attn_mask=None."""
+        if not hasattr(batch, "attn_bias"):
+            raise AttributeError("GPSLayer('BiasedTransformer') reads batch.attn_bias [num_graphs * heads, Nmax, Nmax], "
+                                 "which this batch does not have (Graphormer's BiasEncoder writes it)")
+        ab = batch.attn_bias
+        if ab is None:
+            return None
+        if not torch.is_tensor(ab) or ab.dtype != torch.float32 or ab.device != x.device:
+            raise TypeError("batch.attn_bias must be a float32 tensor on the device of batch.x (got "
+                            f"{getattr(ab, 'dtype', type(ab))} on {getattr(ab, 'device', None)})")
+        want = (gs.B * self.num_heads, gs.nmax, gs.nmax)
+        if tuple(ab.shape) != want:
+            raise ValueError(f"batch.attn_bias must have shape [num_graphs * heads, Nmax, Nmax] = {list(want)} "
+                             f"(got {list(ab.shape)})")
+        if gs.nmax == 0:   # no nodes: nothing attends
+            return None
+        return ab.contiguous()
 
     def extra_repr(self):
         return (f"summary: dim_h={self.dim_h}, local_gnn_type={self.local_gnn_type}, "

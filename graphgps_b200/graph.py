@@ -48,6 +48,20 @@ class GraphStructure:
         _lib.check(rc, "gps_graph_build")
         self.key = (edge_index.data_ptr(), batch.data_ptr(), self.N, self.E, edge_index._version, batch._version)
 
+    @property
+    def nmax(self) -> int:
+        """Size of the largest graph (to_dense_batch's Nmax, the side of batch.attn_bias).  Read from the device once
+        per batch and cached; inside a CUDA-graph capture it must already be cached (GPSStack.capture reads it in its
+        warm-up), because the read synchronises."""
+        v = self.__dict__.get("_nmax")
+        if v is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("GraphStructure.nmax is read from the device and cannot be read inside a CUDA-graph "
+                                   "capture: read graph_of(batch).nmax before capturing")
+            v = int(torch.diff(self.graph_ptr).max()) if self.B > 0 else 0
+            self.__dict__["_nmax"] = v
+        return v
+
     def _view(self, addr, n):
         off = addr - self.storage.data_ptr()
         return self.storage[off:off + 4 * n].view(torch.int32)

@@ -52,8 +52,8 @@ class GPSStack(nn.Module):
         """Records `bucket.zero_(); out = stack(batch); backward(out, cotangents); collective()` into one CUDA graph.
 
         `batch` must be resident on the GPU with its graph structure already built (graph.graph_of); its x / edge_attr
-        are the graph's static inputs (copy new data into them before replay()), and so is its pe_EquivStableLapPE when it
-        has one (every layer built with equivstable_pe=True reads that one tensor; its gradient sums over the layers).
+        are the graph's static inputs (copy new data into them before replay()), and so are its pe_EquivStableLapPE and
+        attn_bias when it has them (every layer that reads one reads that one tensor; its gradient sums over the layers).
         Returns a CapturedStep."""
         from .batch import GraphBatch
         from .graph import graph_of
@@ -62,7 +62,12 @@ class GPSStack(nn.Module):
         e_in = batch.edge_attr.detach().requires_grad_(True) if getattr(batch, "edge_attr", None) is not None else None
         pe = getattr(batch, "pe_EquivStableLapPE", None)
         pe_in = pe.detach().requires_grad_(True) if pe is not None else None
+        ab = getattr(batch, "attn_bias", None)
+        ab_in = ab.detach().requires_grad_(True) if ab is not None else None
         extra = {"pe_EquivStableLapPE": pe_in} if pe_in is not None else {}
+        if ab_in is not None:
+            extra["attn_bias"] = ab_in
+            gs.nmax   # read from the device now: the capture cannot
         params = [p for p in self.parameters()]
         res = {}
 
@@ -75,6 +80,8 @@ class GPSStack(nn.Module):
                 e_in.grad = None
             if pe_in is not None:
                 pe_in.grad = None
+            if ab_in is not None:
+                ab_in.grad = None
             if bucket is not None:
                 bucket.zero_()
             else:
@@ -100,15 +107,16 @@ class GPSStack(nn.Module):
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, capture_error_mode="thread_local"):
             body()
-        return CapturedStep(g, x_in, e_in, res["x"], res["e"], pe_in)
+        return CapturedStep(g, x_in, e_in, res["x"], res["e"], pe_in, ab_in)
 
 
 class CapturedStep:
     """One captured forward+backward of a GPSStack: static inputs, outputs and input gradients."""
 
-    def __init__(self, graph, x_in, e_in, x_out, e_out, pe_in=None):
+    def __init__(self, graph, x_in, e_in, x_out, e_out, pe_in=None, attn_bias_in=None):
         self.graph, self.x_in, self.e_in, self.x_out, self.e_out = graph, x_in, e_in, x_out, e_out
         self.pe_in = pe_in
+        self.attn_bias_in = attn_bias_in
 
     def replay(self):
         self.graph.replay()
@@ -125,3 +133,8 @@ class CapturedStep:
     def grad_pe(self):
         """Gradient w.r.t. batch.pe_EquivStableLapPE, summed over the layers (None when the batch has no PE)."""
         return self.pe_in.grad if self.pe_in is not None else None
+
+    @property
+    def grad_attn_bias(self):
+        """Gradient w.r.t. batch.attn_bias, summed over the layers (None when the batch has no attention bias)."""
+        return self.attn_bias_in.grad if self.attn_bias_in is not None else None

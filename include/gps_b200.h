@@ -234,6 +234,25 @@ int gps_layer_plan(const GpsLayerArgs* args, GpsLayerPlan* plan);
 int gps_layer_forward(const GpsLayerArgs* args, void* stream);
 int gps_layer_backward(const GpsLayerArgs* args, void* stream);
 
+/* Additive attention bias of the BiasedTransformer global model (gps_layer.py:104-106,202-204,234-241; Graphormer's
+ * batch.attn_bias): bias [B*heads, nmax, nmax] row-major float32, row g*heads + h of graph g and head h, entry (il, jl)
+ * for local query il and local key jl; nmax >= the largest graph of the batch (to_dense_batch's Nmax).  The scores
+ * become S = (q . k) / sqrt(hd) + bias[g*heads + h, il, jl]; padded entries (il or jl >= n_g) are not read.  grad_bias
+ * (backward; NULL = not needed) has the same layout and is written whole: dL/dS at every in-graph entry, 0 at every
+ * padded one. */
+typedef struct {
+  const float* bias;
+  int64_t nmax;
+  float* grad_bias;
+} GpsAttnBias;
+
+/* gps_layer_forward / _backward with an attention bias.  bias == NULL is the unbiased call; a non-NULL bias needs
+ * global_type == GPS_GLOBAL_TRANSFORMER, nmax >= 1 and bias->bias != NULL (else GPS_ERR_ARG before any CUDA call).
+ * The bias changes neither gps_layer_plan's sizes nor the GpsLayerArgs fields; forward and backward must see the same
+ * bias tensor. */
+int gps_layer_forward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream);
+int gps_layer_backward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Stage-level entry points (the same kernels the layer calls; exported so the parity tests can
  * pin each stage against the oracle separately).
@@ -361,6 +380,19 @@ int gps_attention_backward(const GpsGraph* g, int64_t heads, int64_t hd, const f
                            const float* dO, int64_t ldo, const float* lse, float* delta,
                            float* dQ, float* dK, float* dV, int64_t ldg, float p_drop,
                            uint64_t seed, uint64_t offset, void* stream);
+/* The three attention stages with a GpsAttnBias (non-NULL, nmax >= 1, bias->bias != NULL, else GPS_ERR_ARG); the
+ * backward writes bias->grad_bias when it is not NULL.  Other arguments as above. */
+int gps_attention_forward_biased(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q, const float* K,
+                                 const float* V, int64_t ld, float* O, int64_t ldo, float* lse, float p_drop,
+                                 uint64_t seed, uint64_t offset, const GpsAttnBias* bias, void* stream);
+int gps_attention_forward_tc_biased(const GpsGraph* g, int64_t heads, int64_t hd, const void* qkv_hi,
+                                    const void* qkv_lo, int64_t ld, float* O, int64_t ldo, float* lse, float p_drop,
+                                    uint64_t seed, uint64_t offset, int32_t precision, const GpsAttnBias* bias,
+                                    void* stream);
+int gps_attention_backward_biased(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q, const float* K,
+                                  const float* V, int64_t ld, const float* O, const float* dO, int64_t ldo,
+                                  const float* lse, float* delta, float* dQ, float* dK, float* dV, int64_t ldg,
+                                  float p_drop, uint64_t seed, uint64_t offset, const GpsAttnBias* bias, void* stream);
 
 /* ABI 3: operand "planes" of the TMA-fed wgmma GEMM (csrc/gemm_tma.cu).  A plane pair is the bf16 image of an
  * fp32 matrix: hi = bf16(v), lo = bf16(v - hi), both plain row-major with pitch ldp (elements, multiple of 8); lo may
