@@ -14,7 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgps_b200.so")
 
 GPS_OK, GPS_ERR_ARG, GPS_ERR_UNSUPPORTED, GPS_ERR_CUDA = 0, -1, -2, -3
-LOCAL = {"None": 0, "CustomGatedGCN": 1, "GINE": 2, "GCN": 3}
+LOCAL = {"None": 0, "CustomGatedGCN": 1, "GINE": 2, "GCN": 3, "GAT": 4}
 GLOBAL = {"None": 0, "Transformer": 1, "Performer": 2}
 ACT = {"relu": 0, "gelu": 1}
 PRECISION = {"fp32": 0, "bf16": 1}
@@ -80,6 +80,12 @@ class GpsAttnBias(C.Structure):
     _fields_ = [("bias", _fp), ("nmax", C.c_int64), ("grad_bias", _fp)]
 
 
+class GpsGat(C.Structure):
+    """GAT local model: lin_src (weight = local_model.lin_src.weight, bias = local_model.bias), lin_edge, att_* [H*C]."""
+    _fields_ = [("lin_src", GpsLinear), ("lin_edge", GpsLinear), ("att_src", _fp), ("att_dst", _fp), ("att_edge", _fp),
+                ("grad_att_src", _fp), ("grad_att_dst", _fp), ("grad_att_edge", _fp)]
+
+
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
                 ("bwd_workspace_bytes", C.c_int64), ("fwd_launches", C.c_int64),
@@ -99,6 +105,8 @@ SYMBOLS = {
     "gps_layer_backward": (C.c_int, [C.POINTER(GpsLayerArgs), _fp]),
     "gps_layer_forward_biased": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsAttnBias), _fp]),
     "gps_layer_backward_biased": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsAttnBias), _fp]),
+    "gps_layer_forward_gat": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGat), C.POINTER(GpsAttnBias), _fp]),
+    "gps_layer_backward_gat": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGat), C.POINTER(GpsAttnBias), _fp]),
     "gps_linear_forward": (C.c_int, [_fp, _i64, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _fp]),
     "gps_gemm": (C.c_int, [_fp, _i64, _i32, _fp, _i64, _i32, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _fp]),
     "gps_gatedgcn_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _i64, _fp, _fp,
@@ -116,6 +124,13 @@ SYMBOLS = {
     "gps_gcn_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _i64, _fp, _fp, _fp, _fp, _f32, _u64, _u64,
                                             _fp, _fp]),
     "gps_gcn_aggregate_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _i64, C.POINTER(GpsPlanes), _fp]),
+    "gps_gat_fold_forward": (C.c_int, [_fp, _fp, _i64, _i64, _fp, _fp]),
+    "gps_gat_fold_backward": (C.c_int, [_fp, _fp, _fp, _i64, _i64, _fp, _fp, _i32, _fp]),
+    "gps_gat_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _i64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp,
+                                  _f32, _u64, _u64, _fp, _fp]),
+    "gps_gat_workspace_bytes": (_i64, [_i64, _i64, _i64, _i64]),
+    "gps_gat_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _i64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i64,
+                                   _fp, _i64, C.POINTER(GpsPlanes), _fp, _fp, _fp, _fp, _fp, _i32, _fp]),
     "gps_performer_prep": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp]),
     "gps_performer_features_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp,
                                                  _fp, _fp]),

@@ -111,6 +111,32 @@ int gcn_fwd(const GpsGraph& g, int64_t d, const float* Y, int64_t ldy, const flo
 int gcn_bwd(const GpsGraph& g, int64_t d, const float* g_h, const float* dinv, float* gY, int64_t ldg,
             cudaStream_t stream, Planes gYp = Planes());
 
+// GAT (PyG GATConv, gat.cu).  H heads of C = d / H channels; Y [N, ldy] = x W_src^T; v [H, d] = fold(W_edge, att_edge).
+// Scores saved by the forward, in one buffer of (4 N + E) H floats: a_src, a_dst, a_self (the added self loop's edge
+// score), lse (log-sum-exp of each (node, head) softmax), each [N, H], then a_edge [E, H] in edge-id order.
+struct GatScores {
+  float *a_src, *a_dst, *a_self, *lse, *a_edge;
+};
+GatScores gat_scores(float* base, int64_t N, int64_t E, int64_t H);
+// H > 0 with d % H == 0 (else GPS_ERR_ARG), d % 4 == 0 and d <= 4096 (else GPS_ERR_UNSUPPORTED)
+int gat_check(int64_t d, int64_t H);
+int gat_fold_fwd(const float* W_edge, const float* att_edge, int64_t d, int64_t H, float* v, cudaStream_t stream);
+// g_W_edge[hC+c, :] = att_edge[hC+c] g_v[h];  g_att_edge[hC+c] = W_edge[hC+c, :] . g_v[h]  (written, or added)
+int gat_fold_bwd(const float* W_edge, const float* att_edge, const float* g_v, int64_t d, int64_t H, float* gW,
+                 float* gatt, bool accumulate, cudaStream_t stream);
+// x_loc = x + drop(GATConv(x) + bias) [+ column sums of x_loc]
+int gat_fwd(const GpsGraph& g, int64_t d, int64_t H, const float* Y, int64_t ldy, const float* ea, const float* v,
+            const float* att_src, const float* att_dst, const float* bias, const float* x, GatScores s, float* xloc,
+            DropCfg drop, double* stats, cudaStream_t stream);
+// floats of scratch gat_bwd needs
+int64_t gat_bwd_workspace_floats(int64_t N, int64_t E, int64_t H, int64_t d);
+// from g_h (the gradient of the aggregation output, bias included): gY [N, ldg] (+ planes), grad_ea [E, d] (NULL = not
+// needed), g_v [H, d] (written), and g_att_src / g_att_dst / g_bias (each NULL = not needed; written, or added)
+int gat_bwd(const GpsGraph& g, int64_t d, int64_t H, const float* Y, int64_t ldy, const float* ea, const float* v,
+            const float* att_src, const float* att_dst, GatScores s, const float* g_h, float* ws, float* gY, int64_t ldg,
+            Planes gYp, float* grad_ea, float* g_v, float* g_att_src, float* g_att_dst, float* g_bias, bool accumulate,
+            cudaStream_t stream);
+
 // ---- attention ------------------------------------------------------------------------------
 int attention_fwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, const float* K, const float* V,
                   int64_t ld, float* O, int64_t ldo, float* lse, float p_drop, uint64_t seed, uint64_t offset,

@@ -221,6 +221,11 @@ struct LayerWeight {
 struct Plan {
   int64_t N, E, d, H, hd, Wy, qkv_off;
   bool gated, gine, gcn, attn, perf;
+  // GAT (gat.cu): the caller's GpsGat (NULL when only sizes are wanted); saved v = fold(W_edge, att_edge) [H, d] and the
+  // scores (GatScores); backward scratch g_v [H, d] then gat_bwd's workspace
+  bool gat;
+  const GpsGat* gatp;
+  float *gat_v, *gat_sc, *gat_ws;
   // GPS_NORM_NONE: no norm1_local / norm1_attn / norm2.  Only the local model's own BatchNorms (BN_X, BN_E) remain, so
   // nbn = 2 statistics slots instead of BN_COUNT; s = x_loc + hA is written by the GEMM that closes the second branch
   // and x_out by the FF2 GEMM.
@@ -296,6 +301,9 @@ static void list_weights(const GpsLayerArgs* a, Plan* P) {
   }
   // GCNConv.lin has no bias; GCNConv.bias is added after the aggregation (scatter.cu)
   if (P->gcn) add(a->gcn_conv, d, d, &Plan::Wcat_p, false);
+  // GATConv.lin_src (= lin_dst) has no bias; GATConv.bias is added after the aggregation (gat.cu)
+  static const GpsLinear kNoLinear = {};
+  if (P->gat) add(P->gatp ? P->gatp->lin_src : kNoLinear, d, d, &Plan::Wcat_p, false);
   P->qkv_off = P->Wy;
   if (P->attn) add(a->attn_in, 3 * d, d, &Plan::Wcat_p);
   if (P->attn || P->perf) add(a->attn_out, d, kout, &Plan::out_p);
@@ -320,7 +328,7 @@ static Planes caller_planes(const GpsPlanes& g, int64_t d, int precision) {
   return Planes{(__nv_bfloat16*)g.hi, lo ? (__nv_bfloat16*)g.lo : nullptr, g.ld};
 }
 
-static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
+static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* gat = nullptr) {
   memset(P, 0, sizeof(*P));
   GPS_REQUIRE(a, GPS_ERR_ARG, "null args");
   P->N = a->graph.N;
@@ -332,8 +340,11 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   P->gated = a->local_type == GPS_LOCAL_GATEDGCN;
   P->gine = a->local_type == GPS_LOCAL_GINE;
   P->gcn = a->local_type == GPS_LOCAL_GCN;
-  GPS_REQUIRE(a->local_type == GPS_LOCAL_NONE || P->gated || P->gine || P->gcn, GPS_ERR_ARG, "unknown local_type %d",
-              a->local_type);
+  P->gat = a->local_type == GPS_LOCAL_GAT;
+  P->gatp = gat;
+  GPS_REQUIRE(a->local_type == GPS_LOCAL_NONE || P->gated || P->gine || P->gcn || P->gat, GPS_ERR_ARG,
+              "unknown local_type %d", a->local_type);
+  if (P->gat) GPS_TRY(gat_check(a->d, a->heads));
   P->eslap = a->pe != nullptr;
   GPS_REQUIRE(!P->eslap || P->gated, GPS_ERR_ARG, "pe (EquivStableLapPE) is read by the GatedGCN local model only");
   GPS_REQUIRE(!P->eslap || a->pe_dim >= 1, GPS_ERR_ARG, "pe_dim must be >= 1 (got %lld)", (long long)a->pe_dim);
@@ -398,7 +409,11 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
     if (gelu) P->h1_pre = S.alloc<float>(N * d);
   }
   if (P->gcn) P->dinv = S.alloc<float>(N);
-  const bool loc = P->gated || P->gine || P->gcn;
+  if (P->gat) {
+    P->gat_v = S.alloc<float>(P->H * d);
+    P->gat_sc = S.alloc<float>((4 * N + E) * P->H);
+  }
+  const bool loc = P->gated || P->gine || P->gcn || P->gat;
   if (loc && !P->nonorm) P->xloc = S.alloc<float>(N * d);   // read by norm1_local's backward
   if (P->attn) {
     P->O = S.alloc<float>(N * d);
@@ -533,6 +548,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
     P->g_agg = Bk.alloc<float>(N * d);
     P->g_xl = Bk.alloc<float>(N * d);
   }
+  if (P->gat) P->gat_ws = Bk.alloc<float>(P->H * d + gat_bwd_workspace_floats(N, E, P->H, d));
   if (P->use_planes) {
     P->gt_p = mkplanes(Bk, N, d);
     P->ghid_p = mkplanes(Bk, N, 2 * d);
@@ -608,7 +624,7 @@ static int check_bn(const GpsBatchNorm& b, const char* name) {
 }
 
 static int check_params(const GpsLayerArgs* a, const Plan& P) {
-  GPS_REQUIRE(a->x && (P.E == 0 || a->edge_attr || !(P.gated || P.gine)), GPS_ERR_ARG,
+  GPS_REQUIRE(a->x && (P.E == 0 || a->edge_attr || !(P.gated || P.gine || P.gat)), GPS_ERR_ARG,
               "missing x / edge_attr");
   if (P.gated) {
     GPS_TRY(check_linear(a->gcn_A, "local_model.A", true));
@@ -628,8 +644,16 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
     GPS_TRY(check_linear(a->gine_lin1, "local_model.nn.2", true));
   }
   if (P.gcn) GPS_TRY(check_linear(a->gcn_conv, "local_model.lin / local_model.bias", true));
+  if (P.gat) {
+    GPS_REQUIRE(P.gatp, GPS_ERR_ARG, "local_type GPS_LOCAL_GAT needs gps_layer_forward_gat / gps_layer_backward_gat "
+                "with a GpsGat");
+    GPS_TRY(check_linear(P.gatp->lin_src, "local_model.lin_src / local_model.bias", true));
+    GPS_TRY(check_linear(P.gatp->lin_edge, "local_model.lin_edge", false));
+    GPS_REQUIRE(P.gatp->att_src && P.gatp->att_dst && P.gatp->att_edge, GPS_ERR_ARG,
+                "missing parameter local_model.att_{src,dst,edge}");
+  }
   const bool bn = !P.nonorm;   // norm1_local / norm1_attn / norm2 exist in BatchNorm mode only
-  if ((P.gated || P.gine || P.gcn) && bn) GPS_TRY(check_bn(a->norm1_local, "norm1_local"));
+  if ((P.gated || P.gine || P.gcn || P.gat) && bn) GPS_TRY(check_bn(a->norm1_local, "norm1_local"));
   if (P.attn) {
     GPS_TRY(check_linear(a->attn_in, "self_attn.in_proj", true));
     GPS_TRY(check_linear(a->attn_out, "self_attn.out_proj", true));
@@ -765,9 +789,9 @@ static int check_bias(const GpsLayerArgs* a, const GpsAttnBias* bias) {
 }
 
 // =================================================================================== forward
-static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaStream_t st) {
+static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, cudaStream_t st) {
   Plan P;
-  GPS_TRY(make_plan(a, &P, true));
+  GPS_TRY(make_plan(a, &P, true, gat));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
   GPS_REQUIRE(a->workspace_bytes >= P.fwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.fwd_bytes);
@@ -784,7 +808,7 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaStr
   Side* sd;
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
-  const bool two_branches = (P.gated || P.gine || P.gcn) && (P.attn || P.perf);
+  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat) && (P.attn || P.perf);
   // GPS_NORM_NONE: the producer that closes the last branch writes s = x_loc + hA with its planes (x_loc = s when the
   // local model is alone)
   const bool local_writes_s = P.nonorm && !(P.attn || P.perf);
@@ -888,6 +912,11 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaStr
     GPS_TRY(gcn_dinv(a->graph, P.dinv, st));
     GPS_TRY(gcn_fwd(a->graph, d, P.Y1, P.Wy, P.dinv, a->gcn_conv.bias, a->x, P.xloc, P.drop(GPS_SITE_LOCAL),
                     stats(BN_L), st));
+  } else if (P.gat) {
+    // x_loc = x + drop(GATConv(x, edge_attr))  (gps_layer.py:70-74,183-189); Y = x W_src^T is column block 0 of Y1
+    GPS_TRY(gat_fold_fwd(gat->lin_edge.weight, gat->att_edge, d, P.H, P.gat_v, st));
+    GPS_TRY(gat_fwd(a->graph, d, P.H, P.Y1, P.Wy, a->edge_attr, P.gat_v, gat->att_src, gat->att_dst, gat->lin_src.bias,
+                    a->x, gat_scores(P.gat_sc, N, E, P.H), P.xloc, P.drop(GPS_SITE_LOCAL), stats(BN_L), st));
   }
   if (local_writes_s && !P.gine && P.s_p.hi && N > 0) {   // the GatedGCN / GCN aggregation kernels write fp32 only
     ToPlanesItem it{P.s, d, (int)N, (int)d, P.s_p};
@@ -943,7 +972,7 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaStr
 
   // ---- s = norm1_local(x_loc) + norm1_attn(hA)   (gps_layer.py:194,217,222)
   if (!P.nonorm) {
-    const bool loc = P.gated || P.gine || P.gcn;
+    const bool loc = P.gated || P.gine || P.gcn || P.gat;
     const float* first = loc ? P.xloc : P.hA;
     BnView bf = loc ? bn_view(P, BN_L, a->norm1_local, N) : bn_view(P, BN_A, a->norm1_attn, N);
     const float* second = (loc && (P.attn || P.perf)) ? P.hA : nullptr;
@@ -974,14 +1003,15 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaStr
 }
 
 // =================================================================================== backward
-static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaStream_t st) {
+static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, cudaStream_t st) {
   Plan P;
-  GPS_TRY(make_plan(a, &P, true));
+  GPS_TRY(make_plan(a, &P, true, gat));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
   GPS_REQUIRE(a->workspace_bytes >= P.bwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.bwd_bytes);
   GPS_TRY(check_params(a, P));
   GPS_REQUIRE(a->grad_x_out && a->grad_x, GPS_ERR_ARG, "grad_x_out / grad_x are required");
+  GPS_REQUIRE(!P.gat || P.E == 0 || a->grad_edge_attr, GPS_ERR_ARG, "grad_edge_attr is required for GAT");
   const int64_t N = P.N, E = P.E, d = P.d;
   const int act = a->act;
   DropCfg nodrop;
@@ -992,7 +1022,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaSt
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
   auto wfork = [&](cudaStream_t from) -> int { return sd->order(from, s2); };
-  const bool two_branches = (P.gated || P.gine || P.gcn) && (P.attn || P.perf);
+  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat) && (P.attn || P.perf);
   cudaStream_t sa = two_branches ? sd->s3 : st;   // stream of the attention-branch backward
   cudaStream_t se = sd->s4;                       // stream of the edge BatchNorm backward (GatedGCN)
   const int opt = opt_flags();
@@ -1076,7 +1106,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaSt
     // reductions ride this GEMM's epilogue instead of two more passes over g_s (GPS_B200_OPT bit 64)
     fused_la = (opt & 64) && !P.nonorm && P.use_planes && g2.Ap.hi && g2.Bp.hi && N > 0 && P.train;
     if (fused_la) {
-      if (P.gated || P.gine || P.gcn) {
+      if (P.gated || P.gine || P.gcn || P.gat) {
         BnView v = bn_view(P, BN_L, a->norm1_local);
         g2.bnred[0].z = P.xloc; g2.bnred[0].ldz = (int)d; g2.bnred[0].mean = v.mean; g2.bnred[0].invstd = v.invstd;
         g2.bnred[0].sums = sums(BN_L);
@@ -1090,7 +1120,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaSt
     GPS_TRY(gemm(g2, st));
   }
 
-  const bool loc = P.gated || P.gine || P.gcn;
+  const bool loc = P.gated || P.gine || P.gcn || P.gat;
   bool chain_x = false;
   // ---- norm1_local / norm1_attn (gps_layer.py:194,217): g_xloc, g_hA
   if (loc && !P.nonorm) {
@@ -1243,6 +1273,19 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, cudaSt
     GPS_TRY(wfork(st));
     GPS_TRY(mid_done());
     g_x_local = g_xloc;
+  } else if (P.gat) {
+    // x_loc = x + drop(GATConv(x) + b): g_h = drop * g_xloc -> gY1[:, 0:d], grad_edge_attr, att_* / bias / lin_edge
+    Operand g_h;
+    GPS_TRY(dropmul(P, {g_xloc, d}, P.g_tmp3, Planes(), GPS_SITE_LOCAL, st, &g_h));
+    float* g_v = P.gat_ws;
+    GPS_TRY(gat_bwd(a->graph, d, P.H, P.Y1, P.Wy, a->edge_attr, P.gat_v, gat->att_src, gat->att_dst,
+                    gat_scores(P.gat_sc, N, E, P.H), g_h.f, P.gat_ws + P.H * d, P.gY1, P.Wy, P.gY1_p, a->grad_edge_attr,
+                    g_v, gat->grad_att_src, gat->grad_att_dst, gat->lin_src.grad_bias, P.grads_accumulate, st));
+    GPS_TRY(gat_fold_bwd(gat->lin_edge.weight, gat->att_edge, g_v, d, P.H, gat->lin_edge.grad_weight, gat->grad_att_edge,
+                         P.grads_accumulate, st));
+    GPS_TRY(wfork(st));
+    GPS_TRY(mid_done());
+    g_x_local = g_xloc;
   }
 
   if (two_branches) GPS_TRY(sd->order(sa, st));
@@ -1327,24 +1370,44 @@ extern "C" int gps_layer_plan(const GpsLayerArgs* args, GpsLayerPlan* plan) {
 
 extern "C" int gps_layer_forward(const GpsLayerArgs* args, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_forward: null args");
-  return layer_forward(args, nullptr, (cudaStream_t)stream);
+  return layer_forward(args, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward(const GpsLayerArgs* args, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_backward: null args");
-  return layer_backward(args, nullptr, (cudaStream_t)stream);
+  return layer_backward(args, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_forward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_forward_biased: null args");
   GPS_TRY(check_bias(args, bias));
-  return layer_forward(args, bias, (cudaStream_t)stream);
+  return layer_forward(args, bias, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_backward_biased: null args");
   GPS_TRY(check_bias(args, bias));
-  return layer_backward(args, bias, (cudaStream_t)stream);
+  return layer_backward(args, bias, nullptr, (cudaStream_t)stream);
+}
+
+static int check_gat(const GpsLayerArgs* a, const GpsGat* gat, const char* what) {
+  GPS_REQUIRE(a && gat, GPS_ERR_ARG, "%s: null args / gat", what);
+  GPS_REQUIRE(a->local_type == GPS_LOCAL_GAT, GPS_ERR_ARG, "%s: a GpsGat needs local_type GPS_LOCAL_GAT (got %d)", what,
+              a->local_type);
+  return GPS_OK;
+}
+
+extern "C" int gps_layer_forward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias, void* stream) {
+  GPS_TRY(check_gat(args, gat, "gps_layer_forward_gat"));
+  GPS_TRY(check_bias(args, bias));
+  return layer_forward(args, bias, gat, (cudaStream_t)stream);
+}
+
+extern "C" int gps_layer_backward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias,
+                                      void* stream) {
+  GPS_TRY(check_gat(args, gat, "gps_layer_backward_gat"));
+  GPS_TRY(check_bias(args, bias));
+  return layer_backward(args, bias, gat, (cudaStream_t)stream);
 }
 
 extern "C" int gps_linear_forward(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias,
@@ -1494,6 +1557,56 @@ extern "C" int gps_gcn_aggregate_backward(const GpsGraph* g, int64_t d, const fl
   Planes yp;
   GPS_TRY(stage_planes(gY_planes, d, &yp, "gcn_aggregate_backward gY_planes"));
   return gcn_bwd(*g, d, g_h, dinv, gY, ldg, (cudaStream_t)stream, yp);
+}
+
+// ---- stage entry points of the GAT local model (gat.cu).  Each validates its arguments before it enqueues anything.
+extern "C" int gps_gat_fold_forward(const float* W_edge, const float* att_edge, int64_t d, int64_t H, float* v,
+                                    void* stream) {
+  GPS_REQUIRE(W_edge && att_edge && v, GPS_ERR_ARG, "gat_fold_forward: null argument");
+  return gat_fold_fwd(W_edge, att_edge, d, H, v, (cudaStream_t)stream);
+}
+
+extern "C" int gps_gat_fold_backward(const float* W_edge, const float* att_edge, const float* g_v, int64_t d, int64_t H,
+                                     float* g_W_edge, float* g_att_edge, int32_t accumulate, void* stream) {
+  GPS_REQUIRE(W_edge && att_edge && g_v, GPS_ERR_ARG, "gat_fold_backward: null argument");
+  return gat_fold_bwd(W_edge, att_edge, g_v, d, H, g_W_edge, g_att_edge, accumulate != 0, (cudaStream_t)stream);
+}
+
+extern "C" int gps_gat_forward(const GpsGraph* g, int64_t d, int64_t H, const float* Y, int64_t ldy,
+                               const float* edge_attr, const float* v, const float* att_src, const float* att_dst,
+                               const float* bias, const float* x, float* scores, float* xloc, float p_drop,
+                               uint64_t seed, uint64_t offset, double* stats, void* stream) {
+  GPS_REQUIRE(g && Y && v && att_src && att_dst && bias && x && scores && xloc && (edge_attr || g->E == 0), GPS_ERR_ARG,
+              "gat_forward: null argument");
+  GPS_TRY(gat_check(d, H));
+  GPS_REQUIRE(ldy >= d && ldy % 4 == 0 && p_drop >= 0.f && p_drop < 1.f, GPS_ERR_ARG,
+              "gat_forward: ldy < d, ldy %% 4 != 0 or p_drop not in [0,1)");
+  DropCfg drop;
+  drop.p = p_drop; drop.seed = seed; drop.offset = offset; drop.site = GPS_SITE_LOCAL;
+  return gat_fwd(*g, d, H, Y, ldy, edge_attr, v, att_src, att_dst, bias, x, gat_scores(scores, g->N, g->E, H), xloc,
+                 drop, stats, (cudaStream_t)stream);
+}
+
+extern "C" int64_t gps_gat_workspace_bytes(int64_t N, int64_t E, int64_t H, int64_t d) {
+  return gat_bwd_workspace_floats(N, E, H, d) * (int64_t)sizeof(float);
+}
+
+extern "C" int gps_gat_backward(const GpsGraph* g, int64_t d, int64_t H, const float* Y, int64_t ldy,
+                                const float* edge_attr, const float* v, const float* att_src, const float* att_dst,
+                                const float* scores, const float* g_h, void* workspace, int64_t workspace_bytes,
+                                float* gY, int64_t ldg, const GpsPlanes* gY_planes, float* grad_edge_attr, float* g_v,
+                                float* g_att_src, float* g_att_dst, float* g_bias, int32_t accumulate, void* stream) {
+  GPS_REQUIRE(g && Y && v && att_src && att_dst && scores && g_h && workspace && gY && g_v && (edge_attr || g->E == 0),
+              GPS_ERR_ARG, "gat_backward: null argument");
+  GPS_TRY(gat_check(d, H));
+  GPS_REQUIRE(ldy >= d && ldg >= d && ldy % 4 == 0 && ldg % 4 == 0, GPS_ERR_ARG,
+              "gat_backward: ldy / ldg < d or not a multiple of 4");
+  GPS_REQUIRE(workspace_bytes >= gps_gat_workspace_bytes(g->N, g->E, H, d), GPS_ERR_ARG, "gat_backward: workspace too small");
+  Planes yp;
+  GPS_TRY(stage_planes(gY_planes, d, &yp, "gat_backward gY_planes"));
+  return gat_bwd(*g, d, H, Y, ldy, edge_attr, v, att_src, att_dst, gat_scores((float*)scores, g->N, g->E, H), g_h,
+                 (float*)workspace, gY, ldg, yp, grad_edge_attr, g_v, g_att_src, g_att_dst, g_bias, accumulate != 0,
+                 (cudaStream_t)stream);
 }
 
 // ---- stage entry points of the Performer (performer.cu, performer_quad.cu).  Each validates its arguments before it

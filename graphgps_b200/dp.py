@@ -27,7 +27,8 @@ import torch.distributed as dist
 _EARLY_PREFIXES = ("ff_linear1.", "ff_linear2.", "norm2.", "norm1_local.", "norm1_attn.",
                    "self_attn.out_proj.", "self_attn.to_out.")
 _LATE_PREFIXES = ("self_attn.in_proj", "self_attn.to_q.", "self_attn.to_k.", "self_attn.to_v.",
-                  "local_model.A.", "local_model.B.", "local_model.D.", "local_model.E.", "local_model.lin.")   # Wcat rows
+                  "local_model.A.", "local_model.B.", "local_model.D.", "local_model.E.", "local_model.lin.",
+                  "local_model.lin_src.")   # Wcat rows
 EARLY, MID, LATE = 0, 1, 2
 
 

@@ -20,9 +20,9 @@ import torch.nn as nn
 from . import _lib
 from .graph import graph_of
 
-_SUPPORTED_LOCAL = ("None", "CustomGatedGCN", "GINE", "GCN")
-_EDGE_LOCAL = ("CustomGatedGCN", "GINE")   # local models that read batch.edge_attr (gps_layer.py:44-53)
-_KNOWN_LOCAL = _SUPPORTED_LOCAL + ("GIN", "GENConv", "GAT", "PNA")
+_SUPPORTED_LOCAL = ("None", "CustomGatedGCN", "GINE", "GCN", "GAT")
+_EDGE_LOCAL = ("CustomGatedGCN", "GINE", "GAT")   # local models that read batch.edge_attr (gps_layer.py:44-53)
+_KNOWN_LOCAL = _SUPPORTED_LOCAL + ("GIN", "GENConv", "PNA")
 _SUPPORTED_GLOBAL = ("None", "Transformer", "BiasedTransformer", "Performer")
 _KNOWN_GLOBAL = _SUPPORTED_GLOBAL + ("BigBird",)
 _MHA_GLOBAL = ("Transformer", "BiasedTransformer")   # torch's MultiheadAttention (gps_layer.py:104-106)
@@ -120,6 +120,34 @@ class _GCNConvParams(nn.Module):
         self.bias = nn.Parameter(torch.zeros(dim))
 
 
+def _glorot_(t):
+    """PyG inits.glorot: U(-a, a), a = sqrt(6 / (size(-2) + size(-1)))."""
+    a = math.sqrt(6.0 / (t.size(-2) + t.size(-1)))
+    with torch.no_grad():
+        t.uniform_(-a, a)
+    return t
+
+
+class _GATConvParams(nn.Module):
+    """Names of PyG 2.2 GATConv(dim_h, dim_h // heads, heads=heads, edge_dim=dim_h) as built at gps_layer.py:70-74:
+    lin_src.weight [d,d] and lin_edge.weight [d,d] (no bias, glorot), att_src / att_dst / att_edge [1,H,C] (glorot over
+    (H, C)), bias [d] (zeros).  lin_dst is the same module as lin_src, so state_dict() holds both lin_src.weight and
+    lin_dst.weight while named_parameters() yields lin_src.weight only."""
+
+    def __init__(self, dim, heads):
+        super().__init__()
+        C = dim // heads
+        self.lin_src = nn.Linear(dim, heads * C, bias=False)
+        self.lin_dst = self.lin_src
+        self.att_src = nn.Parameter(torch.empty(1, heads, C))
+        self.att_dst = nn.Parameter(torch.empty(1, heads, C))
+        self.lin_edge = nn.Linear(dim, heads * C, bias=False)
+        self.att_edge = nn.Parameter(torch.empty(1, heads, C))
+        self.bias = nn.Parameter(torch.zeros(heads * C))
+        for t in (self.lin_src.weight, self.lin_edge.weight, self.att_src, self.att_dst, self.att_edge):
+            _glorot_(t)
+
+
 def _orthogonal_gaussian_matrix(nb_rows, nb_cols):
     """Random-feature projection drawn once at construction (performer_layer.py:163-195, scaling=0)."""
     blocks = []
@@ -183,6 +211,7 @@ class _GPSLayerFn(torch.autograd.Function):
         N, E, d = gs.N, gs.E, layer.dim_h
         x_out = torch.empty_like(x)
         e_out = torch.empty_like(e) if layer.local_gnn_type == "CustomGatedGCN" else None
+        gat = layer._gat_args(named) if layer.local_gnn_type == "GAT" else None
         plan = layer._plan(args, gs)
         saved = torch.empty(max(plan[0], 256), dtype=torch.uint8, device=dev)
         ws = _workspace(dev, plan[1])
@@ -197,7 +226,10 @@ class _GPSLayerFn(torch.autograd.Function):
             args.offset, args.offset_dev = 0, snap.data_ptr()
         stream = torch.cuda.current_stream(dev).cuda_stream
         ctx.nmax = gs.nmax if bias.numel() else 0
-        if ctx.nmax:
+        if gat is not None:
+            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)) if ctx.nmax else None
+            _lib.check(lib.gps_layer_forward_gat(C.byref(args), C.byref(gat), ab, stream), "gps_layer_forward_gat")
+        elif ctx.nmax:
             ab = _lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)
             _lib.check(lib.gps_layer_forward_biased(C.byref(args), C.byref(ab), stream), "gps_layer_forward_biased")
         else:
@@ -262,9 +294,13 @@ class _GPSLayerFn(torch.autograd.Function):
             args.ev_grads_early, args.ev_grads_mid, args.ev_grads_done = (e.cuda_event for e in evs)
         stream = torch.cuda.current_stream(dev).cuda_stream
         g_bias = None
-        if ctx.nmax:
-            if ctx.needs_input_grad[5]:
-                g_bias = torch.empty_like(bias)
+        if ctx.nmax and ctx.needs_input_grad[5]:
+            g_bias = torch.empty_like(bias)
+        if layer.local_gnn_type == "GAT":
+            gat = layer._gat_args(named, grads)
+            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))) if ctx.nmax else None
+            _lib.check(lib.gps_layer_backward_gat(C.byref(args), C.byref(gat), ab, stream), "gps_layer_backward_gat")
+        elif ctx.nmax:
             ab = _lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))
             _lib.check(lib.gps_layer_backward_biased(C.byref(args), C.byref(ab), stream), "gps_layer_backward_biased")
         else:
@@ -331,6 +367,11 @@ class GPSLayer(nn.Module):
         elif local_gnn_type == "GCN":
             self.local_gnn_with_edge_attr = False
             self.local_model = _GCNConvParams(dim_h)
+        elif local_gnn_type == "GAT":
+            # the reference builds GATConv(out_channels=dim_h // num_heads) and only fails at the residual add
+            if num_heads < 1 or dim_h % num_heads != 0:
+                raise ValueError(f"GAT needs dim_h ({dim_h}) divisible by num_heads ({num_heads})")
+            self.local_model = _GATConvParams(dim_h, num_heads)
         else:
             self.local_model = _GatedGCNParams(dim_h, act, self._eslap)
         self.local_gnn_type = local_gnn_type
@@ -536,6 +577,16 @@ class GPSLayer(nn.Module):
             a.norm2 = bn("norm2", self.norm2)
         a.ff1, a.ff2 = lin("ff_linear1"), lin("ff_linear2")
         return a
+
+    def _gat_args(self, named, grads=None):
+        """GpsGat of the GAT local model (gps_b200.h): lin_src carries GATConv.bias, as GCNConv's lin / bias pair."""
+        g = grads or {}
+        p = "local_model."
+        return _lib.GpsGat(
+            _lin(named[p + "lin_src.weight"], named[p + "bias"], g.get(p + "lin_src.weight"), g.get(p + "bias")),
+            _lin(named[p + "lin_edge.weight"], None, g.get(p + "lin_edge.weight")),
+            *(_lib.ptr(named[p + n]) for n in ("att_src", "att_dst", "att_edge")),
+            *(_lib.ptr(g.get(p + n)) for n in ("att_src", "att_dst", "att_edge")))
 
     @property
     def _gine_eps_host(self):

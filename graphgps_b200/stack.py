@@ -107,7 +107,10 @@ class GPSStack(nn.Module):
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, capture_error_mode="thread_local"):
             body()
-        return CapturedStep(g, x_in, e_in, res["x"], res["e"], pe_in, ab_in)
+        step = CapturedStep(g, x_in, e_in, res["x"], res["e"], pe_in, ab_in)
+        # the graph's kernels read the batch's index tensors and its device-side structure: keep them alive with it
+        step._keep = (batch, gs)
+        return step
 
 
 class CapturedStep:

@@ -36,7 +36,7 @@ extern "C" {
 enum { GPS_OK = 0, GPS_ERR_ARG = -1, GPS_ERR_UNSUPPORTED = -2, GPS_ERR_CUDA = -3 };
 
 /* local_gnn_type / global_model_type of GPSLayer.__init__ (gps_layer.py:20-24,44-122) */
-enum { GPS_LOCAL_NONE = 0, GPS_LOCAL_GATEDGCN = 1, GPS_LOCAL_GINE = 2, GPS_LOCAL_GCN = 3 };
+enum { GPS_LOCAL_NONE = 0, GPS_LOCAL_GATEDGCN = 1, GPS_LOCAL_GINE = 2, GPS_LOCAL_GCN = 3, GPS_LOCAL_GAT = 4 };
 enum { GPS_GLOBAL_NONE = 0, GPS_GLOBAL_TRANSFORMER = 1, GPS_GLOBAL_PERFORMER = 2 };
 /* register.act_dict keys used by shipped configs (gps_layer.py:33) */
 enum { GPS_ACT_RELU = 0, GPS_ACT_GELU = 1 };
@@ -253,6 +253,35 @@ typedef struct {
 int gps_layer_forward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream);
 int gps_layer_backward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream);
 
+/* GAT local model (local_type == GPS_LOCAL_GAT): PyG 2.2 GATConv(dim_h, dim_h / heads, heads=heads, edge_dim=dim_h)
+ * with its defaults (concat, negative_slope 0.2, no attention dropout, add_self_loops with fill_value 'mean', bias),
+ * gps_layer.py:70-74,183-189.  H = GpsLayerArgs.heads heads of C = d / H channels each (d % H != 0 is GPS_ERR_ARG).
+ * Existing self-loop edges are dropped and one loop per node is added whose edge attribute is the mean of the node's
+ * remaining in-edge attributes (0 without any); their grad_edge_attr rows are 0.  edge_attr is read (non-NULL when
+ * E > 0) and batch.edge_attr is not updated.  Parameters:
+ *   lin_src   weight = local_model.lin_src.weight [d,d] (lin_dst is the same module), bias = local_model.bias [d]
+ *             (added after the aggregation); its gradients: grad_weight with the fused node projection (final at
+ *             ev_grads_done), grad_bias final at ev_grads_mid;
+ *   lin_edge  weight = local_model.lin_edge.weight [d,d] (no bias);
+ *   att_src / att_dst / att_edge = local_model.att_{src,dst,edge} [1,H,C], and their gradients, final at ev_grads_mid. */
+typedef struct {
+  GpsLinear lin_src;
+  GpsLinear lin_edge;
+  const float* att_src;
+  const float* att_dst;
+  const float* att_edge;
+  float* grad_att_src;
+  float* grad_att_dst;
+  float* grad_att_edge;
+} GpsGat;
+
+/* gps_layer_forward / _backward of a GAT layer; bias: GpsAttnBias of a BiasedTransformer global model or NULL.
+ * gps_layer_plan sizes GAT from local_type alone.  The plain and _biased calls with local_type == GPS_LOCAL_GAT, and
+ * these with a NULL gat, return GPS_ERR_ARG before any CUDA call, as does a NULL edge_attr (E > 0) or, in the
+ * backward, grad_edge_attr (E > 0). */
+int gps_layer_forward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias, void* stream);
+int gps_layer_backward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Stage-level entry points (the same kernels the layer calls; exported so the parity tests can
  * pin each stage against the oracle separately).
@@ -327,6 +356,32 @@ int gps_gcn_aggregate_forward(const GpsGraph* g, int64_t d, const float* Y, int6
 /* its backward: gY [N, ldg] = A_hat^T g_h (+ optional bf16 hi/lo planes of it) */
 int gps_gcn_aggregate_backward(const GpsGraph* g, int64_t d, const float* g_h, const float* dinv, float* gY,
                                int64_t ldg, const GpsPlanes* gY_planes, void* stream);
+
+/* GAT stage entry points (the functions the GAT layer calls).  H > 0 with d % H == 0 and d % 4 == 0, d <= 4096 (else
+ * GPS_ERR_UNSUPPORTED; d % H != 0 is GPS_ERR_ARG); NULL pointers are GPS_ERR_ARG; both before any CUDA call.  C = d / H.
+ * fold: v [H, d] = W_edge[hC:(h+1)C, :]^T att_edge[h] (W_edge = lin_edge.weight [d,d], att_edge [H*C]); its backward
+ * writes (accumulate != 0: adds) g_W_edge [d,d] and g_att_edge [H*C] from g_v [H, d] (either output may be NULL). */
+int gps_gat_fold_forward(const float* W_edge, const float* att_edge, int64_t d, int64_t H, float* v, void* stream);
+int gps_gat_fold_backward(const float* W_edge, const float* att_edge, const float* g_v, int64_t d, int64_t H,
+                          float* g_W_edge, float* g_att_edge, int32_t accumulate, void* stream);
+/* xloc [N,d] = x + dropout(GATConv aggregation of Y + bias) with the local dropout site (gps_dropout_mask site 3);
+ * Y [N, ldy] (ldy % 4 == 0) = x lin_src^T; edge_attr [E,d]; v from the fold; stats: optional double [2][d] column sums
+ * of xloc.  scores: (4N + E) H floats written: a_src, a_dst, a_self (the added loop's edge score), lse (log-sum-exp of
+ * each (node, head) softmax), each [N, H], then a_edge [E, H] in edge-id order. */
+int gps_gat_forward(const GpsGraph* g, int64_t d, int64_t H, const float* Y, int64_t ldy, const float* edge_attr,
+                    const float* v, const float* att_src, const float* att_dst, const float* bias, const float* x,
+                    float* scores, float* xloc, float p_drop, uint64_t seed, uint64_t offset, double* stats,
+                    void* stream);
+/* bytes of scratch gps_gat_backward needs */
+int64_t gps_gat_workspace_bytes(int64_t N, int64_t E, int64_t H, int64_t d);
+/* its backward from g_h [N,d] (the gradient of the aggregation output, i.e. of GATConv's output): gY [N, ldg]
+ * (+ optional bf16 planes), grad_edge_attr [E,d] (NULL = not needed), g_v [H,d], all written; g_att_src / g_att_dst /
+ * g_bias [d] written, or added when accumulate != 0 (each NULL = not needed). */
+int gps_gat_backward(const GpsGraph* g, int64_t d, int64_t H, const float* Y, int64_t ldy, const float* edge_attr,
+                     const float* v, const float* att_src, const float* att_dst, const float* scores, const float* g_h,
+                     void* workspace, int64_t workspace_bytes, float* gY, int64_t ldg, const GpsPlanes* gY_planes,
+                     float* grad_edge_attr, float* g_v, float* g_att_src, float* g_att_dst, float* g_bias,
+                     int32_t accumulate, void* stream);
 
 /* Performer stage entry points (FAVOR+, performer_layer.py:119-144,200-205), the calls one layer makes, in order.
  * They take dim_head == 64 and 256 < m <= 272 features (else GPS_ERR_UNSUPPORTED), H > 0 and N * H * 272 < 2^31 (else
