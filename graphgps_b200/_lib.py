@@ -14,7 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgps_b200.so")
 
 GPS_OK, GPS_ERR_ARG, GPS_ERR_UNSUPPORTED, GPS_ERR_CUDA = 0, -1, -2, -3
-LOCAL = {"None": 0, "CustomGatedGCN": 1, "GINE": 2, "GCN": 3, "GAT": 4}
+LOCAL = {"None": 0, "CustomGatedGCN": 1, "GINE": 2, "GCN": 3, "GAT": 4, "GENConv": 5}
 GLOBAL = {"None": 0, "Transformer": 1, "Performer": 2}
 ACT = {"relu": 0, "gelu": 1}
 PRECISION = {"fp32": 0, "bf16": 1}
@@ -86,6 +86,11 @@ class GpsGat(C.Structure):
                 ("grad_att_src", _fp), ("grad_att_dst", _fp), ("grad_att_edge", _fp)]
 
 
+class GpsGenConv(C.Structure):
+    """GENConv local model: lin0 = local_model.mlp.0, bn = local_model.mlp.1 [2d], lin1 = local_model.mlp.4 (no biases)."""
+    _fields_ = [("lin0", GpsLinear), ("bn", GpsBatchNorm), ("lin1", GpsLinear)]
+
+
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
                 ("bwd_workspace_bytes", C.c_int64), ("fwd_launches", C.c_int64),
@@ -107,6 +112,10 @@ SYMBOLS = {
     "gps_layer_backward_biased": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsAttnBias), _fp]),
     "gps_layer_forward_gat": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGat), C.POINTER(GpsAttnBias), _fp]),
     "gps_layer_backward_gat": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGat), C.POINTER(GpsAttnBias), _fp]),
+    "gps_layer_forward_genconv": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGenConv), C.POINTER(GpsAttnBias),
+                                            _fp]),
+    "gps_layer_backward_genconv": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGenConv), C.POINTER(GpsAttnBias),
+                                             _fp]),
     "gps_linear_forward": (C.c_int, [_fp, _i64, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _fp]),
     "gps_gemm": (C.c_int, [_fp, _i64, _i32, _fp, _i64, _i32, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _fp]),
     "gps_gatedgcn_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _i64, _fp, _fp,
@@ -131,6 +140,9 @@ SYMBOLS = {
     "gps_gat_workspace_bytes": (_i64, [_i64, _i64, _i64, _i64]),
     "gps_gat_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _i64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i64,
                                    _fp, _i64, C.POINTER(GpsPlanes), _fp, _fp, _fp, _fp, _fp, _i32, _fp]),
+    "gps_genconv_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _fp, _fp]),
+    "gps_genconv_aggregate_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp,
+                                                 _fp]),
     "gps_performer_prep": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp]),
     "gps_performer_features_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp,
                                                  _fp, _fp]),

@@ -137,6 +137,14 @@ int gat_bwd(const GpsGraph& g, int64_t d, int64_t H, const float* Y, int64_t ldy
             Planes gYp, float* grad_ea, float* g_v, float* g_att_src, float* g_att_dst, float* g_bias, bool accumulate,
             cudaStream_t stream);
 
+// GENConv (PyG GENConv, softmax aggregation, genconv.cu).  Forward: agg, lse (log-sum-exp of each (node, channel)
+// segment, 0 without in-edges) and u = agg + x, all [N, d], plus u's planes.  Backward, dst ordered:
+// g_e[k] = g_u[dst] alpha_k (1 + m_k - agg[dst]) [x_src + e_k > 0]; the src-ordered pass is gine_bwd_src with eps = 0.
+int genconv_fwd(const GpsGraph& g, int64_t d, const float* x, const float* e, float* agg, float* lse, float* u,
+                cudaStream_t stream, Planes up = Planes());
+int genconv_bwd_dst(const GpsGraph& g, int64_t d, const float* x, const float* e, const float* agg, const float* lse,
+                    const float* g_u, float* g_e, cudaStream_t stream);
+
 // ---- attention ------------------------------------------------------------------------------
 int attention_fwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, const float* K, const float* V,
                   int64_t ld, float* O, int64_t ldo, float* lse, float p_drop, uint64_t seed, uint64_t offset,

@@ -226,6 +226,14 @@ struct Plan {
   bool gat;
   const GpsGat* gatp;
   float *gat_v, *gat_sc, *gat_ws;
+  // GENConv (genconv.cu): the caller's GpsGenConv (NULL when only sizes are wanted).  Saved: agg (in `agg`), lse, u [N,d],
+  // h1 = u W0^T and r = relu(mlp.1(h1)) [N,2d], and mlp.1's batch statistics in a 2d-wide slot of their own (gen_bn:
+  // mean | invstd; the BN_* slots are d wide).  Workspace: mlp.1's column sums (gen_fstats / gen_bsums, [2][2d] doubles),
+  // backward g_r, g_h1 [N,2d] and g_u [N,d].
+  bool gen;
+  const GpsGenConv* genp;
+  float *gen_lse, *gen_u, *gen_h1, *gen_r, *gen_bn, *gen_gr, *gen_gh1, *gen_gu;
+  double *gen_fstats, *gen_bsums;
   // GPS_NORM_NONE: no norm1_local / norm1_attn / norm2.  Only the local model's own BatchNorms (BN_X, BN_E) remain, so
   // nbn = 2 statistics slots instead of BN_COUNT; s = x_loc + hA is written by the GEMM that closes the second branch
   // and x_out by the FF2 GEMM.
@@ -251,6 +259,7 @@ struct Plan {
   Planes x_p, e_p, O_p, s_p, hid_p, agg_p, h1_p, Wcat_p, C_p, out_p, ff1_p, ff2_p, g0_p, g1_p, pq_p, pk_p, pv_p;
   Planes gt_p, ghid_p, ghA_p, ge_p, gY1_p, gtmp_p, gtmp2_p, gtmp3_p, gl1_p, gh1_p;
   Planes gs_p;         // GPS_NORM_NONE: planes of g_s, the upstream gradient of both branches
+  Planes gen_u_p, gen_r_p, gen_gh1_p, mlp0_p, mlp4_p;   // GENConv: u, r, g_h1 and the weights of mlp.0 / mlp.4
   Planes qkv_p;        // Q | K | V per head, padded to hd_pad columns: operands of the wgmma attention
   bool attn_tc;        // softmax attention on the tensor cores (attention_tc.cu)
   // the weights with operand planes, in the order their planes are allocated and converted (list_weights)
@@ -313,6 +322,10 @@ static void list_weights(const GpsLayerArgs* a, Plan* P) {
     add(a->gine_lin0, d, d, &Plan::g0_p);
     add(a->gine_lin1, d, d, &Plan::g1_p);
   }
+  if (P->gen) {   // GENConv's MLP Linears have no bias
+    add(P->genp ? P->genp->lin0 : kNoLinear, 2 * d, d, &Plan::mlp0_p, false);
+    add(P->genp ? P->genp->lin1 : kNoLinear, d, 2 * d, &Plan::mlp4_p, false);
+  }
   if (P->perf) {
     add(a->perf_q, P->inner, d, &Plan::pq_p);
     add(a->perf_k, P->inner, d, &Plan::pk_p);
@@ -328,7 +341,8 @@ static Planes caller_planes(const GpsPlanes& g, int64_t d, int precision) {
   return Planes{(__nv_bfloat16*)g.hi, lo ? (__nv_bfloat16*)g.lo : nullptr, g.ld};
 }
 
-static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* gat = nullptr) {
+static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* gat = nullptr,
+                     const GpsGenConv* gen = nullptr) {
   memset(P, 0, sizeof(*P));
   GPS_REQUIRE(a, GPS_ERR_ARG, "null args");
   P->N = a->graph.N;
@@ -342,9 +356,14 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   P->gcn = a->local_type == GPS_LOCAL_GCN;
   P->gat = a->local_type == GPS_LOCAL_GAT;
   P->gatp = gat;
-  GPS_REQUIRE(a->local_type == GPS_LOCAL_NONE || P->gated || P->gine || P->gcn || P->gat, GPS_ERR_ARG,
+  P->gen = a->local_type == GPS_LOCAL_GENCONV;
+  P->genp = gen;
+  GPS_REQUIRE(a->local_type == GPS_LOCAL_NONE || P->gated || P->gine || P->gcn || P->gat || P->gen, GPS_ERR_ARG,
               "unknown local_type %d", a->local_type);
   if (P->gat) GPS_TRY(gat_check(a->d, a->heads));
+  GPS_REQUIRE(!P->gen || a->d <= 2048, GPS_ERR_UNSUPPORTED,
+              "GENConv needs dim_h <= 2048: its 2 dim_h-wide BatchNorm runs on the row-wise stages (got %lld)",
+              (long long)a->d);
   P->eslap = a->pe != nullptr;
   GPS_REQUIRE(!P->eslap || P->gated, GPS_ERR_ARG, "pe (EquivStableLapPE) is read by the GatedGCN local model only");
   GPS_REQUIRE(!P->eslap || a->pe_dim >= 1, GPS_ERR_ARG, "pe_dim must be >= 1 (got %lld)", (long long)a->pe_dim);
@@ -413,7 +432,15 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     P->gat_v = S.alloc<float>(P->H * d);
     P->gat_sc = S.alloc<float>((4 * N + E) * P->H);
   }
-  const bool loc = P->gated || P->gine || P->gcn || P->gat;
+  if (P->gen) {
+    P->agg = S.alloc<float>(N * d);
+    P->gen_lse = S.alloc<float>(N * d);
+    P->gen_u = S.alloc<float>(N * d);
+    P->gen_h1 = S.alloc<float>(N * 2 * d);
+    P->gen_r = S.alloc<float>(N * 2 * d);
+    P->gen_bn = S.alloc<float>(2 * 2 * d);
+  }
+  const bool loc = P->gated || P->gine || P->gcn || P->gat || P->gen;
   if (loc && !P->nonorm) P->xloc = S.alloc<float>(N * d);   // read by norm1_local's backward
   if (P->attn) {
     P->O = S.alloc<float>(N * d);
@@ -472,6 +499,10 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
       P->agg_p = mkplanes(S, N, d);
       P->h1_p = mkplanes(S, N, d);
     }
+    if (P->gen) {
+      P->gen_u_p = mkplanes(S, N, d);
+      P->gen_r_p = mkplanes(S, N, 2 * d);
+    }
     // weight planes: in the caller's persistent buffer when one is given (packed once per optimiser step), else in `saved`
     Arena Wa(bind ? a->wplanes : nullptr, a->wplanes_bytes);
     Arena& WA = bind && a->wplanes != nullptr ? Wa : S;
@@ -491,6 +522,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   // forward and backward share the caller's workspace (never live at the same time)
   Arena F(bind ? a->workspace : nullptr, a->workspace_bytes);
   P->fstats = F.alloc<double>(P->nbn * 2 * d);
+  if (P->gen) P->gen_fstats = F.alloc<double>(2 * 2 * d);
   if (P->nonorm && loc) {
     // x_loc is an operand of the GEMM that writes s (and of nothing in the backward pass); a lone local model writes s
     P->xloc = (P->attn || P->perf) ? F.alloc<float>(N * d) : P->s;
@@ -549,6 +581,13 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     P->g_xl = Bk.alloc<float>(N * d);
   }
   if (P->gat) P->gat_ws = Bk.alloc<float>(P->H * d + gat_bwd_workspace_floats(N, E, P->H, d));
+  if (P->gen) {
+    P->gen_bsums = Bk.alloc<double>(2 * 2 * d);
+    P->gen_gr = Bk.alloc<float>(N * 2 * d);
+    P->gen_gh1 = Bk.alloc<float>(N * 2 * d);
+    P->gen_gu = Bk.alloc<float>(N * d);
+    P->g_xl = Bk.alloc<float>(N * d);
+  }
   if (P->use_planes) {
     P->gt_p = mkplanes(Bk, N, d);
     P->ghid_p = mkplanes(Bk, N, 2 * d);
@@ -565,6 +604,10 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
       if (!P->nonorm) P->gl1_p = mkplanes(Bk, N, d);
       P->gh1_p = mkplanes(Bk, N, d);
     }
+    if (P->gen) {
+      if (!P->nonorm) P->gl1_p = mkplanes(Bk, N, d);
+      P->gen_gh1_p = mkplanes(Bk, N, 2 * d);
+    }
   }
   P->bwd_bytes = Bk.used;
   return GPS_OK;
@@ -574,14 +617,17 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
 // per-column affine map and its backward has no batch terms.  Training backward: the batch statistics the forward pass
 // saved (mode 0).  Training forward, over fwd_rows rows: the consumer kernel finalises the statistics from the
 // producer's column sums, saves them for the backward and updates the running statistics (mode 1).
-static BnView bn_view(const Plan& P, int which, const GpsBatchNorm& bn, int64_t fwd_rows = -1) {
+// The statistics slot of a BatchNorm over w columns: saved [mean | invstd] (2w floats) and the forward's column sums
+// (2w doubles).
+static BnView bn_view_at(const Plan& P, float* saved, double* fsums, int64_t w, const GpsBatchNorm& bn,
+                         int64_t fwd_rows) {
   const bool fwd = fwd_rows >= 0;
   BnView v;
-  v.mean = P.bnbuf + (int64_t)which * 2 * P.d;
-  v.invstd = v.mean + P.d;
+  v.mean = saved;
+  v.invstd = v.mean + w;
   v.gamma = bn.weight;
   v.beta = bn.bias;
-  if (fwd) v.d = P.d;
+  if (fwd) v.d = w;
   if (fwd || !P.train) {
     v.running_mean = bn.running_mean;
     v.running_var = bn.running_var;
@@ -591,14 +637,21 @@ static BnView bn_view(const Plan& P, int which, const GpsBatchNorm& bn, int64_t 
   } else if (fwd) {
     const int64_t n = fwd_rows;
     v.mode = 1;
-    v.sums = P.fstats + (int64_t)which * 2 * P.d;
+    v.sums = fsums;
     v.inv_n = 1.0 / (double)(n > 0 ? n : 1);
     v.unbias = n > 1 ? (double)n / (double)(n - 1) : 1.0;
-    v.save_mean = P.bnbuf + (int64_t)which * 2 * P.d;
-    v.save_invstd = v.save_mean + P.d;
+    v.save_mean = saved;
+    v.save_invstd = v.save_mean + w;
     v.nbt = (long long*)bn.num_batches_tracked;
   }
   return v;
+}
+static BnView bn_view(const Plan& P, int which, const GpsBatchNorm& bn, int64_t fwd_rows = -1) {
+  return bn_view_at(P, P.bnbuf + (int64_t)which * 2 * P.d, P.fstats + (int64_t)which * 2 * P.d, P.d, bn, fwd_rows);
+}
+// GENConv's mlp.1, a BatchNorm over 2d columns with its own slot
+static BnView gen_bn_view(const Plan& P, const GpsBatchNorm& bn, int64_t fwd_rows = -1) {
+  return bn_view_at(P, P.gen_bn, P.gen_fstats, 2 * P.d, bn, fwd_rows);
 }
 
 static PackDesc pack_desc(const Plan& P) {
@@ -624,7 +677,7 @@ static int check_bn(const GpsBatchNorm& b, const char* name) {
 }
 
 static int check_params(const GpsLayerArgs* a, const Plan& P) {
-  GPS_REQUIRE(a->x && (P.E == 0 || a->edge_attr || !(P.gated || P.gine || P.gat)), GPS_ERR_ARG,
+  GPS_REQUIRE(a->x && (P.E == 0 || a->edge_attr || !(P.gated || P.gine || P.gat || P.gen)), GPS_ERR_ARG,
               "missing x / edge_attr");
   if (P.gated) {
     GPS_TRY(check_linear(a->gcn_A, "local_model.A", true));
@@ -652,8 +705,17 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
     GPS_REQUIRE(P.gatp->att_src && P.gatp->att_dst && P.gatp->att_edge, GPS_ERR_ARG,
                 "missing parameter local_model.att_{src,dst,edge}");
   }
+  if (P.gen) {
+    GPS_REQUIRE(P.genp, GPS_ERR_ARG, "local_type GPS_LOCAL_GENCONV needs gps_layer_forward_genconv / "
+                "gps_layer_backward_genconv with a GpsGenConv");
+    GPS_TRY(check_linear(P.genp->lin0, "local_model.mlp.0", false));
+    GPS_TRY(check_bn(P.genp->bn, "local_model.mlp.1"));
+    GPS_REQUIRE(P.genp->bn.running_mean && P.genp->bn.running_var, GPS_ERR_ARG,
+                "missing buffer local_model.mlp.1.running_{mean,var}");
+    GPS_TRY(check_linear(P.genp->lin1, "local_model.mlp.4", false));
+  }
   const bool bn = !P.nonorm;   // norm1_local / norm1_attn / norm2 exist in BatchNorm mode only
-  if ((P.gated || P.gine || P.gcn || P.gat) && bn) GPS_TRY(check_bn(a->norm1_local, "norm1_local"));
+  if ((P.gated || P.gine || P.gcn || P.gat || P.gen) && bn) GPS_TRY(check_bn(a->norm1_local, "norm1_local"));
   if (P.attn) {
     GPS_TRY(check_linear(a->attn_in, "self_attn.in_proj", true));
     GPS_TRY(check_linear(a->attn_out, "self_attn.out_proj", true));
@@ -789,9 +851,10 @@ static int check_bias(const GpsLayerArgs* a, const GpsAttnBias* bias) {
 }
 
 // =================================================================================== forward
-static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, cudaStream_t st) {
+static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, const GpsGenConv* gen,
+                         cudaStream_t st) {
   Plan P;
-  GPS_TRY(make_plan(a, &P, true, gat));
+  GPS_TRY(make_plan(a, &P, true, gat, gen));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
   GPS_REQUIRE(a->workspace_bytes >= P.fwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.fwd_bytes);
@@ -805,10 +868,11 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
   };
 
   if (P.train) GPS_CUDA(cudaMemsetAsync(P.fstats, 0, (size_t)P.nbn * 2 * d * sizeof(double), st));
+  if (P.train && P.gen) GPS_CUDA(cudaMemsetAsync(P.gen_fstats, 0, (size_t)2 * 2 * d * sizeof(double), st));
   Side* sd;
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
-  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat) && (P.attn || P.perf);
+  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen) && (P.attn || P.perf);
   // GPS_NORM_NONE: the producer that closes the last branch writes s = x_loc + hA with its planes (x_loc = s when the
   // local model is alone)
   const bool local_writes_s = P.nonorm && !(P.attn || P.perf);
@@ -917,8 +981,25 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
     GPS_TRY(gat_fold_fwd(gat->lin_edge.weight, gat->att_edge, d, P.H, P.gat_v, st));
     GPS_TRY(gat_fwd(a->graph, d, P.H, P.Y1, P.Wy, a->edge_attr, P.gat_v, gat->att_src, gat->att_dst, gat->lin_src.bias,
                     a->x, gat_scores(P.gat_sc, N, E, P.H), P.xloc, P.drop(GPS_SITE_LOCAL), stats(BN_L), st));
+  } else if (P.gen) {
+    // u = agg + x, agg = softmax aggregation of relu(x_j + e_ij) + 1e-7 over each node's in-edges (GENConv.forward)
+    GPS_TRY(genconv_fwd(a->graph, d, a->x, a->edge_attr, P.agg, P.gen_lse, P.gen_u, st, P.gen_u_p));
+    // h1 = u W0^T [N, 2d], with mlp.1's column sums in training mode
+    GemmParams g = linear_fwd(P, N, 2 * d, d, {P.gen_u, d, P.gen_u_p}, {gen->lin0.weight, d, P.mlp0_p}, P.gen_h1, 2 * d);
+    g.stats = P.train ? P.gen_fstats : nullptr;
+    GPS_TRY(gemm(g, st));
+    // r = relu(mlp.1(h1)) (mlp.2; mlp.3 is Dropout(0))
+    GPS_TRY(bn_act_residual(P.gen_h1, 2 * d, nullptr, P.gen_r, N, 2 * d, gen_bn_view(P, gen->bn, N), GPS_ACT_RELU,
+                            DropCfg(), nullptr, st, P.gen_r_p));
+    // x_loc = x + drop(r W4^T)  (gps_layer.py:188-189)
+    GemmParams g2 = linear_fwd(P, N, d, 2 * d, {P.gen_r, 2 * d, P.gen_r_p}, {gen->lin1.weight, 2 * d, P.mlp4_p}, P.xloc,
+                               d);
+    g2.R1 = a->x; g2.ldr1 = (int)d; g2.stats = stats(BN_L);
+    if (local_writes_s) g2.Cp = P.s_p;
+    set_dropout(g2, P.drop(GPS_SITE_LOCAL));
+    GPS_TRY(gemm(g2, st));
   }
-  if (local_writes_s && !P.gine && P.s_p.hi && N > 0) {   // the GatedGCN / GCN aggregation kernels write fp32 only
+  if (local_writes_s && !P.gine && !P.gen && P.s_p.hi && N > 0) {   // the GatedGCN / GCN / GAT kernels write fp32 only
     ToPlanesItem it{P.s, d, (int)N, (int)d, P.s_p};
     GPS_TRY(to_planes(&it, 1, st));
   }
@@ -972,7 +1053,7 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
 
   // ---- s = norm1_local(x_loc) + norm1_attn(hA)   (gps_layer.py:194,217,222)
   if (!P.nonorm) {
-    const bool loc = P.gated || P.gine || P.gcn || P.gat;
+    const bool loc = P.gated || P.gine || P.gcn || P.gat || P.gen;
     const float* first = loc ? P.xloc : P.hA;
     BnView bf = loc ? bn_view(P, BN_L, a->norm1_local, N) : bn_view(P, BN_A, a->norm1_attn, N);
     const float* second = (loc && (P.attn || P.perf)) ? P.hA : nullptr;
@@ -1003,26 +1084,29 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
 }
 
 // =================================================================================== backward
-static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, cudaStream_t st) {
+static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, const GpsGenConv* gen,
+                          cudaStream_t st) {
   Plan P;
-  GPS_TRY(make_plan(a, &P, true, gat));
+  GPS_TRY(make_plan(a, &P, true, gat, gen));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
   GPS_REQUIRE(a->workspace_bytes >= P.bwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.bwd_bytes);
   GPS_TRY(check_params(a, P));
   GPS_REQUIRE(a->grad_x_out && a->grad_x, GPS_ERR_ARG, "grad_x_out / grad_x are required");
   GPS_REQUIRE(!P.gat || P.E == 0 || a->grad_edge_attr, GPS_ERR_ARG, "grad_edge_attr is required for GAT");
+  GPS_REQUIRE(!P.gen || P.E == 0 || a->grad_edge_attr, GPS_ERR_ARG, "grad_edge_attr is required for GENConv");
   const int64_t N = P.N, E = P.E, d = P.d;
   const int act = a->act;
   DropCfg nodrop;
   auto sums = [&](int which) { return P.bsums + (int64_t)which * 2 * d; };
   GPS_CUDA(cudaMemsetAsync(P.bsums, 0, (size_t)P.nbn * 2 * d * sizeof(double), st));
+  if (P.gen) GPS_CUDA(cudaMemsetAsync(P.gen_bsums, 0, (size_t)2 * 2 * d * sizeof(double), st));
   // weight-gradient GEMMs run on the side stream, each forked where its operands become final
   Side* sd;
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
   auto wfork = [&](cudaStream_t from) -> int { return sd->order(from, s2); };
-  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat) && (P.attn || P.perf);
+  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen) && (P.attn || P.perf);
   cudaStream_t sa = two_branches ? sd->s3 : st;   // stream of the attention-branch backward
   cudaStream_t se = sd->s4;                       // stream of the edge BatchNorm backward (GatedGCN)
   const int opt = opt_flags();
@@ -1106,7 +1190,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     // reductions ride this GEMM's epilogue instead of two more passes over g_s (GPS_B200_OPT bit 64)
     fused_la = (opt & 64) && !P.nonorm && P.use_planes && g2.Ap.hi && g2.Bp.hi && N > 0 && P.train;
     if (fused_la) {
-      if (P.gated || P.gine || P.gcn || P.gat) {
+      if (P.gated || P.gine || P.gcn || P.gat || P.gen) {
         BnView v = bn_view(P, BN_L, a->norm1_local);
         g2.bnred[0].z = P.xloc; g2.bnred[0].ldz = (int)d; g2.bnred[0].mean = v.mean; g2.bnred[0].invstd = v.invstd;
         g2.bnred[0].sums = sums(BN_L);
@@ -1120,7 +1204,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     GPS_TRY(gemm(g2, st));
   }
 
-  const bool loc = P.gated || P.gine || P.gcn || P.gat;
+  const bool loc = P.gated || P.gine || P.gcn || P.gat || P.gen;
   bool chain_x = false;
   // ---- norm1_local / norm1_attn (gps_layer.py:194,217): g_xloc, g_hA
   if (loc && !P.nonorm) {
@@ -1286,6 +1370,27 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     GPS_TRY(wfork(st));
     GPS_TRY(mid_done());
     g_x_local = g_xloc;
+  } else if (P.gen) {
+    // x_loc = x + drop(r W4^T)
+    Operand g_l;
+    GPS_TRY(dropmul(P, {g_xloc, d, g_xloc_p}, P.g_tmp3, P.gtmp3_p, GPS_SITE_LOCAL, st, &g_l));
+    // g_r = g_l W4 [N, 2d]
+    GPS_TRY(gemm(linear_dgrad(P, N, 2 * d, d, g_l, {gen->lin1.weight, 2 * d, P.mlp4_p}, P.gen_gr, 2 * d), st));
+    // r = relu(mlp.1(h1)): g_h1 and the mlp.1 gradients
+    const BnView vb = gen_bn_view(P, gen->bn);
+    GPS_TRY(bn_bwd_reduce(P.gen_gr, 2 * d, P.gen_h1, 2 * d, N, 2 * d, vb, GPS_ACT_RELU, nodrop, P.gen_bsums, st));
+    GPS_TRY(bn_bwd_apply(P.gen_gr, 2 * d, P.gen_h1, 2 * d, N, 2 * d, vb, GPS_ACT_RELU, nodrop, P.gen_bsums, P.gen_gh1,
+                         2 * d, gen->bn.grad_weight, gen->bn.grad_bias, st, P.grads_accumulate, P.gen_gh1_p));
+    const Operand g_h1{P.gen_gh1, 2 * d, P.gen_gh1_p};
+    GPS_TRY(wfork(st));
+    GPS_TRY(linear_wgrad(P, g_l, {P.gen_r, 2 * d, P.gen_r_p}, N, d, 2 * d, gen->lin1.grad_weight, nullptr, s2));
+    GPS_TRY(linear_wgrad(P, g_h1, {P.gen_u, d, P.gen_u_p}, N, 2 * d, d, gen->lin0.grad_weight, nullptr, s2));
+    GPS_TRY(mid_done());
+    // g_u = g_h1 W0; then grad_edge_attr (dst ordered) and g_x_local = g_u + sum_out grad_edge_attr + g_xloc
+    GPS_TRY(gemm(linear_dgrad(P, N, d, 2 * d, g_h1, {gen->lin0.weight, d, P.mlp0_p}, P.gen_gu, d), st));
+    GPS_TRY(genconv_bwd_dst(a->graph, d, a->x, a->edge_attr, P.agg, P.gen_lse, P.gen_gu, a->grad_edge_attr, st));
+    GPS_TRY(gine_bwd_src(a->graph, d, a->grad_edge_attr, P.gen_gu, 0.f, g_xloc, P.g_xl, st));
+    g_x_local = P.g_xl;
   }
 
   if (two_branches) GPS_TRY(sd->order(sa, st));
@@ -1370,24 +1475,24 @@ extern "C" int gps_layer_plan(const GpsLayerArgs* args, GpsLayerPlan* plan) {
 
 extern "C" int gps_layer_forward(const GpsLayerArgs* args, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_forward: null args");
-  return layer_forward(args, nullptr, nullptr, (cudaStream_t)stream);
+  return layer_forward(args, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward(const GpsLayerArgs* args, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_backward: null args");
-  return layer_backward(args, nullptr, nullptr, (cudaStream_t)stream);
+  return layer_backward(args, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_forward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_forward_biased: null args");
   GPS_TRY(check_bias(args, bias));
-  return layer_forward(args, bias, nullptr, (cudaStream_t)stream);
+  return layer_forward(args, bias, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_backward_biased: null args");
   GPS_TRY(check_bias(args, bias));
-  return layer_backward(args, bias, nullptr, (cudaStream_t)stream);
+  return layer_backward(args, bias, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 static int check_gat(const GpsLayerArgs* a, const GpsGat* gat, const char* what) {
@@ -1400,14 +1505,35 @@ static int check_gat(const GpsLayerArgs* a, const GpsGat* gat, const char* what)
 extern "C" int gps_layer_forward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias, void* stream) {
   GPS_TRY(check_gat(args, gat, "gps_layer_forward_gat"));
   GPS_TRY(check_bias(args, bias));
-  return layer_forward(args, bias, gat, (cudaStream_t)stream);
+  return layer_forward(args, bias, gat, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias,
                                       void* stream) {
   GPS_TRY(check_gat(args, gat, "gps_layer_backward_gat"));
   GPS_TRY(check_bias(args, bias));
-  return layer_backward(args, bias, gat, (cudaStream_t)stream);
+  return layer_backward(args, bias, gat, nullptr, (cudaStream_t)stream);
+}
+
+static int check_genconv(const GpsLayerArgs* a, const GpsGenConv* gen, const char* what) {
+  GPS_REQUIRE(a && gen, GPS_ERR_ARG, "%s: null args / gen", what);
+  GPS_REQUIRE(a->local_type == GPS_LOCAL_GENCONV, GPS_ERR_ARG,
+              "%s: a GpsGenConv needs local_type GPS_LOCAL_GENCONV (got %d)", what, a->local_type);
+  return GPS_OK;
+}
+
+extern "C" int gps_layer_forward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias,
+                                         void* stream) {
+  GPS_TRY(check_genconv(args, gen, "gps_layer_forward_genconv"));
+  GPS_TRY(check_bias(args, bias));
+  return layer_forward(args, bias, nullptr, gen, (cudaStream_t)stream);
+}
+
+extern "C" int gps_layer_backward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias,
+                                          void* stream) {
+  GPS_TRY(check_genconv(args, gen, "gps_layer_backward_genconv"));
+  GPS_TRY(check_bias(args, bias));
+  return layer_backward(args, bias, nullptr, gen, (cudaStream_t)stream);
 }
 
 extern "C" int gps_linear_forward(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias,
@@ -1607,6 +1733,24 @@ extern "C" int gps_gat_backward(const GpsGraph* g, int64_t d, int64_t H, const f
   return gat_bwd(*g, d, H, Y, ldy, edge_attr, v, att_src, att_dst, gat_scores((float*)scores, g->N, g->E, H), g_h,
                  (float*)workspace, gY, ldg, yp, grad_edge_attr, g_v, g_att_src, g_att_dst, g_bias, accumulate != 0,
                  (cudaStream_t)stream);
+}
+
+// ---- stage entry points of the GENConv message passing (genconv.cu; the backward's source-ordered pass is GINE's)
+extern "C" int gps_genconv_aggregate_forward(const GpsGraph* g, int64_t d, const float* x, const float* e, float* agg,
+                                             float* lse, float* u, void* stream) {
+  GPS_REQUIRE(g && x && agg && lse && u && (e || g->E == 0), GPS_ERR_ARG, "genconv_aggregate_forward: null argument");
+  GPS_TRY(stage_width(d, "genconv_aggregate_forward"));
+  return genconv_fwd(*g, d, x, e, agg, lse, u, (cudaStream_t)stream);
+}
+
+extern "C" int gps_genconv_aggregate_backward(const GpsGraph* g, int64_t d, const float* x, const float* e,
+                                              const float* agg, const float* lse, const float* g_u, const float* add,
+                                              float* g_e, float* g_x, void* stream) {
+  GPS_REQUIRE(g && x && agg && lse && g_u && g_x && (g->E == 0 || (e && g_e)), GPS_ERR_ARG,
+              "genconv_aggregate_backward: null argument");
+  GPS_TRY(stage_width(d, "genconv_aggregate_backward"));
+  GPS_TRY(genconv_bwd_dst(*g, d, x, e, agg, lse, g_u, g_e, (cudaStream_t)stream));
+  return gine_bwd_src(*g, d, g_e, g_u, 0.f, add, g_x, (cudaStream_t)stream);
 }
 
 // ---- stage entry points of the Performer (performer.cu, performer_quad.cu).  Each validates its arguments before it

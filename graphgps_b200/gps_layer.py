@@ -20,9 +20,9 @@ import torch.nn as nn
 from . import _lib
 from .graph import graph_of
 
-_SUPPORTED_LOCAL = ("None", "CustomGatedGCN", "GINE", "GCN", "GAT")
-_EDGE_LOCAL = ("CustomGatedGCN", "GINE", "GAT")   # local models that read batch.edge_attr (gps_layer.py:44-53)
-_KNOWN_LOCAL = _SUPPORTED_LOCAL + ("GIN", "GENConv", "PNA")
+_SUPPORTED_LOCAL = ("None", "CustomGatedGCN", "GINE", "GCN", "GAT", "GENConv")
+_EDGE_LOCAL = ("CustomGatedGCN", "GINE", "GAT", "GENConv")   # local models that read batch.edge_attr (gps_layer.py:44-53)
+_KNOWN_LOCAL = _SUPPORTED_LOCAL + ("GIN", "PNA")
 _SUPPORTED_GLOBAL = ("None", "Transformer", "BiasedTransformer", "Performer")
 _KNOWN_GLOBAL = _SUPPORTED_GLOBAL + ("BigBird",)
 _MHA_GLOBAL = ("Transformer", "BiasedTransformer")   # torch's MultiheadAttention (gps_layer.py:104-106)
@@ -148,6 +148,19 @@ class _GATConvParams(nn.Module):
             _glorot_(t)
 
 
+class _GENConvParams(nn.Module):
+    """Names of PyG 2.2 GENConv(dim_h, dim_h) as built at gps_layer.py:60-61 (softmax aggregation with t = 1 as a Python
+    float, so no parameters of its own; no lin_src / lin_dst / lin_edge / lin_aggr_out since in == out and edge_dim is
+    None): mlp = Linear(d, 2d, bias=False), BatchNorm1d(2d), ReLU, Dropout(0), Linear(2d, d, bias=False), i.e. the keys
+    mlp.0.weight, mlp.1.{weight, bias, running_mean, running_var, num_batches_tracked}, mlp.4.weight.  The MLP's
+    activation is ReLU whatever gnn.act is."""
+
+    def __init__(self, dim):
+        super().__init__()
+        self.mlp = nn.Sequential(nn.Linear(dim, 2 * dim, bias=False), nn.BatchNorm1d(2 * dim), nn.ReLU(),
+                                 nn.Dropout(0.0), nn.Linear(2 * dim, dim, bias=False))
+
+
 def _orthogonal_gaussian_matrix(nb_rows, nb_cols):
     """Random-feature projection drawn once at construction (performer_layer.py:163-195, scaling=0)."""
     blocks = []
@@ -212,6 +225,7 @@ class _GPSLayerFn(torch.autograd.Function):
         x_out = torch.empty_like(x)
         e_out = torch.empty_like(e) if layer.local_gnn_type == "CustomGatedGCN" else None
         gat = layer._gat_args(named) if layer.local_gnn_type == "GAT" else None
+        gen = layer._genconv_args(named) if layer.local_gnn_type == "GENConv" else None
         plan = layer._plan(args, gs)
         saved = torch.empty(max(plan[0], 256), dtype=torch.uint8, device=dev)
         ws = _workspace(dev, plan[1])
@@ -229,6 +243,10 @@ class _GPSLayerFn(torch.autograd.Function):
         if gat is not None:
             ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)) if ctx.nmax else None
             _lib.check(lib.gps_layer_forward_gat(C.byref(args), C.byref(gat), ab, stream), "gps_layer_forward_gat")
+        elif gen is not None:
+            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)) if ctx.nmax else None
+            _lib.check(lib.gps_layer_forward_genconv(C.byref(args), C.byref(gen), ab, stream),
+                       "gps_layer_forward_genconv")
         elif ctx.nmax:
             ab = _lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)
             _lib.check(lib.gps_layer_forward_biased(C.byref(args), C.byref(ab), stream), "gps_layer_forward_biased")
@@ -300,6 +318,11 @@ class _GPSLayerFn(torch.autograd.Function):
             gat = layer._gat_args(named, grads)
             ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))) if ctx.nmax else None
             _lib.check(lib.gps_layer_backward_gat(C.byref(args), C.byref(gat), ab, stream), "gps_layer_backward_gat")
+        elif layer.local_gnn_type == "GENConv":
+            gen = layer._genconv_args(named, grads)
+            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))) if ctx.nmax else None
+            _lib.check(lib.gps_layer_backward_genconv(C.byref(args), C.byref(gen), ab, stream),
+                       "gps_layer_backward_genconv")
         elif ctx.nmax:
             ab = _lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))
             _lib.check(lib.gps_layer_backward_biased(C.byref(args), C.byref(ab), stream), "gps_layer_backward_biased")
@@ -358,6 +381,11 @@ class GPSLayer(nn.Module):
                 "GINE with equivstable_pe=True is not built in graphgps_b200: the reference itself fails to construct "
                 "it (GINEConvESLapPE.__init__ calls reset_parameters(), which reads self.mlp_r_ij before it is defined: "
                 "gine_conv_layer.py:35,44 raise AttributeError)")
+        if equivstable_pe and local_gnn_type == "GENConv":
+            raise NotImplementedError(
+                "GENConv with equivstable_pe=True is not built in graphgps_b200: the reference passes "
+                "batch.pe_EquivStableLapPE as GENConv.forward's fourth positional parameter, which is `size` "
+                "(gps_layer.py:176-181), so there is no defined behaviour to match")
         # EquivStableLapPE gate: read by GatedGCN only; GCN and None ignore the flag (gps_layer.py:176-187)
         self._eslap = bool(equivstable_pe) and local_gnn_type == "CustomGatedGCN"
         if local_gnn_type == "None":
@@ -372,6 +400,8 @@ class GPSLayer(nn.Module):
             if num_heads < 1 or dim_h % num_heads != 0:
                 raise ValueError(f"GAT needs dim_h ({dim_h}) divisible by num_heads ({num_heads})")
             self.local_model = _GATConvParams(dim_h, num_heads)
+        elif local_gnn_type == "GENConv":
+            self.local_model = _GENConvParams(dim_h)
         else:
             self.local_model = _GatedGCNParams(dim_h, act, self._eslap)
         self.local_gnn_type = local_gnn_type
@@ -587,6 +617,18 @@ class GPSLayer(nn.Module):
             _lin(named[p + "lin_edge.weight"], None, g.get(p + "lin_edge.weight")),
             *(_lib.ptr(named[p + n]) for n in ("att_src", "att_dst", "att_edge")),
             *(_lib.ptr(g.get(p + n)) for n in ("att_src", "att_dst", "att_edge")))
+
+    def _genconv_args(self, named, grads=None):
+        """GpsGenConv of the GENConv local model (gps_b200.h): mlp.0, mlp.1 (with its running statistics), mlp.4."""
+        g = grads or {}
+        p = "local_model.mlp."
+        bn = self.local_model.mlp[1]
+        return _lib.GpsGenConv(
+            _lin(named[p + "0.weight"], None, g.get(p + "0.weight")),
+            _lib.GpsBatchNorm(_lib.ptr(named[p + "1.weight"]), _lib.ptr(named[p + "1.bias"]), _lib.ptr(bn.running_mean),
+                              _lib.ptr(bn.running_var), _lib.ptr(bn.num_batches_tracked),
+                              _lib.ptr(g.get(p + "1.weight")), _lib.ptr(g.get(p + "1.bias"))),
+            _lin(named[p + "4.weight"], None, g.get(p + "4.weight")))
 
     @property
     def _gine_eps_host(self):

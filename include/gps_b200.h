@@ -36,7 +36,8 @@ extern "C" {
 enum { GPS_OK = 0, GPS_ERR_ARG = -1, GPS_ERR_UNSUPPORTED = -2, GPS_ERR_CUDA = -3 };
 
 /* local_gnn_type / global_model_type of GPSLayer.__init__ (gps_layer.py:20-24,44-122) */
-enum { GPS_LOCAL_NONE = 0, GPS_LOCAL_GATEDGCN = 1, GPS_LOCAL_GINE = 2, GPS_LOCAL_GCN = 3, GPS_LOCAL_GAT = 4 };
+enum { GPS_LOCAL_NONE = 0, GPS_LOCAL_GATEDGCN = 1, GPS_LOCAL_GINE = 2, GPS_LOCAL_GCN = 3, GPS_LOCAL_GAT = 4,
+       GPS_LOCAL_GENCONV = 5 };
 enum { GPS_GLOBAL_NONE = 0, GPS_GLOBAL_TRANSFORMER = 1, GPS_GLOBAL_PERFORMER = 2 };
 /* register.act_dict keys used by shipped configs (gps_layer.py:33) */
 enum { GPS_ACT_RELU = 0, GPS_ACT_GELU = 1 };
@@ -282,6 +283,30 @@ typedef struct {
 int gps_layer_forward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias, void* stream);
 int gps_layer_backward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias, void* stream);
 
+/* GENConv local model (local_type == GPS_LOCAL_GENCONV): PyG 2.2 GENConv(dim_h, dim_h) with its defaults (softmax
+ * aggregation with t = 1, no message norm, eps 1e-7, MLP d -> 2d -> d with BatchNorm, no bias), gps_layer.py:60-61,
+ * 183-189.  For target i and channel c: m_k = relu(x[src_k] + e_k) + 1e-7, agg_i = sum_k softmax_k(m)_c m_kc over i's
+ * in-edges (0 without any; self loops and duplicates are ordinary edges), u = agg + x and
+ * h = lin1(relu(bn(lin0(u)))); x_loc = x + dropout(h).  edge_attr [E, d] is read (non-NULL when E > 0) and
+ * batch.edge_attr is not updated.  d % 4 == 0 and d <= 2048 (the 2d-wide BatchNorm runs on the row-wise stages), else
+ * GPS_ERR_UNSUPPORTED.  Parameters (all non-NULL, else GPS_ERR_ARG), whose gradients are final at ev_grads_mid:
+ *   lin0 = local_model.mlp.0 [2d, d], bias NULL;
+ *   bn   = local_model.mlp.1 [2d]: weight, bias, running_mean, running_var (num_batches_tracked optional); training
+ *          mode normalises with the batch statistics and updates the running ones as torch.nn.BatchNorm1d;
+ *   lin1 = local_model.mlp.4 [d, 2d], bias NULL.  The MLP's activation is ReLU whatever GpsLayerArgs.act is. */
+typedef struct {
+  GpsLinear lin0;
+  GpsBatchNorm bn;
+  GpsLinear lin1;
+} GpsGenConv;
+
+/* gps_layer_forward / _backward of a GENConv layer; bias: GpsAttnBias of a BiasedTransformer global model or NULL.
+ * gps_layer_plan sizes GENConv from local_type alone.  The plain, _biased and _gat calls with local_type ==
+ * GPS_LOCAL_GENCONV, and these with a NULL gen, return GPS_ERR_ARG before any CUDA call, as does a NULL edge_attr
+ * (E > 0) or, in the backward, grad_edge_attr (E > 0). */
+int gps_layer_forward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias, void* stream);
+int gps_layer_backward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Stage-level entry points (the same kernels the layer calls; exported so the parity tests can
  * pin each stage against the oracle separately).
@@ -382,6 +407,17 @@ int gps_gat_backward(const GpsGraph* g, int64_t d, int64_t H, const float* Y, in
                      void* workspace, int64_t workspace_bytes, float* gY, int64_t ldg, const GpsPlanes* gY_planes,
                      float* grad_edge_attr, float* g_v, float* g_att_src, float* g_att_dst, float* g_bias,
                      int32_t accumulate, void* stream);
+
+/* GENConv stage entry points (the kernels the GENConv layer calls around its MLP).  x, e [E,d] (NULL when E == 0).
+ * Forward: agg [N,d] = the softmax aggregation of the messages relu(x_src + e) + 1e-7, lse [N,d] = each (node, channel)
+ * segment's log-sum-exp (0 for a node without in-edges), u [N,d] = agg + x.
+ * Backward from g_u [N,d] (the gradient of u): g_e [E,d] = g_u[dst] alpha (1 + m - agg[dst]) [x_src + e > 0] (NULL
+ * when E == 0), g_x [N,d] = g_u + sum over out-edges of g_e (+ add [N,d], NULL = none). */
+int gps_genconv_aggregate_forward(const GpsGraph* g, int64_t d, const float* x, const float* e, float* agg, float* lse,
+                                  float* u, void* stream);
+int gps_genconv_aggregate_backward(const GpsGraph* g, int64_t d, const float* x, const float* e, const float* agg,
+                                   const float* lse, const float* g_u, const float* add, float* g_e, float* g_x,
+                                   void* stream);
 
 /* Performer stage entry points (FAVOR+, performer_layer.py:119-144,200-205), the calls one layer makes, in order.
  * They take dim_head == 64 and 256 < m <= 272 features (else GPS_ERR_UNSUPPORTED), H > 0 and N * H * 272 < 2^31 (else
