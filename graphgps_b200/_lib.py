@@ -14,7 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgps_b200.so")
 
 GPS_OK, GPS_ERR_ARG, GPS_ERR_UNSUPPORTED, GPS_ERR_CUDA = 0, -1, -2, -3
-LOCAL = {"None": 0, "CustomGatedGCN": 1, "GINE": 2, "GCN": 3, "GAT": 4, "GENConv": 5}
+LOCAL = {"None": 0, "CustomGatedGCN": 1, "GINE": 2, "GCN": 3, "GAT": 4, "GENConv": 5, "PNA": 6}
 GLOBAL = {"None": 0, "Transformer": 1, "Performer": 2}
 ACT = {"relu": 0, "gelu": 1}
 PRECISION = {"fp32": 0, "bf16": 1}
@@ -91,6 +91,12 @@ class GpsGenConv(C.Structure):
     _fields_ = [("lin0", GpsLinear), ("bn", GpsBatchNorm), ("lin1", GpsLinear)]
 
 
+class GpsPna(C.Structure):
+    """PNA local model: edge_encoder [d, edge_dim], pre = pre_nns.0.0 [d, 3d], post = post_nns.0.0 [d, 4d], lin [d, d]."""
+    _fields_ = [("edge_encoder", GpsLinear), ("pre", GpsLinear), ("post", GpsLinear), ("lin", GpsLinear),
+                ("edge_dim", C.c_int64)]
+
+
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
                 ("bwd_workspace_bytes", C.c_int64), ("fwd_launches", C.c_int64),
@@ -116,6 +122,8 @@ SYMBOLS = {
                                             _fp]),
     "gps_layer_backward_genconv": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGenConv), C.POINTER(GpsAttnBias),
                                              _fp]),
+    "gps_layer_forward_pna": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsPna), C.POINTER(GpsAttnBias), _fp]),
+    "gps_layer_backward_pna": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsPna), C.POINTER(GpsAttnBias), _fp]),
     "gps_linear_forward": (C.c_int, [_fp, _i64, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _fp]),
     "gps_gemm": (C.c_int, [_fp, _i64, _i32, _fp, _i64, _i32, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _fp]),
     "gps_gatedgcn_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _i64, _fp, _fp,
@@ -143,6 +151,10 @@ SYMBOLS = {
     "gps_genconv_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _fp, _fp]),
     "gps_genconv_aggregate_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp,
                                                  _fp]),
+    "gps_pna_fold_forward": (C.c_int, [_fp, _fp, _fp, _fp, _i64, _i64, _fp, _fp, _fp]),
+    "gps_pna_fold_backward": (C.c_int, [_fp, _fp, _fp, _fp, _fp, _i64, _i64, _fp, _fp, _fp, _fp, _i32, _fp]),
+    "gps_pna_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _i64, _fp, _fp, _fp, _fp]),
+    "gps_pna_aggregate_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _fp, _i64, _fp, _fp]),
     "gps_performer_prep": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp]),
     "gps_performer_features_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp,
                                                  _fp, _fp]),

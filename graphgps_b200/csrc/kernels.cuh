@@ -145,6 +145,23 @@ int genconv_fwd(const GpsGraph& g, int64_t d, const float* x, const float* e, fl
 int genconv_bwd_dst(const GpsGraph& g, int64_t d, const float* x, const float* e, const float* agg, const float* lse,
                     const float* g_u, float* g_e, cudaStream_t stream);
 
+// PNA (PyG PNAConv, mean / max / sum aggregation, pna.cu).  pna_check: 0 < de <= d, de % 4 == 0.  Fold: F = W_e W_enc
+// [d, de] and c = W_e b_enc + b_pre [d], W_e the column block 2d..3d of W_pre [d, 3d]; its backward writes (or, with
+// accumulate, adds) the gradients of W_pre's block 2d..3d, b_pre, W_enc and b_enc from g_F [d, de] and g_c [d] (each
+// output NULL = not needed).  Forward: m_k = Y[i, 0:d] + Y[j, d:2d] + q[k] (Y = [P_dst | P_src | ...] with pitch ldy),
+// Z = [x | mean | max | sum] [N, 4d] (fp32 when Z != NULL, planes when Zp.hi), arg [N, d] = edge id of the first
+// maximiser (-1 without in-edges).  Backward from g_Z [N, 4d]: g_q [E, d] (+ planes), g_P_dst into gY[:, 0:d] and
+// g_P_src into gY[:, d:2d] (+ planes), g_x = add + g_Z[:, 0:d] (add NULL = none).
+int pna_check(int64_t d, int64_t de);
+int pna_fold_fwd(const float* Wpre, const float* bpre, const float* Wenc, const float* benc, int64_t d, int64_t de,
+                 float* F, float* cvec, cudaStream_t st);
+int pna_fold_bwd(const float* Wpre, const float* Wenc, const float* benc, const float* gF, const float* gc, int64_t d,
+                 int64_t de, float* gWpre, float* gbpre, float* gWenc, float* gbenc, bool accumulate, cudaStream_t st);
+int pna_fwd(const GpsGraph& g, int64_t d, const float* x, const float* Y, int64_t ldy, const float* q, float* Z,
+            Planes Zp, int* arg, cudaStream_t stream);
+int pna_bwd(const GpsGraph& g, int64_t d, const float* gZ, const int* arg, const float* add, float* g_q, Planes gqp,
+            float* gY, int64_t ldg, Planes gYp, float* g_x, cudaStream_t stream);
+
 // ---- attention ------------------------------------------------------------------------------
 int attention_fwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, const float* K, const float* V,
                   int64_t ld, float* O, int64_t ldo, float* lse, float p_drop, uint64_t seed, uint64_t offset,

@@ -154,8 +154,10 @@ static int side_stream(Side** out) {
 }
 
 // ------------------------------------------------------------------------------- weight packing
+// A weight [rows, d] whose rows lie ld floats apart in the caller's tensor (ld > d: a column block of a wider weight,
+// as PNA's pre_nns.0.0 [d, 3d]); its gradient gw has the same pitch.
 struct PackSeg {
-  const float* w; const float* b; float* gw; float* gb; int rows;
+  const float* w; const float* b; float* gw; float* gb; int rows; int ld;
 };
 struct PackDesc {
   PackSeg seg[5];
@@ -167,7 +169,7 @@ __global__ void k_pack(PackDesc pd, float* __restrict__ Wcat, float* __restrict_
   const int r = blockIdx.x;
   int row0 = 0, s = 0;
   while (s < pd.nseg - 1 && r >= row0 + pd.seg[s].rows) row0 += pd.seg[s++].rows;
-  const float* src = pd.seg[s].w + (int64_t)(r - row0) * pd.d;
+  const float* src = pd.seg[s].w + (int64_t)(r - row0) * pd.seg[s].ld;
   float* dst = Wcat + (int64_t)r * pd.d;
   for (int c = threadIdx.x * 4; c < pd.d; c += blockDim.x * 4) st4(dst + c, ld4(src + c));
   if (threadIdx.x == 0) bcat[r] = pd.seg[s].b ? pd.seg[s].b[r - row0] : 0.f;
@@ -177,7 +179,7 @@ __global__ void k_unpack(PackDesc pd, const float* __restrict__ gWcat, const flo
   int row0 = 0, s = 0;
   while (s < pd.nseg - 1 && r >= row0 + pd.seg[s].rows) row0 += pd.seg[s++].rows;
   if (pd.seg[s].gw) {
-    float* dst = pd.seg[s].gw + (int64_t)(r - row0) * pd.d;
+    float* dst = pd.seg[s].gw + (int64_t)(r - row0) * pd.seg[s].ld;
     const float* src = gWcat + (int64_t)r * pd.d;
     for (int c = threadIdx.x * 4; c < pd.d; c += blockDim.x * 4)
       st4(dst + c, accumulate ? f4add(ld4(dst + c), ld4(src + c)) : ld4(src + c));
@@ -234,6 +236,16 @@ struct Plan {
   const GpsGenConv* genp;
   float *gen_lse, *gen_u, *gen_h1, *gen_r, *gen_bn, *gen_gr, *gen_gh1, *gen_gu;
   double *gen_fstats, *gen_bsums;
+  // PNA (pna.cu): the caller's GpsPna (NULL when only sizes are wanted) and de = edge_dim (d, the bound, without it).
+  // Saved: the fold F [d, de] with its planes and c [d]; Z = [x | mean | max | sum] [N, 4d] (planes; fp32 without
+  // planes); the argmax [N, d]; h = post(Z) [N, d] with planes.  Forward workspace: q = e F^T + c [E, d].  Backward:
+  // g_h [N, d], g_Z [N, 4d], g_q [E, d] (+ planes), g_F [d, de] | g_c [d], g_xl.
+  bool pna;
+  const GpsPna* pnap;
+  int64_t de;
+  float *pna_F, *pna_c, *pna_Z, *pna_h, *pna_q, *pna_gh, *pna_gZ, *pna_gq, *pna_gF;
+  int* pna_arg;
+  Planes pna_F_p, pna_Z_p, pna_h_p, pna_gh_p, pna_gq_p, post_p, lin_p;
   // GPS_NORM_NONE: no norm1_local / norm1_attn / norm2.  Only the local model's own BatchNorms (BN_X, BN_E) remain, so
   // nbn = 2 statistics slots instead of BN_COUNT; s = x_loc + hA is written by the GEMM that closes the second branch
   // and x_out by the FF2 GEMM.
@@ -295,12 +307,16 @@ struct Plan {
 // computes [Ax|Bx|Dx|Ex|Q|K|V]; this list is the one statement of that layout and sets Wy and qkv_off.
 static void list_weights(const GpsLayerArgs* a, Plan* P) {
   const int64_t d = P->d, kout = P->perf ? P->inner : d;
-  auto add = [&](const GpsLinear& l, int64_t rows, int64_t cols, Planes Plan::*planes, bool bias = true) {
+  auto add_seg = [&](const PackSeg& seg, int64_t cols, Planes Plan::*planes) {
     const bool wcat = planes == &Plan::Wcat_p;
-    const PackSeg seg{l.weight, bias ? l.bias : nullptr, l.grad_weight, bias ? l.grad_bias : nullptr, (int)rows};
     P->weights[P->nweights++] = LayerWeight{seg, cols, wcat ? P->Wy : 0, planes};
-    if (wcat) P->Wy += rows;
+    if (wcat) P->Wy += seg.rows;
   };
+  auto add = [&](const GpsLinear& l, int64_t rows, int64_t cols, Planes Plan::*planes, bool bias = true) {
+    add_seg(PackSeg{l.weight, bias ? l.bias : nullptr, l.grad_weight, bias ? l.grad_bias : nullptr, (int)rows, (int)cols},
+            cols, planes);
+  };
+  static const GpsLinear kNoLinear = {};
   if (P->gated) {
     add(a->gcn_A, d, d, &Plan::Wcat_p);
     add(a->gcn_B, d, d, &Plan::Wcat_p);
@@ -311,8 +327,16 @@ static void list_weights(const GpsLayerArgs* a, Plan* P) {
   // GCNConv.lin has no bias; GCNConv.bias is added after the aggregation (scatter.cu)
   if (P->gcn) add(a->gcn_conv, d, d, &Plan::Wcat_p, false);
   // GATConv.lin_src (= lin_dst) has no bias; GATConv.bias is added after the aggregation (gat.cu)
-  static const GpsLinear kNoLinear = {};
   if (P->gat) add(P->gatp ? P->gatp->lin_src : kNoLinear, d, d, &Plan::Wcat_p, false);
+  // PNA: the destination and source column blocks of pre_nns.0.0.weight [d, 3d] give P_dst | P_src; pre's bias enters
+  // through the edge term (pna.cu)
+  if (P->pna) {
+    const GpsLinear& pre = P->pnap ? P->pnap->pre : kNoLinear;
+    for (int64_t blk = 0; blk < 2; ++blk)
+      add_seg(PackSeg{pre.weight ? pre.weight + blk * d : nullptr, nullptr,
+                      pre.grad_weight ? pre.grad_weight + blk * d : nullptr, nullptr, (int)d, (int)(3 * d)},
+              d, &Plan::Wcat_p);
+  }
   P->qkv_off = P->Wy;
   if (P->attn) add(a->attn_in, 3 * d, d, &Plan::Wcat_p);
   if (P->attn || P->perf) add(a->attn_out, d, kout, &Plan::out_p);
@@ -325,6 +349,10 @@ static void list_weights(const GpsLayerArgs* a, Plan* P) {
   if (P->gen) {   // GENConv's MLP Linears have no bias
     add(P->genp ? P->genp->lin0 : kNoLinear, 2 * d, d, &Plan::mlp0_p, false);
     add(P->genp ? P->genp->lin1 : kNoLinear, d, 2 * d, &Plan::mlp4_p, false);
+  }
+  if (P->pna) {
+    add(P->pnap ? P->pnap->post : kNoLinear, d, 4 * d, &Plan::post_p);
+    add(P->pnap ? P->pnap->lin : kNoLinear, d, d, &Plan::lin_p);
   }
   if (P->perf) {
     add(a->perf_q, P->inner, d, &Plan::pq_p);
@@ -342,7 +370,7 @@ static Planes caller_planes(const GpsPlanes& g, int64_t d, int precision) {
 }
 
 static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* gat = nullptr,
-                     const GpsGenConv* gen = nullptr) {
+                     const GpsGenConv* gen = nullptr, const GpsPna* pna = nullptr) {
   memset(P, 0, sizeof(*P));
   GPS_REQUIRE(a, GPS_ERR_ARG, "null args");
   P->N = a->graph.N;
@@ -358,8 +386,12 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   P->gatp = gat;
   P->gen = a->local_type == GPS_LOCAL_GENCONV;
   P->genp = gen;
-  GPS_REQUIRE(a->local_type == GPS_LOCAL_NONE || P->gated || P->gine || P->gcn || P->gat || P->gen, GPS_ERR_ARG,
-              "unknown local_type %d", a->local_type);
+  P->pna = a->local_type == GPS_LOCAL_PNA;
+  P->pnap = pna;
+  P->de = pna ? pna->edge_dim : a->d;   // sizes alone: edge_dim <= d is the bound
+  GPS_REQUIRE(a->local_type == GPS_LOCAL_NONE || P->gated || P->gine || P->gcn || P->gat || P->gen || P->pna,
+              GPS_ERR_ARG, "unknown local_type %d", a->local_type);
+  if (P->pna) GPS_TRY(pna_check(a->d, P->de));
   if (P->gat) GPS_TRY(gat_check(a->d, a->heads));
   GPS_REQUIRE(!P->gen || a->d <= 2048, GPS_ERR_UNSUPPORTED,
               "GENConv needs dim_h <= 2048: its 2 dim_h-wide BatchNorm runs on the row-wise stages (got %lld)",
@@ -440,7 +472,13 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     P->gen_r = S.alloc<float>(N * 2 * d);
     P->gen_bn = S.alloc<float>(2 * 2 * d);
   }
-  const bool loc = P->gated || P->gine || P->gcn || P->gat || P->gen;
+  if (P->pna) {
+    P->pna_F = S.alloc<float>(d * P->de);
+    P->pna_c = S.alloc<float>(d);
+    P->pna_arg = S.alloc<int>(N * d);
+    P->pna_h = S.alloc<float>(N * d);
+  }
+  const bool loc = P->gated || P->gine || P->gcn || P->gat || P->gen || P->pna;
   if (loc && !P->nonorm) P->xloc = S.alloc<float>(N * d);   // read by norm1_local's backward
   if (P->attn) {
     P->O = S.alloc<float>(N * d);
@@ -503,6 +541,12 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
       P->gen_u_p = mkplanes(S, N, d);
       P->gen_r_p = mkplanes(S, N, 2 * d);
     }
+    if (P->pna) {   // edge_attr is de wide: planes of its own, never the caller's d-wide ones
+      P->e_p = mkplanes(S, E, P->de);
+      P->pna_F_p = mkplanes(S, d, P->de);
+      P->pna_Z_p = mkplanes(S, N, 4 * d);
+      P->pna_h_p = mkplanes(S, N, d);
+    }
     // weight planes: in the caller's persistent buffer when one is given (packed once per optimiser step), else in `saved`
     Arena Wa(bind ? a->wplanes : nullptr, a->wplanes_bytes);
     Arena& WA = bind && a->wplanes != nullptr ? Wa : S;
@@ -515,6 +559,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     GPS_REQUIRE(!Wa.overflow, GPS_ERR_ARG, "wplanes buffer too small (%lld < %lld)", (long long)a->wplanes_bytes,
                 (long long)P->wplanes_bytes);
   }
+  if (P->pna && !P->use_planes) P->pna_Z = S.alloc<float>(N * 4 * d);
   P->saved_bytes = S.used;
   GPS_REQUIRE(!S.overflow, GPS_ERR_ARG, "saved buffer too small (%lld < %lld)", (long long)a->saved_bytes,
               (long long)S.used);
@@ -523,6 +568,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   Arena F(bind ? a->workspace : nullptr, a->workspace_bytes);
   P->fstats = F.alloc<double>(P->nbn * 2 * d);
   if (P->gen) P->gen_fstats = F.alloc<double>(2 * 2 * d);
+  if (P->pna) P->pna_q = F.alloc<float>(E * d);
   if (P->nonorm && loc) {
     // x_loc is an operand of the GEMM that writes s (and of nothing in the backward pass); a lone local model writes s
     P->xloc = (P->attn || P->perf) ? F.alloc<float>(N * d) : P->s;
@@ -588,6 +634,13 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     P->gen_gu = Bk.alloc<float>(N * d);
     P->g_xl = Bk.alloc<float>(N * d);
   }
+  if (P->pna) {
+    P->pna_gh = Bk.alloc<float>(N * d);
+    P->pna_gZ = Bk.alloc<float>(N * 4 * d);
+    P->pna_gq = Bk.alloc<float>(E * d);
+    P->pna_gF = Bk.alloc<float>(d * P->de + d);   // [g_F | g_c] contiguous: one memset
+    P->g_xl = Bk.alloc<float>(N * d);
+  }
   if (P->use_planes) {
     P->gt_p = mkplanes(Bk, N, d);
     P->ghid_p = mkplanes(Bk, N, 2 * d);
@@ -607,6 +660,11 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     if (P->gen) {
       if (!P->nonorm) P->gl1_p = mkplanes(Bk, N, d);
       P->gen_gh1_p = mkplanes(Bk, N, 2 * d);
+    }
+    if (P->pna) {
+      if (!P->nonorm) P->gl1_p = mkplanes(Bk, N, d);
+      P->pna_gh_p = mkplanes(Bk, N, d);
+      P->pna_gq_p = mkplanes(Bk, E, d);
     }
   }
   P->bwd_bytes = Bk.used;
@@ -677,7 +735,7 @@ static int check_bn(const GpsBatchNorm& b, const char* name) {
 }
 
 static int check_params(const GpsLayerArgs* a, const Plan& P) {
-  GPS_REQUIRE(a->x && (P.E == 0 || a->edge_attr || !(P.gated || P.gine || P.gat || P.gen)), GPS_ERR_ARG,
+  GPS_REQUIRE(a->x && (P.E == 0 || a->edge_attr || !(P.gated || P.gine || P.gat || P.gen || P.pna)), GPS_ERR_ARG,
               "missing x / edge_attr");
   if (P.gated) {
     GPS_TRY(check_linear(a->gcn_A, "local_model.A", true));
@@ -714,8 +772,16 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
                 "missing buffer local_model.mlp.1.running_{mean,var}");
     GPS_TRY(check_linear(P.genp->lin1, "local_model.mlp.4", false));
   }
+  if (P.pna) {
+    GPS_REQUIRE(P.pnap, GPS_ERR_ARG, "local_type GPS_LOCAL_PNA needs gps_layer_forward_pna / gps_layer_backward_pna "
+                "with a GpsPna");
+    GPS_TRY(check_linear(P.pnap->edge_encoder, "local_model.edge_encoder", true));
+    GPS_TRY(check_linear(P.pnap->pre, "local_model.pre_nns.0.0", true));
+    GPS_TRY(check_linear(P.pnap->post, "local_model.post_nns.0.0", true));
+    GPS_TRY(check_linear(P.pnap->lin, "local_model.lin", true));
+  }
   const bool bn = !P.nonorm;   // norm1_local / norm1_attn / norm2 exist in BatchNorm mode only
-  if ((P.gated || P.gine || P.gcn || P.gat || P.gen) && bn) GPS_TRY(check_bn(a->norm1_local, "norm1_local"));
+  if ((P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) && bn) GPS_TRY(check_bn(a->norm1_local, "norm1_local"));
   if (P.attn) {
     GPS_TRY(check_linear(a->attn_in, "self_attn.in_proj", true));
     GPS_TRY(check_linear(a->attn_out, "self_attn.out_proj", true));
@@ -852,9 +918,9 @@ static int check_bias(const GpsLayerArgs* a, const GpsAttnBias* bias) {
 
 // =================================================================================== forward
 static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, const GpsGenConv* gen,
-                         cudaStream_t st) {
+                         const GpsPna* pna, cudaStream_t st) {
   Plan P;
-  GPS_TRY(make_plan(a, &P, true, gat, gen));
+  GPS_TRY(make_plan(a, &P, true, gat, gen, pna));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
   GPS_REQUIRE(a->workspace_bytes >= P.fwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.fwd_bytes);
@@ -872,7 +938,7 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
   Side* sd;
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
-  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen) && (P.attn || P.perf);
+  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) && (P.attn || P.perf);
   // GPS_NORM_NONE: the producer that closes the last branch writes s = x_loc + hA with its planes (x_loc = s when the
   // local model is alone)
   const bool local_writes_s = P.nonorm && !(P.attn || P.perf);
@@ -903,13 +969,27 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
     };
     if (P.x_p.hi != (__nv_bfloat16*)a->x_planes_in.hi) add(a->x, d, N, d, P.x_p);
     if ((P.gated || P.gine) && P.e_p.hi != (__nv_bfloat16*)a->e_planes_in.hi) add(a->edge_attr, d, E, d, P.e_p);
+    if (P.pna) add(a->edge_attr, P.de, E, P.de, P.e_p);
     if (!(a->wplanes && a->wplanes_valid)) {
       for (int i = 0; i < P.nweights; ++i) {
         const LayerWeight& w = P.weights[i];
-        add(w.lin.w, w.cols, w.lin.rows, w.cols, (P.*w.planes).rows(w.row0));
+        add(w.lin.w, w.lin.ld, w.lin.rows, w.cols, (P.*w.planes).rows(w.row0));
       }
     }
     GPS_TRY(to_planes(it, ni, st));
+  }
+  if (P.pna) {   // edge term of the messages, next to the node projections: q = e F^T + c, F = W_e W_enc (pna.cu)
+    GPS_TRY(sd->fork(st));
+    GPS_TRY(pna_fold_fwd(pna->pre.weight, pna->pre.bias, pna->edge_encoder.weight, pna->edge_encoder.bias, d, P.de,
+                         P.pna_F, P.pna_c, s2));
+    if (P.pna_F_p.hi) {
+      ToPlanesItem it{P.pna_F, P.de, (int)d, (int)P.de, P.pna_F_p};
+      GPS_TRY(to_planes(&it, 1, s2));
+    }
+    if (E > 0)
+      GPS_TRY(gemm(linear_fwd(P, E, d, P.de, {a->edge_attr, P.de, P.e_p}, {P.pna_F, P.de, P.pna_F_p}, P.pna_q, d,
+                              P.pna_c),
+                   s2));
   }
   if (P.gated) {   // edge projection has no dependency on the node side: run it next to the node projections
     GPS_REQUIRE(a->edge_out, GPS_ERR_ARG, "edge_out is null");
@@ -947,7 +1027,7 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
   }
 
   // main waits for the edge projection
-  if (P.gated) GPS_TRY(sd->join(st));
+  if (P.gated || P.pna) GPS_TRY(sd->join(st));
 
   // ---- local model
   if (P.gated) {
@@ -998,8 +1078,25 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
     if (local_writes_s) g2.Cp = P.s_p;
     set_dropout(g2, P.drop(GPS_SITE_LOCAL));
     GPS_TRY(gemm(g2, st));
+  } else if (P.pna) {
+    // Z = [x | mean | max | sum] of m = P_dst[i] + P_src[j] + q[k] (PNAConv.forward, DegreeScalerAggregation); P_dst |
+    // P_src is column block 0 of Y1
+    GPS_TRY(pna_fwd(a->graph, d, a->x, P.Y1, P.Wy, P.pna_q, P.pna_Z, P.pna_Z_p, P.pna_arg, st));
+    // h = Z W_post^T + b_post
+    GemmParams g = linear_fwd(P, N, d, 4 * d, {P.pna_Z, 4 * d, P.pna_Z_p}, {pna->post.weight, 4 * d, P.post_p}, P.pna_h,
+                              d, pna->post.bias);
+    g.Cp = P.pna_h_p;
+    GPS_TRY(gemm(g, st));
+    // x_loc = x + drop(h W_lin^T + b_lin)  (gps_layer.py:188-189)
+    GemmParams g2 = linear_fwd(P, N, d, d, {P.pna_h, d, P.pna_h_p}, {pna->lin.weight, d, P.lin_p}, P.xloc, d,
+                               pna->lin.bias);
+    g2.R1 = a->x; g2.ldr1 = (int)d; g2.stats = stats(BN_L);
+    if (local_writes_s) g2.Cp = P.s_p;
+    set_dropout(g2, P.drop(GPS_SITE_LOCAL));
+    GPS_TRY(gemm(g2, st));
   }
-  if (local_writes_s && !P.gine && !P.gen && P.s_p.hi && N > 0) {   // the GatedGCN / GCN / GAT kernels write fp32 only
+  // the GatedGCN / GCN / GAT kernels write fp32 only
+  if (local_writes_s && !P.gine && !P.gen && !P.pna && P.s_p.hi && N > 0) {
     ToPlanesItem it{P.s, d, (int)N, (int)d, P.s_p};
     GPS_TRY(to_planes(&it, 1, st));
   }
@@ -1053,7 +1150,7 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
 
   // ---- s = norm1_local(x_loc) + norm1_attn(hA)   (gps_layer.py:194,217,222)
   if (!P.nonorm) {
-    const bool loc = P.gated || P.gine || P.gcn || P.gat || P.gen;
+    const bool loc = P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna;
     const float* first = loc ? P.xloc : P.hA;
     BnView bf = loc ? bn_view(P, BN_L, a->norm1_local, N) : bn_view(P, BN_A, a->norm1_attn, N);
     const float* second = (loc && (P.attn || P.perf)) ? P.hA : nullptr;
@@ -1085,9 +1182,9 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
 
 // =================================================================================== backward
 static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, const GpsGenConv* gen,
-                          cudaStream_t st) {
+                          const GpsPna* pna, cudaStream_t st) {
   Plan P;
-  GPS_TRY(make_plan(a, &P, true, gat, gen));
+  GPS_TRY(make_plan(a, &P, true, gat, gen, pna));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
   GPS_REQUIRE(a->workspace_bytes >= P.bwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.bwd_bytes);
@@ -1095,6 +1192,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
   GPS_REQUIRE(a->grad_x_out && a->grad_x, GPS_ERR_ARG, "grad_x_out / grad_x are required");
   GPS_REQUIRE(!P.gat || P.E == 0 || a->grad_edge_attr, GPS_ERR_ARG, "grad_edge_attr is required for GAT");
   GPS_REQUIRE(!P.gen || P.E == 0 || a->grad_edge_attr, GPS_ERR_ARG, "grad_edge_attr is required for GENConv");
+  GPS_REQUIRE(!P.pna || P.E == 0 || a->grad_edge_attr, GPS_ERR_ARG, "grad_edge_attr is required for PNA");
   const int64_t N = P.N, E = P.E, d = P.d;
   const int act = a->act;
   DropCfg nodrop;
@@ -1106,7 +1204,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
   auto wfork = [&](cudaStream_t from) -> int { return sd->order(from, s2); };
-  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen) && (P.attn || P.perf);
+  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) && (P.attn || P.perf);
   cudaStream_t sa = two_branches ? sd->s3 : st;   // stream of the attention-branch backward
   cudaStream_t se = sd->s4;                       // stream of the edge BatchNorm backward (GatedGCN)
   const int opt = opt_flags();
@@ -1190,7 +1288,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     // reductions ride this GEMM's epilogue instead of two more passes over g_s (GPS_B200_OPT bit 64)
     fused_la = (opt & 64) && !P.nonorm && P.use_planes && g2.Ap.hi && g2.Bp.hi && N > 0 && P.train;
     if (fused_la) {
-      if (P.gated || P.gine || P.gcn || P.gat || P.gen) {
+      if (P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) {
         BnView v = bn_view(P, BN_L, a->norm1_local);
         g2.bnred[0].z = P.xloc; g2.bnred[0].ldz = (int)d; g2.bnred[0].mean = v.mean; g2.bnred[0].invstd = v.invstd;
         g2.bnred[0].sums = sums(BN_L);
@@ -1204,7 +1302,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     GPS_TRY(gemm(g2, st));
   }
 
-  const bool loc = P.gated || P.gine || P.gcn || P.gat || P.gen;
+  const bool loc = P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna;
   bool chain_x = false;
   // ---- norm1_local / norm1_attn (gps_layer.py:194,217): g_xloc, g_hA
   if (loc && !P.nonorm) {
@@ -1391,6 +1489,38 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     GPS_TRY(genconv_bwd_dst(a->graph, d, a->x, a->edge_attr, P.agg, P.gen_lse, P.gen_gu, a->grad_edge_attr, st));
     GPS_TRY(gine_bwd_src(a->graph, d, a->grad_edge_attr, P.gen_gu, 0.f, g_xloc, P.g_xl, st));
     g_x_local = P.g_xl;
+  } else if (P.pna) {
+    // x_loc = x + drop(h W_lin^T + b_lin), h = Z W_post^T + b_post
+    Operand g_l;
+    GPS_TRY(dropmul(P, {g_xloc, d, g_xloc_p}, P.g_tmp3, P.gtmp3_p, GPS_SITE_LOCAL, st, &g_l));
+    // g_h = g_l W_lin
+    GemmParams g = linear_dgrad(P, N, d, d, g_l, {pna->lin.weight, d, P.lin_p}, P.pna_gh, d);
+    g.Cp = P.pna_gh_p;
+    GPS_TRY(gemm(g, st));
+    const Operand g_h{P.pna_gh, d, P.pna_gh_p};
+    GPS_TRY(wfork(st));
+    GPS_TRY(linear_wgrad(P, g_l, {P.pna_h, d, P.pna_h_p}, N, d, d, pna->lin.grad_weight, pna->lin.grad_bias, s2));
+    GPS_TRY(linear_wgrad(P, g_h, {P.pna_Z, 4 * d, P.pna_Z_p}, N, d, 4 * d, pna->post.grad_weight, pna->post.grad_bias,
+                         s2));
+    // g_Z = g_h W_post [N, 4d]
+    GPS_TRY(gemm(linear_dgrad(P, N, 4 * d, d, g_h, {pna->post.weight, 4 * d, P.post_p}, P.pna_gZ, 4 * d), st));
+    // g_q (every edge's g_m), g_P_dst | g_P_src -> gY1[:, 0:2d], g_x_local = g_xloc + g_Z[:, 0:d]
+    GPS_TRY(pna_bwd(a->graph, d, P.pna_gZ, P.pna_arg, g_xloc, P.pna_gq, P.pna_gq_p, P.gY1, P.Wy, P.gY1_p, P.g_xl, st));
+    // edge term: g_F = g_q^T e, g_c = colsum(g_q), unfolded into edge_encoder, pre's edge block and pre's bias
+    const Operand g_q{P.pna_gq, d, P.pna_gq_p};
+    float* g_F = P.pna_gF;
+    float* g_c = P.pna_gF + d * P.de;
+    GPS_TRY(wfork(st));
+    GPS_CUDA(cudaMemsetAsync(g_F, 0, (size_t)(d * P.de + d) * sizeof(float), s2));
+    GPS_TRY(wgrad_add(P, g_q, {a->edge_attr, P.de, P.e_p}, E, d, P.de, g_F, g_c, s2));
+    GPS_TRY(pna_fold_bwd(pna->pre.weight, pna->edge_encoder.weight, pna->edge_encoder.bias, g_F, g_c, d, P.de,
+                         pna->pre.grad_weight, pna->pre.grad_bias, pna->edge_encoder.grad_weight,
+                         pna->edge_encoder.grad_bias, P.grads_accumulate, s2));
+    GPS_TRY(mid_done());
+    // grad_edge_attr = g_q F
+    if (E > 0)
+      GPS_TRY(gemm(linear_dgrad(P, E, P.de, d, g_q, {P.pna_F, P.de, P.pna_F_p}, a->grad_edge_attr, P.de), st));
+    g_x_local = P.g_xl;
   }
 
   if (two_branches) GPS_TRY(sd->order(sa, st));
@@ -1475,24 +1605,24 @@ extern "C" int gps_layer_plan(const GpsLayerArgs* args, GpsLayerPlan* plan) {
 
 extern "C" int gps_layer_forward(const GpsLayerArgs* args, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_forward: null args");
-  return layer_forward(args, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+  return layer_forward(args, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward(const GpsLayerArgs* args, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_backward: null args");
-  return layer_backward(args, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+  return layer_backward(args, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_forward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_forward_biased: null args");
   GPS_TRY(check_bias(args, bias));
-  return layer_forward(args, bias, nullptr, nullptr, (cudaStream_t)stream);
+  return layer_forward(args, bias, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_backward_biased: null args");
   GPS_TRY(check_bias(args, bias));
-  return layer_backward(args, bias, nullptr, nullptr, (cudaStream_t)stream);
+  return layer_backward(args, bias, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 static int check_gat(const GpsLayerArgs* a, const GpsGat* gat, const char* what) {
@@ -1505,14 +1635,14 @@ static int check_gat(const GpsLayerArgs* a, const GpsGat* gat, const char* what)
 extern "C" int gps_layer_forward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias, void* stream) {
   GPS_TRY(check_gat(args, gat, "gps_layer_forward_gat"));
   GPS_TRY(check_bias(args, bias));
-  return layer_forward(args, bias, gat, nullptr, (cudaStream_t)stream);
+  return layer_forward(args, bias, gat, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias,
                                       void* stream) {
   GPS_TRY(check_gat(args, gat, "gps_layer_backward_gat"));
   GPS_TRY(check_bias(args, bias));
-  return layer_backward(args, bias, gat, nullptr, (cudaStream_t)stream);
+  return layer_backward(args, bias, gat, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 static int check_genconv(const GpsLayerArgs* a, const GpsGenConv* gen, const char* what) {
@@ -1526,14 +1656,35 @@ extern "C" int gps_layer_forward_genconv(const GpsLayerArgs* args, const GpsGenC
                                          void* stream) {
   GPS_TRY(check_genconv(args, gen, "gps_layer_forward_genconv"));
   GPS_TRY(check_bias(args, bias));
-  return layer_forward(args, bias, nullptr, gen, (cudaStream_t)stream);
+  return layer_forward(args, bias, nullptr, gen, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias,
                                           void* stream) {
   GPS_TRY(check_genconv(args, gen, "gps_layer_backward_genconv"));
   GPS_TRY(check_bias(args, bias));
-  return layer_backward(args, bias, nullptr, gen, (cudaStream_t)stream);
+  return layer_backward(args, bias, nullptr, gen, nullptr, (cudaStream_t)stream);
+}
+
+static int check_pna(const GpsLayerArgs* a, const GpsPna* pna, const char* what) {
+  GPS_REQUIRE(a && pna, GPS_ERR_ARG, "%s: null args / pna", what);
+  GPS_REQUIRE(a->local_type == GPS_LOCAL_PNA, GPS_ERR_ARG, "%s: a GpsPna needs local_type GPS_LOCAL_PNA (got %d)", what,
+              a->local_type);
+  return GPS_OK;
+}
+
+extern "C" int gps_layer_forward_pna(const GpsLayerArgs* args, const GpsPna* pna, const GpsAttnBias* bias,
+                                     void* stream) {
+  GPS_TRY(check_pna(args, pna, "gps_layer_forward_pna"));
+  GPS_TRY(check_bias(args, bias));
+  return layer_forward(args, bias, nullptr, nullptr, pna, (cudaStream_t)stream);
+}
+
+extern "C" int gps_layer_backward_pna(const GpsLayerArgs* args, const GpsPna* pna, const GpsAttnBias* bias,
+                                      void* stream) {
+  GPS_TRY(check_pna(args, pna, "gps_layer_backward_pna"));
+  GPS_TRY(check_bias(args, bias));
+  return layer_backward(args, bias, nullptr, nullptr, pna, (cudaStream_t)stream);
 }
 
 extern "C" int gps_linear_forward(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias,
@@ -1751,6 +1902,40 @@ extern "C" int gps_genconv_aggregate_backward(const GpsGraph* g, int64_t d, cons
   GPS_TRY(stage_width(d, "genconv_aggregate_backward"));
   GPS_TRY(genconv_bwd_dst(*g, d, x, e, agg, lse, g_u, g_e, (cudaStream_t)stream));
   return gine_bwd_src(*g, d, g_e, g_u, 0.f, add, g_x, (cudaStream_t)stream);
+}
+
+// ---- stage entry points of the PNA edge fold and message passing (pna.cu)
+extern "C" int gps_pna_fold_forward(const float* pre_w, const float* pre_b, const float* enc_w, const float* enc_b,
+                                    int64_t d, int64_t de, float* F, float* c, void* stream) {
+  GPS_REQUIRE(pre_w && pre_b && enc_w && enc_b && F && c, GPS_ERR_ARG, "pna_fold_forward: null argument");
+  GPS_TRY(stage_width(d, "pna_fold_forward"));
+  return pna_fold_fwd(pre_w, pre_b, enc_w, enc_b, d, de, F, c, (cudaStream_t)stream);
+}
+
+extern "C" int gps_pna_fold_backward(const float* pre_w, const float* enc_w, const float* enc_b, const float* g_F,
+                                     const float* g_c, int64_t d, int64_t de, float* grad_pre_w, float* grad_pre_b,
+                                     float* grad_enc_w, float* grad_enc_b, int32_t accumulate, void* stream) {
+  GPS_REQUIRE(pre_w && enc_w && enc_b && g_F && g_c, GPS_ERR_ARG, "pna_fold_backward: null argument");
+  GPS_TRY(stage_width(d, "pna_fold_backward"));
+  return pna_fold_bwd(pre_w, enc_w, enc_b, g_F, g_c, d, de, grad_pre_w, grad_pre_b, grad_enc_w, grad_enc_b,
+                      accumulate != 0, (cudaStream_t)stream);
+}
+
+extern "C" int gps_pna_aggregate_forward(const GpsGraph* g, int64_t d, const float* x, const float* Y, int64_t ldy,
+                                         const float* q, float* Z, int32_t* arg, void* stream) {
+  GPS_REQUIRE(g && x && Y && Z && arg && (q || g->E == 0), GPS_ERR_ARG, "pna_aggregate_forward: null argument");
+  GPS_TRY(stage_width(d, "pna_aggregate_forward"));
+  GPS_REQUIRE(ldy >= 2 * d && ldy % 4 == 0, GPS_ERR_ARG, "pna_aggregate_forward: ldy must be >= 2d and a multiple of 4");
+  return pna_fwd(*g, d, x, Y, ldy, q, Z, Planes(), arg, (cudaStream_t)stream);
+}
+
+extern "C" int gps_pna_aggregate_backward(const GpsGraph* g, int64_t d, const float* g_Z, const int32_t* arg,
+                                          const float* add, float* g_q, float* gY, int64_t ldg, float* g_x,
+                                          void* stream) {
+  GPS_REQUIRE(g && g_Z && arg && gY && g_x && (g_q || g->E == 0), GPS_ERR_ARG, "pna_aggregate_backward: null argument");
+  GPS_TRY(stage_width(d, "pna_aggregate_backward"));
+  GPS_REQUIRE(ldg >= 2 * d && ldg % 4 == 0, GPS_ERR_ARG, "pna_aggregate_backward: ldg must be >= 2d and a multiple of 4");
+  return pna_bwd(*g, d, g_Z, arg, add, g_q, Planes(), gY, ldg, Planes(), g_x, (cudaStream_t)stream);
 }
 
 // ---- stage entry points of the Performer (performer.cu, performer_quad.cu).  Each validates its arguments before it

@@ -20,9 +20,10 @@ import torch.nn as nn
 from . import _lib
 from .graph import graph_of
 
-_SUPPORTED_LOCAL = ("None", "CustomGatedGCN", "GINE", "GCN", "GAT", "GENConv")
-_EDGE_LOCAL = ("CustomGatedGCN", "GINE", "GAT", "GENConv")   # local models that read batch.edge_attr (gps_layer.py:44-53)
-_KNOWN_LOCAL = _SUPPORTED_LOCAL + ("GIN", "PNA")
+_SUPPORTED_LOCAL = ("None", "CustomGatedGCN", "GINE", "GCN", "GAT", "GENConv", "PNA")
+# local models that read batch.edge_attr (gps_layer.py:44-90)
+_EDGE_LOCAL = ("CustomGatedGCN", "GINE", "GAT", "GENConv", "PNA")
+_KNOWN_LOCAL = _SUPPORTED_LOCAL + ("GIN",)
 _SUPPORTED_GLOBAL = ("None", "Transformer", "BiasedTransformer", "Performer")
 _KNOWN_GLOBAL = _SUPPORTED_GLOBAL + ("BigBird",)
 _MHA_GLOBAL = ("Transformer", "BiasedTransformer")   # torch's MultiheadAttention (gps_layer.py:104-106)
@@ -161,6 +162,37 @@ class _GENConvParams(nn.Module):
                                  nn.Dropout(0.0), nn.Linear(2 * dim, dim, bias=False))
 
 
+class _PNAConvParams(nn.Module):
+    """Names of PyG 2.2 PNAConv(dim_h, dim_h, aggregators=['mean', 'max', 'sum'], scalers=['identity'], deg,
+    edge_dim=min(128, dim_h), towers=1, pre_layers=1, post_layers=1, divide_input=False) as built at gps_layer.py:75-90:
+    edge_encoder [d, de], pre_nns.0.0 [d, 3d], post_nns.0.0 [d, 4d] and lin [d, d], all with bias and torch's default
+    Linear initialisation (PyG's Linear without initialisers).  DegreeScalerAggregation keeps the average degrees as a
+    Python dict, so there are no buffers; with the identity scaler the histogram does not enter the arithmetic."""
+
+    def __init__(self, dim, pna_degrees):
+        super().__init__()
+        self.edge_dim = min(128, dim)
+        self.deg = [int(v) for v in pna_degrees]
+        self.edge_encoder = nn.Linear(self.edge_dim, dim)
+        self.pre_nns = nn.ModuleList([nn.Sequential(nn.Linear(3 * dim, dim))])
+        self.post_nns = nn.ModuleList([nn.Sequential(nn.Linear(4 * dim, dim))])
+        self.lin = nn.Linear(dim, dim)
+
+
+def _pna_histogram(pna_degrees):
+    """cfg.gt.pna_degrees as a list of counts; NotImplementedError where the reference cannot build PNAConv."""
+    if pna_degrees is None:
+        raise NotImplementedError(
+            "PNA needs pna_degrees (cfg.gt.pna_degrees, the in-degree histogram): the reference fails to construct "
+            "the layer without it (torch.from_numpy(np.array(None)) raises TypeError, gps_layer.py:80)")
+    deg = torch.as_tensor(pna_degrees).flatten()
+    if deg.numel() == 0 or bool((deg < 0).any()) or float(deg.sum()) == 0:
+        raise NotImplementedError(
+            "PNA needs a non-empty in-degree histogram with non-negative counts and a positive total: PNAConv divides "
+            f"by the number of nodes it counts when it builds its average degrees (got {deg.tolist()})")
+    return deg.tolist()
+
+
 def _orthogonal_gaussian_matrix(nb_rows, nb_cols):
     """Random-feature projection drawn once at construction (performer_layer.py:163-195, scaling=0)."""
     blocks = []
@@ -226,6 +258,7 @@ class _GPSLayerFn(torch.autograd.Function):
         e_out = torch.empty_like(e) if layer.local_gnn_type == "CustomGatedGCN" else None
         gat = layer._gat_args(named) if layer.local_gnn_type == "GAT" else None
         gen = layer._genconv_args(named) if layer.local_gnn_type == "GENConv" else None
+        pna = layer._pna_args(named) if layer.local_gnn_type == "PNA" else None
         plan = layer._plan(args, gs)
         saved = torch.empty(max(plan[0], 256), dtype=torch.uint8, device=dev)
         ws = _workspace(dev, plan[1])
@@ -247,6 +280,9 @@ class _GPSLayerFn(torch.autograd.Function):
             ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)) if ctx.nmax else None
             _lib.check(lib.gps_layer_forward_genconv(C.byref(args), C.byref(gen), ab, stream),
                        "gps_layer_forward_genconv")
+        elif pna is not None:
+            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)) if ctx.nmax else None
+            _lib.check(lib.gps_layer_forward_pna(C.byref(args), C.byref(pna), ab, stream), "gps_layer_forward_pna")
         elif ctx.nmax:
             ab = _lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)
             _lib.check(lib.gps_layer_forward_biased(C.byref(args), C.byref(ab), stream), "gps_layer_forward_biased")
@@ -323,6 +359,10 @@ class _GPSLayerFn(torch.autograd.Function):
             ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))) if ctx.nmax else None
             _lib.check(lib.gps_layer_backward_genconv(C.byref(args), C.byref(gen), ab, stream),
                        "gps_layer_backward_genconv")
+        elif layer.local_gnn_type == "PNA":
+            pna = layer._pna_args(named, grads)
+            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))) if ctx.nmax else None
+            _lib.check(lib.gps_layer_backward_pna(C.byref(args), C.byref(pna), ab, stream), "gps_layer_backward_pna")
         elif ctx.nmax:
             ab = _lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))
             _lib.check(lib.gps_layer_backward_biased(C.byref(args), C.byref(ab), stream), "gps_layer_backward_biased")
@@ -386,6 +426,11 @@ class GPSLayer(nn.Module):
                 "GENConv with equivstable_pe=True is not built in graphgps_b200: the reference passes "
                 "batch.pe_EquivStableLapPE as GENConv.forward's fourth positional parameter, which is `size` "
                 "(gps_layer.py:176-181), so there is no defined behaviour to match")
+        if equivstable_pe and local_gnn_type == "PNA":
+            raise NotImplementedError(
+                "PNA with equivstable_pe=True is not built in graphgps_b200: the reference passes "
+                "batch.pe_EquivStableLapPE as a fourth positional argument to PNAConv.forward(x, edge_index, edge_attr), "
+                "which fails (gps_layer.py:176-181)")
         # EquivStableLapPE gate: read by GatedGCN only; GCN and None ignore the flag (gps_layer.py:176-187)
         self._eslap = bool(equivstable_pe) and local_gnn_type == "CustomGatedGCN"
         if local_gnn_type == "None":
@@ -402,6 +447,8 @@ class GPSLayer(nn.Module):
             self.local_model = _GATConvParams(dim_h, num_heads)
         elif local_gnn_type == "GENConv":
             self.local_model = _GENConvParams(dim_h)
+        elif local_gnn_type == "PNA":
+            self.local_model = _PNAConvParams(dim_h, _pna_histogram(pna_degrees))
         else:
             self.local_model = _GatedGCNParams(dim_h, act, self._eslap)
         self.local_gnn_type = local_gnn_type
@@ -630,6 +677,17 @@ class GPSLayer(nn.Module):
                               _lib.ptr(g.get(p + "1.weight")), _lib.ptr(g.get(p + "1.bias"))),
             _lin(named[p + "4.weight"], None, g.get(p + "4.weight")))
 
+    def _pna_args(self, named, grads=None):
+        """GpsPna of the PNA local model (gps_b200.h): edge_encoder, pre_nns.0.0, post_nns.0.0, lin and the edge width."""
+        g = grads or {}
+
+        def lin(prefix):
+            p = "local_model." + prefix
+            return _lin(named[p + ".weight"], named[p + ".bias"], g.get(p + ".weight"), g.get(p + ".bias"))
+
+        return _lib.GpsPna(lin("edge_encoder"), lin("pre_nns.0.0"), lin("post_nns.0.0"), lin("lin"),
+                           self.local_model.edge_dim)
+
     @property
     def _gine_eps_host(self):
         # eps is a constant buffer (train_eps=False); read once, no per-step sync
@@ -648,9 +706,14 @@ class GPSLayer(nn.Module):
             raise TypeError("batch.x must be float32")
         x = x.contiguous()
         e = getattr(batch, "edge_attr", None)
-        if self.local_gnn_type in _EDGE_LOCAL:
+        if self.local_gnn_type == "PNA":   # PNAConv(edge_dim=min(128, dim_h)): the edge encoder's input width
+            if e is None or e.dim() != 2 or e.shape[-1] != self.local_model.edge_dim:
+                raise ValueError(f"PNA reads batch.edge_attr of width min(128, dim_h) = {self.local_model.edge_dim} "
+                                 f"(got {None if e is None else tuple(e.shape)})")
+        elif self.local_gnn_type in _EDGE_LOCAL:
             if e is None or e.shape[-1] != self.dim_h:
                 raise ValueError("Node and edge feature dimensionalities do not match")
+        if self.local_gnn_type in _EDGE_LOCAL:
             if e.dtype != torch.float32 or e.device != x.device:
                 raise TypeError("batch.edge_attr must be float32 on the device of batch.x")
             e = e.contiguous()

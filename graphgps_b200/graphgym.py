@@ -45,6 +45,8 @@ def register(name="gpslayer_b200"):
             # GPSModel passes cfg.posenc_EquivStableLapPE.enable as equivstable_pe (gps_model.py:92)
             pe_cfg = getattr(cfg, "posenc_EquivStableLapPE", None)
             kwargs.setdefault("equivstable_pe", bool(pe_cfg.enable) if pe_cfg is not None else False)
+            # PNA's in-degree histogram (gt_config.py:34-37; master_loader.py:226-231 fills it for PNA layer types)
+            kwargs.setdefault("pna_degrees", getattr(cfg.gt, "pna_degrees", None))
             super().__init__(dim_h=layer_config.dim_out, local_gnn_type=local, global_model_type=glob,
                              num_heads=cfg.gt.n_heads, act=cfg.gnn.act, dropout=cfg.gt.dropout,
                              attn_dropout=cfg.gt.attn_dropout, layer_norm=cfg.gt.layer_norm,

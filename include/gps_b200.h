@@ -37,7 +37,7 @@ enum { GPS_OK = 0, GPS_ERR_ARG = -1, GPS_ERR_UNSUPPORTED = -2, GPS_ERR_CUDA = -3
 
 /* local_gnn_type / global_model_type of GPSLayer.__init__ (gps_layer.py:20-24,44-122) */
 enum { GPS_LOCAL_NONE = 0, GPS_LOCAL_GATEDGCN = 1, GPS_LOCAL_GINE = 2, GPS_LOCAL_GCN = 3, GPS_LOCAL_GAT = 4,
-       GPS_LOCAL_GENCONV = 5 };
+       GPS_LOCAL_GENCONV = 5, GPS_LOCAL_PNA = 6 };
 enum { GPS_GLOBAL_NONE = 0, GPS_GLOBAL_TRANSFORMER = 1, GPS_GLOBAL_PERFORMER = 2 };
 /* register.act_dict keys used by shipped configs (gps_layer.py:33) */
 enum { GPS_ACT_RELU = 0, GPS_ACT_GELU = 1 };
@@ -307,6 +307,36 @@ typedef struct {
 int gps_layer_forward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias, void* stream);
 int gps_layer_backward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias, void* stream);
 
+/* PNA local model (local_type == GPS_LOCAL_PNA): PyG 2.2 PNAConv(dim_h, dim_h, aggregators=['mean','max','sum'],
+ * scalers=['identity'], edge_dim=edge_dim, towers=1, pre_layers=1, post_layers=1, divide_input=False),
+ * gps_layer.py:75-90,183-189.  For edge k from j to i:
+ *   m_k = pre.weight [x_i ; x_j ; edge_encoder(e_k)] + pre.bias
+ * and per target i and channel the mean, max and sum of m over i's in-edges (0 in all three without any; self loops
+ * and duplicates are ordinary edges); x_loc = x + dropout(lin(post([x | mean | max | sum]))).  The max gradient goes
+ * whole to the first maximising in-edge in edge_index order (torch_scatter's scatter_max).  The degree histogram never
+ * enters the arithmetic with the identity scaler, so it is not an argument.  edge_attr and grad_edge_attr are
+ * [E, edge_dim] (non-NULL when E > 0); batch.edge_attr is not updated.  0 < edge_dim <= d and edge_dim % 4 == 0, else
+ * GPS_ERR_UNSUPPORTED.  Parameters (weights and biases non-NULL, else GPS_ERR_ARG):
+ *   edge_encoder = local_model.edge_encoder [d, edge_dim] + [d]; gradients final at ev_grads_mid;
+ *   pre  = local_model.pre_nns.0.0 [d, 3d] + [d] (column blocks: destination, source, encoded edge); gradients final
+ *          at ev_grads_done (the first two blocks come with the fused node projection);
+ *   post = local_model.post_nns.0.0 [d, 4d] + [d]; gradients final at ev_grads_mid;
+ *   lin  = local_model.lin [d, d] + [d]; gradients final at ev_grads_mid. */
+typedef struct {
+  GpsLinear edge_encoder;
+  GpsLinear pre;
+  GpsLinear post;
+  GpsLinear lin;
+  int64_t edge_dim;
+} GpsPna;
+
+/* gps_layer_forward / _backward of a PNA layer; bias: GpsAttnBias of a BiasedTransformer global model or NULL.
+ * gps_layer_plan sizes PNA from local_type alone, with edge_dim <= d as the bound.  The plain, _biased, _gat and
+ * _genconv calls with local_type == GPS_LOCAL_PNA, and these with a NULL pna or another local_type, return GPS_ERR_ARG
+ * before any CUDA call, as does a NULL edge_attr (E > 0) or, in the backward, grad_edge_attr (E > 0). */
+int gps_layer_forward_pna(const GpsLayerArgs* args, const GpsPna* pna, const GpsAttnBias* bias, void* stream);
+int gps_layer_backward_pna(const GpsLayerArgs* args, const GpsPna* pna, const GpsAttnBias* bias, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Stage-level entry points (the same kernels the layer calls; exported so the parity tests can
  * pin each stage against the oracle separately).
@@ -418,6 +448,27 @@ int gps_genconv_aggregate_forward(const GpsGraph* g, int64_t d, const float* x, 
 int gps_genconv_aggregate_backward(const GpsGraph* g, int64_t d, const float* x, const float* e, const float* agg,
                                    const float* lse, const float* g_u, const float* add, float* g_e, float* g_x,
                                    void* stream);
+
+/* PNA stage entry points (the kernels the PNA layer calls between its dense products).  W_e is the column block
+ * 2d..3d of pre_w [d, 3d]; de = edge_dim (0 < de <= d, de % 4 == 0, else GPS_ERR_UNSUPPORTED).
+ * Fold: F [d, de] = W_e enc_w, c [d] = W_e enc_b + pre_b, so that pre's edge term is e F^T + c.
+ * Fold backward from g_F [d, de] and g_c [d]: the gradients of pre_w's block 2d..3d (the other blocks are not
+ * touched), pre_b, enc_w [d, de] and enc_b, written, or added when accumulate != 0 (each NULL = not needed).
+ * Aggregate forward: m_k = Y[i, 0:d] + Y[j, d:2d] + q[k] for edge k from j to i (Y [N, ldy], q [E, d], NULL when
+ * E == 0); Z [N, 4d] = [x | mean | max | sum] of m over each node's in-edges (0 without any), arg [N, d] int32 = edge
+ * id of the first maximiser (-1 without in-edges).
+ * Aggregate backward from g_Z [N, 4d]: g_q [E, d] (g_m of every edge), gY[:, 0:d] = the sum of g_m over in-edges,
+ * gY[:, d:2d] = the sum of g_m over out-edges (gY [N, ldg], ldg >= 2d), g_x [N, d] = g_Z[:, 0:d] (+ add, NULL =
+ * none). */
+int gps_pna_fold_forward(const float* pre_w, const float* pre_b, const float* enc_w, const float* enc_b, int64_t d,
+                         int64_t de, float* F, float* c, void* stream);
+int gps_pna_fold_backward(const float* pre_w, const float* enc_w, const float* enc_b, const float* g_F,
+                          const float* g_c, int64_t d, int64_t de, float* grad_pre_w, float* grad_pre_b,
+                          float* grad_enc_w, float* grad_enc_b, int32_t accumulate, void* stream);
+int gps_pna_aggregate_forward(const GpsGraph* g, int64_t d, const float* x, const float* Y, int64_t ldy,
+                              const float* q, float* Z, int32_t* arg, void* stream);
+int gps_pna_aggregate_backward(const GpsGraph* g, int64_t d, const float* g_Z, const int32_t* arg, const float* add,
+                               float* g_q, float* gY, int64_t ldg, float* g_x, void* stream);
 
 /* Performer stage entry points (FAVOR+, performer_layer.py:119-144,200-205), the calls one layer makes, in order.
  * They take dim_head == 64 and 256 < m <= 272 features (else GPS_ERR_UNSUPPORTED), H > 0 and N * H * 272 < 2^31 (else
