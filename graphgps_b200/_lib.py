@@ -16,6 +16,9 @@ LIB_PATH = os.path.join(_HERE, "libgps_b200.so")
 GPS_OK, GPS_ERR_ARG, GPS_ERR_UNSUPPORTED, GPS_ERR_CUDA = 0, -1, -2, -3
 LOCAL = {"None": 0, "CustomGatedGCN": 1, "GINE": 2, "GCN": 3, "GAT": 4, "GENConv": 5, "PNA": 6}
 GLOBAL = {"None": 0, "Transformer": 1, "Performer": 2}
+# the BigBird global model: reached through gps_layer_{forward,backward}_bigbird only, so not in GLOBAL
+GLOBAL_BIGBIRD = 3
+BIGBIRD_ACT = {"relu": 0, "sigmoid": 1}   # GpsBigBird.hidden_act
 ACT = {"relu": 0, "gelu": 1}
 PRECISION = {"fp32": 0, "bf16": 1}
 NORM = {"batch": 0, "none": 1}
@@ -97,6 +100,16 @@ class GpsPna(C.Structure):
                 ("edge_dim", C.c_int64)]
 
 
+class GpsBigBird(C.Structure):
+    """BigBird global model: block geometry, the per-head block lists (device int32) and the eight parameters of
+    self_attn.encoder.layers.0 (query, key, value, attention.output.dense / .LayerNorm, intermediate.dense,
+    output.dense / .LayerNorm)."""
+    _fields_ = [("block_size", C.c_int64), ("num_blocks", C.c_int64), ("hidden_act", C.c_int32), ("ln_eps", C.c_float),
+                ("key_ptr", _fp), ("key_idx", _fp), ("query_ptr", _fp), ("query_idx", _fp),
+                ("query", GpsLinear), ("key", GpsLinear), ("value", GpsLinear), ("self_out", GpsLinear),
+                ("ln1", GpsLinear), ("intermediate", GpsLinear), ("output", GpsLinear), ("ln2", GpsLinear)]
+
+
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
                 ("bwd_workspace_bytes", C.c_int64), ("fwd_launches", C.c_int64),
@@ -124,6 +137,16 @@ SYMBOLS = {
                                              _fp]),
     "gps_layer_forward_pna": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsPna), C.POINTER(GpsAttnBias), _fp]),
     "gps_layer_backward_pna": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsPna), C.POINTER(GpsAttnBias), _fp]),
+    "gps_layer_forward_bigbird": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsBigBird), C.POINTER(GpsGat),
+                                            C.POINTER(GpsGenConv), C.POINTER(GpsPna), _fp]),
+    "gps_layer_backward_bigbird": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsBigBird), C.POINTER(GpsGat),
+                                             C.POINTER(GpsGenConv), C.POINTER(GpsPna), _fp]),
+    "gps_bigbird_attention_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, C.POINTER(GpsBigBird), _fp, _fp, _fp,
+                                                _i64, _fp, _i64, _fp, _fp]),
+    "gps_bigbird_attention_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, C.POINTER(GpsBigBird), _fp, _fp, _fp,
+                                                 _i64, _fp, _fp, _i64, _fp, _fp, _fp, _fp, _fp, _i64, _fp]),
+    "gps_layernorm_forward": (C.c_int, [_fp, _i64, _i64, _fp, _fp, _f32, _fp, _fp, _fp, _fp]),
+    "gps_layernorm_backward": (C.c_int, [_fp, _fp, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i32, _fp]),
     "gps_linear_forward": (C.c_int, [_fp, _i64, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _fp]),
     "gps_gemm": (C.c_int, [_fp, _i64, _i32, _fp, _i64, _i32, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _fp]),
     "gps_gatedgcn_aggregate_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _fp, _fp, _fp, _fp, _i64, _fp, _fp,

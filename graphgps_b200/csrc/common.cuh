@@ -169,7 +169,10 @@ __device__ __forceinline__ float4 dropout_scale4(float p, uint64_t seed, uint64_
 // dropout sites (Philox stream ids); attention uses GPS_SITE_ATTN_P + head
 enum {
   GPS_SITE_GCN_X = 1, GPS_SITE_GCN_E = 2, GPS_SITE_LOCAL = 3, GPS_SITE_ATTN_OUT = 4,
-  GPS_SITE_FF1 = 5, GPS_SITE_FF2 = 6, GPS_SITE_PERF_OUT = 7, GPS_SITE_ATTN_P = 16
+  GPS_SITE_FF1 = 5, GPS_SITE_FF2 = 6, GPS_SITE_PERF_OUT = 7,
+  GPS_SITE_BB_SELF_OUT = 8,   // BigBird attention.output.dropout, on dense(ctx) before LayerNorm 1
+  GPS_SITE_BB_OUTPUT = 9,     // BigBird output.dropout, on dense(u) before LayerNorm 2
+  GPS_SITE_ATTN_P = 16
 };
 
 __device__ __forceinline__ float warp_sum(float v) {

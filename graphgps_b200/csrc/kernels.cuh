@@ -174,6 +174,29 @@ int attention_bwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, 
                   cudaStream_t stream, const unsigned long long* offset_dev = nullptr, Planes dQp = Planes(),
                   Planes dKp = Planes(), Planes dVp = Planes(), const GpsAttnBias* bias = nullptr);
 
+// BigBird (bigbird.cu).  bb_check: a usable GpsBigBird for d / H (GPS_ERR_ARG, or GPS_ERR_UNSUPPORTED for hd > 128).
+// Block-sparse attention over the packed rows: forward O, lse [N, H]; backward delta [N, H], then dQ, dK, dV written
+// whole.  LayerNorm: out = [R1 +] drop(LN(z)) [+ R2] (+ planes, + double column sums into stats [2][d]), mean / rstd
+// [rows] saved.  Its backward from g' = gdrop(g): out1 = drop1(dz) (+ planes), out2 = dz (+ add) (each NULL = not
+// wanted), grad_gamma / grad_beta through part (layernorm_part_floats(d) floats), written or added.
+int bb_check(int64_t d, int64_t H, const GpsBigBird* bb);
+int bb_attn_fwd(const GpsGraph& g, int64_t H, int64_t hd, const GpsBigBird& bb, const float* Q, const float* K,
+                const float* V, int64_t ld, float* O, int64_t ldo, float* lse, cudaStream_t stream);
+int bb_attn_bwd(const GpsGraph& g, int64_t H, int64_t hd, const GpsBigBird& bb, const float* Q, const float* K,
+                const float* V, int64_t ld, const float* O, const float* dO, int64_t ldo, const float* lse, float* delta,
+                float* dQ, float* dK, float* dV, int64_t ldg, cudaStream_t stream);
+int64_t layernorm_part_floats(int64_t d);
+int layernorm_fwd(const float* z, int64_t rows, int64_t d, const float* gamma, const float* beta, float eps, float* mean,
+                  float* rstd, float* out, Planes outp, const float* R1, const float* R2, DropCfg drop, double* stats,
+                  cudaStream_t stream);
+int layernorm_bwd(const float* g, DropCfg gdrop, const float* z, int64_t rows, int64_t d, const float* gamma,
+                  const float* mean, const float* rstd, float* out1, Planes out1p, DropCfg drop1, float* out2,
+                  const float* add, float* part, float* grad_gamma, float* grad_beta, bool accumulate,
+                  cudaStream_t stream);
+// sigmoid in place (+ planes); its backward g *= s (1 - s) in place (+ planes)
+int sigmoid_fwd(float* x, int64_t rows, int64_t d, Planes p, cudaStream_t stream);
+int sigmoid_bwd(float* g, const float* s, int64_t rows, int64_t d, Planes p, cudaStream_t stream);
+
 // wgmma version (attention_tc.cu): Q, K, V from bf16 hi/lo planes in the per-head padded layout
 // column (which * H + h) * hd_pad + k, hd_pad = attention_tc_hd_pad(hd), pad columns zero
 void attention_tc_set_debug(float* buf);   // bring-up: 3 x 128 x 128 floats (S, P, raw O of CTA (0,0))

@@ -160,7 +160,7 @@ struct PackSeg {
   const float* w; const float* b; float* gw; float* gb; int rows; int ld;
 };
 struct PackDesc {
-  PackSeg seg[5];
+  PackSeg seg[8];
   int nseg; int d; int total_rows;
 };
 
@@ -258,6 +258,15 @@ struct Plan {
   bool perf_pairwise;     // mean graph size <= 48: n^2 (m+64) < 2 n m 64
   float *g_pfq, *g_pfk, *g_pQ, *g_pK, *g_pV, *g_pgmax, *g_xp;   // backward workspace (Performer)
   float* g_pgrow;         // [N*H] per-row stabiliser gradients, summed per (graph, head) in a fixed order
+  // BigBird (bigbird.cu): the caller's GpsBigBird (NULL when only sizes are wanted).  The attention output and lse are O /
+  // lse.  Saved: z1 = drop(ctx Wso^T + bso) + x, a = LN1(z1) (+ planes), u = act(a Wi^T + bi) (+ planes),
+  // z2 = drop(u Wo^T + bo) + a, and the row statistics mean1 | rstd1 | mean2 | rstd2 [4][N].  Backward: g_od (gradient of
+  // output.dense, + planes), dz2, g_u (+ planes), g_a, g_so (gradient of attention.output.dense, + planes), g_x part
+  // dz1 + g_hA, and the LayerNorm partials.
+  bool bb;
+  const GpsBigBird* bbp;
+  float *bb_z1, *bb_a, *bb_u, *bb_z2, *bb_stat, *bb_god, *bb_dz2, *bb_gu, *bb_ga, *bb_gso, *bb_gx, *bb_part;
+  Planes bb_a_p, bb_u_p, bb_so_p, bb_in_p, bb_out_p, bb_god_p, bb_gu_p, bb_gso_p;
   // saved
   float *Wcat, *bcat, *Y1, *ehat, *xt, *xloc, *O, *lse, *hA, *s, *hid, *hid_pre, *t, *bnbuf;
   float *agg, *h1, *h1_pre;
@@ -275,7 +284,7 @@ struct Plan {
   Planes qkv_p;        // Q | K | V per head, padded to hd_pad columns: operands of the wgmma attention
   bool attn_tc;        // softmax attention on the tensor cores (attention_tc.cu)
   // the weights with operand planes, in the order their planes are allocated and converted (list_weights)
-  LayerWeight weights[12];
+  LayerWeight weights[16];
   int nweights;
   int64_t saved_bytes;
   int64_t wplanes_bytes;
@@ -340,6 +349,15 @@ static void list_weights(const GpsLayerArgs* a, Plan* P) {
   P->qkv_off = P->Wy;
   if (P->attn) add(a->attn_in, 3 * d, d, &Plan::Wcat_p);
   if (P->attn || P->perf) add(a->attn_out, d, kout, &Plan::out_p);
+  if (P->bb) {   // attention.self.{query,key,value} (bias only with use_bias) fill the in_proj rows of Wcat
+    const GpsBigBird& b = P->bbp ? *P->bbp : GpsBigBird{};
+    add(b.query, d, d, &Plan::Wcat_p);
+    add(b.key, d, d, &Plan::Wcat_p);
+    add(b.value, d, d, &Plan::Wcat_p);
+    add(b.self_out, d, d, &Plan::bb_so_p);
+    add(b.intermediate, d, d, &Plan::bb_in_p);
+    add(b.output, d, d, &Plan::bb_out_p);
+  }
   add(a->ff1, 2 * d, d, &Plan::ff1_p);
   add(a->ff2, d, 2 * d, &Plan::ff2_p);
   if (P->gine) {
@@ -370,7 +388,7 @@ static Planes caller_planes(const GpsPlanes& g, int64_t d, int precision) {
 }
 
 static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* gat = nullptr,
-                     const GpsGenConv* gen = nullptr, const GpsPna* pna = nullptr) {
+                     const GpsGenConv* gen = nullptr, const GpsPna* pna = nullptr, const GpsBigBird* bb = nullptr) {
   memset(P, 0, sizeof(*P));
   GPS_REQUIRE(a, GPS_ERR_ARG, "null args");
   P->N = a->graph.N;
@@ -400,10 +418,20 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   GPS_REQUIRE(!P->eslap || P->gated, GPS_ERR_ARG, "pe (EquivStableLapPE) is read by the GatedGCN local model only");
   GPS_REQUIRE(!P->eslap || a->pe_dim >= 1, GPS_ERR_ARG, "pe_dim must be >= 1 (got %lld)", (long long)a->pe_dim);
   GPS_REQUIRE(a->global_type == GPS_GLOBAL_NONE || a->global_type == GPS_GLOBAL_TRANSFORMER ||
-                  a->global_type == GPS_GLOBAL_PERFORMER,
+                  a->global_type == GPS_GLOBAL_PERFORMER || a->global_type == GPS_GLOBAL_BIGBIRD,
               GPS_ERR_ARG, "unknown global_type %d", a->global_type);
   P->attn = a->global_type == GPS_GLOBAL_TRANSFORMER;
   P->perf = a->global_type == GPS_GLOBAL_PERFORMER;
+  P->bb = a->global_type == GPS_GLOBAL_BIGBIRD;
+  P->bbp = bb;
+  GPS_REQUIRE(!bind || P->bb == (bb != nullptr), GPS_ERR_ARG,
+              P->bb ? "global_type GPS_GLOBAL_BIGBIRD needs gps_layer_forward_bigbird / gps_layer_backward_bigbird"
+                    : "a GpsBigBird needs global_type GPS_GLOBAL_BIGBIRD");
+  if (P->bb) {   // any head dim (the shipped BigBird config has hd = 7)
+    GPS_REQUIRE(a->heads > 0 && a->d % a->heads == 0, GPS_ERR_ARG, "dim_h %% num_heads != 0");
+    P->hd = a->d / a->heads;
+    if (bb) GPS_TRY(bb_check(a->d, a->heads, bb));
+  }
   if (P->perf) {
     GPS_TRY(perf_supported(a->perf_dim_head, a->perf_features));
     GPS_REQUIRE(a->heads > 0, GPS_ERR_ARG, "num_heads must be positive");
@@ -412,7 +440,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     P->mp = perf_mp();
     P->m = a->perf_features;
   }
-  GPS_REQUIRE(a->local_type != GPS_LOCAL_NONE || P->attn || P->perf, GPS_ERR_ARG,
+  GPS_REQUIRE(a->local_type != GPS_LOCAL_NONE || P->attn || P->perf || P->bb, GPS_ERR_ARG,
               "GPSLayer needs a local model or a global model");
   GPS_REQUIRE(a->norm_type == GPS_NORM_BATCH || a->norm_type == GPS_NORM_NONE, GPS_ERR_UNSUPPORTED,
               "norm_type %d is not built (GPS_NORM_BATCH = 0, GPS_NORM_NONE = 1)", a->norm_type);
@@ -502,6 +530,16 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     P->O = S.alloc<float>(N * P->inner);
     if (!P->nonorm) P->hA = S.alloc<float>(N * d);
   }
+  if (P->bb) {
+    P->O = S.alloc<float>(N * d);
+    P->lse = S.alloc<float>(N * P->H);
+    if (!P->nonorm) P->hA = S.alloc<float>(N * d);
+    P->bb_z1 = S.alloc<float>(N * d);
+    P->bb_a = S.alloc<float>(N * d);
+    P->bb_u = S.alloc<float>(N * d);
+    P->bb_z2 = S.alloc<float>(N * d);
+    P->bb_stat = S.alloc<float>(4 * N);
+  }
   P->s = S.alloc<float>(N * d);
   P->hid = S.alloc<float>(N * 2 * d);
   if (gelu) P->hid_pre = S.alloc<float>(N * 2 * d);
@@ -524,7 +562,11 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
       P->e_p = caller_planes(a->e_planes_in, d, a->precision);
       if (!P->e_p.hi) P->e_p = mkplanes(S, E, d);
     }
-    if (P->attn || P->perf) P->O_p = mkplanes(S, N, kout);
+    if (P->attn || P->perf || P->bb) P->O_p = mkplanes(S, N, kout);
+    if (P->bb) {
+      P->bb_a_p = mkplanes(S, N, d);
+      P->bb_u_p = mkplanes(S, N, d);
+    }
     // Forward softmax attention on the tensor cores (attention_tc.cu) when the batch's graphs are large enough for
     // 128 x 128 tiles to pay: at the PCQM4M shape (mean 14 nodes per graph) a 128-row tile sees ~45 useful keys of 256
     // in one latency-bound wave and the CUDA-core kernel is faster; the tensor-core kernel wins once a graph fills a
@@ -571,7 +613,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   if (P->pna) P->pna_q = F.alloc<float>(E * d);
   if (P->nonorm && loc) {
     // x_loc is an operand of the GEMM that writes s (and of nothing in the backward pass); a lone local model writes s
-    P->xloc = (P->attn || P->perf) ? F.alloc<float>(N * d) : P->s;
+    P->xloc = (P->attn || P->perf || P->bb) ? F.alloc<float>(N * d) : P->s;
   }
   P->fwd_bytes = F.used;
 
@@ -605,6 +647,18 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     P->g_pgrow = Bk.alloc<float>(NH);
     P->g_pden = Bk.alloc<float>(NH);
     P->g_xp = Bk.alloc<float>(N * d);
+  }
+  if (P->bb) {
+    if (!P->nonorm) P->g_hA = Bk.alloc<float>(N * d);
+    P->g_O = Bk.alloc<float>(N * d);
+    P->delta = Bk.alloc<float>(N * P->H);
+    P->bb_god = Bk.alloc<float>(N * d);
+    P->bb_dz2 = Bk.alloc<float>(N * d);
+    P->bb_gu = Bk.alloc<float>(N * d);
+    P->bb_ga = Bk.alloc<float>(N * d);
+    P->bb_gso = Bk.alloc<float>(N * d);
+    P->bb_gx = Bk.alloc<float>(N * d);
+    P->bb_part = Bk.alloc<float>(layernorm_part_floats(d));
   }
   if (P->Wy) {
     P->gY1 = Bk.alloc<float>(N * P->Wy);
@@ -644,7 +698,12 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   if (P->use_planes) {
     P->gt_p = mkplanes(Bk, N, d);
     P->ghid_p = mkplanes(Bk, N, 2 * d);
-    if ((P->attn || P->perf) && !P->nonorm) P->ghA_p = mkplanes(Bk, N, d);
+    if ((P->attn || P->perf || P->bb) && !P->nonorm) P->ghA_p = mkplanes(Bk, N, d);
+    if (P->bb) {
+      P->bb_god_p = mkplanes(Bk, N, d);
+      P->bb_gu_p = mkplanes(Bk, N, d);
+      P->bb_gso_p = mkplanes(Bk, N, d);
+    }
     if (P->nonorm) P->gs_p = mkplanes(Bk, N, d);
     if (P->gated) P->ge_p = mkplanes(Bk, E, d);
     if (P->Wy) P->gY1_p = mkplanes(Bk, N, P->Wy);
@@ -795,6 +854,18 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
     GPS_REQUIRE(a->perf_proj, GPS_ERR_ARG, "missing buffer self_attn.fast_attention.projection_matrix");
     if (bn) GPS_TRY(check_bn(a->norm1_attn, "norm1_attn"));
   }
+  if (P.bb) {
+    const GpsBigBird& b = *P.bbp;
+    GPS_TRY(check_linear(b.query, "self_attn.encoder.layers.0.attention.self.query", false));
+    GPS_TRY(check_linear(b.key, "self_attn.encoder.layers.0.attention.self.key", false));
+    GPS_TRY(check_linear(b.value, "self_attn.encoder.layers.0.attention.self.value", false));
+    GPS_TRY(check_linear(b.self_out, "self_attn.encoder.layers.0.attention.output.dense", true));
+    GPS_TRY(check_linear(b.ln1, "self_attn.encoder.layers.0.attention.output.LayerNorm", true));
+    GPS_TRY(check_linear(b.intermediate, "self_attn.encoder.layers.0.intermediate.dense", true));
+    GPS_TRY(check_linear(b.output, "self_attn.encoder.layers.0.output.dense", true));
+    GPS_TRY(check_linear(b.ln2, "self_attn.encoder.layers.0.output.LayerNorm", true));
+    if (bn) GPS_TRY(check_bn(a->norm1_attn, "norm1_attn"));
+  }
   GPS_TRY(check_linear(a->ff1, "ff_linear1", true));
   GPS_TRY(check_linear(a->ff2, "ff_linear2", true));
   if (bn) GPS_TRY(check_bn(a->norm2, "norm2"));
@@ -918,9 +989,9 @@ static int check_bias(const GpsLayerArgs* a, const GpsAttnBias* bias) {
 
 // =================================================================================== forward
 static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, const GpsGenConv* gen,
-                         const GpsPna* pna, cudaStream_t st) {
+                         const GpsPna* pna, cudaStream_t st, const GpsBigBird* bb = nullptr) {
   Plan P;
-  GPS_TRY(make_plan(a, &P, true, gat, gen, pna));
+  GPS_TRY(make_plan(a, &P, true, gat, gen, pna, bb));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
   GPS_REQUIRE(a->workspace_bytes >= P.fwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.fwd_bytes);
@@ -938,10 +1009,10 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
   Side* sd;
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
-  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) && (P.attn || P.perf);
+  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) && (P.attn || P.perf || P.bb);
   // GPS_NORM_NONE: the producer that closes the last branch writes s = x_loc + hA with its planes (x_loc = s when the
   // local model is alone)
-  const bool local_writes_s = P.nonorm && !(P.attn || P.perf);
+  const bool local_writes_s = P.nonorm && !(P.attn || P.perf || P.bb);
   // GPS_NORM_NONE, attention output projection on stream sg: writes s = x + drop(.) [+ x_loc] and its planes instead of
   // hA; with a local branch, sg first waits for it
   auto close_with_s = [&](GemmParams& g, cudaStream_t sg) -> int {
@@ -1146,6 +1217,54 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
     GPS_TRY(gemm(g, sg));
   }
 
+  // ---- BigBird global model (gps_layer.py:207-208; bigbird_layer.py:1116-1356)
+  if (P.bb) {
+    const GpsBigBird& B = *bb;
+    const float* Q = P.Y1 + P.qkv_off;
+    GPS_TRY(bb_attn_fwd(a->graph, P.H, P.hd, B, Q, Q + d, Q + 2 * d, P.Wy, P.O, d, P.lse, sg));
+    if (P.O_p.hi && N > 0) {
+      ToPlanesItem it{P.O, d, (int)N, (int)d, P.O_p};
+      GPS_TRY(to_planes(&it, 1, sg));
+    }
+    // z1 = drop(ctx Wso^T + bso) + x   (BigBirdSelfOutput)
+    GemmParams g = linear_fwd(P, N, d, d, {P.O, d, P.O_p}, {B.self_out.weight, d, P.bb_so_p}, P.bb_z1, d,
+                              B.self_out.bias);
+    g.R1 = a->x; g.ldr1 = (int)d;
+    set_dropout(g, P.drop(GPS_SITE_BB_SELF_OUT));
+    GPS_TRY(gemm(g, sg));
+    float* stat = P.bb_stat;
+    GPS_TRY(layernorm_fwd(P.bb_z1, N, d, B.ln1.weight, B.ln1.bias, B.ln_eps, stat, stat + N, P.bb_a, P.bb_a_p, nullptr,
+                          nullptr, DropCfg(), nullptr, sg));
+    // u = act(a Wi^T + bi)   (BigBirdIntermediate)
+    const bool relu = B.hidden_act == GPS_BIGBIRD_RELU;
+    GemmParams g2 = linear_fwd(P, N, d, d, {P.bb_a, d, P.bb_a_p}, {B.intermediate.weight, d, P.bb_in_p}, P.bb_u, d,
+                               B.intermediate.bias);
+    if (relu) {
+      g2.act = GPS_ACT_RELU; g2.Cp = P.bb_u_p;
+    }
+    GPS_TRY(gemm(g2, sg));
+    if (!relu) GPS_TRY(sigmoid_fwd(P.bb_u, N, d, P.bb_u_p, sg));
+    // z2 = drop(u Wo^T + bo) + a   (BigBirdOutput)
+    GemmParams g3 = linear_fwd(P, N, d, d, {P.bb_u, d, P.bb_u_p}, {B.output.weight, d, P.bb_out_p}, P.bb_z2, d,
+                               B.output.bias);
+    g3.R1 = P.bb_a; g3.ldr1 = (int)d;
+    set_dropout(g3, P.drop(GPS_SITE_BB_OUTPUT));
+    GPS_TRY(gemm(g3, sg));
+    // hA = x + drop(LN2(z2)) with norm1_attn's column sums; GPS_NORM_NONE: s = x + drop(LN2(z2)) [+ x_loc] with planes
+    float* dst = P.hA;
+    Planes dstp;
+    const float* r2 = nullptr;
+    if (P.nonorm) {
+      dst = P.s; dstp = P.s_p;
+      if (two_branches) {
+        r2 = P.xloc;
+        GPS_TRY(sd->order(st, sg));
+      }
+    }
+    GPS_TRY(layernorm_fwd(P.bb_z2, N, d, B.ln2.weight, B.ln2.bias, B.ln_eps, stat + 2 * N, stat + 3 * N, dst, dstp, a->x,
+                          r2, P.drop(GPS_SITE_ATTN_OUT), stats(BN_A), sg));
+  }
+
   if (two_branches) GPS_TRY(sd->order(sd->s3, st));
 
   // ---- s = norm1_local(x_loc) + norm1_attn(hA)   (gps_layer.py:194,217,222)
@@ -1153,7 +1272,7 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
     const bool loc = P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna;
     const float* first = loc ? P.xloc : P.hA;
     BnView bf = loc ? bn_view(P, BN_L, a->norm1_local, N) : bn_view(P, BN_A, a->norm1_attn, N);
-    const float* second = (loc && (P.attn || P.perf)) ? P.hA : nullptr;
+    const float* second = (loc && (P.attn || P.perf || P.bb)) ? P.hA : nullptr;
     BnView bs = bn_view(P, BN_A, a->norm1_attn, N);
     GPS_TRY(bn_combine(first, bf, second, bs, P.s, N, d, st, P.s_p));
   }
@@ -1182,9 +1301,9 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
 
 // =================================================================================== backward
 static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, const GpsGenConv* gen,
-                          const GpsPna* pna, cudaStream_t st) {
+                          const GpsPna* pna, cudaStream_t st, const GpsBigBird* bb = nullptr) {
   Plan P;
-  GPS_TRY(make_plan(a, &P, true, gat, gen, pna));
+  GPS_TRY(make_plan(a, &P, true, gat, gen, pna, bb));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
   GPS_REQUIRE(a->workspace_bytes >= P.bwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.bwd_bytes);
@@ -1204,7 +1323,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
   auto wfork = [&](cudaStream_t from) -> int { return sd->order(from, s2); };
-  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) && (P.attn || P.perf);
+  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) && (P.attn || P.perf || P.bb);
   cudaStream_t sa = two_branches ? sd->s3 : st;   // stream of the attention-branch backward
   cudaStream_t se = sd->s4;                       // stream of the edge BatchNorm backward (GatedGCN)
   const int opt = opt_flags();
@@ -1293,7 +1412,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
         g2.bnred[0].z = P.xloc; g2.bnred[0].ldz = (int)d; g2.bnred[0].mean = v.mean; g2.bnred[0].invstd = v.invstd;
         g2.bnred[0].sums = sums(BN_L);
       }
-      if (P.attn || P.perf) {
+      if (P.attn || P.perf || P.bb) {
         BnView v = bn_view(P, BN_A, a->norm1_attn);
         g2.bnred[1].z = P.hA; g2.bnred[1].ldz = (int)d; g2.bnred[1].mean = v.mean; g2.bnred[1].invstd = v.invstd;
         g2.bnred[1].sums = sums(BN_A);
@@ -1317,7 +1436,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
       GPS_TRY(bn_bwd_apply(P.g_s, d, P.xloc, d, N, d, v, -1, nodrop, sums(BN_L), P.g_xloc, d,
                            a->norm1_local.grad_weight, a->norm1_local.grad_bias, st, P.grads_accumulate, P.gl1_p));
   }
-  if (!P.attn && !P.perf) {   // no global model: the early group ends with norm1_local's gradients (stream st)
+  if (!P.attn && !P.perf && !P.bb) {   // no global model: the early group ends with norm1_local's gradients (stream st)
     GPS_TRY(wfork(st));
     GPS_TRY(early_done());
   }
@@ -1384,6 +1503,59 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
       GemmParams h = linear_dgrad(P, N, d, inner, {gsrc[i], inner}, {lin[i]->weight, d}, P.g_xp, d);
       h.R1 = i == 0 ? g_hA : P.g_xp; h.ldr1 = (int)d;
       GPS_TRY(gemm(h, sa));
+    }
+  }
+
+  if (P.bb) {
+    const GpsBigBird& B = *bb;
+    if (!P.nonorm) {
+      BnView v = bn_view(P, BN_A, a->norm1_attn);
+      if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
+      GPS_TRY(bn_bwd_apply(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), P.g_hA, d, a->norm1_attn.grad_weight,
+                           a->norm1_attn.grad_bias, sa, P.grads_accumulate));
+    }
+    GPS_TRY(wfork(sa));
+    GPS_TRY(early_done());
+    const float* stat = P.bb_stat;
+    // LN2 from g' = drop(g_hA): dz2 (the residual path into a) and g_od = drop(dz2), the gradient of output.dense
+    GPS_TRY(layernorm_bwd(g_hA, P.drop(GPS_SITE_ATTN_OUT), P.bb_z2, N, d, B.ln2.weight, stat + 2 * N, stat + 3 * N,
+                          P.bb_god, P.bb_god_p, P.drop(GPS_SITE_BB_OUTPUT), P.bb_dz2, nullptr, P.bb_part,
+                          B.ln2.grad_weight, B.ln2.grad_bias, P.grads_accumulate, sa));
+    // output.dense: g_u = (g_od Wo) * act'(u)
+    const bool relu = B.hidden_act == GPS_BIGBIRD_RELU;
+    const Operand g_od{P.bb_god, d, P.bb_god_p}, g_u{P.bb_gu, d, P.bb_gu_p};
+    GemmParams g = linear_dgrad(P, N, d, d, g_od, {B.output.weight, d, P.bb_out_p}, P.bb_gu, d);
+    if (relu) {
+      set_act_mask(g, GPS_ACT_RELU, P.bb_u, nullptr, d);
+      g.Cp = P.bb_gu_p;
+    }
+    GPS_TRY(gemm(g, sa));
+    if (!relu) GPS_TRY(sigmoid_bwd(P.bb_gu, P.bb_u, N, d, P.bb_gu_p, sa));
+    GPS_TRY(wfork(sa));
+    GPS_TRY(linear_wgrad(P, g_od, {P.bb_u, d, P.bb_u_p}, N, d, d, B.output.grad_weight, B.output.grad_bias, s2));
+    GPS_TRY(linear_wgrad(P, g_u, {P.bb_a, d, P.bb_a_p}, N, d, d, B.intermediate.grad_weight, B.intermediate.grad_bias,
+                         s2));
+    // intermediate.dense: g_a = g_u Wi + dz2
+    GemmParams g2 = linear_dgrad(P, N, d, d, g_u, {B.intermediate.weight, d, P.bb_in_p}, P.bb_ga, d);
+    g2.R1 = P.bb_dz2; g2.ldr1 = (int)d;
+    GPS_TRY(gemm(g2, sa));
+    // LN1: g_so = drop(dz1), the gradient of attention.output.dense; dz1 + g_hA is BigBird's share of grad_x
+    GPS_TRY(layernorm_bwd(P.bb_ga, nodrop, P.bb_z1, N, d, B.ln1.weight, stat, stat + N, P.bb_gso, P.bb_gso_p,
+                          P.drop(GPS_SITE_BB_SELF_OUT), P.bb_gx, g_hA, P.bb_part, B.ln1.grad_weight, B.ln1.grad_bias,
+                          P.grads_accumulate, sa));
+    const Operand g_so{P.bb_gso, d, P.bb_gso_p};
+    GPS_TRY(gemm(linear_dgrad(P, N, d, d, g_so, {B.self_out.weight, d, P.bb_so_p}, P.g_O, d), sa));
+    GPS_TRY(wfork(sa));   // the LayerNorm gradients are final here too
+    GPS_TRY(linear_wgrad(P, g_so, {P.O, d, P.O_p}, N, d, d, B.self_out.grad_weight, B.self_out.grad_bias, s2));
+    if (!(P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna)) GPS_TRY(mid_done());
+    // block-sparse attention: dQ | dK | dV into the in_proj columns of gY1
+    const float* Q = P.Y1 + P.qkv_off;
+    float* gQ = P.gY1 + P.qkv_off;
+    GPS_TRY(bb_attn_bwd(a->graph, P.H, P.hd, B, Q, Q + d, Q + 2 * d, P.Wy, P.O, P.g_O, d, P.lse, P.delta, gQ, gQ + d,
+                        gQ + 2 * d, P.Wy, sa));
+    if (P.gY1_p.hi && N > 0) {
+      ToPlanesItem it{gQ, P.Wy, (int)N, (int)(3 * d), P.gY1_p.cols(P.qkv_off)};
+      GPS_TRY(to_planes(&it, 1, sa));
     }
   }
 
@@ -1536,7 +1708,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     GPS_LAUNCH_CHECK();
     GemmParams g = linear_dgrad(P, N, d, P.Wy, gY1, {P.Wcat, d, P.Wcat_p}, a->grad_x, d);
     g.R1 = g_x_local; g.ldr1 = (int)d;
-    g.R2 = P.attn ? g_hA : (P.perf ? P.g_xp : nullptr); g.ldr2 = (int)d;
+    g.R2 = P.attn ? g_hA : (P.perf ? P.g_xp : (P.bb ? P.bb_gx : nullptr)); g.ldr2 = (int)d;
     if (gx_splitk) g.splitk = 4;   // long reduction, few output tiles: split-K fills the machine (grad_x zeroed above)
     GPS_TRY(gemm(g, st));
   } else if (g_x_local) {
@@ -1685,6 +1857,78 @@ extern "C" int gps_layer_backward_pna(const GpsLayerArgs* args, const GpsPna* pn
   GPS_TRY(check_pna(args, pna, "gps_layer_backward_pna"));
   GPS_TRY(check_bias(args, bias));
   return layer_backward(args, bias, nullptr, nullptr, pna, (cudaStream_t)stream);
+}
+
+static int check_bigbird(const GpsLayerArgs* a, const GpsBigBird* bb, const GpsGat* gat, const GpsGenConv* gen,
+                         const GpsPna* pna, const char* what) {
+  GPS_REQUIRE(a && bb, GPS_ERR_ARG, "%s: null args / bb", what);
+  GPS_REQUIRE(a->global_type == GPS_GLOBAL_BIGBIRD, GPS_ERR_ARG,
+              "%s: a GpsBigBird needs global_type GPS_GLOBAL_BIGBIRD (got %d)", what, a->global_type);
+  GPS_TRY(bb_check(a->d, a->heads, bb));
+  GPS_REQUIRE((a->local_type == GPS_LOCAL_GAT) == (gat != nullptr) &&
+                  (a->local_type == GPS_LOCAL_GENCONV) == (gen != nullptr) &&
+                  (a->local_type == GPS_LOCAL_PNA) == (pna != nullptr),
+              GPS_ERR_ARG, "%s: the local model's struct (gat / gen / pna) must match local_type %d", what,
+              a->local_type);
+  return GPS_OK;
+}
+
+extern "C" int gps_layer_forward_bigbird(const GpsLayerArgs* args, const GpsBigBird* bb, const GpsGat* gat,
+                                         const GpsGenConv* gen, const GpsPna* pna, void* stream) {
+  GPS_TRY(check_bigbird(args, bb, gat, gen, pna, "gps_layer_forward_bigbird"));
+  return layer_forward(args, nullptr, gat, gen, pna, (cudaStream_t)stream, bb);
+}
+
+extern "C" int gps_layer_backward_bigbird(const GpsLayerArgs* args, const GpsBigBird* bb, const GpsGat* gat,
+                                          const GpsGenConv* gen, const GpsPna* pna, void* stream) {
+  GPS_TRY(check_bigbird(args, bb, gat, gen, pna, "gps_layer_backward_bigbird"));
+  return layer_backward(args, nullptr, gat, gen, pna, (cudaStream_t)stream, bb);
+}
+
+// ---- stage entry points of the BigBird global model (bigbird.cu)
+static int bb_stage(const GpsGraph* g, int64_t heads, int64_t hd, const GpsBigBird* bb, const char* what) {
+  GPS_REQUIRE(g && bb, GPS_ERR_ARG, "%s: null argument", what);
+  GPS_REQUIRE(hd >= 1 && heads >= 1, GPS_ERR_ARG, "%s: heads and hd must be >= 1", what);
+  return bb_check(heads * hd, heads, bb);
+}
+
+extern "C" int gps_bigbird_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const GpsBigBird* bb,
+                                             const float* Q, const float* K, const float* V, int64_t ld, float* O,
+                                             int64_t ldo, float* lse, void* stream) {
+  GPS_TRY(bb_stage(g, heads, hd, bb, "bigbird_attention_forward"));
+  GPS_REQUIRE(Q && K && V && O && lse, GPS_ERR_ARG, "bigbird_attention_forward: null argument");
+  GPS_REQUIRE(ld >= heads * hd && ldo >= heads * hd, GPS_ERR_ARG, "bigbird_attention_forward: ld / ldo < heads * hd");
+  return bb_attn_fwd(*g, heads, hd, *bb, Q, K, V, ld, O, ldo, lse, (cudaStream_t)stream);
+}
+
+extern "C" int gps_bigbird_attention_backward(const GpsGraph* g, int64_t heads, int64_t hd, const GpsBigBird* bb,
+                                              const float* Q, const float* K, const float* V, int64_t ld,
+                                              const float* O, const float* dO, int64_t ldo, const float* lse,
+                                              float* delta, float* dQ, float* dK, float* dV, int64_t ldg,
+                                              void* stream) {
+  GPS_TRY(bb_stage(g, heads, hd, bb, "bigbird_attention_backward"));
+  GPS_REQUIRE(Q && K && V && O && dO && lse && delta && dQ && dK && dV, GPS_ERR_ARG,
+              "bigbird_attention_backward: null argument");
+  GPS_REQUIRE(ld >= heads * hd && ldo >= heads * hd && ldg >= heads * hd, GPS_ERR_ARG,
+              "bigbird_attention_backward: ld / ldo / ldg < heads * hd");
+  return bb_attn_bwd(*g, heads, hd, *bb, Q, K, V, ld, O, dO, ldo, lse, delta, dQ, dK, dV, ldg, (cudaStream_t)stream);
+}
+
+extern "C" int gps_layernorm_forward(const float* z, int64_t rows, int64_t d, const float* gamma, const float* beta,
+                                     float eps, float* y, float* mean, float* rstd, void* stream) {
+  GPS_REQUIRE(z && gamma && beta && y && mean && rstd && rows >= 0 && eps >= 0.f, GPS_ERR_ARG,
+              "layernorm_forward: null argument, rows < 0 or eps < 0");
+  return layernorm_fwd(z, rows, d, gamma, beta, eps, mean, rstd, y, Planes(), nullptr, nullptr, DropCfg(), nullptr,
+                       (cudaStream_t)stream);
+}
+
+extern "C" int gps_layernorm_backward(const float* g, const float* z, int64_t rows, int64_t d, const float* gamma,
+                                      const float* mean, const float* rstd, float* dz, float* grad_gamma,
+                                      float* grad_beta, void* workspace, int32_t accumulate, void* stream) {
+  GPS_REQUIRE(g && z && gamma && mean && rstd && dz && workspace && rows >= 0, GPS_ERR_ARG,
+              "layernorm_backward: null argument or rows < 0");
+  return layernorm_bwd(g, DropCfg(), z, rows, d, gamma, mean, rstd, nullptr, Planes(), DropCfg(), dz, nullptr,
+                       (float*)workspace, grad_gamma, grad_beta, accumulate != 0, (cudaStream_t)stream);
 }
 
 extern "C" int gps_linear_forward(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias,

@@ -28,7 +28,8 @@ _EARLY_PREFIXES = ("ff_linear1.", "ff_linear2.", "norm2.", "norm1_local.", "norm
                    "self_attn.out_proj.", "self_attn.to_out.")
 _LATE_PREFIXES = ("self_attn.in_proj", "self_attn.to_q.", "self_attn.to_k.", "self_attn.to_v.",
                   "local_model.A.", "local_model.B.", "local_model.D.", "local_model.E.", "local_model.lin.",
-                  "local_model.lin_src.", "local_model.pre_nns.")   # Wcat rows
+                  "local_model.lin_src.", "local_model.pre_nns.",
+                  "self_attn.encoder.layers.0.attention.self.")   # Wcat rows
 EARLY, MID, LATE = 0, 1, 2
 
 

@@ -18,17 +18,18 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from .bigbird import BigBirdConfig, BigBirdParams, device_lists, gps_bigbird, padded_length
 from .graph import graph_of
 
 _SUPPORTED_LOCAL = ("None", "CustomGatedGCN", "GINE", "GCN", "GAT", "GENConv", "PNA")
 # local models that read batch.edge_attr (gps_layer.py:44-90)
 _EDGE_LOCAL = ("CustomGatedGCN", "GINE", "GAT", "GENConv", "PNA")
 _KNOWN_LOCAL = _SUPPORTED_LOCAL + ("GIN",)
-_SUPPORTED_GLOBAL = ("None", "Transformer", "BiasedTransformer", "Performer")
-_KNOWN_GLOBAL = _SUPPORTED_GLOBAL + ("BigBird",)
+_SUPPORTED_GLOBAL = ("None", "Transformer", "BiasedTransformer", "Performer", "BigBird")
+_KNOWN_GLOBAL = _SUPPORTED_GLOBAL
 _MHA_GLOBAL = ("Transformer", "BiasedTransformer")   # torch's MultiheadAttention (gps_layer.py:104-106)
 # the library's global model: BiasedTransformer is the Transformer called with a GpsAttnBias
-_GLOBAL_ABI = dict(_lib.GLOBAL, BiasedTransformer=_lib.GLOBAL["Transformer"])
+_GLOBAL_ABI = dict(_lib.GLOBAL, BiasedTransformer=_lib.GLOBAL["Transformer"], BigBird=_lib.GLOBAL_BIGBIRD)
 _ACT_MODULES = {"relu": nn.ReLU, "gelu": nn.GELU}
 
 _workspaces = {}
@@ -273,7 +274,13 @@ class _GPSLayerFn(torch.autograd.Function):
             args.offset, args.offset_dev = 0, snap.data_ptr()
         stream = torch.cuda.current_stream(dev).cuda_stream
         ctx.nmax = gs.nmax if bias.numel() else 0
-        if gat is not None:
+        ctx.bb = layer.__dict__.pop("_bb_lists", None)
+        if ctx.bb is not None:
+            bbs = layer._bigbird_args(named, None, *ctx.bb)
+            _lib.check(lib.gps_layer_forward_bigbird(C.byref(args), C.byref(bbs), gat and C.byref(gat),
+                                                     gen and C.byref(gen), pna and C.byref(pna), stream),
+                       "gps_layer_forward_bigbird")
+        elif gat is not None:
             ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)) if ctx.nmax else None
             _lib.check(lib.gps_layer_forward_gat(C.byref(args), C.byref(gat), ab, stream), "gps_layer_forward_gat")
         elif gen is not None:
@@ -350,7 +357,15 @@ class _GPSLayerFn(torch.autograd.Function):
         g_bias = None
         if ctx.nmax and ctx.needs_input_grad[5]:
             g_bias = torch.empty_like(bias)
-        if layer.local_gnn_type == "GAT":
+        if ctx.bb is not None:
+            bbs = layer._bigbird_args(named, grads, *ctx.bb)
+            gat = layer._gat_args(named, grads) if layer.local_gnn_type == "GAT" else None
+            gen = layer._genconv_args(named, grads) if layer.local_gnn_type == "GENConv" else None
+            pna = layer._pna_args(named, grads) if layer.local_gnn_type == "PNA" else None
+            _lib.check(lib.gps_layer_backward_bigbird(C.byref(args), C.byref(bbs), gat and C.byref(gat),
+                                                      gen and C.byref(gen), pna and C.byref(pna), stream),
+                       "gps_layer_backward_bigbird")
+        elif layer.local_gnn_type == "GAT":
             gat = layer._gat_args(named, grads)
             ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))) if ctx.nmax else None
             _lib.check(lib.gps_layer_backward_gat(C.byref(args), C.byref(gat), ab, stream), "gps_layer_backward_gat")
@@ -460,6 +475,21 @@ class GPSLayer(nn.Module):
             raise NotImplementedError(f"global model '{global_model_type}' is not built in graphgps_b200")
         if global_model_type == "None":
             self.self_attn = None
+        elif global_model_type == "BigBird":
+            if bigbird_cfg is None:
+                raise NotImplementedError(
+                    "GPSLayer('BigBird') needs bigbird_cfg (cfg.gt.bigbird): the reference writes dim_hidden, n_heads "
+                    "and dropout into it (gps_layer.py:116-118) and fails with AttributeError on None")
+            # the reference's own mutation of the caller's config (gps_layer.py:116-118)
+            bigbird_cfg.dim_hidden = dim_h
+            bigbird_cfg.n_heads = num_heads
+            bigbird_cfg.dropout = dropout
+            bb_cfg = BigBirdConfig(bigbird_cfg)
+            bb_cfg.check()
+            if num_heads < 1 or dim_h % num_heads != 0:
+                raise ValueError(f"BigBird needs dim_h ({dim_h}) divisible by num_heads ({num_heads})")
+            # attn_dropout is accepted and not read, as in the reference (BigBird attention has no dropout)
+            self.self_attn = BigBirdParams(dim_h, num_heads, bb_cfg)
         elif global_model_type in _MHA_GLOBAL:
             if dim_h % num_heads != 0:
                 raise ValueError("embed_dim must be divisible by num_heads")
@@ -677,6 +707,19 @@ class GPSLayer(nn.Module):
                               _lib.ptr(g.get(p + "1.weight")), _lib.ptr(g.get(p + "1.bias"))),
             _lin(named[p + "4.weight"], None, g.get(p + "4.weight")))
 
+    def _bigbird_args(self, named, grads, lists, nb):
+        """GpsBigBird of the BigBird global model (gps_b200.h) for a batch of nb blocks."""
+        return gps_bigbird(self.self_attn, named, grads, "self_attn.", lists, nb)
+
+    def _bigbird_lists(self, x, gs):
+        """(block lists, nb) of this batch: nb from Nmax padded to the block size; NotImplementedError (before any
+        launch) for a batch the reference cannot run."""
+        cfg = self.self_attn.cfg
+        nb = padded_length(gs.nmax, cfg.block_size) // cfg.block_size
+        lists = device_lists(x.device, nb, self.num_heads, cfg.block_size, cfg.num_random_blocks,
+                             cfg.max_position_embeddings)
+        return lists, nb
+
     def _pna_args(self, named, grads=None):
         """GpsPna of the PNA local model (gps_b200.h): edge_encoder, pre_nns.0.0, post_nns.0.0, lin and the edge width."""
         g = grads or {}
@@ -722,6 +765,8 @@ class GPSLayer(nn.Module):
         pe = self._read_pe(batch, x) if self._eslap else None
         gs = graph_of(batch)
         bias = self._read_attn_bias(batch, x, gs) if self.global_model_type == "BiasedTransformer" else None
+        if self.global_model_type == "BigBird":
+            self.__dict__["_bb_lists"] = self._bigbird_lists(x, gs)
         params = [p for _, p in self.named_parameters()]
         e_arg = e if e is not None else x.new_empty(0)
         pe_arg = pe if pe is not None else x.new_empty(0)

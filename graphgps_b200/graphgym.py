@@ -47,6 +47,8 @@ def register(name="gpslayer_b200"):
             kwargs.setdefault("equivstable_pe", bool(pe_cfg.enable) if pe_cfg is not None else False)
             # PNA's in-degree histogram (gt_config.py:34-37; master_loader.py:226-231 fills it for PNA layer types)
             kwargs.setdefault("pna_degrees", getattr(cfg.gt, "pna_degrees", None))
+            # the BigBird global model's configuration (gps_model.py:97)
+            kwargs.setdefault("bigbird_cfg", getattr(cfg.gt, "bigbird", None))
             super().__init__(dim_h=layer_config.dim_out, local_gnn_type=local, global_model_type=glob,
                              num_heads=cfg.gt.n_heads, act=cfg.gnn.act, dropout=cfg.gt.dropout,
                              attn_dropout=cfg.gt.attn_dropout, layer_norm=cfg.gt.layer_norm,

@@ -38,7 +38,8 @@ enum { GPS_OK = 0, GPS_ERR_ARG = -1, GPS_ERR_UNSUPPORTED = -2, GPS_ERR_CUDA = -3
 /* local_gnn_type / global_model_type of GPSLayer.__init__ (gps_layer.py:20-24,44-122) */
 enum { GPS_LOCAL_NONE = 0, GPS_LOCAL_GATEDGCN = 1, GPS_LOCAL_GINE = 2, GPS_LOCAL_GCN = 3, GPS_LOCAL_GAT = 4,
        GPS_LOCAL_GENCONV = 5, GPS_LOCAL_PNA = 6 };
-enum { GPS_GLOBAL_NONE = 0, GPS_GLOBAL_TRANSFORMER = 1, GPS_GLOBAL_PERFORMER = 2 };
+enum { GPS_GLOBAL_NONE = 0, GPS_GLOBAL_TRANSFORMER = 1, GPS_GLOBAL_PERFORMER = 2,
+       GPS_GLOBAL_BIGBIRD = 3 /* gps_layer_{forward,backward}_bigbird only */ };
 /* register.act_dict keys used by shipped configs (gps_layer.py:33) */
 enum { GPS_ACT_RELU = 0, GPS_ACT_GELU = 1 };
 /* arithmetic of the dense products: FP32 = fp32-grade result (split-bf16 x3 on the tensor cores,
@@ -336,6 +337,66 @@ typedef struct {
  * before any CUDA call, as does a NULL edge_attr (E > 0) or, in the backward, grad_edge_attr (E > 0). */
 int gps_layer_forward_pna(const GpsLayerArgs* args, const GpsPna* pna, const GpsAttnBias* bias, void* stream);
 int gps_layer_backward_pna(const GpsLayerArgs* args, const GpsPna* pna, const GpsAttnBias* bias, void* stream);
+
+/* BigBird global model (global_type == GPS_GLOBAL_BIGBIRD): the reference's SingleBigBirdLayer, one BigBirdLayer with
+ * block-sparse self-attention (gps_layer.py:115-119,207-208; bigbird_layer.py:1667-1706).  For graph g of n_g nodes,
+ * local position p is node graph_ptr[g] + p; the batch is padded to S = num_blocks * block_size positions (to_dense_batch's
+ * Nmax rounded up to the block size) and positions >= n_g are masked keys, never queries.  Head h of query block i
+ * attends to the multiset of key blocks key_idx[key_ptr[h*(nb+1) + i] .. key_ptr[h*(nb+1) + i + 1]) (a block listed
+ * twice counts twice in the softmax); query_ptr / query_idx is its transpose (the query blocks of every key block, in
+ * ascending order, with the same multiplicities).  nb = num_blocks >= 4.  Scale 1/sqrt(hd), hd = d / heads (any hd >= 1
+ * up to 128; d % heads != 0 is GPS_ERR_ARG), no attention dropout.  With ctx the attention output [N, d]:
+ *   a   = LN1(drop_8(ctx Wso^T + bso) + x)          (attention.output; dropout site 8 = GPS_SITE_BB_SELF_OUT)
+ *   u   = act(a Wi^T + bi)                           (intermediate; act = hidden_act: 0 relu, 1 sigmoid)
+ *   out = LN2(drop_9(u Wo^T + bo) + a)               (output; dropout site 9 = GPS_SITE_BB_OUTPUT)
+ * LN = nn.LayerNorm(d, eps = ln_eps) over each row; both dropouts use GpsLayerArgs.dropout.  out then takes the place of
+ * the attention output in the GPS layer: hA = x + drop_4(out), norm1_attn, as for the Transformer.  Parameters
+ * (self_attn.encoder.layers.0.*; weights [d, d]): query / key / value = attention.self.{query,key,value} (bias NULL
+ * unless use_bias), self_out = attention.output.dense, ln1 = attention.output.LayerNorm (weight = gamma, bias = beta),
+ * intermediate = intermediate.dense, output = output.dense, ln2 = output.LayerNorm.  Gradients: query / key / value are
+ * final at ev_grads_done (one weight-gradient product with the node projections); the other five at ev_grads_mid. */
+enum { GPS_BIGBIRD_RELU = 0, GPS_BIGBIRD_SIGMOID = 1 };
+typedef struct {
+  int64_t block_size;
+  int64_t num_blocks;          /* nb of the batch: ceil(Nmax / block_size) */
+  int32_t hidden_act;          /* GPS_BIGBIRD_* */
+  float ln_eps;                /* layer_norm_eps */
+  const int32_t* key_ptr;      /* [heads * (nb + 1)], offsets into key_idx */
+  const int32_t* key_idx;
+  const int32_t* query_ptr;    /* [heads * (nb + 1)], offsets into query_idx */
+  const int32_t* query_idx;
+  GpsLinear query, key, value, self_out, ln1, intermediate, output, ln2;
+} GpsBigBird;
+
+/* gps_layer_forward / _backward of a layer with the BigBird global model and any local model (gat / gen / pna: the
+ * local model's struct when local_type needs one, else NULL).  gps_layer_plan sizes BigBird from global_type, N, d and
+ * heads alone.  A NULL bb, global_type != GPS_GLOBAL_BIGBIRD, block_size < 1, num_blocks < 4, a NULL list or weight,
+ * and a local struct that does not match local_type return GPS_ERR_ARG before any CUDA call; so do the plain, _biased,
+ * _gat, _genconv and _pna calls with global_type == GPS_GLOBAL_BIGBIRD. */
+int gps_layer_forward_bigbird(const GpsLayerArgs* args, const GpsBigBird* bb, const GpsGat* gat, const GpsGenConv* gen,
+                              const GpsPna* pna, void* stream);
+int gps_layer_backward_bigbird(const GpsLayerArgs* args, const GpsBigBird* bb, const GpsGat* gat, const GpsGenConv* gen,
+                               const GpsPna* pna, void* stream);
+
+/* BigBird stage entry points.  Q, K, V: [N, heads*hd] slices with row stride ld; O / dO [N, heads*hd] (stride ldo);
+ * lse / delta [N, heads] (per-row log-sum-exp / rowsum(dO * O)); dQ, dK, dV written whole (stride ldg).  Only bb's
+ * geometry and lists are read.  The forward is one warp per (graph, head, query block); the backward a query-major pass
+ * for dQ and a key-major pass over the transposed lists for dK / dV: no atomics, the same bits in every run. */
+int gps_bigbird_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const GpsBigBird* bb, const float* Q,
+                                  const float* K, const float* V, int64_t ld, float* O, int64_t ldo, float* lse,
+                                  void* stream);
+int gps_bigbird_attention_backward(const GpsGraph* g, int64_t heads, int64_t hd, const GpsBigBird* bb, const float* Q,
+                                   const float* K, const float* V, int64_t ld, const float* O, const float* dO,
+                                   int64_t ldo, const float* lse, float* delta, float* dQ, float* dK, float* dV,
+                                   int64_t ldg, void* stream);
+/* Row-wise LayerNorm [rows, d] (d % 4 == 0, d <= 4096): y = (z - mean) * rstd * gamma + beta, mean / rstd [rows] saved.
+ * Backward from g: dz [rows, d], and grad_gamma / grad_beta [d] (each NULL = not needed; written, or added when
+ * accumulate != 0) reduced through per-CTA partials in a fixed order; workspace: 264 * d floats. */
+int gps_layernorm_forward(const float* z, int64_t rows, int64_t d, const float* gamma, const float* beta, float eps,
+                          float* y, float* mean, float* rstd, void* stream);
+int gps_layernorm_backward(const float* g, const float* z, int64_t rows, int64_t d, const float* gamma, const float* mean,
+                           const float* rstd, float* dz, float* grad_gamma, float* grad_beta, void* workspace,
+                           int32_t accumulate, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Stage-level entry points (the same kernels the layer calls; exported so the parity tests can
