@@ -110,6 +110,23 @@ class GpsBigBird(C.Structure):
                 ("ln1", GpsLinear), ("intermediate", GpsLinear), ("output", GpsLinear), ("ln2", GpsLinear)]
 
 
+class GpsGraphormerArgs(C.Structure):
+    """Graphormer layer (graphormer_layer.py): config, dropout stream, graph, tensors, scratch and the six parameters
+    input_norm, attention.in_proj, attention.out_proj, mlp.0, mlp.1, mlp.4."""
+    _fields_ = [("d", C.c_int64), ("heads", C.c_int64), ("training", C.c_int32), ("precision", C.c_int32),
+                ("dropout", C.c_float), ("attn_dropout", C.c_float), ("mlp_dropout", C.c_float), ("flags", C.c_int32),
+                ("seed", C.c_uint64), ("offset", C.c_uint64), ("offset_dev", _fp),
+                ("graph", GpsGraph),
+                ("x", _fp), ("x_out", _fp), ("grad_x_out", _fp), ("grad_x", _fp),
+                ("saved", _fp), ("saved_bytes", C.c_int64), ("workspace", _fp), ("workspace_bytes", C.c_int64),
+                ("input_norm", GpsLinear), ("attn_in", GpsLinear), ("attn_out", GpsLinear), ("mlp_norm", GpsLinear),
+                ("mlp_lin1", GpsLinear), ("mlp_lin2", GpsLinear)]
+
+
+class GpsGraphormerPlan(C.Structure):
+    _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
+
+
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
                 ("bwd_workspace_bytes", C.c_int64), ("fwd_launches", C.c_int64),
@@ -145,6 +162,9 @@ SYMBOLS = {
                                                 _i64, _fp, _i64, _fp, _fp]),
     "gps_bigbird_attention_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, C.POINTER(GpsBigBird), _fp, _fp, _fp,
                                                  _i64, _fp, _fp, _i64, _fp, _fp, _fp, _fp, _fp, _i64, _fp]),
+    "gps_graphormer_plan": (C.c_int, [C.POINTER(GpsGraphormerArgs), C.POINTER(GpsGraphormerPlan)]),
+    "gps_graphormer_forward": (C.c_int, [C.POINTER(GpsGraphormerArgs), C.POINTER(GpsAttnBias), _fp]),
+    "gps_graphormer_backward": (C.c_int, [C.POINTER(GpsGraphormerArgs), C.POINTER(GpsAttnBias), _fp]),
     "gps_layernorm_forward": (C.c_int, [_fp, _i64, _i64, _fp, _fp, _f32, _fp, _fp, _fp, _fp]),
     "gps_layernorm_backward": (C.c_int, [_fp, _fp, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i32, _fp]),
     "gps_linear_forward": (C.c_int, [_fp, _i64, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _fp]),

@@ -8,9 +8,9 @@
 // Mapping (CUDA-core version; the flop share of this stage is <1% of the layer at the PCQM/ZINC
 // shapes, 4*d*sum n_g^2 vs 24*N*d^2 — SURVEY.md 8d): query rows are packed densely into warps
 // regardless of graph boundaries; LPR lanes cooperate on one row, each holding CH float4 chunks
-// of the head dimension, so q/o (fwd) and k/v/dk/dv (bwd) live in registers and a dot product is
-// an LPR-lane shuffle reduction.  Online softmax in fp32; dropout on the probabilities uses the
-// Philox stream (site GPS_SITE_ATTN_P + head).
+// of the head dimension (single floats when the head dim is not a multiple of 4, VW = 1), so q/o (fwd)
+// and k/v/dk/dv (bwd) live in registers and a dot product is an LPR-lane shuffle reduction.
+// Online softmax in fp32; dropout on the probabilities uses the Philox stream (site GPS_SITE_ATTN_P + head).
 // Backward = two passes (query-major for dQ and delta, key-major for dK, dV): no atomics.
 // BIAS (BiasedTransformer, gps_layer.py:202-204): S = (q . k) / sqrt(hd) + bias[g, h, i - gs, j - gs] with the caller's
 // dense [B*H, nmax, nmax] bias.  The query-major backward visits every (query, key, head) once and writes the score
@@ -66,38 +66,66 @@ __device__ __forceinline__ void drop_quad_init(DropQuad& q, float p) {
   q.keep_scale = 1.f / (1.f - p);
 }
 
-// lane-slice helpers: lane `sub` of a row group owns float4 chunks sub, sub+LPR, ... (< nch)
-template <int CH, int LPR>
-__device__ __forceinline__ void load_slice(float4* dst, const float* row, int sub, int nch, bool ok) {
+// Chunks of the head dimension.  VW = 4: float4 chunks, for head dims that are a multiple of 4 with 16-byte aligned rows.
+// VW = 1: one float per chunk, for any other head dim (Graphormer on ZINC has hd = 80 / 8 = 10; an odd hd also leaves
+// each head's columns without 8-byte alignment).  The per-key updates of a float4 chunk are written out per component
+// as before, so the VW = 4 kernels compile to the same instructions.
+template <int VW> struct VecT;
+template <> struct VecT<4> { using T = float4; };
+template <> struct VecT<1> { using T = float; };
+
+template <int VW> __device__ __forceinline__ typename VecT<VW>::T vld(const float* p);
+template <> __device__ __forceinline__ float4 vld<4>(const float* p) { return ld4(p); }
+template <> __device__ __forceinline__ float vld<1>(const float* p) { return *p; }
+template <int VW> __device__ __forceinline__ typename VecT<VW>::T vzero();
+template <> __device__ __forceinline__ float4 vzero<4>() { return f4zero(); }
+template <> __device__ __forceinline__ float vzero<1>() { return 0.f; }
+__device__ __forceinline__ void vst(float* p, float4 v) { st4(p, v); }
+__device__ __forceinline__ void vst(float* p, float v) { *p = v; }
+__device__ __forceinline__ float4 vscale(float4 a, float s) { return f4scale(a, s); }
+__device__ __forceinline__ float vscale(float a, float s) { return a * s; }
+__device__ __forceinline__ float vdot(float4 a, float4 b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }
+__device__ __forceinline__ float vdot(float a, float b) { return a * b; }
+__device__ __forceinline__ void vplanes_store(const Planes& p, int64_t r, int64_t c, float4 v) { planes_store4(p, r, c, v); }
+__device__ __forceinline__ void vplanes_store(const Planes& p, int64_t r, int64_t c, float v) {
+  const __nv_bfloat16 h = __float2bfloat16_rn(v);
+  p.hi[r * p.ld + c] = h;
+  if (p.lo) p.lo[r * p.ld + c] = __float2bfloat16_rn(v - __bfloat162float(h));
+}
+
+// lane-slice helpers: lane `sub` of a row group owns chunks sub, sub+LPR, ... (< nch) of VW floats each
+template <int CH, int LPR, int VW>
+__device__ __forceinline__ void load_slice(typename VecT<VW>::T* dst, const float* row, int sub, int nch, bool ok) {
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
     int ch = sub + c * LPR;
-    dst[c] = (ok && ch < nch) ? ld4(row + ch * 4) : f4zero();
+    dst[c] = (ok && ch < nch) ? vld<VW>(row + ch * VW) : vzero<VW>();
   }
 }
-template <int CH, int LPR>
-__device__ __forceinline__ void store_slice(const float4* src, float* row, int sub, int nch) {
+template <int CH, int LPR, int VW>
+__device__ __forceinline__ void store_slice(const typename VecT<VW>::T* src, float* row, int sub, int nch) {
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
     int ch = sub + c * LPR;
-    if (ch < nch) st4(row + ch * 4, src[c]);
+    if (ch < nch) vst(row + ch * VW, src[c]);
   }
 }
 // the same slice into the bf16 hi/lo planes of the tensor (operand image of the next GEMM), columns col0 ...
-template <int CH, int LPR>
-__device__ __forceinline__ void store_slice_planes(const float4* src, const Planes& p, int64_t r, int64_t col0, int sub, int nch) {
+template <int CH, int LPR, int VW>
+__device__ __forceinline__ void store_slice_planes(const typename VecT<VW>::T* src, const Planes& p, int64_t r, int64_t col0,
+                                                   int sub, int nch) {
   if (!p.hi) return;
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
     int ch = sub + c * LPR;
-    if (ch < nch) planes_store4(p, r, col0 + ch * 4, src[c]);
+    if (ch < nch) vplanes_store(p, r, col0 + ch * VW, src[c]);
   }
 }
-template <int CH>
-__device__ __forceinline__ float dot_slice(const float4* a, const float4* b) {
+template <int CH, typename V>
+__device__ __forceinline__ float dot_slice(const V* a, const V* b) {
   float s = 0.f;
 #pragma unroll
-  for (int c = 0; c < CH; ++c) s += a[c].x * b[c].x + a[c].y * b[c].y + a[c].z * b[c].z + a[c].w * b[c].w;
+  for (int c = 0; c < CH; ++c) s += vdot(a[c], b[c]);
   return s;
 }
 
@@ -127,7 +155,7 @@ struct StagedRows {
   const float* x; int64_t ldx;   // row r of tensor X at x + r * ldx (head offset included)
   const float* y; int64_t ldy;
 };
-template <int RPB>
+template <int RPB, int VW>
 __device__ __forceinline__ StagedRows stage_rows(const AttnArgs& a, const float* X, int64_t ldX, const float* Y, int64_t ldY,
                                                  int h, float* sm) {
   const int64_t hoff = (int64_t)h * a.hd;
@@ -138,13 +166,13 @@ __device__ __forceinline__ StagedRows stage_rows(const AttnArgs& a, const float*
   const int kmin = a.gptr[find_graph(a.gptr, a.B, r0)];
   const int R = a.gptr[find_graph(a.gptr, a.B, last) + 1] - kmin;
   if (R > a.smem_rows) return r;                      // block-uniform
-  const int pitch = a.hd + 4, nch = a.hd >> 2;
+  const int pitch = a.hd + 4, nch = VW == 4 ? a.hd >> 2 : a.hd;
   float* sx = sm;
   float* sy = sm + (int64_t)a.smem_rows * pitch;
   for (int idx = threadIdx.x; idx < R * nch; idx += blockDim.x) {
     const int row = idx / nch, c = idx - row * nch;
-    st4(sx + row * pitch + c * 4, ld4(X + (int64_t)(kmin + row) * ldX + hoff + c * 4));
-    st4(sy + row * pitch + c * 4, ld4(Y + (int64_t)(kmin + row) * ldY + hoff + c * 4));
+    vst(sx + row * pitch + c * VW, vld<VW>(X + (int64_t)(kmin + row) * ldX + hoff + c * VW));
+    vst(sy + row * pitch + c * VW, vld<VW>(Y + (int64_t)(kmin + row) * ldY + hoff + c * VW));
   }
   __syncthreads();
   r.x = sx - (int64_t)kmin * pitch; r.ldx = pitch;
@@ -152,16 +180,17 @@ __device__ __forceinline__ StagedRows stage_rows(const AttnArgs& a, const float*
   return r;
 }
 
-template <int CH, int LPR, bool BIAS>
+template <int CH, int LPR, bool BIAS, int VW>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
   extern __shared__ float attn_sm[];
+  using V = typename VecT<VW>::T;
   constexpr int RPW = 32 / LPR;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int sub = lane % LPR, rloc = lane / LPR;
   const int h = blockIdx.y;
   const int i = (blockIdx.x * kWarpsPerBlock + warp) * RPW + rloc;
   const bool row_ok = i < a.N;
-  const int nch = a.hd / 4;
+  const int nch = a.hd / VW;
   const uint64_t offs = eff_offset(a);
   int gs = 0, n = 0;
   const float* brow = nullptr;   // BIAS: bias row of (graph, head, query)
@@ -173,12 +202,12 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
   }
   const int nloop = warp_max_i(n);
   const int64_t hoff = (int64_t)h * a.hd;
-  float4 q[CH], o[CH];
-  load_slice<CH, LPR>(q, a.Q + (int64_t)(row_ok ? i : 0) * a.ld + hoff, sub, nch, row_ok);
+  V q[CH], o[CH];
+  load_slice<CH, LPR, VW>(q, a.Q + (int64_t)(row_ok ? i : 0) * a.ld + hoff, sub, nch, row_ok);
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
-    q[c] = f4scale(q[c], a.scale);
-    o[c] = f4zero();
+    q[c] = vscale(q[c], a.scale);
+    o[c] = vzero<VW>();
   }
   float m = -INFINITY, l = 0.f;
   const bool use_drop = a.p_drop > 0.f;
@@ -186,10 +215,10 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
   drop_quad_init(dq, a.p_drop);
   // software pipeline: the K/V rows of key jl+1 are in flight while key jl is processed (the loop is a chain of
   // load -> dot -> shuffle -> exp -> fma, i.e. latency bound at these tiny graph sizes)
-  const StagedRows kv = stage_rows<RPW * kWarpsPerBlock>(a, a.K, a.ld, a.V, a.ld, h, attn_sm);
-  float4 kc[CH], vc[CH];
-  load_slice<CH, LPR>(kc, kv.x + (int64_t)gs * kv.ldx, sub, nch, n > 0);
-  load_slice<CH, LPR>(vc, kv.y + (int64_t)gs * kv.ldy, sub, nch, n > 0);
+  const StagedRows kv = stage_rows<RPW * kWarpsPerBlock, VW>(a, a.K, a.ld, a.V, a.ld, h, attn_sm);
+  V kc[CH], vc[CH];
+  load_slice<CH, LPR, VW>(kc, kv.x + (int64_t)gs * kv.ldx, sub, nch, n > 0);
+  load_slice<CH, LPR, VW>(vc, kv.y + (int64_t)gs * kv.ldy, sub, nch, n > 0);
   float bc = 0.f;
   if constexpr (BIAS) bc = n > 0 ? brow[0] : 0.f;
   for (int jl = 0; jl < nloop; ++jl) {
@@ -197,9 +226,9 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
     const bool valid = jl < n;
     const bool nvalid = jl + 1 < n;
     const int jn = gs + (nvalid ? jl + 1 : 0);
-    float4 kn[CH], vn[CH];
-    load_slice<CH, LPR>(kn, kv.x + (int64_t)jn * kv.ldx, sub, nch, nvalid);
-    load_slice<CH, LPR>(vn, kv.y + (int64_t)jn * kv.ldy, sub, nch, nvalid);
+    V kn[CH], vn[CH];
+    load_slice<CH, LPR, VW>(kn, kv.x + (int64_t)jn * kv.ldx, sub, nch, nvalid);
+    load_slice<CH, LPR, VW>(vn, kv.y + (int64_t)jn * kv.ldy, sub, nch, nvalid);
     float bn = 0.f;
     if constexpr (BIAS) bn = nvalid ? brow[jl + 1] : 0.f;
     float s = group_sum<LPR>(dot_slice<CH>(q, kc));
@@ -212,10 +241,14 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
     const float pd = use_drop ? p * drop_quad_scale(dq, jl) : p;
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      o[c].x = o[c].x * corr + pd * vc[c].x;
-      o[c].y = o[c].y * corr + pd * vc[c].y;
-      o[c].z = o[c].z * corr + pd * vc[c].z;
-      o[c].w = o[c].w * corr + pd * vc[c].w;
+      if constexpr (VW == 4) {
+        o[c].x = o[c].x * corr + pd * vc[c].x;
+        o[c].y = o[c].y * corr + pd * vc[c].y;
+        o[c].z = o[c].z * corr + pd * vc[c].z;
+        o[c].w = o[c].w * corr + pd * vc[c].w;
+      } else {
+        o[c] = o[c] * corr + pd * vc[c];
+      }
       kc[c] = kn[c];
       vc[c] = vn[c];
     }
@@ -225,27 +258,29 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
   if (row_ok) {
     const float inv = 1.f / l;
 #pragma unroll
-    for (int c = 0; c < CH; ++c) o[c] = f4scale(o[c], inv);
-    store_slice<CH, LPR>(o, a.O + (int64_t)i * a.ldo + hoff, sub, nch);
-    store_slice_planes<CH, LPR>(o, a.Op, i, hoff, sub, nch);
+    for (int c = 0; c < CH; ++c) o[c] = vscale(o[c], inv);
+    store_slice<CH, LPR, VW>(o, a.O + (int64_t)i * a.ldo + hoff, sub, nch);
+    store_slice_planes<CH, LPR, VW>(o, a.Op, i, hoff, sub, nch);
     if (sub == 0) a.lse[(int64_t)i * a.H + h] = m + __logf(l);
   }
 }
 
-// delta_i = dO_i . O_i per (row, head): 8 lanes per pair read consecutive float4 chunks (128 B per group)
+// delta_i = dO_i . O_i per (row, head): 8 lanes per pair read consecutive chunks (float4: 128 B per group)
+template <int VW>
 __global__ void k_attn_delta(AttnArgs a) {
+  using V = typename VecT<VW>::T;
   const int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 3;
   const int sub = threadIdx.x & 7;
   const bool ok = t < (int64_t)a.N * a.H;
   const int64_t i = ok ? t / a.H : 0;
   const int h = ok ? (int)(t - i * a.H) : 0;
-  const float4* go = reinterpret_cast<const float4*>(a.dO + i * a.ldo + (int64_t)h * a.hd);
-  const float4* oo = reinterpret_cast<const float4*>(a.Oc + i * a.ldo + (int64_t)h * a.hd);
+  const V* go = reinterpret_cast<const V*>(a.dO + i * a.ldo + (int64_t)h * a.hd);
+  const V* oo = reinterpret_cast<const V*>(a.Oc + i * a.ldo + (int64_t)h * a.hd);
   float acc = 0.f;
   if (ok)
-    for (int c = sub; c < a.hd / 4; c += 8) {
-      const float4 x = __ldg(go + c), y = __ldg(oo + c);
-      acc += x.x * y.x + x.y * y.y + x.z * y.z + x.w * y.w;
+    for (int c = sub; c < a.hd / VW; c += 8) {
+      const V x = __ldg(go + c), y = __ldg(oo + c);
+      acc += vdot(x, y);
     }
   acc += __shfl_xor_sync(0xffffffffu, acc, 4);
   acc += __shfl_xor_sync(0xffffffffu, acc, 2);
@@ -254,15 +289,16 @@ __global__ void k_attn_delta(AttnArgs a) {
 }
 
 // query-major backward: dQ_i (delta precomputed by k_attn_delta); BIAS: grad_bias[g, h, i - gs, jl] = ds
-template <int CH, int LPR, bool BIAS>
+template <int CH, int LPR, bool BIAS, int VW>
 __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_sm) {
+  using V = typename VecT<VW>::T;
   constexpr int RPW = 32 / LPR;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int sub = lane % LPR, rloc = lane / LPR;
   const int h = blockIdx.y;
   const int i = (blockIdx.x * kWarpsPerBlock + warp) * RPW + rloc;
   const bool row_ok = i < a.N;
-  const int nch = a.hd / 4;
+  const int nch = a.hd / VW;
   const uint64_t offs = eff_offset(a);
   int gs = 0, n = 0;
   int64_t brow = 0;   // BIAS: offset of the (graph, head, query) row in bias / grad_bias
@@ -275,23 +311,23 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
   const int nloop = warp_max_i(n);
   const int64_t hoff = (int64_t)h * a.hd;
   const int ir = row_ok ? i : 0;
-  float4 q[CH], go[CH], gq[CH];
-  load_slice<CH, LPR>(q, a.Q + (int64_t)ir * a.ld + hoff, sub, nch, row_ok);
-  load_slice<CH, LPR>(go, a.dO + (int64_t)ir * a.ldo + hoff, sub, nch, row_ok);
+  V q[CH], go[CH], gq[CH];
+  load_slice<CH, LPR, VW>(q, a.Q + (int64_t)ir * a.ld + hoff, sub, nch, row_ok);
+  load_slice<CH, LPR, VW>(go, a.dO + (int64_t)ir * a.ldo + hoff, sub, nch, row_ok);
   {
     const float dl = row_ok ? a.deltac[(int64_t)i * a.H + h] : 0.f;
 #pragma unroll
-    for (int c = 0; c < CH; ++c) gq[c] = f4zero();
+    for (int c = 0; c < CH; ++c) gq[c] = vzero<VW>();
     const float lse = row_ok ? a.lsec[(int64_t)i * a.H + h] : 0.f;
 #pragma unroll
-    for (int c = 0; c < CH; ++c) q[c] = f4scale(q[c], a.scale);
+    for (int c = 0; c < CH; ++c) q[c] = vscale(q[c], a.scale);
     const bool use_drop = a.p_drop > 0.f;
     DropQuad dq;
     drop_quad_init(dq, a.p_drop);
-    const StagedRows kv = stage_rows<RPW * kWarpsPerBlock>(a, a.K, a.ld, a.V, a.ld, h, attn_sm);
-    float4 kk[CH], vv[CH];
-    load_slice<CH, LPR>(kk, kv.x + (int64_t)gs * kv.ldx, sub, nch, n > 0);
-    load_slice<CH, LPR>(vv, kv.y + (int64_t)gs * kv.ldy, sub, nch, n > 0);
+    const StagedRows kv = stage_rows<RPW * kWarpsPerBlock, VW>(a, a.K, a.ld, a.V, a.ld, h, attn_sm);
+    V kk[CH], vv[CH];
+    load_slice<CH, LPR, VW>(kk, kv.x + (int64_t)gs * kv.ldx, sub, nch, n > 0);
+    load_slice<CH, LPR, VW>(vv, kv.y + (int64_t)gs * kv.ldy, sub, nch, n > 0);
     float bc = 0.f;
     if constexpr (BIAS) bc = n > 0 ? a.bias[brow] : 0.f;
     for (int jl = 0; jl < nloop; ++jl) {
@@ -299,9 +335,9 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
       const bool valid = jl < n;
       const bool nvalid = jl + 1 < n;
       const int jn = gs + (nvalid ? jl + 1 : 0);
-      float4 kn[CH], vn[CH];
-      load_slice<CH, LPR>(kn, kv.x + (int64_t)jn * kv.ldx, sub, nch, nvalid);
-      load_slice<CH, LPR>(vn, kv.y + (int64_t)jn * kv.ldy, sub, nch, nvalid);
+      V kn[CH], vn[CH];
+      load_slice<CH, LPR, VW>(kn, kv.x + (int64_t)jn * kv.ldx, sub, nch, nvalid);
+      load_slice<CH, LPR, VW>(vn, kv.y + (int64_t)jn * kv.ldy, sub, nch, nvalid);
       float bn = 0.f;
       if constexpr (BIAS) bn = nvalid ? a.bias[brow + jl + 1] : 0.f;
       float s = dot_slice<CH>(q, kk), dp = dot_slice<CH>(go, vv);
@@ -319,10 +355,14 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
       }
 #pragma unroll
       for (int c = 0; c < CH; ++c) {
-        gq[c].x += ds * kk[c].x;
-        gq[c].y += ds * kk[c].y;
-        gq[c].z += ds * kk[c].z;
-        gq[c].w += ds * kk[c].w;
+        if constexpr (VW == 4) {
+          gq[c].x += ds * kk[c].x;
+          gq[c].y += ds * kk[c].y;
+          gq[c].z += ds * kk[c].z;
+          gq[c].w += ds * kk[c].w;
+        } else {
+          gq[c] += ds * kk[c];
+        }
         kk[c] = kn[c];
         vv[c] = vn[c];
       }
@@ -330,22 +370,23 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
   }
   if (row_ok) {
 #pragma unroll
-    for (int c = 0; c < CH; ++c) gq[c] = f4scale(gq[c], a.scale);
-    store_slice<CH, LPR>(gq, a.dQ + (int64_t)i * a.ldg + hoff, sub, nch);
-    store_slice_planes<CH, LPR>(gq, a.dQp, i, hoff, sub, nch);
+    for (int c = 0; c < CH; ++c) gq[c] = vscale(gq[c], a.scale);
+    store_slice<CH, LPR, VW>(gq, a.dQ + (int64_t)i * a.ldg + hoff, sub, nch);
+    store_slice_planes<CH, LPR, VW>(gq, a.dQp, i, hoff, sub, nch);
   }
 }
 
 // key-major backward: dK_j, dV_j (BIAS: p recomputed with the bias column of key j)
-template <int CH, int LPR, bool BIAS>
+template <int CH, int LPR, bool BIAS, int VW>
 __device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_sm) {
+  using V = typename VecT<VW>::T;
   constexpr int RPW = 32 / LPR;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int sub = lane % LPR, rloc = lane / LPR;
   const int h = blockIdx.y;
   const int j = (blockIdx.x * kWarpsPerBlock + warp) * RPW + rloc;
   const bool row_ok = j < a.N;
-  const int nch = a.hd / 4;
+  const int nch = a.hd / VW;
   const uint64_t offs = eff_offset(a);
   int gs = 0, n = 0;
   const float* bcol = nullptr;   // BIAS: bias column of (graph, head, key); query il at bcol[il * nmax]
@@ -359,26 +400,26 @@ __device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_
   const int jl = j - gs;
   const int64_t hoff = (int64_t)h * a.hd;
   const int jr = row_ok ? j : 0;
-  float4 kk[CH], vv[CH], gk[CH], gv[CH];
-  load_slice<CH, LPR>(kk, a.K + (int64_t)jr * a.ld + hoff, sub, nch, row_ok);
-  load_slice<CH, LPR>(vv, a.V + (int64_t)jr * a.ld + hoff, sub, nch, row_ok);
+  V kk[CH], vv[CH], gk[CH], gv[CH];
+  load_slice<CH, LPR, VW>(kk, a.K + (int64_t)jr * a.ld + hoff, sub, nch, row_ok);
+  load_slice<CH, LPR, VW>(vv, a.V + (int64_t)jr * a.ld + hoff, sub, nch, row_ok);
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
-    gk[c] = f4zero();
-    gv[c] = f4zero();
+    gk[c] = vzero<VW>();
+    gv[c] = vzero<VW>();
   }
-  const StagedRows qd = stage_rows<RPW * kWarpsPerBlock>(a, a.Q, a.ld, a.dO, a.ldo, h, attn_sm);
-  float4 q[CH], go[CH];
-  load_slice<CH, LPR>(q, qd.x + (int64_t)gs * qd.ldx, sub, nch, n > 0);
-  load_slice<CH, LPR>(go, qd.y + (int64_t)gs * qd.ldy, sub, nch, n > 0);
+  const StagedRows qd = stage_rows<RPW * kWarpsPerBlock, VW>(a, a.Q, a.ld, a.dO, a.ldo, h, attn_sm);
+  V q[CH], go[CH];
+  load_slice<CH, LPR, VW>(q, qd.x + (int64_t)gs * qd.ldx, sub, nch, n > 0);
+  load_slice<CH, LPR, VW>(go, qd.y + (int64_t)gs * qd.ldy, sub, nch, n > 0);
   for (int il = 0; il < nloop; ++il) {
     const bool valid = il < n;
     const int i = gs + (valid ? il : 0);
     const bool nvalid = il + 1 < n;
     const int in_ = gs + (nvalid ? il + 1 : 0);
-    float4 qn[CH], gon[CH];
-    load_slice<CH, LPR>(qn, qd.x + (int64_t)in_ * qd.ldx, sub, nch, nvalid);
-    load_slice<CH, LPR>(gon, qd.y + (int64_t)in_ * qd.ldy, sub, nch, nvalid);
+    V qn[CH], gon[CH];
+    load_slice<CH, LPR, VW>(qn, qd.x + (int64_t)in_ * qd.ldx, sub, nch, nvalid);
+    load_slice<CH, LPR, VW>(gon, qd.y + (int64_t)in_ * qd.ldy, sub, nch, nvalid);
     float s = dot_slice<CH>(q, kk), dp = dot_slice<CH>(go, vv);
 #pragma unroll
     for (int ofs = LPR / 2; ofs > 0; ofs >>= 1) {
@@ -401,33 +442,43 @@ __device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_
     const float ds = p * (dp * dsc - dl) * a.scale;
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      gk[c].x += ds * q[c].x; gk[c].y += ds * q[c].y; gk[c].z += ds * q[c].z; gk[c].w += ds * q[c].w;
-      gv[c].x += pd * go[c].x; gv[c].y += pd * go[c].y; gv[c].z += pd * go[c].z; gv[c].w += pd * go[c].w;
+      if constexpr (VW == 4) {
+        gk[c].x += ds * q[c].x; gk[c].y += ds * q[c].y; gk[c].z += ds * q[c].z; gk[c].w += ds * q[c].w;
+        gv[c].x += pd * go[c].x; gv[c].y += pd * go[c].y; gv[c].z += pd * go[c].z; gv[c].w += pd * go[c].w;
+      } else {
+        gk[c] += ds * q[c];
+        gv[c] += pd * go[c];
+      }
       q[c] = qn[c];
       go[c] = gon[c];
     }
   }
   if (row_ok) {
-    store_slice<CH, LPR>(gk, a.dK + (int64_t)j * a.ldg + hoff, sub, nch);
-    store_slice<CH, LPR>(gv, a.dV + (int64_t)j * a.ldg + hoff, sub, nch);
-    store_slice_planes<CH, LPR>(gk, a.dKp, j, hoff, sub, nch);
-    store_slice_planes<CH, LPR>(gv, a.dVp, j, hoff, sub, nch);
+    store_slice<CH, LPR, VW>(gk, a.dK + (int64_t)j * a.ldg + hoff, sub, nch);
+    store_slice<CH, LPR, VW>(gv, a.dV + (int64_t)j * a.ldg + hoff, sub, nch);
+    store_slice_planes<CH, LPR, VW>(gk, a.dKp, j, hoff, sub, nch);
+    store_slice_planes<CH, LPR, VW>(gv, a.dVp, j, hoff, sub, nch);
   }
 }
 
 // both backward passes in one grid (blockIdx.z picks the pass) so they share the SMs instead of queueing
-template <int CH, int LPR, bool BIAS>
+template <int CH, int LPR, bool BIAS, int VW>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_bwd(AttnArgs a) {
   extern __shared__ float attn_sm[];
-  if (blockIdx.z == 0) attn_bwd_kv_body<CH, LPR, BIAS>(a, attn_sm);
-  else attn_bwd_q_body<CH, LPR, BIAS>(a, attn_sm);
+  if (blockIdx.z == 0) attn_bwd_kv_body<CH, LPR, BIAS, VW>(a, attn_sm);
+  else attn_bwd_q_body<CH, LPR, BIAS, VW>(a, attn_sm);
 }
 
 enum { KFWD = 0, KBWD = 1 };
 
 constexpr int kStageBytes = 72 * 1024;   // two staging tiles per block; 3 blocks per SM still fit
 
-template <int CH, int LPR, bool BIAS>
+// whether the float4 kernels take these head dim and leading dimensions (else the VW = 1 kernels run)
+static bool attn_vec4(const AttnArgs& a, int which) {
+  return a.hd % 4 == 0 && a.ld % 4 == 0 && a.ldo % 4 == 0 && (which == KFWD || a.ldg % 4 == 0);
+}
+
+template <int CH, int LPR, bool BIAS, int VW>
 static void launch_one(int which, const AttnArgs& a0, cudaStream_t stream) {
   constexpr int RPW = 32 / LPR;
   AttnArgs a = a0;
@@ -444,37 +495,41 @@ static void launch_one(int which, const AttnArgs& a0, cudaStream_t stream) {
   const size_t smem = a.smem_rows > 0 ? (size_t)2 * a.smem_rows * pitch * 4 : 0;
   static bool attr_done[2] = {false, false};
   if (smem > 0 && !attr_done[which]) {
-    if (which == KFWD) cudaFuncSetAttribute(k_attn_fwd<CH, LPR, BIAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
-    else cudaFuncSetAttribute(k_attn_bwd<CH, LPR, BIAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
+    if (which == KFWD)
+      cudaFuncSetAttribute(k_attn_fwd<CH, LPR, BIAS, VW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
+    else cudaFuncSetAttribute(k_attn_bwd<CH, LPR, BIAS, VW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
     attr_done[which] = true;
   }
   dim3 grid((unsigned)ceil_div(a.N, (int64_t)RPW * kWarpsPerBlock), (unsigned)a.H, which == KFWD ? 1 : 2);
   dim3 block(kWarpsPerBlock * 32);
-  if (which == KFWD) k_attn_fwd<CH, LPR, BIAS><<<grid, block, smem, stream>>>(a);
-  else k_attn_bwd<CH, LPR, BIAS><<<grid, block, smem, stream>>>(a);
+  if (which == KFWD) k_attn_fwd<CH, LPR, BIAS, VW><<<grid, block, smem, stream>>>(a);
+  else k_attn_bwd<CH, LPR, BIAS, VW><<<grid, block, smem, stream>>>(a);
 }
 
 static int dispatch(int which, const AttnArgs& a, cudaStream_t stream) {
-  GPS_REQUIRE(a.hd > 0 && a.hd % 4 == 0, GPS_ERR_UNSUPPORTED, "attention: head dim %d must be a multiple of 4", a.hd);
-  GPS_REQUIRE(a.ld % 4 == 0 && a.ldo % 4 == 0 && (which == KFWD || a.ldg % 4 == 0), GPS_ERR_UNSUPPORTED,
-              "attention: leading dimensions must be multiples of 4");
-  const int nch = a.hd / 4;
-  GPS_REQUIRE(nch <= 48, GPS_ERR_UNSUPPORTED, "attention: head dim %d > 192 not supported", a.hd);
+  GPS_REQUIRE(a.hd > 0 && a.hd <= 192, GPS_ERR_UNSUPPORTED, "attention: head dim %d must be in 1..192", a.hd);
   if (a.N == 0) return GPS_OK;
-  // smallest power-of-two lane group with <= 6 float4 chunks per lane
+  const int vw = attn_vec4(a, which) ? 4 : 1;
+  const int nch = a.hd / vw;
+  // smallest power-of-two lane group with <= 6 chunks per lane
   int lpr = 1;
   while ((nch + lpr - 1) / lpr > 6) lpr *= 2;
   const int ch = (nch + lpr - 1) / lpr;
-#define GPS_ATTN_CASE(CHV, LPRV)                                  \
-  if (ch == CHV && lpr == LPRV) {                                 \
-    if (a.bias) launch_one<CHV, LPRV, true>(which, a, stream);    \
-    else launch_one<CHV, LPRV, false>(which, a, stream);          \
-    GPS_LAUNCH_CHECK();                                           \
-    return GPS_OK;                                                \
+#define GPS_ATTN_CASE(VWV, CHV, LPRV)                                  \
+  if (vw == VWV && ch == CHV && lpr == LPRV) {                         \
+    if (a.bias) launch_one<CHV, LPRV, true, VWV>(which, a, stream);    \
+    else launch_one<CHV, LPRV, false, VWV>(which, a, stream);          \
+    GPS_LAUNCH_CHECK();                                                \
+    return GPS_OK;                                                     \
   }
-  GPS_ATTN_CASE(1, 1) GPS_ATTN_CASE(2, 1) GPS_ATTN_CASE(3, 1) GPS_ATTN_CASE(4, 1) GPS_ATTN_CASE(5, 1)
-  GPS_ATTN_CASE(6, 1) GPS_ATTN_CASE(4, 2) GPS_ATTN_CASE(5, 2) GPS_ATTN_CASE(6, 2) GPS_ATTN_CASE(4, 4)
-  GPS_ATTN_CASE(5, 4) GPS_ATTN_CASE(6, 4) GPS_ATTN_CASE(4, 8) GPS_ATTN_CASE(5, 8) GPS_ATTN_CASE(6, 8)
+  GPS_ATTN_CASE(4, 1, 1) GPS_ATTN_CASE(4, 2, 1) GPS_ATTN_CASE(4, 3, 1) GPS_ATTN_CASE(4, 4, 1) GPS_ATTN_CASE(4, 5, 1)
+  GPS_ATTN_CASE(4, 6, 1) GPS_ATTN_CASE(4, 4, 2) GPS_ATTN_CASE(4, 5, 2) GPS_ATTN_CASE(4, 6, 2) GPS_ATTN_CASE(4, 4, 4)
+  GPS_ATTN_CASE(4, 5, 4) GPS_ATTN_CASE(4, 6, 4) GPS_ATTN_CASE(4, 4, 8) GPS_ATTN_CASE(4, 5, 8) GPS_ATTN_CASE(4, 6, 8)
+  GPS_ATTN_CASE(1, 1, 1) GPS_ATTN_CASE(1, 2, 1) GPS_ATTN_CASE(1, 3, 1) GPS_ATTN_CASE(1, 4, 1) GPS_ATTN_CASE(1, 5, 1)
+  GPS_ATTN_CASE(1, 6, 1) GPS_ATTN_CASE(1, 4, 2) GPS_ATTN_CASE(1, 5, 2) GPS_ATTN_CASE(1, 6, 2) GPS_ATTN_CASE(1, 4, 4)
+  GPS_ATTN_CASE(1, 5, 4) GPS_ATTN_CASE(1, 6, 4) GPS_ATTN_CASE(1, 4, 8) GPS_ATTN_CASE(1, 5, 8) GPS_ATTN_CASE(1, 6, 8)
+  GPS_ATTN_CASE(1, 4, 16) GPS_ATTN_CASE(1, 5, 16) GPS_ATTN_CASE(1, 6, 16) GPS_ATTN_CASE(1, 4, 32)
+  GPS_ATTN_CASE(1, 5, 32) GPS_ATTN_CASE(1, 6, 32)
 #undef GPS_ATTN_CASE
   set_error("attention: no kernel for head dim %d", a.hd);
   return GPS_ERR_UNSUPPORTED;
@@ -510,9 +565,11 @@ int attention_bwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, 
   a.scale = 1.f / sqrtf((float)hd); a.p_drop = p_drop; a.seed = seed; a.offset = offset;
   if (a.gbias)   // entries of padded rows / columns stay 0; the kernel writes every in-graph (query, key) pair
     GPS_CUDA(cudaMemsetAsync(a.gbias, 0, (size_t)(g.B * heads * a.nmax * a.nmax) * sizeof(float), stream));
+  GPS_REQUIRE(a.hd > 0 && a.hd <= 192, GPS_ERR_UNSUPPORTED, "attention: head dim %d must be in 1..192", a.hd);
   if (a.N == 0) return GPS_OK;
   const int64_t nt = (int64_t)a.N * a.H * 8;
-  k_attn_delta<<<(unsigned)ceil_div(nt, (int64_t)256), 256, 0, stream>>>(a);
+  if (attn_vec4(a, KBWD)) k_attn_delta<4><<<(unsigned)ceil_div(nt, (int64_t)256), 256, 0, stream>>>(a);
+  else k_attn_delta<1><<<(unsigned)ceil_div(nt, (int64_t)256), 256, 0, stream>>>(a);
   GPS_LAUNCH_CHECK();
   return dispatch(KBWD, a, stream);
 }

@@ -172,6 +172,9 @@ enum {
   GPS_SITE_FF1 = 5, GPS_SITE_FF2 = 6, GPS_SITE_PERF_OUT = 7,
   GPS_SITE_BB_SELF_OUT = 8,   // BigBird attention.output.dropout, on dense(ctx) before LayerNorm 1
   GPS_SITE_BB_OUTPUT = 9,     // BigBird output.dropout, on dense(u) before LayerNorm 2
+  GPS_SITE_GR_ATTN = 10,      // Graphormer layer: dropout on the attention output projection
+  GPS_SITE_GR_MLP = 11,       // Graphormer layer: mlp.3, on GELU(mlp.1(.))
+  GPS_SITE_GR_OUT = 12,       // Graphormer layer: mlp.5, on mlp.4(.)
   GPS_SITE_ATTN_P = 16
 };
 

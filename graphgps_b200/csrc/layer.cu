@@ -16,8 +16,7 @@
 #include <algorithm>
 #include <atomic>
 
-#include "gemm.cuh"
-#include "kernels.cuh"
+#include "layer_ops.cuh"
 
 namespace gps {
 
@@ -99,37 +98,6 @@ int gemm(const GemmParams& p, cudaStream_t stream) {
 
 namespace {
 
-// ------------------------------------------------------------------------------- side stream (fork / join)
-// Independent stages run concurrently with the main chain: the edge projection next to the node projections, the
-// attention branch next to the message-passing branch (gps_layer.py:161-218 computes both from the same h_in1),
-// and every weight-gradient GEMM next to the data-gradient chain.  Fork = event on the caller's stream that the
-// side stream waits on; join = the reverse.  All of it is capturable into a CUDA graph.
-struct Side {
-  cudaStream_t s = nullptr;    // weight gradients / edge projection / forward attention branch
-  cudaStream_t s3 = nullptr;   // backward attention branch (next to the message-passing backward)
-  cudaStream_t s4 = nullptr;   // edge-side BatchNorm backward (depends on grad_edge_out only, so it starts at once)
-  cudaEvent_t ev[32];
-  int next = 0;
-  bool ok = false;
-  int init() {
-    if (ok) return GPS_OK;
-    GPS_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-    GPS_CUDA(cudaStreamCreateWithFlags(&s3, cudaStreamNonBlocking));
-    GPS_CUDA(cudaStreamCreateWithFlags(&s4, cudaStreamNonBlocking));
-    for (int i = 0; i < 32; ++i) GPS_CUDA(cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
-    ok = true;
-    return GPS_OK;
-  }
-  int order(cudaStream_t from, cudaStream_t to) {   // `to` waits for everything enqueued on `from` so far
-    cudaEvent_t e = ev[next++ & 31];
-    GPS_CUDA(cudaEventRecord(e, from));
-    GPS_CUDA(cudaStreamWaitEvent(to, e, 0));
-    return GPS_OK;
-  }
-  int fork(cudaStream_t main) { return order(main, s); }
-  int join(cudaStream_t main) { return order(s, main); }
-};
-
 // Backward-pass fusions, off by default (GPS_B200_OPT bit mask): 32 reduces local_model.bn_node_x inside the
 // norm1_local apply pass, 64 reduces norm1_local / norm1_attn in the epilogue of the GEMM producing g_s.  Each saves a
 // launch, but the fused kernels run as few fat CTAs and delay the branches behind them.
@@ -139,18 +107,6 @@ static int opt_flags() {
     return e ? atoi(e) : 0;
   }();
   return v;
-}
-
-// the side streams of the current device, created on its first use
-static int side_stream(Side** out) {
-  static thread_local Side sides[64];
-  int dev = 0;
-  GPS_CUDA(cudaGetDevice(&dev));
-  GPS_REQUIRE(dev >= 0 && dev < 64, GPS_ERR_ARG, "device index %d out of range: side streams exist for devices 0..63",
-              dev);
-  GPS_TRY(sides[dev].init());
-  *out = &sides[dev];
-  return GPS_OK;
 }
 
 // ------------------------------------------------------------------------------- weight packing
@@ -872,93 +828,6 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
   return GPS_OK;
 }
 
-// ------------------------------------------------------------------------------- dense products
-// An operand: fp32 values with leading dimension ld and, where the layer keeps them, their bf16 planes.
-struct Operand {
-  const float* f;
-  int64_t ld;
-  Planes p;
-};
-
-// y[M,N] = x[M,K] W[N,K]^T (+ bias[N]); the caller adds the rest of the epilogue
-static GemmParams linear_fwd(const Plan& P, int64_t M, int64_t N, int64_t K, Operand x, Operand W, float* y, int64_t ldy,
-                             const float* bias = nullptr) {
-  GemmParams g;
-  g.M = (int)M; g.N = (int)N; g.K = (int)K;
-  g.A = x.f; g.lda = (int)x.ld; g.Ap = x.p;
-  g.B = W.f; g.ldb = (int)W.ld; g.Bp = W.p;
-  g.C = y; g.ldc = (int)ldy;
-  g.bias = bias;
-  g.precision = P.prec;
-  return g;
-}
-
-// g_x[M,N] = g[M,K] W[K,N]: the input gradient of linear_fwd
-static GemmParams linear_dgrad(const Plan& P, int64_t M, int64_t N, int64_t K, Operand g, Operand W, float* gx,
-                               int64_t ldgx) {
-  GemmParams p = linear_fwd(P, M, N, K, g, W, gx, ldgx);
-  p.tb = 1;
-  return p;
-}
-
-static void set_dropout(GemmParams& g, const DropCfg& c) {
-  g.p_drop = c.p; g.seed = c.seed; g.offset = c.offset; g.site = c.site; g.offset_dev = c.offset_dev;
-}
-
-// multiply by act'(pre-activation); ReLU reads the mask off the stored post-activation value instead
-static void set_act_mask(GemmParams& g, int act, const float* post, const float* pre, int64_t ld) {
-  if (act == GPS_ACT_RELU) {
-    g.mask_src = post; g.mask_is_post = 1;
-  } else {
-    g.mask_src = pre; g.mask_act = act;
-  }
-  g.ldmask = (int)ld;
-}
-
-static int splitk_for(int64_t rows, int64_t out, int64_t in) {
-  // Weight gradients reduce over `rows` (nodes/edges) into a small [out, in] tile grid: split the reduction so
-  // that tiles x splits ~ 300 CTAs (two per SM), at least 4 k-blocks of 64 rows per CTA (tools/gemm_tune.py).
-  const int64_t tiles = ceil_div(out, 128) * ceil_div(in, in >= 160 ? 160 : 64);
-  int64_t s = ceil_div(300, tiles > 0 ? tiles : 1);
-  const int64_t max_s = rows / 256;
-  if (s > max_s) s = max_s;
-  if (s < 1) s = 1;
-  if (s > 64) s = 64;
-  return (int)s;
-}
-
-// dW[out,in] += G[rows,out]^T X[rows,in], db[out] += colsum(G), into zeroed dW / db
-static int wgrad_add(const Plan& P, Operand G, Operand X, int64_t rows, int64_t out, int64_t in, float* dW, float* db,
-                     cudaStream_t st) {
-  if (rows == 0) return GPS_OK;
-  GemmParams p;
-  p.M = (int)out; p.N = (int)in; p.K = (int)rows;
-  p.A = G.f; p.lda = (int)G.ld; p.ta = 1; p.Ap = G.p;
-  p.B = X.f; p.ldb = (int)X.ld; p.tb = 1; p.Bp = X.p;
-  p.C = dW; p.ldc = (int)in;
-  p.splitk = std::max(2, splitk_for(rows, out, in));   // the accumulating split-K path also for tiny inputs
-  p.colsum_a = db;
-  p.precision = P.prec;
-  if (P.prec == GPS_PREC_BF16 && G.p.hi && db) {
-    // bf16 mode stores no lo plane: summing ~N bf16-rounded rows would put ~sqrt(N) 2^-9 of noise on a bias gradient
-    // that is often a near-cancelling sum (every Linear here feeds a BatchNorm) -> exact fp32 column sum instead
-    p.colsum_a = nullptr;
-    GPS_TRY(colsum(G.f, G.ld, rows, out, db, st));
-  }
-  return gemm(p, st);
-}
-
-// weight gradient of a Linear into the caller's buffers: dW[out,in] = G[rows,out]^T X[rows,in], db[out] = colsum(G)
-static int linear_wgrad(const Plan& P, Operand G, Operand X, int64_t rows, int64_t out, int64_t in, float* dW, float* db,
-                        cudaStream_t st) {
-  if (!dW) return GPS_OK;
-  if (!P.grads_prezeroed) {
-    GPS_CUDA(cudaMemsetAsync(dW, 0, (size_t)(out * in) * sizeof(float), st));
-    if (db) GPS_CUDA(cudaMemsetAsync(db, 0, (size_t)out * sizeof(float), st));
-  }
-  return wgrad_add(P, G, X, rows, out, in, dW, db, st);
-}
-
 // The [N, d] gradient g in front of the dropout at `site` (and, p2 > 0, of the inner one at site2 before it): g times
 // the dropout scales, written to the temporary tmp (and its planes tmp_p), when a dropout is active, else g itself.
 static int dropmul(const Plan& P, Operand g, float* tmp, Planes tmp_p, int site, cudaStream_t st, Operand* out,
@@ -966,16 +835,31 @@ static int dropmul(const Plan& P, Operand g, float* tmp, Planes tmp_p, int site,
   *out = g;
   if (!(P.dropout.p > 0.f || p2 > 0.f)) return GPS_OK;
   *out = Operand{tmp, P.d, tmp_p};
-  const int64_t n4 = P.N * P.d / 4;
-  if (n4 == 0) return GPS_OK;
-  const DropCfg c = P.drop(site);
-  k_dropmul<<<(unsigned)std::min<int64_t>(ceil_div(n4, 256), kNumSMs * 8), 256, 0, st>>>(
-      g.f, tmp, n4, P.d / 4, c.p, c.seed, c.offset, c.site, c.offset_dev, p2, site2, tmp_p);
-  GPS_LAUNCH_CHECK();
-  return GPS_OK;
+  return dropmul_rows(g.f, tmp, P.N, P.d, P.drop(site), p2, site2, tmp_p, st);
 }
 
 }  // namespace
+
+int side_stream(Side** out) {
+  static thread_local Side sides[64];
+  int dev = 0;
+  GPS_CUDA(cudaGetDevice(&dev));
+  GPS_REQUIRE(dev >= 0 && dev < 64, GPS_ERR_ARG, "device index %d out of range: side streams exist for devices 0..63",
+              dev);
+  GPS_TRY(sides[dev].init());
+  *out = &sides[dev];
+  return GPS_OK;
+}
+
+int dropmul_rows(const float* src, float* dst, int64_t rows, int64_t d, const DropCfg& c, float p2, int site2,
+                 Planes dstp, cudaStream_t st) {
+  const int64_t n4 = rows * d / 4;
+  if (n4 == 0) return GPS_OK;
+  k_dropmul<<<(unsigned)std::min<int64_t>(ceil_div(n4, 256), kNumSMs * 8), 256, 0, st>>>(
+      src, dst, n4, d / 4, c.p, c.seed, c.offset, c.site, c.offset_dev, p2, site2, dstp);
+  GPS_LAUNCH_CHECK();
+  return GPS_OK;
+}
 
 // attention bias of the BiasedTransformer (gps_b200.h GpsAttnBias): checked before any CUDA call
 static int check_bias(const GpsLayerArgs* a, const GpsAttnBias* bias) {

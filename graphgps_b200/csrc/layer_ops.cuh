@@ -1,0 +1,142 @@
+// layer_ops.cuh — host-side building blocks of the layer orchestrations (layer.cu: GPSLayer, graphormer.cu: the
+// Graphormer layer): side streams, the dense products of a Linear and its gradients, and the dropout-only pass.
+// The plan-typed helpers read P.prec (GPS_PREC_*), and linear_wgrad also P.grads_prezeroed.
+#pragma once
+#include <algorithm>
+
+#include "gemm.cuh"
+#include "kernels.cuh"
+
+namespace gps {
+
+// ------------------------------------------------------------------------------- side stream (fork / join)
+// Independent stages run concurrently with the main chain: the edge projection next to the node projections, the
+// attention branch next to the message-passing branch (gps_layer.py:161-218 computes both from the same h_in1),
+// and every weight-gradient GEMM next to the data-gradient chain.  Fork = event on the caller's stream that the
+// side stream waits on; join = the reverse.  All of it is capturable into a CUDA graph.
+struct Side {
+  cudaStream_t s = nullptr;    // weight gradients / edge projection / forward attention branch
+  cudaStream_t s3 = nullptr;   // backward attention branch (next to the message-passing backward)
+  cudaStream_t s4 = nullptr;   // edge-side BatchNorm backward (depends on grad_edge_out only, so it starts at once)
+  cudaEvent_t ev[32];
+  int next = 0;
+  bool ok = false;
+  int init() {
+    if (ok) return GPS_OK;
+    GPS_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    GPS_CUDA(cudaStreamCreateWithFlags(&s3, cudaStreamNonBlocking));
+    GPS_CUDA(cudaStreamCreateWithFlags(&s4, cudaStreamNonBlocking));
+    for (int i = 0; i < 32; ++i) GPS_CUDA(cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
+    ok = true;
+    return GPS_OK;
+  }
+  int order(cudaStream_t from, cudaStream_t to) {   // `to` waits for everything enqueued on `from` so far
+    cudaEvent_t e = ev[next++ & 31];
+    GPS_CUDA(cudaEventRecord(e, from));
+    GPS_CUDA(cudaStreamWaitEvent(to, e, 0));
+    return GPS_OK;
+  }
+  int fork(cudaStream_t main) { return order(main, s); }
+  int join(cudaStream_t main) { return order(s, main); }
+};
+
+// the side streams of the current device, created on its first use (layer.cu)
+int side_stream(Side** out);
+
+// ------------------------------------------------------------------------------- dense products
+// An operand: fp32 values with leading dimension ld and, where the layer keeps them, their bf16 planes.
+struct Operand {
+  const float* f;
+  int64_t ld;
+  Planes p;
+};
+
+// y[M,N] = x[M,K] W[N,K]^T (+ bias[N]); the caller adds the rest of the epilogue
+template <class PlanT>
+inline GemmParams linear_fwd(const PlanT& P, int64_t M, int64_t N, int64_t K, Operand x, Operand W, float* y,
+                             int64_t ldy, const float* bias = nullptr) {
+  GemmParams g;
+  g.M = (int)M; g.N = (int)N; g.K = (int)K;
+  g.A = x.f; g.lda = (int)x.ld; g.Ap = x.p;
+  g.B = W.f; g.ldb = (int)W.ld; g.Bp = W.p;
+  g.C = y; g.ldc = (int)ldy;
+  g.bias = bias;
+  g.precision = P.prec;
+  return g;
+}
+
+// g_x[M,N] = g[M,K] W[K,N]: the input gradient of linear_fwd
+template <class PlanT>
+inline GemmParams linear_dgrad(const PlanT& P, int64_t M, int64_t N, int64_t K, Operand g, Operand W, float* gx,
+                               int64_t ldgx) {
+  GemmParams p = linear_fwd(P, M, N, K, g, W, gx, ldgx);
+  p.tb = 1;
+  return p;
+}
+
+inline void set_dropout(GemmParams& g, const DropCfg& c) {
+  g.p_drop = c.p; g.seed = c.seed; g.offset = c.offset; g.site = c.site; g.offset_dev = c.offset_dev;
+}
+
+// multiply by act'(pre-activation); ReLU reads the mask off the stored post-activation value instead
+inline void set_act_mask(GemmParams& g, int act, const float* post, const float* pre, int64_t ld) {
+  if (act == GPS_ACT_RELU) {
+    g.mask_src = post; g.mask_is_post = 1;
+  } else {
+    g.mask_src = pre; g.mask_act = act;
+  }
+  g.ldmask = (int)ld;
+}
+
+inline int splitk_for(int64_t rows, int64_t out, int64_t in) {
+  // Weight gradients reduce over `rows` (nodes/edges) into a small [out, in] tile grid: split the reduction so
+  // that tiles x splits ~ 300 CTAs (two per SM), at least 4 k-blocks of 64 rows per CTA (tools/gemm_tune.py).
+  const int64_t tiles = ceil_div(out, 128) * ceil_div(in, in >= 160 ? 160 : 64);
+  int64_t s = ceil_div(300, tiles > 0 ? tiles : 1);
+  const int64_t max_s = rows / 256;
+  if (s > max_s) s = max_s;
+  if (s < 1) s = 1;
+  if (s > 64) s = 64;
+  return (int)s;
+}
+
+// dW[out,in] += G[rows,out]^T X[rows,in], db[out] += colsum(G), into zeroed dW / db
+template <class PlanT>
+inline int wgrad_add(const PlanT& P, Operand G, Operand X, int64_t rows, int64_t out, int64_t in, float* dW, float* db,
+                     cudaStream_t st) {
+  if (rows == 0) return GPS_OK;
+  GemmParams p;
+  p.M = (int)out; p.N = (int)in; p.K = (int)rows;
+  p.A = G.f; p.lda = (int)G.ld; p.ta = 1; p.Ap = G.p;
+  p.B = X.f; p.ldb = (int)X.ld; p.tb = 1; p.Bp = X.p;
+  p.C = dW; p.ldc = (int)in;
+  p.splitk = std::max(2, splitk_for(rows, out, in));   // the accumulating split-K path also for tiny inputs
+  p.colsum_a = db;
+  p.precision = P.prec;
+  if (P.prec == GPS_PREC_BF16 && G.p.hi && db) {
+    // bf16 mode stores no lo plane: summing ~N bf16-rounded rows would put ~sqrt(N) 2^-9 of noise on a bias gradient
+    // that is often a near-cancelling sum (every Linear here feeds a BatchNorm) -> exact fp32 column sum instead
+    p.colsum_a = nullptr;
+    GPS_TRY(colsum(G.f, G.ld, rows, out, db, st));
+  }
+  return gemm(p, st);
+}
+
+// weight gradient of a Linear into the caller's buffers: dW[out,in] = G[rows,out]^T X[rows,in], db[out] = colsum(G)
+template <class PlanT>
+inline int linear_wgrad(const PlanT& P, Operand G, Operand X, int64_t rows, int64_t out, int64_t in, float* dW,
+                        float* db, cudaStream_t st) {
+  if (!dW) return GPS_OK;
+  if (!P.grads_prezeroed) {
+    GPS_CUDA(cudaMemsetAsync(dW, 0, (size_t)(out * in) * sizeof(float), st));
+    if (db) GPS_CUDA(cudaMemsetAsync(db, 0, (size_t)out * sizeof(float), st));
+  }
+  return wgrad_add(P, G, X, rows, out, in, dW, db, st);
+}
+
+// dst [rows, d] = src times the dropout scales of c (and, p2 > 0, of the site site2 as well), with dst's planes when
+// dstp.hi is set (layer.cu)
+int dropmul_rows(const float* src, float* dst, int64_t rows, int64_t d, const DropCfg& c, float p2, int site2,
+                 Planes dstp, cudaStream_t st);
+
+}  // namespace gps

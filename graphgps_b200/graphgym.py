@@ -25,6 +25,19 @@ def install(gps_model_module=None):
     return previous
 
 
+def install_graphormer(graphormer_module=None):
+    """Rebind ``GraphormerLayer`` inside ``graphgps.network.graphormer`` so ``GraphormerModel`` builds the H100 layer.
+
+    Call after ``import graphgps`` and before ``create_model()``.  Returns the class it replaced so a caller can restore
+    it."""
+    from .graphormer import GraphormerLayer
+    if graphormer_module is None:
+        graphormer_module = importlib.import_module("graphgps.network.graphormer")
+    previous = getattr(graphormer_module, "GraphormerLayer", None)
+    graphormer_module.GraphormerLayer = GraphormerLayer
+    return previous
+
+
 def register(name="gpslayer_b200"):
     """Register a LayerConfig-style wrapper under ``name`` in GraphGym's layer registry.
 

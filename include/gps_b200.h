@@ -399,6 +399,58 @@ int gps_layernorm_backward(const float* g, const float* z, int64_t rows, int64_t
                            int32_t accumulate, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Graphormer layer (graphgps/layer/graphormer_layer.py:5-49), the building block of GraphormerModel:
+ *   h   = input_norm(x)                                    LayerNorm(d), eps 1e-5
+ *   a   = MHA(h) over each graph's own nodes                scale 1/sqrt(hd), + attn_bias after scaling when given,
+ *                                                           attn_dropout on the probabilities (site 16 + head)
+ *   x1  = x + drop_10(a)                                    dropout, site 10
+ *   out = x1 + drop_12(W2 drop_11(GELU(W1 mlp_norm(x1) + b1)) + b2)
+ *                                                           mlp_dropout at site 11, dropout at site 12
+ * Any head dim hd = d / heads (d % heads != 0 is GPS_ERR_ARG); d % 4 == 0 and d <= 4096, hd <= 192, else
+ * GPS_ERR_UNSUPPORTED.  Parameters (all non-NULL, else GPS_ERR_ARG):
+ *   input_norm = input_norm (weight = gamma, bias = beta), attn_in = attention.in_proj_{weight,bias} [3d, d],
+ *   attn_out = attention.out_proj [d, d], mlp_norm = mlp.0 (gamma / beta), mlp_lin1 = mlp.1, mlp_lin2 = mlp.4 [d, d].
+ * Backward writes grad_x and every non-NULL parameter gradient; the weight products run on a side stream that joins the
+ * caller's stream before the call returns; the LayerNorm gradients are reduced through per-CTA partials in a fixed
+ * order.  No float atomics: two runs give the same bits.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  int64_t d;                 /* embed_dim                                                     */
+  int64_t heads;             /* num_heads                                                     */
+  int32_t training;          /* 1: dropout active                                             */
+  int32_t precision;         /* GPS_PREC_*                                                    */
+  float dropout;             /* after the attention and after the MLP (sites 10, 12)          */
+  float attn_dropout;        /* on the attention probabilities                                */
+  float mlp_dropout;         /* inside the MLP, after GELU (site 11)                          */
+  int32_t flags;             /* backward: bit 0: parameter-gradient buffers are already zero; bit 1: gradients are
+                                added to the buffers (as GpsLayerArgs.reserved0)                */
+  uint64_t seed;             /* Philox key of this call's dropout masks                      */
+  uint64_t offset;           /* Philox counter base                                           */
+  const uint64_t* offset_dev;/* optional device-resident addend to offset (CUDA-graph replays); NULL = none */
+  GpsGraph graph;
+  const float* x;            /* [N, d] batch.x                                                */
+  float* x_out;              /* [N, d] new batch.x (forward)                                  */
+  const float* grad_x_out;   /* [N, d] (backward)                                             */
+  float* grad_x;             /* [N, d] (backward)                                             */
+  void* saved; int64_t saved_bytes;         /* written by forward, read by backward           */
+  void* workspace; int64_t workspace_bytes; /* transient                                      */
+  GpsLinear input_norm, attn_in, attn_out, mlp_norm, mlp_lin1, mlp_lin2;
+} GpsGraphormerArgs;
+
+typedef struct {
+  int64_t saved_bytes;
+  int64_t fwd_workspace_bytes;
+  int64_t bwd_workspace_bytes;
+} GpsGraphormerPlan;
+
+/* Sizes for the configuration and graph of args (only d, heads, precision and graph.N / graph.B are read). */
+int gps_graphormer_plan(const GpsGraphormerArgs* args, GpsGraphormerPlan* plan);
+/* bias: GpsAttnBias (layout as for the BiasedTransformer: [B*heads, nmax, nmax], row g*heads + h), or NULL for none.
+ * The backward writes bias->grad_bias when it is not NULL. */
+int gps_graphormer_forward(const GpsGraphormerArgs* args, const GpsAttnBias* bias, void* stream);
+int gps_graphormer_backward(const GpsGraphormerArgs* args, const GpsAttnBias* bias, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Stage-level entry points (the same kernels the layer calls; exported so the parity tests can
  * pin each stage against the oracle separately).
  * ---------------------------------------------------------------------------------------- */
@@ -566,7 +618,8 @@ int gps_performer_features_backward(const GpsGraph* g, int64_t H, int64_t dim_he
 
 /* Dense softmax attention over each graph's own nodes — replaces to_dense_batch +
  * nn.MultiheadAttention core + [mask] (gps_layer.py:199-201,234-241) without padding.
- * Q,K,V: [N, heads*hd] slices with row stride ld; O [N, heads*hd] (row stride ldo); lse [N,heads]. */
+ * Q,K,V: [N, heads*hd] slices with row stride ld; O [N, heads*hd] (row stride ldo); lse [N,heads].  Any head dim
+ * 1 <= hd <= 192 (else GPS_ERR_UNSUPPORTED); float4 kernels when hd and the leading dimensions are multiples of 4. */
 int gps_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q,
                           const float* K, const float* V, int64_t ld, float* O, int64_t ldo,
                           float* lse, float p_drop, uint64_t seed, uint64_t offset, void* stream);
