@@ -3,6 +3,7 @@
 Public surface (mirrors the reference's module boundary, SURVEY.md section 8b):
     GPSLayer      drop-in for graphgps.layer.gps_layer.GPSLayer
     GraphormerLayer  drop-in for graphgps.layer.graphormer_layer.GraphormerLayer
+    SANLayer      drop-in for graphgps.layer.san_layer.SANLayer
     GraphBatch    duck-typed stand-in for a collated PyG Batch (PyG is optional)
     make_batch    seeded synthetic batches of the BASELINE shapes
     GPSStack      the L-layer stack of a GPSModel (shared graph structure, plane hand-off, one gradient bucket, capture)
@@ -12,9 +13,10 @@ Public surface (mirrors the reference's module boundary, SURVEY.md section 8b):
 from .batch import GraphBatch, SHAPES, make_batch, batch_from_lists  # noqa: F401
 from .gps_layer import GPSLayer  # noqa: F401
 from .graphormer import GraphormerLayer  # noqa: F401
+from .san import SANLayer  # noqa: F401
 from .dp import GradBucket  # noqa: F401
 from .stack import GPSStack  # noqa: F401
 from .loader import BatchPrefetcher, collate  # noqa: F401
 
-__all__ = ["GPSLayer", "GraphormerLayer", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
+__all__ = ["GPSLayer", "GraphormerLayer", "SANLayer", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
            "batch_from_lists"]

@@ -175,6 +175,8 @@ enum {
   GPS_SITE_GR_ATTN = 10,      // Graphormer layer: dropout on the attention output projection
   GPS_SITE_GR_MLP = 11,       // Graphormer layer: mlp.3, on GELU(mlp.1(.))
   GPS_SITE_GR_OUT = 12,       // Graphormer layer: mlp.5, on mlp.4(.)
+  GPS_SITE_SAN_ATTN = 13,     // SAN layer: dropout on the concatenated attention heads, before O_h
+  GPS_SITE_SAN_FFN = 14,      // SAN layer: dropout on relu(FFN_h_layer1(.))
   GPS_SITE_ATTN_P = 16
 };
 

@@ -134,6 +134,40 @@ inline int linear_wgrad(const PlanT& P, Operand G, Operand X, int64_t rows, int6
   return wgrad_add(P, G, X, rows, out, in, dW, db, st);
 }
 
+// A BatchNorm as its consumer kernels see it.  Eval: the running statistics (mode 2); BatchNorm is then a per-column
+// affine map and its backward has no batch terms.  Training backward: the batch statistics the forward pass saved (mode
+// 0).  Training forward, over fwd_rows rows: the consumer kernel finalises the statistics from the producer's column
+// sums, saves them for the backward and updates the running statistics (mode 1).  The statistics slot of a BatchNorm
+// over w columns: saved [mean | invstd] (2w floats) and the forward's column sums (2w doubles).  Reads P.train.
+template <class PlanT>
+inline BnView bn_view_at(const PlanT& P, float* saved, double* fsums, int64_t w, const GpsBatchNorm& bn,
+                         int64_t fwd_rows) {
+  const bool fwd = fwd_rows >= 0;
+  BnView v;
+  v.mean = saved;
+  v.invstd = v.mean + w;
+  v.gamma = bn.weight;
+  v.beta = bn.bias;
+  if (fwd) v.d = w;
+  if (fwd || !P.train) {
+    v.running_mean = bn.running_mean;
+    v.running_var = bn.running_var;
+  }
+  if (!P.train) {
+    v.mode = 2;
+  } else if (fwd) {
+    const int64_t n = fwd_rows;
+    v.mode = 1;
+    v.sums = fsums;
+    v.inv_n = 1.0 / (double)(n > 0 ? n : 1);
+    v.unbias = n > 1 ? (double)n / (double)(n - 1) : 1.0;
+    v.save_mean = saved;
+    v.save_invstd = v.save_mean + w;
+    v.nbt = (long long*)bn.num_batches_tracked;
+  }
+  return v;
+}
+
 // dst [rows, d] = src times the dropout scales of c (and, p2 > 0, of the site site2 as well), with dst's planes when
 // dstp.hi is set (layer.cu)
 int dropmul_rows(const float* src, float* dst, int64_t rows, int64_t d, const DropCfg& c, float p2, int site2,

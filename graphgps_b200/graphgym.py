@@ -38,6 +38,20 @@ def install_graphormer(graphormer_module=None):
     return previous
 
 
+def install_san(san_module=None):
+    """Rebind ``SANLayer`` inside ``graphgps.network.san_transformer`` so ``SANTransformer`` builds the H100 layer.
+    ``SAN2Layer`` (learned gamma, softmax scores) stays the reference's.
+
+    Call after ``import graphgps`` and before ``create_model()``.  Returns the class it replaced so a caller can restore
+    it."""
+    from .san import SANLayer
+    if san_module is None:
+        san_module = importlib.import_module("graphgps.network.san_transformer")
+    previous = getattr(san_module, "SANLayer", None)
+    san_module.SANLayer = SANLayer
+    return previous
+
+
 def register(name="gpslayer_b200"):
     """Register a LayerConfig-style wrapper under ``name`` in GraphGym's layer registry.
 

@@ -451,6 +451,83 @@ int gps_graphormer_forward(const GpsGraphormerArgs* args, const GpsAttnBias* bia
 int gps_graphormer_backward(const GpsGraphormerArgs* args, const GpsAttnBias* bias, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * SAN layer (graphgps/layer/san_layer.py:10-210), the building block of SANTransformer, as every shipped config runs
+ * it (full_graph, batch_norm, residual, no layer_norm, no Linear biases in the attention, in_dim == out_dim == d):
+ *   [Q|K|V|Q2|K2] = x W^T, E = edge_attr W_E^T, E2 = W_E2 fake_edge_emb
+ *   attn = sum over real edges j->i and fake pairs of s V[j] / (sum s + 1e-6), per head of hd = d / heads channels:
+ *     real edge k: s = exp(clamp(sum_c K[j] Q[i] E[k] / sqrt(hd), -5, 5)) / (gamma + 1)   (per edge: duplicates count
+ *                  twice, self loops are real edges)
+ *     fake pair:   s = gamma exp(clamp(sum_c K2[j] Q2[i] E2 / sqrt(hd), -5, 5)) / (gamma + 1), for every j != i of i's
+ *                  graph without a real edge j -> i
+ *   h1  = BN1(x + O_h(drop_13(attn)))                     dropout site 13
+ *   out = BN2(h1 + FFN2(drop_14(relu(FFN1(h1)))))         dropout site 14, FFN1 [2d, d], FFN2 [d, 2d]
+ * d % heads != 0 is GPS_ERR_ARG; d % 4 == 0, d <= 4096 and hd <= 192, else GPS_ERR_UNSUPPORTED.  nmax is the size of
+ * the largest graph of the batch (to_dense_batch's Nmax); the exclusion bitmap is [N, ceil(nmax / 32)] words of saved
+ * memory.  Parameters (weights non-NULL, else GPS_ERR_ARG): Q, K, V, Q2, K2, E, E2 = attention.{Q,K,V,Q_2,K_2,E,E_2}
+ * [d, d], bias NULL; O_h [d, d], ffn1, ffn2 with biases; bn1, bn2 = batch_norm{1,2}_h with running statistics (updated
+ * in training mode as torch.nn.BatchNorm1d, momentum 0.1); fake_edge_emb [d] (attention.fake_edge_emb.weight, one row).
+ * Backward writes grad_x, grad_edge_attr (NULL = not needed), every non-NULL parameter gradient and
+ * grad_fake_edge_emb; the weight products run on a side stream that joins the caller's stream before the call
+ * returns.  When Q..K2's grad_weight buffers are consecutive [5d, d] (K = Q + d*d, ...) they take one product.  No
+ * float atomics: two runs give the same bits.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  int64_t d;                 /* in_dim == out_dim                                              */
+  int64_t heads;             /* num_heads                                                      */
+  int32_t training;          /* 1: batch statistics and dropout; 0: running statistics         */
+  int32_t precision;         /* GPS_PREC_*                                                     */
+  float gamma;               /* cfg.gt.gamma, a constant                                       */
+  float dropout;             /* sites 13 and 14                                                */
+  int32_t flags;             /* backward: bit 0: parameter-gradient buffers are already zero; bit 1: gradients are
+                                added to the buffers (as GpsGraphormerArgs.flags)               */
+  int32_t reserved;
+  uint64_t seed;             /* Philox key of this call's dropout masks                       */
+  uint64_t offset;           /* Philox counter base                                            */
+  const uint64_t* offset_dev;/* optional device-resident addend to offset (CUDA-graph replays); NULL = none */
+  GpsGraph graph;
+  int64_t nmax;              /* largest graph of the batch                                     */
+  const float* x;            /* [N, d] batch.x                                                 */
+  const float* edge_attr;    /* [E, d] batch.edge_attr (non-NULL when E > 0)                   */
+  float* x_out;              /* [N, d] new batch.x (forward)                                   */
+  const float* grad_x_out;   /* [N, d] (backward)                                              */
+  float* grad_x;             /* [N, d] (backward)                                              */
+  float* grad_edge_attr;     /* [E, d] (backward, NULL = not needed)                           */
+  void* saved; int64_t saved_bytes;         /* written by forward, read by backward            */
+  void* workspace; int64_t workspace_bytes; /* transient                                       */
+  GpsLinear Q, K, V, Q2, K2, E, E2, O_h, ffn1, ffn2;
+  GpsBatchNorm bn1, bn2;
+  const float* fake_edge_emb;
+  float* grad_fake_edge_emb;
+} GpsSanArgs;
+
+typedef struct {
+  int64_t saved_bytes;
+  int64_t fwd_workspace_bytes;
+  int64_t bwd_workspace_bytes;
+} GpsSanPlan;
+
+/* Sizes for the configuration and graph of args (only d, heads, precision, training, dropout, gamma, nmax and
+ * graph.N / graph.E / graph.B are read). */
+int gps_san_plan(const GpsSanArgs* args, GpsSanPlan* plan);
+int gps_san_forward(const GpsSanArgs* args, void* stream);
+int gps_san_backward(const GpsSanArgs* args, void* stream);
+
+/* SAN attention stage (the kernels the layer calls).  Y [N, ld] holds the column blocks Q | K | V | Q2 | K2 (each
+ * heads * hd wide, ld >= 5 heads hd); E [E, heads * hd] the edge projection in edge-id order; E2 [heads * hd] the
+ * projected fake-edge embedding.  Forward: O [N, ldo] = the attention output, rz [N, heads] = 1 / (Z + 1e-6).
+ * Backward from dO: dY [N, ldg] = the gradients of the five blocks (dQ2 with respect to Q2 itself), dE [E, heads * hd]
+ * and dE2 [heads * hd], all written.  workspace: gps_san_attention_workspace_bytes.  Bad arguments are GPS_ERR_ARG (or
+ * GPS_ERR_UNSUPPORTED for the shape limits of the layer) before any CUDA call. */
+int64_t gps_san_attention_workspace_bytes(int64_t N, int64_t d, int64_t heads, int64_t nmax);
+int gps_san_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Y, int64_t ld, const float* E,
+                              const float* E2, float gamma, int64_t nmax, void* workspace, int64_t workspace_bytes,
+                              float* O, int64_t ldo, float* rz, void* stream);
+int gps_san_attention_backward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Y, int64_t ld,
+                               const float* E, const float* E2, float gamma, int64_t nmax, void* workspace,
+                               int64_t workspace_bytes, const float* O, const float* dO, int64_t ldo, const float* rz,
+                               float* dY, int64_t ldg, float* dE, float* dE2, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Stage-level entry points (the same kernels the layer calls; exported so the parity tests can
  * pin each stage against the oracle separately).
  * ---------------------------------------------------------------------------------------- */
