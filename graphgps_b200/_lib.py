@@ -147,6 +147,29 @@ class GpsSanPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
 
 
+class GpsCustomGnnArgs(C.Structure):
+    """CustomGNN's GatedGCNLayer / GINEConvLayer (custom_gnn.py): config, dropout stream, graph, tensors, scratch, the
+    persistent weight buffer, GatedGCN's A..E and two BatchNorms, GINE's model.nn.0 / model.nn.2."""
+    _fields_ = [("d", C.c_int64), ("kind", C.c_int32), ("act", C.c_int32), ("training", C.c_int32),
+                ("precision", C.c_int32), ("residual", C.c_int32), ("flags", C.c_int32), ("dropout", C.c_float),
+                ("gine_eps", C.c_float), ("seed", C.c_uint64), ("offset", C.c_uint64), ("offset_dev", _fp),
+                ("graph", GpsGraph),
+                ("x", _fp), ("edge_attr", _fp), ("x_out", _fp), ("edge_out", _fp), ("grad_x_out", _fp),
+                ("grad_edge_out", _fp), ("grad_x", _fp), ("grad_edge_attr", _fp),
+                ("saved", _fp), ("saved_bytes", C.c_int64), ("workspace", _fp), ("workspace_bytes", C.c_int64),
+                ("wplanes", _fp), ("wplanes_bytes", C.c_int64), ("wplanes_valid", C.c_int32), ("reserved", C.c_int32),
+                ("A", GpsLinear), ("B", GpsLinear), ("C", GpsLinear), ("D", GpsLinear), ("E", GpsLinear),
+                ("bn_node_x", GpsBatchNorm), ("bn_edge_e", GpsBatchNorm), ("nn0", GpsLinear), ("nn2", GpsLinear)]
+
+
+class GpsCustomGnnPlan(C.Structure):
+    _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64),
+                ("wplanes_bytes", C.c_int64)]
+
+
+CUSTOM_GATEDGCN, CUSTOM_GINE = 0, 1
+
+
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
                 ("bwd_workspace_bytes", C.c_int64), ("fwd_launches", C.c_int64),
@@ -188,6 +211,9 @@ SYMBOLS = {
     "gps_san_plan": (C.c_int, [C.POINTER(GpsSanArgs), C.POINTER(GpsSanPlan)]),
     "gps_san_forward": (C.c_int, [C.POINTER(GpsSanArgs), _fp]),
     "gps_san_backward": (C.c_int, [C.POINTER(GpsSanArgs), _fp]),
+    "gps_custom_gnn_plan": (C.c_int, [C.POINTER(GpsCustomGnnArgs), C.POINTER(GpsCustomGnnPlan)]),
+    "gps_custom_gnn_forward": (C.c_int, [C.POINTER(GpsCustomGnnArgs), _fp]),
+    "gps_custom_gnn_backward": (C.c_int, [C.POINTER(GpsCustomGnnArgs), _fp]),
     "gps_san_attention_workspace_bytes": (_i64, [_i64, _i64, _i64, _i64]),
     "gps_san_attention_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _i64, _fp, _fp, _f32, _i64, _fp, _i64,
                                             _fp, _i64, _fp, _fp]),

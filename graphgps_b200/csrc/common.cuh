@@ -177,7 +177,11 @@ enum {
   GPS_SITE_GR_OUT = 12,       // Graphormer layer: mlp.5, on mlp.4(.)
   GPS_SITE_SAN_ATTN = 13,     // SAN layer: dropout on the concatenated attention heads, before O_h
   GPS_SITE_SAN_FFN = 14,      // SAN layer: dropout on relu(FFN_h_layer1(.))
-  GPS_SITE_ATTN_P = 16
+  GPS_SITE_CG_X = 15,         // CustomGNN layers (custom_gnn.cu): GatedGCN's node output, GINE's output
+  GPS_SITE_ATTN_P = 16,       // + head: the attention probabilities
+  // CustomGNN GatedGCN's edge output: its own id, the last of the 4096 a call's Philox counter window holds (the layers
+  // advance the dropout offset by 4096 per call), far above any attention head's 16 + head
+  GPS_SITE_CG_E = 4095
 };
 
 __device__ __forceinline__ float warp_sum(float v) {

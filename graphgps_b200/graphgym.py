@@ -52,6 +52,21 @@ def install_san(san_module=None):
     return previous
 
 
+def install_custom_gnn(module=None):
+    """Rebind ``GatedGCNLayer`` and ``GINEConvLayer`` inside ``graphgps.network.custom_gnn`` so ``CustomGNN`` builds the
+    H100 layers: ``CustomGNN.build_conv_model`` returns those module globals.
+
+    Call after ``import graphgps`` and before ``create_model()``.  Returns the classes it replaced, as a dict by name,
+    so a caller can restore them."""
+    from .custom_gnn import GatedGCNLayer, GINEConvLayer
+    if module is None:
+        module = importlib.import_module("graphgps.network.custom_gnn")
+    previous = {n: getattr(module, n, None) for n in ("GatedGCNLayer", "GINEConvLayer")}
+    module.GatedGCNLayer = GatedGCNLayer
+    module.GINEConvLayer = GINEConvLayer
+    return previous
+
+
 def register(name="gpslayer_b200"):
     """Register a LayerConfig-style wrapper under ``name`` in GraphGym's layer registry.
 

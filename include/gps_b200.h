@@ -512,6 +512,71 @@ int gps_san_plan(const GpsSanArgs* args, GpsSanPlan* plan);
 int gps_san_forward(const GpsSanArgs* args, void* stream);
 int gps_san_backward(const GpsSanArgs* args, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * The message-passing layers of CustomGNN (graphgps/network/custom_gnn.py:31-37), standalone as the LRGB GatedGCN and
+ * GINE configs stack them, in_dim == out_dim == d:
+ *   GPS_CUSTOM_GATEDGCN  GatedGCNLayer (gatedgcn_layer.py:11-136, no EquivStableLapPE gate):
+ *       [Ax|Bx|Dx|Ex] = x W^T + b, Ce = edge_attr C^T + bC, e_ij = Dx_i + Ex_j + Ce, sigma = sigmoid(e_ij),
+ *       xt = Ax + sum sigma Bx_j / (sum sigma + 1e-6)
+ *       x_out = [x +] drop_15(act(bn_node_x(xt))),  edge_out = [edge_attr +] drop_4095(act(bn_edge_e(e_ij)))
+ *   GPS_CUSTOM_GINE      GINEConvLayer (gine_conv_layer.py:90-116), GINEConv(nn.0, ReLU, nn.2) with eps = gine_eps:
+ *       x_out = [x +] drop_15(relu(nn.2(relu(nn.0((1 + eps) x + sum_j relu(x_j + e_ij))))))
+ * [..] only with residual != 0; dropout sites 15 and 4095.  Any 1 <= d <= 4096 (else GPS_ERR_UNSUPPORTED): at
+ * d % 8 != 0 every intermediate runs at the pitch dp = round_up(d, 8) with zero pad columns, and the inputs, outputs,
+ * running statistics and gradients cross the call at pitch d.  Parameters (all non-NULL, else GPS_ERR_ARG): GatedGCN
+ * A..E [d, d] with biases, bn_node_x / bn_edge_e with running statistics (updated in training mode as
+ * torch.nn.BatchNorm1d, momentum 0.1); GINE nn0 = model.nn.0, nn2 = model.nn.2 [d, d] with biases.  wplanes: a
+ * caller-owned buffer (GpsCustomGnnPlan.wplanes_bytes) for the padded weight planes, biases and BatchNorm affine
+ * parameters; wplanes_valid != 0: it already holds them for the current parameters (packed once per optimiser step);
+ * the backward always reads it as the forward left it.  Backward writes grad_x, grad_edge_attr (NULL = not needed) and
+ * every non-NULL parameter gradient; grad_edge_out NULL = zero (GatedGCN).  The weight products run on a side stream
+ * that joins the caller's stream before the call returns.  Every width runs the same kernels at a pitch that is a
+ * multiple of 8, where the weight products take the deterministic split-K path: two runs give the same bits.
+ * ---------------------------------------------------------------------------------------- */
+enum { GPS_CUSTOM_GATEDGCN = 0, GPS_CUSTOM_GINE = 1 };
+typedef struct {
+  int64_t d;                 /* in_dim == out_dim                                              */
+  int32_t kind;              /* GPS_CUSTOM_*                                                   */
+  int32_t act;               /* GatedGCN: GPS_ACT_RELU / GPS_ACT_GELU; GINE: ReLU, not read     */
+  int32_t training;          /* 1: batch statistics and dropout; 0: running statistics         */
+  int32_t precision;         /* GPS_PREC_*                                                     */
+  int32_t residual;          /* 1: add the layer's input to its output(s)                      */
+  int32_t flags;             /* reserved, 0                                                    */
+  float dropout;             /* sites 15 (node output) and 4095 (GatedGCN edge output)         */
+  float gine_eps;            /* model.eps buffer value (GINE)                                  */
+  uint64_t seed;             /* Philox key of this call's dropout masks                       */
+  uint64_t offset;           /* Philox counter base                                            */
+  const uint64_t* offset_dev;/* optional device-resident addend to offset (CUDA-graph replays); NULL = none */
+  GpsGraph graph;
+  const float* x;            /* [N, d] batch.x                                                 */
+  const float* edge_attr;    /* [E, d] batch.edge_attr (non-NULL when E > 0)                   */
+  float* x_out;              /* [N, d] new batch.x (forward)                                   */
+  float* edge_out;           /* [E, d] new batch.edge_attr (forward, GatedGCN)                 */
+  const float* grad_x_out;   /* [N, d] (backward)                                              */
+  const float* grad_edge_out;/* [E, d] (backward, GatedGCN; NULL = zero)                       */
+  float* grad_x;             /* [N, d] (backward)                                              */
+  float* grad_edge_attr;     /* [E, d] (backward, NULL = not needed)                           */
+  void* saved; int64_t saved_bytes;         /* written by forward, read by backward            */
+  void* workspace; int64_t workspace_bytes; /* transient                                       */
+  void* wplanes; int64_t wplanes_bytes; int32_t wplanes_valid; int32_t reserved;
+  GpsLinear A, B, C, D, E;   /* GatedGCN                                                        */
+  GpsBatchNorm bn_node_x, bn_edge_e;
+  GpsLinear nn0, nn2;        /* GINE                                                            */
+} GpsCustomGnnArgs;
+
+typedef struct {
+  int64_t saved_bytes;
+  int64_t fwd_workspace_bytes;
+  int64_t bwd_workspace_bytes;
+  int64_t wplanes_bytes;
+} GpsCustomGnnPlan;
+
+/* Sizes for the configuration and graph of args (only d, kind, act, precision, training, residual, dropout, flags and
+ * graph.N / graph.E / graph.B are read). */
+int gps_custom_gnn_plan(const GpsCustomGnnArgs* args, GpsCustomGnnPlan* plan);
+int gps_custom_gnn_forward(const GpsCustomGnnArgs* args, void* stream);
+int gps_custom_gnn_backward(const GpsCustomGnnArgs* args, void* stream);
+
 /* SAN attention stage (the kernels the layer calls).  Y [N, ld] holds the column blocks Q | K | V | Q2 | K2 (each
  * heads * hd wide, ld >= 5 heads hd); E [E, heads * hd] the edge projection in edge-id order; E2 [heads * hd] the
  * projected fake-edge embedding.  Forward: O [N, ldo] = the attention output, rz [N, heads] = 1 / (Z + 1e-6).
