@@ -15,13 +15,14 @@ LIB_PATH = os.path.join(_HERE, "libgps_b200.so")
 
 GPS_OK, GPS_ERR_ARG, GPS_ERR_UNSUPPORTED, GPS_ERR_CUDA = 0, -1, -2, -3
 LOCAL = {"None": 0, "CustomGatedGCN": 1, "GINE": 2, "GCN": 3, "GAT": 4, "GENConv": 5, "PNA": 6}
-GLOBAL = {"None": 0, "Transformer": 1, "Performer": 2}
-# the BigBird global model: reached through gps_layer_{forward,backward}_bigbird only, so not in GLOBAL
-GLOBAL_BIGBIRD = 3
+GLOBAL = {"None": 0, "Transformer": 1, "Performer": 2, "BigBird": 3}
+GLOBAL_BIGBIRD = GLOBAL["BigBird"]   # the name existing binders import; the same value
 BIGBIRD_ACT = {"relu": 0, "sigmoid": 1}   # GpsBigBird.hidden_act
 ACT = {"relu": 0, "gelu": 1}
 PRECISION = {"fp32": 0, "bf16": 1}
 NORM = {"batch": 0, "none": 1}
+# GpsLayerArgs.flags (backward), also GpsGraphormerArgs.flags and GpsSanArgs.flags
+FLAG_GRADS_ZEROED, FLAG_GRADS_ACCUMULATE = 1, 2
 
 _fp = C.c_void_p  # device pointers travel as void*
 
@@ -43,39 +44,6 @@ class GpsLinear(C.Structure):
 
 class GpsPlanes(C.Structure):
     _fields_ = [("hi", _fp), ("lo", _fp), ("ld", C.c_int64)]
-
-
-class GpsLayerArgs(C.Structure):
-    _fields_ = [
-        ("d", C.c_int64), ("heads", C.c_int64),
-        ("local_type", C.c_int32), ("global_type", C.c_int32), ("act", C.c_int32),
-        ("training", C.c_int32), ("precision", C.c_int32), ("reserved0", C.c_int32),
-        ("dropout", C.c_float), ("attn_dropout", C.c_float),
-        ("seed", C.c_uint64), ("offset", C.c_uint64),
-        ("gine_eps", C.c_float), ("norm_type", C.c_int32),   # NORM (formerly reserved1)
-        ("graph", GpsGraph),
-        ("x", _fp), ("edge_attr", _fp), ("x_out", _fp), ("edge_out", _fp),
-        ("gcn_A", GpsLinear), ("gcn_B", GpsLinear), ("gcn_C", GpsLinear), ("gcn_D", GpsLinear),
-        ("gcn_E", GpsLinear),
-        ("bn_node_x", GpsBatchNorm), ("bn_edge_e", GpsBatchNorm),
-        ("gine_lin0", GpsLinear), ("gine_lin1", GpsLinear),
-        ("attn_in", GpsLinear), ("attn_out", GpsLinear),
-        ("perf_q", GpsLinear), ("perf_k", GpsLinear), ("perf_v", GpsLinear),
-        ("perf_proj", _fp), ("perf_features", C.c_int64), ("perf_dim_head", C.c_int64),
-        ("norm1_local", GpsBatchNorm), ("norm1_attn", GpsBatchNorm), ("norm2", GpsBatchNorm),
-        ("ff1", GpsLinear), ("ff2", GpsLinear),
-        ("grad_x_out", _fp), ("grad_edge_out", _fp), ("grad_x", _fp), ("grad_edge_attr", _fp),
-        ("saved", _fp), ("saved_bytes", C.c_int64),
-        ("workspace", _fp), ("workspace_bytes", C.c_int64),
-        ("offset_dev", _fp),
-        ("gcn_conv", GpsLinear),
-        ("ev_grads_early", _fp),
-        ("x_planes_in", GpsPlanes), ("e_planes_in", GpsPlanes), ("x_planes_out", GpsPlanes), ("e_planes_out", GpsPlanes),
-        ("wplanes", _fp), ("wplanes_bytes", C.c_int64), ("wplanes_valid", C.c_int32), ("reserved2", C.c_int32),
-        ("ev_grads_mid", _fp), ("ev_grads_done", _fp),
-        # appended extension: EquivStableLapPE edge gate (equivstable_pe=True)
-        ("pe", _fp), ("pe_dim", C.c_int64), ("grad_pe", _fp), ("pe_mlp0", GpsLinear), ("pe_mlp1", GpsLinear),
-    ]
 
 
 class GpsAttnBias(C.Structure):
@@ -108,6 +76,39 @@ class GpsBigBird(C.Structure):
                 ("key_ptr", _fp), ("key_idx", _fp), ("query_ptr", _fp), ("query_idx", _fp),
                 ("query", GpsLinear), ("key", GpsLinear), ("value", GpsLinear), ("self_out", GpsLinear),
                 ("ln1", GpsLinear), ("intermediate", GpsLinear), ("output", GpsLinear), ("ln2", GpsLinear)]
+
+
+class GpsLayerArgs(C.Structure):
+    _fields_ = [
+        ("d", C.c_int64), ("heads", C.c_int64),
+        ("local_type", C.c_int32), ("global_type", C.c_int32), ("act", C.c_int32),
+        ("training", C.c_int32), ("precision", C.c_int32), ("flags", C.c_int32),
+        ("dropout", C.c_float), ("attn_dropout", C.c_float),
+        ("seed", C.c_uint64), ("offset", C.c_uint64),
+        ("gine_eps", C.c_float), ("norm_type", C.c_int32),
+        ("graph", GpsGraph),
+        ("x", _fp), ("edge_attr", _fp), ("x_out", _fp), ("edge_out", _fp),
+        ("gcn_A", GpsLinear), ("gcn_B", GpsLinear), ("gcn_C", GpsLinear), ("gcn_D", GpsLinear),
+        ("gcn_E", GpsLinear),
+        ("bn_node_x", GpsBatchNorm), ("bn_edge_e", GpsBatchNorm),
+        ("gine_lin0", GpsLinear), ("gine_lin1", GpsLinear),
+        ("attn_in", GpsLinear), ("attn_out", GpsLinear),
+        ("perf_q", GpsLinear), ("perf_k", GpsLinear), ("perf_v", GpsLinear),
+        ("perf_proj", _fp), ("perf_features", C.c_int64), ("perf_dim_head", C.c_int64),
+        ("norm1_local", GpsBatchNorm), ("norm1_attn", GpsBatchNorm), ("norm2", GpsBatchNorm),
+        ("ff1", GpsLinear), ("ff2", GpsLinear),
+        ("grad_x_out", _fp), ("grad_edge_out", _fp), ("grad_x", _fp), ("grad_edge_attr", _fp),
+        ("saved", _fp), ("saved_bytes", C.c_int64),
+        ("workspace", _fp), ("workspace_bytes", C.c_int64),
+        ("offset_dev", _fp),
+        ("gcn_conv", GpsLinear),
+        ("ev_grads_early", _fp),
+        ("x_planes_in", GpsPlanes), ("e_planes_in", GpsPlanes), ("x_planes_out", GpsPlanes), ("e_planes_out", GpsPlanes),
+        ("wplanes", _fp), ("wplanes_bytes", C.c_int64), ("wplanes_valid", C.c_int32), ("reserved2", C.c_int32),
+        ("ev_grads_mid", _fp), ("ev_grads_done", _fp),
+        ("pe", _fp), ("pe_dim", C.c_int64), ("grad_pe", _fp), ("pe_mlp0", GpsLinear), ("pe_mlp1", GpsLinear),
+        ("attn_bias", GpsAttnBias), ("gat", GpsGat), ("genconv", GpsGenConv), ("pna", GpsPna), ("bigbird", GpsBigBird),
+    ]
 
 
 class GpsGraphormerArgs(C.Structure):
@@ -172,8 +173,7 @@ CUSTOM_GATEDGCN, CUSTOM_GINE = 0, 1
 
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
-                ("bwd_workspace_bytes", C.c_int64), ("fwd_launches", C.c_int64),
-                ("bwd_launches", C.c_int64), ("wplanes_bytes", C.c_int64)]
+                ("bwd_workspace_bytes", C.c_int64), ("wplanes_bytes", C.c_int64)]
 
 
 # every symbol include/gps_b200.h declares: name -> (restype, argtypes)
@@ -187,20 +187,6 @@ SYMBOLS = {
     "gps_layer_plan": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsLayerPlan)]),
     "gps_layer_forward": (C.c_int, [C.POINTER(GpsLayerArgs), _fp]),
     "gps_layer_backward": (C.c_int, [C.POINTER(GpsLayerArgs), _fp]),
-    "gps_layer_forward_biased": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsAttnBias), _fp]),
-    "gps_layer_backward_biased": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsAttnBias), _fp]),
-    "gps_layer_forward_gat": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGat), C.POINTER(GpsAttnBias), _fp]),
-    "gps_layer_backward_gat": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGat), C.POINTER(GpsAttnBias), _fp]),
-    "gps_layer_forward_genconv": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGenConv), C.POINTER(GpsAttnBias),
-                                            _fp]),
-    "gps_layer_backward_genconv": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsGenConv), C.POINTER(GpsAttnBias),
-                                             _fp]),
-    "gps_layer_forward_pna": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsPna), C.POINTER(GpsAttnBias), _fp]),
-    "gps_layer_backward_pna": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsPna), C.POINTER(GpsAttnBias), _fp]),
-    "gps_layer_forward_bigbird": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsBigBird), C.POINTER(GpsGat),
-                                            C.POINTER(GpsGenConv), C.POINTER(GpsPna), _fp]),
-    "gps_layer_backward_bigbird": (C.c_int, [C.POINTER(GpsLayerArgs), C.POINTER(GpsBigBird), C.POINTER(GpsGat),
-                                             C.POINTER(GpsGenConv), C.POINTER(GpsPna), _fp]),
     "gps_bigbird_attention_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, C.POINTER(GpsBigBird), _fp, _fp, _fp,
                                                 _i64, _fp, _i64, _fp, _fp]),
     "gps_bigbird_attention_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, C.POINTER(GpsBigBird), _fp, _fp, _fp,
@@ -303,7 +289,7 @@ def load():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing
         fn.restype = res
         fn.argtypes = args
-    if lib.gps_abi_version() != 3:
+    if lib.gps_abi_version() != 4:
         raise RuntimeError("libgps_b200.so ABI version mismatch")
     _lib = lib
     return lib

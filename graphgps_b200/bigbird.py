@@ -285,8 +285,9 @@ def device_lists(device, nb, heads, bs, r, max_len):
     return hit
 
 
-def gps_bigbird(params: BigBirdParams, named, grads, prefix, lists, nb):
-    """GpsBigBird of the C ABI from the container's parameters (named / grads: name -> tensor)."""
+def gps_bigbird(params: BigBirdParams, named, grads, prefix):
+    """GpsBigBird of the C ABI from the container's parameters (named / grads: name -> tensor).  num_blocks and the
+    block lists belong to the batch and are left 0 / NULL."""
     cfg = params.cfg
     g = grads or {}
     p = prefix + "encoder.layers.0."
@@ -295,8 +296,7 @@ def gps_bigbird(params: BigBirdParams, named, grads, prefix, lists, nb):
         return _lib.GpsLinear(_lib.ptr(named[p + name + ".weight"]), _lib.ptr(named.get(p + name + ".bias")),
                               _lib.ptr(g.get(p + name + ".weight")), _lib.ptr(g.get(p + name + ".bias")))
 
-    return _lib.GpsBigBird(cfg.block_size, nb, _lib.BIGBIRD_ACT[cfg.hidden_act], cfg.layer_norm_eps,
-                           *(t.data_ptr() for t in lists),
+    return _lib.GpsBigBird(cfg.block_size, 0, _lib.BIGBIRD_ACT[cfg.hidden_act], cfg.layer_norm_eps, 0, 0, 0, 0,
                            lin("attention.self.query"), lin("attention.self.key"), lin("attention.self.value"),
                            lin("attention.output.dense"), lin("attention.output.LayerNorm"),
                            lin("intermediate.dense"), lin("output.dense"), lin("output.LayerNorm"))

@@ -55,8 +55,8 @@ int make_plan(const GpsGraphormerArgs* a, GrPlan* P, bool bind) {
   P->N = N; P->d = d; P->H = a->heads; P->hd = d / a->heads;
   P->prec = a->precision;
   P->train = a->training != 0;
-  P->grads_accumulate = (a->flags & 2) != 0;
-  P->grads_prezeroed = (a->flags & 1) != 0 || P->grads_accumulate;
+  P->grads_accumulate = (a->flags & GPS_FLAG_GRADS_ACCUMULATE) != 0;
+  P->grads_prezeroed = (a->flags & GPS_FLAG_GRADS_ZEROED) != 0 || P->grads_accumulate;
   auto drop = [&](float p, int site) {
     DropCfg c;
     c.p = P->train ? p : 0.f;

@@ -179,25 +179,23 @@ struct LayerWeight {
 struct Plan {
   int64_t N, E, d, H, hd, Wy, qkv_off;
   bool gated, gine, gcn, attn, perf;
-  // GAT (gat.cu): the caller's GpsGat (NULL when only sizes are wanted); saved v = fold(W_edge, att_edge) [H, d] and the
-  // scores (GatScores); backward scratch g_v [H, d] then gat_bwd's workspace
+  bool loc, glob;   // the layer has a local model / a global model
+  const GpsAttnBias* bias;   // the BiasedTransformer's GpsLayerArgs.attn_bias; NULL when unbiased or only sizing
+  // GAT (gat.cu): saved v = fold(W_edge, att_edge) [H, d] and the scores (GatScores); backward scratch g_v [H, d] then
+  // gat_bwd's workspace
   bool gat;
-  const GpsGat* gatp;
   float *gat_v, *gat_sc, *gat_ws;
-  // GENConv (genconv.cu): the caller's GpsGenConv (NULL when only sizes are wanted).  Saved: agg (in `agg`), lse, u [N,d],
-  // h1 = u W0^T and r = relu(mlp.1(h1)) [N,2d], and mlp.1's batch statistics in a 2d-wide slot of their own (gen_bn:
-  // mean | invstd; the BN_* slots are d wide).  Workspace: mlp.1's column sums (gen_fstats / gen_bsums, [2][2d] doubles),
-  // backward g_r, g_h1 [N,2d] and g_u [N,d].
+  // GENConv (genconv.cu).  Saved: agg (in `agg`), lse, u [N,d], h1 = u W0^T and r = relu(mlp.1(h1)) [N,2d], and mlp.1's
+  // batch statistics in a 2d-wide slot of their own (gen_bn: mean | invstd; the BN_* slots are d wide).  Workspace:
+  // mlp.1's column sums (gen_fstats / gen_bsums, [2][2d] doubles), backward g_r, g_h1 [N,2d] and g_u [N,d].
   bool gen;
-  const GpsGenConv* genp;
   float *gen_lse, *gen_u, *gen_h1, *gen_r, *gen_bn, *gen_gr, *gen_gh1, *gen_gu;
   double *gen_fstats, *gen_bsums;
-  // PNA (pna.cu): the caller's GpsPna (NULL when only sizes are wanted) and de = edge_dim (d, the bound, without it).
-  // Saved: the fold F [d, de] with its planes and c [d]; Z = [x | mean | max | sum] [N, 4d] (planes; fp32 without
-  // planes); the argmax [N, d]; h = post(Z) [N, d] with planes.  Forward workspace: q = e F^T + c [E, d].  Backward:
+  // PNA (pna.cu): de = edge_dim (d, the bound, when only sizes are wanted).  Saved: the fold F [d, de] with its planes
+  // and c [d]; Z = [x | mean | max | sum] [N, 4d] (planes; fp32 without planes); the argmax [N, d]; h = post(Z) [N, d]
+  // with planes.  Forward workspace: q = e F^T + c [E, d].  Backward:
   // g_h [N, d], g_Z [N, 4d], g_q [E, d] (+ planes), g_F [d, de] | g_c [d], g_xl.
   bool pna;
-  const GpsPna* pnap;
   int64_t de;
   float *pna_F, *pna_c, *pna_Z, *pna_h, *pna_q, *pna_gh, *pna_gZ, *pna_gq, *pna_gF;
   int* pna_arg;
@@ -214,13 +212,11 @@ struct Plan {
   bool perf_pairwise;     // mean graph size <= 48: n^2 (m+64) < 2 n m 64
   float *g_pfq, *g_pfk, *g_pQ, *g_pK, *g_pV, *g_pgmax, *g_xp;   // backward workspace (Performer)
   float* g_pgrow;         // [N*H] per-row stabiliser gradients, summed per (graph, head) in a fixed order
-  // BigBird (bigbird.cu): the caller's GpsBigBird (NULL when only sizes are wanted).  The attention output and lse are O /
-  // lse.  Saved: z1 = drop(ctx Wso^T + bso) + x, a = LN1(z1) (+ planes), u = act(a Wi^T + bi) (+ planes),
-  // z2 = drop(u Wo^T + bo) + a, and the row statistics mean1 | rstd1 | mean2 | rstd2 [4][N].  Backward: g_od (gradient of
-  // output.dense, + planes), dz2, g_u (+ planes), g_a, g_so (gradient of attention.output.dense, + planes), g_x part
-  // dz1 + g_hA, and the LayerNorm partials.
+  // BigBird (bigbird.cu): the attention output and lse are O / lse.  Saved: z1 = drop(ctx Wso^T + bso) + x,
+  // a = LN1(z1) (+ planes), u = act(a Wi^T + bi) (+ planes), z2 = drop(u Wo^T + bo) + a, and the row statistics
+  // mean1 | rstd1 | mean2 | rstd2 [4][N].  Backward: g_od (gradient of output.dense, + planes), dz2, g_u (+ planes), g_a,
+  // g_so (gradient of attention.output.dense, + planes), g_x part dz1 + g_hA, and the LayerNorm partials.
   bool bb;
-  const GpsBigBird* bbp;
   float *bb_z1, *bb_a, *bb_u, *bb_z2, *bb_stat, *bb_god, *bb_dz2, *bb_gu, *bb_ga, *bb_gso, *bb_gx, *bb_part;
   Planes bb_a_p, bb_u_p, bb_so_p, bb_in_p, bb_out_p, bb_god_p, bb_gu_p, bb_gso_p;
   // saved
@@ -257,10 +253,11 @@ struct Plan {
   int prec;                // GPS_PREC_*
   DropCfg dropout;         // GPSLayer.dropout: p = 0 in eval mode; the site is set per use (drop())
   float pa;                // attn_dropout, 0 in eval mode
-  bool grads_prezeroed;    // GpsLayerArgs.reserved0 bit 0: the caller already zeroed every parameter-gradient buffer
+  bool grads_prezeroed;    // GPS_FLAG_GRADS_ZEROED: the caller already zeroed every parameter-gradient buffer
                            // (one multi-tensor fill instead of a memset per weight and bias)
-  bool grads_accumulate;   // bit 1: parameter gradients are ADDED to the caller's buffers (torch's .grad accumulation
-                           // semantics on a static gradient bucket: graphgps_b200/dp.py); implies bit 0
+  bool grads_accumulate;   // GPS_FLAG_GRADS_ACCUMULATE: parameter gradients are ADDED to the caller's buffers (torch's
+                           // .grad accumulation semantics on a static gradient bucket: graphgps_b200/dp.py); implies
+                           // grads_prezeroed
   DropCfg drop(int site) const {
     DropCfg c = dropout;
     c.site = site;
@@ -281,7 +278,6 @@ static void list_weights(const GpsLayerArgs* a, Plan* P) {
     add_seg(PackSeg{l.weight, bias ? l.bias : nullptr, l.grad_weight, bias ? l.grad_bias : nullptr, (int)rows, (int)cols},
             cols, planes);
   };
-  static const GpsLinear kNoLinear = {};
   if (P->gated) {
     add(a->gcn_A, d, d, &Plan::Wcat_p);
     add(a->gcn_B, d, d, &Plan::Wcat_p);
@@ -292,11 +288,11 @@ static void list_weights(const GpsLayerArgs* a, Plan* P) {
   // GCNConv.lin has no bias; GCNConv.bias is added after the aggregation (scatter.cu)
   if (P->gcn) add(a->gcn_conv, d, d, &Plan::Wcat_p, false);
   // GATConv.lin_src (= lin_dst) has no bias; GATConv.bias is added after the aggregation (gat.cu)
-  if (P->gat) add(P->gatp ? P->gatp->lin_src : kNoLinear, d, d, &Plan::Wcat_p, false);
+  if (P->gat) add(a->gat.lin_src, d, d, &Plan::Wcat_p, false);
   // PNA: the destination and source column blocks of pre_nns.0.0.weight [d, 3d] give P_dst | P_src; pre's bias enters
   // through the edge term (pna.cu)
   if (P->pna) {
-    const GpsLinear& pre = P->pnap ? P->pnap->pre : kNoLinear;
+    const GpsLinear& pre = a->pna.pre;
     for (int64_t blk = 0; blk < 2; ++blk)
       add_seg(PackSeg{pre.weight ? pre.weight + blk * d : nullptr, nullptr,
                       pre.grad_weight ? pre.grad_weight + blk * d : nullptr, nullptr, (int)d, (int)(3 * d)},
@@ -306,7 +302,7 @@ static void list_weights(const GpsLayerArgs* a, Plan* P) {
   if (P->attn) add(a->attn_in, 3 * d, d, &Plan::Wcat_p);
   if (P->attn || P->perf) add(a->attn_out, d, kout, &Plan::out_p);
   if (P->bb) {   // attention.self.{query,key,value} (bias only with use_bias) fill the in_proj rows of Wcat
-    const GpsBigBird& b = P->bbp ? *P->bbp : GpsBigBird{};
+    const GpsBigBird& b = a->bigbird;
     add(b.query, d, d, &Plan::Wcat_p);
     add(b.key, d, d, &Plan::Wcat_p);
     add(b.value, d, d, &Plan::Wcat_p);
@@ -321,12 +317,12 @@ static void list_weights(const GpsLayerArgs* a, Plan* P) {
     add(a->gine_lin1, d, d, &Plan::g1_p);
   }
   if (P->gen) {   // GENConv's MLP Linears have no bias
-    add(P->genp ? P->genp->lin0 : kNoLinear, 2 * d, d, &Plan::mlp0_p, false);
-    add(P->genp ? P->genp->lin1 : kNoLinear, d, 2 * d, &Plan::mlp4_p, false);
+    add(a->genconv.lin0, 2 * d, d, &Plan::mlp0_p, false);
+    add(a->genconv.lin1, d, 2 * d, &Plan::mlp4_p, false);
   }
   if (P->pna) {
-    add(P->pnap ? P->pnap->post : kNoLinear, d, 4 * d, &Plan::post_p);
-    add(P->pnap ? P->pnap->lin : kNoLinear, d, d, &Plan::lin_p);
+    add(a->pna.post, d, 4 * d, &Plan::post_p);
+    add(a->pna.lin, d, d, &Plan::lin_p);
   }
   if (P->perf) {
     add(a->perf_q, P->inner, d, &Plan::pq_p);
@@ -343,8 +339,7 @@ static Planes caller_planes(const GpsPlanes& g, int64_t d, int precision) {
   return Planes{(__nv_bfloat16*)g.hi, lo ? (__nv_bfloat16*)g.lo : nullptr, g.ld};
 }
 
-static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* gat = nullptr,
-                     const GpsGenConv* gen = nullptr, const GpsPna* pna = nullptr, const GpsBigBird* bb = nullptr) {
+static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   memset(P, 0, sizeof(*P));
   GPS_REQUIRE(a, GPS_ERR_ARG, "null args");
   P->N = a->graph.N;
@@ -357,14 +352,11 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   P->gine = a->local_type == GPS_LOCAL_GINE;
   P->gcn = a->local_type == GPS_LOCAL_GCN;
   P->gat = a->local_type == GPS_LOCAL_GAT;
-  P->gatp = gat;
   P->gen = a->local_type == GPS_LOCAL_GENCONV;
-  P->genp = gen;
   P->pna = a->local_type == GPS_LOCAL_PNA;
-  P->pnap = pna;
-  P->de = pna ? pna->edge_dim : a->d;   // sizes alone: edge_dim <= d is the bound
-  GPS_REQUIRE(a->local_type == GPS_LOCAL_NONE || P->gated || P->gine || P->gcn || P->gat || P->gen || P->pna,
-              GPS_ERR_ARG, "unknown local_type %d", a->local_type);
+  P->loc = P->gated || P->gine || P->gcn || P->gat || P->gen || P->pna;
+  P->de = bind ? a->pna.edge_dim : a->d;   // sizes alone: edge_dim <= d is the bound
+  GPS_REQUIRE(a->local_type == GPS_LOCAL_NONE || P->loc, GPS_ERR_ARG, "unknown local_type %d", a->local_type);
   if (P->pna) GPS_TRY(pna_check(a->d, P->de));
   if (P->gat) GPS_TRY(gat_check(a->d, a->heads));
   GPS_REQUIRE(!P->gen || a->d <= 2048, GPS_ERR_UNSUPPORTED,
@@ -379,14 +371,21 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   P->attn = a->global_type == GPS_GLOBAL_TRANSFORMER;
   P->perf = a->global_type == GPS_GLOBAL_PERFORMER;
   P->bb = a->global_type == GPS_GLOBAL_BIGBIRD;
-  P->bbp = bb;
-  GPS_REQUIRE(!bind || P->bb == (bb != nullptr), GPS_ERR_ARG,
-              P->bb ? "global_type GPS_GLOBAL_BIGBIRD needs gps_layer_forward_bigbird / gps_layer_backward_bigbird"
-                    : "a GpsBigBird needs global_type GPS_GLOBAL_BIGBIRD");
+  P->glob = P->attn || P->perf || P->bb;
+  if (bind) {   // attention bias of the BiasedTransformer; NULL bias = none
+    const GpsAttnBias& ab = a->attn_bias;
+    GPS_REQUIRE(ab.bias || (ab.nmax == 0 && !ab.grad_bias), GPS_ERR_ARG,
+                "attention bias: null bias pointer with nmax %lld / grad_bias set", (long long)ab.nmax);
+    GPS_REQUIRE(!ab.bias || P->attn, GPS_ERR_ARG, "an attention bias needs global_type GPS_GLOBAL_TRANSFORMER (got %d)",
+                a->global_type);
+    GPS_REQUIRE(!ab.bias || ab.nmax >= 1, GPS_ERR_ARG, "attention bias: nmax must be >= 1 (got %lld)",
+                (long long)ab.nmax);
+    P->bias = ab.bias ? &ab : nullptr;
+  }
   if (P->bb) {   // any head dim (the shipped BigBird config has hd = 7)
     GPS_REQUIRE(a->heads > 0 && a->d % a->heads == 0, GPS_ERR_ARG, "dim_h %% num_heads != 0");
     P->hd = a->d / a->heads;
-    if (bb) GPS_TRY(bb_check(a->d, a->heads, bb));
+    if (bind) GPS_TRY(bb_check(a->d, a->heads, &a->bigbird));
   }
   if (P->perf) {
     GPS_TRY(perf_supported(a->perf_dim_head, a->perf_features));
@@ -396,7 +395,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     P->mp = perf_mp();
     P->m = a->perf_features;
   }
-  GPS_REQUIRE(a->local_type != GPS_LOCAL_NONE || P->attn || P->perf || P->bb, GPS_ERR_ARG,
+  GPS_REQUIRE(a->local_type != GPS_LOCAL_NONE || P->glob, GPS_ERR_ARG,
               "GPSLayer needs a local model or a global model");
   GPS_REQUIRE(a->norm_type == GPS_NORM_BATCH || a->norm_type == GPS_NORM_NONE, GPS_ERR_UNSUPPORTED,
               "norm_type %d is not built (GPS_NORM_BATCH = 0, GPS_NORM_NONE = 1)", a->norm_type);
@@ -417,8 +416,8 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   P->dropout.offset = a->offset;
   P->dropout.offset_dev = (const unsigned long long*)a->offset_dev;
   P->pa = P->train ? a->attn_dropout : 0.f;
-  P->grads_accumulate = (a->reserved0 & 2) != 0;
-  P->grads_prezeroed = (a->reserved0 & 1) != 0 || P->grads_accumulate;
+  P->grads_accumulate = (a->flags & GPS_FLAG_GRADS_ACCUMULATE) != 0;
+  P->grads_prezeroed = (a->flags & GPS_FLAG_GRADS_ZEROED) != 0 || P->grads_accumulate;
   list_weights(a, P);
   const int64_t N = P->N, E = P->E, d = P->d;
   const bool gelu = a->act == GPS_ACT_GELU;
@@ -462,8 +461,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     P->pna_arg = S.alloc<int>(N * d);
     P->pna_h = S.alloc<float>(N * d);
   }
-  const bool loc = P->gated || P->gine || P->gcn || P->gat || P->gen || P->pna;
-  if (loc && !P->nonorm) P->xloc = S.alloc<float>(N * d);   // read by norm1_local's backward
+  if (P->loc && !P->nonorm) P->xloc = S.alloc<float>(N * d);   // read by norm1_local's backward
   if (P->attn) {
     P->O = S.alloc<float>(N * d);
     P->lse = S.alloc<float>(N * P->H);
@@ -518,7 +516,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
       P->e_p = caller_planes(a->e_planes_in, d, a->precision);
       if (!P->e_p.hi) P->e_p = mkplanes(S, E, d);
     }
-    if (P->attn || P->perf || P->bb) P->O_p = mkplanes(S, N, kout);
+    if (P->glob) P->O_p = mkplanes(S, N, kout);
     if (P->bb) {
       P->bb_a_p = mkplanes(S, N, d);
       P->bb_u_p = mkplanes(S, N, d);
@@ -567,9 +565,9 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   P->fstats = F.alloc<double>(P->nbn * 2 * d);
   if (P->gen) P->gen_fstats = F.alloc<double>(2 * 2 * d);
   if (P->pna) P->pna_q = F.alloc<float>(E * d);
-  if (P->nonorm && loc) {
+  if (P->nonorm && P->loc) {
     // x_loc is an operand of the GEMM that writes s (and of nothing in the backward pass); a lone local model writes s
-    P->xloc = (P->attn || P->perf || P->bb) ? F.alloc<float>(N * d) : P->s;
+    P->xloc = P->glob ? F.alloc<float>(N * d) : P->s;
   }
   P->fwd_bytes = F.used;
 
@@ -584,7 +582,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
     P->g_tmp3 = Bk.alloc<float>(N * d);
   }
   // GPS_NORM_NONE: the upstream gradients of x_loc and hA are both g_s
-  if (loc && !P->nonorm) P->g_xloc = Bk.alloc<float>(N * d);
+  if (P->loc && !P->nonorm) P->g_xloc = Bk.alloc<float>(N * d);
   if (P->attn) {
     if (!P->nonorm) P->g_hA = Bk.alloc<float>(N * d);
     P->g_O = Bk.alloc<float>(N * d);
@@ -654,7 +652,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind, const GpsGat* ga
   if (P->use_planes) {
     P->gt_p = mkplanes(Bk, N, d);
     P->ghid_p = mkplanes(Bk, N, 2 * d);
-    if ((P->attn || P->perf || P->bb) && !P->nonorm) P->ghA_p = mkplanes(Bk, N, d);
+    if (P->glob && !P->nonorm) P->ghA_p = mkplanes(Bk, N, d);
     if (P->bb) {
       P->bb_god_p = mkplanes(Bk, N, d);
       P->bb_gu_p = mkplanes(Bk, N, d);
@@ -739,32 +737,26 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
   }
   if (P.gcn) GPS_TRY(check_linear(a->gcn_conv, "local_model.lin / local_model.bias", true));
   if (P.gat) {
-    GPS_REQUIRE(P.gatp, GPS_ERR_ARG, "local_type GPS_LOCAL_GAT needs gps_layer_forward_gat / gps_layer_backward_gat "
-                "with a GpsGat");
-    GPS_TRY(check_linear(P.gatp->lin_src, "local_model.lin_src / local_model.bias", true));
-    GPS_TRY(check_linear(P.gatp->lin_edge, "local_model.lin_edge", false));
-    GPS_REQUIRE(P.gatp->att_src && P.gatp->att_dst && P.gatp->att_edge, GPS_ERR_ARG,
+    GPS_TRY(check_linear(a->gat.lin_src, "local_model.lin_src / local_model.bias", true));
+    GPS_TRY(check_linear(a->gat.lin_edge, "local_model.lin_edge", false));
+    GPS_REQUIRE(a->gat.att_src && a->gat.att_dst && a->gat.att_edge, GPS_ERR_ARG,
                 "missing parameter local_model.att_{src,dst,edge}");
   }
   if (P.gen) {
-    GPS_REQUIRE(P.genp, GPS_ERR_ARG, "local_type GPS_LOCAL_GENCONV needs gps_layer_forward_genconv / "
-                "gps_layer_backward_genconv with a GpsGenConv");
-    GPS_TRY(check_linear(P.genp->lin0, "local_model.mlp.0", false));
-    GPS_TRY(check_bn(P.genp->bn, "local_model.mlp.1"));
-    GPS_REQUIRE(P.genp->bn.running_mean && P.genp->bn.running_var, GPS_ERR_ARG,
+    GPS_TRY(check_linear(a->genconv.lin0, "local_model.mlp.0", false));
+    GPS_TRY(check_bn(a->genconv.bn, "local_model.mlp.1"));
+    GPS_REQUIRE(a->genconv.bn.running_mean && a->genconv.bn.running_var, GPS_ERR_ARG,
                 "missing buffer local_model.mlp.1.running_{mean,var}");
-    GPS_TRY(check_linear(P.genp->lin1, "local_model.mlp.4", false));
+    GPS_TRY(check_linear(a->genconv.lin1, "local_model.mlp.4", false));
   }
   if (P.pna) {
-    GPS_REQUIRE(P.pnap, GPS_ERR_ARG, "local_type GPS_LOCAL_PNA needs gps_layer_forward_pna / gps_layer_backward_pna "
-                "with a GpsPna");
-    GPS_TRY(check_linear(P.pnap->edge_encoder, "local_model.edge_encoder", true));
-    GPS_TRY(check_linear(P.pnap->pre, "local_model.pre_nns.0.0", true));
-    GPS_TRY(check_linear(P.pnap->post, "local_model.post_nns.0.0", true));
-    GPS_TRY(check_linear(P.pnap->lin, "local_model.lin", true));
+    GPS_TRY(check_linear(a->pna.edge_encoder, "local_model.edge_encoder", true));
+    GPS_TRY(check_linear(a->pna.pre, "local_model.pre_nns.0.0", true));
+    GPS_TRY(check_linear(a->pna.post, "local_model.post_nns.0.0", true));
+    GPS_TRY(check_linear(a->pna.lin, "local_model.lin", true));
   }
   const bool bn = !P.nonorm;   // norm1_local / norm1_attn / norm2 exist in BatchNorm mode only
-  if ((P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) && bn) GPS_TRY(check_bn(a->norm1_local, "norm1_local"));
+  if (P.loc && bn) GPS_TRY(check_bn(a->norm1_local, "norm1_local"));
   if (P.attn) {
     GPS_TRY(check_linear(a->attn_in, "self_attn.in_proj", true));
     GPS_TRY(check_linear(a->attn_out, "self_attn.out_proj", true));
@@ -779,7 +771,7 @@ static int check_params(const GpsLayerArgs* a, const Plan& P) {
     if (bn) GPS_TRY(check_bn(a->norm1_attn, "norm1_attn"));
   }
   if (P.bb) {
-    const GpsBigBird& b = *P.bbp;
+    const GpsBigBird& b = a->bigbird;
     GPS_TRY(check_linear(b.query, "self_attn.encoder.layers.0.attention.self.query", false));
     GPS_TRY(check_linear(b.key, "self_attn.encoder.layers.0.attention.self.key", false));
     GPS_TRY(check_linear(b.value, "self_attn.encoder.layers.0.attention.self.value", false));
@@ -829,21 +821,13 @@ int dropmul_rows(const float* src, float* dst, int64_t rows, int64_t d, const Dr
   return GPS_OK;
 }
 
-// attention bias of the BiasedTransformer (gps_b200.h GpsAttnBias): checked before any CUDA call
-static int check_bias(const GpsLayerArgs* a, const GpsAttnBias* bias) {
-  if (!bias) return GPS_OK;
-  GPS_REQUIRE(a->global_type == GPS_GLOBAL_TRANSFORMER, GPS_ERR_ARG,
-              "an attention bias needs global_type GPS_GLOBAL_TRANSFORMER (got %d)", a->global_type);
-  GPS_REQUIRE(bias->nmax >= 1, GPS_ERR_ARG, "attention bias: nmax must be >= 1 (got %lld)", (long long)bias->nmax);
-  GPS_REQUIRE(bias->bias, GPS_ERR_ARG, "attention bias: null bias pointer");
-  return GPS_OK;
-}
-
 // =================================================================================== forward
-static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, const GpsGenConv* gen,
-                         const GpsPna* pna, cudaStream_t st, const GpsBigBird* bb = nullptr) {
+static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
   Plan P;
-  GPS_TRY(make_plan(a, &P, true, gat, gen, pna, bb));
+  const GpsGat& gat = a->gat;   // the local model's parameters: read when local_type selects it
+  const GpsGenConv& gen = a->genconv;
+  const GpsPna& pna = a->pna;
+  GPS_TRY(make_plan(a, &P, true));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
   GPS_REQUIRE(a->workspace_bytes >= P.fwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.fwd_bytes);
@@ -861,10 +845,10 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
   Side* sd;
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
-  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) && (P.attn || P.perf || P.bb);
+  const bool two_branches = P.loc && P.glob;
   // GPS_NORM_NONE: the producer that closes the last branch writes s = x_loc + hA with its planes (x_loc = s when the
   // local model is alone)
-  const bool local_writes_s = P.nonorm && !(P.attn || P.perf || P.bb);
+  const bool local_writes_s = P.nonorm && !P.glob;
   // GPS_NORM_NONE, attention output projection on stream sg: writes s = x + drop(.) [+ x_loc] and its planes instead of
   // hA; with a local branch, sg first waits for it
   auto close_with_s = [&](GemmParams& g, cudaStream_t sg) -> int {
@@ -903,7 +887,7 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
   }
   if (P.pna) {   // edge term of the messages, next to the node projections: q = e F^T + c, F = W_e W_enc (pna.cu)
     GPS_TRY(sd->fork(st));
-    GPS_TRY(pna_fold_fwd(pna->pre.weight, pna->pre.bias, pna->edge_encoder.weight, pna->edge_encoder.bias, d, P.de,
+    GPS_TRY(pna_fold_fwd(pna.pre.weight, pna.pre.bias, pna.edge_encoder.weight, pna.edge_encoder.bias, d, P.de,
                          P.pna_F, P.pna_c, s2));
     if (P.pna_F_p.hi) {
       ToPlanesItem it{P.pna_F, P.de, (int)d, (int)P.de, P.pna_F_p};
@@ -981,21 +965,21 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
                     stats(BN_L), st));
   } else if (P.gat) {
     // x_loc = x + drop(GATConv(x, edge_attr))  (gps_layer.py:70-74,183-189); Y = x W_src^T is column block 0 of Y1
-    GPS_TRY(gat_fold_fwd(gat->lin_edge.weight, gat->att_edge, d, P.H, P.gat_v, st));
-    GPS_TRY(gat_fwd(a->graph, d, P.H, P.Y1, P.Wy, a->edge_attr, P.gat_v, gat->att_src, gat->att_dst, gat->lin_src.bias,
+    GPS_TRY(gat_fold_fwd(gat.lin_edge.weight, gat.att_edge, d, P.H, P.gat_v, st));
+    GPS_TRY(gat_fwd(a->graph, d, P.H, P.Y1, P.Wy, a->edge_attr, P.gat_v, gat.att_src, gat.att_dst, gat.lin_src.bias,
                     a->x, gat_scores(P.gat_sc, N, E, P.H), P.xloc, P.drop(GPS_SITE_LOCAL), stats(BN_L), st));
   } else if (P.gen) {
     // u = agg + x, agg = softmax aggregation of relu(x_j + e_ij) + 1e-7 over each node's in-edges (GENConv.forward)
     GPS_TRY(genconv_fwd(a->graph, d, a->x, a->edge_attr, P.agg, P.gen_lse, P.gen_u, st, P.gen_u_p));
     // h1 = u W0^T [N, 2d], with mlp.1's column sums in training mode
-    GemmParams g = linear_fwd(P, N, 2 * d, d, {P.gen_u, d, P.gen_u_p}, {gen->lin0.weight, d, P.mlp0_p}, P.gen_h1, 2 * d);
+    GemmParams g = linear_fwd(P, N, 2 * d, d, {P.gen_u, d, P.gen_u_p}, {gen.lin0.weight, d, P.mlp0_p}, P.gen_h1, 2 * d);
     g.stats = P.train ? P.gen_fstats : nullptr;
     GPS_TRY(gemm(g, st));
     // r = relu(mlp.1(h1)) (mlp.2; mlp.3 is Dropout(0))
-    GPS_TRY(bn_act_residual(P.gen_h1, 2 * d, nullptr, P.gen_r, N, 2 * d, gen_bn_view(P, gen->bn, N), GPS_ACT_RELU,
+    GPS_TRY(bn_act_residual(P.gen_h1, 2 * d, nullptr, P.gen_r, N, 2 * d, gen_bn_view(P, gen.bn, N), GPS_ACT_RELU,
                             DropCfg(), nullptr, st, P.gen_r_p));
     // x_loc = x + drop(r W4^T)  (gps_layer.py:188-189)
-    GemmParams g2 = linear_fwd(P, N, d, 2 * d, {P.gen_r, 2 * d, P.gen_r_p}, {gen->lin1.weight, 2 * d, P.mlp4_p}, P.xloc,
+    GemmParams g2 = linear_fwd(P, N, d, 2 * d, {P.gen_r, 2 * d, P.gen_r_p}, {gen.lin1.weight, 2 * d, P.mlp4_p}, P.xloc,
                                d);
     g2.R1 = a->x; g2.ldr1 = (int)d; g2.stats = stats(BN_L);
     if (local_writes_s) g2.Cp = P.s_p;
@@ -1006,13 +990,13 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
     // P_src is column block 0 of Y1
     GPS_TRY(pna_fwd(a->graph, d, a->x, P.Y1, P.Wy, P.pna_q, P.pna_Z, P.pna_Z_p, P.pna_arg, st));
     // h = Z W_post^T + b_post
-    GemmParams g = linear_fwd(P, N, d, 4 * d, {P.pna_Z, 4 * d, P.pna_Z_p}, {pna->post.weight, 4 * d, P.post_p}, P.pna_h,
-                              d, pna->post.bias);
+    GemmParams g = linear_fwd(P, N, d, 4 * d, {P.pna_Z, 4 * d, P.pna_Z_p}, {pna.post.weight, 4 * d, P.post_p}, P.pna_h,
+                              d, pna.post.bias);
     g.Cp = P.pna_h_p;
     GPS_TRY(gemm(g, st));
     // x_loc = x + drop(h W_lin^T + b_lin)  (gps_layer.py:188-189)
-    GemmParams g2 = linear_fwd(P, N, d, d, {P.pna_h, d, P.pna_h_p}, {pna->lin.weight, d, P.lin_p}, P.xloc, d,
-                               pna->lin.bias);
+    GemmParams g2 = linear_fwd(P, N, d, d, {P.pna_h, d, P.pna_h_p}, {pna.lin.weight, d, P.lin_p}, P.xloc, d,
+                               pna.lin.bias);
     g2.R1 = a->x; g2.ldr1 = (int)d; g2.stats = stats(BN_L);
     if (local_writes_s) g2.Cp = P.s_p;
     set_dropout(g2, P.drop(GPS_SITE_LOCAL));
@@ -1029,10 +1013,10 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
     const float* Q = P.Y1 + P.qkv_off;
     if (P.attn_tc)
       GPS_TRY(attention_tc_fwd(a->graph, P.H, P.hd, P.qkv_p, P.O, d, P.O_p, P.lse, P.pa, a->seed, a->offset,
-                               (const unsigned long long*)a->offset_dev, P.prec, sg, bias));
+                               (const unsigned long long*)a->offset_dev, P.prec, sg, P.bias));
     else
       GPS_TRY(attention_fwd(a->graph, P.H, P.hd, Q, Q + d, Q + 2 * d, P.Wy, P.O, d, P.lse, P.pa, a->seed, a->offset,
-                            sg, (const unsigned long long*)a->offset_dev, P.O_p, bias));
+                            sg, (const unsigned long long*)a->offset_dev, P.O_p, P.bias));
     // hA = x + drop(O Wo^T + bo)
     GemmParams g = linear_fwd(P, N, d, d, {P.O, d, P.O_p}, {a->attn_out.weight, d, P.out_p}, P.hA, d, a->attn_out.bias);
     g.R1 = a->x; g.ldr1 = (int)d; g.stats = stats(BN_A);
@@ -1071,7 +1055,7 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
 
   // ---- BigBird global model (gps_layer.py:207-208; bigbird_layer.py:1116-1356)
   if (P.bb) {
-    const GpsBigBird& B = *bb;
+    const GpsBigBird& B = a->bigbird;
     const float* Q = P.Y1 + P.qkv_off;
     GPS_TRY(bb_attn_fwd(a->graph, P.H, P.hd, B, Q, Q + d, Q + 2 * d, P.Wy, P.O, d, P.lse, sg));
     if (P.O_p.hi && N > 0) {
@@ -1121,10 +1105,9 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
 
   // ---- s = norm1_local(x_loc) + norm1_attn(hA)   (gps_layer.py:194,217,222)
   if (!P.nonorm) {
-    const bool loc = P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna;
-    const float* first = loc ? P.xloc : P.hA;
-    BnView bf = loc ? bn_view(P, BN_L, a->norm1_local, N) : bn_view(P, BN_A, a->norm1_attn, N);
-    const float* second = (loc && (P.attn || P.perf || P.bb)) ? P.hA : nullptr;
+    const float* first = P.loc ? P.xloc : P.hA;
+    BnView bf = P.loc ? bn_view(P, BN_L, a->norm1_local, N) : bn_view(P, BN_A, a->norm1_attn, N);
+    const float* second = (P.loc && P.glob) ? P.hA : nullptr;
     BnView bs = bn_view(P, BN_A, a->norm1_attn, N);
     GPS_TRY(bn_combine(first, bf, second, bs, P.s, N, d, st, P.s_p));
   }
@@ -1152,10 +1135,12 @@ static int layer_forward(const GpsLayerArgs* a, const GpsAttnBias* bias, const G
 }
 
 // =================================================================================== backward
-static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const GpsGat* gat, const GpsGenConv* gen,
-                          const GpsPna* pna, cudaStream_t st, const GpsBigBird* bb = nullptr) {
+static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   Plan P;
-  GPS_TRY(make_plan(a, &P, true, gat, gen, pna, bb));
+  const GpsGat& gat = a->gat;   // the local model's parameters: read when local_type selects it
+  const GpsGenConv& gen = a->genconv;
+  const GpsPna& pna = a->pna;
+  GPS_TRY(make_plan(a, &P, true));
   GPS_REQUIRE(a->saved && a->workspace, GPS_ERR_ARG, "saved/workspace buffers are required");
   GPS_REQUIRE(a->workspace_bytes >= P.bwd_bytes, GPS_ERR_ARG, "workspace too small (%lld < %lld)",
               (long long)a->workspace_bytes, (long long)P.bwd_bytes);
@@ -1175,7 +1160,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
   GPS_TRY(side_stream(&sd));
   cudaStream_t s2 = sd->s;
   auto wfork = [&](cudaStream_t from) -> int { return sd->order(from, s2); };
-  const bool two_branches = (P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) && (P.attn || P.perf || P.bb);
+  const bool two_branches = P.loc && P.glob;
   cudaStream_t sa = two_branches ? sd->s3 : st;   // stream of the attention-branch backward
   cudaStream_t se = sd->s4;                       // stream of the edge BatchNorm backward (GatedGCN)
   const int opt = opt_flags();
@@ -1259,12 +1244,12 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     // reductions ride this GEMM's epilogue instead of two more passes over g_s (GPS_B200_OPT bit 64)
     fused_la = (opt & 64) && !P.nonorm && P.use_planes && g2.Ap.hi && g2.Bp.hi && N > 0 && P.train;
     if (fused_la) {
-      if (P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna) {
+      if (P.loc) {
         BnView v = bn_view(P, BN_L, a->norm1_local);
         g2.bnred[0].z = P.xloc; g2.bnred[0].ldz = (int)d; g2.bnred[0].mean = v.mean; g2.bnred[0].invstd = v.invstd;
         g2.bnred[0].sums = sums(BN_L);
       }
-      if (P.attn || P.perf || P.bb) {
+      if (P.glob) {
         BnView v = bn_view(P, BN_A, a->norm1_attn);
         g2.bnred[1].z = P.hA; g2.bnred[1].ldz = (int)d; g2.bnred[1].mean = v.mean; g2.bnred[1].invstd = v.invstd;
         g2.bnred[1].sums = sums(BN_A);
@@ -1273,10 +1258,9 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     GPS_TRY(gemm(g2, st));
   }
 
-  const bool loc = P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna;
   bool chain_x = false;
   // ---- norm1_local / norm1_attn (gps_layer.py:194,217): g_xloc, g_hA
-  if (loc && !P.nonorm) {
+  if (P.loc && !P.nonorm) {
     BnView v = bn_view(P, BN_L, a->norm1_local);
     if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.xloc, d, N, d, v, -1, nodrop, sums(BN_L), st));
     chain_x = P.gated && N > 0 && (opt & 32) && P.train;
@@ -1312,7 +1296,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     float* gQ = P.gY1 + P.qkv_off;
     GPS_TRY(attention_bwd(a->graph, P.H, P.hd, Q, Q + d, Q + 2 * d, P.Wy, P.O, P.g_O, d, P.lse, P.delta, gQ, gQ + d,
                           gQ + 2 * d, P.Wy, P.pa, a->seed, a->offset, sa, (const unsigned long long*)a->offset_dev,
-                          P.gY1_p.cols(P.qkv_off), P.gY1_p.cols(P.qkv_off + d), P.gY1_p.cols(P.qkv_off + 2 * d), bias));
+                          P.gY1_p.cols(P.qkv_off), P.gY1_p.cols(P.qkv_off + d), P.gY1_p.cols(P.qkv_off + 2 * d), P.bias));
   }
 
   if (P.perf) {
@@ -1359,7 +1343,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
   }
 
   if (P.bb) {
-    const GpsBigBird& B = *bb;
+    const GpsBigBird& B = a->bigbird;
     if (!P.nonorm) {
       BnView v = bn_view(P, BN_A, a->norm1_attn);
       if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
@@ -1399,7 +1383,7 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     GPS_TRY(gemm(linear_dgrad(P, N, d, d, g_so, {B.self_out.weight, d, P.bb_so_p}, P.g_O, d), sa));
     GPS_TRY(wfork(sa));   // the LayerNorm gradients are final here too
     GPS_TRY(linear_wgrad(P, g_so, {P.O, d, P.O_p}, N, d, d, B.self_out.grad_weight, B.self_out.grad_bias, s2));
-    if (!(P.gated || P.gine || P.gcn || P.gat || P.gen || P.pna)) GPS_TRY(mid_done());
+    if (!P.loc) GPS_TRY(mid_done());
     // block-sparse attention: dQ | dK | dV into the in_proj columns of gY1
     const float* Q = P.Y1 + P.qkv_off;
     float* gQ = P.gY1 + P.qkv_off;
@@ -1484,10 +1468,10 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     Operand g_h;
     GPS_TRY(dropmul(P, {g_xloc, d}, P.g_tmp3, Planes(), GPS_SITE_LOCAL, st, &g_h));
     float* g_v = P.gat_ws;
-    GPS_TRY(gat_bwd(a->graph, d, P.H, P.Y1, P.Wy, a->edge_attr, P.gat_v, gat->att_src, gat->att_dst,
+    GPS_TRY(gat_bwd(a->graph, d, P.H, P.Y1, P.Wy, a->edge_attr, P.gat_v, gat.att_src, gat.att_dst,
                     gat_scores(P.gat_sc, N, E, P.H), g_h.f, P.gat_ws + P.H * d, P.gY1, P.Wy, P.gY1_p, a->grad_edge_attr,
-                    g_v, gat->grad_att_src, gat->grad_att_dst, gat->lin_src.grad_bias, P.grads_accumulate, st));
-    GPS_TRY(gat_fold_bwd(gat->lin_edge.weight, gat->att_edge, g_v, d, P.H, gat->lin_edge.grad_weight, gat->grad_att_edge,
+                    g_v, gat.grad_att_src, gat.grad_att_dst, gat.lin_src.grad_bias, P.grads_accumulate, st));
+    GPS_TRY(gat_fold_bwd(gat.lin_edge.weight, gat.att_edge, g_v, d, P.H, gat.lin_edge.grad_weight, gat.grad_att_edge,
                          P.grads_accumulate, st));
     GPS_TRY(wfork(st));
     GPS_TRY(mid_done());
@@ -1497,19 +1481,19 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     Operand g_l;
     GPS_TRY(dropmul(P, {g_xloc, d, g_xloc_p}, P.g_tmp3, P.gtmp3_p, GPS_SITE_LOCAL, st, &g_l));
     // g_r = g_l W4 [N, 2d]
-    GPS_TRY(gemm(linear_dgrad(P, N, 2 * d, d, g_l, {gen->lin1.weight, 2 * d, P.mlp4_p}, P.gen_gr, 2 * d), st));
+    GPS_TRY(gemm(linear_dgrad(P, N, 2 * d, d, g_l, {gen.lin1.weight, 2 * d, P.mlp4_p}, P.gen_gr, 2 * d), st));
     // r = relu(mlp.1(h1)): g_h1 and the mlp.1 gradients
-    const BnView vb = gen_bn_view(P, gen->bn);
+    const BnView vb = gen_bn_view(P, gen.bn);
     GPS_TRY(bn_bwd_reduce(P.gen_gr, 2 * d, P.gen_h1, 2 * d, N, 2 * d, vb, GPS_ACT_RELU, nodrop, P.gen_bsums, st));
     GPS_TRY(bn_bwd_apply(P.gen_gr, 2 * d, P.gen_h1, 2 * d, N, 2 * d, vb, GPS_ACT_RELU, nodrop, P.gen_bsums, P.gen_gh1,
-                         2 * d, gen->bn.grad_weight, gen->bn.grad_bias, st, P.grads_accumulate, P.gen_gh1_p));
+                         2 * d, gen.bn.grad_weight, gen.bn.grad_bias, st, P.grads_accumulate, P.gen_gh1_p));
     const Operand g_h1{P.gen_gh1, 2 * d, P.gen_gh1_p};
     GPS_TRY(wfork(st));
-    GPS_TRY(linear_wgrad(P, g_l, {P.gen_r, 2 * d, P.gen_r_p}, N, d, 2 * d, gen->lin1.grad_weight, nullptr, s2));
-    GPS_TRY(linear_wgrad(P, g_h1, {P.gen_u, d, P.gen_u_p}, N, 2 * d, d, gen->lin0.grad_weight, nullptr, s2));
+    GPS_TRY(linear_wgrad(P, g_l, {P.gen_r, 2 * d, P.gen_r_p}, N, d, 2 * d, gen.lin1.grad_weight, nullptr, s2));
+    GPS_TRY(linear_wgrad(P, g_h1, {P.gen_u, d, P.gen_u_p}, N, 2 * d, d, gen.lin0.grad_weight, nullptr, s2));
     GPS_TRY(mid_done());
     // g_u = g_h1 W0; then grad_edge_attr (dst ordered) and g_x_local = g_u + sum_out grad_edge_attr + g_xloc
-    GPS_TRY(gemm(linear_dgrad(P, N, d, 2 * d, g_h1, {gen->lin0.weight, d, P.mlp0_p}, P.gen_gu, d), st));
+    GPS_TRY(gemm(linear_dgrad(P, N, d, 2 * d, g_h1, {gen.lin0.weight, d, P.mlp0_p}, P.gen_gu, d), st));
     GPS_TRY(genconv_bwd_dst(a->graph, d, a->x, a->edge_attr, P.agg, P.gen_lse, P.gen_gu, a->grad_edge_attr, st));
     GPS_TRY(gine_bwd_src(a->graph, d, a->grad_edge_attr, P.gen_gu, 0.f, g_xloc, P.g_xl, st));
     g_x_local = P.g_xl;
@@ -1518,16 +1502,16 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     Operand g_l;
     GPS_TRY(dropmul(P, {g_xloc, d, g_xloc_p}, P.g_tmp3, P.gtmp3_p, GPS_SITE_LOCAL, st, &g_l));
     // g_h = g_l W_lin
-    GemmParams g = linear_dgrad(P, N, d, d, g_l, {pna->lin.weight, d, P.lin_p}, P.pna_gh, d);
+    GemmParams g = linear_dgrad(P, N, d, d, g_l, {pna.lin.weight, d, P.lin_p}, P.pna_gh, d);
     g.Cp = P.pna_gh_p;
     GPS_TRY(gemm(g, st));
     const Operand g_h{P.pna_gh, d, P.pna_gh_p};
     GPS_TRY(wfork(st));
-    GPS_TRY(linear_wgrad(P, g_l, {P.pna_h, d, P.pna_h_p}, N, d, d, pna->lin.grad_weight, pna->lin.grad_bias, s2));
-    GPS_TRY(linear_wgrad(P, g_h, {P.pna_Z, 4 * d, P.pna_Z_p}, N, d, 4 * d, pna->post.grad_weight, pna->post.grad_bias,
+    GPS_TRY(linear_wgrad(P, g_l, {P.pna_h, d, P.pna_h_p}, N, d, d, pna.lin.grad_weight, pna.lin.grad_bias, s2));
+    GPS_TRY(linear_wgrad(P, g_h, {P.pna_Z, 4 * d, P.pna_Z_p}, N, d, 4 * d, pna.post.grad_weight, pna.post.grad_bias,
                          s2));
     // g_Z = g_h W_post [N, 4d]
-    GPS_TRY(gemm(linear_dgrad(P, N, 4 * d, d, g_h, {pna->post.weight, 4 * d, P.post_p}, P.pna_gZ, 4 * d), st));
+    GPS_TRY(gemm(linear_dgrad(P, N, 4 * d, d, g_h, {pna.post.weight, 4 * d, P.post_p}, P.pna_gZ, 4 * d), st));
     // g_q (every edge's g_m), g_P_dst | g_P_src -> gY1[:, 0:2d], g_x_local = g_xloc + g_Z[:, 0:d]
     GPS_TRY(pna_bwd(a->graph, d, P.pna_gZ, P.pna_arg, g_xloc, P.pna_gq, P.pna_gq_p, P.gY1, P.Wy, P.gY1_p, P.g_xl, st));
     // edge term: g_F = g_q^T e, g_c = colsum(g_q), unfolded into edge_encoder, pre's edge block and pre's bias
@@ -1537,9 +1521,9 @@ static int layer_backward(const GpsLayerArgs* a, const GpsAttnBias* bias, const 
     GPS_TRY(wfork(st));
     GPS_CUDA(cudaMemsetAsync(g_F, 0, (size_t)(d * P.de + d) * sizeof(float), s2));
     GPS_TRY(wgrad_add(P, g_q, {a->edge_attr, P.de, P.e_p}, E, d, P.de, g_F, g_c, s2));
-    GPS_TRY(pna_fold_bwd(pna->pre.weight, pna->edge_encoder.weight, pna->edge_encoder.bias, g_F, g_c, d, P.de,
-                         pna->pre.grad_weight, pna->pre.grad_bias, pna->edge_encoder.grad_weight,
-                         pna->edge_encoder.grad_bias, P.grads_accumulate, s2));
+    GPS_TRY(pna_fold_bwd(pna.pre.weight, pna.edge_encoder.weight, pna.edge_encoder.bias, g_F, g_c, d, P.de,
+                         pna.pre.grad_weight, pna.pre.grad_bias, pna.edge_encoder.grad_weight,
+                         pna.edge_encoder.grad_bias, P.grads_accumulate, s2));
     GPS_TRY(mid_done());
     // grad_edge_attr = g_q F
     if (E > 0)
@@ -1621,120 +1605,18 @@ extern "C" int gps_layer_plan(const GpsLayerArgs* args, GpsLayerPlan* plan) {
   plan->saved_bytes = P.saved_bytes;
   plan->fwd_workspace_bytes = P.fwd_bytes;
   plan->bwd_workspace_bytes = P.bwd_bytes;
-  plan->fwd_launches = 0;
-  plan->bwd_launches = 0;
   plan->wplanes_bytes = P.wplanes_bytes;
   return GPS_OK;
 }
 
 extern "C" int gps_layer_forward(const GpsLayerArgs* args, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_forward: null args");
-  return layer_forward(args, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+  return layer_forward(args, (cudaStream_t)stream);
 }
 
 extern "C" int gps_layer_backward(const GpsLayerArgs* args, void* stream) {
   GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_backward: null args");
-  return layer_backward(args, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
-}
-
-extern "C" int gps_layer_forward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream) {
-  GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_forward_biased: null args");
-  GPS_TRY(check_bias(args, bias));
-  return layer_forward(args, bias, nullptr, nullptr, nullptr, (cudaStream_t)stream);
-}
-
-extern "C" int gps_layer_backward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream) {
-  GPS_REQUIRE(args, GPS_ERR_ARG, "gps_layer_backward_biased: null args");
-  GPS_TRY(check_bias(args, bias));
-  return layer_backward(args, bias, nullptr, nullptr, nullptr, (cudaStream_t)stream);
-}
-
-static int check_gat(const GpsLayerArgs* a, const GpsGat* gat, const char* what) {
-  GPS_REQUIRE(a && gat, GPS_ERR_ARG, "%s: null args / gat", what);
-  GPS_REQUIRE(a->local_type == GPS_LOCAL_GAT, GPS_ERR_ARG, "%s: a GpsGat needs local_type GPS_LOCAL_GAT (got %d)", what,
-              a->local_type);
-  return GPS_OK;
-}
-
-extern "C" int gps_layer_forward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias, void* stream) {
-  GPS_TRY(check_gat(args, gat, "gps_layer_forward_gat"));
-  GPS_TRY(check_bias(args, bias));
-  return layer_forward(args, bias, gat, nullptr, nullptr, (cudaStream_t)stream);
-}
-
-extern "C" int gps_layer_backward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias,
-                                      void* stream) {
-  GPS_TRY(check_gat(args, gat, "gps_layer_backward_gat"));
-  GPS_TRY(check_bias(args, bias));
-  return layer_backward(args, bias, gat, nullptr, nullptr, (cudaStream_t)stream);
-}
-
-static int check_genconv(const GpsLayerArgs* a, const GpsGenConv* gen, const char* what) {
-  GPS_REQUIRE(a && gen, GPS_ERR_ARG, "%s: null args / gen", what);
-  GPS_REQUIRE(a->local_type == GPS_LOCAL_GENCONV, GPS_ERR_ARG,
-              "%s: a GpsGenConv needs local_type GPS_LOCAL_GENCONV (got %d)", what, a->local_type);
-  return GPS_OK;
-}
-
-extern "C" int gps_layer_forward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias,
-                                         void* stream) {
-  GPS_TRY(check_genconv(args, gen, "gps_layer_forward_genconv"));
-  GPS_TRY(check_bias(args, bias));
-  return layer_forward(args, bias, nullptr, gen, nullptr, (cudaStream_t)stream);
-}
-
-extern "C" int gps_layer_backward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias,
-                                          void* stream) {
-  GPS_TRY(check_genconv(args, gen, "gps_layer_backward_genconv"));
-  GPS_TRY(check_bias(args, bias));
-  return layer_backward(args, bias, nullptr, gen, nullptr, (cudaStream_t)stream);
-}
-
-static int check_pna(const GpsLayerArgs* a, const GpsPna* pna, const char* what) {
-  GPS_REQUIRE(a && pna, GPS_ERR_ARG, "%s: null args / pna", what);
-  GPS_REQUIRE(a->local_type == GPS_LOCAL_PNA, GPS_ERR_ARG, "%s: a GpsPna needs local_type GPS_LOCAL_PNA (got %d)", what,
-              a->local_type);
-  return GPS_OK;
-}
-
-extern "C" int gps_layer_forward_pna(const GpsLayerArgs* args, const GpsPna* pna, const GpsAttnBias* bias,
-                                     void* stream) {
-  GPS_TRY(check_pna(args, pna, "gps_layer_forward_pna"));
-  GPS_TRY(check_bias(args, bias));
-  return layer_forward(args, bias, nullptr, nullptr, pna, (cudaStream_t)stream);
-}
-
-extern "C" int gps_layer_backward_pna(const GpsLayerArgs* args, const GpsPna* pna, const GpsAttnBias* bias,
-                                      void* stream) {
-  GPS_TRY(check_pna(args, pna, "gps_layer_backward_pna"));
-  GPS_TRY(check_bias(args, bias));
-  return layer_backward(args, bias, nullptr, nullptr, pna, (cudaStream_t)stream);
-}
-
-static int check_bigbird(const GpsLayerArgs* a, const GpsBigBird* bb, const GpsGat* gat, const GpsGenConv* gen,
-                         const GpsPna* pna, const char* what) {
-  GPS_REQUIRE(a && bb, GPS_ERR_ARG, "%s: null args / bb", what);
-  GPS_REQUIRE(a->global_type == GPS_GLOBAL_BIGBIRD, GPS_ERR_ARG,
-              "%s: a GpsBigBird needs global_type GPS_GLOBAL_BIGBIRD (got %d)", what, a->global_type);
-  GPS_TRY(bb_check(a->d, a->heads, bb));
-  GPS_REQUIRE((a->local_type == GPS_LOCAL_GAT) == (gat != nullptr) &&
-                  (a->local_type == GPS_LOCAL_GENCONV) == (gen != nullptr) &&
-                  (a->local_type == GPS_LOCAL_PNA) == (pna != nullptr),
-              GPS_ERR_ARG, "%s: the local model's struct (gat / gen / pna) must match local_type %d", what,
-              a->local_type);
-  return GPS_OK;
-}
-
-extern "C" int gps_layer_forward_bigbird(const GpsLayerArgs* args, const GpsBigBird* bb, const GpsGat* gat,
-                                         const GpsGenConv* gen, const GpsPna* pna, void* stream) {
-  GPS_TRY(check_bigbird(args, bb, gat, gen, pna, "gps_layer_forward_bigbird"));
-  return layer_forward(args, nullptr, gat, gen, pna, (cudaStream_t)stream, bb);
-}
-
-extern "C" int gps_layer_backward_bigbird(const GpsLayerArgs* args, const GpsBigBird* bb, const GpsGat* gat,
-                                          const GpsGenConv* gen, const GpsPna* pna, void* stream) {
-  GPS_TRY(check_bigbird(args, bb, gat, gen, pna, "gps_layer_backward_bigbird"));
-  return layer_backward(args, nullptr, gat, gen, pna, (cudaStream_t)stream, bb);
+  return layer_backward(args, (cudaStream_t)stream);
 }
 
 // ---- stage entry points of the BigBird global model (bigbird.cu)

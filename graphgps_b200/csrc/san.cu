@@ -625,8 +625,8 @@ int make_plan(const GpsSanArgs* a, SanPlan* P, bool bind) {
   P->prec = a->precision;
   P->gamma = a->gamma;
   P->train = a->training != 0;
-  P->grads_accumulate = (a->flags & 2) != 0;
-  P->grads_prezeroed = (a->flags & 1) != 0 || P->grads_accumulate;
+  P->grads_accumulate = (a->flags & GPS_FLAG_GRADS_ACCUMULATE) != 0;
+  P->grads_prezeroed = (a->flags & GPS_FLAG_GRADS_ZEROED) != 0 || P->grads_accumulate;
   auto drop = [&](int site) {
     DropCfg c;
     c.p = P->train ? a->dropout : 0.f;

@@ -8,7 +8,7 @@ graphgps/train/custom_train.py:32-38; the reference itself has no distributed co
 
 `GradBucket` is the product path: ONE static flat fp32 buffer holds the gradients of a set of layers;
 every parameter's `.grad` is a view of it and `gps_layer_backward` adds its gradients straight into
-those views (GpsLayerArgs.reserved0 bit 1).  CUDA-graph replays, the optimiser and the collective
+those views (GpsLayerArgs.flags, GPS_FLAG_GRADS_ACCUMULATE).  CUDA-graph replays, the optimiser and the collective
 therefore all see the same memory: the all-reduce runs in place on the bucket (ReduceOp.AVG on NCCL,
 no copy-in / scale / copy-out) and can be captured in the same CUDA graph as the step.  Parameters are
 laid out in three contiguous groups per layer in the order the backward pass finishes them - "early" (FFN,

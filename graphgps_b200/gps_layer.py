@@ -28,8 +28,8 @@ _KNOWN_LOCAL = _SUPPORTED_LOCAL + ("GIN",)
 _SUPPORTED_GLOBAL = ("None", "Transformer", "BiasedTransformer", "Performer", "BigBird")
 _KNOWN_GLOBAL = _SUPPORTED_GLOBAL
 _MHA_GLOBAL = ("Transformer", "BiasedTransformer")   # torch's MultiheadAttention (gps_layer.py:104-106)
-# the library's global model: BiasedTransformer is the Transformer called with a GpsAttnBias
-_GLOBAL_ABI = dict(_lib.GLOBAL, BiasedTransformer=_lib.GLOBAL["Transformer"], BigBird=_lib.GLOBAL_BIGBIRD)
+# the library's global model: BiasedTransformer is the Transformer with GpsLayerArgs.attn_bias set
+_GLOBAL_ABI = dict(_lib.GLOBAL, BiasedTransformer=_lib.GLOBAL["Transformer"])
 _ACT_MODULES = {"relu": nn.ReLU, "gelu": nn.GELU}
 
 _workspaces = {}
@@ -252,14 +252,11 @@ class _GPSLayerFn(torch.autograd.Function):
         named = dict(zip(layer._param_names, params))
         pe_k = pe.shape[1] if layer._eslap else 0
         args = layer._base_args(gs, named, pe_k=pe_k)
-        if pe_k:
-            args.pe = pe.data_ptr()
-        N, E, d = gs.N, gs.E, layer.dim_h
+        ctx.nmax = gs.nmax if bias.numel() else 0
+        ctx.bb = layer.__dict__.pop("_bb_lists", None)
+        layer._batch_args(args, pe, bias, ctx.nmax, ctx.bb)
         x_out = torch.empty_like(x)
         e_out = torch.empty_like(e) if layer.local_gnn_type == "CustomGatedGCN" else None
-        gat = layer._gat_args(named) if layer.local_gnn_type == "GAT" else None
-        gen = layer._genconv_args(named) if layer.local_gnn_type == "GENConv" else None
-        pna = layer._pna_args(named) if layer.local_gnn_type == "PNA" else None
         plan = layer._plan(args, gs)
         saved = torch.empty(max(plan[0], 256), dtype=torch.uint8, device=dev)
         ws = _workspace(dev, plan[1])
@@ -273,28 +270,7 @@ class _GPSLayerFn(torch.autograd.Function):
             snap = _next_dropout_offset(dev)
             args.offset, args.offset_dev = 0, snap.data_ptr()
         stream = torch.cuda.current_stream(dev).cuda_stream
-        ctx.nmax = gs.nmax if bias.numel() else 0
-        ctx.bb = layer.__dict__.pop("_bb_lists", None)
-        if ctx.bb is not None:
-            bbs = layer._bigbird_args(named, None, *ctx.bb)
-            _lib.check(lib.gps_layer_forward_bigbird(C.byref(args), C.byref(bbs), gat and C.byref(gat),
-                                                     gen and C.byref(gen), pna and C.byref(pna), stream),
-                       "gps_layer_forward_bigbird")
-        elif gat is not None:
-            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)) if ctx.nmax else None
-            _lib.check(lib.gps_layer_forward_gat(C.byref(args), C.byref(gat), ab, stream), "gps_layer_forward_gat")
-        elif gen is not None:
-            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)) if ctx.nmax else None
-            _lib.check(lib.gps_layer_forward_genconv(C.byref(args), C.byref(gen), ab, stream),
-                       "gps_layer_forward_genconv")
-        elif pna is not None:
-            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)) if ctx.nmax else None
-            _lib.check(lib.gps_layer_forward_pna(C.byref(args), C.byref(pna), ab, stream), "gps_layer_forward_pna")
-        elif ctx.nmax:
-            ab = _lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)
-            _lib.check(lib.gps_layer_forward_biased(C.byref(args), C.byref(ab), stream), "gps_layer_forward_biased")
-        else:
-            _lib.check(lib.gps_layer_forward(C.byref(args), stream), "gps_layer_forward")
+        _lib.check(lib.gps_layer_forward(C.byref(args), stream), "gps_layer_forward")
         ctx.layer, ctx.gs, ctx.saved_buf, ctx.snap = layer, gs, saved, snap
         ctx.hand = hand
         ctx.seed, ctx.offset, ctx.training = args.seed, args.offset, bool(args.training)
@@ -318,18 +294,20 @@ class _GPSLayerFn(torch.autograd.Function):
             # gradient all-reduce see the same memory
             grads = bucket
             args = layer._base_args(gs, named, grads, pe_k=pe_k)
-            args.reserved0 = 3
+            args.flags = _lib.FLAG_GRADS_ACCUMULATE
         else:
             grads = {n: torch.empty_like(p) for n, p in named.items()}
             torch._foreach_zero_(list(grads.values()))   # one multi-tensor fill; the library then skips its memsets
             args = layer._base_args(gs, named, grads, pe_k=pe_k)
-            args.reserved0 = 1
+            args.flags = _lib.FLAG_GRADS_ZEROED
         g_pe = None
-        if pe_k:
-            args.pe = pe.data_ptr()
-            if ctx.needs_input_grad[4]:
-                g_pe = torch.empty_like(pe)
-                args.grad_pe = g_pe.data_ptr()
+        if pe_k and ctx.needs_input_grad[4]:
+            g_pe = torch.empty_like(pe)
+            args.grad_pe = g_pe.data_ptr()
+        g_bias = None
+        if ctx.nmax and ctx.needs_input_grad[5]:
+            g_bias = torch.empty_like(bias)
+        layer._batch_args(args, pe, bias, ctx.nmax, ctx.bb, g_bias)
         args.seed, args.offset, args.training = ctx.seed, ctx.offset, 1 if ctx.training else 0
         if ctx.snap is not None:
             args.offset_dev = ctx.snap.data_ptr()
@@ -354,35 +332,7 @@ class _GPSLayerFn(torch.autograd.Function):
         if evs is not None:
             args.ev_grads_early, args.ev_grads_mid, args.ev_grads_done = (e.cuda_event for e in evs)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        g_bias = None
-        if ctx.nmax and ctx.needs_input_grad[5]:
-            g_bias = torch.empty_like(bias)
-        if ctx.bb is not None:
-            bbs = layer._bigbird_args(named, grads, *ctx.bb)
-            gat = layer._gat_args(named, grads) if layer.local_gnn_type == "GAT" else None
-            gen = layer._genconv_args(named, grads) if layer.local_gnn_type == "GENConv" else None
-            pna = layer._pna_args(named, grads) if layer.local_gnn_type == "PNA" else None
-            _lib.check(lib.gps_layer_backward_bigbird(C.byref(args), C.byref(bbs), gat and C.byref(gat),
-                                                      gen and C.byref(gen), pna and C.byref(pna), stream),
-                       "gps_layer_backward_bigbird")
-        elif layer.local_gnn_type == "GAT":
-            gat = layer._gat_args(named, grads)
-            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))) if ctx.nmax else None
-            _lib.check(lib.gps_layer_backward_gat(C.byref(args), C.byref(gat), ab, stream), "gps_layer_backward_gat")
-        elif layer.local_gnn_type == "GENConv":
-            gen = layer._genconv_args(named, grads)
-            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))) if ctx.nmax else None
-            _lib.check(lib.gps_layer_backward_genconv(C.byref(args), C.byref(gen), ab, stream),
-                       "gps_layer_backward_genconv")
-        elif layer.local_gnn_type == "PNA":
-            pna = layer._pna_args(named, grads)
-            ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))) if ctx.nmax else None
-            _lib.check(lib.gps_layer_backward_pna(C.byref(args), C.byref(pna), ab, stream), "gps_layer_backward_pna")
-        elif ctx.nmax:
-            ab = _lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))
-            _lib.check(lib.gps_layer_backward_biased(C.byref(args), C.byref(ab), stream), "gps_layer_backward_biased")
-        else:
-            _lib.check(lib.gps_layer_backward(C.byref(args), stream), "gps_layer_backward")
+        _lib.check(lib.gps_layer_backward(C.byref(args), stream), "gps_layer_backward")
         # (ctx.saved_buf stays alive with the autograd node: backward(retain_graph=True) may run again)
         if bucket is not None:
             return (None, None, g_x, g_e, g_pe, g_bias) + (None,) * len(layer._param_names)
@@ -668,6 +618,19 @@ class GPSLayer(nn.Module):
         elif self.local_gnn_type == "GCN":
             a.gcn_conv = _lin(named["local_model.lin.weight"], named["local_model.bias"],
                               g.get("local_model.lin.weight"), g.get("local_model.bias"))
+        elif self.local_gnn_type == "GAT":   # lin_src carries GATConv.bias, as GCNConv's lin / bias pair
+            p = "local_model."
+            a.gat = _lib.GpsGat(
+                _lin(named[p + "lin_src.weight"], named[p + "bias"], g.get(p + "lin_src.weight"), g.get(p + "bias")),
+                lin(p + "lin_edge", False),
+                *(_lib.ptr(named[p + n]) for n in ("att_src", "att_dst", "att_edge")),
+                *(_lib.ptr(g.get(p + n)) for n in ("att_src", "att_dst", "att_edge")))
+        elif self.local_gnn_type == "GENConv":
+            a.genconv = _lib.GpsGenConv(lin("local_model.mlp.0", False), bn("local_model.mlp.1", self.local_model.mlp[1]),
+                                        lin("local_model.mlp.4", False))
+        elif self.local_gnn_type == "PNA":
+            a.pna = _lib.GpsPna(lin("local_model.edge_encoder"), lin("local_model.pre_nns.0.0"),
+                                lin("local_model.post_nns.0.0"), lin("local_model.lin"), self.local_model.edge_dim)
         if self.global_model_type in _MHA_GLOBAL:
             a.attn_in = _lin(named["self_attn.in_proj_weight"], named["self_attn.in_proj_bias"],
                              g.get("self_attn.in_proj_weight"), g.get("self_attn.in_proj_bias"))
@@ -678,6 +641,8 @@ class GPSLayer(nn.Module):
             a.attn_out = lin("self_attn.to_out")
             pm = self.self_attn.fast_attention.projection_matrix
             a.perf_proj, a.perf_features, a.perf_dim_head = pm.data_ptr(), pm.shape[0], pm.shape[1]
+        elif self.global_model_type == "BigBird":   # num_blocks and the block lists are set per batch
+            a.bigbird = gps_bigbird(self.self_attn, named, grads, "self_attn.")
         if self.batch_norm:   # else the three structs stay zero: the library does not read them
             a.norm1_local = bn("norm1_local", self.norm1_local)
             a.norm1_attn = bn("norm1_attn", self.norm1_attn)
@@ -685,31 +650,18 @@ class GPSLayer(nn.Module):
         a.ff1, a.ff2 = lin("ff_linear1"), lin("ff_linear2")
         return a
 
-    def _gat_args(self, named, grads=None):
-        """GpsGat of the GAT local model (gps_b200.h): lin_src carries GATConv.bias, as GCNConv's lin / bias pair."""
-        g = grads or {}
-        p = "local_model."
-        return _lib.GpsGat(
-            _lin(named[p + "lin_src.weight"], named[p + "bias"], g.get(p + "lin_src.weight"), g.get(p + "bias")),
-            _lin(named[p + "lin_edge.weight"], None, g.get(p + "lin_edge.weight")),
-            *(_lib.ptr(named[p + n]) for n in ("att_src", "att_dst", "att_edge")),
-            *(_lib.ptr(g.get(p + n)) for n in ("att_src", "att_dst", "att_edge")))
-
-    def _genconv_args(self, named, grads=None):
-        """GpsGenConv of the GENConv local model (gps_b200.h): mlp.0, mlp.1 (with its running statistics), mlp.4."""
-        g = grads or {}
-        p = "local_model.mlp."
-        bn = self.local_model.mlp[1]
-        return _lib.GpsGenConv(
-            _lin(named[p + "0.weight"], None, g.get(p + "0.weight")),
-            _lib.GpsBatchNorm(_lib.ptr(named[p + "1.weight"]), _lib.ptr(named[p + "1.bias"]), _lib.ptr(bn.running_mean),
-                              _lib.ptr(bn.running_var), _lib.ptr(bn.num_batches_tracked),
-                              _lib.ptr(g.get(p + "1.weight")), _lib.ptr(g.get(p + "1.bias"))),
-            _lin(named[p + "4.weight"], None, g.get(p + "4.weight")))
-
-    def _bigbird_args(self, named, grads, lists, nb):
-        """GpsBigBird of the BigBird global model (gps_b200.h) for a batch of nb blocks."""
-        return gps_bigbird(self.self_attn, named, grads, "self_attn.", lists, nb)
+    def _batch_args(self, args, pe, bias, nmax, bb, g_bias=None):
+        """Fills the fields of args that change with every batch, and so never enter the cached struct: the
+        EquivStableLapPE pointer, the BiasedTransformer's attention bias and BigBird's block count and lists."""
+        if self._eslap:
+            args.pe = pe.data_ptr()
+        if nmax:
+            args.attn_bias = _lib.GpsAttnBias(bias.data_ptr(), nmax, _lib.ptr(g_bias))
+        if bb is not None:
+            lists, nb = bb
+            b = args.bigbird   # a view into args
+            b.num_blocks = nb
+            b.key_ptr, b.key_idx, b.query_ptr, b.query_idx = (t.data_ptr() for t in lists)
 
     def _bigbird_lists(self, x, gs):
         """(block lists, nb) of this batch: nb from Nmax padded to the block size; NotImplementedError (before any
@@ -719,17 +671,6 @@ class GPSLayer(nn.Module):
         lists = device_lists(x.device, nb, self.num_heads, cfg.block_size, cfg.num_random_blocks,
                              cfg.max_position_embeddings)
         return lists, nb
-
-    def _pna_args(self, named, grads=None):
-        """GpsPna of the PNA local model (gps_b200.h): edge_encoder, pre_nns.0.0, post_nns.0.0, lin and the edge width."""
-        g = grads or {}
-
-        def lin(prefix):
-            p = "local_model." + prefix
-            return _lin(named[p + ".weight"], named[p + ".bias"], g.get(p + ".weight"), g.get(p + ".bias"))
-
-        return _lib.GpsPna(lin("edge_encoder"), lin("pre_nns.0.0"), lin("post_nns.0.0"), lin("lin"),
-                           self.local_model.edge_dim)
 
     @property
     def _gine_eps_host(self):

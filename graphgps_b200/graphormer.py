@@ -64,7 +64,7 @@ class _GraphormerFn(torch.autograd.Function):
         grads = {n: torch.empty_like(p) for n, p in named.items()}
         torch._foreach_zero_(list(grads.values()))   # one multi-tensor fill; the library then skips its memsets
         args = layer._args(gs, named, grads)
-        args.flags = 1
+        args.flags = _lib.FLAG_GRADS_ZEROED
         args.seed, args.offset, args.training = ctx.seed, ctx.offset, 1 if ctx.training else 0
         if ctx.snap is not None:
             args.offset_dev = ctx.snap.data_ptr()

@@ -75,7 +75,7 @@ class _SANFn(torch.autograd.Function):
                 grads[n] = torch.empty_like(p)
         torch._foreach_zero_([packed] + [g for n, g in grads.items() if n not in _NODE])
         args = layer._args(gs, ctx.nmax, named, grads)
-        args.flags = 1
+        args.flags = _lib.FLAG_GRADS_ZEROED
         args.seed, args.offset, args.training = ctx.seed, ctx.offset, 1 if ctx.training else 0
         if ctx.snap is not None:
             args.offset_dev = ctx.snap.data_ptr()

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define GPS_ABI_VERSION 3
+#define GPS_ABI_VERSION 4
 
 enum { GPS_OK = 0, GPS_ERR_ARG = -1, GPS_ERR_UNSUPPORTED = -2, GPS_ERR_CUDA = -3 };
 
@@ -39,7 +39,7 @@ enum { GPS_OK = 0, GPS_ERR_ARG = -1, GPS_ERR_UNSUPPORTED = -2, GPS_ERR_CUDA = -3
 enum { GPS_LOCAL_NONE = 0, GPS_LOCAL_GATEDGCN = 1, GPS_LOCAL_GINE = 2, GPS_LOCAL_GCN = 3, GPS_LOCAL_GAT = 4,
        GPS_LOCAL_GENCONV = 5, GPS_LOCAL_PNA = 6 };
 enum { GPS_GLOBAL_NONE = 0, GPS_GLOBAL_TRANSFORMER = 1, GPS_GLOBAL_PERFORMER = 2,
-       GPS_GLOBAL_BIGBIRD = 3 /* gps_layer_{forward,backward}_bigbird only */ };
+       GPS_GLOBAL_BIGBIRD = 3 };
 /* register.act_dict keys used by shipped configs (gps_layer.py:33) */
 enum { GPS_ACT_RELU = 0, GPS_ACT_GELU = 1 };
 /* arithmetic of the dense products: FP32 = fp32-grade result (split-bf16 x3 on the tensor cores,
@@ -124,8 +124,125 @@ typedef struct {
 
 /* ------------------------------------------------------------------------------------------
  * GPSLayer forward / backward  (gps_layer.py:155-257; GatedGCN gatedgcn_layer.py:45-136)
- * state_dict names in comments are the reference's (SURVEY.md §8b).
+ * state_dict names in comments are the reference's (SURVEY.md §8b).  GpsLayerArgs carries every local and global
+ * model; local_type / global_type choose which of its members are read.  The structs below are members of it.
  * ---------------------------------------------------------------------------------------- */
+
+/* Additive attention bias of the BiasedTransformer global model (gps_layer.py:104-106,202-204,234-241; Graphormer's
+ * batch.attn_bias): bias [B*heads, nmax, nmax] row-major float32, row g*heads + h of graph g and head h, entry (il, jl)
+ * for local query il and local key jl; nmax >= the largest graph of the batch (to_dense_batch's Nmax).  The scores
+ * become S = (q . k) / sqrt(hd) + bias[g*heads + h, il, jl]; padded entries (il or jl >= n_g) are not read.  grad_bias
+ * (backward; NULL = not needed) has the same layout and is written whole: dL/dS at every in-graph entry, 0 at every
+ * padded one. */
+typedef struct {
+  const float* bias;
+  int64_t nmax;
+  float* grad_bias;
+} GpsAttnBias;
+
+/* GAT local model (local_type == GPS_LOCAL_GAT): PyG 2.2 GATConv(dim_h, dim_h / heads, heads=heads, edge_dim=dim_h)
+ * with its defaults (concat, negative_slope 0.2, no attention dropout, add_self_loops with fill_value 'mean', bias),
+ * gps_layer.py:70-74,183-189.  H = GpsLayerArgs.heads heads of C = d / H channels each (d % H != 0 is GPS_ERR_ARG).
+ * Existing self-loop edges are dropped and one loop per node is added whose edge attribute is the mean of the node's
+ * remaining in-edge attributes (0 without any); their grad_edge_attr rows are 0.  edge_attr and, in the backward,
+ * grad_edge_attr are required (non-NULL when E > 0) and batch.edge_attr is not updated.  Parameters (non-NULL, else
+ * GPS_ERR_ARG):
+ *   lin_src   weight = local_model.lin_src.weight [d,d] (lin_dst is the same module), bias = local_model.bias [d]
+ *             (added after the aggregation); its gradients: grad_weight with the fused node projection (final at
+ *             ev_grads_done), grad_bias final at ev_grads_mid;
+ *   lin_edge  weight = local_model.lin_edge.weight [d,d] (no bias);
+ *   att_src / att_dst / att_edge = local_model.att_{src,dst,edge} [1,H,C], and their gradients, final at ev_grads_mid. */
+typedef struct {
+  GpsLinear lin_src;
+  GpsLinear lin_edge;
+  const float* att_src;
+  const float* att_dst;
+  const float* att_edge;
+  float* grad_att_src;
+  float* grad_att_dst;
+  float* grad_att_edge;
+} GpsGat;
+
+/* GENConv local model (local_type == GPS_LOCAL_GENCONV): PyG 2.2 GENConv(dim_h, dim_h) with its defaults (softmax
+ * aggregation with t = 1, no message norm, eps 1e-7, MLP d -> 2d -> d with BatchNorm, no bias), gps_layer.py:60-61,
+ * 183-189.  For target i and channel c: m_k = relu(x[src_k] + e_k) + 1e-7, agg_i = sum_k softmax_k(m)_c m_kc over i's
+ * in-edges (0 without any; self loops and duplicates are ordinary edges), u = agg + x and
+ * h = lin1(relu(bn(lin0(u)))); x_loc = x + dropout(h).  edge_attr [E, d] and, in the backward, grad_edge_attr are
+ * required (non-NULL when E > 0) and batch.edge_attr is not updated.  d % 4 == 0 and d <= 2048 (the 2d-wide BatchNorm
+ * runs on the row-wise stages), else GPS_ERR_UNSUPPORTED.  Parameters (all non-NULL, else GPS_ERR_ARG), whose
+ * gradients are final at ev_grads_mid:
+ *   lin0 = local_model.mlp.0 [2d, d], bias NULL;
+ *   bn   = local_model.mlp.1 [2d]: weight, bias, running_mean, running_var (num_batches_tracked optional); training
+ *          mode normalises with the batch statistics and updates the running ones as torch.nn.BatchNorm1d;
+ *   lin1 = local_model.mlp.4 [d, 2d], bias NULL.  The MLP's activation is ReLU whatever GpsLayerArgs.act is. */
+typedef struct {
+  GpsLinear lin0;
+  GpsBatchNorm bn;
+  GpsLinear lin1;
+} GpsGenConv;
+
+/* PNA local model (local_type == GPS_LOCAL_PNA): PyG 2.2 PNAConv(dim_h, dim_h, aggregators=['mean','max','sum'],
+ * scalers=['identity'], edge_dim=edge_dim, towers=1, pre_layers=1, post_layers=1, divide_input=False),
+ * gps_layer.py:75-90,183-189.  For edge k from j to i:
+ *   m_k = pre.weight [x_i ; x_j ; edge_encoder(e_k)] + pre.bias
+ * and per target i and channel the mean, max and sum of m over i's in-edges (0 in all three without any; self loops
+ * and duplicates are ordinary edges); x_loc = x + dropout(lin(post([x | mean | max | sum]))).  The max gradient goes
+ * whole to the first maximising in-edge in edge_index order (torch_scatter's scatter_max).  The degree histogram never
+ * enters the arithmetic with the identity scaler, so it is not an argument.  edge_attr and grad_edge_attr are
+ * [E, edge_dim] and required (non-NULL when E > 0); batch.edge_attr is not updated.  0 < edge_dim <= d and
+ * edge_dim % 4 == 0, else GPS_ERR_UNSUPPORTED; gps_layer_plan does not read edge_dim and sizes for its bound d.
+ * Parameters (weights and biases non-NULL, else GPS_ERR_ARG):
+ *   edge_encoder = local_model.edge_encoder [d, edge_dim] + [d]; gradients final at ev_grads_mid;
+ *   pre  = local_model.pre_nns.0.0 [d, 3d] + [d] (column blocks: destination, source, encoded edge); gradients final
+ *          at ev_grads_done (the first two blocks come with the fused node projection);
+ *   post = local_model.post_nns.0.0 [d, 4d] + [d]; gradients final at ev_grads_mid;
+ *   lin  = local_model.lin [d, d] + [d]; gradients final at ev_grads_mid. */
+typedef struct {
+  GpsLinear edge_encoder;
+  GpsLinear pre;
+  GpsLinear post;
+  GpsLinear lin;
+  int64_t edge_dim;
+} GpsPna;
+
+/* BigBird global model (global_type == GPS_GLOBAL_BIGBIRD): the reference's SingleBigBirdLayer, one BigBirdLayer with
+ * block-sparse self-attention (gps_layer.py:115-119,207-208; bigbird_layer.py:1667-1706).  For graph g of n_g nodes,
+ * local position p is node graph_ptr[g] + p; the batch is padded to S = num_blocks * block_size positions (to_dense_batch's
+ * Nmax rounded up to the block size) and positions >= n_g are masked keys, never queries.  Head h of query block i
+ * attends to the multiset of key blocks key_idx[key_ptr[h*(nb+1) + i] .. key_ptr[h*(nb+1) + i + 1]) (a block listed
+ * twice counts twice in the softmax); query_ptr / query_idx is its transpose (the query blocks of every key block, in
+ * ascending order, with the same multiplicities).  nb = num_blocks >= 4, block_size >= 1 and the four lists non-NULL,
+ * else GPS_ERR_ARG.  Scale 1/sqrt(hd), hd = d / heads (any hd >= 1 up to 128; d % heads != 0 is GPS_ERR_ARG), no
+ * attention dropout.  With ctx the attention output [N, d]:
+ *   a   = LN1(drop_8(ctx Wso^T + bso) + x)          (attention.output; dropout site 8 = GPS_SITE_BB_SELF_OUT)
+ *   u   = act(a Wi^T + bi)                           (intermediate; act = hidden_act: 0 relu, 1 sigmoid)
+ *   out = LN2(drop_9(u Wo^T + bo) + a)               (output; dropout site 9 = GPS_SITE_BB_OUTPUT)
+ * LN = nn.LayerNorm(d, eps = ln_eps) over each row; both dropouts use GpsLayerArgs.dropout.  out then takes the place of
+ * the attention output in the GPS layer: hA = x + drop_4(out), norm1_attn, as for the Transformer.  Parameters
+ * (self_attn.encoder.layers.0.*; weights [d, d]; non-NULL, else GPS_ERR_ARG): query / key / value =
+ * attention.self.{query,key,value} (bias NULL unless use_bias), self_out = attention.output.dense, ln1 =
+ * attention.output.LayerNorm (weight = gamma, bias = beta), intermediate = intermediate.dense, output = output.dense,
+ * ln2 = output.LayerNorm.  Gradients: query / key / value are final at ev_grads_done (one weight-gradient product with
+ * the node projections); the other five at ev_grads_mid.  gps_layer_plan sizes BigBird from N, d and heads alone. */
+enum { GPS_BIGBIRD_RELU = 0, GPS_BIGBIRD_SIGMOID = 1 };
+typedef struct {
+  int64_t block_size;
+  int64_t num_blocks;          /* nb of the batch: ceil(Nmax / block_size) */
+  int32_t hidden_act;          /* GPS_BIGBIRD_* */
+  float ln_eps;                /* layer_norm_eps */
+  const int32_t* key_ptr;      /* [heads * (nb + 1)], offsets into key_idx */
+  const int32_t* key_idx;
+  const int32_t* query_ptr;    /* [heads * (nb + 1)], offsets into query_idx */
+  const int32_t* query_idx;
+  GpsLinear query, key, value, self_out, ln1, intermediate, output, ln2;
+} GpsBigBird;
+
+/* GpsLayerArgs.flags (backward) */
+enum {
+  GPS_FLAG_GRADS_ZEROED = 1,     /* the parameter-gradient buffers are already zero */
+  GPS_FLAG_GRADS_ACCUMULATE = 2  /* parameter gradients are added to the buffers (implies GPS_FLAG_GRADS_ZEROED) */
+};
+
 typedef struct {
   /* configuration */
   int64_t d;                 /* dim_h                                               */
@@ -135,17 +252,17 @@ typedef struct {
   int32_t act;               /* GPS_ACT_*                                           */
   int32_t training;          /* 1: batch statistics + dropout; 0: running stats     */
   int32_t precision;         /* GPS_PREC_*                                          */
-  int32_t reserved0;         /* flags; bit 0 (backward): parameter-gradient buffers are already zero; bit 1: gradients are added to the buffers */
+  int32_t flags;             /* GPS_FLAG_* (backward)                               */
   float dropout;             /* cfg.gt.dropout       (gps_layer.py:92-96,139-140,152-153) */
   float attn_dropout;        /* cfg.gt.attn_dropout  (gps_layer.py:105-106,112-114)       */
   uint64_t seed;             /* Philox key for this call's dropout masks            */
   uint64_t offset;           /* Philox counter base (caller advances per call)      */
   float gine_eps;            /* local_model.eps buffer value (GINE)                 */
-  /* ABI 3 (formerly reserved1, zero in every earlier caller): normalisation of the GPSLayer (gps_layer.py:125-151,
-   * 191-229), GPS_NORM_*.  BATCH: norm1_local, norm1_attn and norm2 are BatchNorm1d.  NONE (batch_norm=False,
-   * layer_norm=False): the three modules do not exist and are not read; x_loc = x + local(x), hA = x + MHA(x),
-   * s = x_loc + hA, x_out = s + FFN(s).  GatedGCN's bn_node_x / bn_edge_e belong to the local model and are required
-   * in both modes.  Any other value makes gps_layer_plan / _forward / _backward return GPS_ERR_UNSUPPORTED. */
+  /* normalisation of the GPSLayer (gps_layer.py:125-151, 191-229), GPS_NORM_*.  BATCH: norm1_local, norm1_attn and
+   * norm2 are BatchNorm1d.  NONE (batch_norm=False, layer_norm=False): the three modules do not exist and are not read;
+   * x_loc = x + local(x), hA = x + MHA(x), s = x_loc + hA, x_out = s + FFN(s).  GatedGCN's bn_node_x / bn_edge_e belong
+   * to the local model and are required in both modes.  Any other value makes gps_layer_plan / _forward / _backward
+   * return GPS_ERR_UNSUPPORTED. */
   int32_t norm_type;
 
   GpsGraph graph;
@@ -183,18 +300,18 @@ typedef struct {
    * lets a captured CUDA graph draw fresh dropout masks on every replay. NULL = use `offset` only. */
   const uint64_t* offset_dev;
 
-  /* ABI 2: PyG GCNConv(dim_h, dim_h) local model (gps_layer.py:49-51): weight = local_model.lin.weight [d,d]
-   * (its Linear has no bias), bias = local_model.bias [d], added after the normalised aggregation. */
+  /* PyG GCNConv(dim_h, dim_h) local model (gps_layer.py:49-51): weight = local_model.lin.weight [d,d] (its Linear has
+   * no bias), bias = local_model.bias [d], added after the normalised aggregation. */
   GpsLinear gcn_conv;
 
-  /* ABI 3 (backward, optional): a cudaEvent_t the library records as soon as the "early" parameter gradients are
-   * final - ff_linear1/2, the attention output projection, norm2, norm1_local, norm1_attn - a few hundred microseconds
-   * before the pass ends.  A data-parallel caller makes its communication stream wait on it and all-reduces that
-   * part of the gradient bucket under the rest of the backward pass (graphgps_b200/dp.py).  NULL = not recorded. */
+  /* backward, optional: a cudaEvent_t the library records as soon as the "early" parameter gradients are final -
+   * ff_linear1/2, the attention output projection, norm2, norm1_local, norm1_attn - a few hundred microseconds before
+   * the pass ends.  A data-parallel caller makes its communication stream wait on it and all-reduces that part of the
+   * gradient bucket under the rest of the backward pass (graphgps_b200/dp.py).  NULL = not recorded. */
   void* ev_grads_early;
 
-  /* ABI 3 (optional): operand-plane hand-off between consecutive layers of a GPSModel (network/gps_model.py:100,105-108)
-   * and persistent weight planes.  A plane pair is the bf16 hi/lo image of an fp32 tensor (see gps_to_planes).
+  /* optional: operand-plane hand-off between consecutive layers of a GPSModel (network/gps_model.py:100,105-108) and
+   * persistent weight planes.  A plane pair is the bf16 hi/lo image of an fp32 tensor (see gps_to_planes).
    *  x_planes_in / e_planes_in   planes of x / edge_attr written by the previous layer: the layer skips its own
    *                              conversion of the inputs (hi == NULL: convert here, into `saved`);
    *  x_planes_out / e_planes_out caller-owned plane buffers the layer fills next to x_out / edge_out;
@@ -202,181 +319,46 @@ typedef struct {
    *                              wplanes_valid != 0: it already holds this layer's current weights (packed once per
    *                              optimiser step instead of once per forward call). */
   GpsPlanes x_planes_in, e_planes_in, x_planes_out, e_planes_out;
-  void* wplanes; int64_t wplanes_bytes; int32_t wplanes_valid; int32_t reserved2;
+  void* wplanes; int64_t wplanes_bytes; int32_t wplanes_valid; int32_t reserved2 /* padding */;
 
-  /* ABI 3 (backward, optional): two more cudaEvent_t of the same kind as ev_grads_early.  ev_grads_mid: the local
-   * model's gradients outside the fused node projection (C / GINE nn / GCN bias, bn_node_x, bn_edge_e) are final; A, B,
-   * D, E / GCN lin share one weight-gradient GEMM with in_proj at the end of the pass.  ev_grads_done: every gradient
-   * of this layer is final. */
+  /* backward, optional: two more cudaEvent_t of the same kind as ev_grads_early.  ev_grads_mid: the local model's
+   * gradients outside the fused node projection (C / GINE nn / GCN bias, bn_node_x, bn_edge_e) are final; A, B, D, E /
+   * GCN lin share one weight-gradient GEMM with in_proj at the end of the pass.  ev_grads_done: every gradient of this
+   * layer is final. */
   void* ev_grads_mid;
   void* ev_grads_done;
 
-  /* ABI 3, appended extension (optional): the EquivStableLapPE edge gate of GatedGCN (equivstable_pe=True,
-   * gatedgcn_layer.py:29-35,101-104).  pe = batch.pe_EquivStableLapPE, row-major contiguous [N, pe_dim], pe_dim >= 1.
-   * For edge j->i: r = sum_c (pe_i - pe_j)^2, rho = mlp_r_ij(r) and the gate becomes sigmoid(e_ij) * rho.
-   * pe == NULL: no gate (the fields below are not read).  pe != NULL with a local_type other than GPS_LOCAL_GATEDGCN
-   * is GPS_ERR_ARG.  Backward writes grad_pe [N, pe_dim] (NULL = not needed) and the gradients of pe_mlp0 / pe_mlp1,
-   * which are final when ev_grads_mid fires. */
+  /* optional: the EquivStableLapPE edge gate of GatedGCN (equivstable_pe=True, gatedgcn_layer.py:29-35,101-104).
+   * pe = batch.pe_EquivStableLapPE, row-major contiguous [N, pe_dim], pe_dim >= 1.  For edge j->i:
+   * r = sum_c (pe_i - pe_j)^2, rho = mlp_r_ij(r) and the gate becomes sigmoid(e_ij) * rho.  pe == NULL: no gate (the
+   * fields below are not read).  pe != NULL with a local_type other than GPS_LOCAL_GATEDGCN is GPS_ERR_ARG.  Backward
+   * writes grad_pe [N, pe_dim] (NULL = not needed) and the gradients of pe_mlp0 / pe_mlp1, which are final when
+   * ev_grads_mid fires. */
   const float* pe; int64_t pe_dim;
   float* grad_pe;
   GpsLinear pe_mlp0 /* mlp_r_ij.0 [d,1] */, pe_mlp1 /* mlp_r_ij.2 [1,d] */;
+
+  /* BiasedTransformer: bias == NULL is the unbiased Transformer (nmax and grad_bias must then be 0 / NULL).  A non-NULL
+   * bias needs global_type == GPS_GLOBAL_TRANSFORMER and nmax >= 1, else GPS_ERR_ARG.  gps_layer_plan does not read it;
+   * forward and backward must see the same bias tensor. */
+  GpsAttnBias attn_bias;
+  GpsGat gat;                /* read when local_type == GPS_LOCAL_GAT                */
+  GpsGenConv genconv;        /* read when local_type == GPS_LOCAL_GENCONV            */
+  GpsPna pna;                /* read when local_type == GPS_LOCAL_PNA                */
+  GpsBigBird bigbird;        /* read when global_type == GPS_GLOBAL_BIGBIRD         */
 } GpsLayerArgs;
 
 typedef struct {
   int64_t saved_bytes;          /* activations kept for backward (0 needed if eval-only) */
   int64_t fwd_workspace_bytes;
   int64_t bwd_workspace_bytes;
-  int64_t fwd_launches;         /* reserved, always 0 */
-  int64_t bwd_launches;         /* reserved, always 0 */
-  int64_t wplanes_bytes;        /* ABI 3: size of the optional persistent weight-plane buffer (GpsLayerArgs.wplanes) */
+  int64_t wplanes_bytes;        /* size of the optional persistent weight-plane buffer (GpsLayerArgs.wplanes) */
 } GpsLayerPlan;
 
 /* Sizes for the given configuration/graph (only sizes and type fields of args are read). */
 int gps_layer_plan(const GpsLayerArgs* args, GpsLayerPlan* plan);
 int gps_layer_forward(const GpsLayerArgs* args, void* stream);
 int gps_layer_backward(const GpsLayerArgs* args, void* stream);
-
-/* Additive attention bias of the BiasedTransformer global model (gps_layer.py:104-106,202-204,234-241; Graphormer's
- * batch.attn_bias): bias [B*heads, nmax, nmax] row-major float32, row g*heads + h of graph g and head h, entry (il, jl)
- * for local query il and local key jl; nmax >= the largest graph of the batch (to_dense_batch's Nmax).  The scores
- * become S = (q . k) / sqrt(hd) + bias[g*heads + h, il, jl]; padded entries (il or jl >= n_g) are not read.  grad_bias
- * (backward; NULL = not needed) has the same layout and is written whole: dL/dS at every in-graph entry, 0 at every
- * padded one. */
-typedef struct {
-  const float* bias;
-  int64_t nmax;
-  float* grad_bias;
-} GpsAttnBias;
-
-/* gps_layer_forward / _backward with an attention bias.  bias == NULL is the unbiased call; a non-NULL bias needs
- * global_type == GPS_GLOBAL_TRANSFORMER, nmax >= 1 and bias->bias != NULL (else GPS_ERR_ARG before any CUDA call).
- * The bias changes neither gps_layer_plan's sizes nor the GpsLayerArgs fields; forward and backward must see the same
- * bias tensor. */
-int gps_layer_forward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream);
-int gps_layer_backward_biased(const GpsLayerArgs* args, const GpsAttnBias* bias, void* stream);
-
-/* GAT local model (local_type == GPS_LOCAL_GAT): PyG 2.2 GATConv(dim_h, dim_h / heads, heads=heads, edge_dim=dim_h)
- * with its defaults (concat, negative_slope 0.2, no attention dropout, add_self_loops with fill_value 'mean', bias),
- * gps_layer.py:70-74,183-189.  H = GpsLayerArgs.heads heads of C = d / H channels each (d % H != 0 is GPS_ERR_ARG).
- * Existing self-loop edges are dropped and one loop per node is added whose edge attribute is the mean of the node's
- * remaining in-edge attributes (0 without any); their grad_edge_attr rows are 0.  edge_attr is read (non-NULL when
- * E > 0) and batch.edge_attr is not updated.  Parameters:
- *   lin_src   weight = local_model.lin_src.weight [d,d] (lin_dst is the same module), bias = local_model.bias [d]
- *             (added after the aggregation); its gradients: grad_weight with the fused node projection (final at
- *             ev_grads_done), grad_bias final at ev_grads_mid;
- *   lin_edge  weight = local_model.lin_edge.weight [d,d] (no bias);
- *   att_src / att_dst / att_edge = local_model.att_{src,dst,edge} [1,H,C], and their gradients, final at ev_grads_mid. */
-typedef struct {
-  GpsLinear lin_src;
-  GpsLinear lin_edge;
-  const float* att_src;
-  const float* att_dst;
-  const float* att_edge;
-  float* grad_att_src;
-  float* grad_att_dst;
-  float* grad_att_edge;
-} GpsGat;
-
-/* gps_layer_forward / _backward of a GAT layer; bias: GpsAttnBias of a BiasedTransformer global model or NULL.
- * gps_layer_plan sizes GAT from local_type alone.  The plain and _biased calls with local_type == GPS_LOCAL_GAT, and
- * these with a NULL gat, return GPS_ERR_ARG before any CUDA call, as does a NULL edge_attr (E > 0) or, in the
- * backward, grad_edge_attr (E > 0). */
-int gps_layer_forward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias, void* stream);
-int gps_layer_backward_gat(const GpsLayerArgs* args, const GpsGat* gat, const GpsAttnBias* bias, void* stream);
-
-/* GENConv local model (local_type == GPS_LOCAL_GENCONV): PyG 2.2 GENConv(dim_h, dim_h) with its defaults (softmax
- * aggregation with t = 1, no message norm, eps 1e-7, MLP d -> 2d -> d with BatchNorm, no bias), gps_layer.py:60-61,
- * 183-189.  For target i and channel c: m_k = relu(x[src_k] + e_k) + 1e-7, agg_i = sum_k softmax_k(m)_c m_kc over i's
- * in-edges (0 without any; self loops and duplicates are ordinary edges), u = agg + x and
- * h = lin1(relu(bn(lin0(u)))); x_loc = x + dropout(h).  edge_attr [E, d] is read (non-NULL when E > 0) and
- * batch.edge_attr is not updated.  d % 4 == 0 and d <= 2048 (the 2d-wide BatchNorm runs on the row-wise stages), else
- * GPS_ERR_UNSUPPORTED.  Parameters (all non-NULL, else GPS_ERR_ARG), whose gradients are final at ev_grads_mid:
- *   lin0 = local_model.mlp.0 [2d, d], bias NULL;
- *   bn   = local_model.mlp.1 [2d]: weight, bias, running_mean, running_var (num_batches_tracked optional); training
- *          mode normalises with the batch statistics and updates the running ones as torch.nn.BatchNorm1d;
- *   lin1 = local_model.mlp.4 [d, 2d], bias NULL.  The MLP's activation is ReLU whatever GpsLayerArgs.act is. */
-typedef struct {
-  GpsLinear lin0;
-  GpsBatchNorm bn;
-  GpsLinear lin1;
-} GpsGenConv;
-
-/* gps_layer_forward / _backward of a GENConv layer; bias: GpsAttnBias of a BiasedTransformer global model or NULL.
- * gps_layer_plan sizes GENConv from local_type alone.  The plain, _biased and _gat calls with local_type ==
- * GPS_LOCAL_GENCONV, and these with a NULL gen, return GPS_ERR_ARG before any CUDA call, as does a NULL edge_attr
- * (E > 0) or, in the backward, grad_edge_attr (E > 0). */
-int gps_layer_forward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias, void* stream);
-int gps_layer_backward_genconv(const GpsLayerArgs* args, const GpsGenConv* gen, const GpsAttnBias* bias, void* stream);
-
-/* PNA local model (local_type == GPS_LOCAL_PNA): PyG 2.2 PNAConv(dim_h, dim_h, aggregators=['mean','max','sum'],
- * scalers=['identity'], edge_dim=edge_dim, towers=1, pre_layers=1, post_layers=1, divide_input=False),
- * gps_layer.py:75-90,183-189.  For edge k from j to i:
- *   m_k = pre.weight [x_i ; x_j ; edge_encoder(e_k)] + pre.bias
- * and per target i and channel the mean, max and sum of m over i's in-edges (0 in all three without any; self loops
- * and duplicates are ordinary edges); x_loc = x + dropout(lin(post([x | mean | max | sum]))).  The max gradient goes
- * whole to the first maximising in-edge in edge_index order (torch_scatter's scatter_max).  The degree histogram never
- * enters the arithmetic with the identity scaler, so it is not an argument.  edge_attr and grad_edge_attr are
- * [E, edge_dim] (non-NULL when E > 0); batch.edge_attr is not updated.  0 < edge_dim <= d and edge_dim % 4 == 0, else
- * GPS_ERR_UNSUPPORTED.  Parameters (weights and biases non-NULL, else GPS_ERR_ARG):
- *   edge_encoder = local_model.edge_encoder [d, edge_dim] + [d]; gradients final at ev_grads_mid;
- *   pre  = local_model.pre_nns.0.0 [d, 3d] + [d] (column blocks: destination, source, encoded edge); gradients final
- *          at ev_grads_done (the first two blocks come with the fused node projection);
- *   post = local_model.post_nns.0.0 [d, 4d] + [d]; gradients final at ev_grads_mid;
- *   lin  = local_model.lin [d, d] + [d]; gradients final at ev_grads_mid. */
-typedef struct {
-  GpsLinear edge_encoder;
-  GpsLinear pre;
-  GpsLinear post;
-  GpsLinear lin;
-  int64_t edge_dim;
-} GpsPna;
-
-/* gps_layer_forward / _backward of a PNA layer; bias: GpsAttnBias of a BiasedTransformer global model or NULL.
- * gps_layer_plan sizes PNA from local_type alone, with edge_dim <= d as the bound.  The plain, _biased, _gat and
- * _genconv calls with local_type == GPS_LOCAL_PNA, and these with a NULL pna or another local_type, return GPS_ERR_ARG
- * before any CUDA call, as does a NULL edge_attr (E > 0) or, in the backward, grad_edge_attr (E > 0). */
-int gps_layer_forward_pna(const GpsLayerArgs* args, const GpsPna* pna, const GpsAttnBias* bias, void* stream);
-int gps_layer_backward_pna(const GpsLayerArgs* args, const GpsPna* pna, const GpsAttnBias* bias, void* stream);
-
-/* BigBird global model (global_type == GPS_GLOBAL_BIGBIRD): the reference's SingleBigBirdLayer, one BigBirdLayer with
- * block-sparse self-attention (gps_layer.py:115-119,207-208; bigbird_layer.py:1667-1706).  For graph g of n_g nodes,
- * local position p is node graph_ptr[g] + p; the batch is padded to S = num_blocks * block_size positions (to_dense_batch's
- * Nmax rounded up to the block size) and positions >= n_g are masked keys, never queries.  Head h of query block i
- * attends to the multiset of key blocks key_idx[key_ptr[h*(nb+1) + i] .. key_ptr[h*(nb+1) + i + 1]) (a block listed
- * twice counts twice in the softmax); query_ptr / query_idx is its transpose (the query blocks of every key block, in
- * ascending order, with the same multiplicities).  nb = num_blocks >= 4.  Scale 1/sqrt(hd), hd = d / heads (any hd >= 1
- * up to 128; d % heads != 0 is GPS_ERR_ARG), no attention dropout.  With ctx the attention output [N, d]:
- *   a   = LN1(drop_8(ctx Wso^T + bso) + x)          (attention.output; dropout site 8 = GPS_SITE_BB_SELF_OUT)
- *   u   = act(a Wi^T + bi)                           (intermediate; act = hidden_act: 0 relu, 1 sigmoid)
- *   out = LN2(drop_9(u Wo^T + bo) + a)               (output; dropout site 9 = GPS_SITE_BB_OUTPUT)
- * LN = nn.LayerNorm(d, eps = ln_eps) over each row; both dropouts use GpsLayerArgs.dropout.  out then takes the place of
- * the attention output in the GPS layer: hA = x + drop_4(out), norm1_attn, as for the Transformer.  Parameters
- * (self_attn.encoder.layers.0.*; weights [d, d]): query / key / value = attention.self.{query,key,value} (bias NULL
- * unless use_bias), self_out = attention.output.dense, ln1 = attention.output.LayerNorm (weight = gamma, bias = beta),
- * intermediate = intermediate.dense, output = output.dense, ln2 = output.LayerNorm.  Gradients: query / key / value are
- * final at ev_grads_done (one weight-gradient product with the node projections); the other five at ev_grads_mid. */
-enum { GPS_BIGBIRD_RELU = 0, GPS_BIGBIRD_SIGMOID = 1 };
-typedef struct {
-  int64_t block_size;
-  int64_t num_blocks;          /* nb of the batch: ceil(Nmax / block_size) */
-  int32_t hidden_act;          /* GPS_BIGBIRD_* */
-  float ln_eps;                /* layer_norm_eps */
-  const int32_t* key_ptr;      /* [heads * (nb + 1)], offsets into key_idx */
-  const int32_t* key_idx;
-  const int32_t* query_ptr;    /* [heads * (nb + 1)], offsets into query_idx */
-  const int32_t* query_idx;
-  GpsLinear query, key, value, self_out, ln1, intermediate, output, ln2;
-} GpsBigBird;
-
-/* gps_layer_forward / _backward of a layer with the BigBird global model and any local model (gat / gen / pna: the
- * local model's struct when local_type needs one, else NULL).  gps_layer_plan sizes BigBird from global_type, N, d and
- * heads alone.  A NULL bb, global_type != GPS_GLOBAL_BIGBIRD, block_size < 1, num_blocks < 4, a NULL list or weight,
- * and a local struct that does not match local_type return GPS_ERR_ARG before any CUDA call; so do the plain, _biased,
- * _gat, _genconv and _pna calls with global_type == GPS_GLOBAL_BIGBIRD. */
-int gps_layer_forward_bigbird(const GpsLayerArgs* args, const GpsBigBird* bb, const GpsGat* gat, const GpsGenConv* gen,
-                              const GpsPna* pna, void* stream);
-int gps_layer_backward_bigbird(const GpsLayerArgs* args, const GpsBigBird* bb, const GpsGat* gat, const GpsGenConv* gen,
-                               const GpsPna* pna, void* stream);
 
 /* BigBird stage entry points.  Q, K, V: [N, heads*hd] slices with row stride ld; O / dO [N, heads*hd] (stride ldo);
  * lse / delta [N, heads] (per-row log-sum-exp / rowsum(dO * O)); dQ, dK, dV written whole (stride ldg).  Only bb's
@@ -422,8 +404,7 @@ typedef struct {
   float dropout;             /* after the attention and after the MLP (sites 10, 12)          */
   float attn_dropout;        /* on the attention probabilities                                */
   float mlp_dropout;         /* inside the MLP, after GELU (site 11)                          */
-  int32_t flags;             /* backward: bit 0: parameter-gradient buffers are already zero; bit 1: gradients are
-                                added to the buffers (as GpsLayerArgs.reserved0)                */
+  int32_t flags;             /* GPS_FLAG_* (backward), as GpsLayerArgs.flags                  */
   uint64_t seed;             /* Philox key of this call's dropout masks                      */
   uint64_t offset;           /* Philox counter base                                           */
   const uint64_t* offset_dev;/* optional device-resident addend to offset (CUDA-graph replays); NULL = none */
@@ -478,8 +459,7 @@ typedef struct {
   int32_t precision;         /* GPS_PREC_*                                                     */
   float gamma;               /* cfg.gt.gamma, a constant                                       */
   float dropout;             /* sites 13 and 14                                                */
-  int32_t flags;             /* backward: bit 0: parameter-gradient buffers are already zero; bit 1: gradients are
-                                added to the buffers (as GpsGraphormerArgs.flags)               */
+  int32_t flags;             /* GPS_FLAG_* (backward), as GpsLayerArgs.flags                   */
   int32_t reserved;
   uint64_t seed;             /* Philox key of this call's dropout masks                       */
   uint64_t offset;           /* Philox counter base                                            */
@@ -765,7 +745,7 @@ int gps_performer_features_backward(const GpsGraph* g, int64_t H, int64_t dim_he
 int gps_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q,
                           const float* K, const float* V, int64_t ld, float* O, int64_t ldo,
                           float* lse, float p_drop, uint64_t seed, uint64_t offset, void* stream);
-/* ABI 3: the same forward on the tensor cores (csrc/attention_tc.cu: wgmma S = QK^T and O += PV, TMA-staged tiles,
+/* The same forward on the tensor cores (csrc/attention_tc.cu: wgmma S = QK^T and O += PV, TMA-staged tiles,
  * block-diagonal graph mask applied in-kernel).  qkv_hi/qkv_lo: bf16 hi/lo planes [N, ld] holding Q | K | V per head in
  * the padded layout column (which * heads + h) * hd_pad + k with hd_pad = round_up(hd, 16) and zero pad columns
  * (qkv_lo NULL for GPS_PREC_BF16).  Same O / lse conventions as gps_attention_forward, so either backward applies. */
@@ -792,7 +772,7 @@ int gps_attention_backward_biased(const GpsGraph* g, int64_t heads, int64_t hd, 
                                   const float* lse, float* delta, float* dQ, float* dK, float* dV, int64_t ldg,
                                   float p_drop, uint64_t seed, uint64_t offset, const GpsAttnBias* bias, void* stream);
 
-/* ABI 3: operand "planes" of the TMA-fed wgmma GEMM (csrc/gemm_tma.cu).  A plane pair is the bf16 image of an
+/* Operand "planes" of the TMA-fed wgmma GEMM (csrc/gemm_tma.cu).  A plane pair is the bf16 image of an
  * fp32 matrix: hi = bf16(v), lo = bf16(v - hi), both plain row-major with pitch ldp (elements, multiple of 8); lo may
  * be NULL for GPS_PREC_BF16.  gps_to_planes converts; gps_gemm_planes multiplies plane operands stored as
  * A: [M,K] (ta = 0) or [K,M] (ta = 1), B: [N,K] (tb = 0, an nn.Linear weight) or [K,N] (tb = 1), writes fp32 C

@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(lib, s), f"libgps_b200.so does not export {s}"
         assert s in _lib.SYMBOLS, f"ctypes binding missing for {s}"
-    assert lib.gps_abi_version() == 3
+    assert lib.gps_abi_version() == 4
     assert lib.gps_build_arch() == b"sm_90a"
 
 

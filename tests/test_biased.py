@@ -153,16 +153,12 @@ def test_graphgym_register_builds_gine_biased_transformer(monkeypatch):
     assert layer.attn_dropout == 0.5 and layer.num_heads == 4
 
 
-def test_layer_args_and_abi_unchanged():
-    """The bias travels in a struct of its own: GpsLayerArgs keeps its fields, size and ABI version."""
-    names = [f[0] for f in _lib.GpsLayerArgs._fields_]
-    assert names[-5:] == ["pe", "pe_dim", "grad_pe", "pe_mlp0", "pe_mlp1"]
-    assert names.index("ev_grads_done") == len(names) - 6
-    assert len(names) == 67 and C.sizeof(_lib.GpsLayerArgs) == 1272
+def test_attn_bias_fields_and_abi_version():
+    """The bias travels in GpsLayerArgs.attn_bias; the BiasedTransformer is the Transformer global type."""
     assert [f[0] for f in _lib.GpsAttnBias._fields_] == ["bias", "nmax", "grad_bias"]
-    assert C.sizeof(_lib.GpsAttnBias) == 24
-    assert _lib.load().gps_abi_version() == 3
-    assert _lib.GLOBAL == {"None": 0, "Transformer": 1, "Performer": 2}
+    assert dict(_lib.GpsLayerArgs._fields_)["attn_bias"] is _lib.GpsAttnBias
+    assert _lib.load().gps_abi_version() == 4
+    assert _lib.GLOBAL == {"None": 0, "Transformer": 1, "Performer": 2, "BigBird": 3}
 
 
 def _args(glob="Transformer", N=50, E=120, B=4):
@@ -172,18 +168,27 @@ def _args(glob="Transformer", N=50, E=120, B=4):
     return a
 
 
-@pytest.mark.parametrize("fn", ["gps_layer_forward_biased", "gps_layer_backward_biased"])
+@pytest.mark.parametrize("fn", ["gps_layer_forward", "gps_layer_backward"])
 def test_layer_entry_points_reject_bad_biases(fn):
-    """GPS_ERR_ARG before any CUDA call: a bias with another global type, nmax < 1, a NULL bias pointer."""
+    """GPS_ERR_ARG before any CUDA call: a bias with another global type, nmax < 1, a NULL bias pointer with nmax or
+    grad_bias set, NULL args."""
     lib = _lib.load()
     f = getattr(lib, fn)
+
+    def call(bias, glob="Transformer"):
+        a = _args(glob)
+        a.attn_bias = bias
+        return f(C.byref(a), None)
+
     good = _lib.GpsAttnBias(0x1000, 37, 0)
     for glob in ("Performer", "None"):
-        assert f(C.byref(_args(glob)), C.byref(good), None) == _lib.GPS_ERR_ARG
+        assert call(good, glob) == _lib.GPS_ERR_ARG
     for nmax in (0, -1):
-        assert f(C.byref(_args()), C.byref(_lib.GpsAttnBias(0x1000, nmax, 0)), None) == _lib.GPS_ERR_ARG
-    assert f(C.byref(_args()), C.byref(_lib.GpsAttnBias(0, 37, 0x2000)), None) == _lib.GPS_ERR_ARG
-    assert f(None, C.byref(good), None) == _lib.GPS_ERR_ARG
+        assert call(_lib.GpsAttnBias(0x1000, nmax, 0)) == _lib.GPS_ERR_ARG
+    assert call(_lib.GpsAttnBias(0, 37, 0x2000)) == _lib.GPS_ERR_ARG
+    assert call(_lib.GpsAttnBias(0, 37, 0)) == _lib.GPS_ERR_ARG
+    assert call(_lib.GpsAttnBias(0, 0, 0x2000)) == _lib.GPS_ERR_ARG
+    assert f(None, None) == _lib.GPS_ERR_ARG
     assert b"nmax" in lib.gps_last_error() or b"null" in lib.gps_last_error() or b"args" in lib.gps_last_error()
 
 

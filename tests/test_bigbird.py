@@ -260,10 +260,12 @@ def _lib_or_skip():
         pytest.skip(str(e))
 
 
-def _args(global_type=_lib.GLOBAL_BIGBIRD, local=_lib.LOCAL["GINE"], d=56, heads=8):
+def _args(global_type=_lib.GLOBAL["BigBird"], local=_lib.LOCAL["GINE"], d=56, heads=8, bb=None):
     a = _lib.GpsLayerArgs()
     a.d, a.heads, a.local_type, a.global_type = d, heads, local, global_type
     a.graph.N, a.graph.E, a.graph.B = 10, 0, 1
+    if bb is not None:
+        a.bigbird = bb
     return a
 
 
@@ -276,8 +278,8 @@ def _bb(nb=4, bs=3, lists=True):
 
 
 def test_abi_constants():
-    assert _lib.GLOBAL == {"None": 0, "Transformer": 1, "Performer": 2}
-    assert _lib.GLOBAL_BIGBIRD == 3
+    assert _lib.GLOBAL == {"None": 0, "Transformer": 1, "Performer": 2, "BigBird": 3}
+    assert _lib.GLOBAL_BIGBIRD == _lib.GLOBAL["BigBird"] == 3
     hdr = open(os.path.join(os.path.dirname(GOLDEN_DIR), "..", "include", "gps_b200.h")).read()
     assert "GPS_GLOBAL_BIGBIRD = 3" in hdr
 
@@ -285,32 +287,18 @@ def test_abi_constants():
 def test_entry_points_refuse_malformed_arguments():
     lib = _lib_or_skip()
     ARG = _lib.GPS_ERR_ARG
-    for fwd, bwd in ((lib.gps_layer_forward_bigbird, lib.gps_layer_backward_bigbird),):
-        for fn in (fwd, bwd):
-            assert fn(C.byref(_args()), None, None, None, None, None) == ARG                     # NULL bb
-            assert fn(C.byref(_args(global_type=1)), C.byref(_bb()), None, None, None, None) == ARG
-            assert fn(C.byref(_args()), C.byref(_bb(nb=3)), None, None, None, None) == ARG       # nb < 4
-            assert fn(C.byref(_args()), C.byref(_bb(bs=0)), None, None, None, None) == ARG
-            assert fn(C.byref(_args()), C.byref(_bb(lists=False)), None, None, None, None) == ARG
-            assert fn(C.byref(_args(heads=5)), C.byref(_bb()), None, None, None, None) == ARG   # d % heads
-            gat = _lib.GpsGat()
-            assert fn(C.byref(_args()), C.byref(_bb()), C.byref(gat), None, None, None) == ARG  # GAT struct, GINE
-            assert fn(C.byref(_args(local=_lib.LOCAL["GAT"])), C.byref(_bb()), None, None, None, None) == ARG
-            # well-formed structs with missing parameters: refused by the parameter check
-            assert fn(C.byref(_args()), C.byref(_bb()), None, None, None, None) == ARG
-    # the other entry points with global_type BigBird
-    a = _args()
+    for fn in (lib.gps_layer_forward, lib.gps_layer_backward):
+        assert fn(C.byref(_args()), None) == ARG                                  # GpsBigBird left empty
+        assert fn(C.byref(_args(bb=_bb(nb=3))), None) == ARG                      # nb < 4
+        assert fn(C.byref(_args(bb=_bb(bs=0))), None) == ARG
+        assert fn(C.byref(_args(bb=_bb(lists=False))), None) == ARG
+        assert fn(C.byref(_args(heads=5, bb=_bb())), None) == ARG                 # d % heads
+        # a well-formed GpsBigBird with missing parameters: refused by the parameter check
+        assert fn(C.byref(_args(bb=_bb())), None) == ARG
+    # an attention bias needs the Transformer
+    a = _args(bb=_bb())
+    a.attn_bias = _lib.GpsAttnBias(16, 4, 0)
     assert lib.gps_layer_forward(C.byref(a), None) == ARG
-    assert lib.gps_layer_backward(C.byref(a), None) == ARG
-    assert lib.gps_layer_forward_biased(C.byref(a), C.byref(_lib.GpsAttnBias(16, 4, 0)), None) == ARG
-    ag = _args(local=_lib.LOCAL["GAT"])
-    assert lib.gps_layer_forward_gat(C.byref(ag), C.byref(_lib.GpsGat()), None, None) == ARG
-    agen = _args(local=_lib.LOCAL["GENConv"])
-    assert lib.gps_layer_forward_genconv(C.byref(agen), C.byref(_lib.GpsGenConv()), None, None) == ARG
-    ap = _args(local=_lib.LOCAL["PNA"])
-    pna = _lib.GpsPna()
-    pna.edge_dim = 56
-    assert lib.gps_layer_forward_pna(C.byref(ap), C.byref(pna), None, None) == ARG
     # stages
     g = _lib.GpsGraph()
     assert lib.gps_bigbird_attention_forward(C.byref(g), 8, 7, None, 16, 16, 16, 56, 16, 56, 16, None) == ARG

@@ -159,23 +159,33 @@ def test_error_contract_before_any_cuda_call():
     a = _args("GAT")
     a.x, a.edge_attr, a.x_out, a.saved, a.saved_bytes, a.workspace, a.workspace_bytes = 8, 8, 8, 8, 1 << 40, 8, 1 << 40
     a.grad_x_out, a.grad_x = 8, 8
-    gat = _lib.GpsGat()
-    assert lib.gps_layer_forward(C.byref(a), None) == _lib.GPS_ERR_ARG
+    assert lib.gps_layer_forward(C.byref(a), None) == _lib.GPS_ERR_ARG   # null parameters
     assert lib.gps_layer_backward(C.byref(a), None) == _lib.GPS_ERR_ARG
-    ab = _lib.GpsAttnBias(8, 4, 0)
-    assert lib.gps_layer_forward_biased(C.byref(a), C.byref(ab), None) == _lib.GPS_ERR_ARG
-    assert lib.gps_layer_backward_biased(C.byref(a), C.byref(ab), None) == _lib.GPS_ERR_ARG
-    assert lib.gps_layer_forward_gat(C.byref(a), None, None, None) == _lib.GPS_ERR_ARG
-    assert lib.gps_layer_backward_gat(C.byref(a), None, None, None) == _lib.GPS_ERR_ARG
-    assert lib.gps_layer_forward_gat(C.byref(a), C.byref(gat), None, None) == _lib.GPS_ERR_ARG   # null parameters
+
+    def full_gat():
+        gat = _lib.GpsGat()
+        gat.lin_src.weight = gat.lin_src.bias = gat.lin_edge.weight = gat.att_src = gat.att_dst = gat.att_edge = 8
+        return gat
+
+    for field, what in (("lin_src.weight", "lin_src"), ("lin_src.bias", "lin_src"), ("lin_edge.weight", "lin_edge"),
+                        ("att_src", "att_"), ("att_dst", "att_"), ("att_edge", "att_")):
+        a.gat = full_gat()
+        obj, f = (getattr(a.gat, field.split(".")[0]), field.split(".")[1]) if "." in field else (a.gat, field)
+        setattr(obj, f, 0)
+        for fn in (lib.gps_layer_forward, lib.gps_layer_backward):
+            assert fn(C.byref(a), None) == _lib.GPS_ERR_ARG, field
+            assert what in lib.gps_last_error().decode(), field
+    a.gat = full_gat()
     a.edge_attr = 0
-    assert lib.gps_layer_forward_gat(C.byref(a), C.byref(gat), None, None) == _lib.GPS_ERR_ARG
+    assert lib.gps_layer_forward(C.byref(a), None) == _lib.GPS_ERR_ARG
     a.edge_attr = 8
-    gat.lin_src.weight = gat.lin_src.bias = gat.lin_edge.weight = gat.att_src = gat.att_dst = gat.att_edge = 8
     a.grad_edge_attr = 0
-    assert lib.gps_layer_backward_gat(C.byref(a), C.byref(gat), None, None) == _lib.GPS_ERR_ARG
+    assert lib.gps_layer_backward(C.byref(a), None) == _lib.GPS_ERR_ARG
+    n = _args("GAT", glob="None")   # an attention bias needs the Transformer
+    n.gat, n.attn_bias = full_gat(), _lib.GpsAttnBias(8, 4, 0)
+    assert lib.gps_layer_forward(C.byref(n), None) == _lib.GPS_ERR_ARG
     a.heads = 3
-    assert lib.gps_layer_forward_gat(C.byref(a), C.byref(gat), None, None) == _lib.GPS_ERR_ARG
+    assert lib.gps_layer_forward(C.byref(a), None) == _lib.GPS_ERR_ARG
     g = _lib.GpsGraph()
     g.N, g.E = 4, 4
     assert lib.gps_gat_fold_forward(None, 8, 64, 4, 8, None) == _lib.GPS_ERR_ARG

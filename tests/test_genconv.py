@@ -281,47 +281,36 @@ def test_error_contract_before_any_cuda_call():
         lin.weight = lin.bias = 8
     for bn in (a.norm1_local, a.norm1_attn, a.norm2):
         bn.weight = bn.bias = 8
-    ab = _lib.GpsAttnBias(8, 4, 0)
-    # the plain, _biased and _gat calls
-    assert lib.gps_layer_forward(C.byref(a), None) == ARG and "gps_layer_forward_genconv" in _err()
-    assert lib.gps_layer_backward(C.byref(a), None) == ARG and "GpsGenConv" in _err()
-    assert lib.gps_layer_forward_biased(C.byref(a), C.byref(ab), None) == ARG
-    assert lib.gps_layer_backward_biased(C.byref(a), C.byref(ab), None) == ARG
-    gat = _lib.GpsGat()
-    gat.lin_src.weight = gat.lin_src.bias = gat.lin_edge.weight = gat.att_src = gat.att_dst = gat.att_edge = 8
-    assert lib.gps_layer_forward_gat(C.byref(a), C.byref(gat), None, None) == ARG and "GPS_LOCAL_GAT" in _err()
-    assert lib.gps_layer_backward_gat(C.byref(a), C.byref(gat), None, None) == ARG
-    # a NULL gen, a GpsGenConv on another local type, NULL parameters one at a time
-    assert lib.gps_layer_forward_genconv(C.byref(a), None, None, None) == ARG
-    assert lib.gps_layer_backward_genconv(C.byref(a), None, None, None) == ARG
-    gine = _args("GINE")
-    assert lib.gps_layer_forward_genconv(C.byref(gine), C.byref(_full_gen()), None, None) == ARG
-    assert "GPS_LOCAL_GENCONV" in _err()
+    # NULL parameters: all of them, then one at a time
+    assert lib.gps_layer_forward(C.byref(a), None) == ARG and "local_model.mlp.0" in _err()
+    assert lib.gps_layer_backward(C.byref(a), None) == ARG and "local_model.mlp.0" in _err()
     for field, what in (("lin0.weight", "mlp.0"), ("bn.weight", "mlp.1"), ("bn.bias", "mlp.1"),
                         ("bn.running_mean", "mlp.1.running"), ("bn.running_var", "mlp.1.running"),
                         ("lin1.weight", "mlp.4")):
-        gen = _full_gen()
+        a.genconv = _full_gen()
         s, f = field.split(".")
-        setattr(getattr(gen, s), f, 0)
-        for fn in (lib.gps_layer_forward_genconv, lib.gps_layer_backward_genconv):
-            assert fn(C.byref(a), C.byref(gen), None, None) == ARG, field
+        setattr(getattr(a.genconv, s), f, 0)
+        for fn in (lib.gps_layer_forward, lib.gps_layer_backward):
+            assert fn(C.byref(a), None) == ARG, field
             assert what in _err(), (field, _err())
-    gen = _full_gen()
+    a.genconv = _full_gen()
     # edge_attr / grad_edge_attr with E > 0
     a.edge_attr = 0
-    assert lib.gps_layer_forward_genconv(C.byref(a), C.byref(gen), None, None) == ARG and "edge_attr" in _err()
+    assert lib.gps_layer_forward(C.byref(a), None) == ARG and "edge_attr" in _err()
     a.edge_attr = 8
     a.grad_edge_attr = 0
-    assert lib.gps_layer_backward_genconv(C.byref(a), C.byref(gen), None, None) == ARG
+    assert lib.gps_layer_backward(C.byref(a), None) == ARG
     assert "grad_edge_attr" in _err()
     # an attention bias needs the Transformer
     n = _args("GENConv", glob="None")
-    assert lib.gps_layer_forward_genconv(C.byref(n), C.byref(gen), C.byref(ab), None) == ARG
+    n.genconv, n.attn_bias = _full_gen(), _lib.GpsAttnBias(8, 4, 0)
+    assert lib.gps_layer_forward(C.byref(n), None) == ARG and "GPS_GLOBAL_TRANSFORMER" in _err()
     # widths
     for d in (66, 2052):
         w = _args("GENConv", d=d, H=2)
         w.x, w.edge_attr, w.x_out, w.saved, w.workspace = 8, 8, 8, 8, 8
-        assert lib.gps_layer_forward_genconv(C.byref(w), C.byref(gen), None, None) == UNS
+        w.genconv = _full_gen()
+        assert lib.gps_layer_forward(C.byref(w), None) == UNS
     # stage entry points
     g = _lib.GpsGraph()
     g.N, g.E = 4, 4

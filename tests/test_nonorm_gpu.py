@@ -234,7 +234,7 @@ def test_two_layer_stack_matches_oracle_and_capture_replays_eager():
 
 
 def test_bucket_gradients_equal_plain_gradients():
-    """dp.GradBucket's in-place accumulation path (GpsLayerArgs.reserved0 bit 1) on layers without norms."""
+    """dp.GradBucket's in-place accumulation path (GpsLayerArgs.flags, GPS_FLAG_GRADS_ACCUMULATE) on layers without norms."""
     b = node_shape_batch("webkb", seed=6).to(DEV)
     torch.manual_seed(7)
     stack = graphgps_b200.GPSStack(2, 64, "GCN", "Transformer", 4, act="gelu", batch_norm=False).to(DEV).train()

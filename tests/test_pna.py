@@ -289,50 +289,31 @@ def test_error_contract_before_any_cuda_call():
         lin.weight = lin.bias = 8
     for bn in (a.norm1_local, a.norm1_attn, a.norm2):
         bn.weight = bn.bias = 8
-    ab = _lib.GpsAttnBias(8, 4, 0)
-    # the plain, _biased, _gat and _genconv calls
-    assert lib.gps_layer_forward(C.byref(a), None) == ARG and "gps_layer_forward_pna" in _err()
-    assert lib.gps_layer_backward(C.byref(a), None) == ARG and "GpsPna" in _err()
-    assert lib.gps_layer_forward_biased(C.byref(a), C.byref(ab), None) == ARG
-    assert lib.gps_layer_backward_biased(C.byref(a), C.byref(ab), None) == ARG
-    gat = _lib.GpsGat()
-    gat.lin_src.weight = gat.lin_src.bias = gat.lin_edge.weight = gat.att_src = gat.att_dst = gat.att_edge = 8
-    assert lib.gps_layer_forward_gat(C.byref(a), C.byref(gat), None, None) == ARG and "GPS_LOCAL_GAT" in _err()
-    assert lib.gps_layer_backward_gat(C.byref(a), C.byref(gat), None, None) == ARG
-    gen = _lib.GpsGenConv()
-    gen.lin0.weight = gen.lin1.weight = 8
-    gen.bn.weight = gen.bn.bias = gen.bn.running_mean = gen.bn.running_var = 8
-    assert lib.gps_layer_forward_genconv(C.byref(a), C.byref(gen), None, None) == ARG
-    assert "GPS_LOCAL_GENCONV" in _err()
-    assert lib.gps_layer_backward_genconv(C.byref(a), C.byref(gen), None, None) == ARG
-    # a NULL pna, a GpsPna on another local type, NULL parameters one at a time
-    assert lib.gps_layer_forward_pna(C.byref(a), None, None, None) == ARG
-    assert lib.gps_layer_backward_pna(C.byref(a), None, None, None) == ARG
-    gine = _args("GINE")
-    assert lib.gps_layer_forward_pna(C.byref(gine), C.byref(_full_pna()), None, None) == ARG
-    assert "GPS_LOCAL_PNA" in _err()
+    # NULL parameters one at a time
     for s, what in (("edge_encoder", "edge_encoder"), ("pre", "pre_nns"), ("post", "post_nns"), ("lin", "local_model.lin")):
         for f in ("weight", "bias"):
-            pna = _full_pna()
-            setattr(getattr(pna, s), f, 0)
-            for fn in (lib.gps_layer_forward_pna, lib.gps_layer_backward_pna):
-                assert fn(C.byref(a), C.byref(pna), None, None) == ARG, (s, f)
+            a.pna = _full_pna()
+            setattr(getattr(a.pna, s), f, 0)
+            for fn in (lib.gps_layer_forward, lib.gps_layer_backward):
+                assert fn(C.byref(a), None) == ARG, (s, f)
                 assert what in _err(), (s, f, _err())
-    pna = _full_pna()
+    a.pna = _full_pna()
     # edge_attr / grad_edge_attr with E > 0
     a.edge_attr = 0
-    assert lib.gps_layer_forward_pna(C.byref(a), C.byref(pna), None, None) == ARG and "edge_attr" in _err()
+    assert lib.gps_layer_forward(C.byref(a), None) == ARG and "edge_attr" in _err()
     a.edge_attr = 8
     a.grad_edge_attr = 0
-    assert lib.gps_layer_backward_pna(C.byref(a), C.byref(pna), None, None) == ARG
+    assert lib.gps_layer_backward(C.byref(a), None) == ARG
     assert "grad_edge_attr" in _err()
     # an attention bias needs the Transformer
     n = _args("PNA", glob="None")
-    assert lib.gps_layer_forward_pna(C.byref(n), C.byref(pna), C.byref(ab), None) == ARG
-    # edge widths: 0 < edge_dim <= d, edge_dim % 4 == 0
+    n.pna, n.attn_bias = _full_pna(), _lib.GpsAttnBias(8, 4, 0)
+    assert lib.gps_layer_forward(C.byref(n), None) == ARG and "GPS_GLOBAL_TRANSFORMER" in _err()
+    # edge widths: 0 < edge_dim <= d, edge_dim % 4 == 0 (0: the GpsPna left empty)
     for de in (0, -4, 6, 68):
-        assert lib.gps_layer_forward_pna(C.byref(a), C.byref(_full_pna(de)), None, None) == UNS, de
-        assert lib.gps_layer_backward_pna(C.byref(a), C.byref(_full_pna(de)), None, None) == UNS, de
+        a.pna = _full_pna(de)
+        assert lib.gps_layer_forward(C.byref(a), None) == UNS, de
+        assert lib.gps_layer_backward(C.byref(a), None) == UNS, de
     assert _plan(_args("PNA", d=66, glob="None"))[0] == UNS
     # stage entry points
     g = _lib.GpsGraph()
