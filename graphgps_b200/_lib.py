@@ -128,6 +128,24 @@ class GpsGraphormerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
 
 
+class GpsGraphormerBiasArgs(C.Structure):
+    """Graphormer's BiasEncoder (graphormer_encoder.py:103-183): sizes, the collated pair attributes (int64), the four
+    parameters, attn_bias / grad_attn_bias [B*H, N', N'], the parameter gradients and the backward's scratch."""
+    _fields_ = [("num_pairs", C.c_int64), ("num_graphs", C.c_int64), ("nmax", C.c_int64), ("heads", C.c_int64),
+                ("num_spatial_types", C.c_int64), ("num_edge_types", C.c_int64), ("use_graph_token", C.c_int32),
+                ("reserved", C.c_int32),
+                ("spatial_types", _fp), ("graph_index", _fp), ("shortest_path_types", _fp), ("node_ptr", _fp),
+                ("spatial_weight", _fp), ("edge_dis_weight", _fp), ("edge_weight", _fp), ("graph_token", _fp),
+                ("attn_bias", _fp), ("grad_attn_bias", _fp),
+                ("grad_spatial_weight", _fp), ("grad_edge_dis_weight", _fp), ("grad_edge_weight", _fp),
+                ("grad_graph_token", _fp),
+                ("workspace", _fp), ("workspace_bytes", C.c_int64)]
+
+
+class GpsGraphormerBiasPlan(C.Structure):
+    _fields_ = [("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
+
+
 class GpsSanArgs(C.Structure):
     """SAN layer (san_layer.py): config, dropout stream, graph and nmax, tensors, scratch, the ten Linears
     attention.{Q,K,V,Q_2,K_2,E,E_2}, O_h, FFN_h_layer1, FFN_h_layer2, batch_norm{1,2}_h and attention.fake_edge_emb."""
@@ -194,6 +212,9 @@ SYMBOLS = {
     "gps_graphormer_plan": (C.c_int, [C.POINTER(GpsGraphormerArgs), C.POINTER(GpsGraphormerPlan)]),
     "gps_graphormer_forward": (C.c_int, [C.POINTER(GpsGraphormerArgs), C.POINTER(GpsAttnBias), _fp]),
     "gps_graphormer_backward": (C.c_int, [C.POINTER(GpsGraphormerArgs), C.POINTER(GpsAttnBias), _fp]),
+    "gps_graphormer_bias_plan": (C.c_int, [C.POINTER(GpsGraphormerBiasArgs), C.POINTER(GpsGraphormerBiasPlan)]),
+    "gps_graphormer_bias_forward": (C.c_int, [C.POINTER(GpsGraphormerBiasArgs), _fp]),
+    "gps_graphormer_bias_backward": (C.c_int, [C.POINTER(GpsGraphormerBiasArgs), _fp]),
     "gps_san_plan": (C.c_int, [C.POINTER(GpsSanArgs), C.POINTER(GpsSanPlan)]),
     "gps_san_forward": (C.c_int, [C.POINTER(GpsSanArgs), _fp]),
     "gps_san_backward": (C.c_int, [C.POINTER(GpsSanArgs), _fp]),

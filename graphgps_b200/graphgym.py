@@ -38,6 +38,21 @@ def install_graphormer(graphormer_module=None):
     return previous
 
 
+def install_graphormer_bias(module=None):
+    """Rebind ``BiasEncoder`` inside ``graphgps.encoder.graphormer_encoder`` so the ``GraphormerBias`` node encoder, and
+    every composed ``*+GraphormerBias`` encoder, builds the H100 attention-bias encoder: ``GraphormerEncoder.__init__``
+    looks that module global up at construction time.  Its ``NodeEncoder`` stays the reference's.
+
+    Call after ``import graphgps`` and before ``create_model()``.  Returns the class it replaced so a caller can restore
+    it."""
+    from .graphormer_bias import BiasEncoder
+    if module is None:
+        module = importlib.import_module("graphgps.encoder.graphormer_encoder")
+    previous = getattr(module, "BiasEncoder", None)
+    module.BiasEncoder = BiasEncoder
+    return previous
+
+
 def install_san(san_module=None):
     """Rebind ``SANLayer`` inside ``graphgps.network.san_transformer`` so ``SANTransformer`` builds the H100 layer.
     ``SAN2Layer`` (learned gamma, softmax scores) stays the reference's.

@@ -432,6 +432,64 @@ int gps_graphormer_forward(const GpsGraphormerArgs* args, const GpsAttnBias* bia
 int gps_graphormer_backward(const GpsGraphormerArgs* args, const GpsAttnBias* bias, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Graphormer's attention-bias encoder (graphgps/encoder/graphormer_encoder.py:103-183, BiasEncoder), the producer of
+ * the GpsAttnBias both consumers above read.  Inputs are graphormer_pre_processing's attributes, PyG-collated: pair p
+ * has global nodes i = graph_index[0, p], j = graph_index[1, p] of one graph b (node_ptr[b] <= i, j < node_ptr[b+1]),
+ * spatial type s_p = spatial_types[p] in [0, S] and, when shortest_path_types is not NULL, path types
+ * t_pk = shortest_path_types[p * S + k] in [0, T).  With sd_p = max(1, s_p), il = i - node_ptr[b], jl = j - node_ptr[b]
+ * and o = 1 with the graph token (else 0):
+ *   attn_bias[b*H + h, o + il, o + jl] = spatial_weight[s_p, h]
+ *                     + (1 / sd_p) sum_{k<S} sum_{h'} edge_weight[t_pk, h'] edge_dis_weight[(k*H + h')*H + h]
+ * (the edge term only with shortest_path_types).  The output [B*H, N', N'], N' = nmax + o, is written whole: entries
+ * no pair covers are 0 and, with the graph token, row 0 and column 0 of every graph hold graph_token[h].
+ * Precondition: each ordered pair of a graph appears at most once (as graphormer_pre_processing emits them); each pair
+ * is written with a plain store and their order is free.  A pair whose nodes or spatial type are out of range is
+ * skipped, and a path type out of range adds nothing: no input is dereferenced out of bounds (the Python module rejects
+ * such inputs before the call).
+ * Backward from grad_attn_bias writes (each NULL = not needed) grad_spatial_weight [S+1, H], grad_edge_dis_weight
+ * [S*H*H], grad_edge_weight [T, H] and grad_graph_token [H] through per-CTA partials summed in a fixed order: no float
+ * atomics, two runs give the same bits.
+ * Staged sizes: H <= 32, (S+1)*H <= 4096 and S*T*H <= 8192 floats, S*T + S + 1 <= 384 per-thread slots of the backward
+ * (S*T counted only with shortest_path_types); anything larger is GPS_ERR_UNSUPPORTED.  Pair x position offsets are
+ * 64-bit.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  int64_t num_pairs;         /* P                                                             */
+  int64_t num_graphs;        /* B = batch.max() + 1 (to_dense_adj's batch size)               */
+  int64_t nmax;              /* largest graph of the batch                                    */
+  int64_t heads;             /* H = num_heads                                                 */
+  int64_t num_spatial_types; /* S                                                             */
+  int64_t num_edge_types;    /* T                                                             */
+  int32_t use_graph_token;   /* 1: pad by one row and column and write graph_token there      */
+  int32_t reserved;
+  const int64_t* spatial_types;       /* [P]                                                  */
+  const int64_t* graph_index;         /* [2, P] global node ids                               */
+  const int64_t* shortest_path_types; /* [P, S] or NULL (no edge term)                        */
+  const int64_t* node_ptr;            /* [B+1] first node of each graph                       */
+  const float* spatial_weight;        /* spatial_encoder.weight [S+1, H]                      */
+  const float* edge_dis_weight;       /* edge_dis_encoder.weight [S*H*H, 1]                   */
+  const float* edge_weight;           /* edge_encoder.weight [T, H]                           */
+  const float* graph_token;           /* graph_token [1, H, 1] (use_graph_token)              */
+  float* attn_bias;                   /* [B*H, N', N'] (forward)                              */
+  const float* grad_attn_bias;        /* [B*H, N', N'] (backward)                             */
+  float* grad_spatial_weight;
+  float* grad_edge_dis_weight;
+  float* grad_edge_weight;
+  float* grad_graph_token;
+  void* workspace; int64_t workspace_bytes; /* transient (backward)                           */
+} GpsGraphormerBiasArgs;
+
+typedef struct {
+  int64_t fwd_workspace_bytes;
+  int64_t bwd_workspace_bytes;
+} GpsGraphormerBiasPlan;
+
+/* Sizes for args (only the sizes, use_graph_token and whether shortest_path_types is NULL are read). */
+int gps_graphormer_bias_plan(const GpsGraphormerBiasArgs* args, GpsGraphormerBiasPlan* plan);
+int gps_graphormer_bias_forward(const GpsGraphormerBiasArgs* args, void* stream);
+int gps_graphormer_bias_backward(const GpsGraphormerBiasArgs* args, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * SAN layer (graphgps/layer/san_layer.py:10-210), the building block of SANTransformer, as every shipped config runs
  * it (full_graph, batch_norm, residual, no layer_norm, no Linear biases in the attention, in_dim == out_dim == d):
  *   [Q|K|V|Q2|K2] = x W^T, E = edge_attr W_E^T, E2 = W_E2 fake_edge_emb
