@@ -175,28 +175,14 @@ int make_plan(const GpsCustomGnnArgs* a, CgPlan* P, bool bind) {
   P->pad = dp != d;
   P->residual = a->residual != 0;
   P->eps = a->gine_eps;
-  auto drop = [&](int site) {
-    DropCfg c;
-    c.p = P->train ? a->dropout : 0.f;
-    c.seed = a->seed; c.offset = a->offset; c.site = site;
-    c.offset_dev = (const unsigned long long*)a->offset_dev;
-    return c;
-  };
-  P->drop_x = drop(GPS_SITE_CG_X);
-  P->drop_e = drop(GPS_SITE_CG_E);
+  P->drop_x = drop_cfg(a->dropout, P->train, a->seed, a->offset, a->offset_dev, GPS_SITE_CG_X);
+  P->drop_e = drop_cfg(a->dropout, P->train, a->seed, a->offset, a->offset_dev, GPS_SITE_CG_E);
   const bool lo = a->precision == GPS_PREC_FP32;
-  auto mkplanes = [&](Arena& A, int64_t rows, int64_t ld = 0) {
-    Planes q;
-    q.ld = ld ? ld : dp;
-    q.hi = A.alloc<__nv_bfloat16>(rows * q.ld + 8);
-    q.lo = lo ? A.alloc<__nv_bfloat16>(rows * q.ld + 8) : nullptr;
-    return q;
-  };
   const int64_t wrows = P->gated ? 4 * dp : dp;   // rows of the first product's weight
 
   Arena W(bind ? a->wplanes : nullptr, a->wplanes_bytes);
-  P->W_p = mkplanes(W, wrows);
-  P->W2_p = mkplanes(W, dp);
+  P->W_p = arena_planes(W, wrows, dp, lo);
+  P->W2_p = arena_planes(W, dp, dp, lo);
   P->b1 = W.alloc<float>(wrows);
   P->b2 = W.alloc<float>(dp);
   if (P->gated) P->bnw = W.alloc<float>(4 * dp);
@@ -210,8 +196,8 @@ int make_plan(const GpsCustomGnnArgs* a, CgPlan* P, bool bind) {
     P->e = S.alloc<float>(E * dp);
   }
   if (P->gated) {
-    P->x_p = mkplanes(S, N);
-    P->e_p = mkplanes(S, E);
+    P->x_p = arena_planes(S, N, dp, lo);
+    P->e_p = arena_planes(S, E, dp, lo);
     P->Y = S.alloc<float>(N * 4 * dp);
     P->ehat = S.alloc<float>(E * dp);
     P->xt = S.alloc<float>(N * dp);
@@ -219,9 +205,9 @@ int make_plan(const GpsCustomGnnArgs* a, CgPlan* P, bool bind) {
     if (P->pad) P->rs = S.alloc<float>(4 * dp);
   } else {
     P->agg = S.alloc<float>(N * dp);
-    P->agg_p = mkplanes(S, N);
+    P->agg_p = arena_planes(S, N, dp, lo);
     P->h = S.alloc<float>(N * dp);
-    P->h_p = mkplanes(S, N);
+    P->h_p = arena_planes(S, N, dp, lo);
     P->pre2 = S.alloc<float>(N * dp);
   }
   P->saved_bytes = S.used;
@@ -255,14 +241,14 @@ int make_plan(const GpsCustomGnnArgs* a, CgPlan* P, bool bind) {
   P->ge = Bk.alloc<float>(E * dp);
   if (P->gated) {
     P->gY = Bk.alloc<float>(N * 4 * dp);
-    P->gY_p = mkplanes(Bk, N, 4 * dp);
-    P->ge_p = mkplanes(Bk, E);
+    P->gY_p = arena_planes(Bk, N, 4 * dp, lo);
+    P->ge_p = arena_planes(Bk, E, dp, lo);
     P->gnum = Bk.alloc<float>(N * dp);
   } else {
     P->g2 = Bk.alloc<float>(N * dp);
-    P->g2_p = mkplanes(Bk, N);
+    P->g2_p = arena_planes(Bk, N, dp, lo);
     P->gh = Bk.alloc<float>(N * dp);
-    P->gh_p = mkplanes(Bk, N);
+    P->gh_p = arena_planes(Bk, N, dp, lo);
     P->gagg = Bk.alloc<float>(N * dp);
   }
   P->bwd_bytes = Bk.used;

@@ -55,29 +55,13 @@ int make_plan(const GpsGraphormerArgs* a, GrPlan* P, bool bind) {
   P->N = N; P->d = d; P->H = a->heads; P->hd = d / a->heads;
   P->prec = a->precision;
   P->train = a->training != 0;
-  P->grads_accumulate = (a->flags & GPS_FLAG_GRADS_ACCUMULATE) != 0;
-  P->grads_prezeroed = (a->flags & GPS_FLAG_GRADS_ZEROED) != 0 || P->grads_accumulate;
-  auto drop = [&](float p, int site) {
-    DropCfg c;
-    c.p = P->train ? p : 0.f;
-    c.seed = a->seed; c.offset = a->offset; c.site = site;
-    c.offset_dev = (const unsigned long long*)a->offset_dev;
-    return c;
-  };
-  P->drop_attn = drop(a->dropout, GPS_SITE_GR_ATTN);
-  P->drop_mlp = drop(a->mlp_dropout, GPS_SITE_GR_MLP);
-  P->drop_out = drop(a->dropout, GPS_SITE_GR_OUT);
+  set_grad_flags(P, a->flags);
+  P->drop_attn = drop_cfg(a->dropout, P->train, a->seed, a->offset, a->offset_dev, GPS_SITE_GR_ATTN);
+  P->drop_mlp = drop_cfg(a->mlp_dropout, P->train, a->seed, a->offset, a->offset_dev, GPS_SITE_GR_MLP);
+  P->drop_out = drop_cfg(a->dropout, P->train, a->seed, a->offset, a->offset_dev, GPS_SITE_GR_OUT);
   P->pa = P->train ? a->attn_dropout : 0.f;
   P->use_planes = d % 8 == 0;
   const bool lo = a->precision == GPS_PREC_FP32;
-  auto mkplanes = [&](Arena& A, int64_t rows, int64_t cols) {
-    Planes q;
-    if (!P->use_planes) return q;
-    q.ld = round_up(cols, 8);
-    q.hi = A.alloc<__nv_bfloat16>(rows * q.ld + 8);
-    q.lo = lo ? A.alloc<__nv_bfloat16>(rows * q.ld + 8) : nullptr;
-    return q;
-  };
 
   Arena S(bind ? a->saved : nullptr, a->saved_bytes);
   P->stat = S.alloc<float>(4 * N);
@@ -89,14 +73,16 @@ int make_plan(const GpsGraphormerArgs* a, GrPlan* P, bool bind) {
   P->h2 = S.alloc<float>(N * d);
   P->hid = S.alloc<float>(N * d);
   P->hid_pre = S.alloc<float>(N * d);
-  P->h_p = mkplanes(S, N, d);
-  P->O_p = mkplanes(S, N, d);
-  P->h2_p = mkplanes(S, N, d);
-  P->hid_p = mkplanes(S, N, d);
-  P->win_p = mkplanes(S, 3 * d, d);
-  P->wout_p = mkplanes(S, d, d);
-  P->w1_p = mkplanes(S, d, d);
-  P->w2_p = mkplanes(S, d, d);
+  if (P->use_planes) {
+    P->h_p = arena_planes(S, N, d, lo);
+    P->O_p = arena_planes(S, N, d, lo);
+    P->h2_p = arena_planes(S, N, d, lo);
+    P->hid_p = arena_planes(S, N, d, lo);
+    P->win_p = arena_planes(S, 3 * d, d, lo);
+    P->wout_p = arena_planes(S, d, d, lo);
+    P->w1_p = arena_planes(S, d, d, lo);
+    P->w2_p = arena_planes(S, d, d, lo);
+  }
   P->saved_bytes = S.used;
   GPS_REQUIRE(!S.overflow, GPS_ERR_ARG, "graphormer: saved buffer too small (%lld < %lld)", (long long)a->saved_bytes,
               (long long)S.used);
@@ -104,7 +90,7 @@ int make_plan(const GpsGraphormerArgs* a, GrPlan* P, bool bind) {
   // the wgmma forward when the graphs fill its tiles (as GPSLayer decides, layer.cu)
   P->attn_tc = P->use_planes && attention_tc_supported(P->hd) && a->graph.B > 0 && N >= 64 * a->graph.B;
   Arena F(bind ? a->workspace : nullptr, a->workspace_bytes);
-  if (P->attn_tc) P->qkv_p = mkplanes(F, N, 3 * P->H * attention_tc_hd_pad(P->hd));
+  if (P->attn_tc) P->qkv_p = arena_planes(F, N, 3 * P->H * attention_tc_hd_pad(P->hd), lo);
   P->fwd_bytes = F.used;
 
   Arena Bk(bind ? a->workspace : nullptr, a->workspace_bytes);
@@ -118,10 +104,12 @@ int make_plan(const GpsGraphormerArgs* a, GrPlan* P, bool bind) {
   P->gY = Bk.alloc<float>(N * 3 * d);
   P->g_h = Bk.alloc<float>(N * d);
   P->part = Bk.alloc<float>(layernorm_part_floats(d));
-  P->ga_p = mkplanes(Bk, N, d);
-  P->ghid_p = mkplanes(Bk, N, d);
-  P->gb_p = mkplanes(Bk, N, d);
-  P->gY_p = mkplanes(Bk, N, 3 * d);
+  if (P->use_planes) {
+    P->ga_p = arena_planes(Bk, N, d, lo);
+    P->ghid_p = arena_planes(Bk, N, d, lo);
+    P->gb_p = arena_planes(Bk, N, d, lo);
+    P->gY_p = arena_planes(Bk, N, 3 * d, lo);
+  }
   P->bwd_bytes = Bk.used;
   return GPS_OK;
 }
@@ -238,11 +226,7 @@ int graphormer_backward(const GpsGraphormerArgs* a, const GpsAttnBias* bias, cud
     if (!P.grads_prezeroed) {
       const GpsLinear* ls[6] = {&a->input_norm, &a->attn_in, &a->attn_out, &a->mlp_norm, &a->mlp_lin1, &a->mlp_lin2};
       const int64_t rows[6] = {d, 3 * d, d, d, d, d}, cols[6] = {1, d, d, 1, d, d};
-      for (int i = 0; i < 6; ++i) {
-        if (ls[i]->grad_weight)
-          GPS_CUDA(cudaMemsetAsync(ls[i]->grad_weight, 0, (size_t)(rows[i] * cols[i]) * sizeof(float), st));
-        if (ls[i]->grad_bias) GPS_CUDA(cudaMemsetAsync(ls[i]->grad_bias, 0, (size_t)rows[i] * sizeof(float), st));
-      }
+      GPS_TRY(zero_linear_grads(ls, rows, cols, 6, st));
     }
     if (bias && bias->grad_bias)
       GPS_CUDA(cudaMemsetAsync(bias->grad_bias, 0, (size_t)(a->graph.B * P.H * bias->nmax * bias->nmax) * sizeof(float),

@@ -411,13 +411,9 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
               GPS_ERR_ARG, "dropout probabilities must be in [0,1)");
   P->train = a->training != 0;
   P->prec = a->precision;
-  P->dropout.p = P->train && a->dropout > 0.f ? a->dropout : 0.f;
-  P->dropout.seed = a->seed;
-  P->dropout.offset = a->offset;
-  P->dropout.offset_dev = (const unsigned long long*)a->offset_dev;
+  P->dropout = drop_cfg(a->dropout, P->train, a->seed, a->offset, a->offset_dev, 0);
   P->pa = P->train ? a->attn_dropout : 0.f;
-  P->grads_accumulate = (a->flags & GPS_FLAG_GRADS_ACCUMULATE) != 0;
-  P->grads_prezeroed = (a->flags & GPS_FLAG_GRADS_ZEROED) != 0 || P->grads_accumulate;
+  set_grad_flags(P, a->flags);
   list_weights(a, P);
   const int64_t N = P->N, E = P->E, d = P->d;
   const bool gelu = a->act == GPS_ACT_GELU;
@@ -500,48 +496,41 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
   if (!P->nonorm) P->t = S.alloc<float>(N * d);   // norm2's input
   P->use_planes = (d % 8 == 0) && (!P->perf || P->inner % 8 == 0);
   const bool lo = a->precision == GPS_PREC_FP32;
-  auto mkplanes = [&](Arena& A, int64_t rows, int64_t cols) {
-    Planes q;
-    q.ld = round_up(cols, 8);
-    q.hi = A.alloc<__nv_bfloat16>(rows * q.ld + 8);
-    q.lo = lo ? A.alloc<__nv_bfloat16>(rows * q.ld + 8) : nullptr;
-    return q;
-  };
   if (P->use_planes) {
     const int64_t kout = P->perf ? P->inner : d;
     // inputs: the planes written by the previous layer of the stack when it hands them over
     P->x_p = caller_planes(a->x_planes_in, d, a->precision);
-    if (!P->x_p.hi) P->x_p = mkplanes(S, N, d);
+    if (!P->x_p.hi) P->x_p = arena_planes(S, N, d, lo);
     if (P->gated || P->gine) {
       P->e_p = caller_planes(a->e_planes_in, d, a->precision);
-      if (!P->e_p.hi) P->e_p = mkplanes(S, E, d);
+      if (!P->e_p.hi) P->e_p = arena_planes(S, E, d, lo);
     }
-    if (P->glob) P->O_p = mkplanes(S, N, kout);
+    if (P->glob) P->O_p = arena_planes(S, N, kout, lo);
     if (P->bb) {
-      P->bb_a_p = mkplanes(S, N, d);
-      P->bb_u_p = mkplanes(S, N, d);
+      P->bb_a_p = arena_planes(S, N, d, lo);
+      P->bb_u_p = arena_planes(S, N, d, lo);
     }
     // Forward softmax attention on the tensor cores (attention_tc.cu) when the batch's graphs are large enough for
     // 128 x 128 tiles to pay: at the PCQM4M shape (mean 14 nodes per graph) a 128-row tile sees ~45 useful keys of 256
     // in one latency-bound wave and the CUDA-core kernel is faster; the tensor-core kernel wins once a graph fills a
     // tile (ogbg-code2 shape, mean 125 / max ~1000 nodes).
     P->attn_tc = P->attn && attention_tc_supported(P->hd) && a->graph.B > 0 && N >= 64 * a->graph.B;
-    if (P->attn_tc) P->qkv_p = mkplanes(S, N, 3 * P->H * attention_tc_hd_pad(P->hd));
-    P->s_p = mkplanes(S, N, d);
-    P->hid_p = mkplanes(S, N, 2 * d);
+    if (P->attn_tc) P->qkv_p = arena_planes(S, N, 3 * P->H * attention_tc_hd_pad(P->hd), lo);
+    P->s_p = arena_planes(S, N, d, lo);
+    P->hid_p = arena_planes(S, N, 2 * d, lo);
     if (P->gine) {
-      P->agg_p = mkplanes(S, N, d);
-      P->h1_p = mkplanes(S, N, d);
+      P->agg_p = arena_planes(S, N, d, lo);
+      P->h1_p = arena_planes(S, N, d, lo);
     }
     if (P->gen) {
-      P->gen_u_p = mkplanes(S, N, d);
-      P->gen_r_p = mkplanes(S, N, 2 * d);
+      P->gen_u_p = arena_planes(S, N, d, lo);
+      P->gen_r_p = arena_planes(S, N, 2 * d, lo);
     }
     if (P->pna) {   // edge_attr is de wide: planes of its own, never the caller's d-wide ones
-      P->e_p = mkplanes(S, E, P->de);
-      P->pna_F_p = mkplanes(S, d, P->de);
-      P->pna_Z_p = mkplanes(S, N, 4 * d);
-      P->pna_h_p = mkplanes(S, N, d);
+      P->e_p = arena_planes(S, E, P->de, lo);
+      P->pna_F_p = arena_planes(S, d, P->de, lo);
+      P->pna_Z_p = arena_planes(S, N, 4 * d, lo);
+      P->pna_h_p = arena_planes(S, N, d, lo);
     }
     // weight planes: in the caller's persistent buffer when one is given (packed once per optimiser step), else in `saved`
     Arena Wa(bind ? a->wplanes : nullptr, a->wplanes_bytes);
@@ -549,7 +538,7 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
     const int64_t w0 = WA.used;
     for (int i = 0; i < P->nweights; ++i) {
       const LayerWeight& w = P->weights[i];
-      if (w.row0 == 0) P->*w.planes = mkplanes(WA, w.planes == &Plan::Wcat_p ? P->Wy : w.lin.rows, w.cols);
+      if (w.row0 == 0) P->*w.planes = arena_planes(WA, w.planes == &Plan::Wcat_p ? P->Wy : w.lin.rows, w.cols, lo);
     }
     P->wplanes_bytes = WA.used - w0;
     GPS_REQUIRE(!Wa.overflow, GPS_ERR_ARG, "wplanes buffer too small (%lld < %lld)", (long long)a->wplanes_bytes,
@@ -650,34 +639,34 @@ static int make_plan(const GpsLayerArgs* a, Plan* P, bool bind) {
     P->g_xl = Bk.alloc<float>(N * d);
   }
   if (P->use_planes) {
-    P->gt_p = mkplanes(Bk, N, d);
-    P->ghid_p = mkplanes(Bk, N, 2 * d);
-    if (P->glob && !P->nonorm) P->ghA_p = mkplanes(Bk, N, d);
+    P->gt_p = arena_planes(Bk, N, d, lo);
+    P->ghid_p = arena_planes(Bk, N, 2 * d, lo);
+    if (P->glob && !P->nonorm) P->ghA_p = arena_planes(Bk, N, d, lo);
     if (P->bb) {
-      P->bb_god_p = mkplanes(Bk, N, d);
-      P->bb_gu_p = mkplanes(Bk, N, d);
-      P->bb_gso_p = mkplanes(Bk, N, d);
+      P->bb_god_p = arena_planes(Bk, N, d, lo);
+      P->bb_gu_p = arena_planes(Bk, N, d, lo);
+      P->bb_gso_p = arena_planes(Bk, N, d, lo);
     }
-    if (P->nonorm) P->gs_p = mkplanes(Bk, N, d);
-    if (P->gated) P->ge_p = mkplanes(Bk, E, d);
-    if (P->Wy) P->gY1_p = mkplanes(Bk, N, P->Wy);
+    if (P->nonorm) P->gs_p = arena_planes(Bk, N, d, lo);
+    if (P->gated) P->ge_p = arena_planes(Bk, E, d, lo);
+    if (P->Wy) P->gY1_p = arena_planes(Bk, N, P->Wy, lo);
     if (a->dropout > 0.f || (P->perf && a->attn_dropout > 0.f)) {
-      P->gtmp_p = mkplanes(Bk, N, d);
-      P->gtmp2_p = mkplanes(Bk, N, d);
-      P->gtmp3_p = mkplanes(Bk, N, d);
+      P->gtmp_p = arena_planes(Bk, N, d, lo);
+      P->gtmp2_p = arena_planes(Bk, N, d, lo);
+      P->gtmp3_p = arena_planes(Bk, N, d, lo);
     }
     if (P->gine) {
-      if (!P->nonorm) P->gl1_p = mkplanes(Bk, N, d);
-      P->gh1_p = mkplanes(Bk, N, d);
+      if (!P->nonorm) P->gl1_p = arena_planes(Bk, N, d, lo);
+      P->gh1_p = arena_planes(Bk, N, d, lo);
     }
     if (P->gen) {
-      if (!P->nonorm) P->gl1_p = mkplanes(Bk, N, d);
-      P->gen_gh1_p = mkplanes(Bk, N, 2 * d);
+      if (!P->nonorm) P->gl1_p = arena_planes(Bk, N, d, lo);
+      P->gen_gh1_p = arena_planes(Bk, N, 2 * d, lo);
     }
     if (P->pna) {
-      if (!P->nonorm) P->gl1_p = mkplanes(Bk, N, d);
-      P->pna_gh_p = mkplanes(Bk, N, d);
-      P->pna_gq_p = mkplanes(Bk, E, d);
+      if (!P->nonorm) P->gl1_p = arena_planes(Bk, N, d, lo);
+      P->pna_gh_p = arena_planes(Bk, N, d, lo);
+      P->pna_gq_p = arena_planes(Bk, E, d, lo);
     }
   }
   P->bwd_bytes = Bk.used;

@@ -1,5 +1,6 @@
-// layer_ops.cuh — host-side building blocks of the layer orchestrations (layer.cu: GPSLayer, graphormer.cu: the
-// Graphormer layer): side streams, the dense products of a Linear and its gradients, and the dropout-only pass.
+// layer_ops.cuh — host-side building blocks of the layer orchestrations (layer.cu: GPSLayer, graphormer.cu, san.cu,
+// custom_gnn.cu): side streams, the plan prologue, the dense products of a Linear and its gradients, and the
+// dropout-only pass.
 // The plan-typed helpers read P.prec (GPS_PREC_*), and linear_wgrad also P.grads_prezeroed.
 #pragma once
 #include <algorithm>
@@ -42,6 +43,44 @@ struct Side {
 
 // the side streams of the current device, created on its first use (layer.cu)
 int side_stream(Side** out);
+
+// ------------------------------------------------------------------------------- plan prologue
+// The bf16 planes of a [rows, cols] operand, carved from A: ld = cols rounded up to 8, rows * ld + 8 elements per
+// plane, and the lo plane only in fp32 mode (lo = true).
+inline Planes arena_planes(Arena& A, int64_t rows, int64_t cols, bool lo) {
+  Planes q;
+  q.ld = round_up(cols, 8);
+  q.hi = A.alloc<__nv_bfloat16>(rows * q.ld + 8);
+  q.lo = lo ? A.alloc<__nv_bfloat16>(rows * q.ld + 8) : nullptr;
+  return q;
+}
+
+// One dropout site of a call; p = 0 in eval mode
+inline DropCfg drop_cfg(float p, bool train, uint64_t seed, uint64_t offset, const uint64_t* offset_dev, int site) {
+  DropCfg c;
+  c.p = train ? p : 0.f;
+  c.seed = seed; c.offset = offset; c.site = site;
+  c.offset_dev = (const unsigned long long*)offset_dev;
+  return c;
+}
+
+// P->grads_accumulate / P->grads_prezeroed from GPS_FLAG_GRADS_*: accumulating buffers are never zeroed either
+template <class PlanT>
+inline void set_grad_flags(PlanT* P, int flags) {
+  P->grads_accumulate = (flags & GPS_FLAG_GRADS_ACCUMULATE) != 0;
+  P->grads_prezeroed = (flags & GPS_FLAG_GRADS_ZEROED) != 0 || P->grads_accumulate;
+}
+
+// zero the gradients of n Linears, weight [rows[i], cols[i]] and bias [rows[i]]: a backward over no rows writes none
+inline int zero_linear_grads(const GpsLinear* const* ls, const int64_t* rows, const int64_t* cols, int n,
+                             cudaStream_t st) {
+  for (int i = 0; i < n; ++i) {
+    if (ls[i]->grad_weight)
+      GPS_CUDA(cudaMemsetAsync(ls[i]->grad_weight, 0, (size_t)(rows[i] * cols[i]) * sizeof(float), st));
+    if (ls[i]->grad_bias) GPS_CUDA(cudaMemsetAsync(ls[i]->grad_bias, 0, (size_t)rows[i] * sizeof(float), st));
+  }
+  return GPS_OK;
+}
 
 // ------------------------------------------------------------------------------- dense products
 // An operand: fp32 values with leading dimension ld and, where the layer keeps them, their bf16 planes.

@@ -625,27 +625,11 @@ int make_plan(const GpsSanArgs* a, SanPlan* P, bool bind) {
   P->prec = a->precision;
   P->gamma = a->gamma;
   P->train = a->training != 0;
-  P->grads_accumulate = (a->flags & GPS_FLAG_GRADS_ACCUMULATE) != 0;
-  P->grads_prezeroed = (a->flags & GPS_FLAG_GRADS_ZEROED) != 0 || P->grads_accumulate;
-  auto drop = [&](int site) {
-    DropCfg c;
-    c.p = P->train ? a->dropout : 0.f;
-    c.seed = a->seed; c.offset = a->offset; c.site = site;
-    c.offset_dev = (const unsigned long long*)a->offset_dev;
-    return c;
-  };
-  P->drop_attn = drop(GPS_SITE_SAN_ATTN);
-  P->drop_ffn = drop(GPS_SITE_SAN_FFN);
+  set_grad_flags(P, a->flags);
+  P->drop_attn = drop_cfg(a->dropout, P->train, a->seed, a->offset, a->offset_dev, GPS_SITE_SAN_ATTN);
+  P->drop_ffn = drop_cfg(a->dropout, P->train, a->seed, a->offset, a->offset_dev, GPS_SITE_SAN_FFN);
   P->use_planes = d % 8 == 0;
   const bool lo = a->precision == GPS_PREC_FP32;
-  auto mkplanes = [&](Arena& A, int64_t rows, int64_t cols) {
-    Planes q;
-    if (!P->use_planes) return q;
-    q.ld = round_up(cols, 8);
-    q.hi = A.alloc<__nv_bfloat16>(rows * q.ld + 8);
-    q.lo = lo ? A.alloc<__nv_bfloat16>(rows * q.ld + 8) : nullptr;
-    return q;
-  };
 
   Arena S(bind ? a->saved : nullptr, a->saved_bytes);
   if (!P->use_planes) P->Wcat = S.alloc<float>(5 * d * d);
@@ -661,16 +645,18 @@ int make_plan(const GpsSanArgs* a, SanPlan* P, bool bind) {
   P->hid = S.alloc<float>(N * 2 * d);
   P->z2 = S.alloc<float>(N * d);
   P->bnbuf = S.alloc<float>(2 * 2 * d);
-  P->Wcat_p = mkplanes(S, 5 * d, d);
-  P->WE_p = mkplanes(S, d, d);
-  P->WO_p = mkplanes(S, d, d);
-  P->W1_p = mkplanes(S, 2 * d, d);
-  P->W2_p = mkplanes(S, d, 2 * d);
-  P->x_p = mkplanes(S, N, d);
-  P->e_p = mkplanes(S, E, d);
-  P->attnd_p = mkplanes(S, N, d);
-  P->h1_p = mkplanes(S, N, d);
-  P->hid_p = mkplanes(S, N, 2 * d);
+  if (P->use_planes) {
+    P->Wcat_p = arena_planes(S, 5 * d, d, lo);
+    P->WE_p = arena_planes(S, d, d, lo);
+    P->WO_p = arena_planes(S, d, d, lo);
+    P->W1_p = arena_planes(S, 2 * d, d, lo);
+    P->W2_p = arena_planes(S, d, 2 * d, lo);
+    P->x_p = arena_planes(S, N, d, lo);
+    P->e_p = arena_planes(S, E, d, lo);
+    P->attnd_p = arena_planes(S, N, d, lo);
+    P->h1_p = arena_planes(S, N, d, lo);
+    P->hid_p = arena_planes(S, N, 2 * d, lo);
+  }
   P->saved_bytes = S.used;
   GPS_REQUIRE(!S.overflow, GPS_ERR_ARG, "san: saved buffer too small (%lld < %lld)", (long long)a->saved_bytes,
               (long long)S.used);
@@ -691,11 +677,13 @@ int make_plan(const GpsSanArgs* a, SanPlan* P, bool bind) {
   P->Dq = Bk.alloc<float>(N * P->H);
   P->pq = Bk.alloc<float>(N * d);
   P->part = Bk.alloc<float>(san_parts(N) * d);
-  P->gz2_p = mkplanes(Bk, N, d);
-  P->ghid_p = mkplanes(Bk, N, 2 * d);
-  P->gz1_p = mkplanes(Bk, N, d);
-  P->gY_p = mkplanes(Bk, N, 5 * d);
-  P->gE_p = mkplanes(Bk, E, d);
+  if (P->use_planes) {
+    P->gz2_p = arena_planes(Bk, N, d, lo);
+    P->ghid_p = arena_planes(Bk, N, 2 * d, lo);
+    P->gz1_p = arena_planes(Bk, N, d, lo);
+    P->gY_p = arena_planes(Bk, N, 5 * d, lo);
+    P->gE_p = arena_planes(Bk, E, d, lo);
+  }
   P->bwd_bytes = Bk.used;
   return GPS_OK;
 }
@@ -808,11 +796,7 @@ int zero_grads(const GpsSanArgs* a, const SanPlan& P, cudaStream_t st) {
   const int64_t d = P.d;
   const GpsLinear* ls[10] = {&a->Q, &a->K, &a->V, &a->Q2, &a->K2, &a->E, &a->E2, &a->O_h, &a->ffn1, &a->ffn2};
   const int64_t rows[10] = {d, d, d, d, d, d, d, d, 2 * d, d}, cols[10] = {d, d, d, d, d, d, d, d, d, 2 * d};
-  for (int i = 0; i < 10; ++i) {
-    if (ls[i]->grad_weight)
-      GPS_CUDA(cudaMemsetAsync(ls[i]->grad_weight, 0, (size_t)(rows[i] * cols[i]) * sizeof(float), st));
-    if (ls[i]->grad_bias) GPS_CUDA(cudaMemsetAsync(ls[i]->grad_bias, 0, (size_t)rows[i] * sizeof(float), st));
-  }
+  GPS_TRY(zero_linear_grads(ls, rows, cols, 10, st));
   for (const GpsBatchNorm* b : {&a->bn1, &a->bn2}) {
     if (b->grad_weight) GPS_CUDA(cudaMemsetAsync(b->grad_weight, 0, (size_t)d * sizeof(float), st));
     if (b->grad_bias) GPS_CUDA(cudaMemsetAsync(b->grad_bias, 0, (size_t)d * sizeof(float), st));

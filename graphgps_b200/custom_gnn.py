@@ -19,80 +19,18 @@ GINE leaves batch.edge_attr unchanged; it still receives its gradient.  There is
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 import torch.nn as nn
 
 from . import _lib
-from .gps_layer import _bn, _lin, _next_dropout_offset, _workspace
+from ._call import LayerFn, PlanCache, batch_norm, check_params, linear, read_edge_attr, read_x, weight_planes
 from .graph import graph_of
 
-_dropout_calls = [0]
 _ACTS = ("relu", "gelu")
 
 
-class _CustomGnnFn(torch.autograd.Function):
-    """One autograd node for the layer: forward = gps_custom_gnn_forward, backward = gps_custom_gnn_backward."""
-
-    @staticmethod
-    def forward(ctx, layer, gs, x, e, *params):
-        lib = _lib.load()
-        dev = x.device
-        named = dict(zip(layer._param_names, params))
-        args = layer._args(gs, named)
-        saved_bytes, ws_bytes, wp_bytes = layer._plan(args, gs)
-        x_out = torch.empty_like(x)
-        e_out = torch.empty_like(e) if layer._gated else None
-        saved = torch.empty(max(saved_bytes, 256), dtype=torch.uint8, device=dev)
-        ws = _workspace(dev, ws_bytes)
-        wp = layer._weight_buffer(dev, wp_bytes, params, args)
-        args.x, args.edge_attr, args.x_out, args.edge_out = x.data_ptr(), e.data_ptr(), x_out.data_ptr(), _lib.ptr(e_out)
-        args.saved, args.saved_bytes = saved.data_ptr(), saved.numel()
-        args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-        snap = None
-        if layer.training and layer.dropout > 0:
-            snap = _next_dropout_offset(dev)
-            args.offset, args.offset_dev = 0, snap.data_ptr()
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gps_custom_gnn_forward(C.byref(args), stream), "gps_custom_gnn_forward")
-        ctx.layer, ctx.gs, ctx.saved_buf, ctx.wp, ctx.snap = layer, gs, saved, wp, snap
-        ctx.seed, ctx.offset, ctx.training = args.seed, args.offset, bool(args.training)
-        ctx.save_for_backward(x, e, *params)
-        return (x_out, e_out) if layer._gated else x_out
-
-    @staticmethod
-    def backward(ctx, g_x_out, g_e_out=None):
-        lib = _lib.load()
-        layer, gs = ctx.layer, ctx.gs
-        x, e, *params = ctx.saved_tensors
-        dev = x.device
-        named = dict(zip(layer._param_names, params))
-        grads = {n: torch.empty_like(p) for n, p in named.items()}   # written whole by the library
-        args = layer._args(gs, named, grads)
-        args.seed, args.offset, args.training = ctx.seed, ctx.offset, 1 if ctx.training else 0
-        if ctx.snap is not None:
-            args.offset_dev = ctx.snap.data_ptr()
-        g_x_out = g_x_out.contiguous()
-        g_e_out = g_e_out.contiguous() if g_e_out is not None else None
-        g_x = torch.empty_like(x)
-        g_e = torch.empty_like(e) if ctx.needs_input_grad[3] else None
-        _, ws_bytes, _ = layer._plan(args, gs)
-        ws = _workspace(dev, ws_bytes)
-        args.x, args.edge_attr = x.data_ptr(), e.data_ptr()
-        args.grad_x_out, args.grad_edge_out = g_x_out.data_ptr(), _lib.ptr(g_e_out)
-        args.grad_x, args.grad_edge_attr = g_x.data_ptr(), _lib.ptr(g_e)
-        args.saved, args.saved_bytes = ctx.saved_buf.data_ptr(), ctx.saved_buf.numel()
-        args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-        args.wplanes, args.wplanes_bytes, args.wplanes_valid = ctx.wp.data_ptr(), ctx.wp.numel(), 1
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gps_custom_gnn_backward(C.byref(args), stream), "gps_custom_gnn_backward")
-        # (ctx.saved_buf stays alive with the autograd node: backward(retain_graph=True) may run again)
-        return (None, None, g_x, g_e) + tuple(grads[n] for n in layer._param_names)
-
-
 class _CustomGnnBase(nn.Module):
-    """What both layers share: argument block, plan cache, persistent weight buffer and forward."""
+    """What both layers share: argument block, plan key, weight planes and forward."""
 
     _gated = False
 
@@ -107,12 +45,15 @@ class _CustomGnnBase(nn.Module):
         if not 1 <= int(out_dim) <= 4096:
             raise NotImplementedError(f"graphgps_b200.{name}: needs 1 <= out_dim <= 4096 (got {out_dim})")
 
-    def _args(self, gs, named, grads=None):
+    # ------------------------------------------------------------------ hooks of _call.LayerFn; call = the graph
+    _entry = "gps_custom_gnn"
+
+    def _dropout_live(self):
+        return self.dropout > 0
+
+    def _args(self, gs, inputs, named, grads=None):
         g = grads or {}
-        for n, t in named.items():
-            if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
-                raise TypeError(f"graphgps_b200.{type(self).__name__}: parameter '{n}' must be a contiguous float32 "
-                                f"CUDA tensor (got {t.dtype} on {t.device})")
+        check_params(self, named)
         a = _lib.GpsCustomGnnArgs()
         a.d = self.out_dim
         a.kind = _lib.CUSTOM_GATEDGCN if self._gated else _lib.CUSTOM_GINE
@@ -121,82 +62,50 @@ class _CustomGnnBase(nn.Module):
         a.precision = _lib.PRECISION[self.precision]
         a.residual = 1 if self.residual else 0
         a.dropout = float(self.dropout)
-        a.seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
-        _dropout_calls[0] += 1
-        a.offset = _dropout_calls[0] * 4096
         a.graph = gs.desc
 
         def lin(prefix):
             w, b = prefix + ".weight", prefix + ".bias"
-            return _lin(named[w], named[b], g.get(w), g.get(b))
+            return linear(named[w], named[b], g.get(w), g.get(b))
 
         if self._gated:
             a.A, a.B, a.C, a.D, a.E = (lin(n) for n in "ABCDE")
-            a.bn_node_x = _bn(self.bn_node_x, g.get("bn_node_x.weight"), g.get("bn_node_x.bias"))
-            a.bn_edge_e = _bn(self.bn_edge_e, g.get("bn_edge_e.weight"), g.get("bn_edge_e.bias"))
+            a.bn_node_x = batch_norm(self.bn_node_x, g.get("bn_node_x.weight"), g.get("bn_node_x.bias"))
+            a.bn_edge_e = batch_norm(self.bn_edge_e, g.get("bn_edge_e.weight"), g.get("bn_edge_e.bias"))
         else:
             a.nn0, a.nn2 = lin("model.nn.0"), lin("model.nn.2")
             a.gine_eps = self._eps_host()
         return a
 
     def _plan(self, args, gs):
-        """(saved_bytes, workspace_bytes, wplanes_bytes); gps_custom_gnn_plan is pure in its arguments' sizes and
-        modes."""
-        key = (gs.N, gs.E, self.precision, bool(args.training), self.dropout > 0)
-        hit = self._plan_cache.get(key)
-        if hit is None:
-            plan = _lib.GpsCustomGnnPlan()
-            _lib.check(_lib.load().gps_custom_gnn_plan(C.byref(args), C.byref(plan)), "gps_custom_gnn_plan")
-            hit = (int(plan.saved_bytes), int(max(plan.fwd_workspace_bytes, plan.bwd_workspace_bytes)),
-                   int(plan.wplanes_bytes))
-            if len(self._plan_cache) > 64:
-                self._plan_cache.clear()
-            self._plan_cache[key] = hit
-        return hit
+        """gps_custom_gnn_plan is pure in its arguments' sizes and modes."""
+        return self._plans((gs.N, gs.E, self.precision, bool(args.training), self.dropout > 0), args)
 
-    def _weight_buffer(self, dev, nbytes, params, args):
-        """The padded weight planes this forward and its backward read (the autograd node holds the buffer).
+    def _bind_forward(self, args, gs, inputs, plan, params):
+        x, e = inputs
+        x_out = torch.empty_like(x)
+        e_out = torch.empty_like(e) if self._gated else None
+        wp = weight_planes(self, args, plan[2], params, x.device)
+        args.x, args.edge_attr, args.x_out, args.edge_out = x.data_ptr(), e.data_ptr(), x_out.data_ptr(), _lib.ptr(e_out)
+        return ((x_out, e_out) if self._gated else (x_out,)), (), wp
 
-        A packed buffer is never written again: while every parameter is the same tensor at the same version, forwards
-        share the layer's current buffer without packing (once per optimiser step); otherwise the forward packs into a
-        fresh one, so a backward still outstanding reads the weights its own forward used.  Under CUDA-graph capture
-        each call packs into a buffer of its own from the graph's pool, which every replay re-packs."""
-        def fresh():
-            return torch.empty(max(nbytes, 256), dtype=torch.uint8, device=dev)
+    def _grads(self, named):
+        grads = {n: torch.empty_like(p) for n, p in named.items()}   # the library writes every gradient whole
+        return grads, 0, tuple(grads[n] for n in self._param_names)
 
-        valid = 0
-        if torch.cuda.is_current_stream_capturing():
-            buf = fresh()
-        else:
-            key = (tuple((p.data_ptr(), p._version) for p in params), self.precision, dev)
-            cur = self.__dict__.get("_wplanes")
-            if cur is not None and cur[1] == key and cur[0].numel() >= nbytes:
-                buf, valid = cur[0], 1
-            else:
-                buf = fresh()
-                self.__dict__["_wplanes"] = (buf, key)
-        args.wplanes, args.wplanes_bytes, args.wplanes_valid = buf.data_ptr(), buf.numel(), valid
-        return buf
+    def _bind_backward(self, args, gs, inputs, g_outs, needs, wp):
+        x, e = inputs
+        g_x = torch.empty_like(x)
+        g_e = torch.empty_like(e) if needs[1] else None
+        args.x, args.edge_attr = x.data_ptr(), e.data_ptr()
+        args.grad_x_out, args.grad_edge_out = g_outs[0].data_ptr(), _lib.ptr(g_outs[1]) if self._gated else 0
+        args.grad_x, args.grad_edge_attr = g_x.data_ptr(), _lib.ptr(g_e)
+        args.wplanes, args.wplanes_bytes, args.wplanes_valid = wp.data_ptr(), wp.numel(), 1
+        return (g_x, g_e), ()
 
     def forward(self, batch):
-        x = batch.x
-        name = type(self).__name__
-        if not x.is_cuda:
-            raise RuntimeError(f"graphgps_b200.{name} runs on CUDA tensors only; there is no CPU fallback")
-        if x.dtype != torch.float32:
-            raise TypeError("batch.x must be float32")
-        d = self.out_dim
-        if x.dim() != 2 or x.shape[1] != d:
-            raise ValueError(f"batch.x must have shape [num_nodes, {d}] (got {tuple(x.shape)})")
-        e = getattr(batch, "edge_attr", None)
-        if e is None:
-            raise ValueError(f"graphgps_b200.{name} needs batch.edge_attr")
-        if not torch.is_tensor(e) or e.dtype != torch.float32 or e.device != x.device:
-            raise TypeError("batch.edge_attr must be a float32 tensor on the device of batch.x")
-        E = int(batch.edge_index.shape[1])
-        if e.dim() != 2 or tuple(e.shape) != (E, d):
-            raise ValueError(f"batch.edge_attr must have shape [num_edges, {d}] = [{E}, {d}] (got {tuple(e.shape)})")
-        x, e = x.contiguous(), e.contiguous()
+        x = read_x(batch, self, self.out_dim)
+        e = read_edge_attr(batch, x, self, self.out_dim)
         gs = graph_of(batch)
         if self._gated and self.training:
             # a BatchNorm over no rows counts the batch and leaves its running statistics alone, as torch's does;
@@ -207,7 +116,7 @@ class _CustomGnnBase(nn.Module):
                 if gs.E == 0:
                     self.bn_edge_e.num_batches_tracked.add_(1)
         params = [p for _, p in self.named_parameters()]
-        out = _CustomGnnFn.apply(self, gs, x, e, *params)
+        out = LayerFn.apply(self, gs, x, e, *params)
         if self._gated:
             batch.x, batch.edge_attr = out
         else:
@@ -247,7 +156,7 @@ class GatedGCNLayer(_CustomGnnBase):
         self.EquivStablePE = False
         self.precision = precision
         self._param_names = [n for n, _ in self.named_parameters()]
-        self._plan_cache = {}
+        self._plans = PlanCache(self._entry, _lib.GpsCustomGnnPlan)
 
     def __repr__(self):
         return "{}({}, {}, residual={}, act={}, backend=libgps_b200(sm_90a), precision={})".format(
@@ -277,7 +186,7 @@ class GINEConvLayer(_CustomGnnBase):
         self.model = _GINEConvParams(dim_in, dim_out)
         self.precision = precision
         self._param_names = [n for n, _ in self.named_parameters()]
-        self._plan_cache = {}
+        self._plans = PlanCache(self._entry, _lib.GpsCustomGnnPlan)
 
     def _eps_host(self):
         """model.eps as a float, read from the buffer once per change of it (load_state_dict bumps its version)."""

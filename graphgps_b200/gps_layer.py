@@ -11,7 +11,6 @@ There is NO fallback: CPU tensors or a missing library raise.
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 
 import torch
@@ -19,7 +18,10 @@ import torch.nn as nn
 
 from . import _lib
 from .bigbird import BigBirdConfig, BigBirdParams, device_lists, gps_bigbird, padded_length
-from .graph import graph_of
+from ._call import _drop_counters  # noqa: F401  (the dropout counters, reachable here as before)
+from ._call import (LayerFn, PlanCache, check_params, linear, read_attn_bias, read_x, weight_planes,
+                    zeroed_grads)
+from .graph import _cache_get, _cache_put, graph_of
 
 _SUPPORTED_LOCAL = ("None", "CustomGatedGCN", "GINE", "GCN", "GAT", "GENConv", "PNA")
 # local models that read batch.edge_attr (gps_layer.py:44-90)
@@ -32,59 +34,7 @@ _MHA_GLOBAL = ("Transformer", "BiasedTransformer")   # torch's MultiheadAttentio
 _GLOBAL_ABI = dict(_lib.GLOBAL, BiasedTransformer=_lib.GLOBAL["Transformer"])
 _ACT_MODULES = {"relu": nn.ReLU, "gelu": nn.GELU}
 
-_workspaces = {}
-_dropout_calls = [0]
-_drop_counters = {}
-
-
-def _next_dropout_offset(device):
-    """Device-resident Philox offset for this call: counter += 4096; snapshot = counter.
-
-    Kept on the device (two tiny stream-ordered ops) so that a captured CUDA graph draws fresh dropout
-    masks on every replay; the snapshot tensor is what forward and backward of this call both read."""
-    ctr = _drop_counters.get(device)
-    if ctr is None:
-        ctr = torch.zeros(1, dtype=torch.int64, device=device)
-        _drop_counters[device] = ctr
-    ctr.add_(4096)
-    return ctr.clone()
-
-
-def _workspace(device, nbytes):
-    """Transient scratch for one C call, one buffer per (device, stream): layers running on different streams never
-    share it, and a buffer is never freed while the process lives (a captured CUDA graph may hold its address) -
-    growth keeps the old ones.  Under stream capture the buffer is allocated from the graph's own pool instead."""
-    if torch.cuda.is_current_stream_capturing():
-        return torch.empty(int(nbytes) + 256, dtype=torch.uint8, device=device)
-    key = (device, torch.cuda.current_stream(device).cuda_stream)
-    held = _workspaces.setdefault(key, [])
-    if not held or held[-1].numel() < nbytes:
-        held.append(torch.empty(int(nbytes * 1.25) + 256, dtype=torch.uint8, device=device))
-    return held[-1]
-
-
 _PLANES_ATTR = "_gps_b200_planes"
-
-
-def _batch_planes_get(batch):
-    try:
-        v = getattr(batch, _PLANES_ATTR, None)
-    except Exception:
-        v = None
-    return v if isinstance(v, dict) else None
-
-
-def _batch_planes_put(batch, produced, lo):
-    """Remember, on the batch object, the operand planes this layer wrote next to its outputs, keyed by the identity
-    (address, version, shape) of the tensors they mirror: the next GPSLayer uses them only if batch.x / batch.edge_attr
-    are still exactly those tensors."""
-    rec = {}
-    for name, (t, buf) in (produced or {}).items():
-        rec[name] = ((t.data_ptr(), t._version, tuple(t.shape), lo), buf)
-    try:
-        setattr(batch, _PLANES_ATTR, rec)
-    except Exception:
-        pass
 
 
 class _GatedGCNParams(nn.Module):
@@ -232,120 +182,6 @@ class _PerformerParams(nn.Module):
         self.to_out = nn.Linear(inner, dim, bias=True)
 
 
-def _lin(weight, bias, gw=None, gb=None):
-    return _lib.GpsLinear(_lib.ptr(weight), _lib.ptr(bias), _lib.ptr(gw), _lib.ptr(gb))
-
-
-def _bn(mod, gw=None, gb=None):
-    return _lib.GpsBatchNorm(_lib.ptr(mod.weight), _lib.ptr(mod.bias), _lib.ptr(mod.running_mean),
-                             _lib.ptr(mod.running_var), _lib.ptr(mod.num_batches_tracked),
-                             _lib.ptr(gw), _lib.ptr(gb))
-
-
-class _GPSLayerFn(torch.autograd.Function):
-    """One autograd node for the whole layer: forward = gps_layer_forward, backward = gps_layer_backward."""
-
-    @staticmethod
-    def forward(ctx, layer, gs, x, e, pe, bias, *params):
-        lib = _lib.load()
-        dev = x.device
-        named = dict(zip(layer._param_names, params))
-        pe_k = pe.shape[1] if layer._eslap else 0
-        args = layer._base_args(gs, named, pe_k=pe_k)
-        ctx.nmax = gs.nmax if bias.numel() else 0
-        ctx.bb = layer.__dict__.pop("_bb_lists", None)
-        layer._batch_args(args, pe, bias, ctx.nmax, ctx.bb)
-        x_out = torch.empty_like(x)
-        e_out = torch.empty_like(e) if layer.local_gnn_type == "CustomGatedGCN" else None
-        plan = layer._plan(args, gs)
-        saved = torch.empty(max(plan[0], 256), dtype=torch.uint8, device=dev)
-        ws = _workspace(dev, plan[1])
-        args.x, args.edge_attr = x.data_ptr(), _lib.ptr(e)
-        args.x_out, args.edge_out = x_out.data_ptr(), _lib.ptr(e_out)
-        args.saved, args.saved_bytes = saved.data_ptr(), saved.numel()
-        args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-        hand = layer._handoff_args(args, plan, params, x, e, x_out, e_out)
-        snap = None
-        if layer.training and (layer.dropout > 0 or layer.attn_dropout > 0):
-            snap = _next_dropout_offset(dev)
-            args.offset, args.offset_dev = 0, snap.data_ptr()
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gps_layer_forward(C.byref(args), stream), "gps_layer_forward")
-        ctx.layer, ctx.gs, ctx.saved_buf, ctx.snap = layer, gs, saved, snap
-        ctx.hand = hand
-        ctx.seed, ctx.offset, ctx.training = args.seed, args.offset, bool(args.training)
-        ctx.save_for_backward(x, e, pe, bias, *params)
-        if e_out is not None:
-            return x_out, e_out
-        return x_out
-
-    @staticmethod
-    def backward(ctx, g_x_out, g_e_out=None):
-        lib = _lib.load()
-        layer, gs = ctx.layer, ctx.gs
-        x, e, pe, bias, *params = ctx.saved_tensors
-        dev = x.device
-        named = dict(zip(layer._param_names, params))
-        pe_k = pe.shape[1] if layer._eslap else 0
-        bucket = layer._bucket_grads(named)
-        if bucket is not None:
-            # static gradient bucket (graphgps_b200.dp.GradBucket): the library ADDS this call's gradients to the
-            # parameters' .grad views in place (torch's accumulation semantics), so CUDA-graph replays and the
-            # gradient all-reduce see the same memory
-            grads = bucket
-            args = layer._base_args(gs, named, grads, pe_k=pe_k)
-            args.flags = _lib.FLAG_GRADS_ACCUMULATE
-        else:
-            grads = {n: torch.empty_like(p) for n, p in named.items()}
-            torch._foreach_zero_(list(grads.values()))   # one multi-tensor fill; the library then skips its memsets
-            args = layer._base_args(gs, named, grads, pe_k=pe_k)
-            args.flags = _lib.FLAG_GRADS_ZEROED
-        g_pe = None
-        if pe_k and ctx.needs_input_grad[4]:
-            g_pe = torch.empty_like(pe)
-            args.grad_pe = g_pe.data_ptr()
-        g_bias = None
-        if ctx.nmax and ctx.needs_input_grad[5]:
-            g_bias = torch.empty_like(bias)
-        layer._batch_args(args, pe, bias, ctx.nmax, ctx.bb, g_bias)
-        args.seed, args.offset, args.training = ctx.seed, ctx.offset, 1 if ctx.training else 0
-        if ctx.snap is not None:
-            args.offset_dev = ctx.snap.data_ptr()
-        g_x_out = g_x_out.contiguous()
-        gated = layer.local_gnn_type == "CustomGatedGCN"
-        if g_e_out is not None:
-            g_e_out = g_e_out.contiguous()
-        g_x = torch.empty_like(x)
-        g_e = torch.empty_like(e) if layer.local_gnn_type in _EDGE_LOCAL else None
-        plan = layer._plan(args, gs)
-        ws = _workspace(dev, plan[1])
-        args.x, args.edge_attr = x.data_ptr(), _lib.ptr(e)
-        args.grad_x_out = g_x_out.data_ptr()
-        args.grad_edge_out = _lib.ptr(g_e_out) if gated else 0
-        args.grad_x, args.grad_edge_attr = g_x.data_ptr(), _lib.ptr(g_e)
-        args.saved, args.saved_bytes = ctx.saved_buf.data_ptr(), ctx.saved_buf.numel()
-        args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-        if ctx.hand is not None:
-            args.x_planes_in, args.e_planes_in, args.wplanes, args.wplanes_bytes = ctx.hand[:4]
-            args.wplanes_valid = 1
-        evs = layer.__dict__.get("grad_events")
-        if evs is not None:
-            args.ev_grads_early, args.ev_grads_mid, args.ev_grads_done = (e.cuda_event for e in evs)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gps_layer_backward(C.byref(args), stream), "gps_layer_backward")
-        # (ctx.saved_buf stays alive with the autograd node: backward(retain_graph=True) may run again)
-        if bucket is not None:
-            return (None, None, g_x, g_e, g_pe, g_bias) + (None,) * len(layer._param_names)
-        # parameters the configuration never reads get no gradient (as under autograd in the reference)
-        unused = []
-        if layer.local_gnn_type == "None":
-            unused.append("norm1_local.")
-        if layer.global_model_type == "None":
-            unused.append("norm1_attn.")
-        pg = tuple(None if any(n.startswith(u) for u in unused) else grads[n] for n in layer._param_names)
-        return (None, None, g_x, g_e, g_pe, g_bias) + pg
-
-
 class GPSLayer(nn.Module):
     """Local MPNN + full graph attention x-former layer (reference: gps_layer.py:16-264)."""
 
@@ -469,15 +305,107 @@ class GPSLayer(nn.Module):
         self._grad_shapes = [tuple(p.shape) for _, p in self.named_parameters()]
         self._grad_sizes = [p.numel() for _, p in self.named_parameters()]
         self._grad_numel = sum(self._grad_sizes)
-        self._plan_cache = {}
+        self._plans = PlanCache(self._entry, _lib.GpsLayerPlan)
+
+    # ------------------------------------------------------------------ hooks of _call.LayerFn
+    _entry = "gps_layer"
+    _check_params = check_params
+
+    def _dropout_live(self):
+        return self.dropout > 0 or self.attn_dropout > 0
+
+    def _args(self, call, inputs, named, grads=None):
+        """GpsLayerArgs with configuration, graph, parameter (+gradient) and per-batch pointers filled in.
+
+        The forward-direction struct (no gradient pointers) only depends on the parameter addresses and the
+        module flags, so it is cached and copied; building ~30 nested ctypes structs per call costs more host
+        time than the GPU needs for the whole layer at the ZINC shape.  The per-batch fields never enter the cache:
+        the EquivStableLapPE pointer, the BiasedTransformer's attention bias and BigBird's block count and lists."""
+        x, e, pe, bias = inputs
+        pe_k = pe.shape[1] if self._eslap else 0
+        if grads is None:
+            key = (tuple(t.data_ptr() for t in named.values()), self.training, self.precision,
+                   float(self.dropout), float(self.attn_dropout), pe_k > 0, pe_k)
+            cached = self.__dict__.get("_args_cache")
+            if cached is None or cached[0] != key:
+                self._check_params(named)
+                cached = (key, self._build_args(named, None, pe_k))
+                self.__dict__["_args_cache"] = cached
+            a = _lib.GpsLayerArgs.from_buffer_copy(cached[1])
+        else:
+            a = self._build_args(named, grads, pe_k)
+        a.graph = call["gs"].desc
+        if self._eslap:
+            a.pe = pe.data_ptr()
+        if call["nmax"]:
+            a.attn_bias = _lib.GpsAttnBias(bias.data_ptr(), call["nmax"], 0)
+        if call["bb"] is not None:
+            lists, nb = call["bb"]
+            b = a.bigbird   # a view into a
+            b.num_blocks = nb
+            b.key_ptr, b.key_idx, b.query_ptr, b.query_idx = (t.data_ptr() for t in lists)
+        return a
+
+    def _plan(self, args, call):
+        """gps_layer_plan is pure in (config, N, E, B, training, precision, PE width)."""
+        gs = call["gs"]
+        return self._plans((gs.N, gs.E, gs.B, bool(self.training), self.precision, float(self.dropout),
+                            float(self.attn_dropout), bool(args.pe), int(args.pe_dim)), args)
+
+    def _bind_forward(self, args, call, inputs, plan, params):
+        x, e = inputs[:2]
+        x_out = torch.empty_like(x)
+        e_out = torch.empty_like(e) if self.local_gnn_type == "CustomGatedGCN" else None
+        args.x, args.edge_attr = x.data_ptr(), _lib.ptr(e)
+        args.x_out, args.edge_out = x_out.data_ptr(), _lib.ptr(e_out)
+        hand = self._handoff_args(args, plan, params, call, x, e, x_out, e_out)
+        return ((x_out,) if e_out is None else (x_out, e_out)), (), hand
+
+    def _grads(self, named):
+        bucket = self._bucket_grads(named)
+        if bucket is not None:
+            # static gradient bucket (graphgps_b200.dp.GradBucket): the library ADDS this call's gradients to the
+            # parameters' .grad views in place (torch's accumulation semantics), so CUDA-graph replays and the
+            # gradient all-reduce see the same memory
+            return bucket, _lib.FLAG_GRADS_ACCUMULATE, (None,) * len(self._param_names)
+        grads = zeroed_grads(named)
+        # parameters the configuration never reads get no gradient (as under autograd in the reference)
+        unused = []
+        if self.local_gnn_type == "None":
+            unused.append("norm1_local.")
+        if self.global_model_type == "None":
+            unused.append("norm1_attn.")
+        pg = tuple(None if any(n.startswith(u) for u in unused) else grads[n] for n in self._param_names)
+        return grads, _lib.FLAG_GRADS_ZEROED, pg
+
+    def _bind_backward(self, args, call, inputs, g_outs, needs, hand):
+        x, e, pe, bias = inputs
+        g_pe = torch.empty_like(pe) if self._eslap and needs[2] else None
+        g_bias = torch.empty_like(bias) if call["nmax"] and needs[3] else None
+        g_x = torch.empty_like(x)
+        g_e = torch.empty_like(e) if self.local_gnn_type in _EDGE_LOCAL else None
+        args.grad_pe = _lib.ptr(g_pe)
+        args.attn_bias.grad_bias = _lib.ptr(g_bias)
+        args.x, args.edge_attr = x.data_ptr(), _lib.ptr(e)
+        args.grad_x_out = g_outs[0].data_ptr()
+        args.grad_edge_out = _lib.ptr(g_outs[1]) if self.local_gnn_type == "CustomGatedGCN" else 0
+        args.grad_x, args.grad_edge_attr = g_x.data_ptr(), _lib.ptr(g_e)
+        if hand is not None:
+            args.x_planes_in, args.e_planes_in, args.wplanes, args.wplanes_bytes = hand[:4]
+            args.wplanes_valid = 1
+        evs = self.__dict__.get("grad_events")
+        if evs is not None:
+            args.ev_grads_early, args.ev_grads_mid, args.ev_grads_done = (ev.cuda_event for ev in evs)
+        return (g_x, g_e, g_pe, g_bias), ()
 
     # ------------------------------------------------------------------ operand planes across layers / steps
-    def _handoff_args(self, args, plan, params, x, e, x_out, e_out):
-        """Fills the ABI-3 plane fields: (i) the bf16 hi/lo planes of x / edge_attr that the previous GPSLayer of the
+    def _handoff_args(self, args, plan, params, call, x, e, x_out, e_out):
+        """Fills the plane fields: (i) the bf16 hi/lo planes of x / edge_attr that the previous GPSLayer of the
         model wrote next to its outputs (gps_model.py:100,105-108 chains the layers on one batch object), so this layer
         skips converting its inputs; (ii) plane buffers for this layer's own outputs; (iii) the persistent weight-plane
-        buffer, re-packed only when a parameter changed (once per optimiser step, not once per forward call).
-        Returns what backward needs to see again, and keeps the buffers alive through the autograd node."""
+        buffer (_call.weight_planes).  Returns what backward needs to see again, and keeps the buffers alive through
+        the autograd node."""
+        src = call.pop("planes_in") or {}
         if plan[2] <= 0 or not self.__dict__.get("plane_handoff", True):
             return None
         dev = x.device
@@ -490,7 +418,6 @@ class GPSLayer(nn.Module):
         keep = []
         zero = _lib.GpsPlanes(0, 0, 0)
         xin, ein = zero, zero
-        src = self.__dict__.pop("_planes_in", None) or {}
         for name, t in (("x", x), ("e", e)):
             h = src.get(name)
             if h is not None and h[0] == (t.data_ptr(), t._version, tuple(t.shape), lo):
@@ -507,18 +434,8 @@ class GPSLayer(nn.Module):
         if e_out is not None:
             eb, args.e_planes_out = planes_of(e_out)
             out["e"] = (e_out, eb)
-        self.__dict__["_planes_out"] = out
-        # persistent weight planes
-        key = (tuple((p.data_ptr(), p._version) for p in params), self.precision, plan[2])
-        wp = self.__dict__.get("_wplanes")
-        if wp is None or wp[0].numel() < plan[2] or wp[0].device != dev:
-            wp = [torch.empty(plan[2] + 256, dtype=torch.uint8, device=dev), None]
-            self.__dict__["_wplanes"] = wp
-        args.wplanes, args.wplanes_bytes = wp[0].data_ptr(), wp[0].numel()
-        capturing = torch.cuda.is_current_stream_capturing()
-        args.wplanes_valid = 1 if (wp[1] == key and not capturing) else 0   # a captured graph always re-packs
-        wp[1] = key
-        keep.append(wp[0])
+        call["planes_out"] = out
+        keep.append(weight_planes(self, args, plan[2], params, dev))
         return (xin, ein, args.wplanes, args.wplanes_bytes, keep)
 
     def _bucket_grads(self, named):
@@ -535,53 +452,7 @@ class GPSLayer(nn.Module):
             out[n] = g
         return out
 
-    def _plan(self, args, gs):
-        """(saved_bytes, workspace_bytes); gps_layer_plan is pure in (config, N, E, B, training, precision, PE width)."""
-        key = (gs.N, gs.E, gs.B, bool(self.training), self.precision, float(self.dropout), float(self.attn_dropout),
-               bool(args.pe), int(args.pe_dim))
-        hit = self._plan_cache.get(key)
-        if hit is None:
-            plan = _lib.GpsLayerPlan()
-            _lib.check(_lib.load().gps_layer_plan(C.byref(args), C.byref(plan)), "gps_layer_plan")
-            hit = (int(plan.saved_bytes), int(max(plan.fwd_workspace_bytes, plan.bwd_workspace_bytes)),
-                   int(plan.wplanes_bytes))
-            if len(self._plan_cache) > 64:
-                self._plan_cache.clear()
-            self._plan_cache[key] = hit
-        return hit
-
     # ------------------------------------------------------------------------------------
-    def _base_args(self, gs, named, grads=None, pe_k=0):
-        """GpsLayerArgs with configuration, graph and parameter (+gradient) pointers filled in.
-
-        The forward-direction struct (no gradient pointers) only depends on the parameter addresses and the
-        module flags, so it is cached and copied; building ~30 nested ctypes structs per call costs more host
-        time than the GPU needs for the whole layer at the ZINC shape."""
-        if grads is None:
-            key = (tuple(t.data_ptr() for t in named.values()), self.training, self.precision,
-                   float(self.dropout), float(self.attn_dropout), pe_k > 0, pe_k)
-            cached = self.__dict__.get("_args_cache")
-            if cached is None or cached[0] != key:
-                self._check_params(named)
-                cached = (key, self._build_args(named, None, pe_k))
-                self.__dict__["_args_cache"] = cached
-            a = _lib.GpsLayerArgs.from_buffer_copy(cached[1])
-        else:
-            a = self._build_args(named, grads, pe_k)
-        a.seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
-        _dropout_calls[0] += 1
-        a.offset = _dropout_calls[0] * 4096
-        a.graph = gs.desc
-        return a
-
-    def _check_params(self, named):
-        """The library reads raw fp32 device pointers: refuse anything else (the reference would cast or raise)."""
-        bufs = {n: b for n, b in self.named_buffers() if b.is_floating_point()}
-        for n, t in list(named.items()) + list(bufs.items()):
-            if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
-                raise TypeError(f"graphgps_b200.GPSLayer: parameter/buffer '{n}' must be a contiguous float32 CUDA "
-                                f"tensor (got {t.dtype} on {t.device})")
-
     def _build_args(self, named, grads, pe_k=0):
         g = grads or {}
         a = _lib.GpsLayerArgs()
@@ -595,7 +466,7 @@ class GPSLayer(nn.Module):
         a.norm_type = _lib.NORM["batch" if self.batch_norm else "none"]
 
         def lin(prefix, bias=True):
-            return _lin(named[prefix + ".weight"], named.get(prefix + ".bias") if bias else None,
+            return linear(named[prefix + ".weight"], named.get(prefix + ".bias") if bias else None,
                         g.get(prefix + ".weight"), g.get(prefix + ".bias") if bias else None)
 
         def bn(prefix, mod):
@@ -616,12 +487,12 @@ class GPSLayer(nn.Module):
             a.gine_lin0, a.gine_lin1 = lin("local_model.nn.0"), lin("local_model.nn.2")
             a.gine_eps = float(self._gine_eps_host)
         elif self.local_gnn_type == "GCN":
-            a.gcn_conv = _lin(named["local_model.lin.weight"], named["local_model.bias"],
+            a.gcn_conv = linear(named["local_model.lin.weight"], named["local_model.bias"],
                               g.get("local_model.lin.weight"), g.get("local_model.bias"))
         elif self.local_gnn_type == "GAT":   # lin_src carries GATConv.bias, as GCNConv's lin / bias pair
             p = "local_model."
             a.gat = _lib.GpsGat(
-                _lin(named[p + "lin_src.weight"], named[p + "bias"], g.get(p + "lin_src.weight"), g.get(p + "bias")),
+                linear(named[p + "lin_src.weight"], named[p + "bias"], g.get(p + "lin_src.weight"), g.get(p + "bias")),
                 lin(p + "lin_edge", False),
                 *(_lib.ptr(named[p + n]) for n in ("att_src", "att_dst", "att_edge")),
                 *(_lib.ptr(g.get(p + n)) for n in ("att_src", "att_dst", "att_edge")))
@@ -632,7 +503,7 @@ class GPSLayer(nn.Module):
             a.pna = _lib.GpsPna(lin("local_model.edge_encoder"), lin("local_model.pre_nns.0.0"),
                                 lin("local_model.post_nns.0.0"), lin("local_model.lin"), self.local_model.edge_dim)
         if self.global_model_type in _MHA_GLOBAL:
-            a.attn_in = _lin(named["self_attn.in_proj_weight"], named["self_attn.in_proj_bias"],
+            a.attn_in = linear(named["self_attn.in_proj_weight"], named["self_attn.in_proj_bias"],
                              g.get("self_attn.in_proj_weight"), g.get("self_attn.in_proj_bias"))
             a.attn_out = lin("self_attn.out_proj")
         elif self.global_model_type == "Performer":
@@ -649,19 +520,6 @@ class GPSLayer(nn.Module):
             a.norm2 = bn("norm2", self.norm2)
         a.ff1, a.ff2 = lin("ff_linear1"), lin("ff_linear2")
         return a
-
-    def _batch_args(self, args, pe, bias, nmax, bb, g_bias=None):
-        """Fills the fields of args that change with every batch, and so never enter the cached struct: the
-        EquivStableLapPE pointer, the BiasedTransformer's attention bias and BigBird's block count and lists."""
-        if self._eslap:
-            args.pe = pe.data_ptr()
-        if nmax:
-            args.attn_bias = _lib.GpsAttnBias(bias.data_ptr(), nmax, _lib.ptr(g_bias))
-        if bb is not None:
-            lists, nb = bb
-            b = args.bigbird   # a view into args
-            b.num_blocks = nb
-            b.key_ptr, b.key_idx, b.query_ptr, b.query_idx = (t.data_ptr() for t in lists)
 
     def _bigbird_lists(self, x, gs):
         """(block lists, nb) of this batch: nb from Nmax padded to the block size; NotImplementedError (before any
@@ -682,13 +540,7 @@ class GPSLayer(nn.Module):
         return v
 
     def forward(self, batch):
-        x = batch.x
-        if not x.is_cuda:
-            raise RuntimeError("graphgps_b200.GPSLayer runs on CUDA tensors only; there is no CPU fallback "
-                               "(use the oracle under oracle/ for CPU checks)")
-        if x.dtype != torch.float32:
-            raise TypeError("batch.x must be float32")
-        x = x.contiguous()
+        x = read_x(batch, self)
         e = getattr(batch, "edge_attr", None)
         if self.local_gnn_type == "PNA":   # PNAConv(edge_dim=min(128, dim_h)): the edge encoder's input width
             if e is None or e.dim() != 2 or e.shape[-1] != self.local_model.edge_dim:
@@ -705,21 +557,24 @@ class GPSLayer(nn.Module):
             e = None
         pe = self._read_pe(batch, x) if self._eslap else None
         gs = graph_of(batch)
-        bias = self._read_attn_bias(batch, x, gs) if self.global_model_type == "BiasedTransformer" else None
-        if self.global_model_type == "BigBird":
-            self.__dict__["_bb_lists"] = self._bigbird_lists(x, gs)
+        # batch.attn_bias (gps_layer.py:202-204): missing is an AttributeError, as in the reference
+        bias = read_attn_bias(batch, x, gs, self, True) if self.global_model_type == "BiasedTransformer" else None
+        call = {"gs": gs, "nmax": gs.nmax if bias is not None else 0,
+                "bb": self._bigbird_lists(x, gs) if self.global_model_type == "BigBird" else None,
+                "planes_in": _cache_get(batch, _PLANES_ATTR, dict)}
         params = [p for _, p in self.named_parameters()]
-        e_arg = e if e is not None else x.new_empty(0)
-        pe_arg = pe if pe is not None else x.new_empty(0)
-        bias_arg = bias if bias is not None else x.new_empty(0)
-        self.__dict__["_planes_in"] = _batch_planes_get(batch)
-        out = _GPSLayerFn.apply(self, gs, x, e_arg, pe_arg, bias_arg, *params)
-        produced = self.__dict__.pop("_planes_out", None)
+        empty = x.new_empty(0)
+        out = LayerFn.apply(self, call, x, empty if e is None else e, empty if pe is None else pe,
+                            empty if bias is None else bias, *params)
         if self.local_gnn_type == "CustomGatedGCN":
             batch.x, batch.edge_attr = out           # gps_layer.py:173-174, :231
         else:
             batch.x = out
-        _batch_planes_put(batch, produced, self.precision == "fp32")
+        # the operand planes this layer wrote next to its outputs, keyed by the identity (address, version, shape) of
+        # the tensors they mirror: the next GPSLayer uses them only if batch.x / batch.edge_attr are still those tensors
+        lo = self.precision == "fp32"
+        _cache_put(batch, {name: ((t.data_ptr(), t._version, tuple(t.shape), lo), buf)
+                           for name, (t, buf) in call.pop("planes_out", {}).items()}, _PLANES_ATTR)
         return batch
 
     @staticmethod
@@ -736,27 +591,6 @@ class GPSLayer(nn.Module):
             raise ValueError(f"batch.pe_EquivStableLapPE must have shape [num_nodes={x.shape[0]}, k >= 1] "
                              f"(got {tuple(pe.shape)})")
         return pe.contiguous()
-
-    def _read_attn_bias(self, batch, x, gs):
-        """batch.attn_bias [num_graphs * heads, Nmax, Nmax] (gps_layer.py:202-204), row g * heads + h for graph g and
-        head h, Nmax = the largest graph: float32 on the device of x.  Missing: AttributeError, as in the reference;
-        None: no bias, as torch's MultiheadAttention treats attn_mask=None."""
-        if not hasattr(batch, "attn_bias"):
-            raise AttributeError("GPSLayer('BiasedTransformer') reads batch.attn_bias [num_graphs * heads, Nmax, Nmax], "
-                                 "which this batch does not have (Graphormer's BiasEncoder writes it)")
-        ab = batch.attn_bias
-        if ab is None:
-            return None
-        if not torch.is_tensor(ab) or ab.dtype != torch.float32 or ab.device != x.device:
-            raise TypeError("batch.attn_bias must be a float32 tensor on the device of batch.x (got "
-                            f"{getattr(ab, 'dtype', type(ab))} on {getattr(ab, 'device', None)})")
-        want = (gs.B * self.num_heads, gs.nmax, gs.nmax)
-        if tuple(ab.shape) != want:
-            raise ValueError(f"batch.attn_bias must have shape [num_graphs * heads, Nmax, Nmax] = {list(want)} "
-                             f"(got {list(ab.shape)})")
-        if gs.nmax == 0:   # no nodes: nothing attends
-            return None
-        return ab.contiguous()
 
     def extra_repr(self):
         return (f"summary: dim_h={self.dim_h}, local_gnn_type={self.local_gnn_type}, "

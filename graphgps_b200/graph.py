@@ -95,34 +95,35 @@ def _num_graphs(batch_obj) -> int:
     return int(b[-1].item()) + 1 if b.numel() else 0
 
 
-_side_cache = weakref.WeakKeyDictionary()   # batch objects whose attribute protocol does not round-trip
+_side_cache = weakref.WeakKeyDictionary()   # {attribute: value} of batch objects whose attributes do not round-trip
 
 
-def _cache_get(batch_obj):
+def _cache_get(batch_obj, attr=_CACHE_ATTR, typ=GraphStructure):
+    """The value cached on `batch_obj` under `attr` if it is a `typ`, else None (by default its graph structure)."""
     # PyG Data/Batch route setattr/getattr through their storage object (underscore names included), so read the
     # way we write; a plain __dict__ lookup would never hit there and the CSR build would rerun in every layer
     try:
-        hit = getattr(batch_obj, _CACHE_ATTR, None)
+        hit = getattr(batch_obj, attr, None)
     except Exception:
         hit = None
     if hit is None:
         try:
-            hit = _side_cache.get(batch_obj)
+            hit = _side_cache.get(batch_obj, {}).get(attr)
         except TypeError:
             hit = None
-    return hit if isinstance(hit, GraphStructure) else None
+    return hit if isinstance(hit, typ) else None
 
 
-def _cache_put(batch_obj, gs):
+def _cache_put(batch_obj, value, attr=_CACHE_ATTR):
     try:
-        setattr(batch_obj, _CACHE_ATTR, gs)
-        if getattr(batch_obj, _CACHE_ATTR, None) is gs:
+        setattr(batch_obj, attr, value)
+        if getattr(batch_obj, attr, None) is value:
             return
     except Exception:
         pass
     try:
-        _side_cache[batch_obj] = gs
-    except TypeError:  # not weak-referenceable: still works, just rebuilds per layer
+        _side_cache.setdefault(batch_obj, {})[attr] = value
+    except TypeError:  # not weak-referenceable: still works, the value is recomputed per call
         pass
 
 

@@ -19,68 +19,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .gps_layer import _lin, _next_dropout_offset, _workspace
+from ._call import LayerFn, PlanCache, check_params, linear, read_attn_bias, read_x, zeroed_grads
 from .graph import graph_of
-
-_dropout_calls = [0]
-
-
-class _GraphormerFn(torch.autograd.Function):
-    """One autograd node for the layer: forward = gps_graphormer_forward, backward = gps_graphormer_backward."""
-
-    @staticmethod
-    def forward(ctx, layer, gs, x, bias, *params):
-        lib = _lib.load()
-        dev = x.device
-        named = dict(zip(layer._param_names, params))
-        args = layer._args(gs, named)
-        plan = layer._plan(args, gs)
-        x_out = torch.empty_like(x)
-        saved = torch.empty(max(plan[0], 256), dtype=torch.uint8, device=dev)
-        ws = _workspace(dev, plan[1])
-        args.x, args.x_out = x.data_ptr(), x_out.data_ptr()
-        args.saved, args.saved_bytes = saved.data_ptr(), saved.numel()
-        args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-        snap = None
-        if layer.training and layer._any_dropout:
-            snap = _next_dropout_offset(dev)
-            args.offset, args.offset_dev = 0, snap.data_ptr()
-        ctx.nmax = bias.shape[-1] if bias.numel() else 0
-        ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, 0)) if ctx.nmax else None
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gps_graphormer_forward(C.byref(args), ab, stream), "gps_graphormer_forward")
-        ctx.layer, ctx.gs, ctx.saved_buf, ctx.snap = layer, gs, saved, snap
-        ctx.seed, ctx.offset, ctx.training = args.seed, args.offset, bool(args.training)
-        ctx.save_for_backward(x, bias, *params)
-        return x_out
-
-    @staticmethod
-    def backward(ctx, g_x_out):
-        lib = _lib.load()
-        layer, gs = ctx.layer, ctx.gs
-        x, bias, *params = ctx.saved_tensors
-        dev = x.device
-        named = dict(zip(layer._param_names, params))
-        grads = {n: torch.empty_like(p) for n, p in named.items()}
-        torch._foreach_zero_(list(grads.values()))   # one multi-tensor fill; the library then skips its memsets
-        args = layer._args(gs, named, grads)
-        args.flags = _lib.FLAG_GRADS_ZEROED
-        args.seed, args.offset, args.training = ctx.seed, ctx.offset, 1 if ctx.training else 0
-        if ctx.snap is not None:
-            args.offset_dev = ctx.snap.data_ptr()
-        g_x_out = g_x_out.contiguous()
-        g_x = torch.empty_like(x)
-        plan = layer._plan(args, gs)
-        ws = _workspace(dev, plan[1])
-        args.x, args.grad_x_out, args.grad_x = x.data_ptr(), g_x_out.data_ptr(), g_x.data_ptr()
-        args.saved, args.saved_bytes = ctx.saved_buf.data_ptr(), ctx.saved_buf.numel()
-        args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-        g_bias = torch.empty_like(bias) if ctx.nmax and ctx.needs_input_grad[3] else None
-        ab = C.byref(_lib.GpsAttnBias(bias.data_ptr(), ctx.nmax, _lib.ptr(g_bias))) if ctx.nmax else None
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gps_graphormer_backward(C.byref(args), ab, stream), "gps_graphormer_backward")
-        # (ctx.saved_buf stays alive with the autograd node: backward(retain_graph=True) may run again)
-        return (None, None, g_x, g_bias) + tuple(grads[n] for n in layer._param_names)
 
 
 class GraphormerLayer(nn.Module):
@@ -109,18 +49,17 @@ class GraphormerLayer(nn.Module):
         self.p_dropout, self.p_attn, self.p_mlp = float(dropout), float(attention_dropout), float(mlp_dropout)
         self.precision = precision
         self._param_names = [n for n, _ in self.named_parameters()]
-        self._plan_cache = {}
+        self._plans = PlanCache(self._entry, _lib.GpsGraphormerPlan)
 
-    @property
-    def _any_dropout(self):
+    # ------------------------------------------------------------------ hooks of _call.LayerFn; call = the graph
+    _entry = "gps_graphormer"
+
+    def _dropout_live(self):
         return self.p_dropout > 0 or self.p_attn > 0 or self.p_mlp > 0
 
-    def _args(self, gs, named, grads=None):
+    def _args(self, gs, inputs, named, grads=None):
         g = grads or {}
-        for n, t in named.items():
-            if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
-                raise TypeError(f"graphgps_b200.GraphormerLayer: parameter '{n}' must be a contiguous float32 CUDA "
-                                f"tensor (got {t.dtype} on {t.device})")
+        check_params(self, named)
         a = _lib.GpsGraphormerArgs()
         a.d, a.heads = self.embed_dim, self.num_heads
         a.training = 1 if self.training else 0
@@ -128,7 +67,7 @@ class GraphormerLayer(nn.Module):
         a.dropout, a.attn_dropout, a.mlp_dropout = self.p_dropout, self.p_attn, self.p_mlp
 
         def lin(w, b):
-            return _lin(named[w], named[b], g.get(w), g.get(b))
+            return linear(named[w], named[b], g.get(w), g.get(b))
 
         a.input_norm = lin("input_norm.weight", "input_norm.bias")
         a.attn_in = lin("attention.in_proj_weight", "attention.in_proj_bias")
@@ -136,56 +75,42 @@ class GraphormerLayer(nn.Module):
         a.mlp_norm = lin("mlp.0.weight", "mlp.0.bias")
         a.mlp_lin1 = lin("mlp.1.weight", "mlp.1.bias")
         a.mlp_lin2 = lin("mlp.4.weight", "mlp.4.bias")
-        a.seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
-        _dropout_calls[0] += 1
-        a.offset = _dropout_calls[0] * 4096
         a.graph = gs.desc
         return a
 
     def _plan(self, args, gs):
-        """(saved_bytes, workspace_bytes); gps_graphormer_plan is pure in (d, heads, precision, N, B)."""
-        key = (gs.N, gs.B, self.precision)
-        hit = self._plan_cache.get(key)
-        if hit is None:
-            plan = _lib.GpsGraphormerPlan()
-            _lib.check(_lib.load().gps_graphormer_plan(C.byref(args), C.byref(plan)), "gps_graphormer_plan")
-            hit = (int(plan.saved_bytes), int(max(plan.fwd_workspace_bytes, plan.bwd_workspace_bytes)))
-            if len(self._plan_cache) > 64:
-                self._plan_cache.clear()
-            self._plan_cache[key] = hit
-        return hit
+        """gps_graphormer_plan is pure in (d, heads, precision, N, B)."""
+        return self._plans((gs.N, gs.B, self.precision), args)
 
-    def _read_attn_bias(self, batch, x, gs):
-        """The reference's hasattr test (graphormer_layer.py:43-46): no attribute or None = no bias, else
-        batch.attn_bias [num_graphs * heads, Nmax, Nmax], row g * heads + h, float32 on the device of x."""
-        ab = getattr(batch, "attn_bias", None)
-        if ab is None:
-            return None
-        if not torch.is_tensor(ab) or ab.dtype != torch.float32 or ab.device != x.device:
-            raise TypeError("batch.attn_bias must be a float32 tensor on the device of batch.x (got "
-                            f"{getattr(ab, 'dtype', type(ab))} on {getattr(ab, 'device', None)})")
-        want = (gs.B * self.num_heads, gs.nmax, gs.nmax)
-        if tuple(ab.shape) != want:
-            raise ValueError(f"batch.attn_bias must have shape [num_graphs * heads, Nmax, Nmax] = {list(want)} "
-                             f"(got {list(ab.shape)})")
-        if gs.nmax == 0:
-            return None
-        return ab.contiguous()
+    @staticmethod
+    def _attn_bias(bias, g_bias):
+        """The library's second argument: the bias of a batch that has one, else NULL."""
+        return C.byref(_lib.GpsAttnBias(bias.data_ptr(), bias.shape[-1], _lib.ptr(g_bias))) if bias.numel() else None
+
+    def _bind_forward(self, args, gs, inputs, plan, params):
+        x, bias = inputs
+        x_out = torch.empty_like(x)
+        args.x, args.x_out = x.data_ptr(), x_out.data_ptr()
+        return (x_out,), (self._attn_bias(bias, None),), None
+
+    def _grads(self, named):
+        grads = zeroed_grads(named)
+        return grads, _lib.FLAG_GRADS_ZEROED, tuple(grads[n] for n in self._param_names)
+
+    def _bind_backward(self, args, gs, inputs, g_outs, needs, keep):
+        x, bias = inputs
+        g_x = torch.empty_like(x)
+        g_bias = torch.empty_like(bias) if bias.numel() and needs[1] else None
+        args.x, args.grad_x_out, args.grad_x = x.data_ptr(), g_outs[0].data_ptr(), g_x.data_ptr()
+        return (g_x, g_bias), (self._attn_bias(bias, g_bias),)
 
     def forward(self, batch):
-        x = batch.x
-        if not x.is_cuda:
-            raise RuntimeError("graphgps_b200.GraphormerLayer runs on CUDA tensors only; there is no CPU fallback")
-        if x.dtype != torch.float32:
-            raise TypeError("batch.x must be float32")
-        if x.dim() != 2 or x.shape[1] != self.embed_dim:
-            raise ValueError(f"batch.x must have shape [num_nodes, {self.embed_dim}] (got {tuple(x.shape)})")
-        x = x.contiguous()
+        x = read_x(batch, self, self.embed_dim)
         gs = graph_of(batch)
-        bias = self._read_attn_bias(batch, x, gs)
+        # the reference's hasattr test (graphormer_layer.py:43-46): no attribute or None = no bias
+        bias = read_attn_bias(batch, x, gs, self, False)
         params = [p for _, p in self.named_parameters()]
-        bias_arg = bias if bias is not None else x.new_empty(0)
-        batch.x = _GraphormerFn.apply(self, gs, x, bias_arg, *params)
+        batch.x = LayerFn.apply(self, gs, x, x.new_empty(0) if bias is None else bias, *params)
         return batch
 
     def extra_repr(self):

@@ -15,16 +15,15 @@ first call.
 from __future__ import annotations
 
 import ctypes as C
-import weakref
 
 import torch
 import torch.nn as nn
 
 from . import _lib
-from .gps_layer import _workspace
+from ._call import workspace
+from .graph import _cache_get, _cache_put
 
 _META_ATTR = "_gps_b200_bias_meta"
-_side_cache = weakref.WeakKeyDictionary()   # batch objects whose attribute protocol does not round-trip
 
 
 class _BatchMeta:
@@ -39,39 +38,13 @@ def _key(*ts):
     return tuple(None if t is None else (t.data_ptr(), t._version, tuple(t.shape)) for t in ts)
 
 
-def _cache_get(data):
-    try:
-        hit = getattr(data, _META_ATTR, None)
-    except Exception:
-        hit = None
-    if hit is None:
-        try:
-            hit = _side_cache.get(data)
-        except TypeError:
-            hit = None
-    return hit if isinstance(hit, _BatchMeta) else None
-
-
-def _cache_put(data, meta):
-    try:
-        setattr(data, _META_ATTR, meta)
-        if getattr(data, _META_ATTR, None) is meta:
-            return
-    except Exception:
-        pass
-    try:
-        _side_cache[data] = meta
-    except TypeError:   # not weak-referenceable: still correct, the read repeats per call
-        pass
-
-
 def _batch_meta(data, st, gi, spt):
     """Node offsets [>= B+1] on the device and, from one host read, Nmax, B = batch.max() + 1 (to_dense_adj's batch
     size), the number of pairs whose nodes are not both in one graph, and the ranges of the type tensors."""
     bvec = data.batch
     ptr_attr = getattr(data, "ptr", None)
     key = _key(st, gi, spt, bvec, ptr_attr)
-    hit = _cache_get(data)
+    hit = _cache_get(data, _META_ATTR, _BatchMeta)
     if hit is not None and hit.key == key:
         return hit
     if torch.cuda.is_current_stream_capturing():
@@ -103,7 +76,7 @@ def _batch_meta(data, st, gi, spt):
     vals = torch.stack(stats).tolist()   # the one host read per batch
     meta = _BatchMeta(key, ptr, int(vals[0]), int(vals[1]), int(vals[2]) if P else 0,
                       (vals[3], vals[4]) if P else None, (vals[5], vals[6]) if len(vals) > 5 else None)
-    _cache_put(data, meta)
+    _cache_put(data, meta, _META_ATTR)
     return meta
 
 
@@ -141,7 +114,7 @@ class _BiasFn(torch.autograd.Function):
         args.grad_edge_weight, args.grad_graph_token = _lib.ptr(g_ew), _lib.ptr(g_tok)
         plan = _lib.GpsGraphormerBiasPlan()
         _lib.check(lib.gps_graphormer_bias_plan(C.byref(args), C.byref(plan)), "gps_graphormer_bias_plan")
-        ws = _workspace(st.device, plan.bwd_workspace_bytes)
+        ws = workspace(st.device, plan.bwd_workspace_bytes)
         args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
         stream = torch.cuda.current_stream(st.device).cuda_stream
         _lib.check(lib.gps_graphormer_bias_backward(C.byref(args), stream), "gps_graphormer_bias_backward")

@@ -17,81 +17,16 @@ batch (Q_h, K_h, E, wV, Z, ...) are internals and are not reproduced; batch.edge
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 import torch.nn as nn
 
 from . import _lib
-from .gps_layer import _bn, _lin, _next_dropout_offset, _workspace
+from ._call import LayerFn, PlanCache, batch_norm, check_params, linear, read_edge_attr, read_x
 from .graph import graph_of
 
-_dropout_calls = [0]
 # the five node projections, in the order of the fused product [Q | K | V | Q2 | K2]
 _NODE = ("attention.Q.weight", "attention.K.weight", "attention.V.weight", "attention.Q_2.weight",
          "attention.K_2.weight")
-
-
-class _SANFn(torch.autograd.Function):
-    """One autograd node for the layer: forward = gps_san_forward, backward = gps_san_backward."""
-
-    @staticmethod
-    def forward(ctx, layer, gs, nmax, x, e, *params):
-        lib = _lib.load()
-        dev = x.device
-        named = dict(zip(layer._param_names, params))
-        args = layer._args(gs, nmax, named)
-        plan = layer._plan(args, gs, nmax)
-        x_out = torch.empty_like(x)
-        saved = torch.empty(max(plan[0], 256), dtype=torch.uint8, device=dev)
-        ws = _workspace(dev, plan[1])
-        args.x, args.edge_attr, args.x_out = x.data_ptr(), e.data_ptr(), x_out.data_ptr()
-        args.saved, args.saved_bytes = saved.data_ptr(), saved.numel()
-        args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-        snap = None
-        if layer.training and layer.p_dropout > 0:
-            snap = _next_dropout_offset(dev)
-            args.offset, args.offset_dev = 0, snap.data_ptr()
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gps_san_forward(C.byref(args), stream), "gps_san_forward")
-        ctx.layer, ctx.gs, ctx.nmax, ctx.saved_buf, ctx.snap = layer, gs, nmax, saved, snap
-        ctx.seed, ctx.offset, ctx.training = args.seed, args.offset, bool(args.training)
-        ctx.save_for_backward(x, e, *params)
-        return x_out
-
-    @staticmethod
-    def backward(ctx, g_x_out):
-        lib = _lib.load()
-        layer, gs = ctx.layer, ctx.gs
-        x, e, *params = ctx.saved_tensors
-        dev = x.device
-        named = dict(zip(layer._param_names, params))
-        d = layer.out_channels
-        # the five node-projection gradients as views of one [5d, d] buffer: one weight product in the library
-        packed = torch.empty(5 * d, d, device=dev)
-        grads = {n: packed[i * d:(i + 1) * d] for i, n in enumerate(_NODE)}
-        for n, p in named.items():
-            if n not in grads:
-                grads[n] = torch.empty_like(p)
-        torch._foreach_zero_([packed] + [g for n, g in grads.items() if n not in _NODE])
-        args = layer._args(gs, ctx.nmax, named, grads)
-        args.flags = _lib.FLAG_GRADS_ZEROED
-        args.seed, args.offset, args.training = ctx.seed, ctx.offset, 1 if ctx.training else 0
-        if ctx.snap is not None:
-            args.offset_dev = ctx.snap.data_ptr()
-        g_x_out = g_x_out.contiguous()
-        g_x = torch.empty_like(x)
-        g_e = torch.empty_like(e) if ctx.needs_input_grad[4] else None
-        plan = layer._plan(args, gs, ctx.nmax)
-        ws = _workspace(dev, plan[1])
-        args.x, args.edge_attr = x.data_ptr(), e.data_ptr()
-        args.grad_x_out, args.grad_x, args.grad_edge_attr = g_x_out.data_ptr(), g_x.data_ptr(), _lib.ptr(g_e)
-        args.saved, args.saved_bytes = ctx.saved_buf.data_ptr(), ctx.saved_buf.numel()
-        args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gps_san_backward(C.byref(args), stream), "gps_san_backward")
-        # (ctx.saved_buf stays alive with the autograd node: backward(retain_graph=True) may run again)
-        return (None, None, None, g_x, g_e) + tuple(grads[n] for n in layer._param_names)
 
 
 class _SANAttentionParams(nn.Module):
@@ -153,14 +88,17 @@ class SANLayer(nn.Module):
         self.p_dropout = float(dropout)
         self.precision = precision
         self._param_names = [n for n, _ in self.named_parameters()]
-        self._plan_cache = {}
+        self._plans = PlanCache(self._entry, _lib.GpsSanPlan)
 
-    def _args(self, gs, nmax, named, grads=None):
+    # ------------------------------------------------------------------ hooks of _call.LayerFn; call = the graph
+    _entry = "gps_san"
+
+    def _dropout_live(self):
+        return self.p_dropout > 0
+
+    def _args(self, gs, inputs, named, grads=None):
         g = grads or {}
-        for n, t in named.items():
-            if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
-                raise TypeError(f"graphgps_b200.SANLayer: parameter '{n}' must be a contiguous float32 CUDA tensor "
-                                f"(got {t.dtype} on {t.device})")
+        check_params(self, named)
         a = _lib.GpsSanArgs()
         a.d, a.heads = self.out_channels, self.num_heads
         a.training = 1 if self.training else 0
@@ -168,7 +106,7 @@ class SANLayer(nn.Module):
         a.gamma, a.dropout = self.gamma, self.p_dropout
 
         def lin(w, b=None):
-            return _lin(named[w], named[b] if b else None, g.get(w), g.get(b) if b else None)
+            return linear(named[w], named[b] if b else None, g.get(w), g.get(b) if b else None)
 
         a.Q, a.K, a.V = lin("attention.Q.weight"), lin("attention.K.weight"), lin("attention.V.weight")
         a.Q2, a.K2 = lin("attention.Q_2.weight"), lin("attention.K_2.weight")
@@ -176,52 +114,49 @@ class SANLayer(nn.Module):
         a.O_h = lin("O_h.weight", "O_h.bias")
         a.ffn1 = lin("FFN_h_layer1.weight", "FFN_h_layer1.bias")
         a.ffn2 = lin("FFN_h_layer2.weight", "FFN_h_layer2.bias")
-        a.bn1 = _bn(self.batch_norm1_h, g.get("batch_norm1_h.weight"), g.get("batch_norm1_h.bias"))
-        a.bn2 = _bn(self.batch_norm2_h, g.get("batch_norm2_h.weight"), g.get("batch_norm2_h.bias"))
+        a.bn1 = batch_norm(self.batch_norm1_h, g.get("batch_norm1_h.weight"), g.get("batch_norm1_h.bias"))
+        a.bn2 = batch_norm(self.batch_norm2_h, g.get("batch_norm2_h.weight"), g.get("batch_norm2_h.bias"))
         a.fake_edge_emb = named["attention.fake_edge_emb.weight"].data_ptr()
         a.grad_fake_edge_emb = _lib.ptr(g.get("attention.fake_edge_emb.weight"))
-        a.seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
-        _dropout_calls[0] += 1
-        a.offset = _dropout_calls[0] * 4096
         a.graph = gs.desc
-        a.nmax = nmax
+        a.nmax = gs.nmax
         return a
 
-    def _plan(self, args, gs, nmax):
-        """(saved_bytes, workspace_bytes); gps_san_plan is pure in its arguments' sizes and modes."""
-        key = (gs.N, gs.E, gs.B, nmax, self.precision, bool(args.training), self.p_dropout > 0)
-        hit = self._plan_cache.get(key)
-        if hit is None:
-            plan = _lib.GpsSanPlan()
-            _lib.check(_lib.load().gps_san_plan(C.byref(args), C.byref(plan)), "gps_san_plan")
-            hit = (int(plan.saved_bytes), int(max(plan.fwd_workspace_bytes, plan.bwd_workspace_bytes)))
-            if len(self._plan_cache) > 64:
-                self._plan_cache.clear()
-            self._plan_cache[key] = hit
-        return hit
+    def _plan(self, args, gs):
+        """gps_san_plan is pure in its arguments' sizes and modes."""
+        return self._plans((gs.N, gs.E, gs.B, gs.nmax, self.precision, bool(args.training), self.p_dropout > 0), args)
+
+    def _bind_forward(self, args, gs, inputs, plan, params):
+        x, e = inputs
+        x_out = torch.empty_like(x)
+        args.x, args.edge_attr, args.x_out = x.data_ptr(), e.data_ptr(), x_out.data_ptr()
+        return (x_out,), (), None
+
+    def _grads(self, named):
+        d = self.out_channels
+        # the five node-projection gradients as views of one [5d, d] buffer: one weight product in the library
+        packed = torch.empty(5 * d, d, device=named[_NODE[0]].device)
+        grads = {n: packed[i * d:(i + 1) * d] for i, n in enumerate(_NODE)}
+        for n, p in named.items():
+            if n not in grads:
+                grads[n] = torch.empty_like(p)
+        torch._foreach_zero_([packed] + [g for n, g in grads.items() if n not in _NODE])
+        return grads, _lib.FLAG_GRADS_ZEROED, tuple(grads[n] for n in self._param_names)
+
+    def _bind_backward(self, args, gs, inputs, g_outs, needs, keep):
+        x, e = inputs
+        g_x = torch.empty_like(x)
+        g_e = torch.empty_like(e) if needs[1] else None
+        args.x, args.edge_attr = x.data_ptr(), e.data_ptr()
+        args.grad_x_out, args.grad_x, args.grad_edge_attr = g_outs[0].data_ptr(), g_x.data_ptr(), _lib.ptr(g_e)
+        return (g_x, g_e), ()
 
     def forward(self, batch):
-        x = batch.x
-        if not x.is_cuda:
-            raise RuntimeError("graphgps_b200.SANLayer runs on CUDA tensors only; there is no CPU fallback")
-        if x.dtype != torch.float32:
-            raise TypeError("batch.x must be float32")
-        d = self.out_channels
-        if x.dim() != 2 or x.shape[1] != d:
-            raise ValueError(f"batch.x must have shape [num_nodes, {d}] (got {tuple(x.shape)})")
-        e = getattr(batch, "edge_attr", None)
-        if e is None:
-            raise ValueError("graphgps_b200.SANLayer needs batch.edge_attr (the reference projects it with attention.E)")
-        if not torch.is_tensor(e) or e.dtype != torch.float32 or e.device != x.device:
-            raise TypeError("batch.edge_attr must be a float32 tensor on the device of batch.x")
-        E = int(batch.edge_index.shape[1])
-        if e.dim() != 2 or tuple(e.shape) != (E, d):
-            raise ValueError(f"batch.edge_attr must have shape [num_edges, {d}] = [{E}, {d}] (got {tuple(e.shape)})")
-        x, e = x.contiguous(), e.contiguous()
+        x = read_x(batch, self, self.out_channels)
+        e = read_edge_attr(batch, x, self, self.out_channels)
         gs = graph_of(batch)
-        nmax = gs.nmax
         params = [p for _, p in self.named_parameters()]
-        batch.x = _SANFn.apply(self, gs, nmax, x, e, *params)
+        batch.x = LayerFn.apply(self, gs, x, e, *params)
         return batch
 
     def __repr__(self):

@@ -16,7 +16,7 @@ from graphgps_b200.batch import batch_from_lists, make_batch
 from graphgps_b200.graph import graph_of
 from biased_oracle import OracleGPSLayerBiased
 from biased_util import PAD_VALUE, biased_batch, biased_names, compare_biased, load_biased, make_bias, run_biased
-from util import rel_err, rel_l2
+from util import pin_dropout_counter, rel_err, rel_l2
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -220,16 +220,6 @@ def test_layer_large_graphs_take_the_wgmma_forward_and_match_the_oracle():
         assert rel_err(a, r) < 1e-3 or rel_l2(a, r) < 5e-3
 
 
-def _set_dropout_counter(value):
-    from graphgps_b200 import gps_layer
-    dev = torch.device(DEV)
-    ctr = gps_layer._drop_counters.get(dev)
-    if ctr is None:
-        ctr = torch.zeros(1, dtype=torch.int64, device=dev)
-        gps_layer._drop_counters[dev] = ctr
-    ctr.fill_(value)
-
-
 def test_biased_dropout_forward_backward_consistent():
     """With the Philox offset pinned, the layer with attention dropout 0.5 is a deterministic smooth (GELU) function of x
     and attn_bias: its backward equals a central finite difference of its forward along a direction in each."""
@@ -246,7 +236,7 @@ def test_biased_dropout_forward_backward_consistent():
     vb = torch.randn(ab0.shape, generator=g).to(DEV)
 
     def f(x, ab):
-        _set_dropout_counter(7 * 4096)
+        pin_dropout_counter(DEV, 7 * 4096)
         bb = graphgps_b200.GraphBatch(x=x, edge_index=b.edge_index, edge_attr=b.edge_attr.clone(), batch=b.batch,
                                       num_graphs=b.num_graphs, attn_bias=ab)
         out = layer(bb)

@@ -18,7 +18,7 @@ import graphgps_b200
 from graphgps_b200 import _lib, bigbird as bbmod
 from graphgps_b200.graph import graph_of
 from bigbird_oracle import attach_bigbird, bb_batch, bigbird_cfg, bigbird_oracle_layer, multiplicity
-from util import GOLDEN_DIR, compare, golden_batch, rel_err, run_layer
+from util import GOLDEN_DIR, compare, golden_batch, pin_dropout_counter, rel_err, run_layer
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -239,16 +239,6 @@ def test_same_graph_in_two_batches_differs_and_matches_oracle():
     assert float((outs[0] - outs[1]).abs().max()) > 1e-3
 
 
-def _set_dropout_counter(value):
-    from graphgps_b200 import gps_layer
-    dev = torch.device(DEV)
-    ctr = gps_layer._drop_counters.get(dev)
-    if ctr is None:
-        ctr = torch.zeros(1, dtype=torch.int64, device=dev)
-        gps_layer._drop_counters[dev] = ctr
-    ctr.fill_(value)
-
-
 def test_dropout_matches_oracle_with_injected_masks():
     """BigBird's two dropouts (sites 8 and 9) and the GPS dropouts (4: dropout_attn, 5 / 6: the FFN) replayed through
     gps_dropout_mask and injected into the oracle: the comparison is exact up to rounding."""
@@ -263,7 +253,7 @@ def test_dropout_matches_oracle_with_injected_masks():
     b = bb_batch([23, 17, 30, 21, 12], d, seed=2)
     N = b.x.shape[0]
     base = 33 * 4096
-    _set_dropout_counter(base)
+    pin_dropout_counter(DEV, base)
     seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
     masks = {}
     for site, cols in ((4, d), (5, 2 * d), (6, d), (8, d), (9, d)):

@@ -9,11 +9,11 @@ import torch
 import torch.nn as nn
 
 import graphgps_b200
-from graphgps_b200 import _lib, gps_layer
+from graphgps_b200 import _lib
 from graphgps_b200.batch import GraphBatch
 from graphgps_b200.graph import graph_of
 from custom_gnn_oracle import oracle_layer, run_stack, san_batch
-from util import GOLDEN_DIR, rel_err, rel_l2
+from util import GOLDEN_DIR, pin_dropout_counter, rel_err, rel_l2
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -138,15 +138,6 @@ def test_fixture(name, precision):
 
 
 # ------------------------------------------------------------------------------------------ float64 on the GPU
-def _pin(value):
-    dev = torch.device(DEV)
-    ctr = gps_layer._drop_counters.get(dev)
-    if ctr is None:
-        ctr = torch.zeros(1, dtype=torch.int64, device=dev)
-        gps_layer._drop_counters[dev] = ctr
-    ctr.fill_(value)
-
-
 def _mask(rows, cols, p, offset, site, d):
     """The library's keep-mask of a [rows, cols] site at pitch cols, cut to the layer's d columns, scaled."""
     m = torch.empty(rows, cols, device=DEV)
@@ -190,7 +181,7 @@ def _compare_live(kind, d, layers, bkind, sizes, seed, act="relu", residual=True
     N, E, dp = sb.x.shape[0], sb.edge_attr.shape[0], (d + 7) // 8 * 8
     masks = None
     if p > 0:
-        _pin(4096 * 300)
+        pin_dropout_counter(DEV, 4096 * 300)
         masks = [(_mask(N, dp, p, 4096 * (301 + i), 15, d), _mask(E, dp, p, 4096 * (301 + i), 4095, d))
                  for i in range(layers)]
     before = {k: v.clone() for k, v in mod.state_dict().items()}
@@ -314,7 +305,7 @@ def _check_capture(kind, d, p, layers, bkind, sizes, train):
     ct = torch.randn(sb.x.shape, device=DEV)
     x = sb.x.clone().requires_grad_(True)
     e = sb.edge_attr.clone().requires_grad_(True)
-    _pin(4096 * 1000)
+    pin_dropout_counter(DEV, 4096 * 1000)
     eager_g, eager_out = _step(seq, x, e, b, ct)
     eager_out = eager_out.detach()
     x = x.detach().clone().requires_grad_(True)
@@ -328,7 +319,7 @@ def _check_capture(kind, d, p, layers, bkind, sizes, train):
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph, capture_error_mode="thread_local"):
         cap_g, cap_out = _step(seq, x, e, b, ct)
-    _pin(4096 * 1000)
+    pin_dropout_counter(DEV, 4096 * 1000)
     graph.replay()
     torch.cuda.synchronize()
     first = cap_out.clone()

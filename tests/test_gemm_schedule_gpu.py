@@ -6,7 +6,7 @@ import pytest
 import torch
 
 import graphgps_b200
-from graphgps_b200 import _lib, gps_layer
+from graphgps_b200 import _call, _lib
 from graphgps_b200.graph import graph_of
 from util import rel_err
 
@@ -99,8 +99,7 @@ def _layer_step(wl, precision, drop, adrop):
     """One GPSLayer fwd + bwd on the workload's batch: every Linear epilogue of the layer runs (bias, ReLU, dropout,
     residuals, plane outputs, BatchNorm statistics and the fused BatchNorm-backward sums)."""
     spec = graphgps_b200.SHAPES[wl]
-    gps_layer._drop_counters.clear()   # the same dropout masks in every run
-    gps_layer._dropout_calls[0] = 0
+    _call._drop_counters.clear()   # the same dropout masks in every run
     torch.manual_seed(0)
     layer = graphgps_b200.GPSLayer(spec.dim, spec.local_gnn, spec.global_model, spec.heads, dropout=drop,
                                    attn_dropout=adrop, precision=precision).to(DEV).train()
@@ -123,7 +122,7 @@ def _layer_step(wl, precision, drop, adrop):
 
 
 @pytest.mark.parametrize("precision,drop,adrop", [("fp32", 0.0, 0.5), ("fp32", 0.2, 0.2), ("bf16", 0.0, 0.5)])
-def test_layer_bitwise_across_tile_widths(precision, drop, adrop):
+def test_layer_step_bitwise_across_tile_widths(precision, drop, adrop):
     """The pcqm4m-small layer (d = 304, ~3600 nodes) with the policy's widths, run twice, and with every GEMM forced to
     64-wide tiles: all outputs, input and parameter gradients and BatchNorm running statistics are bitwise equal."""
     try:

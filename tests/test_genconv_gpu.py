@@ -24,7 +24,7 @@ from graphgps_b200.graph import graph_of
 import genconv_reference as R
 from biased_util import compare_biased
 from genconv_oracle import dead_node, genconv_batch, genconv_oracle_layer
-from util import GOLDEN_DIR, golden_batch, rel_err, rel_l2, run_layer
+from util import GOLDEN_DIR, golden_batch, pin_dropout_counter, rel_err, rel_l2, run_layer
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -238,16 +238,6 @@ def test_layer_matches_genconv_golden(name, precision):
     assert _lib.load().gps_fallback_count() == fb0
 
 
-def _set_dropout_counter(value):
-    from graphgps_b200 import gps_layer
-    dev = torch.device(DEV)
-    ctr = gps_layer._drop_counters.get(dev)
-    if ctr is None:
-        ctr = torch.zeros(1, dtype=torch.int64, device=dev)
-        gps_layer._drop_counters[dev] = ctr
-    ctr.fill_(value)
-
-
 def test_genconv_dropout_forward_backward_consistent():
     """With the Philox offset pinned, the GENConv+Transformer layer with dropout 0.2 is a deterministic function of x and
     edge_attr: its backward equals a central finite difference of its forward along a direction in each."""
@@ -261,7 +251,7 @@ def test_genconv_dropout_forward_backward_consistent():
     ve = torch.randn(b.edge_attr.shape, generator=g).to(DEV)
 
     def f(x, e):
-        _set_dropout_counter(7 * 4096)
+        pin_dropout_counter(DEV, 7 * 4096)
         bb = GraphBatch(x=x, edge_index=b.edge_index, edge_attr=e, batch=b.batch, num_graphs=b.num_graphs)
         out = layer(bb)
         return (out.x * ct_x).sum(), out

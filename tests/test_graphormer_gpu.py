@@ -9,11 +9,11 @@ import torch
 import torch.nn as nn
 
 import graphgps_b200
-from graphgps_b200 import _lib, gps_layer
+from graphgps_b200 import _lib
 from graphgps_b200.batch import GraphBatch
 from graphgps_b200.graph import graph_of
 from graphormer_oracle import attention, graphormer_batch, graphormer_forward, random_bias
-from util import GOLDEN_DIR, rel_err
+from util import GOLDEN_DIR, pin_dropout_counter, rel_err
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -196,15 +196,6 @@ def test_full_size_actor_graphormer():
 
 
 # ------------------------------------------------------------------------------------------ dropout
-def _pin(value):
-    dev = torch.device(DEV)
-    ctr = gps_layer._drop_counters.get(dev)
-    if ctr is None:
-        ctr = torch.zeros(1, dtype=torch.int64, device=dev)
-        gps_layer._drop_counters[dev] = ctr
-    ctr.fill_(value)
-
-
 def test_dropout_backward_is_derivative_of_forward():
     """All four sites active, offset pinned: the layer is a fixed smooth function; its backward equals a central finite
     difference of its forward along a random direction (x, bias and one weight)."""
@@ -219,7 +210,7 @@ def test_dropout_backward_is_derivative_of_forward():
     vx, vb, vw = (torch.randn(t.shape, generator=g).to(DEV) for t in (x0, ab0, w))
 
     def f(eps, grad=False):
-        _pin(4096 * 77)
+        pin_dropout_counter(DEV, 4096 * 77)
         b = _batch((x0 + eps * vx).requires_grad_(grad), ei, batch, fix["num_graphs"])
         b.attn_bias = (ab0 + eps * vb).requires_grad_(grad)
         xin, abin = b.x, b.attn_bias
@@ -257,7 +248,7 @@ def test_dropout_kept_fraction_scaling_and_fresh_masks():
     x = bb.x.to(DEV)
 
     def run(offset):
-        _pin(offset)
+        pin_dropout_counter(DEV, offset)
         b = _batch(x.clone(), bb.edge_index.to(DEV), bb.batch.to(DEV), len(sizes))
         return (layer(b).x - x).detach()
 
@@ -318,7 +309,7 @@ def test_captured_two_layer_stack(p):
     graph_of(b).nmax   # read before capture (the read synchronises)
     ct = torch.randn(bb.x.shape, device=DEV)
     x = bb.x.to(DEV).clone().requires_grad_(True)
-    _pin(4096 * 1000)
+    pin_dropout_counter(DEV, 4096 * 1000)
     eager_g, eager_out = _seq_step(seq, x, b, ct)
     eager_out = eager_out.detach()
     x = x.detach().clone().requires_grad_(True)   # the graph's static input, a fresh leaf
@@ -331,7 +322,7 @@ def test_captured_two_layer_stack(p):
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph, capture_error_mode="thread_local"):
         cap_g, cap_out = _seq_step(seq, x, b, ct)
-    _pin(4096 * 1000)   # the first replay's two layers draw the eager step's offsets
+    pin_dropout_counter(DEV, 4096 * 1000)   # the first replay's two layers draw the eager step's offsets
     graph.replay()
     torch.cuda.synchronize()
     first = cap_out.clone()

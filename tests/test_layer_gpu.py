@@ -13,7 +13,7 @@ from graphgps_b200 import _lib
 from graphgps_b200.batch import batch_from_lists, make_batch
 from graphgps_b200.graph import GraphStructure, graph_of
 from oracle.gps_oracle import OracleGPSLayer
-from util import compare, golden_batch, golden_names, load_golden, rel_err, rel_l2, run_layer
+from util import compare, golden_batch, golden_names, load_golden, pin_dropout_counter, rel_err, rel_l2, run_layer
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -314,7 +314,7 @@ def test_gcn_self_loops_duplicates_isolated_nodes_and_dropout_consistency():
     vx = torch.randn(bb.x.shape, generator=g).to(DEV)
 
     def f(x):
-        _set_dropout_counter(11 * 4096)
+        pin_dropout_counter(DEV, 11 * 4096)
         out = layer(graphgps_b200.GraphBatch(x=x, edge_index=bb.edge_index, edge_attr=bb.edge_attr, batch=bb.batch,
                                              num_graphs=bb.num_graphs))
         return (out.x * ct).sum()
@@ -386,16 +386,6 @@ def test_dropout_mask_keep_rate_and_determinism():
         assert not torch.equal(m1, m2)
 
 
-def _set_dropout_counter(value):
-    from graphgps_b200 import gps_layer
-    dev = torch.device(DEV)
-    ctr = gps_layer._drop_counters.get(dev)
-    if ctr is None:
-        ctr = torch.zeros(1, dtype=torch.int64, device=dev)
-        gps_layer._drop_counters[dev] = ctr
-    ctr.fill_(value)
-
-
 def test_dropout_forward_backward_consistent():
     """With the Philox offset pinned, the dropout layer is a deterministic smooth (GELU) function: its
     backward must equal a central finite difference of its forward along a random direction, i.e. the
@@ -412,7 +402,7 @@ def test_dropout_forward_backward_consistent():
     vx = torch.randn(b.x.shape, generator=g).to(DEV)
 
     def f(x):
-        _set_dropout_counter(7 * 4096)
+        pin_dropout_counter(DEV, 7 * 4096)
         bb = graphgps_b200.GraphBatch(x=x, edge_index=b.edge_index, edge_attr=b.edge_attr.clone(), batch=b.batch,
                                       num_graphs=b.num_graphs)
         out = layer(bb)
@@ -432,7 +422,7 @@ def test_dropout_forward_backward_consistent():
     assert abs(numeric - analytic) <= 3e-2 * max(1.0, abs(analytic)), (numeric, analytic)
     # different offsets => different masks; eval mode => no dropout
     with torch.no_grad():
-        _set_dropout_counter(9 * 4096)
+        pin_dropout_counter(DEV, 9 * 4096)
         other = layer(graphgps_b200.GraphBatch(x=b.x.clone(), edge_index=b.edge_index, edge_attr=b.edge_attr.clone(),
                                                batch=b.batch, num_graphs=b.num_graphs))
     assert not torch.equal(other.x, out0.x.detach())
@@ -492,7 +482,7 @@ def test_performer_attn_dropout_matches_oracle_with_injected_masks():
     b = make_batch("zinc-gatedgcn", seed=8, dim=d, num_graphs=9)
     N = b.num_nodes
     base = 21 * 4096
-    _set_dropout_counter(base)
+    pin_dropout_counter(DEV, base)
     seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
     masks = {}
     for site, p in ((7, pa), (4, pd), (1, pd), (2, pd), (5, pd), (6, pd)):
@@ -637,3 +627,24 @@ def test_eval_mode_backward_matches_oracle():
     tgt = {k: ref[k] for k in ("out_x", "out_e", "grad_x", "grad_e")}
     tgt["grad_params"], tgt["state_after"] = ref["grad_params"], ref["state_after"]
     compare(res, tgt, 1e-3, "eval-mode forward + backward", grad_l2_tol=5e-3)
+
+
+@pytest.mark.parametrize("family", ["GPSLayer", "GraphormerLayer", "SANLayer", "GatedGCNLayer"])
+def test_in_place_parameter_update_before_backward_is_refused(family):
+    """Every layer saves its parameters for backward, so an in-place update between a forward and its backward raises
+    autograd's version-counter error: a backward never reads weight planes packed from other values than its forward's."""
+    torch.manual_seed(0)
+    d = 16
+    layer = {"GPSLayer": lambda: graphgps_b200.GPSLayer(d, "GINE", "Transformer", 4),
+             "GraphormerLayer": lambda: graphgps_b200.GraphormerLayer(d, 4, 0.0, 0.0, 0.0),
+             "SANLayer": lambda: graphgps_b200.SANLayer(0.1, d, d, 4, True, torch.nn.Embedding(1, d)),
+             "GatedGCNLayer": lambda: graphgps_b200.GatedGCNLayer(d, d, 0.0, True)}[family]().to(DEV).train()
+    ei = torch.cat([torch.randint(0, 20, (2, 60)), torch.randint(20, 40, (2, 60))], 1)
+    b = graphgps_b200.GraphBatch(x=torch.randn(40, d, device=DEV), edge_index=ei.to(DEV),
+                                 edge_attr=torch.randn(120, d, device=DEV),
+                                 batch=torch.arange(40, device=DEV) // 20, num_graphs=2)
+    loss = layer(b).x.sum()
+    with torch.no_grad():
+        next(layer.parameters()).add_(1.0)
+    with pytest.raises(RuntimeError, match="modified by an inplace operation"):
+        loss.backward()

@@ -13,7 +13,7 @@ from graphgps_b200 import _lib
 from graphgps_b200.graph import graph_of
 from oracle.gps_oracle import OracleGPSLayer
 from nonorm_util import NODE_SHAPES, load_nonorm, node_graph, node_shape_batch, nonorm_names, with_edge_cases
-from util import compare, golden_batch, rel_err, rel_l2, run_layer
+from util import compare, golden_batch, pin_dropout_counter, rel_err, rel_l2, run_layer
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -102,16 +102,6 @@ def test_node_level_full_size_matches_oracle_fp64(shape, precision):
 
 
 # ------------------------------------------------------------------------------------------ dropout
-def _set_dropout_counter(value):
-    from graphgps_b200 import gps_layer
-    dev = torch.device(DEV)
-    ctr = gps_layer._drop_counters.get(dev)
-    if ctr is None:
-        ctr = torch.zeros(1, dtype=torch.int64, device=dev)
-        gps_layer._drop_counters[dev] = ctr
-    ctr.fill_(value)
-
-
 @pytest.mark.parametrize("local,glob", [("GCN", "Transformer"), ("GCN", "None"), ("GINE", "Transformer"),
                                         ("CustomGatedGCN", "Performer")])
 def test_dropout_forward_backward_consistent(local, glob):
@@ -131,7 +121,7 @@ def test_dropout_forward_backward_consistent(local, glob):
     vx = torch.randn(b.x.shape, generator=g).to(DEV)
 
     def f(x, counter=7 * 4096):
-        _set_dropout_counter(counter)
+        pin_dropout_counter(DEV, counter)
         out = layer(graphgps_b200.GraphBatch(x=x, edge_index=b.edge_index, edge_attr=b.edge_attr.clone(), batch=b.batch,
                                              num_graphs=1))
         loss = (out.x * ct_x).sum()

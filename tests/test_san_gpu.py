@@ -11,11 +11,11 @@ import torch
 import torch.nn as nn
 
 import graphgps_b200
-from graphgps_b200 import _lib, gps_layer
+from graphgps_b200 import _lib
 from graphgps_b200.batch import GraphBatch
 from graphgps_b200.graph import graph_of
 from san_oracle import dataset_sizes, fake_pairs, san_attention, san_batch, san_forward
-from util import GOLDEN_DIR, rel_err, rel_l2
+from util import GOLDEN_DIR, pin_dropout_counter, rel_err, rel_l2
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -210,15 +210,6 @@ def test_attention_stage_head_dims(hd, H, kind, gamma):
 
 
 # ------------------------------------------------------------------------------------------ dropout
-def _pin(value):
-    dev = torch.device(DEV)
-    ctr = gps_layer._drop_counters.get(dev)
-    if ctr is None:
-        ctr = torch.zeros(1, dtype=torch.int64, device=dev)
-        gps_layer._drop_counters[dev] = ctr
-    ctr.fill_(value)
-
-
 def _mask(rows, cols, p, offset, site):
     m = torch.empty(rows, cols, device=DEV)
     lib = _lib.load()
@@ -259,7 +250,7 @@ def test_dropout_both_sites_with_injected_masks():
     b = _gb(sb.x.clone().requires_grad_(True), sb.edge_attr.clone().requires_grad_(True), sb.edge_index, sb.batch, 8)
     ct = torch.randn(sb.x.shape, device=DEV)
     N = sb.x.shape[0]
-    _pin(4096 * 50)
+    pin_dropout_counter(DEV, 4096 * 50)
     off = 4096 * 51                      # the call's snapshot of the counter
     masks = (_mask(N, 56, p, off, 13), _mask(N, 112, p, off, 14))
     x_in, e_in = b.x, b.edge_attr
@@ -325,7 +316,7 @@ def test_captured_two_layer_stack(p):
     ct = torch.randn(sb.x.shape, device=DEV)
     x = sb.x.clone().requires_grad_(True)
     e = sb.edge_attr.clone().requires_grad_(True)
-    _pin(4096 * 1000)
+    pin_dropout_counter(DEV, 4096 * 1000)
     eager_g, eager_out = _seq_step(seq, x, e, b, ct)
     eager_out = eager_out.detach()
     x = x.detach().clone().requires_grad_(True)
@@ -339,7 +330,7 @@ def test_captured_two_layer_stack(p):
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph, capture_error_mode="thread_local"):
         cap_g, cap_out = _seq_step(seq, x, e, b, ct)
-    _pin(4096 * 1000)
+    pin_dropout_counter(DEV, 4096 * 1000)
     graph.replay()
     torch.cuda.synchronize()
     first = cap_out.clone()
@@ -386,7 +377,7 @@ def _full(kind, B, d, H, gamma, p, seed):
     N = sb.x.shape[0]
     masks = None
     if p > 0:
-        _pin(4096 * 300)
+        pin_dropout_counter(DEV, 4096 * 300)
         off = 4096 * 301
         masks = [(_mask(N, d, p, off, 13), _mask(N, 2 * d, p, off, 14))]
     x_in, e_in = b.x, b.edge_attr

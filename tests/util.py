@@ -47,6 +47,13 @@ def run_layer(layer, batch, fix, backward=True):
     return res
 
 
+def pin_dropout_counter(device, value):
+    """Sets the library's device-resident dropout counter, so the next layer call draws the masks of offset
+    value + 4096."""
+    from graphgps_b200 import _call
+    _call.dropout_counter(torch.device(device)).fill_(value)
+
+
 def rel_err(a, b):
     """max |a-b| / max(1, max|b|): absolute on O(1) (BatchNorm-normalised) data, relative on large."""
     a, b = a.double(), b.double()

@@ -22,7 +22,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import graphgps_b200  # noqa: E402
-from graphgps_b200 import _lib, gps_layer  # noqa: E402
+from graphgps_b200 import _call, _lib  # noqa: E402
 from graphgps_b200.batch import GraphBatch  # noqa: E402
 from graphgps_b200.graph import graph_of  # noqa: E402
 from san_oracle import dataset_sizes, san_batch, san_forward  # noqa: E402
@@ -147,7 +147,7 @@ def main():
     for cfg in CONFIGS:
         if args.only and cfg[0] not in args.only.split(","):
             continue
-        gps_layer._drop_counters.clear()
+        _call._drop_counters.clear()
         lib_fn, torch_fn, launches, N = setup(cfg)
         for _ in range(args.warmup):
             lib_fn()
