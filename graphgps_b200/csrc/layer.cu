@@ -1246,6 +1246,9 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     }
     GPS_TRY(gemm(g2, st));
   }
+  // the attention-branch backward needs g_s (and hA) only: it forks here and runs next to norm1_local's backward and
+  // the local-model backward (with GPS_B200_OPT bit 64 both BatchNorm reductions are already in g_s's epilogue)
+  if (two_branches) GPS_TRY(sd->order(st, sa));
 
   bool chain_x = false;
   // ---- norm1_local / norm1_attn (gps_layer.py:194,217): g_xloc, g_hA
@@ -1261,11 +1264,11 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
       GPS_TRY(bn_bwd_apply(P.g_s, d, P.xloc, d, N, d, v, -1, nodrop, sums(BN_L), P.g_xloc, d,
                            a->norm1_local.grad_weight, a->norm1_local.grad_bias, st, P.grads_accumulate, P.gl1_p));
   }
-  if (!P.attn && !P.perf && !P.bb) {   // no global model: the early group ends with norm1_local's gradients (stream st)
-    GPS_TRY(wfork(st));
-    GPS_TRY(early_done());
-  }
-  if (two_branches) GPS_TRY(sd->order(st, sa));   // attention-branch backward runs next to the local-model backward
+  // norm1_local's gradients belong to the early group: the weight-gradient stream takes them in before the attention
+  // branch (forked before them) records the group's event there; with no global model the group ends here
+  const bool glob_model = P.attn || P.perf || P.bb;
+  if (!glob_model || (P.loc && !P.nonorm)) GPS_TRY(wfork(st));
+  if (!glob_model) GPS_TRY(early_done());
   if (P.attn) {
     if (!P.nonorm) {
       BnView v = bn_view(P, BN_A, a->norm1_attn);
@@ -1397,10 +1400,11 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     // message/aggregate backward (SURVEY Appendix C)
     GPS_TRY(gatedgcn_bwd_dst(a->graph, d, P.gY1, P.Wy, P.ehat, P.Y1 + d, P.Wy, P.g_e, P.g_num, P.gY1 + 2 * d, st, P.ge_p,
                              P.gY1_p.cols(2 * d), P.pe_rho, P.g_den));
-    // EquivStableLapPE gate: mlp_r_ij gradients (mid group) and grad_pe need g_num / g_den only, so they run on the
-    // (by now idle) edge-BatchNorm stream next to the src-ordered pass and the weight gradients
+    // g_e, g_num and g_den are final here.  The EquivStableLapPE gate's mlp_r_ij gradients (mid group) and grad_pe need
+    // g_num / g_den only, so they run on the (by now idle) edge-BatchNorm stream next to the src-ordered pass and the
+    // weight gradients
+    GPS_TRY(sd->order(st, se));
     if (P.eslap) {
-      GPS_TRY(sd->order(st, se));
       GPS_TRY(eslap_bwd(a->graph, a->pe, a->pe_dim, d, act, P.g_num, P.g_den, P.Y1 + d, P.Wy, P.ehat, P.pe_r, P.pe_rho,
                         a->pe_mlp0.weight, a->pe_mlp0.bias, a->pe_mlp1.weight, P.pe_gz, P.pe_gr, P.pe_part, a->grad_pe,
                         a->pe_mlp0.grad_weight, a->pe_mlp0.grad_bias, a->pe_mlp1.grad_weight, a->pe_mlp1.grad_bias,
@@ -1414,10 +1418,12 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     GPS_TRY(linear_wgrad(P, g_e, {a->edge_attr, d, P.e_p}, E, d, d, a->gcn_C.grad_weight, a->gcn_C.grad_bias, s2));
     if (P.eslap) GPS_TRY(sd->order(se, s2));   // the mlp_r_ij gradients are final at ev_grads_mid; grad_pe joins at the end
     GPS_TRY(mid_done());
+    // an output only: on the edge stream (after the gate's backward there), off the local branch and the weight-gradient
+    // chain; joined at the end
     if (a->grad_edge_attr && E > 0) {
       GemmParams g = linear_dgrad(P, E, d, d, g_e, {a->gcn_C.weight, d, P.C_p}, a->grad_edge_attr, d);
       g.R1 = a->grad_edge_out; g.ldr1 = (int)d;
-      GPS_TRY(gemm(g, st));
+      GPS_TRY(gemm(g, se));
     }
     g_x_local = g_xloc;  // residual x_in + ...
   } else if (P.gine) {
@@ -1542,6 +1548,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     GPS_TRY(add3(P.g_xp, d, nullptr, 0, nullptr, 0, a->grad_x, d, N, d, st));   // Performer only
   }
   GPS_TRY(sd->join(st));
+  if (P.gated) GPS_TRY(sd->order(se, st));   // grad_edge_attr and the gate's grad_pe
   GPS_TRY(record_ev(a->ev_grads_done, st));
   return GPS_OK;
 }
