@@ -138,51 +138,14 @@ struct AttnArgs {
   float scale; float p_drop; uint64_t seed, offset;
   const unsigned long long* offset_dev;
   Planes Op, dQp, dKp, dVp;   // optional bf16 hi/lo plane copies of O (forward) / dQ, dK, dV (backward)
-  int smem_rows;              // rows of the two per-block staging tiles (0: no staging)
   const float* bias; int64_t nmax; float* gbias;   // BIAS kernels only: [B*H, nmax, nmax], grad_bias (may be NULL)
 };
 __device__ __forceinline__ uint64_t eff_offset(const AttnArgs& a) {
   return a.offset + ((a.p_drop > 0.f && a.offset_dev) ? *a.offset_dev : 0ull);
 }
 
-// Shared-memory staging for batches of small graphs.  The 32 rows of a block belong to a few consecutive graphs, so
-// every row it walks (keys for the forward / query-major pass, queries for the key-major pass) lies in the contiguous
-// node range [start of the first row's graph, end of the last row's graph).  When that range fits (smem_rows), the
-// block copies head h of the two tensors it walks into shared memory once (coalesced 128-bit loads) and the
-// per-key loop reads shared memory instead of chasing L2 latency on every iteration (measured at the PCQM4M shape:
-// the loop was ~600 cycles per key).  Larger ranges (ogbg-code2) keep the global-memory path.
-struct StagedRows {
-  const float* x; int64_t ldx;   // row r of tensor X at x + r * ldx (head offset included)
-  const float* y; int64_t ldy;
-};
-template <int RPB, int VW>
-__device__ __forceinline__ StagedRows stage_rows(const AttnArgs& a, const float* X, int64_t ldX, const float* Y, int64_t ldY,
-                                                 int h, float* sm) {
-  const int64_t hoff = (int64_t)h * a.hd;
-  StagedRows r{X + hoff, ldX, Y + hoff, ldY};
-  const int r0 = blockIdx.x * RPB;
-  if (a.smem_rows <= 0 || r0 >= a.N) return r;
-  const int last = min(r0 + RPB, a.N) - 1;
-  const int kmin = a.gptr[find_graph(a.gptr, a.B, r0)];
-  const int R = a.gptr[find_graph(a.gptr, a.B, last) + 1] - kmin;
-  if (R > a.smem_rows) return r;                      // block-uniform
-  const int pitch = a.hd + 4, nch = VW == 4 ? a.hd >> 2 : a.hd;
-  float* sx = sm;
-  float* sy = sm + (int64_t)a.smem_rows * pitch;
-  for (int idx = threadIdx.x; idx < R * nch; idx += blockDim.x) {
-    const int row = idx / nch, c = idx - row * nch;
-    vst(sx + row * pitch + c * VW, vld<VW>(X + (int64_t)(kmin + row) * ldX + hoff + c * VW));
-    vst(sy + row * pitch + c * VW, vld<VW>(Y + (int64_t)(kmin + row) * ldY + hoff + c * VW));
-  }
-  __syncthreads();
-  r.x = sx - (int64_t)kmin * pitch; r.ldx = pitch;
-  r.y = sy - (int64_t)kmin * pitch; r.ldy = pitch;
-  return r;
-}
-
 template <int CH, int LPR, bool BIAS, int VW>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
-  extern __shared__ float attn_sm[];
   using V = typename VecT<VW>::T;
   constexpr int RPW = 32 / LPR;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -215,10 +178,9 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
   drop_quad_init(dq, a.p_drop);
   // software pipeline: the K/V rows of key jl+1 are in flight while key jl is processed (the loop is a chain of
   // load -> dot -> shuffle -> exp -> fma, i.e. latency bound at these tiny graph sizes)
-  const StagedRows kv = stage_rows<RPW * kWarpsPerBlock, VW>(a, a.K, a.ld, a.V, a.ld, h, attn_sm);
   V kc[CH], vc[CH];
-  load_slice<CH, LPR, VW>(kc, kv.x + (int64_t)gs * kv.ldx, sub, nch, n > 0);
-  load_slice<CH, LPR, VW>(vc, kv.y + (int64_t)gs * kv.ldy, sub, nch, n > 0);
+  load_slice<CH, LPR, VW>(kc, a.K + (int64_t)gs * a.ld + hoff, sub, nch, n > 0);
+  load_slice<CH, LPR, VW>(vc, a.V + (int64_t)gs * a.ld + hoff, sub, nch, n > 0);
   float bc = 0.f;
   if constexpr (BIAS) bc = n > 0 ? brow[0] : 0.f;
   for (int jl = 0; jl < nloop; ++jl) {
@@ -227,8 +189,8 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_fwd(AttnArgs a) {
     const bool nvalid = jl + 1 < n;
     const int jn = gs + (nvalid ? jl + 1 : 0);
     V kn[CH], vn[CH];
-    load_slice<CH, LPR, VW>(kn, kv.x + (int64_t)jn * kv.ldx, sub, nch, nvalid);
-    load_slice<CH, LPR, VW>(vn, kv.y + (int64_t)jn * kv.ldy, sub, nch, nvalid);
+    load_slice<CH, LPR, VW>(kn, a.K + (int64_t)jn * a.ld + hoff, sub, nch, nvalid);
+    load_slice<CH, LPR, VW>(vn, a.V + (int64_t)jn * a.ld + hoff, sub, nch, nvalid);
     float bn = 0.f;
     if constexpr (BIAS) bn = nvalid ? brow[jl + 1] : 0.f;
     float s = group_sum<LPR>(dot_slice<CH>(q, kc));
@@ -290,7 +252,7 @@ __global__ void k_attn_delta(AttnArgs a) {
 
 // query-major backward: dQ_i (delta precomputed by k_attn_delta); BIAS: grad_bias[g, h, i - gs, jl] = ds
 template <int CH, int LPR, bool BIAS, int VW>
-__device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_sm) {
+__device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a) {
   using V = typename VecT<VW>::T;
   constexpr int RPW = 32 / LPR;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -324,10 +286,9 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
     const bool use_drop = a.p_drop > 0.f;
     DropQuad dq;
     drop_quad_init(dq, a.p_drop);
-    const StagedRows kv = stage_rows<RPW * kWarpsPerBlock, VW>(a, a.K, a.ld, a.V, a.ld, h, attn_sm);
     V kk[CH], vv[CH];
-    load_slice<CH, LPR, VW>(kk, kv.x + (int64_t)gs * kv.ldx, sub, nch, n > 0);
-    load_slice<CH, LPR, VW>(vv, kv.y + (int64_t)gs * kv.ldy, sub, nch, n > 0);
+    load_slice<CH, LPR, VW>(kk, a.K + (int64_t)gs * a.ld + hoff, sub, nch, n > 0);
+    load_slice<CH, LPR, VW>(vv, a.V + (int64_t)gs * a.ld + hoff, sub, nch, n > 0);
     float bc = 0.f;
     if constexpr (BIAS) bc = n > 0 ? a.bias[brow] : 0.f;
     for (int jl = 0; jl < nloop; ++jl) {
@@ -336,8 +297,8 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
       const bool nvalid = jl + 1 < n;
       const int jn = gs + (nvalid ? jl + 1 : 0);
       V kn[CH], vn[CH];
-      load_slice<CH, LPR, VW>(kn, kv.x + (int64_t)jn * kv.ldx, sub, nch, nvalid);
-      load_slice<CH, LPR, VW>(vn, kv.y + (int64_t)jn * kv.ldy, sub, nch, nvalid);
+      load_slice<CH, LPR, VW>(kn, a.K + (int64_t)jn * a.ld + hoff, sub, nch, nvalid);
+      load_slice<CH, LPR, VW>(vn, a.V + (int64_t)jn * a.ld + hoff, sub, nch, nvalid);
       float bn = 0.f;
       if constexpr (BIAS) bn = nvalid ? a.bias[brow + jl + 1] : 0.f;
       float s = dot_slice<CH>(q, kk), dp = dot_slice<CH>(go, vv);
@@ -378,7 +339,7 @@ __device__ __forceinline__ void attn_bwd_q_body(const AttnArgs& a, float* attn_s
 
 // key-major backward: dK_j, dV_j (BIAS: p recomputed with the bias column of key j)
 template <int CH, int LPR, bool BIAS, int VW>
-__device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_sm) {
+__device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a) {
   using V = typename VecT<VW>::T;
   constexpr int RPW = 32 / LPR;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -408,18 +369,17 @@ __device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_
     gk[c] = vzero<VW>();
     gv[c] = vzero<VW>();
   }
-  const StagedRows qd = stage_rows<RPW * kWarpsPerBlock, VW>(a, a.Q, a.ld, a.dO, a.ldo, h, attn_sm);
   V q[CH], go[CH];
-  load_slice<CH, LPR, VW>(q, qd.x + (int64_t)gs * qd.ldx, sub, nch, n > 0);
-  load_slice<CH, LPR, VW>(go, qd.y + (int64_t)gs * qd.ldy, sub, nch, n > 0);
+  load_slice<CH, LPR, VW>(q, a.Q + (int64_t)gs * a.ld + hoff, sub, nch, n > 0);
+  load_slice<CH, LPR, VW>(go, a.dO + (int64_t)gs * a.ldo + hoff, sub, nch, n > 0);
   for (int il = 0; il < nloop; ++il) {
     const bool valid = il < n;
     const int i = gs + (valid ? il : 0);
     const bool nvalid = il + 1 < n;
     const int in_ = gs + (nvalid ? il + 1 : 0);
     V qn[CH], gon[CH];
-    load_slice<CH, LPR, VW>(qn, qd.x + (int64_t)in_ * qd.ldx, sub, nch, nvalid);
-    load_slice<CH, LPR, VW>(gon, qd.y + (int64_t)in_ * qd.ldy, sub, nch, nvalid);
+    load_slice<CH, LPR, VW>(qn, a.Q + (int64_t)in_ * a.ld + hoff, sub, nch, nvalid);
+    load_slice<CH, LPR, VW>(gon, a.dO + (int64_t)in_ * a.ldo + hoff, sub, nch, nvalid);
     float s = dot_slice<CH>(q, kk), dp = dot_slice<CH>(go, vv);
 #pragma unroll
     for (int ofs = LPR / 2; ofs > 0; ofs >>= 1) {
@@ -464,14 +424,11 @@ __device__ __forceinline__ void attn_bwd_kv_body(const AttnArgs& a, float* attn_
 // both backward passes in one grid (blockIdx.z picks the pass) so they share the SMs instead of queueing
 template <int CH, int LPR, bool BIAS, int VW>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_attn_bwd(AttnArgs a) {
-  extern __shared__ float attn_sm[];
-  if (blockIdx.z == 0) attn_bwd_kv_body<CH, LPR, BIAS, VW>(a, attn_sm);
-  else attn_bwd_q_body<CH, LPR, BIAS, VW>(a, attn_sm);
+  if (blockIdx.z == 0) attn_bwd_kv_body<CH, LPR, BIAS, VW>(a);
+  else attn_bwd_q_body<CH, LPR, BIAS, VW>(a);
 }
 
 enum { KFWD = 0, KBWD = 1 };
-
-constexpr int kStageBytes = 72 * 1024;   // two staging tiles per block; 3 blocks per SM still fit
 
 // whether the float4 kernels take these head dim and leading dimensions (else the VW = 1 kernels run)
 static bool attn_vec4(const AttnArgs& a, int which) {
@@ -479,31 +436,12 @@ static bool attn_vec4(const AttnArgs& a, int which) {
 }
 
 template <int CH, int LPR, bool BIAS, int VW>
-static void launch_one(int which, const AttnArgs& a0, cudaStream_t stream) {
+static void launch_one(int which, const AttnArgs& a, cudaStream_t stream) {
   constexpr int RPW = 32 / LPR;
-  AttnArgs a = a0;
-  static const bool stage_on = [] {
-    const char* e = getenv("GPS_B200_ATTN_STAGE");   // off by default: the staged kernels are faster in isolation but
-    return e && e[0] == '1';                          // their 72 KB blocks crowd the GEMMs running next to them
-                                                      // (pcqm4m-small fp32, H100 80GB HBM3 at 400 W: 0.854 on vs
-                                                      // 0.846 ms/step off)
-  }();
-  // staging pays when graphs are small (a block's 32 rows then see few distinct key rows); with large graphs every
-  // block would exceed the tile anyway
-  const int pitch = a.hd + 4;
-  a.smem_rows = (stage_on && a.B > 0 && a.N < 64LL * a.B) ? kStageBytes / (2 * pitch * 4) : 0;
-  const size_t smem = a.smem_rows > 0 ? (size_t)2 * a.smem_rows * pitch * 4 : 0;
-  static bool attr_done[2] = {false, false};
-  if (smem > 0 && !attr_done[which]) {
-    if (which == KFWD)
-      cudaFuncSetAttribute(k_attn_fwd<CH, LPR, BIAS, VW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
-    else cudaFuncSetAttribute(k_attn_bwd<CH, LPR, BIAS, VW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kStageBytes);
-    attr_done[which] = true;
-  }
   dim3 grid((unsigned)ceil_div(a.N, (int64_t)RPW * kWarpsPerBlock), (unsigned)a.H, which == KFWD ? 1 : 2);
   dim3 block(kWarpsPerBlock * 32);
-  if (which == KFWD) k_attn_fwd<CH, LPR, BIAS, VW><<<grid, block, smem, stream>>>(a);
-  else k_attn_bwd<CH, LPR, BIAS, VW><<<grid, block, smem, stream>>>(a);
+  if (which == KFWD) k_attn_fwd<CH, LPR, BIAS, VW><<<grid, block, 0, stream>>>(a);
+  else k_attn_bwd<CH, LPR, BIAS, VW><<<grid, block, 0, stream>>>(a);
 }
 
 static int dispatch(int which, const AttnArgs& a, cudaStream_t stream) {

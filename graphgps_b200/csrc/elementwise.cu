@@ -274,40 +274,6 @@ struct OpBnBwdApply {
   }
 };
 
-// BatchNorm backward apply of one norm fused with the backward REDUCE of the next one down the chain:
-//   v = dL/dz of BN_1 (as OpBnBwdApply), written out;  g2' = v * act'(BN_2(z2)) * drop2;
-//   sums2[0] += sum_r g2', sums2[1] += sum_r g2' * zhat2       (what bn_bwd_reduce(v, z2, BN_2) would compute)
-// Used for norm1_local -> local_model.bn_node_x (gps_layer.py:194 after gatedgcn_layer.py:72-83): one launch less on the
-// critical path of the backward pass.
-struct OpBnBwdApplyChain {
-  static constexpr int NS = 2;
-  OpBnBwdApply a;
-  const float* z2; int64_t ldz2; BnView bn2; int act2; DropCfg drop2; double* sums2;
-  BnRegs reg2;
-  __device__ void prepare(int c4) {
-    a.prepare(c4);
-    reg2.load(bn2, c4);
-    if (drop2.p > 0.f && drop2.offset_dev) drop2.offset += *drop2.offset_dev;
-  }
-  __device__ void row(int64_t r, int c4, float4* acc) {
-    float4 zh = a.reg.zhat(ld4(a.z + r * a.ldz + c4 * 4));
-    float4 gp = bn_bwd_gprime(a.g, a.ldg, r, c4, zh, a.reg, a.act, a.drop, a.d);
-    float4 v = make_float4(a.gs.x * (gp.x - a.m1.x - zh.x * a.m2.x), a.gs.y * (gp.y - a.m1.y - zh.y * a.m2.y),
-                           a.gs.z * (gp.z - a.m1.z - zh.z * a.m2.z), a.gs.w * (gp.w - a.m1.w - zh.w * a.m2.w));
-    st4(a.out + r * a.ldo + c4 * 4, v);
-    if (a.outp.hi) planes_store4(a.outp, r, c4 * 4, v);
-    float4 zh2 = reg2.zhat(ld4(z2 + r * ldz2 + c4 * 4));
-    float4 g2 = v;
-    if (drop2.p > 0.f)
-      g2 = f4mul(g2, dropout_scale4(drop2.p, drop2.seed, drop2.offset, drop2.site, (uint64_t)r * (a.d >> 2) + c4));
-    if (act2 >= 0) g2 = f4mul(g2, dact4(act2, f4fma(zh2, reg2.gamma, reg2.beta)));
-    acc[0] = f4add(acc[0], g2);
-    acc[1] = f4fma(g2, zh2, acc[1]);
-  }
-  __device__ double* stat_ptr(int s) { return sums2 + (int64_t)s * a.d; }
-  __device__ void finish(int c4, int ry) { a.finish(c4, ry); }
-};
-
 struct OpAdd3 {
   static constexpr int NS = 0;
   const float* a; int64_t lda; const float* b; int64_t ldb; const float* c; int64_t ldc;
@@ -397,17 +363,6 @@ int bn_act_residual2(const float* zx, const float* Rx, float* outx, int64_t N, B
   k_rowwise2<<<dim3((unsigned)(g.grid.x + gb)), g.block, g.smem, stream>>>(opx, N, (int)g.grid.x, ope, E);
   GPS_LAUNCH_CHECK();
   return GPS_OK;
-}
-
-int bn_bwd_apply_chain(const float* g, int64_t ldg, const float* z, int64_t ldz, int64_t rows, int64_t d, BnView bn,
-                       const double* sums, float* out, int64_t ldo, float* grad_gamma, float* grad_beta, bool accumulate,
-                       Planes outp, const float* z2, int64_t ldz2, BnView bn2, int act2, DropCfg drop2, double* sums2,
-                       cudaStream_t stream) {
-  GPS_REQUIRE(rows > 0, GPS_ERR_ARG, "bn_bwd_apply_chain: no rows");
-  OpBnBwdApply a{g, ldg, z, ldz, d, bn, -1, DropCfg(), sums, 1.f / (float)rows, out, ldo, grad_gamma, grad_beta,
-                 accumulate ? 1 : 0, outp};
-  OpBnBwdApplyChain op{a, z2, ldz2, bn2, act2, drop2, sums2};
-  return launch_rowwise(op, rows, d, stream);
 }
 
 int bn_combine(const float* a, BnView bna, const float* b, BnView bnb, float* out, int64_t rows, int64_t d,

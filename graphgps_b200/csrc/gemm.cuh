@@ -39,12 +39,7 @@ struct GemmParams {
   Planes Ap, Bp, Cp;
   // Cp column remap for the attention operands: output column c lands at (c / cp_hd) * cp_hd_pad + c % cp_hd and the
   // cp_hd_pad - cp_hd pad columns of every head are written as zeros (per-head layout padded to a multiple of 16)
-  int cp_hd = 0, cp_hd_pad = 0, cp_col0 = 0;
-  // Backward-reduce of up to two BatchNorms that consume this GEMM's output C as their upstream gradient (TMA kernel
-  // only): with zhat_k = (z_k - mean_k) * invstd_k, sums_k[0][n] += sum_m C[m,n], sums_k[1][n] += sum_m C[m,n] * zhat_k[m,n]
-  // (what bn_bwd_reduce(C, z_k, ...) computes; norm1_local / norm1_attn both read g_s, gps_layer.py:194,217,222)
-  struct BnRed { const float* z = nullptr; int ldz = 0; const float* mean = nullptr; const float* invstd = nullptr; double* sums = nullptr; };
-  BnRed bnred[2];   // cp_col0: first output column of the remapped block
+  int cp_hd = 0, cp_hd_pad = 0, cp_col0 = 0;   // cp_col0: first output column of the remapped block
 };
 
 struct ToPlanesItem { const float* src; int64_t ld; int rows; int cols; Planes dst; };

@@ -50,7 +50,6 @@ constexpr int kMaxSplits = 8;           // split-K splits of a tile = cluster si
 struct TmaArgs {
   GemmParams p;
   int BN, nb_blocks, stages, kb_per_split, planes;
-  int debug;                   // bring-up: 1 no global stores in the epilogue
   unsigned long long* trace;   // bring-up: 16 globaltimer stamps per CTA (first 256 CTAs), see tools/gemm_trace.py
 };
 
@@ -275,7 +274,7 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     const int col = n0 + cg * 4;
     const bool col_ok = rip < rpp && col < p.N;
     const int rows_here = min(BM, p.M - m0);
-    const bool colstats = p.stats || p.bnred[0].sums || p.bnred[1].sums;
+    const bool colstats = p.stats != nullptr;
     if (col_ok) {
       // rows of this thread: r = rip + k * rpp, k < nrows.  Everything is addressed through per-thread base pointers
       // advanced by a constant stride, and the loop is unrolled by 4 rows so that the shared/global loads of a group are
@@ -348,7 +347,8 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
               if (k + u >= nrows) continue;
-              if (cp && !(a.debug & 1)) st4(cp + (k + u) * c_st, w[u]);
+              if (colstats) *reinterpret_cast<float4*>(sp + (k + u) * s_st) = w[u];
+              if (cp) st4(cp + (k + u) * c_st, w[u]);
               if (ph) {
                 __nv_bfloat162 h0 = __floats2bfloat162_rn(w[u].x, w[u].y), h1 = __floats2bfloat162_rn(w[u].z, w[u].w);
                 *reinterpret_cast<uint2*>(ph + (k + u) * p_st) =
@@ -364,7 +364,6 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
                   if (pl) *reinterpret_cast<uint2*>(pl + (k + u) * p_st + 4 + z) = make_uint2(0u, 0u);
                 }
               }
-              if (colstats) *reinterpret_cast<float4*>(sp + (k + u) * s_st) = w[u];
             }
           }
         } else {
@@ -400,56 +399,37 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     }
     if (colstats) {
       // BatchNorm column sums over this tile's rows, in the same order for every tile width: task (y, g) sums rows
-      // y, y + 16, ... of column group g (sum w, sum w^2, sum w*zhat_0, sum w*zhat_1, zhat_k = (z_k - mean_k) invstd_k)
-      // and leaves the four partials in rows y, y + 16, y + 32, y + 48 of its own row class; then one thread per
-      // column group adds the 16 classes in order: one double atomic per column per CTA and accumulator.
+      // y, y + 16, ... of column group g (sum w, sum w^2) and leaves the two partials in rows y, y + 16 of its own row
+      // class; then one thread per column group adds the 16 classes in order: one double atomic per column per CTA and
+      // statistic.
       asm volatile("bar.sync 1, 256;" ::: "memory");
       for (int t = tid; t < 16 * G; t += kEpiWarps * 32) {
         const int y = t / G, g = t - y * G, c = n0 + g * 4;
         if (c >= p.N) continue;
-        const GemmParams::BnRed& b0 = p.bnred[0];
-        const GemmParams::BnRed& b1 = p.bnred[1];
-        float4 bm0 = f4zero(), bi0 = f4zero(), bm1 = f4zero(), bi1 = f4zero();
-        if (b0.sums) { bm0 = f4scale(ld4(b0.mean + c), -1.f); bi0 = ld4(b0.invstd + c); }
-        if (b1.sums) { bm1 = f4scale(ld4(b1.mean + c), -1.f); bi1 = ld4(b1.invstd + c); }
-        float4 s1 = f4zero(), s2 = f4zero(), q0 = f4zero(), q1 = f4zero();
+        float4 s1 = f4zero(), s2 = f4zero();
         for (int r = y; r < rows_here; r += 16) {
           const float4 w = *reinterpret_cast<const float4*>(stage + r * sld + g * 4);
-          const int64_t row = m0 + r;
           s1 = f4add(s1, w);
           s2 = f4fma(w, w, s2);
-          if (b0.sums) q0 = f4fma(w, f4mul(f4add(ld4(b0.z + row * b0.ldz + c), bm0), bi0), q0);
-          if (b1.sums) q1 = f4fma(w, f4mul(f4add(ld4(b1.z + row * b1.ldz + c), bm1), bi1), q1);
         }
         float* o = stage + y * sld + g * 4;
         *reinterpret_cast<float4*>(o) = s1;
         *reinterpret_cast<float4*>(o + 16 * sld) = s2;
-        *reinterpret_cast<float4*>(o + 32 * sld) = q0;
-        *reinterpret_cast<float4*>(o + 48 * sld) = q1;
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
       if (tid < G && n0 + tid * 4 < p.N) {
-        float4 t[4] = {f4zero(), f4zero(), f4zero(), f4zero()};
-        for (int y = 0; y < 16; ++y)
-#pragma unroll
-          for (int k = 0; k < 4; ++k) t[k] = f4add(t[k], *reinterpret_cast<const float4*>(stage + (y + 16 * k) * sld + tid * 4));
+        float4 t[2] = {f4zero(), f4zero()};
+        for (int y = 0; y < 16; ++y) {
+          t[0] = f4add(t[0], *reinterpret_cast<const float4*>(stage + y * sld + tid * 4));
+          t[1] = f4add(t[1], *reinterpret_cast<const float4*>(stage + (y + 16) * sld + tid * 4));
+        }
         const int c0 = n0 + tid * 4;
         auto add4 = [&](double* dst, float4 v) {
           atomic_add_f64(dst + 0, (double)v.x); atomic_add_f64(dst + 1, (double)v.y);
           atomic_add_f64(dst + 2, (double)v.z); atomic_add_f64(dst + 3, (double)v.w);
         };
-        if (p.stats) {
-          add4(p.stats + c0, t[0]);
-          add4(p.stats + (int64_t)p.N + c0, t[1]);
-        }
-        if (p.bnred[0].sums) {
-          add4(p.bnred[0].sums + c0, t[0]);
-          add4(p.bnred[0].sums + (int64_t)p.N + c0, t[2]);
-        }
-        if (p.bnred[1].sums) {
-          add4(p.bnred[1].sums + c0, t[0]);
-          add4(p.bnred[1].sums + (int64_t)p.N + c0, t[3]);
-        }
+        add4(p.stats + c0, t[0]);
+        add4(p.stats + (int64_t)p.N + c0, t[1]);
       }
     }
   }
@@ -578,11 +558,10 @@ int launch(const CUtensorMap& tA, const CUtensorMap& tB, const TmaArgs& a, dim3 
 
 int g_tma_force_bn = 0;
 unsigned long long* g_tma_trace = nullptr;
-int g_tma_debug = 0;
 
 }  // namespace
 
-void gemm_tma_set_force_bn(int bn) { g_tma_force_bn = bn & 0xFFFF; g_tma_debug = bn >> 16; }
+void gemm_tma_set_force_bn(int bn) { g_tma_force_bn = bn; }
 void gemm_tma_set_trace(unsigned long long* buf) { g_tma_trace = buf; }
 
 int gemm_tma(const GemmParams& p, cudaStream_t stream) {
@@ -608,12 +587,6 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream) {
   }
   if (p.colsum_a && !p.ta) {
     set_error("gemm: colsum_a needs ta == 1");
-    return GPS_ERR_ARG;
-  }
-  if ((p.bnred[0].sums || p.bnred[1].sums) &&
-      (p.splitk > 1 || p.C_pre || (p.mask_src && !p.mask_is_post) || p.p_drop != 0.f || p.p_drop2 != 0.f ||
-       (p.act >= 0 && p.act != GPS_ACT_RELU))) {
-    set_error("gemm: fused BatchNorm-backward reductions need the plain epilogue (no split-K / dropout / GELU)");
     return GPS_ERR_ARG;
   }
   const int mt = (int)ceil_div(p.M, BM);
@@ -666,7 +639,6 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream) {
   splitk = (int)ceil_div(nkb, a.kb_per_split);
   a.p.splitk = p.splitk > 1 ? 2 : 1;   // "accumulate atomically" flag
   a.trace = g_tma_trace;
-  a.debug = g_tma_debug;
   const bool amn = p.ta != 0, bmn = p.tb != 0;
   // planes are addressed as stored: Aop[m,k] = A[m, k] (ta = 0: rows = M, cols = K) or A[k, m] (ta = 1: rows = K, cols = M)
   CUtensorMap tA, tB;

@@ -53,13 +53,6 @@ int bn_bwd_reduce(const float* g, int64_t ldg, const float* z, int64_t ldz, int6
 int bn_bwd_apply(const float* g, int64_t ldg, const float* z, int64_t ldz, int64_t rows, int64_t d, BnView bn,
                  int act, DropCfg drop, const double* sums, float* out, int64_t ldo, float* grad_gamma,
                  float* grad_beta, cudaStream_t stream, bool accumulate = false, Planes outp = Planes());
-// bn_bwd_apply of one BatchNorm (no activation / dropout in front of it) fused with the bn_bwd_reduce of the NEXT
-// BatchNorm down the backward chain, which consumes this one's output: sums2 gets what
-// bn_bwd_reduce(out, z2, bn2, act2, drop2) would have produced.
-int bn_bwd_apply_chain(const float* g, int64_t ldg, const float* z, int64_t ldz, int64_t rows, int64_t d, BnView bn,
-                       const double* sums, float* out, int64_t ldo, float* grad_gamma, float* grad_beta, bool accumulate,
-                       Planes outp, const float* z2, int64_t ldz2, BnView bn2, int act2, DropCfg drop2, double* sums2,
-                       cudaStream_t stream);
 // out = a + b (+ c)   row-wise with independent leading dimensions
 int add3(const float* a, int64_t lda, const float* b, int64_t ldb, const float* c, int64_t ldc, float* out,
          int64_t ldo, int64_t rows, int64_t d, cudaStream_t stream);

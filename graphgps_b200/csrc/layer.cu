@@ -75,8 +75,6 @@ int gemm(const GemmParams& p, cudaStream_t stream) {
     if (rc != GPS_ERR_UNSUPPORTED) return rc;
   }
   GPS_REQUIRE(p.A && p.B && p.C, GPS_ERR_UNSUPPORTED, "gemm: plane operands rejected and no fp32 operands to fall back to");
-  GPS_REQUIRE(!p.bnred[0].sums && !p.bnred[1].sums, GPS_ERR_UNSUPPORTED,
-              "gemm: fused BatchNorm-backward reductions exist in the TMA kernel only");
   GemmParams q = p;
   if (q.Cp.hi) {   // the fp32 kernels do not write planes: convert afterwards
     q.Cp = Planes();
@@ -97,17 +95,6 @@ int gemm(const GemmParams& p, cudaStream_t stream) {
 }
 
 namespace {
-
-// Backward-pass fusions, off by default (GPS_B200_OPT bit mask): 32 reduces local_model.bn_node_x inside the
-// norm1_local apply pass, 64 reduces norm1_local / norm1_attn in the epilogue of the GEMM producing g_s.  Each saves a
-// launch, but the fused kernels run as few fat CTAs and delay the branches behind them.
-static int opt_flags() {
-  static const int v = [] {
-    const char* e = getenv("GPS_B200_OPT");
-    return e ? atoi(e) : 0;
-  }();
-  return v;
-}
 
 // ------------------------------------------------------------------------------- weight packing
 // A weight [rows, d] whose rows lie ld floats apart in the caller's tensor (ld > d: a column block of a wider weight,
@@ -1152,7 +1139,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   const bool two_branches = P.loc && P.glob;
   cudaStream_t sa = two_branches ? sd->s3 : st;   // stream of the attention-branch backward
   cudaStream_t se = sd->s4;                       // stream of the edge BatchNorm backward (GatedGCN)
-  const int opt = opt_flags();
   // data-parallel hook: the caller's event is recorded on the weight-gradient stream once the early gradient group
   // (FFN, attention output projection, norm2 / norm1_local / norm1_attn) has been enqueued there
   // (recorded as EXTERNAL events under stream capture, so that collectives enqueued outside the captured graph can wait
@@ -1210,7 +1196,6 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   const float* g_hA = P.nonorm ? P.g_s : P.g_hA;
   const Planes g_hA_p = P.nonorm ? P.gs_p : P.ghA_p;
 
-  bool fused_la = false;
   // ---- FFN (gps_layer.py:253-257)
   {
     Operand g_ff2;   // gradient at the output of ff_linear2 (after ff_dropout2)
@@ -1229,40 +1214,18 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     GemmParams g2 = linear_dgrad(P, N, d, 2 * d, g_hid, {a->ff1.weight, d, P.ff1_p}, P.g_s, d);
     g2.R1 = g_t; g2.ldr1 = (int)d;
     g2.Cp = P.gs_p;   // GPS_NORM_NONE only: the branches' products read g_s
-    // norm1_local and norm1_attn both take g_s as their upstream gradient (gps_layer.py:194,217,222): their backward
-    // reductions ride this GEMM's epilogue instead of two more passes over g_s (GPS_B200_OPT bit 64)
-    fused_la = (opt & 64) && !P.nonorm && P.use_planes && g2.Ap.hi && g2.Bp.hi && N > 0 && P.train;
-    if (fused_la) {
-      if (P.loc) {
-        BnView v = bn_view(P, BN_L, a->norm1_local);
-        g2.bnred[0].z = P.xloc; g2.bnred[0].ldz = (int)d; g2.bnred[0].mean = v.mean; g2.bnred[0].invstd = v.invstd;
-        g2.bnred[0].sums = sums(BN_L);
-      }
-      if (P.glob) {
-        BnView v = bn_view(P, BN_A, a->norm1_attn);
-        g2.bnred[1].z = P.hA; g2.bnred[1].ldz = (int)d; g2.bnred[1].mean = v.mean; g2.bnred[1].invstd = v.invstd;
-        g2.bnred[1].sums = sums(BN_A);
-      }
-    }
     GPS_TRY(gemm(g2, st));
   }
   // the attention-branch backward needs g_s (and hA) only: it forks here and runs next to norm1_local's backward and
-  // the local-model backward (with GPS_B200_OPT bit 64 both BatchNorm reductions are already in g_s's epilogue)
+  // the local-model backward
   if (two_branches) GPS_TRY(sd->order(st, sa));
 
-  bool chain_x = false;
   // ---- norm1_local / norm1_attn (gps_layer.py:194,217): g_xloc, g_hA
   if (P.loc && !P.nonorm) {
     BnView v = bn_view(P, BN_L, a->norm1_local);
-    if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.xloc, d, N, d, v, -1, nodrop, sums(BN_L), st));
-    chain_x = P.gated && N > 0 && (opt & 32) && P.train;
-    if (chain_x)   // ... and the reduction of local_model.bn_node_x's backward in the same pass (one launch less)
-      GPS_TRY(bn_bwd_apply_chain(P.g_s, d, P.xloc, d, N, d, v, sums(BN_L), P.g_xloc, d, a->norm1_local.grad_weight,
-                                 a->norm1_local.grad_bias, P.grads_accumulate, P.gl1_p, P.xt, d,
-                                 bn_view(P, BN_X, a->bn_node_x), act, P.drop(GPS_SITE_GCN_X), sums(BN_X), st));
-    else
-      GPS_TRY(bn_bwd_apply(P.g_s, d, P.xloc, d, N, d, v, -1, nodrop, sums(BN_L), P.g_xloc, d,
-                           a->norm1_local.grad_weight, a->norm1_local.grad_bias, st, P.grads_accumulate, P.gl1_p));
+    GPS_TRY(bn_bwd_reduce(P.g_s, d, P.xloc, d, N, d, v, -1, nodrop, sums(BN_L), st));
+    GPS_TRY(bn_bwd_apply(P.g_s, d, P.xloc, d, N, d, v, -1, nodrop, sums(BN_L), P.g_xloc, d,
+                         a->norm1_local.grad_weight, a->norm1_local.grad_bias, st, P.grads_accumulate, P.gl1_p));
   }
   // norm1_local's gradients belong to the early group: the weight-gradient stream takes them in before the attention
   // branch (forked before them) records the group's event there; with no global model the group ends here
@@ -1272,7 +1235,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   if (P.attn) {
     if (!P.nonorm) {
       BnView v = bn_view(P, BN_A, a->norm1_attn);
-      if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
+      GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
       GPS_TRY(bn_bwd_apply(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), P.g_hA, d, a->norm1_attn.grad_weight,
                            a->norm1_attn.grad_bias, sa, P.grads_accumulate, P.ghA_p));
     }
@@ -1295,7 +1258,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     const int64_t inner = P.inner, NH = N * P.H, dh = a->perf_dim_head;
     if (!P.nonorm) {
       BnView v = bn_view(P, BN_A, a->norm1_attn);
-      if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
+      GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
       GPS_TRY(bn_bwd_apply(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), P.g_hA, d, a->norm1_attn.grad_weight,
                            a->norm1_attn.grad_bias, sa, P.grads_accumulate));
     }
@@ -1338,7 +1301,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     const GpsBigBird& B = a->bigbird;
     if (!P.nonorm) {
       BnView v = bn_view(P, BN_A, a->norm1_attn);
-      if (!fused_la) GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
+      GPS_TRY(bn_bwd_reduce(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), sa));
       GPS_TRY(bn_bwd_apply(P.g_s, d, P.hA, d, N, d, v, -1, nodrop, sums(BN_A), P.g_hA, d, a->norm1_attn.grad_weight,
                            a->norm1_attn.grad_bias, sa, P.grads_accumulate));
     }
@@ -1392,8 +1355,7 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   if (P.gated) {
     // x_loc = x + drop(act(BN_x(x~))): g_x~ -> gY1[:, 0:d]  (gatedgcn_layer.py:72-83)
     BnView vx = bn_view(P, BN_X, a->bn_node_x);
-    if (!chain_x)
-      GPS_TRY(bn_bwd_reduce(g_xloc, d, P.xt, d, N, d, vx, act, P.drop(GPS_SITE_GCN_X), sums(BN_X), st));
+    GPS_TRY(bn_bwd_reduce(g_xloc, d, P.xt, d, N, d, vx, act, P.drop(GPS_SITE_GCN_X), sums(BN_X), st));
     GPS_TRY(bn_bwd_apply(g_xloc, d, P.xt, d, N, d, vx, act, P.drop(GPS_SITE_GCN_X), sums(BN_X), P.gY1, P.Wy,
                          a->bn_node_x.grad_weight, a->bn_node_x.grad_bias, st, P.grads_accumulate, P.gY1_p));
     GPS_TRY(sd->order(se, st));

@@ -97,7 +97,7 @@ def test_widths_a_layout_cannot_take_are_rejected(bn, ta, tb):
 
 def _layer_step(wl, precision, drop, adrop):
     """One GPSLayer fwd + bwd on the workload's batch: every Linear epilogue of the layer runs (bias, ReLU, dropout,
-    residuals, plane outputs, BatchNorm statistics and the fused BatchNorm-backward sums)."""
+    residuals, plane outputs and BatchNorm statistics)."""
     spec = graphgps_b200.SHAPES[wl]
     _call._drop_counters.clear()   # the same dropout masks in every run
     torch.manual_seed(0)
@@ -140,7 +140,7 @@ def test_layer_step_bitwise_across_tile_widths(precision, drop, adrop):
 def test_layer_with_128_wide_tiles_matches_fp64_oracle():
     """Every GEMM of the pcqm4m-small layer forced to 128-wide tiles (a width every layout takes) against the fp64
     oracle at the tolerances of test_layer_gpu.py: the epilogues (bias, ReLU, residuals, plane outputs, BatchNorm
-    statistics, fused BatchNorm-backward sums, split-K) checked independently of the 64-wide path.  The policy's own
+    statistics, split-K) checked independently of the 64-wide path.  The policy's own
     widths are checked the same way by test_layer_gpu.py::test_layer_matches_oracle_full_size."""
     from test_layer_gpu import _full_size
     _forced(128)
