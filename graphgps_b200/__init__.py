@@ -5,6 +5,7 @@ Public surface (mirrors the reference's module boundary, SURVEY.md section 8b):
     GraphormerLayer  drop-in for graphgps.layer.graphormer_layer.GraphormerLayer
     BiasEncoder   drop-in for graphgps.encoder.graphormer_encoder.BiasEncoder (Graphormer's attn_bias)
     SANLayer      drop-in for graphgps.layer.san_layer.SANLayer
+    SAN2Layer     drop-in for graphgps.layer.san2_layer.SAN2Layer
     GatedGCNLayer, GINEConvLayer  drop-ins for CustomGNN's graphgps.layer.gatedgcn_layer.GatedGCNLayer and
                   graphgps.layer.gine_conv_layer.GINEConvLayer
     GraphBatch    duck-typed stand-in for a collated PyG Batch (PyG is optional)
@@ -17,11 +18,11 @@ from .batch import GraphBatch, SHAPES, make_batch, batch_from_lists  # noqa: F40
 from .gps_layer import GPSLayer  # noqa: F401
 from .graphormer import GraphormerLayer  # noqa: F401
 from .graphormer_bias import BiasEncoder  # noqa: F401
-from .san import SANLayer  # noqa: F401
+from .san import SAN2Layer, SANLayer  # noqa: F401
 from .custom_gnn import GatedGCNLayer, GINEConvLayer  # noqa: F401
 from .dp import GradBucket  # noqa: F401
 from .stack import GPSStack  # noqa: F401
 from .loader import BatchPrefetcher, collate  # noqa: F401
 
-__all__ = ["GPSLayer", "GraphormerLayer", "BiasEncoder", "SANLayer", "GatedGCNLayer", "GINEConvLayer", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
+__all__ = ["GPSLayer", "GraphormerLayer", "BiasEncoder", "SANLayer", "SAN2Layer", "GatedGCNLayer", "GINEConvLayer", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
            "batch_from_lists"]

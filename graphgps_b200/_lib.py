@@ -147,10 +147,11 @@ class GpsGraphormerBiasPlan(C.Structure):
 
 
 class GpsSanArgs(C.Structure):
-    """SAN layer (san_layer.py): config, dropout stream, graph and nmax, tensors, scratch, the ten Linears
-    attention.{Q,K,V,Q_2,K_2,E,E_2}, O_h, FFN_h_layer1, FFN_h_layer2, batch_norm{1,2}_h and attention.fake_edge_emb."""
+    """SAN layer (san_layer.py, variant 0) or SAN2 layer (san2_layer.py, variant 1): config, dropout stream, graph and
+    nmax, tensors, scratch, the ten Linears attention.{Q,K,V,Q_2,K_2,E,E_2}, O_h, FFN_h_layer1, FFN_h_layer2,
+    batch_norm{1,2}_h, attention.fake_edge_emb and (variant 1) the float64 attention.gamma and its gradient."""
     _fields_ = [("d", C.c_int64), ("heads", C.c_int64), ("training", C.c_int32), ("precision", C.c_int32),
-                ("gamma", C.c_float), ("dropout", C.c_float), ("flags", C.c_int32), ("reserved", C.c_int32),
+                ("gamma", C.c_float), ("dropout", C.c_float), ("flags", C.c_int32), ("variant", C.c_int32),
                 ("seed", C.c_uint64), ("offset", C.c_uint64), ("offset_dev", _fp),
                 ("graph", GpsGraph), ("nmax", C.c_int64),
                 ("x", _fp), ("edge_attr", _fp), ("x_out", _fp), ("grad_x_out", _fp), ("grad_x", _fp),
@@ -159,7 +160,7 @@ class GpsSanArgs(C.Structure):
                 ("Q", GpsLinear), ("K", GpsLinear), ("V", GpsLinear), ("Q2", GpsLinear), ("K2", GpsLinear),
                 ("E", GpsLinear), ("E2", GpsLinear), ("O_h", GpsLinear), ("ffn1", GpsLinear), ("ffn2", GpsLinear),
                 ("bn1", GpsBatchNorm), ("bn2", GpsBatchNorm),
-                ("fake_edge_emb", _fp), ("grad_fake_edge_emb", _fp)]
+                ("fake_edge_emb", _fp), ("grad_fake_edge_emb", _fp), ("gamma_param", _fp), ("grad_gamma", _fp)]
 
 
 class GpsSanPlan(C.Structure):
@@ -226,6 +227,11 @@ SYMBOLS = {
                                             _fp, _i64, _fp, _fp]),
     "gps_san_attention_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _i64, _fp, _fp, _f32, _i64, _fp,
                                              _i64, _fp, _fp, _i64, _fp, _fp, _i64, _fp, _fp, _fp]),
+    "gps_san2_attention_workspace_bytes": (_i64, [_i64, _i64, _i64, _i64]),
+    "gps_san2_attention_forward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _i64, _fp, _fp, _fp, _i64, _fp,
+                                             _i64, _fp, _i64, _fp, _fp, _fp, _fp]),
+    "gps_san2_attention_backward": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _i64, _fp, _fp, _fp, _i64, _fp,
+                                              _i64, _fp, _fp, _fp, _fp, _i64, _fp, _i64, _fp, _fp, _fp, _fp]),
     "gps_layernorm_forward": (C.c_int, [_fp, _i64, _i64, _fp, _fp, _f32, _fp, _fp, _fp, _fp]),
     "gps_layernorm_backward": (C.c_int, [_fp, _fp, _i64, _i64, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _i32, _fp]),
     "gps_linear_forward": (C.c_int, [_fp, _i64, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64, _i32, _i32, _fp]),

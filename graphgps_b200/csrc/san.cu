@@ -17,6 +17,10 @@
 // the CSC, fake part over the graph's queries, scores recomputed), then the fixed-order column sum
 // g_E2 = sum_i g_Q2'[i] (.) Q2[i] and the fold's backward.  No float atomics: two runs give the same bits.
 //
+// SAN2Layer (GpsSanArgs.variant = 1) shares the layer and swaps the attention stage: k_san2_fwd / k_san2_bwd_q /
+// k_san2_bwd_k / k_san2_gamma below (softmax per set with a running max, the learned float64 gamma read on the
+// device); only the attention's saved buffers differ (R, F, lse in place of rz).
+//
 // Layer (one C call per direction; dense products on the TMA GEMM through layer_ops.cuh, BatchNorms through the bn_*
 // stages of kernels.cuh):
 //   forward:  planes -> bitmap + E2 -> [Q|K|V|Q2|K2] = x Wcat^T  (and E = edge_attr W_E^T on the side stream)
@@ -515,6 +519,446 @@ __global__ void k_san_fold_bwd(const float* __restrict__ part, int nparts, int64
   }
 }
 
+// =================================================================================== SAN2 attention
+// SAN2Layer (graphgps/layer/san2_layer.py): per (i, h) a softmax over the real in-edges and one over the fake pairs,
+//   R = sum_k alpha_k V[j_k],  alpha = exp(t - max) / (sum exp(t - max) + 1e-16)     (pyg_softmax, san2_layer.py:11-33)
+//   F = sum_p beta_p V[j_p],   beta likewise over the fake scores u
+//   attn = (R + gamma F) / (gamma + 1)
+// with gamma one float64 read on the device.  No clamp: each set keeps a running max, its accumulators are rescaled
+// when the max grows, and its log-sum-exp lse = max + log(sum) is saved, so the backward recomputes alpha = exp(t -
+// lse) and beta = exp(u - lse_f).  Backward, per (i, h), with g = g_attn[i]:
+//   Dr = g . R, Df = g . F;  g_t = alpha (g . V[j] - Dr) / (gamma + 1),  g_u = gamma beta (g . V[j] - Df) / (gamma + 1)
+//   g_gamma = sum_{i,h} (Df - Dr) / (gamma + 1)^2
+constexpr float kSan2Eps = 1e-16f;   // pyg_softmax's denominator term (san2_layer.py:31)
+
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+struct San2Mix {
+  float cr, cf;   // 1 / (gamma + 1), gamma / (gamma + 1), formed in float64 as the SAN path forms them on the host
+};
+
+__device__ __forceinline__ San2Mix san2_mix(const double* gamma) {
+  const double gm = *gamma;
+  return {(float)(1.0 / (gm + 1.0)), (float)(gm / (gm + 1.0))};
+}
+
+// One set's online softmax over chunks of 32 keys: the lane's score t (-inf when the lane has no key), value row v.
+struct San2Acc {
+  float acc[kSanCh];
+  float m, z;   // running max (warp-uniform) and this lane's share of the sum
+  __device__ __forceinline__ void init() {
+#pragma unroll
+    for (int c = 0; c < kSanCh; ++c) acc[c] = 0.f;
+    m = -INFINITY;
+    z = 0.f;
+  }
+  // s_s / s_v: the warp's staging rows.  Returns after the chunk's values are accumulated.
+  __device__ __forceinline__ void chunk(float t, const float* vrow, float* s_s, const float** s_v, int nk, int lane,
+                                        int hd) {
+    const float cm = warp_max(t);
+    if (cm == -INFINITY) return;   // no key in this chunk (warp-uniform)
+    const float mn = fmaxf(m, cm);
+    const float corr = expf(m - mn);   // 0 on the first chunk (m = -inf), when acc and z are 0
+    const float s = t == -INFINITY ? 0.f : expf(t - mn);
+    z = z * corr + s;
+#pragma unroll
+    for (int c = 0; c < kSanCh; ++c) acc[c] *= corr;
+    m = mn;
+    s_s[lane] = s;
+    s_v[lane] = vrow;
+    __syncwarp();
+    for (int kk = 0; kk < nk; ++kk) {
+      const float sk = s_s[kk];
+      if (sk == 0.f) continue;
+      const float* v = s_v[kk];
+#pragma unroll
+      for (int c = 0; c < kSanCh; ++c) {
+        const int cc = lane + 32 * c;
+        if (cc < hd) acc[c] = fmaf(sk, v[cc], acc[c]);
+      }
+    }
+    __syncwarp();
+  }
+};
+
+// one warp per (i, h): R, F (pitch d), lse [2, N, H]; attn = cr R + cf F into O (and times the dropout scales into Od
+// when drop.p > 0, with Od's planes)
+__global__ void __launch_bounds__(32 * kSanWarps) k_san2_fwd(SanAttn a, const double* __restrict__ gamma,
+                                                             float* __restrict__ O, float* __restrict__ Od, int64_t ldo,
+                                                             Planes Odp, float* __restrict__ R, float* __restrict__ F,
+                                                             float* __restrict__ lse, DropCfg drop) {
+  __shared__ float s_q[kSanWarps][kSanMaxHd], s_q2[kSanWarps][kSanMaxHd];
+  __shared__ float s_s[kSanWarps][32];
+  __shared__ const float* s_v[kSanWarps][32];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t item = (int64_t)blockIdx.x * kSanWarps + w;
+  if (item >= a.g.N * a.H) return;
+  const int i = (int)(item / a.H), h = (int)(item % a.H), hd = a.hd;
+  const int64_t col = (int64_t)h * hd, NH = a.g.N * a.H;
+  const San2Mix mx = san2_mix(gamma);
+  float* q = s_q[w];
+  float* q2 = s_q2[w];
+  for (int c = lane; c < hd; c += 32) {
+    q[c] = a.Q[(int64_t)i * a.ld + col + c];
+    q2[c] = a.Q2[(int64_t)i * a.ld + col + c] * __ldg(a.E2 + col + c);
+  }
+  __syncwarp();
+  const int gi = graph_of_node(a.g.graph_ptr, a.g.B, i);
+  const int g0 = a.g.graph_ptr[gi], g1 = a.g.graph_ptr[gi + 1];
+  float o[kSanCh];
+  // fake pairs: every key of the graph but i itself and the real sources of i
+  San2Acc st;
+  st.init();
+  for (int j0 = g0; j0 < g1; j0 += 32) {
+    const int j = j0 + lane;
+    float t = -INFINITY;
+    const float* vrow = nullptr;
+    if (j < g1 && j != i && !is_real(a, i, j - g0)) {
+      const float* k2 = a.K2 + (int64_t)j * a.ld + col;
+      float u = 0.f;
+      for (int c = 0; c < hd; ++c) u = fmaf(k2[c], q2[c], u);
+      t = u * a.scale;
+      vrow = a.V + (int64_t)j * a.ld + col;
+    }
+    st.chunk(t, vrow, s_s[w], s_v[w], min(32, g1 - j0), lane, hd);
+  }
+  float z = warp_sum(st.z);
+  float r = 1.f / (z + kSan2Eps);
+  if (lane == 0) lse[NH + item] = z > 0.f ? st.m + logf(z) : 0.f;
+#pragma unroll
+  for (int m = 0; m < kSanCh; ++m) {
+    const int c = lane + 32 * m;
+    const float f = st.acc[m] * r;
+    o[m] = mx.cf * f;
+    if (c < hd) F[(int64_t)i * a.d + col + c] = f;
+  }
+  // real edges into i, in CSR order
+  st.init();
+  const int e0 = a.g.dst_ptr[i], e1 = a.g.dst_ptr[i + 1];
+  for (int eb = e0; eb < e1; eb += 32) {
+    const int e = eb + lane;
+    float t = -INFINITY;
+    const float* vrow = nullptr;
+    if (e < e1) {
+      const int j = a.g.dst_src[e];
+      const int64_t k = a.g.dst_eid[e];
+      const float* kr = a.K + (int64_t)j * a.ld + col;
+      const float* er = a.E + k * a.d + col;
+      float u = 0.f;
+      for (int c = 0; c < hd; ++c) u = fmaf(kr[c] * q[c], er[c], u);
+      t = u * a.scale;
+      vrow = a.V + (int64_t)j * a.ld + col;
+    }
+    st.chunk(t, vrow, s_s[w], s_v[w], min(32, e1 - eb), lane, hd);
+  }
+  z = warp_sum(st.z);
+  r = 1.f / (z + kSan2Eps);
+  if (lane == 0) lse[item] = z > 0.f ? st.m + logf(z) : 0.f;
+#pragma unroll
+  for (int m = 0; m < kSanCh; ++m) {
+    const int c = lane + 32 * m;
+    if (c >= hd) continue;
+    const float rr = st.acc[m] * r;
+    const int64_t cc = col + c;
+    R[(int64_t)i * a.d + cc] = rr;
+    const float ov = fmaf(mx.cr, rr, o[m]);
+    O[(int64_t)i * ldo + cc] = ov;
+    float od = ov;
+    if (drop.p > 0.f) {
+      od = ov * drop_scale1(drop, (int64_t)i * a.d + cc);
+      Od[(int64_t)i * ldo + cc] = od;
+    }
+    plane_store1(Odp, i, cc, od);
+  }
+}
+
+// Query-major pass, one warp per (i, h): Dr, Df [N, H]; g_Q2' -> g_Q2 = g_Q2' (.) E2 and pq = g_Q2' (.) Q2; g_Q and
+// each real edge's g_E row.
+__global__ void __launch_bounds__(32 * kSanWarps) k_san2_bwd_q(SanAttn a, const double* __restrict__ gamma,
+                                                               const float* __restrict__ R,
+                                                               const float* __restrict__ F,
+                                                               const float* __restrict__ lse,
+                                                               const float* __restrict__ gO, int64_t ldo,
+                                                               float* __restrict__ Dr, float* __restrict__ Df,
+                                                               SanGrad G, float* __restrict__ pq) {
+  __shared__ float s_q[kSanWarps][kSanMaxHd], s_q2[kSanWarps][kSanMaxHd], s_g[kSanWarps][kSanMaxHd];
+  __shared__ float s_t[kSanWarps][32];
+  __shared__ int s_j[kSanWarps][32], s_k[kSanWarps][32];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t item = (int64_t)blockIdx.x * kSanWarps + w;
+  if (item >= a.g.N * a.H) return;
+  const int i = (int)(item / a.H), h = (int)(item % a.H), hd = a.hd;
+  const int64_t col = (int64_t)h * hd, NH = a.g.N * a.H;
+  const San2Mix mx = san2_mix(gamma);
+  float* q = s_q[w];
+  float* q2 = s_q2[w];
+  float* gw = s_g[w];
+  float dr = 0.f, df = 0.f;
+  for (int c = lane; c < hd; c += 32) {
+    q[c] = a.Q[(int64_t)i * a.ld + col + c];
+    q2[c] = a.Q2[(int64_t)i * a.ld + col + c] * __ldg(a.E2 + col + c);
+    const float go = gO[(int64_t)i * ldo + col + c];
+    gw[c] = go;
+    dr = fmaf(go, R[(int64_t)i * a.d + col + c], dr);
+    df = fmaf(go, F[(int64_t)i * a.d + col + c], df);
+  }
+  dr = warp_sum(dr);
+  df = warp_sum(df);
+  if (lane == 0) {
+    Dr[item] = dr;
+    Df[item] = df;
+  }
+  const float lr = lse[item], lf = lse[NH + item];
+  __syncwarp();
+  const int gi = graph_of_node(a.g.graph_ptr, a.g.B, i);
+  const int g0 = a.g.graph_ptr[gi], g1 = a.g.graph_ptr[gi + 1];
+  float acc[kSanCh];
+#pragma unroll
+  for (int m = 0; m < kSanCh; ++m) acc[m] = 0.f;
+  for (int j0 = g0; j0 < g1; j0 += 32) {
+    const int j = j0 + lane;
+    float gt = 0.f;
+    if (j < g1 && j != i && !is_real(a, i, j - g0)) {
+      const float* k2 = a.K2 + (int64_t)j * a.ld + col;
+      const float* v = a.V + (int64_t)j * a.ld + col;
+      float t = 0.f, gv = 0.f;
+      for (int c = 0; c < hd; ++c) {
+        t = fmaf(k2[c], q2[c], t);
+        gv = fmaf(gw[c], v[c], gv);
+      }
+      gt = mx.cf * expf(t * a.scale - lf) * (gv - df) * a.scale;
+    }
+    s_t[w][lane] = gt;
+    __syncwarp();
+    const int nk = min(32, g1 - j0);
+    for (int kk = 0; kk < nk; ++kk) {
+      const float g = s_t[w][kk];
+      if (g == 0.f) continue;
+      const float* k2 = a.K2 + (int64_t)(j0 + kk) * a.ld + col;
+#pragma unroll
+      for (int m = 0; m < kSanCh; ++m) {
+        const int c = lane + 32 * m;
+        if (c < hd) acc[m] = fmaf(g, k2[c], acc[m]);
+      }
+    }
+    __syncwarp();
+  }
+#pragma unroll
+  for (int m = 0; m < kSanCh; ++m) {   // acc = g_Q2'
+    const int c = lane + 32 * m;
+    if (c >= hd) continue;
+    const int64_t cc = col + c;
+    const float gq2 = acc[m] * __ldg(a.E2 + cc);
+    G.gQ2[(int64_t)i * G.ldg + cc] = gq2;
+    plane_store1(G.gQ2p, i, cc, gq2);
+    pq[(int64_t)i * a.d + cc] = acc[m] * a.Q2[(int64_t)i * a.ld + cc];
+    acc[m] = 0.f;
+  }
+  const int e0 = a.g.dst_ptr[i], e1 = a.g.dst_ptr[i + 1];
+  for (int eb = e0; eb < e1; eb += 32) {
+    const int e = eb + lane;
+    float gt = 0.f;
+    int j = 0, k = 0;
+    if (e < e1) {
+      j = a.g.dst_src[e];
+      k = a.g.dst_eid[e];
+      const float* kr = a.K + (int64_t)j * a.ld + col;
+      const float* er = a.E + (int64_t)k * a.d + col;
+      const float* v = a.V + (int64_t)j * a.ld + col;
+      float t = 0.f, gv = 0.f;
+      for (int c = 0; c < hd; ++c) {
+        t = fmaf(kr[c] * q[c], er[c], t);
+        gv = fmaf(gw[c], v[c], gv);
+      }
+      gt = mx.cr * expf(t * a.scale - lr) * (gv - dr) * a.scale;
+    }
+    s_t[w][lane] = gt;
+    s_j[w][lane] = j;
+    s_k[w][lane] = k;
+    __syncwarp();
+    const int nk = min(32, e1 - eb);
+    for (int kk = 0; kk < nk; ++kk) {
+      const float g = s_t[w][kk];
+      const int jj = s_j[w][kk], ke = s_k[w][kk];
+      const float* kr = a.K + (int64_t)jj * a.ld + col;
+      const float* er = a.E + (int64_t)ke * a.d + col;
+#pragma unroll
+      for (int m = 0; m < kSanCh; ++m) {
+        const int c = lane + 32 * m;
+        if (c >= hd) continue;
+        const float kc = kr[c];
+        acc[m] = fmaf(g * kc, er[c], acc[m]);
+        const float ge = g * kc * q[c];
+        G.gE[(int64_t)ke * a.d + col + c] = ge;
+        plane_store1(G.gEp, ke, col + c, ge);
+      }
+    }
+    __syncwarp();
+  }
+#pragma unroll
+  for (int m = 0; m < kSanCh; ++m) {
+    const int c = lane + 32 * m;
+    if (c >= hd) continue;
+    G.gQ[(int64_t)i * G.ldg + col + c] = acc[m];
+    plane_store1(G.gQp, i, col + c, acc[m]);
+  }
+}
+
+// Key-major pass, one warp per (j, h): g_K (real edges out of j, over the CSC), g_K2 (fake pairs: the graph's queries
+// i != j without a real edge j -> i) and g_V (both), the weights recomputed from the saved log-sum-exps.
+__global__ void __launch_bounds__(32 * kSanWarps) k_san2_bwd_k(SanAttn a, const double* __restrict__ gamma,
+                                                               const float* __restrict__ lse,
+                                                               const float* __restrict__ gO, int64_t ldo,
+                                                               const float* __restrict__ Dr,
+                                                               const float* __restrict__ Df, SanGrad G) {
+  __shared__ float s_k[kSanWarps][kSanMaxHd], s_k2[kSanWarps][kSanMaxHd], s_v[kSanWarps][kSanMaxHd];
+  __shared__ float s_t[kSanWarps][32], s_s[kSanWarps][32];
+  __shared__ int s_i[kSanWarps][32], s_e[kSanWarps][32];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t item = (int64_t)blockIdx.x * kSanWarps + w;
+  if (item >= a.g.N * a.H) return;
+  const int j = (int)(item / a.H), h = (int)(item % a.H), hd = a.hd;
+  const int64_t col = (int64_t)h * hd, NH = a.g.N * a.H;
+  const San2Mix mx = san2_mix(gamma);
+  float* kk_ = s_k[w];
+  float* k2 = s_k2[w];
+  float* vj = s_v[w];
+  for (int c = lane; c < hd; c += 32) {
+    kk_[c] = a.K[(int64_t)j * a.ld + col + c];
+    k2[c] = a.K2[(int64_t)j * a.ld + col + c];
+    vj[c] = a.V[(int64_t)j * a.ld + col + c];
+  }
+  __syncwarp();
+  const int gi = graph_of_node(a.g.graph_ptr, a.g.B, j);
+  const int g0 = a.g.graph_ptr[gi], g1 = a.g.graph_ptr[gi + 1];
+  float gk[kSanCh], gv[kSanCh];
+#pragma unroll
+  for (int m = 0; m < kSanCh; ++m) gk[m] = gv[m] = 0.f;
+  // fake pairs j -> i
+  for (int i0 = g0; i0 < g1; i0 += 32) {
+    const int i = i0 + lane;
+    float gt = 0.f, sr = 0.f;
+    if (i < g1 && i != j && !is_real(a, i, j - g0)) {
+      const float* q2 = a.Q2 + (int64_t)i * a.ld + col;
+      const float* go = gO + (int64_t)i * ldo + col;
+      float t = 0.f, gvv = 0.f;
+      for (int c = 0; c < hd; ++c) {
+        t = fmaf(k2[c], q2[c] * __ldg(a.E2 + col + c), t);
+        gvv = fmaf(go[c], vj[c], gvv);
+      }
+      const int64_t ih = (int64_t)i * a.H + h;
+      sr = mx.cf * expf(t * a.scale - lse[NH + ih]);
+      gt = sr * (gvv - Df[ih]) * a.scale;
+    }
+    s_t[w][lane] = gt;
+    s_s[w][lane] = sr;
+    __syncwarp();
+    const int nq = min(32, g1 - i0);
+    for (int qq = 0; qq < nq; ++qq) {
+      const float s = s_s[w][qq];
+      if (s == 0.f) continue;
+      const float g = s_t[w][qq];
+      const float* q2 = a.Q2 + (int64_t)(i0 + qq) * a.ld + col;
+      const float* go = gO + (int64_t)(i0 + qq) * ldo + col;
+#pragma unroll
+      for (int m = 0; m < kSanCh; ++m) {
+        const int c = lane + 32 * m;
+        if (c >= hd) continue;
+        gk[m] = fmaf(g, q2[c] * __ldg(a.E2 + col + c), gk[m]);   // g_K2
+        gv[m] = fmaf(s, go[c], gv[m]);
+      }
+    }
+    __syncwarp();
+  }
+#pragma unroll
+  for (int m = 0; m < kSanCh; ++m) {
+    const int c = lane + 32 * m;
+    if (c >= hd) continue;
+    G.gK2[(int64_t)j * G.ldg + col + c] = gk[m];
+    plane_store1(G.gK2p, j, col + c, gk[m]);
+    gk[m] = 0.f;
+  }
+  // real edges j -> i, in CSC order
+  const int e0 = a.g.src_ptr[j], e1 = a.g.src_ptr[j + 1];
+  for (int eb = e0; eb < e1; eb += 32) {
+    const int e = eb + lane;
+    float gt = 0.f, sr = 0.f;
+    int i = 0, k = 0;
+    if (e < e1) {
+      i = a.g.src_dst[e];
+      k = a.g.src_eid[e];
+      const float* q = a.Q + (int64_t)i * a.ld + col;
+      const float* er = a.E + (int64_t)k * a.d + col;
+      const float* go = gO + (int64_t)i * ldo + col;
+      float t = 0.f, gvv = 0.f;
+      for (int c = 0; c < hd; ++c) {
+        t = fmaf(kk_[c] * q[c], er[c], t);
+        gvv = fmaf(go[c], vj[c], gvv);
+      }
+      const int64_t ih = (int64_t)i * a.H + h;
+      sr = mx.cr * expf(t * a.scale - lse[ih]);
+      gt = sr * (gvv - Dr[ih]) * a.scale;
+    }
+    s_t[w][lane] = gt;
+    s_s[w][lane] = sr;
+    s_i[w][lane] = i;
+    s_e[w][lane] = k;
+    __syncwarp();
+    const int nq = min(32, e1 - eb);
+    for (int qq = 0; qq < nq; ++qq) {
+      const float g = s_t[w][qq], s = s_s[w][qq];
+      const int ii = s_i[w][qq], ke = s_e[w][qq];
+      const float* q = a.Q + (int64_t)ii * a.ld + col;
+      const float* er = a.E + (int64_t)ke * a.d + col;
+      const float* go = gO + (int64_t)ii * ldo + col;
+#pragma unroll
+      for (int m = 0; m < kSanCh; ++m) {
+        const int c = lane + 32 * m;
+        if (c >= hd) continue;
+        gk[m] = fmaf(g * q[c], er[c], gk[m]);
+        gv[m] = fmaf(s, go[c], gv[m]);
+      }
+    }
+    __syncwarp();
+  }
+#pragma unroll
+  for (int m = 0; m < kSanCh; ++m) {
+    const int c = lane + 32 * m;
+    if (c >= hd) continue;
+    G.gK[(int64_t)j * G.ldg + col + c] = gk[m];
+    plane_store1(G.gKp, j, col + c, gk[m]);
+    G.gV[(int64_t)j * G.ldg + col + c] = gv[m];
+    plane_store1(G.gVp, j, col + c, gv[m]);
+  }
+}
+
+// g_gamma = sum over (i, h) of (Df - Dr) / (gamma + 1)^2, one CTA: each thread sums a fixed stride of items in float64,
+// then a fixed tree; written, or added when accumulate
+constexpr int kSan2GammaThreads = 256;
+__global__ void __launch_bounds__(kSan2GammaThreads) k_san2_gamma(const float* __restrict__ Dr,
+                                                                  const float* __restrict__ Df, int64_t n,
+                                                                  const double* __restrict__ gamma,
+                                                                  double* __restrict__ gg, int accumulate) {
+  __shared__ double s[kSan2GammaThreads];
+  double acc = 0.0;
+  for (int64_t t = threadIdx.x; t < n; t += kSan2GammaThreads) acc += (double)Df[t] - (double)Dr[t];
+  s[threadIdx.x] = acc;
+  __syncthreads();
+  for (int o = kSan2GammaThreads / 2; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double gp1 = *gamma + 1.0;
+    const double v = s[0] / (gp1 * gp1);
+    *gg = accumulate ? *gg + v : v;
+  }
+}
+
 // ------------------------------------------------------------------------------- launchers
 int san_check(int64_t d, int64_t H) {
   GPS_REQUIRE(H > 0 && d > 0 && d % H == 0, GPS_ERR_ARG, "san: d %lld must be a positive multiple of heads %lld",
@@ -561,6 +1005,22 @@ int san_attn_fwd(const SanAttn& a, float* O, float* Od, int64_t ldo, Planes Odp,
 
 int64_t san_parts(int64_t N) { return ceil_div(N > 0 ? N : 1, kSanRowChunk); }
 
+// the fixed-order column sum g_E2 = sum_i pq[i] and the fold's backward (gW / gemb NULL: not wanted)
+int san_e2_bwd(const float* pq, int64_t N, int64_t d, float* part, const float* We2, const float* emb, float* gE2,
+               float* gW, float* gemb, bool accumulate, cudaStream_t st) {
+  const int64_t nparts = san_parts(N);
+  if (N > 0) {
+    k_san_colsum_part<<<dim3((unsigned)nparts, (unsigned)ceil_div(d, 128)), 128, 0, st>>>(pq, N, d, part);
+    GPS_LAUNCH_CHECK();
+  } else {
+    GPS_CUDA(cudaMemsetAsync(part, 0, (size_t)d * sizeof(float), st));
+  }
+  k_san_fold_bwd<<<(unsigned)ceil_div(d, 32), 256, (size_t)d * sizeof(float), st>>>(part, (int)nparts, d, We2, emb, gE2,
+                                                                                  gW, gemb, accumulate ? 1 : 0);
+  GPS_LAUNCH_CHECK();
+  return GPS_OK;
+}
+
 // both passes, then the g_E2 column sum and the fold's backward (gW / gemb NULL: not wanted)
 int san_attn_bwd(const SanAttn& a, const float* O, const float* gO, int64_t ldo, const float* rz, float* Dq,
                  const SanGrad& G, float* pq, float* part, const float* We2, const float* emb, float* gE2, float* gW,
@@ -572,17 +1032,44 @@ int san_attn_bwd(const SanAttn& a, const float* O, const float* gO, int64_t ldo,
     k_san_bwd_k<<<(unsigned)ceil_div(items, kSanWarps), 32 * kSanWarps, 0, st>>>(a, gO, ldo, rz, Dq, G);
     GPS_LAUNCH_CHECK();
   }
-  const int64_t nparts = san_parts(a.g.N);
-  if (a.g.N > 0) {
-    k_san_colsum_part<<<dim3((unsigned)nparts, (unsigned)ceil_div(d, 128)), 128, 0, st>>>(pq, a.g.N, d, part);
-    GPS_LAUNCH_CHECK();
-  } else {
-    GPS_CUDA(cudaMemsetAsync(part, 0, (size_t)d * sizeof(float), st));
-  }
-  k_san_fold_bwd<<<(unsigned)ceil_div(d, 32), 256, (size_t)d * sizeof(float), st>>>(part, (int)nparts, d, We2, emb, gE2,
-                                                                                  gW, gemb, accumulate ? 1 : 0);
+  return san_e2_bwd(pq, a.g.N, d, part, We2, emb, gE2, gW, gemb, accumulate, st);
+}
+
+// SAN2's saved attention state: R, F [N, d] and lse [2, N, H]
+struct San2Saved {
+  float *R, *F, *lse;
+};
+
+int san2_attn_fwd(const SanAttn& a, const double* gamma, float* O, float* Od, int64_t ldo, Planes Odp,
+                  const San2Saved& S, const DropCfg& drop, cudaStream_t st) {
+  const int64_t items = a.g.N * a.H;
+  if (items == 0) return GPS_OK;
+  k_san2_fwd<<<(unsigned)ceil_div(items, kSanWarps), 32 * kSanWarps, 0, st>>>(a, gamma, O, Od, ldo, Odp, S.R, S.F,
+                                                                               S.lse, drop);
   GPS_LAUNCH_CHECK();
   return GPS_OK;
+}
+
+// both passes, the g_gamma reduction (gg NULL: not wanted), then the g_E2 column sum and the fold's backward as SAN's.
+// D: [2, N, H] scratch (Dr, Df)
+int san2_attn_bwd(const SanAttn& a, const double* gamma, const float* R, const float* F, const float* lse,
+                  const float* gO, int64_t ldo, float* D,
+                  const SanGrad& G, double* gg, float* pq, float* part, const float* We2, const float* emb, float* gE2,
+                  float* gW, float* gemb, bool accumulate, cudaStream_t st) {
+  const int64_t items = a.g.N * a.H, d = a.d;
+  float *Dr = D, *Df = D + items;
+  if (items > 0) {
+    k_san2_bwd_q<<<(unsigned)ceil_div(items, kSanWarps), 32 * kSanWarps, 0, st>>>(a, gamma, R, F, lse, gO, ldo, Dr,
+                                                                                   Df, G, pq);
+    GPS_LAUNCH_CHECK();
+    k_san2_bwd_k<<<(unsigned)ceil_div(items, kSanWarps), 32 * kSanWarps, 0, st>>>(a, gamma, lse, gO, ldo, Dr, Df, G);
+    GPS_LAUNCH_CHECK();
+  }
+  if (gg) {
+    k_san2_gamma<<<1, kSan2GammaThreads, 0, st>>>(Dr, Df, items, gamma, gg, accumulate ? 1 : 0);
+    GPS_LAUNCH_CHECK();
+  }
+  return san_e2_bwd(pq, a.g.N, d, part, We2, emb, gE2, gW, gemb, accumulate, st);
 }
 
 // =================================================================================== layer
@@ -590,10 +1077,13 @@ struct SanPlan {
   int64_t N, E, d, H, hd, nmax;
   int prec;
   bool train, grads_prezeroed, grads_accumulate, use_planes;
-  float gamma;
+  int variant;                   // 0: SANLayer, 1: SAN2Layer
+  float gamma;                   // variant 0
+  const double* gamma_dev;       // variant 1: the learned gamma on the device
   DropCfg drop_attn, drop_ffn;   // sites 13, 14 (p = 0 in eval mode)
   // saved
   float *Wcat, *Y, *Ee, *E2, *rz, *attn, *attn_d, *z1, *h1, *hid, *z2, *bnbuf;
+  San2Saved s2;                  // variant 1, in place of rz
   uint32_t* bits;
   Planes Wcat_p, WE_p, WO_p, W1_p, W2_p, x_p, e_p, attnd_p, h1_p, hid_p;
   int64_t saved_bytes;
@@ -602,7 +1092,7 @@ struct SanPlan {
   int64_t fwd_bytes;
   // backward workspace
   double* bsums;
-  float *g_z2, *g_hid, *g_h1, *g_z1, *g_attn, *gY, *gE, *Dq, *pq, *part;
+  float *g_z2, *g_hid, *g_h1, *g_z1, *g_attn, *gY, *gE, *Dq, *pq, *part;   // Dq: [N, H], variant 1 [2, N, H]
   Planes gz2_p, ghid_p, gz1_p, gY_p, gE_p;
   int64_t bwd_bytes;
 };
@@ -619,11 +1109,15 @@ int make_plan(const GpsSanArgs* a, SanPlan* P, bool bind) {
               "san: nmax %lld must be the size of the largest graph (N = %lld)", (long long)a->nmax,
               (long long)a->graph.N);
   GPS_REQUIRE(a->dropout >= 0.f && a->dropout < 1.f, GPS_ERR_ARG, "san: dropout must be in [0,1)");
-  GPS_REQUIRE(a->gamma >= 0.f, GPS_ERR_ARG, "san: gamma must be >= 0");
+  GPS_REQUIRE(a->variant == 0 || a->variant == 1, GPS_ERR_UNSUPPORTED, "san: unknown variant %d (0: SANLayer, "
+              "1: SAN2Layer)", a->variant);
+  GPS_REQUIRE(a->variant == 1 || a->gamma >= 0.f, GPS_ERR_ARG, "san: gamma must be >= 0");
   const int64_t N = a->graph.N, E = a->graph.E, d = a->d;
   P->N = N; P->E = E; P->d = d; P->H = a->heads; P->hd = d / a->heads; P->nmax = a->nmax;
   P->prec = a->precision;
+  P->variant = a->variant;
   P->gamma = a->gamma;
+  P->gamma_dev = a->gamma_param;
   P->train = a->training != 0;
   set_grad_flags(P, a->flags);
   P->drop_attn = drop_cfg(a->dropout, P->train, a->seed, a->offset, a->offset_dev, GPS_SITE_SAN_ATTN);
@@ -637,7 +1131,13 @@ int make_plan(const GpsSanArgs* a, SanPlan* P, bool bind) {
   P->Ee = S.alloc<float>(E * d);
   P->E2 = S.alloc<float>(d);
   P->bits = S.alloc<uint32_t>(N * san_words(a->nmax));
-  P->rz = S.alloc<float>(N * P->H);
+  if (P->variant == 0) {
+    P->rz = S.alloc<float>(N * P->H);
+  } else {
+    P->s2.lse = S.alloc<float>(2 * N * P->H);
+    P->s2.R = S.alloc<float>(N * d);
+    P->s2.F = S.alloc<float>(N * d);
+  }
   P->attn = S.alloc<float>(N * d);
   P->attn_d = P->drop_attn.p > 0.f ? S.alloc<float>(N * d) : P->attn;
   P->z1 = S.alloc<float>(N * d);
@@ -674,7 +1174,7 @@ int make_plan(const GpsSanArgs* a, SanPlan* P, bool bind) {
   P->g_attn = Bk.alloc<float>(N * d);
   P->gY = Bk.alloc<float>(N * 5 * d);
   P->gE = Bk.alloc<float>(E * d);
-  P->Dq = Bk.alloc<float>(N * P->H);
+  P->Dq = Bk.alloc<float>((P->variant == 0 ? 1 : 2) * N * P->H);
   P->pq = Bk.alloc<float>(N * d);
   P->part = Bk.alloc<float>(san_parts(N) * d);
   if (P->use_planes) {
@@ -708,6 +1208,7 @@ int check_params(const GpsSanArgs* a) {
               "san: missing parameter or buffer of batch_norm1_h");
   GPS_REQUIRE(a->bn2.weight && a->bn2.bias && a->bn2.running_mean && a->bn2.running_var, GPS_ERR_ARG,
               "san: missing parameter or buffer of batch_norm2_h");
+  GPS_REQUIRE(a->variant == 0 || a->gamma_param, GPS_ERR_ARG, "san: missing parameter attention.gamma (SAN2Layer)");
   return GPS_OK;
 }
 
@@ -767,7 +1268,8 @@ int san_forward(const GpsSanArgs* a, cudaStream_t st) {
   GPS_TRY(gemm(linear_fwd(P, N, 5 * d, d, {a->x, d, P.x_p}, {Wcat, d, P.Wcat_p}, P.Y, 5 * d), st));
   if (E > 0) GPS_TRY(sd->join(st));
   const SanAttn at = san_attn(a->graph, P.H, P.hd, P.Y, 5 * d, P.Ee, P.E2, P.bits, P.nmax, P.gamma);
-  GPS_TRY(san_attn_fwd(at, P.attn, P.attn_d, d, P.attnd_p, P.rz, P.drop_attn, st));
+  if (P.variant == 0) GPS_TRY(san_attn_fwd(at, P.attn, P.attn_d, d, P.attnd_p, P.rz, P.drop_attn, st));
+  else GPS_TRY(san2_attn_fwd(at, P.gamma_dev, P.attn, P.attn_d, d, P.attnd_p, P.s2, P.drop_attn, st));
   // z1 = x + O_h(drop(attn)), BN1's column sums
   GemmParams g = linear_fwd(P, N, d, d, {P.attn_d, d, P.attnd_p}, {a->O_h.weight, d, P.WO_p}, P.z1, d, a->O_h.bias);
   g.R1 = a->x; g.ldr1 = (int)d;
@@ -802,6 +1304,7 @@ int zero_grads(const GpsSanArgs* a, const SanPlan& P, cudaStream_t st) {
     if (b->grad_bias) GPS_CUDA(cudaMemsetAsync(b->grad_bias, 0, (size_t)d * sizeof(float), st));
   }
   if (a->grad_fake_edge_emb) GPS_CUDA(cudaMemsetAsync(a->grad_fake_edge_emb, 0, (size_t)d * sizeof(float), st));
+  if (P.variant == 1 && a->grad_gamma) GPS_CUDA(cudaMemsetAsync(a->grad_gamma, 0, sizeof(double), st));
   return GPS_OK;
 }
 
@@ -855,8 +1358,12 @@ int san_backward(const GpsSanArgs* a, cudaStream_t st) {
   G.gQp = P.gY_p.cols(0); G.gKp = P.gY_p.cols(d); G.gVp = P.gY_p.cols(2 * d); G.gQ2p = P.gY_p.cols(3 * d);
   G.gK2p = P.gY_p.cols(4 * d);
   G.gE = P.gE; G.gEp = P.gE_p;
-  GPS_TRY(san_attn_bwd(at, P.attn, P.g_attn, d, P.rz, P.Dq, G, P.pq, P.part, a->E2.weight, a->fake_edge_emb, nullptr,
-                       a->E2.grad_weight, a->grad_fake_edge_emb, P.grads_accumulate, st));
+  if (P.variant == 0)
+    GPS_TRY(san_attn_bwd(at, P.attn, P.g_attn, d, P.rz, P.Dq, G, P.pq, P.part, a->E2.weight, a->fake_edge_emb, nullptr,
+                         a->E2.grad_weight, a->grad_fake_edge_emb, P.grads_accumulate, st));
+  else
+    GPS_TRY(san2_attn_bwd(at, P.gamma_dev, P.s2.R, P.s2.F, P.s2.lse, P.g_attn, d, P.Dq, G, a->grad_gamma, P.pq, P.part, a->E2.weight,
+                          a->fake_edge_emb, nullptr, a->E2.grad_weight, a->grad_fake_edge_emb, P.grads_accumulate, st));
   // weight gradients of the five node projections (one product when the caller's buffers are consecutive) and of E
   GPS_TRY(sd->fork(st));
   const Operand gY{P.gY, 5 * d, P.gY_p};
@@ -971,4 +1478,75 @@ extern "C" int gps_san_attention_backward(const GpsGraph* g, int64_t heads, int6
   G.ldg = ldg;
   G.gE = dE;
   return san_attn_bwd(a, O, dO, ldo, rz, Dq, G, pq, part, nullptr, nullptr, dE2, nullptr, nullptr, false, st);
+}
+
+extern "C" int64_t gps_san2_attention_workspace_bytes(int64_t N, int64_t d, int64_t heads, int64_t nmax) {
+  Arena A(nullptr, 0);
+  A.alloc<uint32_t>(N * san_words(nmax));
+  A.alloc<float>(2 * N * (heads > 0 ? heads : 1));
+  A.alloc<float>(N * d);
+  A.alloc<float>(san_parts(N) * d);
+  return A.used;
+}
+
+namespace {
+// SAN2's stage calls: the SAN stage's checks with the workspace carve-up (bitmap | Dr, Df | pq | part)
+int san2_stage_setup(const GpsGraph* g, int64_t heads, int64_t hd, int64_t nmax, int64_t ld, const double* gamma,
+                     void* ws, int64_t ws_bytes, uint32_t** bits, float** D, float** pq, float** part) {
+  GPS_REQUIRE(g, GPS_ERR_ARG, "san2 attention: null graph");
+  GPS_REQUIRE(heads > 0 && hd > 0, GPS_ERR_ARG, "san2 attention: heads and hd must be positive");
+  GPS_TRY(san_check(heads * hd, heads));
+  const int64_t d = heads * hd;
+  GPS_REQUIRE(ld >= 5 * d, GPS_ERR_ARG, "san2 attention: ld %lld < 5 d", (long long)ld);
+  GPS_REQUIRE(nmax >= 0 && (g->N == 0 || nmax >= 1) && nmax <= g->N, GPS_ERR_ARG, "san2 attention: bad nmax %lld",
+              (long long)nmax);
+  GPS_REQUIRE(gamma, GPS_ERR_ARG, "san2 attention: null gamma");
+  GPS_REQUIRE(ws && ws_bytes >= gps_san2_attention_workspace_bytes(g->N, d, heads, nmax), GPS_ERR_ARG,
+              "san2 attention: workspace too small");
+  Arena A(ws, ws_bytes);
+  *bits = A.alloc<uint32_t>(g->N * san_words(nmax));
+  *D = A.alloc<float>(2 * g->N * heads);
+  *pq = A.alloc<float>(g->N * d);
+  *part = A.alloc<float>(san_parts(g->N) * d);
+  return GPS_OK;
+}
+}  // namespace
+
+extern "C" int gps_san2_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Y, int64_t ld,
+                                          const float* E, const float* E2, const double* gamma, int64_t nmax,
+                                          void* workspace, int64_t workspace_bytes, float* O, int64_t ldo, float* R,
+                                          float* F, float* lse, void* stream) {
+  uint32_t* bits;
+  float *D, *pq, *part;
+  GPS_TRY(san2_stage_setup(g, heads, hd, nmax, ld, gamma, workspace, workspace_bytes, &bits, &D, &pq, &part));
+  GPS_REQUIRE(Y && E2 && O && R && F && lse && (g->E == 0 || E), GPS_ERR_ARG, "san2 attention: null pointer");
+  GPS_REQUIRE(ldo >= heads * hd, GPS_ERR_ARG, "san2 attention: ldo too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  GPS_TRY(san_prep(*g, bits, nmax, nullptr, nullptr, nullptr, heads * hd, st));
+  const SanAttn a = san_attn(*g, heads, hd, Y, ld, E, E2, bits, nmax, 0.f);
+  San2Saved S;
+  S.R = R; S.F = F; S.lse = lse;
+  return san2_attn_fwd(a, gamma, O, O, ldo, Planes(), S, DropCfg(), st);
+}
+
+extern "C" int gps_san2_attention_backward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Y, int64_t ld,
+                                           const float* E, const float* E2, const double* gamma, int64_t nmax,
+                                           void* workspace, int64_t workspace_bytes, const float* R, const float* F,
+                                           const float* lse, const float* dO, int64_t ldo, float* dY, int64_t ldg,
+                                           float* dE, float* dE2, double* dgamma, void* stream) {
+  uint32_t* bits;
+  float *D, *pq, *part;
+  GPS_TRY(san2_stage_setup(g, heads, hd, nmax, ld, gamma, workspace, workspace_bytes, &bits, &D, &pq, &part));
+  GPS_REQUIRE(Y && E2 && R && F && lse && dO && dY && dE2 && dgamma && (g->E == 0 || (E && dE)), GPS_ERR_ARG,
+              "san2 attention: null pointer");
+  GPS_REQUIRE(ldo >= heads * hd && ldg >= 5 * heads * hd, GPS_ERR_ARG, "san2 attention: ldo / ldg too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t d = heads * hd;
+  GPS_TRY(san_prep(*g, bits, nmax, nullptr, nullptr, nullptr, d, st));
+  const SanAttn a = san_attn(*g, heads, hd, Y, ld, E, E2, bits, nmax, 0.f);
+  SanGrad G;
+  G.gQ = dY; G.gK = dY + d; G.gV = dY + 2 * d; G.gQ2 = dY + 3 * d; G.gK2 = dY + 4 * d;
+  G.ldg = ldg;
+  G.gE = dE;
+  return san2_attn_bwd(a, gamma, R, F, lse, dO, ldo, D, G, dgamma, pq, part, nullptr, nullptr, dE2, nullptr, nullptr, false, st);
 }

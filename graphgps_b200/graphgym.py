@@ -55,7 +55,7 @@ def install_graphormer_bias(module=None):
 
 def install_san(san_module=None):
     """Rebind ``SANLayer`` inside ``graphgps.network.san_transformer`` so ``SANTransformer`` builds the H100 layer.
-    ``SAN2Layer`` (learned gamma, softmax scores) stays the reference's.
+    ``SAN2Layer`` is left as it is (``install_san2`` rebinds it).
 
     Call after ``import graphgps`` and before ``create_model()``.  Returns the class it replaced so a caller can restore
     it."""
@@ -64,6 +64,20 @@ def install_san(san_module=None):
         san_module = importlib.import_module("graphgps.network.san_transformer")
     previous = getattr(san_module, "SANLayer", None)
     san_module.SANLayer = SANLayer
+    return previous
+
+
+def install_san2(san_module=None):
+    """Rebind ``SAN2Layer`` inside ``graphgps.network.san_transformer`` so ``SANTransformer`` with
+    ``cfg.gt.layer_type: SAN2Layer`` builds the H100 layer.  ``SANLayer`` is left as it is (``install_san`` rebinds it).
+
+    Call after ``import graphgps`` and before ``create_model()``.  Returns the class it replaced so a caller can restore
+    it."""
+    from .san import SAN2Layer
+    if san_module is None:
+        san_module = importlib.import_module("graphgps.network.san_transformer")
+    previous = getattr(san_module, "SAN2Layer", None)
+    san_module.SAN2Layer = SAN2Layer
     return previous
 
 

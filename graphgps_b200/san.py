@@ -14,6 +14,14 @@ d = out_dim, H = num_heads, hd = d / H:
 
 in one C call per direction (libgps_b200.so, sm_90a).  There is no CPU fallback.  The reference's side effects on the
 batch (Q_h, K_h, E, wV, Z, ...) are internals and are not reproduced; batch.edge_attr is left unchanged.
+
+`SAN2Layer` is the drop-in for `graphgps.layer.san2_layer.SAN2Layer`, SANTransformer's other layer: the same trunk and
+modules, plus `attention.gamma` (float64, learned, first in the state_dict as the reference creates it), with
+
+    attn = (softmax over the real in-edges . V + gamma softmax over the fake pairs . V) / (gamma + 1)
+
+(pyg_softmax per set and head, no clamp).  The library reads gamma on the device, so an optimiser step or a replayed
+CUDA graph uses its current value; the constructor's `gamma` argument is ignored, as in the reference.
 """
 from __future__ import annotations
 
@@ -31,10 +39,13 @@ _NODE = ("attention.Q.weight", "attention.K.weight", "attention.V.weight", "atte
 
 class _SANAttentionParams(nn.Module):
     """Parameter container with the names and construction order of MultiHeadAttentionLayer (san_layer.py:17-36) as
-    SANLayer builds it: Q, K, E, Q_2, K_2, E_2 (no biases), the shared fake_edge_emb, V."""
+    SANLayer builds it: Q, K, E, Q_2, K_2, E_2 (no biases), the shared fake_edge_emb, V.  With `learned_gamma`, that of
+    MultiHeadAttention2Layer (san2_layer.py:43-63): the float64 gamma = 0.5 first."""
 
-    def __init__(self, in_dim, out_dim, num_heads, fake_edge_emb):
+    def __init__(self, in_dim, out_dim, num_heads, fake_edge_emb, learned_gamma=False):
         super().__init__()
+        if learned_gamma:
+            self.gamma = nn.Parameter(torch.tensor(0.5, dtype=torch.float64), requires_grad=True)
         self.Q = nn.Linear(in_dim, out_dim * num_heads, bias=False)
         self.K = nn.Linear(in_dim, out_dim * num_heads, bias=False)
         self.E = nn.Linear(in_dim, out_dim * num_heads, bias=False)
@@ -48,6 +59,8 @@ class _SANAttentionParams(nn.Module):
 class SANLayer(nn.Module):
     """SAN GraphTransformerLayer (reference: graphgps/layer/san_layer.py:123-216)."""
 
+    _variant = 0   # GpsSanArgs.variant
+
     def __init__(self, gamma, in_dim, out_dim, num_heads, full_graph, fake_edge_emb, dropout=0.0, layer_norm=False,
                  batch_norm=True, residual=True, use_bias=False, precision="fp32"):
         super().__init__()
@@ -57,16 +70,16 @@ class SANLayer(nn.Module):
                           (not batch_norm, "batch_norm=False"), (not residual, "residual=False"),
                           (use_bias, "use_bias=True")):
             if off:
-                raise NotImplementedError(f"graphgps_b200.SANLayer: {what} is not built (no shipped SAN config uses "
-                                          "it)")
+                raise NotImplementedError(f"graphgps_b200.{type(self).__name__}: {what} is not built (no shipped SAN "
+                                          "config uses it)")
         if in_dim != out_dim:
-            raise NotImplementedError(f"graphgps_b200.SANLayer: in_dim != out_dim ({in_dim} != {out_dim}) is not built "
+            raise NotImplementedError(f"graphgps_b200.{type(self).__name__}: in_dim != out_dim ({in_dim} != {out_dim}) is not built "
                                       "(SANTransformer always passes dim_hidden for both)")
         if num_heads < 1 or out_dim % num_heads != 0:
             raise ValueError(f"out_dim {out_dim} must be divisible by num_heads {num_heads} (the reference fails at "
                              "its view of the concatenated heads)")
         if out_dim % 4 != 0 or out_dim // num_heads > 192:
-            raise NotImplementedError(f"graphgps_b200.SANLayer: needs out_dim % 4 == 0 and a head dim <= 192 (got "
+            raise NotImplementedError(f"graphgps_b200.{type(self).__name__}: needs out_dim % 4 == 0 and a head dim <= 192 (got "
                                       f"out_dim {out_dim}, {num_heads} heads)")
         if not isinstance(fake_edge_emb, nn.Embedding) or tuple(fake_edge_emb.weight.shape) != (1, out_dim):
             raise ValueError(f"fake_edge_emb must be an nn.Embedding(1, {out_dim})")
@@ -78,13 +91,15 @@ class SANLayer(nn.Module):
         self.layer_norm = layer_norm
         self.batch_norm = batch_norm
         # the reference's modules, in its order (same state_dict keys, same draws from the same seed)
-        self.attention = _SANAttentionParams(in_dim, out_dim // num_heads, num_heads, fake_edge_emb)
+        self.attention = _SANAttentionParams(in_dim, out_dim // num_heads, num_heads, fake_edge_emb,
+                                             learned_gamma=self._variant == 1)
         self.O_h = nn.Linear(out_dim, out_dim)
         self.batch_norm1_h = nn.BatchNorm1d(out_dim)
         self.FFN_h_layer1 = nn.Linear(out_dim, out_dim * 2)
         self.FFN_h_layer2 = nn.Linear(out_dim * 2, out_dim)
         self.batch_norm2_h = nn.BatchNorm1d(out_dim)
-        self.gamma = float(gamma)
+        if self._variant == 0:
+            self.gamma = float(gamma)
         self.p_dropout = float(dropout)
         self.precision = precision
         self._param_names = [n for n, _ in self.named_parameters()]
@@ -98,12 +113,19 @@ class SANLayer(nn.Module):
 
     def _args(self, gs, inputs, named, grads=None):
         g = grads or {}
-        check_params(self, named)
         a = _lib.GpsSanArgs()
+        if self._variant == 0:
+            check_params(self, named)
+            a.gamma = self.gamma
+        else:   # attention.gamma is float64, checked by forward
+            check_params(self, {n: t for n, t in named.items() if n != "attention.gamma"})
+            a.variant = 1
+            a.gamma_param = named["attention.gamma"].data_ptr()
+            a.grad_gamma = _lib.ptr(g.get("attention.gamma"))
         a.d, a.heads = self.out_channels, self.num_heads
         a.training = 1 if self.training else 0
         a.precision = _lib.PRECISION[self.precision]
-        a.gamma, a.dropout = self.gamma, self.p_dropout
+        a.dropout = self.p_dropout
 
         def lin(w, b=None):
             return linear(named[w], named[b] if b else None, g.get(w), g.get(b) if b else None)
@@ -152,6 +174,12 @@ class SANLayer(nn.Module):
         return (g_x, g_e), ()
 
     def forward(self, batch):
+        if self._variant == 1:
+            gamma = self.attention.gamma
+            if gamma.dtype != torch.float64 or gamma.numel() != 1 or gamma.device != batch.x.device:
+                raise TypeError(f"graphgps_b200.{type(self).__name__}: parameter 'attention.gamma' must be one float64 "
+                                f"value on the device of batch.x (got {gamma.dtype} of shape {tuple(gamma.shape)} on "
+                                f"{gamma.device})")
         x = read_x(batch, self, self.out_channels)
         e = read_edge_attr(batch, x, self, self.out_channels)
         gs = graph_of(batch)
@@ -163,3 +191,11 @@ class SANLayer(nn.Module):
         return "{}(in_channels={}, out_channels={}, heads={}, residual={}, backend=libgps_b200(sm_90a), " \
                "precision={})".format(self.__class__.__name__, self.in_channels, self.out_channels, self.num_heads,
                                       self.residual, self.precision)
+
+
+class SAN2Layer(SANLayer):
+    """SAN2Layer (reference: graphgps/layer/san2_layer.py:145-238): SANLayer's trunk around softmax attention over the
+    real edges and the fake pairs, mixed by the learned float64 `attention.gamma`.  `gamma` is accepted and ignored, as
+    the reference ignores it."""
+
+    _variant = 1

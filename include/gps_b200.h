@@ -509,16 +509,27 @@ int gps_graphormer_bias_backward(const GpsGraphormerBiasArgs* args, void* stream
  * grad_fake_edge_emb; the weight products run on a side stream that joins the caller's stream before the call
  * returns.  When Q..K2's grad_weight buffers are consecutive [5d, d] (K = Q + d*d, ...) they take one product.  No
  * float atomics: two runs give the same bits.
+ *
+ * variant 1 is SAN2Layer (graphgps/layer/san2_layer.py, the same trunk): the attention is a softmax (running max, no
+ * clamp) taken separately over the real in-edges and over the fake pairs of each destination, mixed by the learned
+ * float64 gamma = *gamma_param, read on the device by the kernels (an optimiser step or a CUDA-graph replay sees the
+ * current value):
+ *     real edge k: alpha = softmax over i's real in-edges of sum_c K[j] Q[i] E[k] / sqrt(hd)       (+1e-16 in the sum)
+ *     fake pair:   beta  = softmax over i's fake pairs of sum_c K2[j] Q2[i] E2 / sqrt(hd)           (+1e-16 in the sum)
+ *     attn[i] = (sum alpha V[j] + gamma sum beta V[j]) / (gamma + 1)      (an empty set contributes 0)
+ * The gamma field is not read; gamma_param is required (GPS_ERR_ARG); backward writes *grad_gamma (added with
+ * GPS_FLAG_GRADS_ACCUMULATE), reduced in float64 in a fixed order.  Any other variant is GPS_ERR_UNSUPPORTED.  All
+ * these checks happen before any CUDA call.
  * ---------------------------------------------------------------------------------------- */
 typedef struct {
   int64_t d;                 /* in_dim == out_dim                                              */
   int64_t heads;             /* num_heads                                                      */
   int32_t training;          /* 1: batch statistics and dropout; 0: running statistics         */
   int32_t precision;         /* GPS_PREC_*                                                     */
-  float gamma;               /* cfg.gt.gamma, a constant                                       */
+  float gamma;               /* cfg.gt.gamma, a constant (variant 0; not read by variant 1)    */
   float dropout;             /* sites 13 and 14                                                */
   int32_t flags;             /* GPS_FLAG_* (backward), as GpsLayerArgs.flags                   */
-  int32_t reserved;
+  int32_t variant;           /* 0: SANLayer; 1: SAN2Layer (softmax attention, learned gamma)   */
   uint64_t seed;             /* Philox key of this call's dropout masks                       */
   uint64_t offset;           /* Philox counter base                                            */
   const uint64_t* offset_dev;/* optional device-resident addend to offset (CUDA-graph replays); NULL = none */
@@ -536,6 +547,8 @@ typedef struct {
   GpsBatchNorm bn1, bn2;
   const float* fake_edge_emb;
   float* grad_fake_edge_emb;
+  const double* gamma_param; /* variant 1: attention.gamma, one float64 on the device, read by the kernels */
+  double* grad_gamma;        /* variant 1 (backward): its gradient, one float64 (NULL = not needed)       */
 } GpsSanArgs;
 
 typedef struct {
@@ -544,8 +557,8 @@ typedef struct {
   int64_t bwd_workspace_bytes;
 } GpsSanPlan;
 
-/* Sizes for the configuration and graph of args (only d, heads, precision, training, dropout, gamma, nmax and
- * graph.N / graph.E / graph.B are read). */
+/* Sizes for the configuration and graph of args (only d, heads, precision, training, dropout, gamma, variant, nmax
+ * and graph.N / graph.E / graph.B are read). */
 int gps_san_plan(const GpsSanArgs* args, GpsSanPlan* plan);
 int gps_san_forward(const GpsSanArgs* args, void* stream);
 int gps_san_backward(const GpsSanArgs* args, void* stream);
@@ -629,6 +642,21 @@ int gps_san_attention_backward(const GpsGraph* g, int64_t heads, int64_t hd, con
                                const float* E, const float* E2, float gamma, int64_t nmax, void* workspace,
                                int64_t workspace_bytes, const float* O, const float* dO, int64_t ldo, const float* rz,
                                float* dY, int64_t ldg, float* dE, float* dE2, void* stream);
+
+/* SAN2 attention stage (variant 1 of the layer), arguments as the SAN stage but with gamma one float64 on the device.
+ * Forward: O [N, ldo] = the attention output, R and F [N, heads * hd] = the unscaled real-edge and fake-pair softmax
+ * outputs (sum alpha V, sum beta V), lse [2, N, heads] = their log-sum-exps (real, then fake).  Backward from dO and
+ * the forward's R, F and lse: dY, dE, dE2 as the SAN stage, and *dgamma (float64), all written. */
+int64_t gps_san2_attention_workspace_bytes(int64_t N, int64_t d, int64_t heads, int64_t nmax);
+int gps_san2_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Y, int64_t ld,
+                               const float* E, const float* E2, const double* gamma, int64_t nmax, void* workspace,
+                               int64_t workspace_bytes, float* O, int64_t ldo, float* R, float* F, float* lse,
+                               void* stream);
+int gps_san2_attention_backward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Y, int64_t ld,
+                                const float* E, const float* E2, const double* gamma, int64_t nmax, void* workspace,
+                                int64_t workspace_bytes, const float* R, const float* F, const float* lse,
+                                const float* dO, int64_t ldo, float* dY, int64_t ldg, float* dE, float* dE2,
+                                double* dgamma, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Stage-level entry points (the same kernels the layer calls; exported so the parity tests can
