@@ -8,6 +8,8 @@ Public surface (mirrors the reference's module boundary, SURVEY.md section 8b):
     SAN2Layer     drop-in for graphgps.layer.san2_layer.SAN2Layer
     GatedGCNLayer, GINEConvLayer  drop-ins for CustomGNN's graphgps.layer.gatedgcn_layer.GatedGCNLayer and
                   graphgps.layer.gine_conv_layer.GINEConvLayer
+    InductiveEdgeHead  drop-in for graphgps.head.inductive_edge.GNNInductiveEdgeHead (PCQM-Contact's link head, dot
+                  decoding, ranking metrics on the device)
     GraphBatch    duck-typed stand-in for a collated PyG Batch (PyG is optional)
     make_batch    seeded synthetic batches of the BASELINE shapes
     GPSStack      the L-layer stack of a GPSModel (shared graph structure, plane hand-off, one gradient bucket, capture)
@@ -20,9 +22,10 @@ from .graphormer import GraphormerLayer  # noqa: F401
 from .graphormer_bias import BiasEncoder  # noqa: F401
 from .san import SAN2Layer, SANLayer  # noqa: F401
 from .custom_gnn import GatedGCNLayer, GINEConvLayer  # noqa: F401
+from .inductive_edge import InductiveEdgeHead  # noqa: F401
 from .dp import GradBucket  # noqa: F401
 from .stack import GPSStack  # noqa: F401
 from .loader import BatchPrefetcher, collate  # noqa: F401
 
-__all__ = ["GPSLayer", "GraphormerLayer", "BiasEncoder", "SANLayer", "SAN2Layer", "GatedGCNLayer", "GINEConvLayer", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
+__all__ = ["GPSLayer", "GraphormerLayer", "BiasEncoder", "SANLayer", "SAN2Layer", "GatedGCNLayer", "GINEConvLayer", "InductiveEdgeHead", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
            "batch_from_lists"]

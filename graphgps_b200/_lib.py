@@ -146,6 +146,21 @@ class GpsGraphormerBiasPlan(C.Structure):
     _fields_ = [("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
 
 
+class GpsLinkHeadArgs(C.Structure):
+    """Inductive link-prediction head (inductive_edge.py, dot decoding, layers_post_mp 1): config, the labeled-pair
+    graph, edge_index_labeled / edge_label, x, layer_post_mp.model.0.model, outputs, gradients and scratch."""
+    _fields_ = [("d", C.c_int64), ("training", C.c_int32), ("precision", C.c_int32), ("flags", C.c_int32),
+                ("label_bytes", C.c_int32), ("seed", C.c_uint64),
+                ("pairs", GpsGraph), ("edge_index_labeled", _fp), ("edge_label", _fp), ("x", _fp),
+                ("lin", GpsLinear), ("y", _fp), ("pred", _fp), ("stats", _fp),
+                ("grad_y", _fp), ("grad_pred", _fp), ("grad_x", _fp),
+                ("saved", _fp), ("saved_bytes", C.c_int64), ("workspace", _fp), ("workspace_bytes", C.c_int64)]
+
+
+class GpsLinkHeadPlan(C.Structure):
+    _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
+
+
 class GpsSanArgs(C.Structure):
     """SAN layer (san_layer.py, variant 0) or SAN2 layer (san2_layer.py, variant 1): config, dropout stream, graph and
     nmax, tensors, scratch, the ten Linears attention.{Q,K,V,Q_2,K_2,E,E_2}, O_h, FFN_h_layer1, FFN_h_layer2,
@@ -216,6 +231,10 @@ SYMBOLS = {
     "gps_graphormer_bias_plan": (C.c_int, [C.POINTER(GpsGraphormerBiasArgs), C.POINTER(GpsGraphormerBiasPlan)]),
     "gps_graphormer_bias_forward": (C.c_int, [C.POINTER(GpsGraphormerBiasArgs), _fp]),
     "gps_graphormer_bias_backward": (C.c_int, [C.POINTER(GpsGraphormerBiasArgs), _fp]),
+    "gps_link_head_plan": (C.c_int, [C.POINTER(GpsLinkHeadArgs), C.POINTER(GpsLinkHeadPlan)]),
+    "gps_link_head_forward": (C.c_int, [C.POINTER(GpsLinkHeadArgs), _fp]),
+    "gps_link_head_backward": (C.c_int, [C.POINTER(GpsLinkHeadArgs), _fp]),
+    "gps_link_rank_metrics": (C.c_int, [C.POINTER(GpsGraph), _fp, _i64, _i64, _fp, _i32, _fp, _fp, _i64, _fp]),
     "gps_san_plan": (C.c_int, [C.POINTER(GpsSanArgs), C.POINTER(GpsSanPlan)]),
     "gps_san_forward": (C.c_int, [C.POINTER(GpsSanArgs), _fp]),
     "gps_san_backward": (C.c_int, [C.POINTER(GpsSanArgs), _fp]),

@@ -31,15 +31,7 @@ namespace gps {
 
 namespace {
 
-// ------------------------------------------------------------------------------- pad / unpad
-// dst [rows_p, cols_p] (pitch ldd) = src [rows, cols] (pitch lds) with zeros beyond rows x cols, and / or the bf16 planes
-// of that block (p.hi set; then cols_p % 4 == 0).  Unpadding is the same copy with rows_p = rows and cols_p = cols.
-struct PadItem {
-  const float* src; int64_t lds; int rows, cols;
-  float* dst; int64_t ldd; int rows_p, cols_p;
-  Planes p;
-};
-constexpr int kPadItems = 24;
+// ------------------------------------------------------------------------------- pad / unpad (PadList: layer_ops.cuh)
 struct PadDesc {
   PadItem it[kPadItems];
   int start[kPadItems + 1];   // first block of each item in the 1-D grid
@@ -66,37 +58,6 @@ __global__ void k_pad(PadDesc d) {
   }
   if (it.p.hi) planes_store4(it.p, r, c, make_float4(v[0], v[1], v[2], v[3]));
 }
-
-struct PadList {
-  PadItem it[kPadItems];
-  int n = 0;
-  bool overflow = false;
-  void add(const float* src, int64_t lds, int64_t rows, int64_t cols, float* dst, int64_t ldd, int64_t rows_p,
-           int64_t cols_p, Planes p = Planes()) {
-    if (!src || rows_p <= 0 || cols_p <= 0 || (!dst && !p.hi)) return;
-    if (n == kPadItems) {
-      overflow = true;
-      return;
-    }
-    it[n++] = PadItem{src, lds, (int)rows, (int)cols, dst, ldd, (int)rows_p, (int)cols_p, p};
-  }
-  int run(cudaStream_t st) const {
-    GPS_REQUIRE(!overflow, GPS_ERR_ARG, "custom_gnn: more than %d pad items in one launch", kPadItems);
-    PadDesc d;
-    int total = 0;
-    for (int i = 0; i < n; ++i) {
-      d.it[i] = it[i];
-      d.start[i] = total;
-      total += (int)ceil_div((int64_t)it[i].rows_p * ((it[i].cols_p + 3) / 4), 256);
-    }
-    d.n = n;
-    d.start[n] = total;
-    if (total == 0) return GPS_OK;
-    k_pad<<<(unsigned)total, 256, 0, st>>>(d);
-    GPS_LAUNCH_CHECK();
-    return GPS_OK;
-  }
-};
 
 // GINE backward head: g2 = g_out * drop * [pre > 0] at pitch dp (+ planes), with g_out read at pitch ldg and its
 // columns >= d taken as zero; gpad != NULL: also the zero-padded copy of g_out (the residual's share of grad_x)
@@ -564,6 +525,23 @@ int cg_backward(const GpsCustomGnnArgs* a, cudaStream_t st) {
 }
 
 }  // namespace
+
+int PadList::run(cudaStream_t st) const {
+  GPS_REQUIRE(!overflow, GPS_ERR_ARG, "pad: more than %d pad items in one launch", kPadItems);
+  PadDesc d;
+  int total = 0;
+  for (int i = 0; i < n; ++i) {
+    d.it[i] = it[i];
+    d.start[i] = total;
+    total += (int)ceil_div((int64_t)it[i].rows_p * ((it[i].cols_p + 3) / 4), 256);
+  }
+  d.n = n;
+  d.start[n] = total;
+  if (total == 0) return GPS_OK;
+  k_pad<<<(unsigned)total, 256, 0, st>>>(d);
+  GPS_LAUNCH_CHECK();
+  return GPS_OK;
+}
 
 }  // namespace gps
 

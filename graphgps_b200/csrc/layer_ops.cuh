@@ -55,6 +55,32 @@ inline Planes arena_planes(Arena& A, int64_t rows, int64_t cols, bool lo) {
   return q;
 }
 
+// ------------------------------------------------------------------------------- pad / unpad
+// dst [rows_p, cols_p] (pitch ldd) = src [rows, cols] (pitch lds) with zeros beyond rows x cols, and / or the bf16 planes
+// of that block (p.hi set; then cols_p % 4 == 0).  Unpadding is the same copy with rows_p = rows and cols_p = cols.
+// Up to kPadItems blocks per launch (run: custom_gnn.cu).
+struct PadItem {
+  const float* src; int64_t lds; int rows, cols;
+  float* dst; int64_t ldd; int rows_p, cols_p;
+  Planes p;
+};
+constexpr int kPadItems = 24;
+struct PadList {
+  PadItem it[kPadItems];
+  int n = 0;
+  bool overflow = false;
+  void add(const float* src, int64_t lds, int64_t rows, int64_t cols, float* dst, int64_t ldd, int64_t rows_p,
+           int64_t cols_p, Planes p = Planes()) {
+    if (!src || rows_p <= 0 || cols_p <= 0 || (!dst && !p.hi)) return;
+    if (n == kPadItems) {
+      overflow = true;
+      return;
+    }
+    it[n++] = PadItem{src, lds, (int)rows, (int)cols, dst, ldd, (int)rows_p, (int)cols_p, p};
+  }
+  int run(cudaStream_t st) const;
+};
+
 // One dropout site of a call; p = 0 in eval mode
 inline DropCfg drop_cfg(float p, bool train, uint64_t seed, uint64_t offset, const uint64_t* offset_dev, int site) {
   DropCfg c;

@@ -96,6 +96,31 @@ def install_custom_gnn(module=None):
     return previous
 
 
+def install_inductive_edge_head(register_module=None):
+    """Set ``register.head_dict['inductive_edge']`` to the H100 head, so GPSModel, CustomGNN and SANTransformer build it
+    for ``gnn.head: inductive_edge``: each looks its head up in that registry at construction time.  The registered class
+    has the reference's ``(dim_in, dim_out)`` constructor and reads ``cfg.model.edge_decoding`` and
+    ``cfg.gnn.layers_post_mp`` when it is built.
+
+    Call after ``import graphgps`` and before ``create_model()``.  Returns the class it replaced so a caller can restore
+    it."""
+    from .inductive_edge import InductiveEdgeHead
+    if register_module is None:
+        register_module = importlib.import_module("torch_geometric.graphgym.register")
+
+    class InductiveEdgeHeadGraphGym(InductiveEdgeHead):
+        """GNNInductiveEdgeHead(dim_in, dim_out) with its decoding and depth from GraphGym's cfg."""
+
+        def __init__(self, dim_in, dim_out):
+            cfg = importlib.import_module("torch_geometric.graphgym.config").cfg
+            super().__init__(dim_in, dim_out, edge_decoding=cfg.model.edge_decoding,
+                             layers_post_mp=cfg.gnn.layers_post_mp)
+
+    previous = register_module.head_dict.get("inductive_edge")
+    register_module.head_dict["inductive_edge"] = InductiveEdgeHeadGraphGym
+    return previous
+
+
 def register(name="gpslayer_b200"):
     """Register a LayerConfig-style wrapper under ``name`` in GraphGym's layer registry.
 

@@ -490,6 +490,58 @@ int gps_graphormer_bias_forward(const GpsGraphormerBiasArgs* args, void* stream)
 int gps_graphormer_bias_backward(const GpsGraphormerBiasArgs* args, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Inductive link-prediction head (graphgps/head/inductive_edge.py, GNNInductiveEdgeHead) with edge_decoding "dot" and
+ * layers_post_mp 1, the head of every PCQM-Contact config:
+ *   y = x W^T + b                          (layer_post_mp.model.0.model, [d, d] and [d]; replaces batch.x)
+ *   pred[k] = <y[s_k], y[t_k]>             (s_k, t_k) = column k of edge_index_labeled [2, K]
+ * `pairs` is gps_graph_build(edge_index_labeled, batch, N, K, B): CSR by target, CSC by source, graph_ptr.
+ * Eval (training == 0) also writes stats [4] float64 = hits@1, hits@3, hits@10, mrr averaged over the B graphs: for a
+ * positive pair (i, j) (edge_label == 1) of graph g, rank = 1 + #{k in g, k != j : <y_i, y_k> > <y_i, y_j>} (the rank a
+ * stable descending sort gives: ties count in the positive's favour); a graph's values are the means over its positives
+ * of rank <= 1, <= 3, <= 10 and 1 / rank, and 0 when it has none.  A positive whose target lies outside its source's
+ * graph is not counted (the Python module rejects such batches in eval).
+ * Backward: dy = grad_y + sum_k g_k (y[t_k] e_{s_k} + y[s_k] e_{t_k}) as two segmented sums in pair order, then
+ * dW = dy^T x, db = sum dy (deterministic split-K) and grad_x = dy W: no float atomics in fp32, two runs give the same
+ * bits.  Indices out of [0, N) are never dereferenced.  d <= 4096.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  int64_t d;                 /* dim_in                                                        */
+  int32_t training;          /* 1: training (no stats), 0: eval (stats)                       */
+  int32_t precision;         /* GPS_PREC_*                                                    */
+  int32_t flags;             /* reserved, 0                                                   */
+  int32_t label_bytes;       /* 4 or 8: edge_label is int32 or int64                          */
+  uint64_t seed;             /* unused (the head has no dropout)                              */
+  GpsGraph pairs;            /* N = nodes, E = K labeled pairs, B = graphs                    */
+  const int64_t* edge_index_labeled; /* [2, K]                                                */
+  const void* edge_label;    /* [K] (eval)                                                    */
+  const float* x;            /* [N, d]                                                        */
+  GpsLinear lin;             /* layer_post_mp.model.0.model: weight [d, d], bias [d], grads   */
+  float* y;                  /* [N, d] (forward)                                              */
+  float* pred;               /* [K] (forward)                                                 */
+  double* stats;             /* [4] (eval forward)                                            */
+  const float* grad_y;       /* [N, d] or NULL (backward)                                     */
+  const float* grad_pred;    /* [K] or NULL (backward)                                        */
+  float* grad_x;             /* [N, d] (backward)                                             */
+  void* saved; int64_t saved_bytes;         /* forward -> backward                            */
+  void* workspace; int64_t workspace_bytes; /* transient                                      */
+} GpsLinkHeadArgs;
+
+typedef struct {
+  int64_t saved_bytes;
+  int64_t fwd_workspace_bytes;
+  int64_t bwd_workspace_bytes;
+} GpsLinkHeadPlan;
+
+/* Sizes for args (only d, precision, training and the pair graph's N, E and B are read). */
+int gps_link_head_plan(const GpsLinkHeadArgs* args, GpsLinkHeadPlan* plan);
+int gps_link_head_forward(const GpsLinkHeadArgs* args, void* stream);
+int gps_link_head_backward(const GpsLinkHeadArgs* args, void* stream);
+/* Stage entry: the eval statistics above for node rows y [N, d] at pitch ld >= d, into stats [4]; workspace >= 32 * B
+ * bytes (per-graph values). */
+int gps_link_rank_metrics(const GpsGraph* pairs, const float* y, int64_t ld, int64_t d, const void* edge_label,
+                          int32_t label_bytes, double* stats, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * SAN layer (graphgps/layer/san_layer.py:10-210), the building block of SANTransformer, as every shipped config runs
  * it (full_graph, batch_norm, residual, no layer_norm, no Linear biases in the attention, in_dim == out_dim == d):
  *   [Q|K|V|Q2|K2] = x W^T, E = edge_attr W_E^T, E2 = W_E2 fake_edge_emb
