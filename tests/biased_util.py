@@ -5,7 +5,7 @@ import os
 import numpy as np
 import torch
 
-from util import GOLDEN_DIR, compare, golden_batch, rel_err, rel_l2, run_layer
+from util import GOLDEN_DIR, compare, golden_batch, run_layer
 
 BIASED_DIR = os.path.join(GOLDEN_DIR, "biased")
 LIVE_NAME = "reference_live_GINE_BiasedTransformer"
@@ -81,14 +81,5 @@ def run_biased(layer, batch, fix, backward=True):
     return res
 
 
-def compare_biased(res, fix, tol, what="", grad_l2_tol=None):
-    """util.compare, and grad_attn_bias under the same gradient criterion (max-abs, or relative L2 when given)."""
-    errs = compare(res, fix, tol, what, grad_l2_tol)
-    if "grad_attn_bias" in fix:
-        e = rel_err(res["grad_attn_bias"], fix["grad_attn_bias"])
-        errs["grad_attn_bias"] = e
-        if e > tol:
-            l2 = rel_l2(res["grad_attn_bias"], fix["grad_attn_bias"])
-            errs["grad_attn_bias(l2)"] = l2
-            assert grad_l2_tol is not None and l2 <= grad_l2_tol, f"{what} grad_attn_bias: max-abs {e}, L2 {l2}"
-    return errs
+# util.compare checks grad_attn_bias itself whenever the fixture has it
+compare_biased = compare

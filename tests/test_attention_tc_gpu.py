@@ -9,14 +9,10 @@ import torch
 from graphgps_b200 import _lib
 from graphgps_b200.batch import batch_from_lists, make_batch
 from graphgps_b200.graph import graph_of
-from util import rel_err
+from util import _stream, rel_err
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def _padded_planes(QKV, H, hd, lo=True):

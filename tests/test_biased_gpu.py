@@ -16,20 +16,12 @@ from graphgps_b200.batch import batch_from_lists, make_batch
 from graphgps_b200.graph import graph_of
 from biased_oracle import OracleGPSLayerBiased
 from biased_util import PAD_VALUE, biased_batch, biased_names, compare_biased, load_biased, make_bias, run_biased
-from util import pin_dropout_counter, rel_err, rel_l2
+from util import _nan, _stream, pin_dropout_counter, rel_err, rel_l2
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 TOL = {"fp32": 1e-3, "bf16": 1e-2}
 GRAD_L2 = {"fp32": 5e-3, "bf16": 1e-1}   # the criterion of tests/test_layer_gpu.py (util.compare)
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _nan(*shape):
-    return torch.full(shape, float("nan"), device=DEV)
 
 
 def _ref(QKV, bias, ptr, H, hd):

@@ -18,7 +18,7 @@ import graphgps_b200
 from graphgps_b200 import _lib, bigbird as bbmod
 from graphgps_b200.graph import graph_of
 from bigbird_oracle import attach_bigbird, bb_batch, bigbird_cfg, bigbird_oracle_layer, multiplicity
-from util import GOLDEN_DIR, compare, golden_batch, pin_dropout_counter, rel_err, run_layer
+from util import _stream, compare, golden_batch, GOLDEN_DIR, pin_dropout_counter, rel_err, run_layer
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -27,10 +27,6 @@ GRAD_L2 = {"fp32": 5e-3, "bf16": 1e-1}
 BB_DIR = os.path.join(GOLDEN_DIR, "bigbird")
 FIXTURES = sorted(os.path.basename(p)[:-3] for p in _glob.glob(os.path.join(BB_DIR, "*.pt"))
                   if not p.endswith("tables.pt"))
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def _load(name):

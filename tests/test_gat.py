@@ -9,6 +9,7 @@ import torch
 import graphgps_b200
 from graphgps_b200 import _lib
 from gat_oracle import GATConvDense, GATConvMP, gat_batch, gat_oracle_layer
+from local_model_harness import _args, _plan
 from util import GOLDEN_DIR, golden_batch
 
 GAT_DIR = os.path.join(GOLDEN_DIR, "gat")
@@ -122,21 +123,6 @@ def test_bucket_groups():
     for n in ("local_model.att_src", "local_model.att_dst", "local_model.att_edge", "local_model.bias",
               "local_model.lin_edge.weight"):
         assert _group(n) == MID, n
-
-
-def _args(local, N=10, E=20, d=64, H=4, glob="Transformer"):
-    a = _lib.GpsLayerArgs()
-    a.d, a.heads = d, H
-    a.local_type = _lib.LOCAL[local]
-    a.global_type = _lib.GLOBAL[glob]
-    a.graph.N, a.graph.E, a.graph.B = N, E, 2
-    return a
-
-
-def _plan(a):
-    p = _lib.GpsLayerPlan()
-    rc = _lib.load().gps_layer_plan(C.byref(a), C.byref(p))
-    return rc, p
 
 
 def test_plan_sizes():

@@ -16,15 +16,11 @@ from graphgps_b200.graph import graph_of
 from oracle.gps_oracle import OracleGPSLayer
 from eslappe_oracle import OracleGPSLayerESLapPE
 from eslappe_util import calibrate_gate, compare_eslap, make_pe, run_eslap
-from util import compare, pin_dropout_counter, run_layer
+from util import _stream, compare, pin_dropout_counter, run_layer
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 SHAPE = "pcqm4m-small"
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def _batch(seed=7, pe=False):

@@ -6,14 +6,10 @@ import pytest
 import torch
 
 from graphgps_b200 import _lib
-from util import rel_err
+from util import _stream, rel_err
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def _planes(x, lo=True, pad=0):

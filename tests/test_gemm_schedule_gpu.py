@@ -8,14 +8,10 @@ import torch
 import graphgps_b200
 from graphgps_b200 import _call, _lib
 from graphgps_b200.graph import graph_of
-from util import rel_err
+from util import _stream, rel_err
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def _planes(x, lo=True):

@@ -13,7 +13,8 @@ from graphgps_b200 import _lib
 from graphgps_b200.batch import batch_from_lists, make_batch
 from graphgps_b200.graph import GraphStructure, graph_of
 from oracle.gps_oracle import OracleGPSLayer
-from util import compare, golden_batch, golden_names, load_golden, pin_dropout_counter, rel_err, rel_l2, run_layer
+from util import (_stream, compare, golden_batch, golden_names, load_golden, pin_dropout_counter, rel_err, rel_l2,
+                  run_layer)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -28,10 +29,6 @@ TOL = {"fp32": 1e-3, "bf16": 1e-2}
 # util.compare reports raw max-abs errors beside the scaled ones.
 GRAD_L2 = {"fp32": 5e-3, "bf16": 1e-1}
 GRAD_L2_FULL = {"fp32": 5e-3, "bf16": 8e-2}   # BASELINE-size batches (thousands of rows per BatchNorm column)
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 # ------------------------------------------------------------------------------- graph structure

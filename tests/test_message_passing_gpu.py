@@ -24,7 +24,7 @@ from oracle.gps_oracle import OracleGPSLayer
 from eslappe_oracle import OracleGPSLayerESLapPE
 from eslappe_util import calibrate_gate, compare_eslap, make_pe, run_eslap
 from nonorm_util import node_graph
-from util import compare, rel_err, run_layer
+from util import _nan, _stream, compare, rel_err, run_layer
 import mp_reference as R
 
 pytestmark = pytest.mark.gpu
@@ -34,10 +34,6 @@ U = 2.0 ** -24          # unit roundoff of fp32 (round to nearest)
 EDGE_TOL = 1e-5         # per-edge outputs, scaled by max(1, max|ref|)
 NUM_SMS = 132
 WORST = {}              # stage -> worst error / bound seen
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def gamma(m):
@@ -153,10 +149,6 @@ def _graph(fam, d):
 
 def _ids(c):
     return f"{c[0]}-d{c[1]}"
-
-
-def _nan(*shape, dtype=torch.float32):
-    return torch.full(shape, float("nan"), device=DEV, dtype=dtype)
 
 
 def _rand(gen, *shape, scale=1.0):

@@ -25,6 +25,7 @@ from graphgps_b200.batch import make_batch
 from graphgps_b200.graph import GraphStructure
 from oracle.gps_oracle import gaussian_orthogonal_random_matrix
 import performer_reference as R
+from util import _nan, _stream
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -54,14 +55,6 @@ def _report():
     yield
     for k in sorted(WORST):
         print(f"worst error / bound  {k:36s} {WORST[k]:.3e}")
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _nan(*shape, dtype=torch.float32):
-    return torch.full(shape, float("nan"), device=DEV, dtype=dtype)
 
 
 def _sizes(shape, seed=2):

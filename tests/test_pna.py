@@ -8,6 +8,7 @@ import torch
 import graphgps_b200
 from graphgps_b200 import _lib
 from pna_oracle import PNAConvLoop, PNAConvMP, pna_batch, pna_conv, pna_oracle_layer, tie_edge
+from local_model_harness import _args, _planes, _plan, _r
 from util import GOLDEN_DIR, golden_batch
 
 PNA_DIR = os.path.join(GOLDEN_DIR, "pna")
@@ -198,32 +199,6 @@ def test_dp_groups():
     for n in _pna_keys(8):
         want = LATE if n.startswith(("local_model.pre_nns.", "local_model.lin.")) else MID
         assert _group(n) == want, n
-
-
-def _args(local, N=10, E=20, d=64, H=4, glob="Transformer", norm="batch"):
-    a = _lib.GpsLayerArgs()
-    a.d, a.heads = d, H
-    a.local_type = _lib.LOCAL[local]
-    a.global_type = _lib.GLOBAL[glob]
-    a.norm_type = _lib.NORM[norm]
-    a.graph.N, a.graph.E, a.graph.B = N, E, 2
-    return a
-
-
-def _plan(a):
-    p = _lib.GpsLayerPlan()
-    rc = _lib.load().gps_layer_plan(C.byref(a), C.byref(p))
-    return rc, p
-
-
-def _r(n):
-    return (n + 255) // 256 * 256
-
-
-def _planes(rows, cols, lo=True):
-    """bytes of one bf16 hi (+ lo) plane pair as the library allocates it"""
-    one = _r(2 * (rows * ((cols + 7) // 8 * 8) + 8))
-    return one * (2 if lo else 1)
 
 
 @pytest.mark.parametrize("N,E,d,glob,norm,prec", [(10, 20, 64, "Transformer", "batch", "fp32"),

@@ -1,6 +1,6 @@
 """SAN layer, CPU side: the float64 restatement against the reference run verbatim, the fake-pair complement, the
 parameter container against the reference's, the constructor contract, the C ABI's plan and argument checks, and
-install_san."""
+install_san.  The checks SAN2Layer runs as well are in tests/san_harness.py."""
 import ctypes as C
 import os
 import types
@@ -11,44 +11,16 @@ import torch.nn as nn
 
 import graphgps_b200
 from graphgps_b200 import _lib, graphgym
-from san_oracle import fake_pairs, san_batch, san_forward
-from util import GOLDEN_DIR
+from san_harness import (NOT_BUILT, VARIANTS, _args, _check_oracle, _load, check_constructor_not_built,
+                         check_shared_embedding)
+from san_oracle import fake_pairs, san_batch
 
-SAN_DIR = os.path.join(GOLDEN_DIR, "san")
+SAN_DIR = VARIANTS["SAN"].dir
 HAVE_REFERENCE = os.path.isfile("/root/reference/graphgps/layer/san_layer.py")
 
 
-def _load(name):
-    return torch.load(os.path.join(SAN_DIR, name + ".pt"), weights_only=False)
-
-
-def _oracle(fix, state, x, e, masks=None):
-    cfg = fix["config"]
-    fake = fake_pairs(fix["edge_index"], fix["batch"], fix["num_graphs"])
-    prefixes = [""] if cfg["layers"] == 1 else [f"{i}." for i in range(cfg["layers"])]
-    h = x
-    for p in prefixes:
-        if p:   # one embedding shared by the layers (state_dict lists it under each; its gradient is layer 0's entry)
-            state[p + "attention.fake_edge_emb.weight"] = state["0.attention.fake_edge_emb.weight"]
-        h = san_forward(state, h, e, fix["edge_index"], fake, cfg["heads"], cfg["gamma"], cfg["training"], masks, p)
-    return h
-
-
-def _check_oracle(fix, tol_out, tol_grad):
-    state = {k: (v.double().requires_grad_(True) if v.is_floating_point() else v) for k, v in fix["state"].items()}
-    x = fix["x"].double().clone().requires_grad_(True)
-    e = fix["edge_attr"].double().clone().requires_grad_(True)
-    out = _oracle(fix, state, x, e)
-    assert float((out.detach() - fix["out"].double()).abs().max()) < tol_out
-    (out * fix["ct"].double()).sum().backward()
-    assert float((x.grad - fix["grad_x"].double()).abs().max()) < tol_grad
-    assert float((e.grad - fix["grad_edge_attr"].double()).abs().max()) < tol_grad
-    for n, g in fix["grad_params"].items():
-        assert float((state[n].grad - g.double()).abs().max()) < tol_grad, n
-
-
 def test_oracle_equals_reference_live():
-    _check_oracle(_load("reference_live"), 1e-10, 1e-9)
+    _check_oracle("SAN", _load("SAN", "reference_live"), 1e-10, 1e-9)
 
 
 @pytest.mark.skipif(not HAVE_REFERENCE, reason="the reference tree is not present; reference_live pins the oracle")
@@ -59,7 +31,7 @@ def test_oracle_equals_reference_run_now():
     san, _ = load_san()
     for case in CASES:
         if case[0] in ("edge_cases_hd6", "two_layer_shared_hd6", "molhiv_hd16_eval", "saturate_hd8"):
-            _check_oracle(run_case(san, *case, dtype=torch.float64), 1e-10, 1e-9)
+            _check_oracle("SAN", run_case(san, *case, dtype=torch.float64), 1e-10, 1e-9)
 
 
 def _complement(edge_index, batch, num_graphs):
@@ -73,7 +45,8 @@ def _complement(edge_index, batch, num_graphs):
 
 
 def test_fake_set_is_the_complement():
-    fix = _load("reference_live")     # self loops, a duplicate, a one-way edge, an isolated node, a one-node graph
+    # self loops, a duplicate, a one-way edge, an isolated node, a one-node graph
+    fix = _load("SAN", "reference_live")
     want = _complement(fix["edge_index"], fix["batch"], fix["num_graphs"])
     ref = {tuple(p) for p in fix["fake_pairs"].t().tolist()}   # negate_edge_index under torch_scatter's scatter_mul
     assert ref == want
@@ -87,7 +60,7 @@ def test_fake_set_is_the_complement():
 
 
 def test_state_dict_matches_reference():
-    fix = _load("reference_live")
+    fix = _load("SAN", "reference_live")
     torch.manual_seed(fix["init_seed"])
     emb = nn.Embedding(1, 56)
     layer = graphgps_b200.SANLayer(0.1, 56, 56, 8, True, emb, 0.2)
@@ -102,7 +75,7 @@ def test_state_dict_matches_reference():
 
 def test_fixture_states_load_strictly():
     for p in sorted(os.listdir(SAN_DIR)):
-        fix = _load(p[:-3])
+        fix = _load("SAN", p[:-3])
         cfg = fix["config"]
         emb = nn.Embedding(1, cfg["d"])
         layers = [graphgps_b200.SANLayer(cfg["gamma"], cfg["d"], cfg["d"], cfg["heads"], True, emb)
@@ -112,21 +85,12 @@ def test_fixture_states_load_strictly():
 
 
 def test_shared_embedding():
-    emb = nn.Embedding(1, 24)
-    a = graphgps_b200.SANLayer(0.1, 24, 24, 4, True, emb)
-    b = graphgps_b200.SANLayer(0.1, 24, 24, 4, True, emb)
-    assert a.attention.fake_edge_emb is emb and b.attention.fake_edge_emb is emb
-    assert "attention.fake_edge_emb.weight" in a.state_dict()
-    assert sum(1 for p in nn.Sequential(a, b).parameters() if p is emb.weight) == 1
+    check_shared_embedding("SAN")
 
 
-@pytest.mark.parametrize("kw", [dict(full_graph=False), dict(layer_norm=True), dict(batch_norm=False),
-                                dict(residual=False), dict(use_bias=True)])
+@pytest.mark.parametrize("kw", NOT_BUILT)
 def test_constructor_not_built(kw):
-    args = dict(gamma=0.1, in_dim=48, out_dim=48, num_heads=8, full_graph=True, fake_edge_emb=nn.Embedding(1, 48))
-    args.update(kw)
-    with pytest.raises(NotImplementedError):
-        graphgps_b200.SANLayer(**args)
+    check_constructor_not_built("SAN", kw)
 
 
 def test_constructor_contract():
@@ -151,27 +115,18 @@ def test_forward_refuses_cpu_tensors_and_missing_edge_attr():
         layer(b)
 
 
-def _args(d=56, heads=8, N=133, E=300, B=6, nmax=30):
-    a = _lib.GpsSanArgs()
-    a.d, a.heads = d, heads
-    a.graph.N, a.graph.E, a.graph.B = N, E, B
-    a.nmax = nmax
-    a.training = 1
-    return a
-
-
 def test_abi_plan():
     lib = _lib.load()
     plan = _lib.GpsSanPlan()
-    assert lib.gps_san_plan(C.byref(_args()), C.byref(plan)) == _lib.GPS_OK
+    assert lib.gps_san_plan(C.byref(_args("SAN")), C.byref(plan)) == _lib.GPS_OK
     N, E, d = 133, 300, 56
     # saved holds at least Y (5d), E, attn, z1, h1, hid (2d), z2 in fp32
     assert plan.saved_bytes >= 4 * (N * d * 11 + E * d)
     assert plan.bwd_workspace_bytes >= 4 * (N * d * 12 + E * d)
     big = _lib.GpsSanPlan()
-    assert lib.gps_san_plan(C.byref(_args(nmax=133)), C.byref(big)) == _lib.GPS_OK
+    assert lib.gps_san_plan(C.byref(_args("SAN", nmax=133)), C.byref(big)) == _lib.GPS_OK
     assert big.saved_bytes >= plan.saved_bytes       # the bitmap grows with nmax
-    drop = _args()
+    drop = _args("SAN")
     drop.dropout = 0.2
     dp = _lib.GpsSanPlan()
     assert lib.gps_san_plan(C.byref(drop), C.byref(dp)) == _lib.GPS_OK
@@ -183,9 +138,9 @@ def test_abi_plan():
 def test_abi_plan_rejects(d, heads, rc):
     lib = _lib.load()
     plan = _lib.GpsSanPlan()
-    assert lib.gps_san_plan(C.byref(_args(d, heads)), C.byref(plan)) == rc
+    assert lib.gps_san_plan(C.byref(_args("SAN", d, heads)), C.byref(plan)) == rc
     assert lib.gps_san_plan(None, C.byref(plan)) == _lib.GPS_ERR_ARG
-    bad = _args()
+    bad = _args("SAN")
     bad.nmax = 0
     assert lib.gps_san_plan(C.byref(bad), C.byref(plan)) == _lib.GPS_ERR_ARG
 
@@ -195,7 +150,7 @@ def test_abi_rejects_before_any_cuda_call():
     lib = _lib.load()
     assert lib.gps_san_forward(None, None) == _lib.GPS_ERR_ARG
     assert lib.gps_san_backward(None, None) == _lib.GPS_ERR_ARG
-    a = _args()
+    a = _args("SAN")
     fake = 1 << 40
     a.x, a.edge_attr, a.x_out, a.saved, a.workspace = fake, fake, fake, fake, fake
     a.saved_bytes = a.workspace_bytes = 1 << 40

@@ -1,5 +1,6 @@
 """SAN2 layer, CPU side: the float64 restatement against the reference run verbatim, the parameter container against
-the reference's, the constructor contract, the C ABI's plan and argument checks for variant 1, and install_san2."""
+the reference's, the constructor contract, the C ABI's plan and argument checks for variant 1, and install_san2.  The
+checks SANLayer runs as well are in tests/san_harness.py."""
 import ctypes as C
 import os
 import types
@@ -10,45 +11,16 @@ import torch.nn as nn
 
 import graphgps_b200
 from graphgps_b200 import _lib, graphgym
-from san2_oracle import san2_forward
+from san_harness import (NOT_BUILT, VARIANTS, _args, _check_oracle, _load, check_constructor_not_built,
+                         check_shared_embedding)
 from san_oracle import fake_pairs
-from util import GOLDEN_DIR
 
-SAN2_DIR = os.path.join(GOLDEN_DIR, "san2")
+SAN2_DIR = VARIANTS["SAN2"].dir
 HAVE_REFERENCE = os.path.isfile("/root/reference/graphgps/layer/san2_layer.py")
 
 
-def _load(name):
-    return torch.load(os.path.join(SAN2_DIR, name + ".pt"), weights_only=False)
-
-
-def _oracle(fix, state, x, e):
-    cfg = fix["config"]
-    fake = fake_pairs(fix["edge_index"], fix["batch"], fix["num_graphs"])
-    prefixes = [""] if cfg["layers"] == 1 else [f"{i}." for i in range(cfg["layers"])]
-    h = x
-    for p in prefixes:
-        if p:   # one embedding shared by the layers (state_dict lists it under each; its gradient is layer 0's entry)
-            state[p + "attention.fake_edge_emb.weight"] = state["0.attention.fake_edge_emb.weight"]
-        h = san2_forward(state, h, e, fix["edge_index"], fake, cfg["heads"], cfg["training"], None, p)
-    return h
-
-
-def _check_oracle(fix, tol_out, tol_grad):
-    state = {k: (v.double().requires_grad_(True) if v.is_floating_point() else v) for k, v in fix["state"].items()}
-    x = fix["x"].double().clone().requires_grad_(True)
-    e = fix["edge_attr"].double().clone().requires_grad_(True)
-    out = _oracle(fix, state, x, e)
-    assert float((out.detach() - fix["out"].double()).abs().max()) < tol_out
-    (out * fix["ct"].double()).sum().backward()
-    assert float((x.grad - fix["grad_x"].double()).abs().max()) < tol_grad
-    assert float((e.grad - fix["grad_edge_attr"].double()).abs().max()) < tol_grad
-    for n, g in fix["grad_params"].items():
-        assert float((state[n].grad - g.double()).abs().max()) < tol_grad, n
-
-
 def test_oracle_equals_reference_live():
-    _check_oracle(_load("reference_live"), 1e-10, 1e-9)
+    _check_oracle("SAN2", _load("SAN2", "reference_live"), 1e-10, 1e-9)
 
 
 @pytest.mark.skipif(not HAVE_REFERENCE, reason="the reference tree is not present; reference_live pins the oracle")
@@ -59,19 +31,19 @@ def test_oracle_equals_reference_run_now():
     san2, _ = load_san2()
     for case in CASES:
         if case[0] in ("edge_cases_hd6", "two_layer_shared_hd6", "molhiv_hd16_eval", "no_clamp_hd8", "gamma_zero_hd7"):
-            _check_oracle(run_case(san2, *case, dtype=torch.float64), 1e-10, 1e-9)
+            _check_oracle("SAN2", run_case(san2, *case, dtype=torch.float64), 1e-10, 1e-9)
 
 
 def test_fixtures_cover_the_cases():
-    live = _load("reference_live")
+    live = _load("SAN2", "reference_live")
     assert live["state"]["0.attention.gamma"].dtype == torch.float64
     assert live["grad_params"]["0.attention.gamma"].dtype == torch.float64
-    clamp = _load("no_clamp_hd8")
+    clamp = _load("SAN2", "no_clamp_hd8")
     assert clamp["max_score"] > 88          # exp would overflow in fp32 without the running max
-    zero = _load("gamma_zero_hd7")
+    zero = _load("SAN2", "gamma_zero_hd7")
     assert float(zero["state"]["attention.gamma"]) == 0.0
     assert abs(float(zero["grad_params"]["attention.gamma"])) > 1e-6   # the fake part has weight 0, its gradient not
-    edge = _load("edge_cases_hd6")
+    edge = _load("SAN2", "edge_cases_hd6")
     fake = fake_pairs(edge["edge_index"], edge["batch"], edge["num_graphs"])
     ei = edge["edge_index"]
     assert not bool((fake[1] >= 11).any() & (fake[1] <= 13).any())   # the complete graph has no fake pair
@@ -80,7 +52,7 @@ def test_fixtures_cover_the_cases():
 
 
 def test_state_dict_matches_reference():
-    fix = _load("reference_live")
+    fix = _load("SAN2", "reference_live")
     torch.manual_seed(fix["init_seed"])
     emb = nn.Embedding(1, 56)
     layer = graphgps_b200.SAN2Layer(0.1, 56, 56, 8, True, emb, 0.2)
@@ -98,7 +70,7 @@ def test_state_dict_matches_reference():
 
 def test_fixture_states_load_strictly():
     for p in sorted(os.listdir(SAN2_DIR)):
-        fix = _load(p[:-3])
+        fix = _load("SAN2", p[:-3])
         cfg = fix["config"]
         emb = nn.Embedding(1, cfg["d"])
         layers = [graphgps_b200.SAN2Layer(0.1, cfg["d"], cfg["d"], cfg["heads"], True, emb)
@@ -121,21 +93,15 @@ def test_gamma_argument_is_ignored():
 
 
 def test_shared_embedding():
-    emb = nn.Embedding(1, 24)
-    a = graphgps_b200.SAN2Layer(0.1, 24, 24, 4, True, emb)
-    b = graphgps_b200.SAN2Layer(0.1, 24, 24, 4, True, emb)
-    assert a.attention.fake_edge_emb is emb and b.attention.fake_edge_emb is emb
-    assert sum(1 for p in nn.Sequential(a, b).parameters() if p is emb.weight) == 1
+    check_shared_embedding("SAN2")
+    a = graphgps_b200.SAN2Layer(0.1, 24, 24, 4, True, nn.Embedding(1, 24))
+    b = graphgps_b200.SAN2Layer(0.1, 24, 24, 4, True, a.attention.fake_edge_emb)
     assert a.attention.gamma is not b.attention.gamma
 
 
-@pytest.mark.parametrize("kw", [dict(full_graph=False), dict(layer_norm=True), dict(batch_norm=False),
-                                dict(residual=False), dict(use_bias=True)])
+@pytest.mark.parametrize("kw", NOT_BUILT)
 def test_constructor_not_built(kw):
-    args = dict(gamma=0.1, in_dim=48, out_dim=48, num_heads=8, full_graph=True, fake_edge_emb=nn.Embedding(1, 48))
-    args.update(kw)
-    with pytest.raises(NotImplementedError, match="SAN2Layer"):
-        graphgps_b200.SAN2Layer(**args)
+    check_constructor_not_built("SAN2", kw, match="SAN2Layer")
 
 
 def test_constructor_contract():
@@ -167,16 +133,6 @@ def test_non_float64_gamma_is_refused():
         layer(b)
 
 
-def _args(d=56, heads=8, N=133, E=300, B=6, nmax=30, variant=1):
-    a = _lib.GpsSanArgs()
-    a.d, a.heads = d, heads
-    a.graph.N, a.graph.E, a.graph.B = N, E, B
-    a.nmax = nmax
-    a.training = 1
-    a.variant = variant
-    return a
-
-
 def _round(n):
     return (n + 255) // 256 * 256
 
@@ -185,15 +141,15 @@ def test_abi_plan_variant1():
     lib = _lib.load()
     N, E, d, H = 133, 300, 56, 8
     p0, p1 = _lib.GpsSanPlan(), _lib.GpsSanPlan()
-    assert lib.gps_san_plan(C.byref(_args(variant=0)), C.byref(p0)) == _lib.GPS_OK
-    assert lib.gps_san_plan(C.byref(_args()), C.byref(p1)) == _lib.GPS_OK
+    assert lib.gps_san_plan(C.byref(_args("SAN")), C.byref(p0)) == _lib.GPS_OK
+    assert lib.gps_san_plan(C.byref(_args("SAN2")), C.byref(p1)) == _lib.GPS_OK
     # R and F [N, d] and the two log-sum-exps [2, N, H] in place of rz [N, H]
     assert p1.saved_bytes - p0.saved_bytes == 2 * _round(4 * N * d) + _round(8 * N * H) - _round(4 * N * H)
     assert p1.bwd_workspace_bytes - p0.bwd_workspace_bytes == _round(8 * N * H) - _round(4 * N * H)   # Dr and Df
     assert p1.fwd_workspace_bytes == p0.fwd_workspace_bytes
     assert p1.saved_bytes >= 4 * (N * d * 13 + E * d)
     z = _lib.GpsSanPlan()                  # a zero-filled args struct is variant 0, as before
-    a = _args(variant=0)
+    a = _args("SAN")
     a.gamma = -1.0
     assert lib.gps_san_plan(C.byref(a), C.byref(z)) == _lib.GPS_ERR_ARG
     a.variant = 1                          # the gamma field is not read by SAN2
@@ -205,14 +161,14 @@ def test_abi_plan_variant1():
 def test_abi_unknown_variant(variant):
     lib = _lib.load()
     plan = _lib.GpsSanPlan()
-    assert lib.gps_san_plan(C.byref(_args(variant=variant)), C.byref(plan)) == _lib.GPS_ERR_UNSUPPORTED
+    assert lib.gps_san_plan(C.byref(_args(variant)), C.byref(plan)) == _lib.GPS_ERR_UNSUPPORTED
     assert "variant" in lib.gps_last_error().decode()
 
 
 def test_abi_rejects_before_any_cuda_call():
     """Bad or NULL arguments of variant 1 return before touching the device (these pointers are never dereferenced)."""
     lib = _lib.load()
-    a = _args()
+    a = _args("SAN2")
     fake = 1 << 40
     a.x, a.edge_attr, a.x_out, a.saved, a.workspace = fake, fake, fake, fake, fake
     a.grad_x_out, a.grad_x = fake, fake
