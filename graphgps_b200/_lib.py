@@ -205,6 +205,21 @@ class GpsCustomGnnPlan(C.Structure):
 CUSTOM_GATEDGCN, CUSTOM_GINE = 0, 1
 
 
+class GpsGemmArgs(C.Structure):
+    """One dense product with its fused epilogue (gps_gemm_epilogue): sizes, fp32 operands, operand / output planes,
+    the epilogue fields in the order they apply, and the arithmetic."""
+    _fields_ = [("M", C.c_int64), ("N", C.c_int64), ("K", C.c_int64),
+                ("A", _fp), ("lda", C.c_int64), ("B", _fp), ("ldb", C.c_int64), ("ta", C.c_int32), ("tb", C.c_int32),
+                ("Ap", GpsPlanes), ("Bp", GpsPlanes), ("Cp", GpsPlanes),
+                ("C", _fp), ("ldc", C.c_int64), ("cp_hd", C.c_int32), ("cp_hd_pad", C.c_int32),
+                ("bias", _fp), ("C_pre", _fp), ("ldpre", C.c_int64), ("mask_src", _fp), ("ldmask", C.c_int64),
+                ("act", C.c_int32), ("mask_act", C.c_int32), ("mask_is_post", C.c_int32),
+                ("p_drop", C.c_float), ("site", C.c_int32), ("p_drop2", C.c_float), ("site2", C.c_int32),
+                ("splitk", C.c_int32), ("seed", C.c_uint64), ("offset", C.c_uint64), ("offset_dev", _fp),
+                ("R1", _fp), ("ldr1", C.c_int64), ("R2", _fp), ("ldr2", C.c_int64),
+                ("stats", _fp), ("colsum_a", _fp), ("precision", C.c_int32), ("reserved", C.c_int32)]
+
+
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
                 ("bwd_workspace_bytes", C.c_int64), ("wplanes_bytes", C.c_int64)]
@@ -310,6 +325,7 @@ SYMBOLS = {
     "gps_to_planes": (C.c_int, [_fp, _i64, _i64, _i64, _fp, _fp, _i64, _fp]),
     "gps_gemm_planes": (C.c_int, [_fp, _fp, _i64, _i32, _fp, _fp, _i64, _i32, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64,
                                   _i32, _i32, _fp, _fp]),
+    "gps_gemm_epilogue": (C.c_int, [C.POINTER(GpsGemmArgs), _i32, _fp]),
     "gps_fallback_count": (C.c_ulonglong, []),
     # not in the header's stage list but part of the ABI: launch counter for bench.py
     "gps_launch_count": (C.c_ulonglong, []),

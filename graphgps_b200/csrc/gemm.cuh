@@ -39,7 +39,7 @@ struct GemmParams {
   Planes Ap, Bp, Cp;
   // Cp column remap for the attention operands: output column c lands at (c / cp_hd) * cp_hd_pad + c % cp_hd and the
   // cp_hd_pad - cp_hd pad columns of every head are written as zeros (per-head layout padded to a multiple of 16)
-  int cp_hd = 0, cp_hd_pad = 0, cp_col0 = 0;   // cp_col0: first output column of the remapped block
+  int cp_hd = 0, cp_hd_pad = 0;
 };
 
 struct ToPlanesItem { const float* src; int64_t ld; int rows; int cols; Planes dst; };

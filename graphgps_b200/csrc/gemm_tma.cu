@@ -308,7 +308,7 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
         // plane column: identity, or the per-head padded layout of the attention operands (cp_hd)
         int pcol = col, npad = 0;
         if (p.cp_hd > 0) {
-          const int cl = col - (p.cp_col0), hq = cl / p.cp_hd, cw = cl - hq * p.cp_hd;
+          const int hq = col / p.cp_hd, cw = col - hq * p.cp_hd;
           pcol = hq * p.cp_hd_pad + cw;
           npad = (cw + 4 == p.cp_hd) ? p.cp_hd_pad - p.cp_hd : 0;   // this thread also zeroes the head's pad columns
         }

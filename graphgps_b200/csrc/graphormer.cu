@@ -166,7 +166,7 @@ int graphormer_forward(const GpsGraphormerArgs* a, const GpsAttnBias* bias, cuda
   GemmParams gq = linear_fwd(P, N, 3 * d, d, {P.h, d, P.h_p}, {a->attn_in.weight, d, P.win_p}, P.Y, 3 * d,
                              a->attn_in.bias);
   if (P.attn_tc) {
-    gq.Cp = P.qkv_p; gq.cp_hd = (int)P.hd; gq.cp_hd_pad = (int)attention_tc_hd_pad(P.hd); gq.cp_col0 = 0;
+    gq.Cp = P.qkv_p; gq.cp_hd = (int)P.hd; gq.cp_hd_pad = (int)attention_tc_hd_pad(P.hd);
   }
   GPS_TRY(gemm(gq, st));
   // attention over each graph's own nodes (to_dense_batch + key_padding_mask + [real_nodes])

@@ -75,6 +75,12 @@ int gemm(const GemmParams& p, cudaStream_t stream) {
     if (rc != GPS_ERR_UNSUPPORTED) return rc;
   }
   GPS_REQUIRE(p.A && p.B && p.C, GPS_ERR_UNSUPPORTED, "gemm: plane operands rejected and no fp32 operands to fall back to");
+  // the conversion below writes the identity layout only: per-head padded planes (the wgmma attention's Q | K | V)
+  // would land at the wrong columns with their pad columns unwritten
+  GPS_REQUIRE(!(p.Cp.hi && p.cp_hd > 0), GPS_ERR_UNSUPPORTED,
+              "gemm: dense product M=%d N=%d K=%d (ta=%d tb=%d) with per-head padded output planes (hd %d, padded to %d) "
+              "was rejected by the TMA kernel, and the fp32 fallback cannot write that layout",
+              p.M, p.N, p.K, p.ta, p.tb, p.cp_hd, p.cp_hd_pad);
   GemmParams q = p;
   if (q.Cp.hi) {   // the fp32 kernels do not write planes: convert afterwards
     q.Cp = Planes();
@@ -902,7 +908,7 @@ static int layer_forward(const GpsLayerArgs* a, cudaStream_t st) {
     if (wg > 0) {
       GemmParams g = linear_fwd(P, N, wg, d, x, {P.Wcat + wl * d, d, P.Wcat_p.rows(wl)}, P.Y1 + wl, P.Wy, P.bcat + wl);
       if (P.attn_tc) {   // Q | K | V additionally as padded per-head operand planes for the wgmma attention
-        g.Cp = P.qkv_p; g.cp_hd = (int)P.hd; g.cp_hd_pad = (int)attention_tc_hd_pad(P.hd); g.cp_col0 = 0;
+        g.Cp = P.qkv_p; g.cp_hd = (int)P.hd; g.cp_hd_pad = (int)attention_tc_hd_pad(P.hd);
       }
       GPS_TRY(gemm(g, sg));
     }
@@ -1548,6 +1554,46 @@ extern "C" int gps_gemm_planes(const void* A_hi, const void* A_lo, int64_t lda, 
   if (rc == GPS_ERR_UNSUPPORTED) set_error("gps_gemm_planes: the TMA kernel does not take this shape/alignment");
   return rc;
 }
+extern "C" int gps_gemm_epilogue(const GpsGemmArgs* a, int32_t impl, void* stream) {
+  GPS_REQUIRE(a, GPS_ERR_ARG, "gps_gemm_epilogue: null args");
+  const int64_t kMax = 0x7FFFFFFF;
+  GPS_REQUIRE(a->M >= 0 && a->N >= 0 && a->K >= 0 && a->M <= kMax && a->N <= kMax && a->K <= kMax, GPS_ERR_ARG,
+              "gps_gemm_epilogue: M, N, K must lie in [0, 2^31)");
+  GPS_REQUIRE(impl >= 0 && impl <= 3, GPS_ERR_ARG, "gps_gemm_epilogue: impl %d is not 0..3", impl);
+  GPS_REQUIRE(a->C || a->Cp.hi, GPS_ERR_ARG, "gps_gemm_epilogue: neither C nor Cp given");
+  // the CUDA-core and register-staged kernels read the fp32 operands and write fp32 C only
+  GPS_REQUIRE(!(impl == 1 || impl == 2) || !a->Cp.hi, GPS_ERR_ARG,
+              "gps_gemm_epilogue: impl %d does not write output planes (Cp)", impl);
+  GPS_REQUIRE(!(impl == 1 || impl == 2) || (a->A && a->B), GPS_ERR_ARG,
+              "gps_gemm_epilogue: impl %d needs the fp32 operands A and B", impl);
+  GemmParams g;
+  g.M = (int)a->M; g.N = (int)a->N; g.K = (int)a->K;
+  g.A = a->A; g.lda = (int)a->lda; g.ta = a->ta;
+  g.B = a->B; g.ldb = (int)a->ldb; g.tb = a->tb;
+  g.Ap = Planes{(__nv_bfloat16*)a->Ap.hi, (__nv_bfloat16*)a->Ap.lo, a->Ap.ld};
+  g.Bp = Planes{(__nv_bfloat16*)a->Bp.hi, (__nv_bfloat16*)a->Bp.lo, a->Bp.ld};
+  g.Cp = Planes{(__nv_bfloat16*)a->Cp.hi, (__nv_bfloat16*)a->Cp.lo, a->Cp.ld};
+  g.C = a->C; g.ldc = (int)a->ldc; g.cp_hd = a->cp_hd; g.cp_hd_pad = a->cp_hd_pad;
+  g.bias = a->bias; g.C_pre = a->C_pre; g.ldpre = (int)a->ldpre; g.act = a->act;
+  g.mask_src = a->mask_src; g.ldmask = (int)a->ldmask; g.mask_act = a->mask_act; g.mask_is_post = a->mask_is_post;
+  g.p_drop = a->p_drop; g.site = a->site; g.p_drop2 = a->p_drop2; g.site2 = a->site2;
+  g.seed = a->seed; g.offset = a->offset; g.offset_dev = a->offset_dev;
+  g.R1 = a->R1; g.ldr1 = (int)a->ldr1; g.R2 = a->R2; g.ldr2 = (int)a->ldr2;
+  g.stats = a->stats; g.colsum_a = a->colsum_a; g.splitk = a->splitk < 1 ? 1 : a->splitk; g.precision = a->precision;
+  const cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  switch (impl) {
+    case 1: rc = gemm_simt(g, st); break;
+    case 2: rc = gemm_tc(g, st); break;
+    case 3: rc = gemm_tma(g, st); break;
+    default: return gemm(g, st);
+  }
+  if (rc == GPS_ERR_UNSUPPORTED)
+    set_error("gps_gemm_epilogue: impl %d does not take M=%d N=%d K=%d (ta=%d tb=%d) with these alignments", impl, g.M,
+              g.N, g.K, g.ta, g.tb);
+  return rc;
+}
+
 extern "C" void gps_debug_set(int v) { gemm_tc_set_debug(v); }
 // bring-up hooks of the TMA GEMM: forced tile width (0 = heuristic) and a device buffer of 256 x 16 uint64 phase stamps
 extern "C" void gps_debug_tma(int force_bn, void* trace) {

@@ -922,6 +922,47 @@ int gps_to_planes(const float* src, int64_t ld, int64_t rows, int64_t cols, void
 int gps_gemm_planes(const void* A_hi, const void* A_lo, int64_t lda, int32_t ta, const void* B_hi, const void* B_lo,
                     int64_t ldb, int32_t tb, float* C, int64_t ldc, void* C_hi, void* C_lo, int64_t ldcp, int64_t M,
                     int64_t N, int64_t K, int32_t splitk, int32_t precision, float* colsum_a, void* stream);
+/* One dense product with the fused epilogue every Linear of the layers runs (the arguments of gps_gemm_planes plus
+ * the epilogue fields), so the epilogue can be tested step by step.  In this order, per output element:
+ *   v = Aop Bop + bias[n]; C_pre = v; v = act(v); v *= act'(mask_src) (mask_is_post, relu only: [mask_src > 0]);
+ *   v *= drop(p_drop2, site2); v *= drop(p_drop, site); v += R1 + R2; C = v; Cp = bf16 hi/lo planes of v;
+ *   stats[0][n] += v, stats[1][n] += v^2 (float64, pre-zeroed by the caller).
+ * act / mask_act: -1 none, GPS_ACT_*.  Dropout (p > 0, N % 4 == 0) draws gps_dropout_mask(M, N, p, seed,
+ * offset + *offset_dev (offset_dev NULL: + 0), site): the index is over a dense [M, N] grid whatever ldc is.
+ * cp_hd > 0 writes Cp in the per-head padded layout of the wgmma attention: column c lands at
+ * (c / cp_hd) * cp_hd_pad + c % cp_hd, and the cp_hd_pad - cp_hd pad columns of every head are zeros.
+ * splitk > 1 adds Aop Bop (+ R1 + R2) into a pre-zeroed C and takes no other epilogue field (GPS_ERR_ARG).
+ * colsum_a (ta = 1 only, else GPS_ERR_ARG) adds the row sums of Aop.
+ * impl: 0 = the dispatcher the layers call (planes when both are given, else or on rejection the fp32 kernels),
+ * 1 = exact CUDA-core kernel, 2 = register-staged tensor-core kernel, 3 = TMA-fed tensor-core kernel.  1 and 2 read the
+ * fp32 A and B and never write planes: Cp, or a NULL A or B, with impl 1 or 2 is GPS_ERR_ARG, as are a NULL args, sizes
+ * outside [0, 2^31), an impl outside 0..3 and neither C nor Cp given, all before any CUDA call.  A kernel that does not take the shape,
+ * layout or alignment returns GPS_ERR_UNSUPPORTED; so does the dispatcher when the TMA kernel rejects a product whose
+ * planes need the per-head layout (the fp32 fallback writes the identity layout only). */
+typedef struct {
+  int64_t M, N, K;
+  const float* A; int64_t lda;
+  const float* B; int64_t ldb;
+  int32_t ta, tb;
+  GpsPlanes Ap, Bp, Cp;
+  float* C; int64_t ldc;
+  int32_t cp_hd, cp_hd_pad;
+  const float* bias;
+  float* C_pre; int64_t ldpre;
+  const float* mask_src; int64_t ldmask;
+  int32_t act, mask_act, mask_is_post;
+  float p_drop; int32_t site;
+  float p_drop2; int32_t site2;
+  int32_t splitk;
+  uint64_t seed, offset;
+  const unsigned long long* offset_dev;
+  const float* R1; int64_t ldr1;
+  const float* R2; int64_t ldr2;
+  double* stats;
+  float* colsum_a;
+  int32_t precision, reserved;
+} GpsGemmArgs;
+int gps_gemm_epilogue(const GpsGemmArgs* a, int32_t impl, void* stream);
 /* number of dense products that fell back from the tensor-core kernels to the exact CUDA-core kernel
  * (unaligned / odd shapes) in this process; with GPS_B200_STRICT=1 in the environment such a fallback is an error */
 unsigned long long gps_fallback_count(void);

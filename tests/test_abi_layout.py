@@ -15,7 +15,8 @@ INCLUDE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "includ
 
 STRUCTS = [_lib.GpsGraph, _lib.GpsBatchNorm, _lib.GpsLinear, _lib.GpsPlanes, _lib.GpsAttnBias, _lib.GpsGat,
            _lib.GpsGenConv, _lib.GpsPna, _lib.GpsBigBird, _lib.GpsLayerArgs, _lib.GpsLayerPlan, _lib.GpsGraphormerArgs,
-           _lib.GpsGraphormerPlan, _lib.GpsSanArgs, _lib.GpsSanPlan, _lib.GpsCustomGnnArgs, _lib.GpsCustomGnnPlan]
+           _lib.GpsGraphormerPlan, _lib.GpsSanArgs, _lib.GpsSanPlan, _lib.GpsCustomGnnArgs, _lib.GpsCustomGnnPlan,
+           _lib.GpsGemmArgs]
 
 # header enum prefix -> the _lib name -> value map it must equal (keys upper-cased, "Custom" dropped: CustomGatedGCN is
 # GPS_LOCAL_GATEDGCN)
