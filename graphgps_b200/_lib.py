@@ -331,6 +331,7 @@ SYMBOLS = {
     "gps_launch_count": (C.c_ulonglong, []),
     "gps_debug_set": (None, [C.c_int]),
     "gps_debug_tma": (None, [C.c_int, _fp]),
+    "gps_debug_tma_splits": (None, [C.c_int]),
     "gps_debug_attn": (None, [_fp]),
 }
 

@@ -12,7 +12,9 @@ namespace gps {
 // Epilogue order: +bias[n] -> (store pre-activation) -> act -> *act'(mask_src) -> dropout ->
 //                 +R1 +R2 -> store -> column statistics (sum, sum of squares, double atomics).
 // With splitk > 1 the partial products are atomically added into a pre-zeroed C and only the
-// plain product is supported.
+// plain product is supported.  (With splitk <= 1 the TMA kernel may still split K when its launch policy finds that
+// faster: a cluster whose ranks sum their partial tiles in rank order and then run the whole epilogue on their own
+// rows, so C is written, not added to.)
 struct GemmParams {
   int M = 0, N = 0, K = 0;
   const float* A = nullptr; int lda = 0; int ta = 0;
@@ -51,6 +53,7 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream);
 int make_tensor_map(const __nv_bfloat16* hi, const __nv_bfloat16* lo, int planes, int64_t rows, int64_t cols, int64_t ld,
                     int box_rows, CUtensorMap* out);
 void gemm_tma_set_force_bn(int bn);
+void gemm_tma_set_force_splits(int s);   // K-splits of every launch that runs the epilogue (0 = the launch policy)
 void gemm_tma_set_trace(unsigned long long* buf);   // bring-up: per-CTA phase timestamps (tools/gemm_trace.py)
 
 // exact fp32 CUDA-core product (validation path and shapes the tensor-core kernel does not take)

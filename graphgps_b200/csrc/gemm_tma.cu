@@ -19,8 +19,10 @@
 // Narrow tiles (BN = 64) are launched two CTAs per SM so one CTA's epilogue overlaps the other's main loop.
 // Split-K: the K-splits of one output tile form a thread-block cluster (at most 8).  Each split stages its fp32 partial
 // tile in shared memory; rank r then sums rows [r RB, (r + 1) RB) of all ranks' tiles in rank order through
-// distributed shared memory and is the only CTA that adds those rows (and the residuals) into C, so the result does not
-// depend on the order in which the splits finish.  The bias-gradient partials of the splits are combined the same way.
+// distributed shared memory (RB a multiple of 16, the row classes of the column sums), so the result does not depend on
+// the order in which the splits finish.  A caller-requested split (splitk > 1) adds the summed rows (and the residuals)
+// into the pre-zeroed C; a split the launch policy chooses runs the full epilogue on them instead, rank r being the
+// only writer of its rows.  The bias-gradient partials of the splits are combined the same way.
 #include <cooperative_groups.h>
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -58,6 +60,19 @@ __device__ __forceinline__ unsigned long long gtimer() {
   asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
   return t;
 }
+// Rows [x, y) of the tile that this CTA's K-split owns after the cluster's reduction (the whole tile without split-K).
+// RB is a multiple of 16, so a rank's rows start on row class 0 of the column sums; trailing ranks may own no rows
+// (5-7 splits).  Read from the special registers at each use (volatile), so that the epilogue keeps no extra registers
+// live across its row loop.
+__device__ __forceinline__ int2 split_rows() {
+  int z, nz;
+  asm volatile("mov.u32 %0, %%ctaid.z;" : "=r"(z));
+  asm volatile("mov.u32 %0, %%nctaid.z;" : "=r"(nz));
+  const int RB = ((BM + nz - 1) / nz + 15) & ~15;
+  const int lo = min(BM, z * RB);
+  return make_int2(lo, min(BM, lo + RB));
+}
+
 #define GPS_TRACE(slot)                                                                         \
   do {                                                                                          \
     if (a.trace && cta_lin < 256) a.trace[cta_lin * 16 + (slot)] = gtimer();                    \
@@ -244,19 +259,48 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
       }
     }
     asm volatile("bar.sync 1, 256;" ::: "memory");
-    // ---- split-K: rank r replaces rows [lo, hi) of its staging tile by the rank-ordered sum over the cluster
-    const int RB = (BM + nsplit - 1) / nsplit;
-    const int lo = (int)blockIdx.z * RB, hi = min(BM, lo + RB);
+    // ---- split-K: rank r replaces rows [lo, hi) of its staging tile by the rank-ordered sum over the cluster and owns
+    // them for the rest of the epilogue
+    const int lo = split_rows().x, hi = split_rows().y;
     if (nsplit > 1) {
       cgrp::cluster_group cluster = cgrp::this_cluster();
       cluster.sync();   // every split's staging tile (and bias-gradient sums) is complete
+      // Each thread keeps U float4s of every rank in flight at once: a distributed shared memory load costs a round
+      // trip, and one element at a time the pass is that latency times the element count.  Only the rows below M are
+      // summed (the epilogue reads no others).  The 64-wide kernels (96 registers) sum one element at a time.
       const int c4n = a.BN >> 2;
-      for (int idx = tid; idx < (hi - lo) * c4n; idx += kEpiWarps * 32) {
-        const int r = lo + idx / c4n, c = (idx % c4n) * 4;
-        float4 sum = f4zero();
-        for (int k = 0; k < nsplit; ++k)
-          sum = f4add(sum, *reinterpret_cast<const float4*>(cluster.map_shared_rank(stage, k) + r * sld + c));
-        *reinterpret_cast<float4*>(stage + r * sld + c) = sum;
+      const int n4 = max(0, min(hi, p.M - m0) - lo) * c4n;
+      constexpr int U = BN_T == 64 ? 1 : 4, kStep = kEpiWarps * 32;
+      if constexpr (U == 1) {
+        for (int idx = tid; idx < n4; idx += kStep) {
+          const int o = (lo + idx / c4n) * sld + (idx % c4n) * 4;
+          float4 sum = f4zero();
+          for (int k = 0; k < nsplit; ++k)
+            sum = f4add(sum, *reinterpret_cast<const float4*>(cluster.map_shared_rank(stage, k) + o));
+          *reinterpret_cast<float4*>(stage + o) = sum;
+        }
+      } else {
+        for (int b = tid; b < n4; b += U * kStep) {
+          int off[U];
+          float4 sum[U];
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            const int idx = min(b + u * kStep, n4 - 1);   // past the end: re-reads a valid element, not stored
+            off[u] = (lo + idx / c4n) * sld + (idx % c4n) * 4;
+            sum[u] = f4zero();
+          }
+          for (int k = 0; k < nsplit; ++k) {
+            const float* src = cluster.map_shared_rank(stage, k);
+            float4 v[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) v[u] = *reinterpret_cast<const float4*>(src + off[u]);
+#pragma unroll
+            for (int u = 0; u < U; ++u) sum[u] = f4add(sum[u], v[u]);
+          }
+#pragma unroll
+          for (int u = 0; u < U; ++u)
+            if (b + u * kStep < n4) *reinterpret_cast<float4*>(stage + off[u]) = sum[u];
+        }
       }
       if (do_colsum && blockIdx.z == 0 && tid < 128 && m0 + tid < p.M) {
         float tot = 0.f;
@@ -268,21 +312,23 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     // ---- phase 2: G = BN/4 threads per row, each owning 4 consecutive columns for all of its rows: every global access
     // (bias, residuals, act' mask, fp32 / plane stores, split-K atomics) is a contiguous row segment and the per-column
     // constants live in registers.  When BatchNorm column sums are wanted, w goes back into the staging tile for them.
+    // The pass covers this CTA's rows [lo, row_end) of the tile: all of them without split-K.
     const int G = a.BN >> 2;
     const int rpp = kEpiWarps * 32 / G;            // rows per pass
     const int rip = tid / G, cg = tid - rip * G;
     const int col = n0 + cg * 4;
     const bool col_ok = rip < rpp && col < p.N;
     const int rows_here = min(BM, p.M - m0);
+    const int row_end = min(hi, rows_here);
     const bool colstats = p.stats != nullptr;
     if (col_ok) {
-      // rows of this thread: r = rip + k * rpp, k < nrows.  Everything is addressed through per-thread base pointers
+      // rows of this thread: r = lo + rip + k * rpp, k < nrows.  Everything is addressed through per-thread base pointers
       // advanced by a constant stride, and the loop is unrolled by 4 rows so that the shared/global loads of a group are
       // in flight together: with 2 epilogue warps per scheduler the pass is instruction-latency bound otherwise
       // (even with the global stores off the critical path).
-      const int nrows = rip < rows_here ? (rows_here - rip + rpp - 1) / rpp : 0;
-      const int64_t row0 = m0 + rip;
-      float* sp = stage + rip * sld + cg * 4;
+      const int nrows = lo + rip < row_end ? (row_end - lo - rip + rpp - 1) / rpp : 0;
+      const int64_t row0 = m0 + lo + rip;
+      float* sp = stage + (lo + rip) * sld + cg * 4;
       const int s_st = rpp * sld;
       float* cp = p.C ? p.C + row0 * p.ldc + col : nullptr;
       const int64_t c_st = (int64_t)rpp * p.ldc;
@@ -397,17 +443,20 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
         }
       }
     }
-    if (colstats) {
-      // BatchNorm column sums over this tile's rows, in the same order for every tile width: task (y, g) sums rows
-      // y, y + 16, ... of column group g (sum w, sum w^2) and leaves the two partials in rows y, y + 16 of its own row
-      // class; then one thread per column group adds the 16 classes in order: one double atomic per column per CTA and
+    const int2 own = split_rows();
+    const int slo = own.x, send = min(own.y, min(BM, p.M - m0));
+    if (colstats && slo < send) {
+      // BatchNorm column sums over this CTA's rows, in the same order for every tile width: task (y, g) sums rows
+      // lo + y, lo + y + 16, ... of column group g (sum w, sum w^2) and leaves the two partials in rows y, y + 16 of its
+      // own row class (lo is a multiple of 16, and after the cluster's last barrier the whole staging tile is this
+      // CTA's); then one thread per column group adds the 16 classes in order: one double atomic per column per CTA and
       // statistic.
       asm volatile("bar.sync 1, 256;" ::: "memory");
       for (int t = tid; t < 16 * G; t += kEpiWarps * 32) {
         const int y = t / G, g = t - y * G, c = n0 + g * 4;
         if (c >= p.N) continue;
         float4 s1 = f4zero(), s2 = f4zero();
-        for (int r = y; r < rows_here; r += 16) {
+        for (int r = slo + y; r < send; r += 16) {
           const float4 w = *reinterpret_cast<const float4*>(stage + r * sld + g * 4);
           s1 = f4add(s1, w);
           s2 = f4fma(w, w, s2);
@@ -557,11 +606,13 @@ int launch(const CUtensorMap& tA, const CUtensorMap& tB, const TmaArgs& a, dim3 
 }
 
 int g_tma_force_bn = 0;
+int g_tma_force_splits = 0;
 unsigned long long* g_tma_trace = nullptr;
 
 }  // namespace
 
 void gemm_tma_set_force_bn(int bn) { g_tma_force_bn = bn; }
+void gemm_tma_set_force_splits(int s) { g_tma_force_splits = s; }
 void gemm_tma_set_trace(unsigned long long* buf) { g_tma_trace = buf; }
 
 int gemm_tma(const GemmParams& p, cudaStream_t stream) {
@@ -591,7 +642,11 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream) {
   }
   const int mt = (int)ceil_div(p.M, BM);
   const int nkb = (int)ceil_div(p.K, BK);
-  const int splits_hint = p.splitk > 1 ? min(kMaxSplits, min(p.splitk, nkb)) : 1;
+  // K-splits actually launched for a requested count s: every split but the last takes ceil(nkb / s) k-blocks
+  const auto splits_of = [&](int s) {
+    s = max(1, min(kMaxSplits, min(s, nkb)));
+    return (int)ceil_div(nkb, ceil_div(nkb, s));
+  };
   // Tile width.  Measured at the layer's shapes, a launch takes time in proportion to the MMA columns its busiest SM
   // issues: waves x BN, where zero-padded columns count (they cost MMAs and staging like real ones) and
   // waves = ceil(tiles / CTA slots).  The epilogue's stores and the operand loads of a tile grow with BN as well, and
@@ -605,14 +660,54 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream) {
   const auto width_ok = [&](int bn) {
     return bn == 64 || bn == 128 || (bn == 152 && !p.tb) || (bn == 256 && !p.ta);
   };
-  int bestBN = 0;
-  long bestCost = 0;
-  for (const int bn : {64, 128, 152, 256}) {
-    if (!width_ok(bn)) continue;
-    const long tiles = (long)mt * ceil_div(p.N, bn) * splits_hint;
-    const long cost = bn != 64 ? ceil_div(tiles, (long)kNumSMs) * bn : tiles <= kNumSMs ? 64 : ceil_div(tiles, 2L * kNumSMs) * 160;
-    if (!bestBN || cost <= bestCost) { bestCost = cost; bestBN = bn; }
+  //
+  // K-splits of a launch that runs the epilogue (splitk <= 1).  A CTA's time is a fixed part (launch, prologue, the
+  // first operand fetch, staging, the epilogue pass) plus its k-blocks, both per column; a split adds the cluster's
+  // barriers and the rank-ordered sum of the staged partial tiles through distributed shared memory.  Fitted to the
+  // per-launch times at d = 304 with the layer's epilogues (H100 SXM, 700 W; 58 tiles of 152 columns: 15.6 us at 5
+  // k-blocks, 22.3 us at 10, 18.8 and 22.8 us for the same launches in 2 splits), the fixed part is worth about 7
+  // k-blocks and a split about 5 more.  So a launch costs waves x BN x (k-blocks per split + 7 (+ 5 when split)), in
+  // quarter k-blocks below.  A split is considered only while the split tiles still fit on the SMs at one CTA each
+  // (tiles <= 132 / splits; a second wave lost every time it was measured) and every split keeps at least 2 k-blocks;
+  // ties go to fewer splits.  At d = 304 no product of the layer is split (10 k-blocks is the break-even); the split
+  // pays for long reductions over few row tiles (g_x at d = 256, M = 4000: 2 splits).  The split depends on the shape alone, never on a forced tile
+  // width, so every width still computes each element with the same wgmma sequence.
+  const auto wave_cost = [&](int bn, long ctas) -> long {
+    return bn != 64 ? ceil_div(ctas, (long)kNumSMs) * bn : ctas <= kNumSMs ? 64 : ceil_div(ctas, 2L * kNumSMs) * 160;
+  };
+  const auto best_width = [&](int s, long* cost_out) {
+    int best = 0;
+    long best_cost = 0;
+    for (const int bn : {64, 128, 152, 256}) {
+      if (!width_ok(bn)) continue;
+      const long cost = wave_cost(bn, (long)mt * ceil_div(p.N, bn) * s);
+      if (!best || cost <= best_cost) { best_cost = cost; best = bn; }
+    }
+    if (cost_out) *cost_out = best_cost;
+    return best;
+  };
+  int nsplit = 1;
+  if (p.splitk > 1) {
+    nsplit = splits_of(p.splitk);
+  } else if (g_tma_force_splits > 0) {
+    nsplit = splits_of(g_tma_force_splits);
+  } else {
+    long best_cost = 0;
+    for (int s = 1; s <= kMaxSplits; ++s) {
+      if (splits_of(s) != s) continue;
+      const int kbps = (int)ceil_div(nkb, s);
+      if (s > 1 && nkb - (s - 1) * kbps < 2) continue;
+      long wc = 0;
+      const int bn = best_width(s, &wc);
+      if (s > 1 && (long)mt * ceil_div(p.N, bn) * s > kNumSMs) continue;
+      // a 64-wide CTA with an SM to itself streams the same A tile per k-block as a 128-wide one and was measured no
+      // faster over a long K (g_x at M = 4000, d = 256: 64 us against 49 us fp32-grade, and 35 us in 2 splits of 128)
+      if (bn == 64) wc = max(wc, 128L);
+      const long cost = wc * (4L * kbps + 28 + (s > 1 ? 20 : 0));
+      if (s == 1 || cost < best_cost) { best_cost = cost; nsplit = s; }
+    }
   }
+  int bestBN = best_width(p.splitk > 1 ? min(kMaxSplits, min(p.splitk, nkb)) : nsplit, nullptr);
   if (g_tma_force_bn) {
     if (!width_ok(g_tma_force_bn)) return GPS_ERR_UNSUPPORTED;
     bestBN = g_tma_force_bn;
@@ -632,11 +727,7 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream) {
   GPS_REQUIRE((size_t)stages * stage_bytes >= (size_t)BM * (a.BN + 4) * 4, GPS_ERR_ARG,
               "gemm_tma: BN %d: the staging tile does not fit the operand stages", a.BN);
   a.stages = stages;
-  int splitk = p.splitk > 1 ? p.splitk : 1;
-  if (splitk > kMaxSplits) splitk = kMaxSplits;
-  if (splitk > nkb) splitk = nkb;
-  a.kb_per_split = (int)ceil_div(nkb, splitk);
-  splitk = (int)ceil_div(nkb, a.kb_per_split);
+  a.kb_per_split = (int)ceil_div(nkb, nsplit);
   a.p.splitk = p.splitk > 1 ? 2 : 1;   // "accumulate atomically" flag
   a.trace = g_tma_trace;
   const bool amn = p.ta != 0, bmn = p.tb != 0;
@@ -645,7 +736,7 @@ int gemm_tma(const GemmParams& p, cudaStream_t stream) {
   GPS_TRY(tensor_map(p.Ap.hi, p.Ap.lo, planes, amn ? p.K : p.M, amn ? p.M : p.K, p.Ap.ld, amn ? 64 : BM, &tA));
   GPS_TRY(tensor_map(p.Bp.hi, p.Bp.lo, planes, bmn ? p.K : p.N, bmn ? p.N : p.K, p.Bp.ld, bmn ? 64 : a.BN, &tB));
   const size_t smem = (size_t)stages * stage_bytes + fixed;
-  dim3 grid((unsigned)ceil_div(p.N, a.BN), (unsigned)mt, (unsigned)splitk);
+  dim3 grid((unsigned)ceil_div(p.N, a.BN), (unsigned)mt, (unsigned)nsplit);
 #define GPS_TMA_CASE(AM, BMN)                                                                              \
   if (amn == AM && bmn == BMN) {                                                                           \
     if (a.BN == 64) return launch<AM, BMN, 64>(tA, tB, a, grid, smem, stream);                            \

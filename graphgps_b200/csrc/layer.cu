@@ -1159,13 +1159,11 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
   };
   auto early_done = [&]() -> int { return record_ev(a->ev_grads_early, s2); };
   auto mid_done = [&]() -> int { return record_ev(a->ev_grads_mid, s2); };   // after the local model's weight gradients
-  // accumulators of the last two GEMMs of the pass are zeroed now, while their streams are idle, instead of on the tail
-  const bool gx_splitk = P.Wy >= 1024 && N > 0;
+  // the accumulator of dWcat is zeroed now, while its stream is idle, instead of on the tail
   if (P.Wy) {
     GPS_TRY(wfork(st));
     GPS_CUDA(cudaMemsetAsync(P.gWcat, 0, (size_t)(P.Wy * d + P.Wy) * sizeof(float), s2));
   }
-  if (gx_splitk) GPS_CUDA(cudaMemsetAsync(a->grad_x, 0, (size_t)(N * d) * sizeof(float), st));
 
   // e_out = e + drop(act(BN_e(e^))) (gatedgcn_layer.py:76-83): g_e^ needs grad_edge_out alone -> off the critical path
   if (P.gated) {
@@ -1508,7 +1506,9 @@ static int layer_backward(const GpsLayerArgs* a, cudaStream_t st) {
     GemmParams g = linear_dgrad(P, N, d, P.Wy, gY1, {P.Wcat, d, P.Wcat_p}, a->grad_x, d);
     g.R1 = g_x_local; g.ldr1 = (int)d;
     g.R2 = P.attn ? g_hA : (P.perf ? P.g_xp : (P.bb ? P.bb_gx : nullptr)); g.ldr2 = (int)d;
-    if (gx_splitk) g.splitk = 4;   // long reduction, few output tiles: split-K fills the machine (grad_x zeroed above)
+    // grad_x is written by the product's epilogue, not accumulated into, and the launch policy picks any K-split: at
+    // d = 304 none (one CTA per output tile reducing all 7d: 55 us fp32-grade / 33 us bf16, where the 4-way split-K
+    // into a zeroed grad_x took 64 / 45 us; H100 SXM, 700 W), and the memset of grad_x goes
     GPS_TRY(gemm(g, st));
   } else if (g_x_local) {
     GPS_TRY(add3(g_x_local, d, P.perf ? P.g_xp : nullptr, d, nullptr, 0, a->grad_x, d, N, d, st));
@@ -1600,6 +1600,7 @@ extern "C" void gps_debug_tma(int force_bn, void* trace) {
   gemm_tma_set_force_bn(force_bn);
   gemm_tma_set_trace((unsigned long long*)trace);
 }
+extern "C" void gps_debug_tma_splits(int splits) { gemm_tma_set_force_splits(splits); }
 extern "C" void gps_debug_attn(void* buf) { attention_tc_set_debug((float*)buf); }
 
 extern "C" int gps_layer_plan(const GpsLayerArgs* args, GpsLayerPlan* plan) {

@@ -62,6 +62,9 @@ void gps_debug_set(int v);
  * GPS_ERR_UNSUPPORTED); trace = device
  * buffer of 256 x 16 uint64 that the first 256 CTAs of each launch fill with globaltimer phase stamps (NULL = off) */
 void gps_debug_tma(int force_bn, void* trace);
+/* test hook of the TMA-fed GEMM: K-splits of every product that runs its epilogue (splitk <= 1), summed across the
+ * cluster before the epilogue; 0 = the launch policy.  The count is clamped to [1, 8] and to the k-blocks of K. */
+void gps_debug_tma_splits(int splits);
 /* bring-up hook of the wgmma attention: device buffer of 3 x 128 x 128 floats that CTA (0,0) fills with its first
  * S tile, P tile and raw O accumulator (NULL = off) */
 void gps_debug_attn(void* buf);

@@ -1,11 +1,12 @@
 """Per-product times of the TMA-fed GEMM at the GPSLayer shapes of one workload (CUDA events, warm L2).
 
-    python tools/gemm_products.py [workload] [precision fp32|bf16] [force_bn ...]
+    python tools/gemm_products.py [workload] [precision fp32|bf16] [force_bn | sN ...]
 
 Each product runs as the layer issues it (forward Linears also write the operand planes of their output) for 200
 back-to-back launches; the time is the mean per launch.  A time marked * belongs to a result that is not bitwise equal
-to the one of the first width in the list.  With force_bn values the tile width is forced (0 = the
-launch policy's choice); a width the kernel does not instantiate for that operand layout is reported as such."""
+to the one of the first column.  With force_bn values the tile width is forced (0 = the launch policy's choice); a
+width the kernel does not instantiate for that operand layout is reported as such.  sN forces N K-splits on the
+products that run their epilogue (split-K 1 below; the policy's width), s0 the policy's split."""
 import os
 import sys
 
@@ -16,7 +17,9 @@ from graphgps_b200 import _lib  # noqa: E402
 
 wl = sys.argv[1] if len(sys.argv) > 1 else "pcqm4m-small"
 prec = {"fp32": 0, "bf16": 1}[sys.argv[2] if len(sys.argv) > 2 else "fp32"]
-force = [int(v) for v in sys.argv[3:]] or [0]
+# columns: (label, forced width or 0 = the policy's, forced K-splits or 0 = the policy's)
+COLS = [(f, 0, int(f[1:])) if f.startswith("s") else ("policy" if f == "0" else "bn=" + f, int(f), 0)
+        for f in sys.argv[3:] or ["0"]]
 batch = graphgps_b200.make_batch(wl, seed=0)
 Nn, E, d = batch.num_nodes, batch.num_edges, graphgps_b200.SHAPES[wl].dim
 lib = _lib.load()
@@ -35,7 +38,7 @@ PRODUCTS = [
     ("FF1 dgrad", Nn, d, 2 * d, 0, 1, 1, False),
     ("out-proj fwd", Nn, d, d, 0, 0, 1, True),
     ("out-proj dgrad", Nn, d, d, 0, 1, 1, False),
-    ("g_x (split-K 4)", Nn, d, 7 * d, 0, 1, 4, False),
+    ("g_x", Nn, d, 7 * d, 0, 1, 1, False),
     ("edge wgrad", d, d, E, 1, 1, 8, False),
     ("node wgrad d x d", d, d, Nn, 1, 1, 8, False),
     ("FF1 wgrad", 2 * d, d, Nn, 1, 1, 8, False),
@@ -59,7 +62,7 @@ def lo(buf):
 
 torch.manual_seed(0)
 print(f"{wl} {'fp32-grade' if prec == 0 else 'bf16'}: N={Nn} E={E} d={d}; mean us per launch over 200 launches")
-print(f"{'product':24s} {'M x N x K':>16s} " + " ".join(f"{'bn=' + str(b) if b else 'policy':>8s}" for b in force))
+print(f"{'product':24s} {'M x N x K':>16s} " + " ".join(f"{label:>8s}" for label, _, _ in COLS))
 for name, M, N, K, ta, tb, sk, pout in PRODUCTS:
     Ap, lda = planes(K, M) if ta else planes(M, K)
     db = torch.zeros(M, device=dev) if ta and prec == 0 else None
@@ -75,8 +78,9 @@ for name, M, N, K, ta, tb, sk, pout in PRODUCTS:
 
     cells = []
     ref = None
-    for fbn in force:
+    for _, fbn, fsplits in COLS:
         lib.gps_debug_tma(fbn, 0)
+        lib.gps_debug_tma_splits(fsplits)
         C.zero_()
         if run() != 0:
             cells.append(f"{'n/a':>8s}")
@@ -85,7 +89,7 @@ for name, M, N, K, ta, tb, sk, pout in PRODUCTS:
         if ref is None:
             ref = C.clone()
         elif not torch.equal(C, ref):
-            same = "*"   # not bitwise equal to the first width's result
+            same = "*"   # not bitwise equal to the first column's result
         for _ in range(10):
             run()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -96,4 +100,5 @@ for name, M, N, K, ta, tb, sk, pout in PRODUCTS:
         torch.cuda.synchronize()
         cells.append(f"{e0.elapsed_time(e1) * 1e3 / 200:7.1f}{same or ' '}")
     lib.gps_debug_tma(0, 0)
+    lib.gps_debug_tma_splits(0)
     print(f"{name:24s} {f'{M}x{N}x{K}':>16s} " + " ".join(cells), flush=True)
