@@ -220,6 +220,28 @@ class GpsGemmArgs(C.Structure):
                 ("stats", _fp), ("colsum_a", _fp), ("precision", C.c_int32), ("reserved", C.c_int32)]
 
 
+# gps_rowwise_stage ops
+ROWWISE = {"bn_act_residual": 0, "bn_act_residual2": 1, "bn_combine": 2, "bn_bwd_reduce": 3, "bn_bwd_apply": 4,
+           "dropmul": 5, "colsum": 6}
+
+
+class GpsRowwiseBn(C.Structure):
+    """A BatchNorm as a row-wise stage reads it: the module, its mode, saved [mean | invstd] (2d floats) and its
+    float64 sums [2][d]."""
+    _fields_ = [("bn", GpsBatchNorm), ("saved", _fp), ("sums", _fp), ("train", C.c_int32), ("reserved", C.c_int32)]
+
+
+class GpsRowwiseArgs(C.Structure):
+    """One row-wise stage (gps_rowwise_stage): sizes, tensors with their pitches, output planes, up to two BatchNorms,
+    the activation, the dropout sites, the accumulate flag and the column statistics output."""
+    _fields_ = [("rows", C.c_int64), ("E", C.c_int64), ("d", C.c_int64),
+                ("x", _fp), ("ldx", C.c_int64), ("x2", _fp), ("g", _fp), ("ldg", C.c_int64), ("R", _fp), ("R2", _fp),
+                ("out", _fp), ("ldo", C.c_int64), ("out2", _fp), ("planes", GpsPlanes), ("bn", GpsRowwiseBn * 2),
+                ("act", C.c_int32), ("p", C.c_float), ("site", C.c_int32), ("p2", C.c_float), ("site2", C.c_int32),
+                ("accumulate", C.c_int32), ("seed", C.c_uint64), ("offset", C.c_uint64), ("offset_dev", _fp),
+                ("stats", _fp)]
+
+
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
                 ("bwd_workspace_bytes", C.c_int64), ("wplanes_bytes", C.c_int64)]
@@ -326,6 +348,7 @@ SYMBOLS = {
     "gps_gemm_planes": (C.c_int, [_fp, _fp, _i64, _i32, _fp, _fp, _i64, _i32, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64,
                                   _i32, _i32, _fp, _fp]),
     "gps_gemm_epilogue": (C.c_int, [C.POINTER(GpsGemmArgs), _i32, _fp]),
+    "gps_rowwise_stage": (C.c_int, [C.POINTER(GpsRowwiseArgs), _i32, _fp]),
     "gps_fallback_count": (C.c_ulonglong, []),
     # not in the header's stage list but part of the ABI: launch counter for bench.py
     "gps_launch_count": (C.c_ulonglong, []),

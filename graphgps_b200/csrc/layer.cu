@@ -795,6 +795,7 @@ int side_stream(Side** out) {
 
 int dropmul_rows(const float* src, float* dst, int64_t rows, int64_t d, const DropCfg& c, float p2, int site2,
                  Planes dstp, cudaStream_t st) {
+  GPS_REQUIRE(d % 4 == 0, GPS_ERR_UNSUPPORTED, "dropout pass needs d %% 4 == 0 (got %lld)", (long long)d);
   const int64_t n4 = rows * d / 4;
   if (n4 == 0) return GPS_OK;
   k_dropmul<<<(unsigned)std::min<int64_t>(ceil_div(n4, 256), kNumSMs * 8), 256, 0, st>>>(
@@ -1592,6 +1593,85 @@ extern "C" int gps_gemm_epilogue(const GpsGemmArgs* a, int32_t impl, void* strea
     set_error("gps_gemm_epilogue: impl %d does not take M=%d N=%d K=%d (ta=%d tb=%d) with these alignments", impl, g.M,
               g.N, g.K, g.ta, g.tb);
   return rc;
+}
+
+namespace {
+struct StagePlan {   // all bn_view_at reads of a plan
+  bool train;
+};
+}  // namespace
+
+extern "C" int gps_rowwise_stage(const GpsRowwiseArgs* a, int32_t op, void* stream) {
+  GPS_REQUIRE(a, GPS_ERR_ARG, "gps_rowwise_stage: null args");
+  GPS_REQUIRE(op >= GPS_ROWWISE_BN_ACT_RESIDUAL && op <= GPS_ROWWISE_COLSUM, GPS_ERR_ARG,
+              "gps_rowwise_stage: unknown op %d", op);
+  const int64_t rows = a->rows, E = a->E, d = a->d;
+  GPS_REQUIRE(rows >= 0 && E >= 0 && d >= 0, GPS_ERR_ARG, "gps_rowwise_stage: negative size (rows %lld, E %lld, d %lld)",
+              (long long)rows, (long long)E, (long long)d);
+  const bool bwd = op == GPS_ROWWISE_BN_BWD_REDUCE || op == GPS_ROWWISE_BN_BWD_APPLY;
+  const int64_t ldx = a->ldx ? a->ldx : d, ldg = a->ldg ? a->ldg : d, ldo = a->ldo ? a->ldo : d;
+  // the ops whose kernels take a pitch for x, g and out; every other tensor has pitch d
+  const bool free_ldx = op == GPS_ROWWISE_BN_ACT_RESIDUAL || bwd || op == GPS_ROWWISE_COLSUM;
+  const bool free_ldo = op == GPS_ROWWISE_BN_BWD_APPLY;
+  const int64_t lds[3] = {ldx, ldg, ldo};
+  const char* ldn[3] = {"ldx", "ldg", "ldo"};
+  const bool ld_free[3] = {free_ldx, bwd, free_ldo};
+  for (int i = 0; i < 3; ++i) {
+    // ld == d is the dense layout, whose alignment is the kernels' d % 4 rule (GPS_ERR_UNSUPPORTED)
+    GPS_REQUIRE(lds[i] >= d && (lds[i] == d || lds[i] % 4 == 0), GPS_ERR_ARG,
+                "gps_rowwise_stage: %s = %lld must be d = %lld, or above it and a multiple of 4", ldn[i],
+                (long long)lds[i], (long long)d);
+    GPS_REQUIRE(ld_free[i] || lds[i] == d, GPS_ERR_ARG, "gps_rowwise_stage: op %d takes %s = d only (got %lld)", op,
+                ldn[i], (long long)lds[i]);
+  }
+  // tensors over rows (E) may be NULL when there are none
+  GPS_REQUIRE(rows == 0 || a->x, GPS_ERR_ARG, "gps_rowwise_stage: op %d needs x", op);
+  GPS_REQUIRE(rows == 0 || op == GPS_ROWWISE_BN_BWD_REDUCE || a->out, GPS_ERR_ARG, "gps_rowwise_stage: op %d needs out",
+              op);
+  GPS_REQUIRE(rows == 0 || !bwd || a->g, GPS_ERR_ARG, "gps_rowwise_stage: op %d needs g", op);
+  GPS_REQUIRE(E == 0 || op != GPS_ROWWISE_BN_ACT_RESIDUAL2 || (a->x2 && a->out2), GPS_ERR_ARG,
+              "gps_rowwise_stage: BN_ACT_RESIDUAL2 needs x2 and out2");
+  // the BatchNorms the op reads: what bn_view_at hands the kernels must be there
+  const int nbn = op == GPS_ROWWISE_BN_ACT_RESIDUAL2 || (op == GPS_ROWWISE_BN_COMBINE && a->x2) ? 2
+                  : op == GPS_ROWWISE_DROPMUL || op == GPS_ROWWISE_COLSUM                     ? 0
+                                                                                              : 1;
+  BnView v[2];
+  for (int i = 0; i < nbn; ++i) {
+    const GpsRowwiseBn& b = a->bn[i];
+    const GpsBatchNorm& m = b.bn;
+    GPS_REQUIRE(m.weight && m.bias, GPS_ERR_ARG, "gps_rowwise_stage: bn[%d] needs weight and bias", i);
+    GPS_REQUIRE(b.train || (m.running_mean && m.running_var), GPS_ERR_ARG,
+                "gps_rowwise_stage: bn[%d] in eval mode needs the running statistics", i);
+    GPS_REQUIRE(!b.train || b.saved, GPS_ERR_ARG, "gps_rowwise_stage: bn[%d] in training mode needs saved", i);
+    GPS_REQUIRE(!(bwd || b.train) || b.sums, GPS_ERR_ARG, "gps_rowwise_stage: bn[%d] needs sums", i);
+    const StagePlan P{b.train != 0};
+    const int64_t fwd_rows = bwd ? -1 : (i == 1 && op == GPS_ROWWISE_BN_ACT_RESIDUAL2 ? E : rows);
+    v[i] = bn_view_at(P, b.saved, b.sums, d, a->bn[i].bn, fwd_rows);
+  }
+  DropCfg drop;
+  drop.p = a->p; drop.seed = a->seed; drop.offset = a->offset; drop.site = a->site; drop.offset_dev = a->offset_dev;
+  DropCfg drop2 = drop;
+  drop2.site = a->site2;
+  const Planes outp{(__nv_bfloat16*)a->planes.hi, (__nv_bfloat16*)a->planes.lo, a->planes.ld};
+  const cudaStream_t st = (cudaStream_t)stream;
+  switch (op) {
+    case GPS_ROWWISE_BN_ACT_RESIDUAL:
+      return bn_act_residual(a->x, ldx, a->R, a->out, rows, d, v[0], a->act, drop, a->stats, st, outp);
+    case GPS_ROWWISE_BN_ACT_RESIDUAL2:
+      return bn_act_residual2(a->x, a->R, a->out, rows, v[0], drop, a->stats, a->x2, a->R2, a->out2, E, v[1], drop2, outp,
+                              d, a->act, st);
+    case GPS_ROWWISE_BN_COMBINE:
+      return bn_combine(a->x, v[0], a->x2, v[1], a->out, rows, d, st, outp);
+    case GPS_ROWWISE_BN_BWD_REDUCE:
+      return bn_bwd_reduce(a->g, ldg, a->x, ldx, rows, d, v[0], a->act, drop, a->bn[0].sums, st);
+    case GPS_ROWWISE_BN_BWD_APPLY:
+      return bn_bwd_apply(a->g, ldg, a->x, ldx, rows, d, v[0], a->act, drop, a->bn[0].sums, a->out, ldo,
+                          a->bn[0].bn.grad_weight, a->bn[0].bn.grad_bias, st, a->accumulate != 0, outp);
+    case GPS_ROWWISE_DROPMUL:
+      return dropmul_rows(a->x, a->out, rows, d, drop, a->p2, a->site2, outp, st);
+    default:
+      return colsum(a->x, ldx, rows, d, a->out, st);
+  }
 }
 
 extern "C" void gps_debug_set(int v) { gemm_tc_set_debug(v); }

@@ -966,6 +966,62 @@ typedef struct {
   int32_t precision, reserved;
 } GpsGemmArgs;
 int gps_gemm_epilogue(const GpsGemmArgs* a, int32_t impl, void* stream);
+
+/* One row-wise stage of the layers (csrc/elementwise.cu, and the dropout-only pass of layer.cu), called exactly as the
+ * layers call it, so the BatchNorm apply, statistics finalisation, backward, dropout-gradient and bias-gradient passes
+ * can be tested alone.  Per op, on rows x d (pitch ldx / ldg / ldo where the op reads it, else d; an ld of 0 means d):
+ *   BN_ACT_RESIDUAL   out = R + drop(p, site)(act(BN0(x)))  [+ out's planes]  [stats[0][c] += out, stats[1][c] += out^2]
+ *   BN_ACT_RESIDUAL2  the GatedGCN outputs: out = R + drop(p, site)(act(BN0(x))) over rows with column sums into stats,
+ *                     and out2 = R2 + drop(p, site2)(act(BN1(x2))) over E rows [+ out2's planes], one launch; stats
+ *                     NULL runs the two-launch form (eval mode), as does rows == 0 or E == 0
+ *   BN_COMBINE        out = BN0(x) [+ BN1(x2)]  [+ out's planes]
+ *   BN_BWD_REDUCE     g' = drop(p, site)(g) * act'(BN0(x)) (act -1: none); bn[0].sums [2][d] += (sum g', sum g' xhat)
+ *   BN_BWD_APPLY      out = gamma invstd (g' - S1/n - xhat S2/n) in training, gamma invstd g' in eval, from
+ *                     bn[0].sums = (S1, S2) [+ out's planes]; grad_weight = S2 and grad_bias = S1 (each NULL = not
+ *                     wanted; added with accumulate), zeroed for rows == 0 unless accumulating
+ *   DROPMUL           out = x * drop(p, site) * drop(p2, site2) [+ out's planes]  (each p 0 = none)
+ *   COLSUM            out[c] += sum_r x[r, c]  (float32, the same bits in every run)
+ * A BatchNorm is a GpsRowwiseBn: the module (weight, bias, running statistics, num_batches_tracked, gradients), its
+ * mode (train), its saved [mean | invstd] (2d floats) and its float64 sums [2][d].  A forward op in training mode
+ * finalises mean / invstd from sums (the producer's column sums over its rows), writes them to saved and updates the
+ * running statistics (momentum 0.1, unbiased variance) and num_batches_tracked; in eval mode it reads the running
+ * statistics.  A backward op reads saved in training mode and the running statistics in eval mode.  Dropout draws
+ * gps_dropout_mask(rows, d, p, seed, offset + *offset_dev (offset_dev NULL: + 0), site).  R and R2 may be NULL.
+ * NULL args, an unknown op, a negative size, an ld below d or above it and not a multiple of 4, an ld other than d
+ * where the op takes pitch d, and a NULL pointer the op needs (a tensor over rows, or E, may be NULL when there are
+ * none) are GPS_ERR_ARG, before any CUDA call; d outside the
+ * row-wise stages' range (d % 4 != 0 or d > 4096; DROPMUL and COLSUM: d % 4 != 0) is GPS_ERR_UNSUPPORTED. */
+enum {
+  GPS_ROWWISE_BN_ACT_RESIDUAL = 0, GPS_ROWWISE_BN_ACT_RESIDUAL2 = 1, GPS_ROWWISE_BN_COMBINE = 2,
+  GPS_ROWWISE_BN_BWD_REDUCE = 3, GPS_ROWWISE_BN_BWD_APPLY = 4, GPS_ROWWISE_DROPMUL = 5, GPS_ROWWISE_COLSUM = 6
+};
+typedef struct {
+  GpsBatchNorm bn;
+  float* saved;
+  double* sums;
+  int32_t train, reserved;
+} GpsRowwiseBn;
+typedef struct {
+  int64_t rows, E, d;
+  const float* x; int64_t ldx;
+  const float* x2;
+  const float* g; int64_t ldg;
+  const float* R;
+  const float* R2;
+  float* out; int64_t ldo;
+  float* out2;
+  GpsPlanes planes;
+  GpsRowwiseBn bn[2];
+  int32_t act;
+  float p; int32_t site;
+  float p2; int32_t site2;
+  int32_t accumulate;
+  uint64_t seed, offset;
+  const unsigned long long* offset_dev;
+  double* stats;
+} GpsRowwiseArgs;
+int gps_rowwise_stage(const GpsRowwiseArgs* a, int32_t op, void* stream);
+
 /* number of dense products that fell back from the tensor-core kernels to the exact CUDA-core kernel
  * (unaligned / odd shapes) in this process; with GPS_B200_STRICT=1 in the environment such a fallback is an error */
 unsigned long long gps_fallback_count(void);
