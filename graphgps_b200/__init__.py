@@ -10,6 +10,8 @@ Public surface (mirrors the reference's module boundary, SURVEY.md section 8b):
                   graphgps.layer.gine_conv_layer.GINEConvLayer
     InductiveEdgeHead  drop-in for graphgps.head.inductive_edge.GNNInductiveEdgeHead (PCQM-Contact's link head, dot
                   decoding, ranking metrics on the device)
+    SANGraphHead, GraphormerHead  drop-ins for graphgps.head.san_graph.SANGraphHead and
+                  graphgps.head.graphormer_graph.GraphormerHead (graph-level pooling and prediction)
     GraphBatch    duck-typed stand-in for a collated PyG Batch (PyG is optional)
     make_batch    seeded synthetic batches of the BASELINE shapes
     GPSStack      the L-layer stack of a GPSModel (shared graph structure, plane hand-off, one gradient bucket, capture)
@@ -23,9 +25,10 @@ from .graphormer_bias import BiasEncoder  # noqa: F401
 from .san import SAN2Layer, SANLayer  # noqa: F401
 from .custom_gnn import GatedGCNLayer, GINEConvLayer  # noqa: F401
 from .inductive_edge import InductiveEdgeHead  # noqa: F401
+from .graph_head import GraphormerHead, SANGraphHead  # noqa: F401
 from .dp import GradBucket  # noqa: F401
 from .stack import GPSStack  # noqa: F401
 from .loader import BatchPrefetcher, collate  # noqa: F401
 
-__all__ = ["GPSLayer", "GraphormerLayer", "BiasEncoder", "SANLayer", "SAN2Layer", "GatedGCNLayer", "GINEConvLayer", "InductiveEdgeHead", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
+__all__ = ["GPSLayer", "GraphormerLayer", "BiasEncoder", "SANLayer", "SAN2Layer", "GatedGCNLayer", "GINEConvLayer", "InductiveEdgeHead", "SANGraphHead", "GraphormerHead", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
            "batch_from_lists"]

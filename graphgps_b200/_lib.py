@@ -161,6 +161,27 @@ class GpsLinkHeadPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
 
 
+GRAPH_HEAD = {"san_graph": 0, "graphormer_graph": 1}
+POOLING = {"mean": 0, "add": 1, "graph_token": 2}
+GRAPH_HEAD_MAX_L = 12
+
+
+class GpsGraphHeadArgs(C.Structure):
+    """Graph-prediction head (san_graph.py's SANGraphHead or graphormer_graph.py's GraphormerHead): config, the batch's
+    graph, x, pred and their gradients, ln (GraphormerHead) and fc[l] = FC_layers.l / layers.0, and scratch."""
+    _fields_ = [("kind", C.c_int32), ("pooling", C.c_int32), ("act", C.c_int32), ("L", C.c_int32),
+                ("dim_in", C.c_int64), ("dim_out", C.c_int64),
+                ("training", C.c_int32), ("precision", C.c_int32), ("flags", C.c_int32), ("reserved", C.c_int32),
+                ("seed", C.c_uint64), ("graph", GpsGraph),
+                ("x", _fp), ("pred", _fp), ("grad_pred", _fp), ("grad_x", _fp),
+                ("ln", GpsLinear), ("fc", GpsLinear * (GRAPH_HEAD_MAX_L + 1)),
+                ("saved", _fp), ("saved_bytes", C.c_int64), ("workspace", _fp), ("workspace_bytes", C.c_int64)]
+
+
+class GpsGraphHeadPlan(C.Structure):
+    _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
+
+
 class GpsSanArgs(C.Structure):
     """SAN layer (san_layer.py, variant 0) or SAN2 layer (san2_layer.py, variant 1): config, dropout stream, graph and
     nmax, tensors, scratch, the ten Linears attention.{Q,K,V,Q_2,K_2,E,E_2}, O_h, FFN_h_layer1, FFN_h_layer2,
@@ -272,6 +293,11 @@ SYMBOLS = {
     "gps_link_head_forward": (C.c_int, [C.POINTER(GpsLinkHeadArgs), _fp]),
     "gps_link_head_backward": (C.c_int, [C.POINTER(GpsLinkHeadArgs), _fp]),
     "gps_link_rank_metrics": (C.c_int, [C.POINTER(GpsGraph), _fp, _i64, _i64, _fp, _i32, _fp, _fp, _i64, _fp]),
+    "gps_graph_head_plan": (C.c_int, [C.POINTER(GpsGraphHeadArgs), C.POINTER(GpsGraphHeadPlan)]),
+    "gps_graph_head_forward": (C.c_int, [C.POINTER(GpsGraphHeadArgs), _fp]),
+    "gps_graph_head_backward": (C.c_int, [C.POINTER(GpsGraphHeadArgs), _fp]),
+    "gps_graph_pool_forward": (C.c_int, [C.POINTER(GpsGraph), _i32, _fp, _i64, _fp, _i64, _fp, _i64, _fp]),
+    "gps_graph_pool_backward": (C.c_int, [C.POINTER(GpsGraph), _i32, _fp, _i64, _i64, _fp, _fp]),
     "gps_san_plan": (C.c_int, [C.POINTER(GpsSanArgs), C.POINTER(GpsSanPlan)]),
     "gps_san_forward": (C.c_int, [C.POINTER(GpsSanArgs), _fp]),
     "gps_san_backward": (C.c_int, [C.POINTER(GpsSanArgs), _fp]),

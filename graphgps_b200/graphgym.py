@@ -121,6 +121,41 @@ def install_inductive_edge_head(register_module=None):
     return previous
 
 
+def install_graph_heads(register_module=None):
+    """Set ``register.head_dict['san_graph']`` and ``['graphormer_graph']`` to the H100 heads, so GPSModel, CustomGNN,
+    SANTransformer and GraphormerModel build them for ``gnn.head: san_graph`` / ``graphormer_graph``: each looks its
+    head up in that registry at construction time.  The registered classes have the reference's ``(dim_in, dim_out)``
+    constructor and read ``cfg.model.graph_pooling`` (and, for san_graph, ``cfg.gnn.act``) when they are built.
+
+    Call after ``import graphgps`` and before ``create_model()``.  Returns the classes it replaced, as a dict by name,
+    so a caller can restore them."""
+    from .graph_head import GraphormerHead, SANGraphHead
+    if register_module is None:
+        register_module = importlib.import_module("torch_geometric.graphgym.register")
+
+    def _cfg():
+        return importlib.import_module("torch_geometric.graphgym.config").cfg
+
+    class SANGraphHeadGraphGym(SANGraphHead):
+        """SANGraphHead(dim_in, dim_out) with its pooling and activation from GraphGym's cfg (L = 2, as GraphGym
+        builds it)."""
+
+        def __init__(self, dim_in, dim_out):
+            cfg = _cfg()
+            super().__init__(dim_in, dim_out, graph_pooling=cfg.model.graph_pooling, act=cfg.gnn.act)
+
+    class GraphormerHeadGraphGym(GraphormerHead):
+        """GraphormerHead(dim_in, dim_out) with its pooling from GraphGym's cfg."""
+
+        def __init__(self, dim_in, dim_out):
+            super().__init__(dim_in, dim_out, graph_pooling=_cfg().model.graph_pooling)
+
+    new = {"san_graph": SANGraphHeadGraphGym, "graphormer_graph": GraphormerHeadGraphGym}
+    previous = {n: register_module.head_dict.get(n) for n in new}
+    register_module.head_dict.update(new)
+    return previous
+
+
 def register(name="gpslayer_b200"):
     """Register a LayerConfig-style wrapper under ``name`` in GraphGym's layer registry.
 

@@ -545,6 +545,71 @@ int gps_link_rank_metrics(const GpsGraph* pairs, const float* y, int64_t ld, int
                           int32_t label_bytes, double* stats, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Graph-prediction heads, the head of every graph-level config:
+ *   GPS_GRAPH_HEAD_SAN (graphgps/head/san_graph.py, SANGraphHead(dim_in, dim_out, L)):
+ *     h_0 = pool(x)                           [B, dim_in]
+ *     h_{l+1} = act(h_l W_l^T + b_l), l < L   fc[l]: [dim_in >> (l+1), dim_in >> l]
+ *     pred = h_L W_L^T + b_L                  fc[L]: [dim_out, dim_in >> L]
+ *   GPS_GRAPH_HEAD_GRAPHORMER (graphgps/head/graphormer_graph.py, GraphormerHead(dim_in, dim_out)), L = 0:
+ *     pred = pool(LayerNorm(x)) W^T + b       ln: gamma / beta [dim_in], eps 1e-5; fc[0]: [dim_out, dim_in]
+ * Pooling over the graphs of `graph` (graph_ptr [B+1] read; rows sorted by graph): mean = per-graph sum / max(count, 1),
+ * add = per-graph sum, graph_token = each graph's first row; an empty graph gives a zero row.  Under graph_token the
+ * LayerNorm runs on the B token rows only (it is row-wise), so grad_x is zero off the token rows; an empty graph's row
+ * stays zero after it, as pooling after the LayerNorm leaves it, so its pred is b and it adds nothing to ln's gradients.
+ * Built: SAN head with mean / add / graph_token and act relu / gelu (exact erf), any L >= 0 with dim_in >> L >= 1;
+ * Graphormer head with graph_token and dim_in % 4 == 0; 1 <= dim_in, dim_out <= 4096.  Anything else is
+ * GPS_ERR_UNSUPPORTED, bad sizes or missing pointers GPS_ERR_ARG, all before any CUDA call.
+ * Widths run at the next multiple of 8 with zero pad columns.  Per-graph sums walk each graph's rows in a fixed order
+ * (a graph spread over several CTAs is combined from their partials in row order) and the weight gradients take the
+ * deterministic split-K path: no float atomics in fp32, two runs give the same bits.  Backward writes grad_x [N, dim_in]
+ * whole and every parameter gradient (the head has no dropout and no running statistics: training is not read).
+ * ---------------------------------------------------------------------------------------- */
+enum { GPS_GRAPH_HEAD_SAN = 0, GPS_GRAPH_HEAD_GRAPHORMER = 1 };
+enum { GPS_POOL_MEAN = 0, GPS_POOL_ADD = 1, GPS_POOL_GRAPH_TOKEN = 2 };
+#define GPS_GRAPH_HEAD_MAX_L 12 /* dim_in <= 4096 leaves a nonzero width for L <= 12 */
+
+typedef struct {
+  int32_t kind;              /* GPS_GRAPH_HEAD_*                                              */
+  int32_t pooling;           /* GPS_POOL_*                                                    */
+  int32_t act;               /* GPS_ACT_* (SAN head; not read by the Graphormer head)         */
+  int32_t L;                 /* hidden layers of the SAN head; 0 for the Graphormer head      */
+  int64_t dim_in, dim_out;
+  int32_t training;          /* not read                                                      */
+  int32_t precision;         /* GPS_PREC_*                                                    */
+  int32_t flags;             /* reserved, 0                                                   */
+  int32_t reserved;
+  uint64_t seed;             /* unused (the head has no dropout)                              */
+  GpsGraph graph;            /* N = rows of x, B = graphs, graph_ptr                          */
+  const float* x;            /* [N, dim_in]                                                   */
+  float* pred;               /* [B, dim_out] (forward)                                        */
+  const float* grad_pred;    /* [B, dim_out] (backward)                                       */
+  float* grad_x;             /* [N, dim_in] (backward)                                        */
+  GpsLinear ln;              /* Graphormer head: ln.weight / ln.bias [dim_in] and their grads */
+  GpsLinear fc[GPS_GRAPH_HEAD_MAX_L + 1]; /* FC_layers.{0..L} / layers.0, with their grads    */
+  void* saved; int64_t saved_bytes;         /* forward -> backward                            */
+  void* workspace; int64_t workspace_bytes; /* transient                                      */
+} GpsGraphHeadArgs;
+
+typedef struct {
+  int64_t saved_bytes;
+  int64_t fwd_workspace_bytes;
+  int64_t bwd_workspace_bytes;
+} GpsGraphHeadPlan;
+
+/* Sizes for args (only kind, pooling, act, L, the widths, precision and the graph's N and B are read). */
+int gps_graph_head_plan(const GpsGraphHeadArgs* args, GpsGraphHeadPlan* plan);
+int gps_graph_head_forward(const GpsGraphHeadArgs* args, void* stream);
+int gps_graph_head_backward(const GpsGraphHeadArgs* args, void* stream);
+/* Stage entries: the pooling alone.  Forward writes out [B, d] at pitch ldo >= d (the columns beyond d are not
+ * written); mean and add need a 16-byte aligned workspace >= 8 * ceil(N / 64) * round_up(d, 4) bytes (per-CTA
+ * partials), graph_token none.
+ * Backward writes grad_x [N, d] whole from grad_out [B, d] at pitch ldg >= d. */
+int gps_graph_pool_forward(const GpsGraph* graph, int32_t pooling, const float* x, int64_t d, float* out, int64_t ldo,
+                           void* workspace, int64_t workspace_bytes, void* stream);
+int gps_graph_pool_backward(const GpsGraph* graph, int32_t pooling, const float* grad_out, int64_t ldg, int64_t d,
+                            float* grad_x, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * SAN layer (graphgps/layer/san_layer.py:10-210), the building block of SANTransformer, as every shipped config runs
  * it (full_graph, batch_norm, residual, no layer_norm, no Linear biases in the attention, in_dim == out_dim == d):
  *   [Q|K|V|Q2|K2] = x W^T, E = edge_attr W_E^T, E2 = W_E2 fake_edge_emb
