@@ -263,6 +263,24 @@ class GpsRowwiseArgs(C.Structure):
                 ("stats", _fp)]
 
 
+# gps_attention_stage ops
+ATTN = {"fwd": 0, "fwd_tc": 1, "bwd": 2}
+
+
+class GpsAttnStageArgs(C.Structure):
+    """One softmax-attention stage (gps_attention_stage): graph, heads, head dim, Q / K / V or the qkv planes, O with its
+    planes and lse, the backward's dO, delta, dQ / dK / dV with their planes, the bias and the dropout stream."""
+    _fields_ = [("graph", GpsGraph), ("heads", C.c_int64), ("hd", C.c_int64),
+                ("Q", _fp), ("K", _fp), ("V", _fp), ("ld", C.c_int64),
+                ("qkv", GpsPlanes), ("precision", C.c_int32), ("reserved", C.c_int32),
+                ("O", _fp), ("ldo", C.c_int64), ("O_planes", GpsPlanes), ("lse", _fp),
+                ("dO", _fp), ("delta", _fp), ("dQ", _fp), ("dK", _fp), ("dV", _fp), ("ldg", C.c_int64),
+                ("dQ_planes", GpsPlanes), ("dK_planes", GpsPlanes), ("dV_planes", GpsPlanes),
+                ("bias", C.POINTER(GpsAttnBias)),
+                ("p_drop", C.c_float), ("reserved2", C.c_int32), ("seed", C.c_uint64), ("offset", C.c_uint64),
+                ("offset_dev", _fp)]
+
+
 class GpsLayerPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64),
                 ("bwd_workspace_bytes", C.c_int64), ("wplanes_bytes", C.c_int64)]
@@ -369,6 +387,7 @@ SYMBOLS = {
     "gps_attention_backward_biased": (C.c_int, [C.POINTER(GpsGraph), _i64, _i64, _fp, _fp, _fp, _i64, _fp, _fp, _i64,
                                                 _fp, _fp, _fp, _fp, _fp, _i64, _f32, _u64, _u64, C.POINTER(GpsAttnBias),
                                                 _fp]),
+    "gps_attention_stage": (C.c_int, [C.POINTER(GpsAttnStageArgs), _i32, _fp]),
     "gps_dropout_mask": (C.c_int, [_fp, _i64, _i64, _f32, _u64, _u64, _i32, _fp]),
     "gps_to_planes": (C.c_int, [_fp, _i64, _i64, _i64, _fp, _fp, _i64, _fp]),
     "gps_gemm_planes": (C.c_int, [_fp, _fp, _i64, _i32, _fp, _fp, _i64, _i32, _fp, _i64, _fp, _fp, _i64, _i64, _i64, _i64,

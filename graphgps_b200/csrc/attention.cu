@@ -501,9 +501,9 @@ int attention_bwd(const GpsGraph& g, int64_t heads, int64_t hd, const float* Q, 
   a.Q = Q; a.K = K; a.V = V; a.ld = ld; a.Oc = O; a.dO = dO; a.ldo = ldo; a.lsec = lse;
   a.delta = delta; a.deltac = delta; a.dQ = dQ; a.dK = dK; a.dV = dV; a.ldg = ldg;
   a.scale = 1.f / sqrtf((float)hd); a.p_drop = p_drop; a.seed = seed; a.offset = offset;
+  GPS_REQUIRE(a.hd > 0 && a.hd <= 192, GPS_ERR_UNSUPPORTED, "attention: head dim %d must be in 1..192", a.hd);
   if (a.gbias)   // entries of padded rows / columns stay 0; the kernel writes every in-graph (query, key) pair
     GPS_CUDA(cudaMemsetAsync(a.gbias, 0, (size_t)(g.B * heads * a.nmax * a.nmax) * sizeof(float), stream));
-  GPS_REQUIRE(a.hd > 0 && a.hd <= 192, GPS_ERR_UNSUPPORTED, "attention: head dim %d must be in 1..192", a.hd);
   if (a.N == 0) return GPS_OK;
   const int64_t nt = (int64_t)a.N * a.H * 8;
   if (attn_vec4(a, KBWD)) k_attn_delta<4><<<(unsigned)ceil_div(nt, (int64_t)256), 256, 0, stream>>>(a);

@@ -2061,58 +2061,161 @@ extern "C" int gps_performer_features_backward(const GpsGraph* g, int64_t H, int
                            (cudaStream_t)stream);
 }
 
+// The attention stages: one argument contract for gps_attention_stage and the six entry points that are calls of it.
+static Planes attn_planes(const GpsPlanes& p) { return Planes{(__nv_bfloat16*)p.hi, (__nv_bfloat16*)p.lo, p.ld}; }
+
+static int attn_check_planes(const GpsPlanes& p, int64_t min_ld, const char* name) {
+  if (!p.hi && !p.lo) return GPS_OK;
+  GPS_REQUIRE(p.hi, GPS_ERR_ARG, "gps_attention_stage: %s has lo without hi", name);
+  GPS_REQUIRE(p.ld >= min_ld, GPS_ERR_ARG, "gps_attention_stage: %s pitch %lld is below %lld", name, (long long)p.ld,
+              (long long)min_ld);
+  GPS_REQUIRE(p.ld % 8 == 0, GPS_ERR_UNSUPPORTED, "gps_attention_stage: %s pitch %lld is not a multiple of 8", name,
+              (long long)p.ld);
+  return GPS_OK;
+}
+
+static int attn_check(const GpsAttnStageArgs* a, int32_t op) {
+  GPS_REQUIRE(a, GPS_ERR_ARG, "gps_attention_stage: null args");
+  GPS_REQUIRE(op == GPS_ATTN_FWD || op == GPS_ATTN_FWD_TC || op == GPS_ATTN_BWD, GPS_ERR_ARG,
+              "gps_attention_stage: unknown op %d", op);
+  const GpsGraph& g = a->graph;
+  GPS_REQUIRE(g.N >= 0 && g.B >= 0 && g.N <= 0x7FFFFFFF && g.B <= 0x7FFFFFFF, GPS_ERR_ARG,
+              "gps_attention_stage: N %lld and B %lld must lie in [0, 2^31)", (long long)g.N, (long long)g.B);
+  GPS_REQUIRE(g.N == 0 || (g.B >= 1 && g.graph_ptr), GPS_ERR_ARG, "gps_attention_stage: %lld nodes need B >= 1 and graph_ptr",
+              (long long)g.N);
+  GPS_REQUIRE(a->heads >= 1, GPS_ERR_ARG, "gps_attention_stage: heads must be >= 1 (got %lld)", (long long)a->heads);
+  GPS_REQUIRE(a->p_drop >= 0.f && a->p_drop < 1.f, GPS_ERR_ARG, "gps_attention_stage: p_drop %g is not in [0, 1)",
+              (double)a->p_drop);
+  if (a->bias) {
+    GPS_REQUIRE(a->bias->bias, GPS_ERR_ARG, "gps_attention_stage: null attention bias");
+    GPS_REQUIRE(a->bias->nmax >= 1, GPS_ERR_ARG, "gps_attention_stage: nmax must be >= 1 (got %lld)",
+                (long long)a->bias->nmax);
+  }
+  const bool tc = op == GPS_ATTN_FWD_TC, bwd = op == GPS_ATTN_BWD;
+  GPS_REQUIRE(a->O && a->lse, GPS_ERR_ARG, "gps_attention_stage: op %d needs O and lse", op);
+  if (tc) {
+    GPS_REQUIRE(a->qkv.hi, GPS_ERR_ARG, "gps_attention_stage: FWD_TC needs the qkv planes");
+    GPS_REQUIRE(a->precision == GPS_PREC_FP32 || a->precision == GPS_PREC_BF16, GPS_ERR_ARG,
+                "gps_attention_stage: precision %d is not GPS_PREC_FP32 or GPS_PREC_BF16", a->precision);
+  } else {
+    GPS_REQUIRE(a->Q && a->K && a->V, GPS_ERR_ARG, "gps_attention_stage: op %d needs Q, K and V", op);
+  }
+  GPS_REQUIRE(!bwd || (a->dO && a->delta && a->dQ && a->dK && a->dV), GPS_ERR_ARG,
+              "gps_attention_stage: BWD needs dO, delta, dQ, dK and dV");
+  GPS_REQUIRE(a->hd >= 1 && a->hd <= 192, GPS_ERR_UNSUPPORTED, "gps_attention_stage: head dim %lld must be in 1..192",
+              (long long)a->hd);
+  const int64_t D = a->heads * a->hd;
+  GPS_REQUIRE(tc || a->ld >= D, GPS_ERR_ARG, "gps_attention_stage: ld %lld is below heads * hd = %lld", (long long)a->ld,
+              (long long)D);
+  GPS_REQUIRE(a->ldo >= D, GPS_ERR_ARG, "gps_attention_stage: ldo %lld is below heads * hd = %lld", (long long)a->ldo,
+              (long long)D);
+  GPS_REQUIRE(!bwd || a->ldg >= D, GPS_ERR_ARG, "gps_attention_stage: ldg %lld is below heads * hd = %lld",
+              (long long)a->ldg, (long long)D);
+  if (bwd) {
+    GPS_TRY(attn_check_planes(a->dQ_planes, D, "dQ_planes"));
+    GPS_TRY(attn_check_planes(a->dK_planes, D, "dK_planes"));
+    GPS_TRY(attn_check_planes(a->dV_planes, D, "dV_planes"));
+  } else {
+    GPS_TRY(attn_check_planes(a->O_planes, D, "O_planes"));
+  }
+  if (tc) {
+    GPS_REQUIRE(attention_tc_supported(a->hd), GPS_ERR_UNSUPPORTED,
+                "gps_attention_stage: FWD_TC takes head dims that are a multiple of 4 up to 128 (got %lld)",
+                (long long)a->hd);
+    GPS_TRY(attn_check_planes(a->qkv, 3 * a->heads * attention_tc_hd_pad(a->hd), "qkv"));
+    GPS_REQUIRE(a->precision != GPS_PREC_FP32 || a->qkv.lo, GPS_ERR_UNSUPPORTED,
+                "gps_attention_stage: FWD_TC in GPS_PREC_FP32 needs qkv.lo");
+  }
+  return GPS_OK;
+}
+
+extern "C" int gps_attention_stage(const GpsAttnStageArgs* a, int32_t op, void* stream) {
+  GPS_TRY(attn_check(a, op));
+  const cudaStream_t st = (cudaStream_t)stream;
+  switch (op) {
+    case GPS_ATTN_FWD:
+      return attention_fwd(a->graph, a->heads, a->hd, a->Q, a->K, a->V, a->ld, a->O, a->ldo, a->lse, a->p_drop, a->seed,
+                           a->offset, st, a->offset_dev, attn_planes(a->O_planes), a->bias);
+    case GPS_ATTN_FWD_TC:
+      return attention_tc_fwd(a->graph, a->heads, a->hd, attn_planes(a->qkv), a->O, a->ldo, attn_planes(a->O_planes),
+                              a->lse, a->p_drop, a->seed, a->offset, a->offset_dev, a->precision, st, a->bias);
+    default:
+      return attention_bwd(a->graph, a->heads, a->hd, a->Q, a->K, a->V, a->ld, a->O, a->dO, a->ldo, a->lse, a->delta,
+                           a->dQ, a->dK, a->dV, a->ldg, a->p_drop, a->seed, a->offset, st, a->offset_dev,
+                           attn_planes(a->dQ_planes), attn_planes(a->dK_planes), attn_planes(a->dV_planes), a->bias);
+  }
+}
+
+// the six fixed-signature entry points: the stage call with the fields they take; the biased ones require a bias
+static GpsAttnStageArgs attn_args(const GpsGraph* g, int64_t heads, int64_t hd, float p_drop, uint64_t seed,
+                                  uint64_t offset, const GpsAttnBias* bias) {
+  GpsAttnStageArgs a{};
+  a.graph = *g;
+  a.heads = heads; a.hd = hd; a.p_drop = p_drop; a.seed = seed; a.offset = offset; a.bias = bias;
+  return a;
+}
+static int attn_fwd_call(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q, const float* K, const float* V,
+                         int64_t ld, float* O, int64_t ldo, float* lse, float p_drop, uint64_t seed, uint64_t offset,
+                         const GpsAttnBias* bias, void* stream) {
+  GPS_REQUIRE(g, GPS_ERR_ARG, "gps_attention_stage: null graph");
+  GpsAttnStageArgs a = attn_args(g, heads, hd, p_drop, seed, offset, bias);
+  a.Q = Q; a.K = K; a.V = V; a.ld = ld; a.O = O; a.ldo = ldo; a.lse = lse;
+  return gps_attention_stage(&a, GPS_ATTN_FWD, stream);
+}
+static int attn_fwd_tc_call(const GpsGraph* g, int64_t heads, int64_t hd, const void* qkv_hi, const void* qkv_lo,
+                            int64_t ld, float* O, int64_t ldo, float* lse, float p_drop, uint64_t seed, uint64_t offset,
+                            int32_t precision, const GpsAttnBias* bias, void* stream) {
+  GPS_REQUIRE(g, GPS_ERR_ARG, "gps_attention_stage: null graph");
+  GpsAttnStageArgs a = attn_args(g, heads, hd, p_drop, seed, offset, bias);
+  a.qkv = GpsPlanes{const_cast<void*>(qkv_hi), const_cast<void*>(qkv_lo), ld};
+  a.precision = precision; a.O = O; a.ldo = ldo; a.lse = lse;
+  return gps_attention_stage(&a, GPS_ATTN_FWD_TC, stream);
+}
+static int attn_bwd_call(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q, const float* K, const float* V,
+                         int64_t ld, const float* O, const float* dO, int64_t ldo, const float* lse, float* delta,
+                         float* dQ, float* dK, float* dV, int64_t ldg, float p_drop, uint64_t seed, uint64_t offset,
+                         const GpsAttnBias* bias, void* stream) {
+  GPS_REQUIRE(g, GPS_ERR_ARG, "gps_attention_stage: null graph");
+  GpsAttnStageArgs a = attn_args(g, heads, hd, p_drop, seed, offset, bias);
+  a.Q = Q; a.K = K; a.V = V; a.ld = ld; a.O = const_cast<float*>(O); a.dO = dO; a.ldo = ldo;
+  a.lse = const_cast<float*>(lse); a.delta = delta; a.dQ = dQ; a.dK = dK; a.dV = dV; a.ldg = ldg;
+  return gps_attention_stage(&a, GPS_ATTN_BWD, stream);
+}
+
 extern "C" int gps_attention_forward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q, const float* K,
                                      const float* V, int64_t ld, float* O, int64_t ldo, float* lse, float p_drop,
                                      uint64_t seed, uint64_t offset, void* stream) {
-  GPS_REQUIRE(g && Q && K && V && O && lse, GPS_ERR_ARG, "attention_forward: null argument");
-  return attention_fwd(*g, heads, hd, Q, K, V, ld, O, ldo, lse, p_drop, seed, offset, (cudaStream_t)stream);
+  return attn_fwd_call(g, heads, hd, Q, K, V, ld, O, ldo, lse, p_drop, seed, offset, nullptr, stream);
 }
 
 extern "C" int gps_attention_forward_tc(const GpsGraph* g, int64_t heads, int64_t hd, const void* qkv_hi, const void* qkv_lo,
                                         int64_t ld, float* O, int64_t ldo, float* lse, float p_drop, uint64_t seed,
                                         uint64_t offset, int32_t precision, void* stream) {
-  GPS_REQUIRE(g && qkv_hi && O && lse, GPS_ERR_ARG, "attention_forward_tc: null argument");
-  Planes q{(__nv_bfloat16*)qkv_hi, (__nv_bfloat16*)qkv_lo, ld};
-  return attention_tc_fwd(*g, heads, hd, q, O, ldo, Planes(), lse, p_drop, seed, offset, nullptr, precision,
-                          (cudaStream_t)stream);
+  return attn_fwd_tc_call(g, heads, hd, qkv_hi, qkv_lo, ld, O, ldo, lse, p_drop, seed, offset, precision, nullptr, stream);
 }
 
 extern "C" int gps_attention_backward(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q, const float* K,
                                       const float* V, int64_t ld, const float* O, const float* dO, int64_t ldo,
                                       const float* lse, float* delta, float* dQ, float* dK, float* dV, int64_t ldg,
                                       float p_drop, uint64_t seed, uint64_t offset, void* stream) {
-  GPS_REQUIRE(g && Q && K && V && O && dO && lse && delta && dQ && dK && dV, GPS_ERR_ARG,
-              "attention_backward: null argument");
-  return attention_bwd(*g, heads, hd, Q, K, V, ld, O, dO, ldo, lse, delta, dQ, dK, dV, ldg, p_drop, seed, offset,
-                       (cudaStream_t)stream);
-}
-
-// the three attention stages with an attention bias
-static int check_stage_bias(const GpsAttnBias* bias, const char* what) {
-  GPS_REQUIRE(bias && bias->bias, GPS_ERR_ARG, "%s: null attention bias", what);
-  GPS_REQUIRE(bias->nmax >= 1, GPS_ERR_ARG, "%s: nmax must be >= 1 (got %lld)", what, (long long)bias->nmax);
-  return GPS_OK;
+  return attn_bwd_call(g, heads, hd, Q, K, V, ld, O, dO, ldo, lse, delta, dQ, dK, dV, ldg, p_drop, seed, offset, nullptr,
+                       stream);
 }
 
 extern "C" int gps_attention_forward_biased(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q,
                                             const float* K, const float* V, int64_t ld, float* O, int64_t ldo,
                                             float* lse, float p_drop, uint64_t seed, uint64_t offset,
                                             const GpsAttnBias* bias, void* stream) {
-  GPS_REQUIRE(g && Q && K && V && O && lse, GPS_ERR_ARG, "attention_forward_biased: null argument");
-  GPS_TRY(check_stage_bias(bias, "attention_forward_biased"));
-  return attention_fwd(*g, heads, hd, Q, K, V, ld, O, ldo, lse, p_drop, seed, offset, (cudaStream_t)stream, nullptr,
-                       Planes(), bias);
+  GPS_REQUIRE(bias, GPS_ERR_ARG, "gps_attention_forward_biased: null attention bias");
+  return attn_fwd_call(g, heads, hd, Q, K, V, ld, O, ldo, lse, p_drop, seed, offset, bias, stream);
 }
 
 extern "C" int gps_attention_forward_tc_biased(const GpsGraph* g, int64_t heads, int64_t hd, const void* qkv_hi,
                                                const void* qkv_lo, int64_t ld, float* O, int64_t ldo, float* lse,
                                                float p_drop, uint64_t seed, uint64_t offset, int32_t precision,
                                                const GpsAttnBias* bias, void* stream) {
-  GPS_REQUIRE(g && qkv_hi && O && lse, GPS_ERR_ARG, "attention_forward_tc_biased: null argument");
-  GPS_TRY(check_stage_bias(bias, "attention_forward_tc_biased"));
-  Planes q{(__nv_bfloat16*)qkv_hi, (__nv_bfloat16*)qkv_lo, ld};
-  return attention_tc_fwd(*g, heads, hd, q, O, ldo, Planes(), lse, p_drop, seed, offset, nullptr, precision,
-                          (cudaStream_t)stream, bias);
+  GPS_REQUIRE(bias, GPS_ERR_ARG, "gps_attention_forward_tc_biased: null attention bias");
+  return attn_fwd_tc_call(g, heads, hd, qkv_hi, qkv_lo, ld, O, ldo, lse, p_drop, seed, offset, precision, bias, stream);
 }
 
 extern "C" int gps_attention_backward_biased(const GpsGraph* g, int64_t heads, int64_t hd, const float* Q,
@@ -2120,11 +2223,9 @@ extern "C" int gps_attention_backward_biased(const GpsGraph* g, int64_t heads, i
                                              const float* dO, int64_t ldo, const float* lse, float* delta, float* dQ,
                                              float* dK, float* dV, int64_t ldg, float p_drop, uint64_t seed,
                                              uint64_t offset, const GpsAttnBias* bias, void* stream) {
-  GPS_REQUIRE(g && Q && K && V && O && dO && lse && delta && dQ && dK && dV, GPS_ERR_ARG,
-              "attention_backward_biased: null argument");
-  GPS_TRY(check_stage_bias(bias, "attention_backward_biased"));
-  return attention_bwd(*g, heads, hd, Q, K, V, ld, O, dO, ldo, lse, delta, dQ, dK, dV, ldg, p_drop, seed, offset,
-                       (cudaStream_t)stream, nullptr, Planes(), Planes(), Planes(), bias);
+  GPS_REQUIRE(bias, GPS_ERR_ARG, "gps_attention_backward_biased: null attention bias");
+  return attn_bwd_call(g, heads, hd, Q, K, V, ld, O, dO, ldo, lse, delta, dQ, dK, dV, ldg, p_drop, seed, offset, bias,
+                       stream);
 }
 
 extern "C" int gps_dropout_mask(float* mask, int64_t rows, int64_t cols, float p, uint64_t seed, uint64_t offset,

@@ -977,6 +977,38 @@ int gps_attention_backward_biased(const GpsGraph* g, int64_t heads, int64_t hd, 
                                   const float* V, int64_t ld, const float* O, const float* dO, int64_t ldo,
                                   const float* lse, float* delta, float* dQ, float* dK, float* dV, int64_t ldg,
                                   float p_drop, uint64_t seed, uint64_t offset, const GpsAttnBias* bias, void* stream);
+/* One softmax-attention stage with every field the layers pass, so each can be tested alone.  The six entry points
+ * above are this call with the fields they do not take left zero; all seven share one argument contract.
+ *   FWD     CUDA-core forward: O, lse from Q, K, V (pitch ld) [+ O_planes]
+ *   FWD_TC  wgmma forward: O, lse from the qkv planes in the per-head padded layout (gps_attention_forward_tc)
+ *           [+ O_planes]; precision GPS_PREC_FP32 reads qkv.lo, GPS_PREC_BF16 ignores it
+ *   BWD     delta, dQ, dK, dV (pitch ldg) [+ their planes] from Q, K, V, O, dO (pitch ldo), lse; bias->grad_bias
+ *           written whole when given
+ * bias NULL = unbiased.  Dropout on the probabilities draws Philox site 16 + head at offset + *offset_dev (offset_dev
+ * NULL: + 0).  GPS_ERR_ARG, before any CUDA call: NULL args, an unknown op, a negative N or B, N > 0 with B < 1 or no
+ * graph_ptr, heads < 1, a NULL tensor the op reads or writes, ld / ldo / ldg below heads * hd (the op's pitches), an
+ * output plane pitch below heads * hd or a qkv plane pitch below 3 * heads * hd_pad, lo planes without hi, precision
+ * other than GPS_PREC_FP32 / GPS_PREC_BF16, p_drop outside [0, 1) or NaN, a bias with bias->bias NULL or nmax < 1.
+ * GPS_ERR_UNSUPPORTED: hd outside 1..192 (FWD_TC: not a multiple of 4 or above 128), a plane pitch that is not a
+ * multiple of 8, and FWD_TC in GPS_PREC_FP32 without qkv.lo. */
+enum { GPS_ATTN_FWD = 0, GPS_ATTN_FWD_TC = 1, GPS_ATTN_BWD = 2 };
+typedef struct {
+  GpsGraph graph;
+  int64_t heads, hd;
+  const float* Q; const float* K; const float* V; int64_t ld;
+  GpsPlanes qkv; int32_t precision, reserved;
+  float* O; int64_t ldo;
+  GpsPlanes O_planes;
+  float* lse;
+  const float* dO; float* delta;
+  float* dQ; float* dK; float* dV; int64_t ldg;
+  GpsPlanes dQ_planes, dK_planes, dV_planes;
+  const GpsAttnBias* bias;
+  float p_drop; int32_t reserved2;
+  uint64_t seed, offset;
+  const unsigned long long* offset_dev;
+} GpsAttnStageArgs;
+int gps_attention_stage(const GpsAttnStageArgs* a, int32_t op, void* stream);
 
 /* Operand "planes" of the TMA-fed wgmma GEMM (csrc/gemm_tma.cu).  A plane pair is the bf16 image of an
  * fp32 matrix: hi = bf16(v), lo = bf16(v - hi), both plain row-major with pitch ldp (elements, multiple of 8); lo may

@@ -16,7 +16,7 @@ INCLUDE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "includ
 STRUCTS = [_lib.GpsGraph, _lib.GpsBatchNorm, _lib.GpsLinear, _lib.GpsPlanes, _lib.GpsAttnBias, _lib.GpsGat,
            _lib.GpsGenConv, _lib.GpsPna, _lib.GpsBigBird, _lib.GpsLayerArgs, _lib.GpsLayerPlan, _lib.GpsGraphormerArgs,
            _lib.GpsGraphormerPlan, _lib.GpsSanArgs, _lib.GpsSanPlan, _lib.GpsCustomGnnArgs, _lib.GpsCustomGnnPlan,
-           _lib.GpsGemmArgs, _lib.GpsRowwiseBn, _lib.GpsRowwiseArgs]
+           _lib.GpsGemmArgs, _lib.GpsRowwiseBn, _lib.GpsRowwiseArgs, _lib.GpsAttnStageArgs]
 
 # header enum prefix -> the _lib name -> value map it must equal (keys upper-cased, "Custom" dropped: CustomGatedGCN is
 # GPS_LOCAL_GATEDGCN)
@@ -30,6 +30,7 @@ ENUMS = {
     "GPS_BIGBIRD_": _lib.BIGBIRD_ACT,
     "GPS_CUSTOM_": {"GATEDGCN": _lib.CUSTOM_GATEDGCN, "GINE": _lib.CUSTOM_GINE},
     "GPS_ROWWISE_": _lib.ROWWISE,
+    "GPS_ATTN_": _lib.ATTN,
 }
 
 

@@ -14,6 +14,7 @@ import graphgps_b200
 from graphgps_b200 import _lib
 from graphgps_b200.batch import batch_from_lists, make_batch
 from graphgps_b200.graph import graph_of
+from attention_reference import padded_planes
 from biased_oracle import OracleGPSLayerBiased
 from biased_util import PAD_VALUE, biased_batch, biased_names, compare_biased, load_biased, make_bias, run_biased
 from util import _nan, _stream, pin_dropout_counter, rel_err, rel_l2
@@ -110,16 +111,6 @@ def test_biased_attention_cuda_core_matches_fp64(case, H, hd, kind):
     assert torch.equal(gb, gb2)                                  # no atomics: the same bits in every run
 
 
-def _padded_planes(QKV, H, hd):
-    N = QKV.shape[0]
-    hp = (hd + 15) // 16 * 16
-    x = torch.zeros(N, 3 * H, hp, device=QKV.device)
-    x[:, :, :hd] = QKV.view(N, 3 * H, hd)
-    x = x.view(N, 3 * H * hp)
-    hi = x.to(torch.bfloat16)
-    return torch.stack([hi, (x - hi.float()).to(torch.bfloat16)]).contiguous(), 3 * H * hp
-
-
 @pytest.mark.parametrize("H,hd", [(4, 16), (4, 64), (2, 128), (4, 76)])
 @pytest.mark.parametrize("precision", [0, 1])
 def test_biased_attention_tc_matches_fp64(H, hd, precision):
@@ -134,7 +125,7 @@ def test_biased_attention_tc_matches_fp64(H, hd, precision):
     torch.manual_seed(12)
     QKV = torch.randn(N, 3 * D, device=DEV)
     ab = make_bias(b.batch, b.num_graphs, H, 5).to(DEV)
-    planes, ld = _padded_planes(QKV, H, hd)
+    planes, ld = padded_planes(QKV, H, hd)
     O, lse = _nan(N, D), _nan(N, H)
     bias = _lib.GpsAttnBias(ab.data_ptr(), gs.nmax, 0)
     _lib.check(lib.gps_attention_forward_tc_biased(C.byref(gs.desc), H, hd, planes[0].data_ptr(),

@@ -101,56 +101,6 @@ def test_gatedgcn_aggregate_forward(shape, d):
     assert rel_err(se[0].cpu(), e_ij.sum(0).cpu()) < 1e-4 and rel_err(se[1].cpu(), (e_ij ** 2).sum(0).cpu()) < 1e-4
 
 
-def _dense_attention_ref(Q, K, V, ptr, H):
-    outs = []
-    N, D = Q.shape
-    hd = D // H
-    for g in range(len(ptr) - 1):
-        s, e = int(ptr[g]), int(ptr[g + 1])
-        if e == s:
-            continue
-        q = Q[s:e].view(e - s, H, hd).transpose(0, 1)
-        k = K[s:e].view(e - s, H, hd).transpose(0, 1)
-        v = V[s:e].view(e - s, H, hd).transpose(0, 1)
-        p = torch.softmax(q @ k.transpose(1, 2) / hd ** 0.5, dim=-1)
-        outs.append((p @ v).transpose(0, 1).reshape(e - s, D))
-    return torch.cat(outs)
-
-
-@pytest.mark.parametrize("shape,H,hd,B", [("pcqm4m-small", 4, 76, 32), ("zinc-gatedgcn", 4, 16, 8),
-                                          ("pcqm4m-small", 16, 24, 16), ("code2", 4, 64, 6)])
-def test_attention_forward_backward(shape, H, hd, B):
-    lib = _lib.load()
-    D = H * hd
-    b = make_batch(shape, seed=4, dim=8, num_graphs=B).to(DEV)
-    gs = graph_of(b)
-    N = b.num_nodes
-    QKV = torch.randn(N, 3 * D, device=DEV)
-    O = torch.empty(N, D, device=DEV)
-    lse = torch.empty(N, H, device=DEV)
-    base = QKV.data_ptr()
-    rc = lib.gps_attention_forward(C.byref(gs.desc), H, hd, base, base + 4 * D, base + 8 * D, 3 * D, O.data_ptr(), D,
-                                   lse.data_ptr(), 0.0, 0, 0, _stream())
-    _lib.check(rc, "attention_forward")
-    q = QKV[:, :D].double().requires_grad_(True)
-    k = QKV[:, D:2 * D].double().requires_grad_(True)
-    v = QKV[:, 2 * D:].double().requires_grad_(True)
-    ref = _dense_attention_ref(q, k, v, b.ptr, H)
-    assert rel_err(O.cpu(), ref.detach().cpu()) < 2e-5
-    dO = torch.randn(N, D, device=DEV)
-    ref.backward(dO.double())
-    dQKV = torch.empty(N, 3 * D, device=DEV)
-    delta = torch.empty(N, H, device=DEV)
-    gb = dQKV.data_ptr()
-    rc = lib.gps_attention_backward(C.byref(gs.desc), H, hd, base, base + 4 * D, base + 8 * D, 3 * D, O.data_ptr(),
-                                    dO.data_ptr(), D, lse.data_ptr(), delta.data_ptr(), gb, gb + 4 * D, gb + 8 * D,
-                                    3 * D, 0.0, 0, 0, _stream())
-    _lib.check(rc, "attention_backward")
-    assert rel_err(dQKV[:, :D].cpu(), q.grad.cpu()) < 5e-5
-    assert rel_err(dQKV[:, D:2 * D].cpu(), k.grad.cpu()) < 5e-5
-    assert rel_err(dQKV[:, 2 * D:].cpu(), v.grad.cpu()) < 5e-5
-
-
 # ------------------------------------------------------------------------------- whole layer
 def _build(cfg, precision="fp32", **kw):
     layer = graphgps_b200.GPSLayer(cfg["d"], cfg["local"], cfg["glob"], cfg["heads"], act=cfg["act"],
