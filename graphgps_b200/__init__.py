@@ -12,6 +12,8 @@ Public surface (mirrors the reference's module boundary, SURVEY.md section 8b):
                   decoding, ranking metrics on the device)
     SANGraphHead, GraphormerHead  drop-ins for graphgps.head.san_graph.SANGraphHead and
                   graphgps.head.graphormer_graph.GraphormerHead (graph-level pooling and prediction)
+    KernelPENodeEncoder, rw_landing_probs  drop-in for graphgps.encoder.kernel_pos_encoder.KernelPENodeEncoder (the
+                  RWSE node encoder) and the random-walk landing probabilities it reads, computed on the device
     GraphBatch    duck-typed stand-in for a collated PyG Batch (PyG is optional)
     make_batch    seeded synthetic batches of the BASELINE shapes
     GPSStack      the L-layer stack of a GPSModel (shared graph structure, plane hand-off, one gradient bucket, capture)
@@ -26,9 +28,10 @@ from .san import SAN2Layer, SANLayer  # noqa: F401
 from .custom_gnn import GatedGCNLayer, GINEConvLayer  # noqa: F401
 from .inductive_edge import InductiveEdgeHead  # noqa: F401
 from .graph_head import GraphormerHead, SANGraphHead  # noqa: F401
+from .rwse import KernelPENodeEncoder, rw_landing_probs  # noqa: F401
 from .dp import GradBucket  # noqa: F401
 from .stack import GPSStack  # noqa: F401
 from .loader import BatchPrefetcher, collate  # noqa: F401
 
-__all__ = ["GPSLayer", "GraphormerLayer", "BiasEncoder", "SANLayer", "SAN2Layer", "GatedGCNLayer", "GINEConvLayer", "InductiveEdgeHead", "SANGraphHead", "GraphormerHead", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
+__all__ = ["GPSLayer", "GraphormerLayer", "BiasEncoder", "SANLayer", "SAN2Layer", "GatedGCNLayer", "GINEConvLayer", "InductiveEdgeHead", "SANGraphHead", "GraphormerHead", "KernelPENodeEncoder", "rw_landing_probs", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
            "batch_from_lists"]

@@ -182,6 +182,23 @@ class GpsGraphHeadPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
 
 
+RWSE_MAX_COLS, RWSE_MAX_STEPS = 64, 256
+
+
+class GpsKernelPeArgs(C.Structure):
+    """KernelPENodeEncoder (kernel_pos_encoder.py, model "linear"): sizes and modes, pestat, x, out and their gradients,
+    linear_x, pe_encoder and raw_norm, and scratch."""
+    _fields_ = [("N", C.c_int64), ("K", C.c_int64), ("dim_in", C.c_int64), ("dim_emb", C.c_int64),
+                ("dim_pe", C.c_int64), ("expand_x", C.c_int32), ("batch_norm", C.c_int32), ("training", C.c_int32),
+                ("flags", C.c_int32), ("pestat", _fp), ("x", _fp), ("out", _fp), ("grad_out", _fp), ("grad_x", _fp),
+                ("linear_x", GpsLinear), ("pe_encoder", GpsLinear), ("raw_norm", GpsBatchNorm),
+                ("saved", _fp), ("saved_bytes", C.c_int64), ("workspace", _fp), ("workspace_bytes", C.c_int64)]
+
+
+class GpsKernelPePlan(C.Structure):
+    _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
+
+
 class GpsSanArgs(C.Structure):
     """SAN layer (san_layer.py, variant 0) or SAN2 layer (san2_layer.py, variant 1): config, dropout stream, graph and
     nmax, tensors, scratch, the ten Linears attention.{Q,K,V,Q_2,K_2,E,E_2}, O_h, FFN_h_layer1, FFN_h_layer2,
@@ -314,6 +331,10 @@ SYMBOLS = {
     "gps_graph_head_plan": (C.c_int, [C.POINTER(GpsGraphHeadArgs), C.POINTER(GpsGraphHeadPlan)]),
     "gps_graph_head_forward": (C.c_int, [C.POINTER(GpsGraphHeadArgs), _fp]),
     "gps_graph_head_backward": (C.c_int, [C.POINTER(GpsGraphHeadArgs), _fp]),
+    "gps_rwse_landing": (C.c_int, [C.POINTER(GpsGraph), C.POINTER(_i32), _i32, _i32, _fp, _fp, _i64, _fp]),
+    "gps_kernel_pe_plan": (C.c_int, [C.POINTER(GpsKernelPeArgs), C.POINTER(GpsKernelPePlan)]),
+    "gps_kernel_pe_forward": (C.c_int, [C.POINTER(GpsKernelPeArgs), _fp]),
+    "gps_kernel_pe_backward": (C.c_int, [C.POINTER(GpsKernelPeArgs), _fp]),
     "gps_graph_pool_forward": (C.c_int, [C.POINTER(GpsGraph), _i32, _fp, _i64, _fp, _i64, _fp, _i64, _fp]),
     "gps_graph_pool_backward": (C.c_int, [C.POINTER(GpsGraph), _i32, _fp, _i64, _i64, _fp, _fp]),
     "gps_san_plan": (C.c_int, [C.POINTER(GpsSanArgs), C.POINTER(GpsSanPlan)]),

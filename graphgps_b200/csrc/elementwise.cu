@@ -98,59 +98,6 @@ __global__ void __launch_bounds__(1024) k_rowwise2(OpA a, int64_t rowsA, int ga,
   }
 }
 
-struct BnRegs {  // per-thread column constants: y = z * sc + sh ; zhat = (z - mean) * invstd
-  float4 mean, invstd, gamma, beta;
-  __device__ void load(const BnView& v, int c4, int vb = -1) {
-    gamma = ld4(v.gamma + c4 * 4);
-    beta = ld4(v.beta + c4 * 4);
-    if (v.mode == 0) {
-      mean = ld4(v.mean + c4 * 4);
-      invstd = ld4(v.invstd + c4 * 4);
-    } else if (v.mode == 2) {
-      mean = ld4(v.running_mean + c4 * 4);
-      const float4 rv = ld4(v.running_var + c4 * 4);
-      invstd = make_float4(rsqrtf(rv.x + kBnEps), rsqrtf(rv.y + kBnEps), rsqrtf(rv.z + kBnEps), rsqrtf(rv.w + kBnEps));
-    } else {
-      float m[4], is[4], var[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const double mu = v.sums[c4 * 4 + j] * v.inv_n;
-        double vv = v.sums[v.d + c4 * 4 + j] * v.inv_n - mu * mu;
-        if (vv < 0.0) vv = 0.0;
-        m[j] = (float)mu;
-        var[j] = (float)(vv * v.unbias);
-        is[j] = (float)(1.0 / sqrt(vv + (double)kBnEps));
-      }
-      mean = make_float4(m[0], m[1], m[2], m[3]);
-      invstd = make_float4(is[0], is[1], is[2], is[3]);
-      if ((vb < 0 ? (int)blockIdx.x : vb) == 0 && threadIdx.y == 0) {   // one CTA publishes the statistics and the running update
-        st4(v.save_mean + c4 * 4, mean);
-        st4(v.save_invstd + c4 * 4, invstd);
-        if (v.running_mean) {
-          const float4 rm = ld4(v.running_mean + c4 * 4);
-          st4(v.running_mean + c4 * 4, make_float4((1.f - kBnMomentum) * rm.x + kBnMomentum * m[0],
-                                                   (1.f - kBnMomentum) * rm.y + kBnMomentum * m[1],
-                                                   (1.f - kBnMomentum) * rm.z + kBnMomentum * m[2],
-                                                   (1.f - kBnMomentum) * rm.w + kBnMomentum * m[3]));
-        }
-        if (v.running_var) {
-          const float4 rv = ld4(v.running_var + c4 * 4);
-          st4(v.running_var + c4 * 4, make_float4((1.f - kBnMomentum) * rv.x + kBnMomentum * var[0],
-                                                  (1.f - kBnMomentum) * rv.y + kBnMomentum * var[1],
-                                                  (1.f - kBnMomentum) * rv.z + kBnMomentum * var[2],
-                                                  (1.f - kBnMomentum) * rv.w + kBnMomentum * var[3]));
-        }
-        if (c4 == 0 && v.nbt) *v.nbt += 1;
-      }
-    }
-  }
-  __device__ float4 zhat(float4 z) const {
-    return make_float4((z.x - mean.x) * invstd.x, (z.y - mean.y) * invstd.y, (z.z - mean.z) * invstd.z,
-                       (z.w - mean.w) * invstd.w);
-  }
-  __device__ float4 apply(float4 z) const { return f4fma(zhat(z), gamma, beta); }
-};
-
 __device__ __forceinline__ float4 act4(int act, float4 v) {
   if (act < 0) return v;
   return make_float4(act_fwd_rt(act, v.x), act_fwd_rt(act, v.y), act_fwd_rt(act, v.z), act_fwd_rt(act, v.w));

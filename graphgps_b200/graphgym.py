@@ -156,6 +156,76 @@ def install_graph_heads(register_module=None):
     return previous
 
 
+_KERNEL_PE = {"RWSE": "RWSENodeEncoder", "HKdiagSE": "HKdiagSENodeEncoder", "ElstaticSE": "ElstaticSENodeEncoder"}
+
+
+def install_rwse(on_device=False, kernel_module=None, register_module=None, loader_module=None):
+    """Rebind ``RWSENodeEncoder``, ``HKdiagSENodeEncoder`` and ``ElstaticSENodeEncoder`` to the H100 kernel-PE encoder:
+    in ``graphgps.encoder.kernel_pos_encoder``, in ``register.node_encoder_dict`` and as ``enc2_cls`` / ``enc3_cls`` of
+    every composed encoder class registered there (``Atom+RWSE``, ``TypeDictNode+RWSE``, ``*+LapPE+RWSE``, ...).  Each
+    keeps the reference's ``(dim_emb, expand_x=True)`` constructor and reads ``cfg.share.dim_in`` and
+    ``cfg.posenc_<type>`` when it is built.
+
+    With ``on_device=True`` the RWSE encoders also compute their statistics on the device from the batch's edges, at
+    ``cfg.posenc_RWSE.kernel.times``, and ``graphgps.loader.master_loader.compute_posenc_stats`` is wrapped to drop
+    ``'RWSE'`` from its ``pe_types``, so the dataset's CPU pre-transform no longer computes them.
+
+    Call after ``import graphgps`` and before the dataset is loaded (``on_device``) and ``create_model()``.  Returns what
+    it replaced, as a dict by name (``compute_posenc_stats`` too with ``on_device``), so a caller can restore it."""
+    from .rwse import KernelPENodeEncoder
+    if kernel_module is None:
+        kernel_module = importlib.import_module("graphgps.encoder.kernel_pos_encoder")
+    if register_module is None:
+        register_module = importlib.import_module("torch_geometric.graphgym.register")
+
+    def _make(kernel_type):
+        class KernelPENodeEncoderGraphGym(KernelPENodeEncoder):
+            """KernelPENodeEncoder(dim_emb, expand_x) with its sizes and settings from GraphGym's cfg."""
+
+            def __init__(self, dim_emb, expand_x=True):
+                cfg = importlib.import_module("torch_geometric.graphgym.config").cfg
+                pecfg = getattr(cfg, f"posenc_{kernel_type}")
+                times = list(pecfg.kernel.times)
+                dim_pe = pecfg.dim_pe
+                # without expand_x the encoder concatenates batch.x as it is: dim_emb - dim_pe columns (the width
+                # composed encoders give their first encoder)
+                dim_in = cfg.share.dim_in if expand_x and dim_emb > dim_pe else dim_emb - dim_pe
+                super().__init__(dim_in, dim_emb, len(times), dim_pe, kernel_type=kernel_type,
+                                 raw_norm_type=pecfg.raw_norm_type, model=pecfg.model, expand_x=expand_x,
+                                 ksteps=times if on_device and kernel_type == "RWSE" else None,
+                                 pass_as_var=pecfg.pass_as_var)
+
+        KernelPENodeEncoderGraphGym.__name__ = _KERNEL_PE[kernel_type]
+        return KernelPENodeEncoderGraphGym
+
+    previous, swap = {}, {}
+    for kernel_type, name in _KERNEL_PE.items():
+        old = getattr(kernel_module, name, None)
+        new = _make(kernel_type)
+        previous[name] = old
+        setattr(kernel_module, name, new)
+        if old is not None:
+            swap[old] = new
+        if kernel_type in register_module.node_encoder_dict or old is not None:
+            register_module.node_encoder_dict[kernel_type] = new
+    for cls in list(register_module.node_encoder_dict.values()):
+        for attr in ("enc2_cls", "enc3_cls"):
+            enc = getattr(cls, attr, None)
+            if enc is not None and enc in swap:
+                setattr(cls, attr, swap[enc])
+    if on_device:
+        if loader_module is None:
+            loader_module = importlib.import_module("graphgps.loader.master_loader")
+        compute = loader_module.compute_posenc_stats
+        previous["compute_posenc_stats"] = compute
+
+        def compute_posenc_stats(data, pe_types, *args, **kwargs):
+            return compute(data, [t for t in pe_types if t != "RWSE"], *args, **kwargs)
+
+        loader_module.compute_posenc_stats = compute_posenc_stats
+    return previous
+
+
 def register(name="gpslayer_b200"):
     """Register a LayerConfig-style wrapper under ``name`` in GraphGym's layer registry.
 

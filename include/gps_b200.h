@@ -610,6 +610,72 @@ int gps_graph_pool_backward(const GpsGraph* graph, int32_t pooling, const float*
                             float* grad_x, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * RWSE, the random-walk structural encoding (graphgps/transform/posenc_stats.py:get_rw_landing_probs and
+ * graphgps/encoder/kernel_pos_encoder.py:KernelPENodeEncoder).
+ *
+ * gps_rwse_landing: out[i, j] = (P^ksteps[j])[i, i] for every node i of `graph`, out [N, nk] float32, with
+ * P = D_out^-1 A built from the graph's edges as the reference builds it from edge_index: A[s, d] counts the edges
+ * s -> d (duplicates add up, self-loops count), D_out is the out-degree, a node without out-edges has a zero row, and
+ * P^0 = I.  P is block-diagonal over the graphs (graph_ptr), so each graph's walks stay inside it.  `ksteps` is a host
+ * array of nk values, copied into the launch arguments: any order, repeats and 0 are allowed.  nmax is the size of the
+ * largest graph (GraphStructure.nmax).  workspace >= 8 * N bytes, 8-byte aligned (the inverse out-degrees in fp64).
+ * Each entry is a fixed-order sum in CSR order, accumulated in fp64 and stored in fp32 after every step: no atomics,
+ * two runs give the same bits.  Limits (else GPS_ERR_UNSUPPORTED): 1 <= nk <= GPS_RWSE_MAX_COLS,
+ * 0 <= ksteps[j] <= GPS_RWSE_MAX_STEPS, and one walk row of the largest graph fits on chip (nmax <= about 28 000).
+ * Bad sizes, missing pointers or a misaligned workspace are GPS_ERR_ARG; both before any CUDA call.
+ * ---------------------------------------------------------------------------------------- */
+#define GPS_RWSE_MAX_COLS 64
+#define GPS_RWSE_MAX_STEPS 256
+int gps_rwse_landing(const GpsGraph* graph, const int32_t* ksteps, int32_t nk, int32_t nmax, float* out,
+                     void* workspace, int64_t workspace_bytes, void* stream);
+
+/* KernelPENodeEncoder (model "linear"), w = dim_emb - dim_pe:
+ *   forward    z = BN(pestat) (batch_norm; the raw statistics otherwise)    pestat [N, K], raw_norm over K columns
+ *              out = [h | z Wp^T + bp]                                      out [N, dim_emb]; pe_encoder Wp [dim_pe, K]
+ *              h = x Wx^T + bx with expand_x (linear_x Wx [w, dim_in]), else h = x (dim_in == w)
+ *   backward   grad_x = g[:, :w] Wx (expand_x) or g[:, :w]; the gradients of Wp, bp, Wx, bx and of the BatchNorm's
+ *              weight and bias (pestat is data and gets no gradient)
+ * BatchNorm as torch.nn.BatchNorm1d: training normalises by the batch statistics (eps 1e-5) and updates running_mean /
+ * running_var (unbiased, momentum 0.1) and num_batches_tracked; eval uses the running statistics.  Every column and
+ * weight-gradient sum runs through per-CTA partials added in a fixed order: no float atomics, two runs give the same
+ * bits.  Built: 1 <= K <= GPS_RWSE_MAX_COLS, 1 <= dim_pe <= dim_emb <= 4096, 1 <= dim_in <= 4096; training with
+ * batch_norm needs N >= 2.  Anything else is GPS_ERR_UNSUPPORTED, bad sizes or missing pointers GPS_ERR_ARG, all
+ * before any CUDA call.  Backward writes grad_x and every parameter gradient whole.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  int64_t N;                 /* rows of pestat, x and out                                     */
+  int64_t K;                 /* columns of pestat (len(kernel.times))                         */
+  int64_t dim_in;            /* columns of x                                                  */
+  int64_t dim_emb;           /* columns of out                                                */
+  int64_t dim_pe;            /* columns of the encoded statistics                             */
+  int32_t expand_x;          /* 1: h = linear_x(x); 0: h = x                                  */
+  int32_t batch_norm;        /* 1: raw_norm is a BatchNorm1d(K); 0: none                      */
+  int32_t training;          /* BatchNorm: batch statistics and running update (1) or eval (0) */
+  int32_t flags;             /* reserved, 0                                                   */
+  const float* pestat;       /* [N, K]                                                        */
+  const float* x;            /* [N, dim_in]                                                   */
+  float* out;                /* [N, dim_emb] (forward)                                        */
+  const float* grad_out;     /* [N, dim_emb] (backward)                                       */
+  float* grad_x;             /* [N, dim_in] (backward)                                        */
+  GpsLinear linear_x;        /* linear_x.weight [w, dim_in] / .bias [w] and grads (expand_x)  */
+  GpsLinear pe_encoder;      /* pe_encoder.weight [dim_pe, K] / .bias [dim_pe] and grads      */
+  GpsBatchNorm raw_norm;     /* raw_norm.* [K] (batch_norm)                                   */
+  void* saved; int64_t saved_bytes;         /* forward -> backward                            */
+  void* workspace; int64_t workspace_bytes; /* transient                                      */
+} GpsKernelPeArgs;
+
+typedef struct {
+  int64_t saved_bytes;
+  int64_t fwd_workspace_bytes;
+  int64_t bwd_workspace_bytes;
+} GpsKernelPePlan;
+
+/* Sizes for args (only N, K, the widths, expand_x, batch_norm and training are read). */
+int gps_kernel_pe_plan(const GpsKernelPeArgs* args, GpsKernelPePlan* plan);
+int gps_kernel_pe_forward(const GpsKernelPeArgs* args, void* stream);
+int gps_kernel_pe_backward(const GpsKernelPeArgs* args, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * SAN layer (graphgps/layer/san_layer.py:10-210), the building block of SANTransformer, as every shipped config runs
  * it (full_graph, batch_norm, residual, no layer_norm, no Linear biases in the attention, in_dim == out_dim == d):
  *   [Q|K|V|Q2|K2] = x W^T, E = edge_attr W_E^T, E2 = W_E2 fake_edge_emb
