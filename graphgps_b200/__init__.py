@@ -12,6 +12,9 @@ Public surface (mirrors the reference's module boundary, SURVEY.md section 8b):
                   decoding, ranking metrics on the device)
     SANGraphHead, GraphormerHead  drop-ins for graphgps.head.san_graph.SANGraphHead and
                   graphgps.head.graphormer_graph.GraphormerHead (graph-level pooling and prediction)
+    InductiveNodeHead, NodeHead, weighted_cross_entropy, cross_entropy  drop-ins for
+                  graphgps.head.inductive_node.GNNInductiveNodeHead, GraphGym's GNNNodeHead and the node losses
+                  (graphgps.loss.weighted_cross_entropy, GraphGym's cross_entropy), with the loss kept on the device
     KernelPENodeEncoder, rw_landing_probs  drop-in for graphgps.encoder.kernel_pos_encoder.KernelPENodeEncoder (the
                   RWSE node encoder) and the random-walk landing probabilities it reads, computed on the device
     GraphBatch    duck-typed stand-in for a collated PyG Batch (PyG is optional)
@@ -28,10 +31,12 @@ from .san import SAN2Layer, SANLayer  # noqa: F401
 from .custom_gnn import GatedGCNLayer, GINEConvLayer  # noqa: F401
 from .inductive_edge import InductiveEdgeHead  # noqa: F401
 from .graph_head import GraphormerHead, SANGraphHead  # noqa: F401
+from .node_head import InductiveNodeHead, NodeHead, cross_entropy, weighted_cross_entropy  # noqa: F401
 from .rwse import KernelPENodeEncoder, rw_landing_probs  # noqa: F401
 from .dp import GradBucket  # noqa: F401
 from .stack import GPSStack  # noqa: F401
 from .loader import BatchPrefetcher, collate  # noqa: F401
 
-__all__ = ["GPSLayer", "GraphormerLayer", "BiasEncoder", "SANLayer", "SAN2Layer", "GatedGCNLayer", "GINEConvLayer", "InductiveEdgeHead", "SANGraphHead", "GraphormerHead", "KernelPENodeEncoder", "rw_landing_probs", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
+__all__ = ["GPSLayer", "GraphormerLayer", "BiasEncoder", "SANLayer", "SAN2Layer", "GatedGCNLayer", "GINEConvLayer", "InductiveEdgeHead", "SANGraphHead", "GraphormerHead", "InductiveNodeHead", "NodeHead",
+           "weighted_cross_entropy", "cross_entropy", "KernelPENodeEncoder", "rw_landing_probs", "GPSStack", "GradBucket", "GraphBatch", "BatchPrefetcher", "collate", "SHAPES", "make_batch",
            "batch_from_lists"]

@@ -182,6 +182,36 @@ class GpsGraphHeadPlan(C.Structure):
     _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
 
 
+NODE_HEAD_MAX_L, NODE_LOSS_MAX_C = 8, 4096
+
+
+class GpsNodeHeadArgs(C.Structure):
+    """Node-prediction head (GraphGym's MLP under inductive_node.py's GNNInductiveNodeHead or GNNNodeHead): L and the
+    widths, x, the optional row selection, y / pred and their gradients, fc[l] = the MLP's Linears in order, scratch."""
+    _fields_ = [("L", C.c_int32), ("precision", C.c_int32), ("flags", C.c_int32), ("training", C.c_int32),
+                ("seed", C.c_uint64), ("dim_in", C.c_int64), ("dim_inner", C.c_int64), ("dim_out", C.c_int64), ("N", C.c_int64),
+                ("M", C.c_int64), ("x", _fp), ("rows", _fp), ("y", _fp), ("pred", _fp), ("grad_y", _fp),
+                ("grad_pred", _fp), ("grad_x", _fp), ("fc", GpsLinear * NODE_HEAD_MAX_L),
+                ("saved", _fp), ("saved_bytes", C.c_int64), ("workspace", _fp), ("workspace_bytes", C.c_int64)]
+
+
+class GpsNodeHeadPlan(C.Structure):
+    _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
+
+
+class GpsNodeLossArgs(C.Structure):
+    """Node loss (weighted_cross_entropy.py or GraphGym's cross_entropy): sizes, mode, pred / label, the device loss,
+    pred_score, their gradients and scratch."""
+    _fields_ = [("M", C.c_int64), ("C", C.c_int64), ("weighted", C.c_int32), ("flags", C.c_int32),
+                ("pred", _fp), ("label", _fp), ("loss", _fp), ("pred_score", _fp), ("grad_loss", _fp),
+                ("grad_score", _fp), ("grad_pred", _fp),
+                ("saved", _fp), ("saved_bytes", C.c_int64), ("workspace", _fp), ("workspace_bytes", C.c_int64)]
+
+
+class GpsNodeLossPlan(C.Structure):
+    _fields_ = [("saved_bytes", C.c_int64), ("fwd_workspace_bytes", C.c_int64), ("bwd_workspace_bytes", C.c_int64)]
+
+
 RWSE_MAX_COLS, RWSE_MAX_STEPS = 64, 256
 
 
@@ -331,6 +361,14 @@ SYMBOLS = {
     "gps_graph_head_plan": (C.c_int, [C.POINTER(GpsGraphHeadArgs), C.POINTER(GpsGraphHeadPlan)]),
     "gps_graph_head_forward": (C.c_int, [C.POINTER(GpsGraphHeadArgs), _fp]),
     "gps_graph_head_backward": (C.c_int, [C.POINTER(GpsGraphHeadArgs), _fp]),
+    "gps_node_head_plan": (C.c_int, [C.POINTER(GpsNodeHeadArgs), C.POINTER(GpsNodeHeadPlan)]),
+    "gps_node_head_forward": (C.c_int, [C.POINTER(GpsNodeHeadArgs), _fp]),
+    "gps_node_head_backward": (C.c_int, [C.POINTER(GpsNodeHeadArgs), _fp]),
+    "gps_row_l2norm_forward": (C.c_int, [_fp, _i64, _i64, _i64, _fp, _fp, _fp]),
+    "gps_row_l2norm_backward": (C.c_int, [_fp, _fp, _fp, _i64, _i64, _i64, _fp, _fp]),
+    "gps_node_loss_plan": (C.c_int, [C.POINTER(GpsNodeLossArgs), C.POINTER(GpsNodeLossPlan)]),
+    "gps_node_loss_forward": (C.c_int, [C.POINTER(GpsNodeLossArgs), _fp]),
+    "gps_node_loss_backward": (C.c_int, [C.POINTER(GpsNodeLossArgs), _fp]),
     "gps_rwse_landing": (C.c_int, [C.POINTER(GpsGraph), C.POINTER(_i32), _i32, _i32, _fp, _fp, _i64, _fp]),
     "gps_kernel_pe_plan": (C.c_int, [C.POINTER(GpsKernelPeArgs), C.POINTER(GpsKernelPePlan)]),
     "gps_kernel_pe_forward": (C.c_int, [C.POINTER(GpsKernelPeArgs), _fp]),

@@ -10,6 +10,8 @@ from __future__ import annotations
 
 import importlib
 
+import torch
+
 from .gps_layer import GPSLayer
 
 
@@ -153,6 +155,81 @@ def install_graph_heads(register_module=None):
     new = {"san_graph": SANGraphHeadGraphGym, "graphormer_graph": GraphormerHeadGraphGym}
     previous = {n: register_module.head_dict.get(n) for n in new}
     register_module.head_dict.update(new)
+    return previous
+
+
+def install_node_heads(register_module=None):
+    """Set ``register.head_dict['inductive_node']`` and ``['node']`` to the H100 heads, so GPSModel, CustomGNN,
+    SANTransformer and GraphormerModel build them for ``gnn.head: inductive_node`` / ``node``: each looks its head up in
+    that registry at construction time.  The registered classes have the reference's ``(dim_in, dim_out)`` constructor
+    and read ``cfg.gnn.layers_post_mp`` and ``cfg.gnn.dim_inner`` when they are built.
+
+    Call after ``import graphgps`` and before ``create_model()``.  Returns the classes it replaced, as a dict by name,
+    so a caller can restore them."""
+    from .node_head import InductiveNodeHead, NodeHead
+    if register_module is None:
+        register_module = importlib.import_module("torch_geometric.graphgym.register")
+
+    def _make(base, name):
+        class NodeHeadGraphGym(base):
+            """The head (dim_in, dim_out) with its MLP's depth and hidden width from GraphGym's cfg."""
+
+            def __init__(self, dim_in, dim_out):
+                cfg = importlib.import_module("torch_geometric.graphgym.config").cfg
+                super().__init__(dim_in, dim_out, layers_post_mp=cfg.gnn.layers_post_mp,
+                                 dim_inner=getattr(cfg.gnn, "dim_inner", None))
+
+        NodeHeadGraphGym.__name__ = name
+        return NodeHeadGraphGym
+
+    new = {"inductive_node": _make(InductiveNodeHead, "InductiveNodeHeadGraphGym"),
+           "node": _make(NodeHead, "NodeHeadGraphGym")}
+    previous = {n: register_module.head_dict.get(n) for n in new}
+    register_module.head_dict.update(new)
+    return previous
+
+
+def install_node_losses(register_module=None, train_module=None):
+    """Put the node losses on the device.
+
+    ``register.loss_dict['weighted_cross_entropy']`` becomes a function that, like the reference's, returns None unless
+    ``cfg.model.loss_fun == 'weighted_cross_entropy'``.  ``graphgps.train.custom_train.compute_loss`` becomes a wrapper
+    that squeezes a trailing size-1 dim as GraphGym's does and computes the multiclass ``cross_entropy`` on the device
+    when ``cfg.model.loss_fun == 'cross_entropy'``, ``cfg.dataset.task_type == 'classification'``, pred is a CUDA
+    float32 [M, C > 1] tensor and the labels are 1-D int64; everything else goes to the previous ``compute_loss``
+    unchanged.
+
+    Call after ``import graphgps`` and before training.  Returns what it replaced, as a dict by name
+    (``weighted_cross_entropy`` and ``compute_loss``), so a caller can restore it."""
+    from . import node_head
+    if register_module is None:
+        register_module = importlib.import_module("torch_geometric.graphgym.register")
+    if train_module is None:
+        train_module = importlib.import_module("graphgps.train.custom_train")
+
+    def _cfg():
+        return importlib.import_module("torch_geometric.graphgym.config").cfg
+
+    def weighted_cross_entropy(pred, true):
+        if _cfg().model.loss_fun == "weighted_cross_entropy":
+            return node_head.weighted_cross_entropy(pred, true)
+        return None
+
+    previous = {"weighted_cross_entropy": register_module.loss_dict.get("weighted_cross_entropy"),
+                "compute_loss": train_module.compute_loss}
+    fallback = previous["compute_loss"]
+
+    def compute_loss(pred, true):
+        cfg = _cfg()
+        p = pred.squeeze(-1) if pred.ndim > 1 else pred
+        t = true.squeeze(-1) if true.ndim > 1 else true
+        if cfg.model.loss_fun == "cross_entropy" and cfg.dataset.task_type == "classification" and p.is_cuda and \
+                p.dtype == torch.float32 and p.ndim == 2 and p.shape[1] > 1 and t.ndim == 1 and t.dtype == torch.int64:
+            return node_head.cross_entropy(p, t)
+        return fallback(pred, true)
+
+    register_module.loss_dict["weighted_cross_entropy"] = weighted_cross_entropy
+    train_module.compute_loss = compute_loss
     return previous
 
 

@@ -610,6 +610,101 @@ int gps_graph_pool_backward(const GpsGraph* graph, int32_t pooling, const float*
                             float* grad_x, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Node-prediction heads, the head of every node-level config: GraphGym's MLP (layers_post_mp = L) under
+ * graphgps/head/inductive_node.py (GNNInductiveNodeHead) and GraphGym's GNNNodeHead (`node`):
+ *   h_0 = x                                                  [N, dim_in]
+ *   h_{l+1} = normalize(relu(h_l W_l^T + b_l)), l < L - 1    fc[l]: [dim_inner, dim_in (l = 0) or dim_inner]
+ *   y = h_{L-1} W_{L-1}^T + b_{L-1}                          fc[L-1]: [dim_out, dim_in (L = 1) or dim_inner]
+ *   pred = y[rows]                                           rows != NULL: M distinct row indices (int64)
+ * normalize(r) = r / max(||r||_2, 1e-12) per row (F.normalize(p=2, dim=1), which GraphGym's hidden layers apply).
+ * Backward: grad_y (NULL = 0) plus grad_pred (NULL = 0) added into rows; grad_x [N, dim_in] and every parameter
+ * gradient written whole.  The normalisation's backward is g_in = (g - h (h.g)) / n for n = ||r|| >= 1e-12 and
+ * g / 1e-12 below, times the ReLU mask.  Widths run at the next multiple of 8 with zero pad columns; every product is
+ * the TMA GEMM, row sums run in a fixed order and the weight gradients take the deterministic split-K path: two runs
+ * give the same bits.  Built: 1 <= L <= GPS_NODE_HEAD_MAX_L, 1 <= dim_in, dim_inner, dim_out <= 4096.  Anything else
+ * is GPS_ERR_UNSUPPORTED, bad sizes or missing pointers GPS_ERR_ARG, all before any CUDA call.  Row indices outside
+ * [0, N) are never dereferenced.
+ * ---------------------------------------------------------------------------------------- */
+#define GPS_NODE_HEAD_MAX_L 8
+
+typedef struct {
+  int32_t L;                 /* layers_post_mp                                                */
+  int32_t precision;         /* GPS_PREC_*                                                    */
+  int32_t flags;             /* reserved, 0                                                   */
+  int32_t training;          /* not read (the head has no dropout and no running statistics)  */
+  uint64_t seed;             /* unused                                                        */
+  int64_t dim_in, dim_inner, dim_out;
+  int64_t N;                 /* rows of x                                                     */
+  int64_t M;                 /* entries of rows (0 without rows)                              */
+  const float* x;            /* [N, dim_in]                                                   */
+  const int64_t* rows;       /* [M] or NULL                                                   */
+  float* y;                  /* [N, dim_out] (forward)                                        */
+  float* pred;               /* [M, dim_out] (forward, with rows)                             */
+  const float* grad_y;       /* [N, dim_out] or NULL (backward)                               */
+  const float* grad_pred;    /* [M, dim_out] or NULL (backward)                               */
+  float* grad_x;             /* [N, dim_in] (backward)                                        */
+  GpsLinear fc[GPS_NODE_HEAD_MAX_L]; /* the L Linears in order, with their grads             */
+  void* saved; int64_t saved_bytes;         /* forward -> backward                            */
+  void* workspace; int64_t workspace_bytes; /* transient                                      */
+} GpsNodeHeadArgs;
+
+typedef struct {
+  int64_t saved_bytes;
+  int64_t fwd_workspace_bytes;
+  int64_t bwd_workspace_bytes;
+} GpsNodeHeadPlan;
+
+/* Sizes for args (only L, the widths, precision and N are read). */
+int gps_node_head_plan(const GpsNodeHeadArgs* args, GpsNodeHeadPlan* plan);
+int gps_node_head_forward(const GpsNodeHeadArgs* args, void* stream);
+int gps_node_head_backward(const GpsNodeHeadArgs* args, void* stream);
+/* Stage entries: the row normalisation alone, over rows x d at pitch ld (d % 4 == 0, ld % 4 == 0, ld >= d, d <= 4096,
+ * else GPS_ERR_UNSUPPORTED).  Forward: out = r / max(||r||, 1e-12) and norm [rows] = ||r||.  Backward from the forward's
+ * out and norm: grad_in = the formula above times the ReLU mask (out > 0).  out may alias r, grad_in may alias g. */
+int gps_row_l2norm_forward(const float* r, int64_t rows, int64_t d, int64_t ld, float* out, float* norm, void* stream);
+int gps_row_l2norm_backward(const float* g, const float* out, const float* norm, int64_t rows, int64_t d, int64_t ld,
+                            float* grad_in, void* stream);
+
+/* The node losses (GraphGym's compute_loss with loss_fun cross_entropy, and graphgps/loss/weighted_cross_entropy.py):
+ *   C > 1    pred_score = log_softmax(pred); loss = sum_i w_{y_i} (-pred_score[i, y_i]) / sum_i w_{y_i}
+ *   C == 1   pred_score = sigmoid(pred); loss = sum_i w_{y_i} bce(pred_i, y_i) / M   (weighted only)
+ * weighted: w_c = (M - count_c) / M * [count_c > 0] in float32 (count_c = labels equal to c, over max(C, 2) classes);
+ * otherwise w = 1.  label: int64 [M] in [0, max(C, 2)).  The loss stays on the device (float32 [1]).  Counts use
+ * integer atomics; every floating-point sum is fp64 through per-CTA partials added in a fixed order: two runs give
+ * the same bits.  A batch whose weights sum to 0 (one class, or M = 0) gives NaN, as torch does.
+ * Backward: grad_pred [M, C] from grad_loss (float32 [1], NULL = 0) and grad_score ([M, C], NULL = 0), reading the
+ * forward's pred_score and saved buffer.  Built: 1 <= C <= GPS_NODE_LOSS_MAX_C (else GPS_ERR_UNSUPPORTED); C == 1
+ * needs weighted. */
+#define GPS_NODE_LOSS_MAX_C 4096
+
+typedef struct {
+  int64_t M;                 /* rows of pred                                                  */
+  int64_t C;                 /* columns of pred; 1 = binary                                   */
+  int32_t weighted;          /* 1: weighted_cross_entropy, 0: cross_entropy                   */
+  int32_t flags;             /* reserved, 0                                                   */
+  const float* pred;         /* [M, C]                                                        */
+  const int64_t* label;      /* [M]                                                           */
+  float* loss;               /* [1] (forward)                                                 */
+  float* pred_score;         /* [M, C] (written by forward, read by backward)                 */
+  const float* grad_loss;    /* [1] or NULL (backward)                                        */
+  const float* grad_score;   /* [M, C] or NULL (backward)                                     */
+  float* grad_pred;          /* [M, C] (backward)                                             */
+  void* saved; int64_t saved_bytes;         /* forward -> backward                            */
+  void* workspace; int64_t workspace_bytes; /* transient                                      */
+} GpsNodeLossArgs;
+
+typedef struct {
+  int64_t saved_bytes;
+  int64_t fwd_workspace_bytes;
+  int64_t bwd_workspace_bytes;
+} GpsNodeLossPlan;
+
+/* Sizes for args (only M, C and weighted are read). */
+int gps_node_loss_plan(const GpsNodeLossArgs* args, GpsNodeLossPlan* plan);
+int gps_node_loss_forward(const GpsNodeLossArgs* args, void* stream);
+int gps_node_loss_backward(const GpsNodeLossArgs* args, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * RWSE, the random-walk structural encoding (graphgps/transform/posenc_stats.py:get_rw_landing_probs and
  * graphgps/encoder/kernel_pos_encoder.py:KernelPENodeEncoder).
  *
